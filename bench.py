@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s of the B200-native KuiperLLama hot path (BASELINE.json `metric`).
+"""bench.py -- decode tokens/s of the H100-native KuiperLLama hot path (BASELINE.json `metric`).
 
 One "step" = one greedy decode position (one token, batch 1) of the workload's model through the
 device-resident decoder (libkllm_b200.so).  The metric is quoted on context 1 -> 1024, so the
@@ -33,7 +33,7 @@ the fp32 Llama-2-7B of configs[4] is measured in the same run and reported under
 --impl reference       the reference's CPU implementation of the path (oracle port; the reference's
                        CMake build needs Armadillo/glog/gtest/sentencepiece, none installed).
 --impl reference-cuda  the reference's own CUDA kernels + model code (oracle/_ref, compiled from
-                       /root/reference for sm_100a) timed on the same GPU: the "reference GPU" row.
+                       a reference checkout for sm_90a) timed on the same GPU: the "reference GPU" row.
 """
 from __future__ import annotations
 
@@ -89,6 +89,9 @@ def parse_args():
     ap.add_argument("--no-secondary", action="store_true", help="N>1: skip the fp32 Llama-2-7B line (configs[4])")
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="budget of the cpu_baseline leg")
     ap.add_argument("--seed", type=int, default=None)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path computed in its last step -- the "
+                         "final logits and the token ids of the timed positions -- as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -181,19 +184,7 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, torch copy)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(workload, kernel_key):
-    """DRAM traffic (dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full` capture)
-    of a kernel, from the committed summary profiles/dominant_kernel_traffic.json, or None."""
-    p = ROOT / "profiles" / "dominant_kernel_traffic.json"
-    if p.exists():
-        try:
-            return json.loads(p.read_text()).get(workload, {}).get(kernel_key)
-        except Exception:
-            return None
-    return None
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def host_cores():
@@ -301,7 +292,7 @@ def run_reference(args, rank, world):
 
 
 def run_reference_cuda(args, rank, world):
-    """--impl reference-cuda: oracle/_ref -- the reference's own .cu/.cpp compiled for sm_100a --
+    """--impl reference-cuda: oracle/_ref -- the reference's own .cu/.cpp compiled for sm_90a --
     decoding the same synthetic checkpoint on this GPU through LLama2Model::predict (rank 0)."""
     if rank != 0:
         return
@@ -343,7 +334,7 @@ def run_reference_cuda(args, rank, world):
                       "dtype": "f32" if shape.group_size == 0 else "int8w/f32",
                       "config": {"workload": WORKLOAD_NAMES[args.workload], "shape": shape.name, "context": f"1->{K}",
                                  "batch": 1, "what": "the reference's own CUDA backend (kuiper/source/op/kernels/cuda/*.cu "
-                                 "+ model/llama3.cpp, unmodified, nvcc 12.9 sm_100a) on this GPU, wall clock of the predict loop"},
+                                 "+ model/llama3.cpp, unmodified, nvcc 12.9 sm_90a) on this GPU, wall clock of the predict loop"},
                       "roofline_frac_of_measured_hbm": shape.weight_bytes_per_token() * K / dt / 1e9 / measured_peaks()[0]})
 
 
@@ -493,7 +484,9 @@ class Bench:
 
     def run(self):
         args, shape = self.args, self.shape
-        K = min(args.steps, shape.seq_len)
+        if args.steps > shape.seq_len:
+            raise SystemExit(f"--steps {args.steps} exceeds the context of {shape.name} ({shape.seq_len})")
+        K = args.steps
         ctx = min(CONTEXT, shape.seq_len)
         windows = plan_windows(K, ctx)
         self.prepass()
@@ -508,6 +501,11 @@ class Bench:
             totals.append(sum(ms)); per_window.append(ms)
         t_wall1 = time.time()
         launches = (self.lib.kllm_launch_count() - launches0) // reps
+        # what a caller of the timed path receives from its last window: the ids of every timed position and
+        # the logits of the last one (the windows reproduce the pre-pass ids, checked in time_windows)
+        import numpy as np
+        outputs = {"logits": self.dec.logits().astype(np.float32),
+                   "token_ids": np.array([i for s, n in windows for i in self.ids[s:s + n]], np.float64)}
         clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
         ms_total = statistics.median(totals)
         med_rep = per_window[totals.index(sorted(totals)[len(totals) // 2])]
@@ -544,21 +542,20 @@ class Bench:
             # events around that launch (state upload 16 B + kernel + id readback on the same stream).
             n_launch = len(windows)
             ach = bytes_gpu * K / (ms_total / 1e3) / 1e9
-            key = "megakernel" if self.world == 1 else f"megakernel_tp{self.world}"
-            traffic = ncu_traffic(self.workload, key)
             res["roofline"] = {
                 "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": traffic["dram_bytes_per_token"] * K / n_launch if traffic else None,
+                "traffic": None,  # measured DRAM bytes: no profiler capture is kept with the benchmark
                 "kernel": "decode_megakernel (persistent: whole forward + argmax, %s positions per launch)" %
                           "/".join(sorted({str(n) for _, n in windows})),
                 "algorithmic_bytes_per_launch": bytes_gpu * K / n_launch, "avg_launch_us": ms_total * 1e3 / n_launch,
                 "launches_timed": n_launch, "peak_source": peak_src, "per_gpu": self.world > 1,
-                "traffic_source": traffic}
+                "traffic_source": None}
         else:
             res["roofline"] = {"bound": "hbm", "achieved": bytes_gpu * tok_s / 1e9, "peak": peak, "unit": "GB/s",
                                "frac": bytes_gpu * tok_s / 1e9 / peak, "traffic": None,
                                "kernel": "graph engine: whole decode step (all launches)", "peak_source": peak_src}
         res["median_rep_window_ms"] = med_rep
+        res["outputs"] = outputs
         return res
 
     def close(self):
@@ -585,6 +582,11 @@ def run_ours(args, rank, world):
     b = Bench(args, rank, world, args.workload, stream, lib)
     shape = b.shape
     res = b.run()
+    if rank == 0 and args.dump_outputs:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in res["outputs"].items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), a)
     line = None
     if rank == 0:
         line = {
@@ -599,7 +601,7 @@ def run_ours(args, rank, world):
                                   f"{res['windows']}", "batch": 1,
                        "reps": args.reps, "reported": "median repetition; per window CUDA events on the decoder's stream, max over ranks",
                        "parallelism": "single GPU" if world == 1 else f"tp{world}",
-                       "l2": "no flush: every step streams %.2f GB of weights per GPU >> 126 MB L2" % (res["bytes_gpu"] / 1e9),
+                       "l2": "no flush: every step streams %.2f GB of weights per GPU >> 50 MB L2" % (res["bytes_gpu"] / 1e9),
                        "weight_bytes_per_token": res["bytes_tok"], "launches_per_step": b.launches_per_step,
                        "engine": b.engine,
                        "numerics": "fast: free summation order (int8 rows as int8 weights x 24-bit fixed-point activations on mma.sync s8 / dp4a, "

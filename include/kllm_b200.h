@@ -1,4 +1,4 @@
-/* kllm_b200.h -- C-ABI of the B200-native KuiperLLama decode path (libkllm_b200.so).
+/* kllm_b200.h -- C-ABI of the H100-native KuiperLLama decode path (libkllm_b200.so).
  *
  * This is the drop-in boundary: plain pointers, ints and an opaque stream, no C++ or torch
  * types.  Every entry point names the reference interface it replaces (paths relative to the
@@ -17,7 +17,7 @@
  *
  * Arithmetic contract: fp32 throughout, each kernel reproduces the reference CUDA kernel's
  * floating-point operation order (see DESIGN.md "Bit-exactness"), so results are bit-identical
- * to the reference's own CUDA path compiled for sm_100a, not merely within tolerance.
+ * to the reference's own CUDA path compiled for sm_90a, not merely within tolerance.
  */
 #ifndef KLLM_B200_H_
 #define KLLM_B200_H_
@@ -128,13 +128,13 @@ typedef struct {
 
 int kllm_gemv_fused(const kllm_gemv_job* job, void* stream);
 
-/* ---- batched prompt GEMM on the tcgen05 tensor cores (TOLERANCED: TF32 multiply, fp32 accumulate) ----
+/* ---- batched prompt GEMM on the Hopper tensor cores (TOLERANCED: TF32 multiply, fp32 accumulate) ----
  * out[n_tokens, out_dim] = x[n_tokens, in_dim] . w[out_dim, in_dim]^T, all fp32 row-major device memory.
  * Replaces the n_tokens single-row GEMVs the reference issues for a prompt, one full forward per
  * prompt token (demo/main.cpp:18-23 -> LLama2Model::predict, llama3.cpp:147-167; MatmulLayer::forward,
  * matmul.cpp:57-80): the weight matrix is streamed once per 256 tokens instead of once per token.
- * TMA tensor-map loads (cp.async.bulk.tensor, 128-byte swizzle) feed tcgen05.mma.kind::tf32 with the
- * accumulator in TMEM.  Results agree with the fp32 GEMV to ~1e-3 relative (10-bit mantissas), NOT
+ * TMA tensor-map loads (cp.async.bulk.tensor, 128-byte swizzle) feed wgmma.mma_async (tf32) with the
+ * accumulators in registers.  Results agree with the fp32 GEMV to ~1e-3 relative (10-bit mantissas), NOT
  * bit for bit: the decode path never uses it.  in_dim % 4 == 0, 16-byte aligned x and w. */
 int kllm_gemm_tf32(const float* x, const float* w, float* out, int n_tokens, int in_dim, int out_dim,
                    void* stream);
@@ -240,7 +240,7 @@ int kllm_decoder_step(kllm_decoder* dec, int32_t token_host, int32_t pos, int is
 int kllm_decoder_prompt(kllm_decoder* dec, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
                         int32_t* next_host);
 /* TOLERANCED batched prefill: the same contract as kllm_decoder_prompt, but the prompt positions go
- * through every layer together -- each projection one GEMM [n, in] x [out, in]^T on the tcgen05
+ * through every layer together -- each projection one GEMM [n, in] x [out, in]^T on the wgmma
  * tensor cores (TF32 multiply, fp32 accumulate, kllm_gemm_tf32), the weights streamed once per 256
  * positions instead of once per position; classifier only for the last position.  KV-cache rows and
  * logits agree with the position-by-position path to ~1e-3 relative, NOT bit for bit (TF32 keeps 10
@@ -279,7 +279,7 @@ const char* kllm_decoder_engine(const kllm_decoder* dec);
  * elements).  Globaltimer ns: [0] phase entered, [1] input vector staged (+normalised), [2] last
  * ring stage consumed, [3] grid barrier passed, [10] input vector polled (before the norm).
  * SM cycles of warp 0: [4] addend prefetch, [5] dot products, [6] reductions, [7] epilogues,
- * [8] waiting for ring stages, [9] rows of a stage.  Measurement aid (profiles/). */
+ * [8] waiting for ring stages, [9] rows of a stage.  Measurement aid (tools/phase_timeline.py). */
 int kllm_decoder_profile(kllm_decoder* dec, int32_t first_token, int32_t start_pos,
                          int32_t n_steps, int32_t profiled_step, uint64_t* stamps_host,
                          int32_t capacity, int32_t* grid_out, int32_t* phases_out);

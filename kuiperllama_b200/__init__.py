@@ -1,4 +1,4 @@
-"""kuiperllama_b200 -- B200-native (sm_100a) single-batch decoder behind KuiperLLama's API.
+"""kuiperllama_b200 -- H100-native (sm_90a) single-batch decoder behind KuiperLLama's API.
 
 The product is native code:
   * ``lib/libkllm_b200.so``  hand-written CUDA kernels + the C-ABI of ``include/kllm_b200.h``;

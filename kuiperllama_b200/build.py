@@ -1,7 +1,7 @@
-"""Build libkllm_b200.so (the C-ABI product library) in-tree with nvcc for sm_100a.
+"""Build libkllm_b200.so (the C-ABI product library) in-tree with nvcc for sm_90a.
 
 Used by __graft_entry__.build(), tests and bench.py.  No JIT cache: the .so lands in
-kuiperllama_b200/lib/ so it travels to the GPU box with the repo snapshot.
+kuiperllama_b200/lib/, next to the sources it was built from.
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libkllm_b200.so"
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def nvcc_path() -> str:

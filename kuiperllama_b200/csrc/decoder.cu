@@ -125,7 +125,7 @@ struct kllm_decoder {
   cudaGraph_t graph_tf = nullptr;
   cudaGraphExec_t exec_tf = nullptr;    // teacher forced
   int launches_per_step = 0;
-  // batched tcgen05 prefill (kllm_decoder_prefill_tf32): activations of one block of prompt positions
+  // batched wgmma prefill (kllm_decoder_prefill_tf32): activations of one block of prompt positions
   float* pf_buf = nullptr;
   PrefillWorkspace pf_ws{};
 };
@@ -491,7 +491,7 @@ int kllm_decoder_prefill_tf32(kllm_decoder* dc, const int32_t* tokens_host, int3
   const kllm_decoder_desc& d = dc->d;
   if (start_pos + n_tokens > d.seq_len) return KLLM_E_INVALID;
   if (d.group_size != 0 || d.tp_size > 1) return KLLM_E_UNSUPPORTED;  // fp32 checkpoints, one GPU
-  constexpr int kBlock = 256;  // prompt positions per pass = the N of the tcgen05.mma
+  constexpr int kBlock = 256;  // prompt positions per pass = the N of the wgmma
   const int hs = dc->head_size, q_rows = d.head_num * hs, kvd = dc->kv_dim;
   if ((d.dim & 3) || (d.hidden_dim & 3) || (q_rows & 3)) return KLLM_E_UNSUPPORTED;
   if (dc->pf_buf == nullptr) {

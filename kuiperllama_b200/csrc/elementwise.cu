@@ -257,7 +257,7 @@ using namespace kllm;
 
 extern "C" {
 
-const char* kllm_version(void) { return "kllm_b200 0.1 (sm_100a)"; }
+const char* kllm_version(void) { return "kllm_b200 0.1 (sm_90a)"; }
 
 const char* kllm_error_string(int code) {
   switch (code) {

@@ -1,4 +1,4 @@
-// Batch-1 weight-streaming GEMV for sm_100a, fp32 and int8-group weights, with the fused
+// Batch-1 weight-streaming GEMV for sm_90a, fp32 and int8-group weights, with the fused
 // prologue/epilogues the decode loop needs (RMSNorm on the input; bias; residual add;
 // SiLU*gate).  Replaces matmul_kernel_cu / matmul_kernel_cu_qint8
 // (kuiper/source/op/kernels/cuda/matmul_kernel.cu:6-134) plus the rmsnorm / add / swiglu
@@ -260,9 +260,9 @@ static int g_sm_count = 0;
 static int sm_count() {
   if (g_sm_count == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-      g_sm_count = 148;
+      g_sm_count = 132;
   }
   return g_sm_count;
 }

@@ -1,7 +1,7 @@
-// Device-side helpers shared by the sm_100a kernels.
+// Device-side helpers shared by the sm_90a kernels.
 //
 // "Reference order" below always means the floating-point operation order of the reference's
-// own CUDA kernels as compiled by nvcc 12.9 for sm_100a (read off the SASS of oracle/_ref,
+// own CUDA kernels as compiled by nvcc 12.9 for sm_90a (read off the SASS of oracle/_ref,
 // see DESIGN.md "Bit-exactness").  All arithmetic that must match is written with explicit
 // round-to-nearest intrinsics so the compiler can neither fuse nor split it differently.
 #pragma once

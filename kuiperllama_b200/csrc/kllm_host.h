@@ -38,7 +38,7 @@ int launch_mha(PosArg pos, int head_num, int layer_index, int seq_len, int kv_di
 // tp_comm.cu: exchange areas [2][world][stride] of 64-bit tagged words, one per rank (peer transport)
 int comm_tagged_areas(kllm_comm* comm, unsigned long long** areas8, int* world, int* rank, int* stride);
 
-// prefill.cu: one block of T prompt positions through every layer with batched tcgen05 GEMMs
+// prefill.cu: one block of T prompt positions through every layer with batched wgmma GEMMs
 struct PrefillModel {
   int dim, hidden_dim, layer_num, head_num, kv_head_num, vocab_size, seq_len, head_size, flavour;
   int mega_layout;  // 1: the persistent engine's head-major K / V cache layout (megakernel.cu)

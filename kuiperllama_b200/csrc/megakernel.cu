@@ -1,22 +1,22 @@
-// Persistent decode megakernel for sm_100a: the whole per-token forward of LLama2Model /
+// Persistent decode megakernel for sm_90a: the whole per-token forward of LLama2Model /
 // Qwen2Model (kuiper/source/model/llama3.cpp:147-167, 600-745) in ONE cooperative launch that
 // can run any number of consecutive positions.
 //
 // Why: at batch 1 the path is a 4-26 GB/token weight stream; with one launch per op (even 6
-// fused launches per layer in a CUDA graph) every kernel boundary drains the HBM pipeline
-// (profiles/r01a: 15-42 % DRAM utilisation per kernel).  Here one CTA per SM stays resident
+// fused launches per layer in a CUDA graph) every kernel boundary drains the HBM pipeline.
+// Here one CTA per SM stays resident
 // and a dedicated producer warp streams that CTA's share of EVERY weight matrix, in schedule
 // order, through a ring of shared-memory stages with TMA bulk copies (cp.async.bulk ->
 // UBLKCP) signalled on mbarriers.  Weights never depend on activations, so the producer runs
-// ahead across every dependency of the token; a second producer warp walks the same schedule a
-// few stages further ahead and only pulls the bytes into L2 (cp.async.bulk.prefetch.L2), so
-// HBM keeps fetching while SMs wait for each other.
+// ahead across every dependency of the token; a second producer warp can walk the same schedule a
+// few stages further ahead and only pull the bytes into L2 (cp.async.bulk.prefetch.L2;
+// KLLM_PREFETCH_STAGES, off by default -- it measured slower on an H100).
 //
 // Schedule per layer:  QKV(+bias) | attention(+RoPE) | Wo | W1,W3->SiLU*gate | W2 ; then
 // classifier + greedy argmax.  RoPE moves into the attention phase so GEMV rows can be split
 // evenly over all SMs.
 //
-// Consumers (CW warps: 8 for fp32 weights, 14 for int8): the rows of a ring stage are handed out as TASKS of
+// Consumers (CW warps, 8 by default for fp32 and int8 weights): the rows of a ring stage are handed out as TASKS of
 // up to four rows to one warp each, round-robin.  A task's rows share every load of the input vector, their
 // dot-product chains interleave (ILP instead of occupancy), their totals are folded with "packed" shuffle trees
 // (kllm_device.cuh) that do the additions of cub's tree only, and one lane per row runs the epilogues side by
@@ -25,7 +25,7 @@
 // No local memory: the ring takes the whole unified L1, so a stack access is a round trip to L2.  The kernel
 // parameters are __grid_constant__ (never copied to the stack), register buffers are always written in full
 // (a conditionally written element forces the array into local memory), nothing indexes an array at run time.
-// `cuobjdump -res-usage` / tools/sass_histogram.py (profiles/r02_sass_histogram.txt) show what is left.
+// `cuobjdump -res-usage` / tools/sass_histogram.py show what is left.
 //
 // Hand-over between phases (KLLM_MEGA_TAGGED=2, default): every produced element is published as
 // one 64-bit {tag, fp32} word and polled in place by the consuming phase -- no fences, flags or
@@ -64,7 +64,7 @@ namespace mega {
 #define KLLM_MBAR_HINT_NS 20000u
 #endif
 // 1: warps without a row in an attention tile skip its wait and block at a hardware barrier instead of
-// spinning on the mbarrier.  Measured on B200 (profiles/README.md, pass M): no gain (826 vs 837 tok/s), so off.
+// spinning on the mbarrier.  Off by default.
 #ifndef KLLM_ATTN_GATE
 #define KLLM_ATTN_GATE 0
 #endif
@@ -542,8 +542,7 @@ __device__ __forceinline__ void accum_w8_dp4a(const uint32_t (&w)[NR], const uin
 }
 
 // ---- int8 weights x fixed-point activations on the tensor cores (TOLERANCED, same numbers as above) ----------
-// The integer dot-product unit runs at a quarter of the FP32 rate on sm_100 (measured: the dp4a rows above are
-// bound by it, 12 IDP.4A per 16 weights), so where a ring stage holds several rows that share the input
+// The dp4a rows above spend 12 IDP.4A per 16 weights on the integer dot-product unit, so where a ring stage holds several rows that share the input
 // vector -- every matrix with 4096-byte rows -- the 64-element groups go through mma.sync m16n8k32 (s8 x s8 ->
 // s32, SASS IMMA.16832.S8.S8) instead:
 //     A (16 x 32, row major)  rows 0..7 = the (up to 8) weight rows of the stage, rows 8..15 mirror them
@@ -806,7 +805,7 @@ __device__ __forceinline__ float attention_inputs(const Params& P, const Phase& 
 }
 
 // ---- attention: SP CTAs per query head, two phases (mha_kernel.cu:47-110 + rope_kernel.cu) ---------
-// The reference gives a head one CTA and so did round 1: 32 of 148 SMs worked while the rest polled,
+// The reference gives a head one CTA and so did round 1: 32 of the SMs worked while the rest polled,
 // and the time grew with the context.  Every score (one left-to-right FFMA chain per timestep) and
 // every output element (one FFMA chain over the timesteps) is independent of the others, so the work
 // splits over SP CTAs per head WITHOUT touching a single chain -- results stay bit-identical:
@@ -1053,7 +1052,7 @@ __device__ KLLM_PHASE_CALL Pipe attention_fused_phase(const Params& P, int head,
     else
       P.attn_out[static_cast<size_t>(head) * hs + tid] = value;
   }
-  if (stamp && tid == 0) {  // SM cycles of thread 0 (profiles/: tools/phase_timeline.py)
+  if (stamp && tid == 0) {  // SM cycles of thread 0 (tools/phase_timeline.py)
     const long long c_end = clock64();
     stamp[4] = static_cast<unsigned long long>(c_rope - c_begin);                             // q/k/v poll + RoPE
     stamp[5] = static_cast<unsigned long long>(c_scores - c_rope - c_wait_scores);            // scores
@@ -2527,12 +2526,11 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     for (int d : dims)
       if (d % m.group_size != 0 || ((d / m.group_size) * 4) % 16 != 0) return KLLM_E_UNSUPPORTED;
   }
-  // consumer warps (+ the ring producer and the L2 prefetcher): fp32 rows 8 x 168 registers; int8 rows 14, so
-  // that the CTA is 16 warps = 4 per scheduler with 128 registers each (16 consumers make 18 warps, which caps
-  // them at 96 registers and spills).  Measured on B200 (profiles/README.md, passes Q-T): fp32 6 vs 8 warps
-  // 1072 = 1072 (TinyLlama), 1218 < 1296 (Qwen2.5-0.5B), 210 < 213 (Llama-2-7B); int8 16 / 14 / 8 warps
-  // 394 / 400 / 375 tok/s.
-  consumer_warps_ = int8 ? 14 : 8;
+  // consumer warps (+ the ring producer and the L2 prefetcher): 8 for fp32 and int8 rows.  With 12 or 14 int8
+  // consumers the CTA is capped at 128 registers a thread and ptxas spills on sm_90a (16 consumers: 96).
+  // Measured on an H100 SXM (700 W), Llama-2-7B int8, fast mode, bench.py --steps 128: 8 warps 261 / 262 tok/s
+  // vs 14 warps 240 / 240 (two runs each).
+  consumer_warps_ = 8;
   if (const char* e = getenv("KLLM_CONSUMER_WARPS")) {
     const int v = atoi(e);
     if (int8 && (v == 6 || v == 8 || v == 12 || v == 14 || v == 16)) consumer_warps_ = v;  // fast mode: CT >= 192 quantises M <= 16384 in <= 6 rounds
@@ -2599,8 +2597,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
          hs % (attn_split_ * 2) == 0)
     attn_split_ *= 2;
   const int attn_split_max = attn_split_;
-  // The split costs one more hand-off per layer (~1.5 us): worth it when a head's K and V are big
-  // (head_size 128: 1 MB per head at context 1024), not for head_size 64 (measured, profiles/README.md).
+  // The split costs one more hand-off per layer: worth it when a head's K and V are big
+  // (head_size 128: 1 MB per head at context 1024), not for head_size 64.
   if (hs < 128) attn_split_ = 1;
   int split_cap = attn_split_max;
   if (fast_) {  // flash: split by timestep, any power of two whose partial triples fit the scores area
@@ -2622,10 +2620,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
 
   // ---- phase table ---------------------------------------------------------------------------------
   std::vector<Phase> ph;
-  // Rows per consumer task (1, 2 or 4) of a phase.  Measured on B200 (profiles/README.md, passes Q and R):
-  // 4 everywhere is best or equal (TinyLlama 1105 vs 1082 "auto" vs 1068 with 2; Llama-2-7B int8 418 / 405 /
-  // 407) -- the four rows of a task share every load of the input vector, and that outweighs the better
-  // balance of small tasks.  KLLM_TASK_ROWS_RT=1|2|4 forces a size, =auto picks per phase with the cost model
+  // Rows per consumer task (1, 2 or 4) of a phase: 4 everywhere by default -- the four rows of a task share
+  // every load of the input vector, which is meant to outweigh the better balance of small tasks.  KLLM_TASK_ROWS_RT=1|2|4 forces a size, =auto picks per phase with the cost model
   // below (rounds x (rows + x_cost), tasks never crossing a ring stage).
   int forced_task_rows = 4;
   if (const char* e = getenv("KLLM_TASK_ROWS_RT")) {
@@ -2634,10 +2630,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     if (std::string(e) == "auto") forced_task_rows = 0;
   }
   // KLLM_INT8_MMA=1: int8 fast rows in the team form -- mma.sync m16n8k32 s8 for stages of 3-8 rows, dp4a with the
-  // columns split over the team for 1-2 long rows.  Correct (the parity suite passes with it) but not faster on
-  // B200: Llama-2-7B int8 398 (teams of 4, 12 warps) / 403 (pairs, 14 warps) vs 407 tok/s for the plain dp4a
-  // rows (profiles/README.md, passes S and T) -- at one byte per weight the shared-memory reads of the
-  // fragments cost what the dp4a arithmetic costs.  Off by default.
+  // columns split over the team for 1-2 long rows.  Correct (the parity suite passes with it); at one byte per
+  // weight the shared-memory reads of the fragments cost about what the dp4a arithmetic costs.  Off by default.
   bool int8_mma = false;
   if (const char* e = getenv("KLLM_INT8_MMA")) int8_mma = atoi(e) != 0;
   auto pick_task_rows = [&](Phase& p) {
@@ -3029,9 +3023,10 @@ int MegaEngine::run(int n_tokens, const int32_t* teacher_dev, unsigned long long
   P.attn_vsplit = attn_vsplit_;
   P.attn_parts = attn_parts_;
   P.scores = d_scores_;
-  // 256 KB per SM = 38 MB of weights in flight towards L2 chip-wide (measured with 32 KB stages: 6-12 stages
-  // best, >= 24 thrashes L2); in stages, so that a smaller stage size keeps the same byte distance
-  P.pf_stages = std::max(4, (256 * 1024) / std::max(1, stage_bytes_));
+  // Off by default: on an H100 (50 MB L2) every run-ahead distance measured slower than none.  H100 SXM at a
+  // 400 W power limit, bench.py --steps 128 --reps 3, tok/s for KLLM_PREFETCH_STAGES = 0 / 4 / 8-9 (256 KB per
+  // SM) / 16 / 24: TinyLlama-1.1B fp32 585 / 566 / 544 / 399 / 379, Llama-2-7B int8 267 / 258 / 244 / 196 / 184.
+  P.pf_stages = 0;
   if (const char* e = getenv("KLLM_PREFETCH_STAGES")) P.pf_stages = std::max(0, atoi(e));
   P.group_size = m.group_size;
   P.dim = m.dim;

@@ -1,4 +1,4 @@
-// Batched prompt prefill around the tcgen05 GEMM (prefill_gemm.cu) -- the TOLERANCED alternative to
+// Batched prompt prefill around the wgmma GEMM (prefill_gemm.cu) -- the TOLERANCED alternative to
 // feeding the prompt position by position (demo/main.cpp:18-23 calls LLama2Model::predict once per
 // prompt token; llama3.cpp:147-167 then runs the whole single-token forward, classifier included).
 //
@@ -190,7 +190,7 @@ int prefill_block(const PrefillModel& m, PrefillWorkspace& ws, const int32_t* to
     count_launch();
     return static_cast<int>(cudaGetLastError());
   };
-  const int ew_grid = 592;  // 4 x 148 SMs for the grid-stride elementwise kernels
+  const int ew_grid = 528;  // 4 x 132 SMs for the grid-stride elementwise kernels
   embed_rows_kernel<<<T, 256, 0, s>>>(tokens_dev, m.tok_emb, ws.x, dim, m.vocab_size);
   PF_TRY(count());
   const CacheLayout cl{m.mega_layout, m.seq_len, kvd, hs, m.attn_split > 0 ? m.attn_split : 1};

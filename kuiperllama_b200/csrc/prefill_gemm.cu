@@ -1,20 +1,22 @@
-// Batched GEMM for prompt prefill on the 5th-generation tensor cores (sm_100a):
-//     out[T, N] = x[T, K] . w[N, K]^T        fp32 storage, TF32 multiply, fp32 accumulate in TMEM
+// Batched GEMM for prompt prefill on the Hopper tensor cores (sm_90a):
+//     out[T, N] = x[T, K] . w[N, K]^T        fp32 storage, TF32 multiply, fp32 accumulate in registers
 //
 // The reference feeds a prompt through one full single-token forward per position (demo/main.cpp:
 // 18-23, llama3.cpp:147-167) -- T GEMVs that stream every weight T times.  With the T prompt rows
-// as the N dimension of a tcgen05.mma the weights are streamed once per 256 tokens.
+// as the N dimension of a wgmma the weights are streamed once per 256 tokens.
 //
 // This is an explicitly TOLERANCED kernel: TF32 keeps 10 mantissa bits of each operand, so results
 // agree with the fp32 GEMV path to ~1e-3 relative, not bit for bit (tests/test_prefill_gpu.py states
 // the bound).  The bit-exact decode path never calls it.
 //
-// Structure (one CTA per 128 weight rows x one block of BN tokens, 6 warps):
-//   warp 0   TMA producer: cp.async.bulk.tensor 2-D tiles of w [128 x 32 fp32] and x [BN x 32 fp32],
-//            128-byte swizzle, into a 4-stage shared-memory ring (SASS: UTMALDG)
-//   warp 1   MMA issuer: one thread, 4 x tcgen05.mma.kind::tf32 (M 128, N BN, K 8) per stage, D in
-//            TMEM; tcgen05.commit frees the stage / signals the epilogue (SASS: UTCHMMA / UTCBAR)
-//   warps 2-5 epilogue: tcgen05.ld 32 lanes x 32 columns per warp (SASS: LDTM), transposed store
+// Structure (one CTA per 128 weight rows x one block of BN tokens, three warpgroups):
+//   warpgroup 0    TMA producer (one thread): cp.async.bulk.tensor 2-D tiles of w [128 x 32 fp32] and
+//                  x [BN x 32 fp32], 128-byte swizzle, into a 4-stage shared-memory ring (SASS: UTMALDG)
+//   warpgroups 1-2 consumers, 64 weight rows each: round the stage's operands to the nearest tf32 in place,
+//                  then 4 x wgmma.mma_async m64nBNk8 tf32 per stage, both
+//                  operands from shared memory, accumulators in registers (SASS: HGMMA); a stage is
+//                  released once the wgmma group after it has been issued and the one reading it retired
+//   epilogue       each consumer thread stores its accumulator fragment straight to out
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -26,12 +28,12 @@
 namespace kllm {
 namespace tc {
 
-constexpr int BM = 128;     // weight rows per CTA = MMA M
+constexpr int BM = 128;     // weight rows per CTA = 2 consumer warpgroups x wgmma M 64
 constexpr int BK = 32;      // fp32 elements per K block = 128 bytes = one swizzle-128B row
-constexpr int UMMA_K = 8;   // tf32: 32 bytes of K per tcgen05.mma
+constexpr int WG_K = 8;     // tf32: 32 bytes of K per wgmma
 constexpr int STAGES = 4;
 constexpr int A_BYTES = BM * BK * 4;  // 16 KB
-constexpr int THREADS = 192;
+constexpr int THREADS = 384;
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -56,27 +58,111 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// Shared-memory matrix descriptor of a K-major tile with 128-byte swizzle (cute::UMMA::SmemDescriptor,
-// cutlass include/cute/arch/mma_sm100_desc.hpp): start address >> 4 in bits [0,14), leading byte
-// offset (unused with swizzle; 1) in [16,30), stride byte offset = 8 rows x 128 B = 1024 B >> 4 in
-// [32,46), descriptor version 1 in [46,48), layout type SWIZZLE_128B = 2 in [61,64).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  return static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D = F32 (1 << 4), A = B = TF32 (2 << 7, 2 << 10),
-// both K-major (bits 15, 16 clear), N >> 3 in [17,23), M >> 4 in [24,29).
-__device__ __forceinline__ uint32_t umma_idesc_tf32(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(BM >> 4) << 24);
+// Shared-memory matrix descriptor of a K-major tile with 128-byte swizzle (PTX ISA, "Matrix Descriptor
+// Format" of wgmma): start address >> 4 in bits [0,14), leading byte offset (unused with swizzle; 1) in
+// [16,30), stride byte offset = 8 rows x 128 B = 1024 B >> 4 in [32,46), base offset 0 (tiles are
+// 1024-byte aligned), swizzle mode 128B = 1 in [62,64).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
+  return static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 8] . B[N x 8]^T, tf32 operands from shared memory, fp32 accumulators: thread t of the
+// warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and columns 8 j + 2 (t % 4) (+ 1), d[4 j .. 4 j + 3].
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-      " tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n .reg .pred p;\n setp.ne.b32 p, %18, 0;\n"
+      " wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n"
+      " wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %66, 0;\n"
+      " wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<256>(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %130, 0;\n"
+      " wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
+// n float4 of shared memory rounded to the nearest tf32 (ties away from zero) by the 128 threads of a warpgroup
+__device__ __forceinline__ void round_tf32(float4* p, int n, int t) {
+  for (int i = t; i < n; i += 128) {
+    float4 v = p[i];
+    float* e = reinterpret_cast<float*>(&v);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      uint32_t r;
+      asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(e[j]));
+      e[j] = __uint_as_float(r);
+    }
+    p[i] = v;
+  }
 }
 
 template <int BN>
@@ -84,7 +170,6 @@ __global__ void __launch_bounds__(THREADS, 1)
 gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x,
                  float* __restrict__ out, int T, int N, int K) {
   constexpr int B_BYTES = BN * BK * 4;
-  constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;  // power of two >= 32
   extern __shared__ uint8_t raw_smem[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* a_tiles = base;
@@ -92,10 +177,8 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
   uint64_t* bars = reinterpret_cast<uint64_t*>(b_tiles + STAGES * B_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int n0 = blockIdx.x * BM;  // first weight row (output feature) of this CTA
   const int t0 = blockIdx.y * BN;  // first token
   const int kblocks = (K + BK - 1) / BK;
@@ -103,24 +186,14 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_addr(&full[s]), 1);
-      mbar_init(smem_addr(&empty[s]), 1);
+      mbar_init(smem_addr(&empty[s]), 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(smem_addr(tmem_full), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {  // one warp allocates the accumulator's TMEM columns and later frees them
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(tmem_slot)),
-                 "r"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {  // ---- TMA producer ----
+  if (wg == 0) {
+    if (t == 0) {  // ---- TMA producer ----
       for (int kb = 0; kb < kblocks; ++kb) {
         const int s = kb % STAGES;
         const uint32_t ph = (kb / STAGES) & 1;
@@ -131,58 +204,45 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
         tma_load_2d(smem_addr(b_tiles + s * B_BYTES), &map_x, bar, kb * BK, t0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ---- MMA issuer ----
-      const uint32_t idesc = umma_idesc_tf32(BN);
-      for (int kb = 0; kb < kblocks; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(smem_addr(&full[s]), ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_addr = smem_addr(a_tiles + s * A_BYTES);
-        const uint32_t b_addr = smem_addr(b_tiles + s * B_BYTES);
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k)  // 32 bytes of K per instruction: step inside the swizzle atom
-          umma_tf32(tmem_d, umma_desc_sw128(a_addr + k * UMMA_K * 4), umma_desc_sw128(b_addr + k * UMMA_K * 4), idesc,
-                    (kb > 0 || k > 0) ? 1u : 0u);
-        umma_commit(smem_addr(&empty[s]));  // the stage may be refilled once these MMAs have read it
-      }
-      umma_commit(smem_addr(tmem_full));  // accumulator complete
-    }
-  } else {
-    // ---- epilogue: TMEM lane = weight row, column = token; a warp may touch lanes 32 (warp % 4) .. +31 ----
-    const int quarter = warp & 3;
-    mbar_wait(smem_addr(tmem_full), 0u);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int row = n0 + quarter * 32 + lane;
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 32) {
-      uint32_t r[32];
-      const uint32_t taddr = tmem_d + (static_cast<uint32_t>(quarter * 32) << 16) + static_cast<uint32_t>(c);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-            "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-            "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-            "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(taddr)
-          : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (row < N) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int t = t0 + c + j;
-          if (t < T) out[static_cast<size_t>(t) * N + row] = __uint_as_float(r[j]);  // lanes = consecutive rows: coalesced
-        }
-      }
-    }
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(TMEM_COLS) : "memory");
+  // ---- consumers: warpgroup wg owns weight rows n0 + 64 (wg - 1) .. + 63 ----
+  float d[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+  const uint32_t a_off = static_cast<uint32_t>(wg - 1) * 64 * BK * 4;  // 8 KB: a multiple of the 1024-byte atom
+  for (int kb = 0; kb < kblocks; ++kb) {
+    const int s = kb % STAGES;
+    mbar_wait(smem_addr(&full[s]), (kb / STAGES) & 1);
+    // The tensor core truncates fp32 operands to tf32; round them to the nearest tf32 in place first, which halves
+    // the per-operand error.  Each warpgroup rounds its own 64 weight rows and half of the token rows, which
+    // both read, so the two meet at a named barrier before the wgmma (async proxy) reads the tiles.
+    round_tf32(reinterpret_cast<float4*>(a_tiles + s * A_BYTES + a_off), 64 * BK / 4, t);
+    round_tf32(reinterpret_cast<float4*>(b_tiles + s * B_BYTES + (wg - 1) * (B_BYTES / 2)), BN * BK / 8, t);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    const uint64_t adesc = wgmma_desc_sw128(smem_addr(a_tiles + s * A_BYTES) + a_off);
+    const uint64_t bdesc = wgmma_desc_sw128(smem_addr(b_tiles + s * B_BYTES));
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+    for (int k = 0; k < BK / WG_K; ++k)  // 32 bytes of K per instruction (2 descriptor units): inside the swizzle atom
+      wgmma_tf32<BN>(d, adesc + 2 * k, bdesc + 2 * k, 1u);
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    // the group of stage kb - 1 has retired: its tiles may be refilled
+    asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+    if (kb > 0 && t == 0) mbar_arrive(smem_addr(&empty[(kb - 1) % STAGES]));
+  }
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+
+  const int row = n0 + (wg - 1) * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+  const int col = t0 + 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const int r = row + 8 * (h >> 1), c = col + 8 * j + (h & 1);
+      if (r < N && c < T) out[static_cast<size_t>(c) * N + r] = d[4 * j + h];
+    }
   }
 }
 
@@ -221,7 +281,7 @@ static int launch(const float* x, const float* w, float* out, int T, int K, int 
   CUtensorMap map_w, map_x;
   if (int rc = make_map(&map_w, w, N, K, BM)) return rc;
   if (int rc = make_map(&map_x, x, T, K, BN)) return rc;
-  const size_t smem = 1024 + static_cast<size_t>(STAGES) * (A_BYTES + BN * BK * 4) + 256;
+  const size_t smem = 1024 + static_cast<size_t>(STAGES) * (A_BYTES + BN * BK * 4) + 128;
   static bool configured = false;
   if (!configured) {
     const cudaError_t e = cudaFuncSetAttribute(gemm_tf32_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,

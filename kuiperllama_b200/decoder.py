@@ -236,7 +236,7 @@ class Decoder:
         return nxt.value
 
     def prefill_tf32(self, tokens, start_pos: int = 0) -> int:
-        """TOLERANCED batched prefill on the tcgen05 tensor cores (TF32); same contract as prompt()."""
+        """TOLERANCED batched prefill on the Hopper tensor cores (wgmma) (TF32); same contract as prompt()."""
         n = len(tokens)
         arr = (ctypes.c_int32 * n)(*[int(t) for t in tokens])
         nxt = ctypes.c_int32(-1)

@@ -14,7 +14,12 @@ from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 VARIANTS = {"llama2": [], "qwen2": ["-DQWEN2_SUPPORT=ON"], "llama3": ["-DLLAMA3_SUPPORT=ON"]}
-REFERENCE = Path("/root/reference")
+
+
+def reference_dir() -> Path | None:
+    """The reference checkout named by KUIPER_REFERENCE_DIR, when its demo sources are readable."""
+    d = os.environ.get("KUIPER_REFERENCE_DIR")
+    return Path(d) if d and os.access(Path(d) / "demo" / "main.cpp", os.R_OK) else None
 
 
 def build_dir(variant: str) -> Path:
@@ -37,8 +42,8 @@ def build(variant: str = "llama2", verbose: bool = False) -> Path:
            "-DCMAKE_CXX_COMPILER=/usr/bin/g++", *VARIANTS[variant]]
     if shutil.which("ninja"):
         cfg += ["-G", "Ninja"]
-    if (REFERENCE / "demo" / "main.cpp").exists():
-        cfg.append(f"-DKUIPER_REFERENCE_DIR={REFERENCE}")
+    if reference_dir() is not None:
+        cfg.append(f"-DKUIPER_REFERENCE_DIR={reference_dir()}")
     quiet = {} if verbose else {"stdout": subprocess.PIPE, "stderr": subprocess.STDOUT}
     for cmd in (cfg, [cmake, "--build", str(out), "-j", str(min(32, os.cpu_count() or 4))]):
         r = subprocess.run(cmd, text=True, **quiet)

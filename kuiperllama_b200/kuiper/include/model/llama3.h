@@ -5,7 +5,7 @@
 // Two per-token paths share one set of uploaded weights:
 //   predict() on an embedding row that came from embedding() / fill_input() -- the only way
 //       demo/main.cpp drives a model -- recovers the token id and runs the fused, device-resident
-//       decoder of libkllm_b200 (include/kllm_b200.h): one persistent sm_100a kernel per token;
+//       decoder of libkllm_b200 (include/kllm_b200.h): one persistent sm_90a kernel per token;
 //   forward() is the layer-by-layer orchestration over the op registry (same arithmetic, one
 //       launch per op) for callers that hand in activations of their own; its named buffers and
 //       KV cache are created on first use.

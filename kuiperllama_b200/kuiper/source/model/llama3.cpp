@@ -1,4 +1,4 @@
-// model::LLama2Model / Qwen2Model on the B200 backend (API of kuiper/include/model/llama3.h,
+// model::LLama2Model / Qwen2Model on the H100 backend (API of kuiper/include/model/llama3.h,
 // behaviour of kuiper/source/model/llama3.cpp + qwen2.cpp in the reference).
 //
 // Loading: the checkpoint is mmap'd, every weight becomes an op layer that views the mapping
@@ -7,7 +7,7 @@
 // shares the weight buffers and owns its activations and KV cache.
 //
 // Per token: predict() recognises the embedding row it is given (the only way demo/main.cpp
-// feeds the model), recovers the token id and runs ONE persistent sm_100a kernel for the whole
+// feeds the model), recovers the token id and runs ONE persistent sm_90a kernel for the whole
 // forward + greedy argmax.  forward() is the reference's layer-by-layer orchestration
 // (llama3.cpp:147-167,600-745) over the op registry, for callers with their own activations;
 // it keeps its own named buffers (allocated on first use) and its own KV cache, so a sequence
@@ -76,7 +76,7 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   if (token_path_.empty()) return error::PathNotValid(token_path_);
   if (device_type != DeviceType::kDeviceCUDA)
     return error::InternalError(
-        "This library is the B200 (sm_100a) backend: init(kDeviceCUDA) is the only supported device; it has "
+        "This library is the H100 (sm_90a) backend: init(kDeviceCUDA) is the only supported device; it has "
         "no CPU path.");
   device_type_ = device_type;
   if (!tp_explicit_) tp_ = TpConfig::from_env();  // tools/kuiper_tp_launch: one process per GPU

@@ -5,7 +5,7 @@
 // passed as `const Tensor&` and written through, as there).
 //
 // Here every getter answers kDeviceCUDA with an adapter (kernels_interfaces.cpp) that unwraps the
-// tensors and calls the sm_100a C-ABI of include/kllm_b200.h.  There is NO CPU backend: asking for
+// tensors and calls the sm_90a C-ABI of include/kllm_b200.h.  There is NO CPU backend: asking for
 // kDeviceCPU is a fatal error saying so (the CPU restatement of the reference lives under oracle/
 // and is test infrastructure only).  The scale / softmax / scale-sum entries exist because the
 // reference's CPU attention is assembled from them; on CUDA attention is one kernel.

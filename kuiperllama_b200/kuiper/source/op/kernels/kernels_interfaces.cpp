@@ -31,7 +31,7 @@ inline T* mut(const tensor::Tensor& t) {
 template <typename Fn>
 Fn no_cpu_backend(const char* op) {
   LOG(FATAL) << "kernel registry: " << op
-             << " requested for a non-CUDA device.  This library is the B200 (sm_100a) backend "
+             << " requested for a non-CUDA device.  This library is the H100 (sm_90a) backend "
                 "only; it has no CPU kernels and never falls back to the host.";
   return nullptr;
 }

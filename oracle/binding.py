@@ -1,7 +1,7 @@
 """ctypes bindings for the two checkers:
 
   Oracle     oracle/_build/liboracle.so      plain-C restatement of the reference CPU path
-  RefCuda    oracle/_ref/libkuiper_ref.so    the reference's own sources compiled for sm_100a
+  RefCuda    oracle/_ref/libkuiper_ref.so    the reference's own sources compiled for sm_90a
              (+ libkuiper_ref_qwen2_kernels.so: its kernels under -DQWEN2_SUPPORT)
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
@@ -20,7 +20,12 @@ HERE = Path(__file__).resolve().parent
 ORACLE_SO = HERE / "_build" / "liboracle.so"
 REF_SO = HERE / "_ref" / "libkuiper_ref.so"
 REF_QWEN_SO = HERE / "_ref" / "libkuiper_ref_qwen2_kernels.so"
-REFERENCE_TREE = Path("/root/reference")
+
+
+def reference_tree() -> Path | None:
+    """The reference checkout named by KUIPER_REFERENCE_DIR, when it is there and readable."""
+    d = os.environ.get("KUIPER_REFERENCE_DIR")
+    return Path(d) if d and os.access(Path(d) / "kuiper", os.R_OK | os.X_OK) else None
 
 FLAVOURS = {"llama2": 0, "llama3": 1, "qwen2": 2, "qwen2file": 3}
 
@@ -31,11 +36,12 @@ def build_oracle() -> Path:
 
 
 def build_ref(jobs: int = 8) -> bool:
-    """Compile oracle/_ref from /root/reference when that tree is present (build container);
-    on the GPU box the prebuilt .so files that travelled with the snapshot are used."""
-    if not REFERENCE_TREE.is_dir():
+    """Compile oracle/_ref from the reference checkout when one is given (KUIPER_REFERENCE_DIR); the
+    tests do without it (tests/golden/reference_cuda.json holds what it computed)."""
+    ref = reference_tree()
+    if ref is None:
         return REF_SO.exists()
-    subprocess.check_call(["make", "-s", f"-j{jobs}", "-C", str(HERE), "ref"])
+    subprocess.check_call(["make", "-s", f"-j{jobs}", "-C", str(HERE), "ref", f"REF={ref}"])
     return True
 
 
@@ -261,7 +267,7 @@ class RefCuda:
     def __init__(self, flavour="llama2"):
         so = REF_SO if flavour == "llama2" else REF_QWEN_SO
         if not so.exists():
-            raise FileNotFoundError(f"{so} not built (run `make -C oracle ref` where /root/reference exists)")
+            raise FileNotFoundError(f"{so} not built (build with KUIPER_REFERENCE_DIR set to a reference checkout)")
         L = ctypes.CDLL(str(so))
         vp = c_void_p
         L.kref_flavour.restype = c_char_p

@@ -1,7 +1,7 @@
 /* kuiper_oracle.c -- CPU restatement of the KuiperLLama decode hot path (see kuiper_oracle.h).
  *
  * TEST INFRASTRUCTURE ONLY: never linked into, loaded by, or called from the product library.
- * Citations are relative to /root/reference.
+ * Citations are relative to the reference checkout's root.
  */
 #define _GNU_SOURCE
 #include "kuiper_oracle.h"
@@ -135,7 +135,7 @@ static float cub_block_sum_128(float v[128]) {
 
 /* cuda/matmul_kernel.cu:27-38: lane t walks float4 packs t, t+128, ...; each pack contributes
  * part = x.x*w.x + x.y*w.y + x.z*w.z + x.w*w.w, which nvcc 12.9 (-fmad=true default) contracts
- * for sm_100a to fma(x.w,w.w, fma(x.z,w.z, fma(x.x,w.x, x.y*w.y))) -- read off the SASS of
+ * for sm_90a to fma(x.w,w.w, fma(x.z,w.z, fma(x.x,w.x, x.y*w.y))) -- read off the SASS of
  * oracle/_ref (FMUL y; FFMA x; FFMA z; FFMA w; FADD acc) -- then sdata[t] += part (plain add). */
 void ko_matmul_f32_cuda_order(const float* x, const float* w, float* out, int M, int K) {
   const int pack_num = M / 4, pack_off = pack_num * 4;

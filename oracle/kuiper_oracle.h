@@ -4,7 +4,7 @@
  * --impl reference legs may build, load or call this.  The product library
  * (kuiperllama_b200/) never links it and has no CPU fallback.
  *
- * Every function restates one piece of /root/reference (paths relative to that root) in
+ * Every function restates one piece of the reference (paths relative to its root) in
  * plain C with fp32 arithmetic in the reference's CPU order.  The reference's CPU matmul
  * delegates to Armadillo 14.0.1 -> OpenBLAS sgemv (un-vendored, version unpinned;
  * kuiper/source/op/kernels/cpu/matmul_kernel.cpp:37-40), whose summation order is not part

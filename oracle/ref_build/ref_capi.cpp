@@ -1,5 +1,5 @@
 // GPU oracle: C-ABI wrappers around the UNMODIFIED reference sources, compiled where they
-// lie under /root/reference by oracle/Makefile into oracle/_ref/libkuiper_ref.so.
+// lie in the reference checkout by oracle/Makefile into oracle/_ref/libkuiper_ref.so.
 //
 // TEST INFRASTRUCTURE ONLY.  Nothing under kuiperllama_b200/ links, loads or calls this
 // library; only tests/, __graft_entry__.smoke() and bench.py's reference leg do, and only

@@ -1,8 +1,8 @@
 """Generate the golden fixtures in this directory by IMPORTING the reference's own PyTorch
 model and exporters (tools/model.py, tools/export.py, tools/model_qwen2.py,
-tools/export_qwen2.py) from /root/reference.  Run in the build container only:
+tools/export_qwen2.py) from a reference checkout:
 
-    python tests/golden/make_golden.py
+    KUIPER_REFERENCE_DIR=/path/to/KuiperLLama python tests/golden/make_golden.py
 
 Outputs (committed):
   tiny_llama2_fp32_shared.bin / .npz     legacy_export (v0), shared classifier
@@ -25,7 +25,7 @@ import sys
 import numpy as np
 import torch
 
-REF_TOOLS = "/root/reference/tools"
+REF_TOOLS = os.path.join(os.environ["KUIPER_REFERENCE_DIR"], "tools")
 sys.path.insert(0, REF_TOOLS)
 HERE = os.path.dirname(os.path.abspath(__file__))
 

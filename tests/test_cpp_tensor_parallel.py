@@ -170,7 +170,7 @@ def test_launcher_sets_the_environment_and_propagates_failure(kllm_lib):
 def _need_gpus(n):
     import torch
     if torch.cuda.device_count() < n:
-        pytest.skip(f"needs {n} GPUs (run under `gpurun --gpus {n}`)")
+        pytest.skip(f"needs {n} GPUs")
 
 
 @pytest.mark.gpu

@@ -1,8 +1,9 @@
 """-m gpu: the device-resident decoder (kllm_decoder_*) against
   - the reference PyTorch logits committed under tests/golden (<= 1e-4, north-star tolerance),
   - the CPU oracle (same tolerance, identical greedy ids),
-  - the reference's OWN CUDA model path run on this GPU (oracle/_ref): bit-identical logits,
-    KV cache and token ids -- including at BASELINE.json's full TinyLlama-1.1B size."""
+  - the reference's OWN CUDA model path (compiled for sm_90a; its outputs on an H100 recorded in
+    tests/golden/reference_cuda.json, see oracle/reference_golden.py): bit-identical logits and
+    token ids -- including at BASELINE.json's full TinyLlama-1.1B size."""
 import ctypes
 import os
 
@@ -26,29 +27,53 @@ def engine(request, monkeypatch):
     return request.param
 
 
-def make_decoder(shape, w):
+def make_decoder(shape, w, refusable=False):
     """Decoder on the engine the `engine` fixture forces.  The persistent ring needs 16-byte
     weight/scale rows; forcing it on a shape it cannot stage must fail loudly (never silently
-    fall back) -- such cases are skipped here and covered by the graph engine run."""
+    fall back).  For callers that pass `refusable` (shapes the graph engine run covers bit for bit)
+    that contract is what gets checked: the forced create fails with KLLM_E_UNSUPPORTED, the
+    decoder picks the graph engine when nothing is forced, and None is returned."""
     from kuiperllama_b200 import Decoder, KllmError
     try:
         return Decoder(shape, w)
     except KllmError as e:
-        if os.environ.get("KLLM_ENGINE") == "persistent" and "unsupported shape" in str(e):
-            pytest.skip(f"{shape.name}: persistent engine refuses this shape (graph engine covers it)")
-        raise
+        forced = os.environ.get("KLLM_ENGINE")
+        if not (refusable and forced == "persistent" and "unsupported shape" in str(e)):
+            raise
+    del os.environ["KLLM_ENGINE"]
+    try:
+        dec = Decoder(shape, w)
+        assert dec.engine == "graph", f"{shape.name}: refused when forced, but the default engine is {dec.engine}"
+        dec.close()
+    finally:
+        os.environ["KLLM_ENGINE"] = forced
+    return None
 
 
-def load_decoder(path, quant=False, flavour="llama2", qkv_bias=None):
+def load_decoder(path, quant=False, flavour="llama2", qkv_bias=None, refusable=False):
     from kuiperllama_b200.checkpoint import read_checkpoint, to_device
     shape, w = read_checkpoint(str(path), quant, flavour, qkv_bias=qkv_bias)
-    return make_decoder(shape, to_device(w)), shape
+    return make_decoder(shape, to_device(w), refusable), shape
 
 
 @pytest.fixture(scope="module")
 def ref():
-    from oracle.binding import RefCuda
-    return RefCuda("llama2")
+    from oracle.reference_golden import Reference
+    return Reference("llama2")
+
+
+def ref_decode(ref, path, quant, vocab, steps):
+    """The reference's demo loop (greedy, feeding its own output from token 1) when it runs live:
+    (ids, final logits); (None, None) otherwise."""
+    if not ref.live:
+        return None, None
+    rm = RefModel(ref, path, quant, vocab)
+    tok, ids = 1, []
+    for pos in range(steps):
+        tok, lg = rm.step(tok, pos, want_logits=(pos == steps - 1))
+        ids.append(tok)
+    rm.close()
+    return ids, lg
 
 
 class RefModel:
@@ -75,7 +100,9 @@ GOLDENS = [("tiny_llama2_fp32_shared", False, "llama2", None), ("tiny_llama2_fp3
 @pytest.mark.parametrize("name,quant,flavour,bias", GOLDENS)
 def test_golden_logits(kllm_lib, oracle, name, quant, flavour, bias):
     g = np.load(GOLDEN / f"{name}.npz")
-    dec, shape = load_decoder(GOLDEN / f"{name}.bin", quant, flavour, bias)
+    dec, shape = load_decoder(GOLDEN / f"{name}.bin", quant, flavour, bias, refusable=True)
+    if dec is None:
+        return  # persistent engine: refused loudly, as make_decoder checked
     om = oracle.open_model(GOLDEN / f"{name}.bin", quant, "qwen2file" if bias else flavour)
     for t, tok in enumerate(g["tokens"]):
         nxt = dec.step(int(tok), t)
@@ -95,14 +122,18 @@ def test_golden_logits(kllm_lib, oracle, name, quant, flavour, bias):
                                         ("tiny_llama2_int8", True)])
 def test_bit_exact_vs_reference_cuda_model_goldens(kllm_lib, ref, name, quant):
     g = np.load(GOLDEN / f"{name}.npz")
-    dec, shape = load_decoder(GOLDEN / f"{name}.bin", quant)
-    rm = RefModel(ref, GOLDEN / f"{name}.bin", quant, shape.vocab_size)
+    dec, shape = load_decoder(GOLDEN / f"{name}.bin", quant, refusable=True)
+    if dec is None:
+        return  # persistent engine: refused loudly, as make_decoder checked
+    rm = RefModel(ref, GOLDEN / f"{name}.bin", quant, shape.vocab_size) if ref.live else None
     for t, tok in enumerate(g["tokens"]):
         nxt = dec.step(int(tok), t)
-        r_next, r_logits = rm.step(int(tok), t)
-        assert_bit_equal(dec.logits(), r_logits, f"{name} logits pos {t}")
-        assert nxt == r_next
-    rm.close(); dec.close()
+        r_next, r_logits = rm.step(int(tok), t) if rm else (None, None)
+        ref.bits(f"model/{name}/logits/{t}", dec.logits(), r_logits, f"{name} logits pos {t}")
+        ref.ids(f"model/{name}/next/{t}", [nxt], [r_next] if rm else None)
+    if rm:
+        rm.close()
+    dec.close()
 
 
 def _synth_file(tmp_path, key, seed):
@@ -122,22 +153,20 @@ def test_free_running_decode_identical_to_reference_cuda(kllm_lib, ref, tmp_path
     reference's CUDA path (demo/main.cpp loop), every position up to seq_len."""
     from kuiperllama_b200 import Decoder
     shape, w, path = _synth_file(tmp_path, key, 100 + steps)
-    dec = make_decoder(shape, w)
-    rm = RefModel(ref, path, shape.group_size > 0, shape.vocab_size)
+    dec = make_decoder(shape, w, refusable=True)
+    if dec is None:
+        return  # persistent engine: refused loudly, as make_decoder checked
+    theirs, lg = ref_decode(ref, path, shape.group_size > 0, shape.vocab_size, steps)
     mine = dec.generate(1, 0, steps)
-    tok, theirs = 1, []
-    for pos in range(steps):
-        tok, lg = rm.step(tok, pos, want_logits=(pos == steps - 1))
-        theirs.append(tok)
-    assert mine == theirs
-    assert_bit_equal(dec.logits(), lg, f"{key}: logits after {steps} free-running steps")
+    ref.ids(f"decode/{key}/{steps}/ids", mine, theirs)
+    ref.bits(f"decode/{key}/{steps}/logits", dec.logits(), lg, f"{key}: logits after {steps} free-running steps")
     # the host-buffer path (predict semantics) walks the same sequence
     tok = 1
     for pos in range(8):
         tok = dec.step(tok, pos)
-        assert tok == theirs[pos]
+        assert tok == mine[pos]
     assert dec.step(5, 3, is_prompt=True) == -1  # predict(..., is_prompt=true) returns -1
-    rm.close(); dec.close()
+    dec.close()
 
 
 @pytest.mark.parametrize("qkey", ["tiny-qwen", "small-qwen"])
@@ -192,16 +221,11 @@ def test_tinyllama_full_size_identical_to_reference_cuda(kllm_lib, ref, tmp_path
         write_checkpoint(path, shape, w)
         dec = make_decoder(shape, w)
         assert dec.engine == engine
-        rm = RefModel(ref, path, False, shape.vocab_size)
         steps = 256
+        theirs, lg = ref_decode(ref, path, False, shape.vocab_size, steps)
         mine = dec.generate(1, 0, steps)
-        tok, theirs = 1, []
-        for pos in range(steps):
-            tok, lg = rm.step(tok, pos, want_logits=(pos == steps - 1))
-            theirs.append(tok)
-        assert mine == theirs
-        assert_bit_equal(dec.logits(), lg, "TinyLlama-1.1B logits after 256 steps")
-        rm.close()
+        ref.ids("decode/tinyllama-1.1b/256/ids", mine, theirs)
+        ref.bits("decode/tinyllama-1.1b/256/logits", dec.logits(), lg, "TinyLlama-1.1B logits after 256 steps")
     finally:
         if os.path.exists(path):
             os.remove(path)
@@ -296,18 +320,12 @@ def test_llama2_7b_int8_full_size_identical_to_reference_cuda(kllm_lib, ref, eng
     shape = case["shape"]
     steps = 128
     if "ref_ids" not in case:
-        rm = RefModel(ref, case["path"], True, shape.vocab_size)
-        tok, theirs = 1, []
-        for pos in range(steps):
-            tok, lg = rm.step(tok, pos, want_logits=(pos == steps - 1))
-            theirs.append(tok)
-        rm.close()
-        case["ref_ids"], case["ref_logits"] = theirs, lg
+        case["ref_ids"], case["ref_logits"] = ref_decode(ref, case["path"], True, shape.vocab_size, steps)
     dec = make_decoder(shape, case["w"])
     assert dec.engine == engine
     mine = dec.generate(1, 0, steps)
-    assert mine == case["ref_ids"]
-    assert_bit_equal(dec.logits(), case["ref_logits"], "Llama-2-7B int8 logits after 128 steps")
+    ref.ids("decode/llama2-7b-int8/128/ids", mine, case["ref_ids"])
+    ref.bits("decode/llama2-7b-int8/128/logits", dec.logits(), case["ref_logits"], "Llama-2-7B int8 logits after 128 steps")
     # host-buffer path (predict semantics) at a late position reproduces the same id
     assert dec.step(mine[steps - 2], steps - 1) == mine[steps - 1]
     dec.close()

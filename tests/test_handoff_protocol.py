@@ -4,7 +4,7 @@
 The kernel replaces grid barriers by tagged 64-bit words: a producer publishes {tag, value} with one
 store, a consumer polls until the tag is the one it expects.  Which buffers may be single-slot, which
 need two slots, and why the plain (untagged) residual-stream buffers can be double-buffered without any
-barrier is an argument about ALL interleavings of 148 CTAs (x N ranks); a GPU test only ever sees a
+barrier is an argument about ALL interleavings of 132 CTAs (x N ranks); a GPU test only ever sees a
 few of them.  This test restates the protocol at the level of individual memory operations and runs it
 under randomised, adversarial schedulers:
 

@@ -1,10 +1,10 @@
-"""-m gpu: the tcgen05 prompt GEMM (kllm_gemm_tf32) -- an explicitly TOLERANCED kernel.
+"""-m gpu: the wgmma prompt GEMM (kllm_gemm_tf32) -- an explicitly TOLERANCED kernel.
 
 out[T, N] = x[T, K] . w[N, K]^T with TF32 operands (10 mantissa bits each) and fp32 accumulation in
-TMEM.  Tolerance, stated: per element |out - exact| <= 4e-3 * sqrt(K) * rms(x row) * rms(w row).
-kind::tf32 TRUNCATES both fp32 operands to 10 mantissa bits (relative error up to 2^-10 each, same
-sign), so an element -- a sum of K such products -- is off by about 6e-4 * sqrt(K) * rms * rms (one
-sigma, measured); the bound is ~6 sigma."""
+registers.  Tolerance, stated: per element |out - exact| <= 4e-3 * sqrt(K) * rms(x row) * rms(w row).
+The kernel rounds both fp32 operands to the nearest tf32 (10 mantissa bits, relative error up to 2^-11
+each) before the MMA, so an element -- a sum of K such products -- is off by a few 1e-4 * sqrt(K) * rms * rms;
+the bound leaves a wide margin over that."""
 import ctypes
 
 import numpy as np
@@ -49,10 +49,10 @@ def test_gemm_tf32_rejects_unaligned(kllm_lib):
 @pytest.mark.parametrize("engine", ["persistent", "graph"])
 @pytest.mark.parametrize("key,n_prompt", [("small", 70), ("small-qwen", 40), ("tinyllama-1.1b", 300)])
 def test_batched_prefill_matches_stepping_within_tf32_tolerance(kllm_lib, monkeypatch, engine, key, n_prompt):
-    """kllm_decoder_prefill_tf32 (tcgen05 GEMMs over the whole prompt) against the bit-exact
+    """kllm_decoder_prefill_tf32 (wgmma GEMMs over the whole prompt) against the bit-exact
     position-by-position prompt path on the same decoder engine.  Stated tolerance: K / V cache rows
-    within 5e-2 * (row rms + 1e-3) per element (the TF32 truncation errors of every earlier layer ride
-    on the residual stream: 2.4e-2 measured at the last of TinyLlama's 22 layers), final logits within 2e-2 * max|logit| of the exact
+    within 5e-2 * (row rms + 1e-3) per element (the TF32 rounding errors of every earlier layer ride
+    on the residual stream), final logits within 2e-2 * max|logit| of the exact
     ones, the same greedy id when the exact top-2 margin exceeds that bound -- and decoding can go on
     from the prefilled cache (16 teacher-forced steps stay within the same logit tolerance)."""
     from kuiperllama_b200 import SHAPES, Decoder, synth_weights

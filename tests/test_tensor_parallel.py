@@ -3,7 +3,7 @@
 not gpu: the sharding arithmetic, and a world_size-2 (and 4) gloo run in which every process
          decodes with ITS shard through the oracle's ops and the partial sums meet in
          dist.all_reduce -- logits <= 1e-4 from the unsharded oracle model, identical greedy ids.
-gpu (needs >= 2 GPUs, run with `gpurun --gpus 2`): kllm_comm all-reduce (peer memory and NCCL)
+gpu (needs >= 2 GPUs): kllm_comm all-reduce (peer memory and NCCL)
          against a host-side sum, 2000 calls back to back; the sharded CUDA decoder against the
          unsharded oracle; peer and NCCL transports agree bit for bit on token ids.
 """
@@ -123,7 +123,7 @@ def test_gloo_tensor_parallel_decode_matches_unsharded_oracle(oracle, tmp_path, 
 def _need_gpus(n):
     import torch
     if torch.cuda.device_count() < n:
-        pytest.skip(f"needs {n} GPUs (run under `gpurun --gpus {n}`)")
+        pytest.skip(f"needs {n} GPUs")
 
 
 def _comm_rank(rank, world, backend, out_dir):

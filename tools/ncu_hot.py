@@ -2,7 +2,7 @@
 """Hot-loop view of an `ncu --set full --import-source on` capture: per SASS instruction the executed
 count and the warp-stall samples by reason, for the N most-sampled instructions plus kernel totals.
 
-    python tools/ncu_hot.py gpurun_out/x.ncu-rep [N] > profiles/rNN_x_hot.txt
+    python tools/ncu_hot.py x.ncu-rep [N] > profiles/rNN_x_hot.txt
 """
 import collections
 import csv

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Summarise ncu outputs brought back in gpurun_out/ into small text files under profiles/.
+"""Summarise ncu outputs into small text files under profiles/.
 
-  python tools/ncu_summarize.py launches gpurun_out/launches_X.csv profiles/rNN_launches.txt
-  python tools/ncu_summarize.py full     gpurun_out/prof_X.ncu-rep profiles/rNN_kernel.txt
+  python tools/ncu_summarize.py launches launches_X.csv profiles/rNN_launches.txt
+  python tools/ncu_summarize.py full     prof_X.ncu-rep profiles/rNN_kernel.txt
 """
 import collections
 import csv

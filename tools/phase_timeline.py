@@ -49,7 +49,7 @@ def main():
     bar = (st[:, :, 3] - st[:, :, 2])            # waiting at the grid barrier
     dur = st[:, :, 3].max(axis=0) - st[:, :, 0].min(axis=0)
     poll = polled - st[:, :, 0]                  # of stage_x: until the input vector is complete
-    ghz = 1.965  # cycles -> us at the B200's boost clock (clocks.max.sm); the split is what matters
+    ghz = 1.98  # cycles -> us at the H100 SXM's boost clock (clocks.max.sm); the split is what matters
     print(f"{'phase':>10} {'count':>5} {'phase_us':>9} {'stage_x':>8} {'(poll)':>7} {'work_med':>9} {'work_max':>9} {'barrier_min':>11} "
           f"{'barrier_med':>11} | warp 0 of the median CTA, us: {'ringwait':>8} {'dots':>6} {'reduce':>6} {'epilog':>6} {'addend':>6}")
 

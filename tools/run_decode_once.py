@@ -6,7 +6,7 @@ The persistent engine decodes `--start` positions in launch #1 (unprofiled conte
 length you asked for (ncu replays a kernel ~40 times, so keep --steps small):
 
     ncu --set full --clock-control none --import-source on -k regex:decode_megakernel \
-        --launch-skip 1 -c 1 -o gpurun_out/mega python tools/run_decode_once.py --steps 8 --start 504
+        --launch-skip 1 -c 1 -o mega python tools/run_decode_once.py --steps 8 --start 504
 
 (without --launch-skip the capture is launch #1: --start tokens, bytes per token = total / start.)
 """

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Instruction histogram of the kernels in libkllm_b200.so (cuobjdump -sass), per kernel: total
-instructions and the mnemonics that prove which hardware paths are used (TMA bulk copies, tcgen05,
-TMEM, mbarriers, dp4a, ...).
+instructions and the mnemonics that prove which hardware paths are used (TMA bulk copies, wgmma,
+mbarriers, dp4a, ...).
 
     python tools/sass_histogram.py > profiles/r02_sass_histogram.txt
 """
@@ -30,7 +30,7 @@ def main():
         if m and cur is not None:
             cur[m.group(1)] += 1
     demangle = subprocess.run(["c++filt"], input="\n".join(kernels), capture_output=True, text=True).stdout.splitlines()
-    print(f"# {LIB.name}: SASS instruction histogram per kernel (sm_100a, cuobjdump -sass); mnemonic families summed over suffixes")
+    print(f"# {LIB.name}: SASS instruction histogram per kernel (sm_90a, cuobjdump -sass); mnemonic families summed over suffixes")
     for (mangled, cnt), name in zip(kernels.items(), demangle):
         fam = collections.Counter()
         for op, n in cnt.items():
