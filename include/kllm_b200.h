@@ -138,6 +138,18 @@ int kllm_gemv_fused(const kllm_gemv_job* job, void* stream);
  * bit for bit: the decode path never uses it.  in_dim % 4 == 0, 16-byte aligned x and w. */
 int kllm_gemm_tf32(const float* x, const float* w, float* out, int n_tokens, int in_dim, int out_dim,
                    void* stream);
+/* The same GEMM for int8 group-quantised weights (export.py --version 3):
+ *   out[n_tokens, out_dim] = x[n_tokens, in_dim] . (s (.) w)[out_dim, in_dim]^T,
+ *   s[n, k] = scales[(n * in_dim + k) / group_size]  -- the weight kllm_gemv_w8 dequantises.
+ * x, out fp32; w int8 row-major; scales fp32; all device memory.  The weight tile is dequantised in
+ * shared memory (scale * w in fp32, rounded to the nearest tf32) and multiplied on the same wgmma
+ * tf32 path, so the error is that of kllm_gemm_tf32: per element within
+ * 4e-3 * sqrt(in_dim) * rms(x row) * rms(dequantised w row) of the exact product
+ * (tests/test_prefill_int8_gpu.py).  KLLM_E_INVALID for NULL pointers or non-positive sizes;
+ * KLLM_E_UNSUPPORTED unless in_dim % 16 == 0, in_dim % group_size == 0, group_size % 32 == 0 and
+ * x, w are 16-byte aligned. */
+int kllm_gemm_w8_tf32(const float* x, const int8_t* w, const float* scales, float* out, int n_tokens, int in_dim,
+                      int out_dim, int group_size, void* stream);
 
 /* ---- tensor-parallel exchange --------------------------------------------------------------
  * Not in the reference (single GPU: llama3.cpp:118 pins device 0); SURVEY.md section 8e.  One
@@ -247,6 +259,14 @@ int kllm_decoder_prompt(kllm_decoder* dec, const int32_t* tokens_host, int32_t n
  * mantissa bits).  fp32 checkpoints on one GPU; KLLM_E_UNSUPPORTED otherwise (use kllm_decoder_prompt). */
 int kllm_decoder_prefill_tf32(kllm_decoder* dec, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
                               int32_t* next_host);
+/* The batched prefill for int8 checkpoints: the contract and the tolerance of kllm_decoder_prefill_tf32
+ * (KV-cache rows within 5e-2 * (row rms + 1e-3), last logits within 2e-2 * max|logit| of the
+ * position-by-position path; tests/test_prefill_int8_gpu.py), each projection one kllm_gemm_w8_tf32.
+ * int8 checkpoints on one GPU whose projections the GEMM accepts (dim, hidden_dim % 16 == 0, both
+ * multiples of group_size, group_size % 32 == 0); KLLM_E_UNSUPPORTED otherwise -- fp32 checkpoints
+ * take kllm_decoder_prefill_tf32, anything else kllm_decoder_prompt. */
+int kllm_decoder_prefill_w8(kllm_decoder* dec, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
+                            int32_t* next_host);
 /* Device-resident greedy loop: positions start_pos .. start_pos+n_steps-1, each step feeding
  * the previous argmax back without leaving the GPU; ids copied to out_tokens_host at the end
  * (one synchronisation).  teacher_host (optional, n_steps ids) forces the inputs instead. */

@@ -49,6 +49,9 @@ struct PrefillModel {
   const float* const* ffn_norm;
   const void* const* wq; const void* const* wk; const void* const* wv; const void* const* wo;
   const void* const* w1; const void* const* w2; const void* const* w3;
+  int group_size;  // 0: fp32 weights (kllm_gemm_tf32); > 0: int8 weights + scales (kllm_gemm_w8_tf32)
+  const float* const* sq; const float* const* sk; const float* const* sv; const float* const* so;
+  const float* const* s1; const float* const* s2; const float* const* s3;
   const float* const* bq; const float* const* bk; const float* const* bv;
   float* key_cache; float* value_cache;
   const float* sin_cache; const float* cos_cache;

@@ -1,5 +1,7 @@
 // Batched GEMM for prompt prefill on the Hopper tensor cores (sm_90a):
 //     out[T, N] = x[T, K] . w[N, K]^T        fp32 storage, TF32 multiply, fp32 accumulate in registers
+// for fp32 weights (kllm_gemm_tf32) and for int8 group-quantised weights (kllm_gemm_w8_tf32), where
+// w[n, k] = scales[(n K + k) / group_size] * q[n, k] is dequantised into the shared-memory tile.
 //
 // The reference feeds a prompt through one full single-token forward per position (demo/main.cpp:
 // 18-23, llama3.cpp:147-167) -- T GEMVs that stream every weight T times.  With the T prompt rows
@@ -17,6 +19,14 @@
 //                  operands from shared memory, accumulators in registers (SASS: HGMMA); a stage is
 //                  released once the wgmma group after it has been issued and the one reading it retired
 //   epilogue       each consumer thread stores its accumulator fragment straight to out
+//
+// int8 weights (template parameter W8): the producer loads the weight tile as bytes [128 x 32 int8] into
+// a 4 KB staging area of the stage; each consumer warpgroup dequantises its 64 rows (scale * q in fp32,
+// rounded to the nearest tf32) into the same 128-byte-swizzled fp32 A tile TMA would have written, so the
+// wgmma descriptors and instructions are the fp32 path's.  The scale of a row is constant over a 32-column
+// K block (group_size % 32 == 0, in_dim % group_size == 0) and is read with an ordinary non-coherent load
+// one K block ahead: scale rows can be 4 bytes, which TMA cannot copy.  A stage is dequantised while the
+// wgmma group of the stage before it is still running.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -33,6 +43,7 @@ constexpr int BK = 32;      // fp32 elements per K block = 128 bytes = one swizz
 constexpr int WG_K = 8;     // tf32: 32 bytes of K per wgmma
 constexpr int STAGES = 4;
 constexpr int A_BYTES = BM * BK * 4;  // 16 KB
+constexpr int W8_BYTES = BM * BK;     // 4 KB: the int8 weight tile as loaded, rows of 32 bytes
 constexpr int THREADS = 384;
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) {
@@ -165,16 +176,38 @@ __device__ __forceinline__ void round_tf32(float4* p, int n, int t) {
   }
 }
 
-template <int BN>
+// Thread (r, half) of a consumer warpgroup turns the 16 int8 weights of columns 16 half .. + 15 of its local
+// row r into scale * q rounded to the nearest tf32, and stores them as four 16-byte chunks of the row in the
+// 128-byte swizzle TMA uses: chunk c of row r lives at r * 128 + (c ^ (r & 7)) * 16.
+__device__ __forceinline__ void dequant_w8(const uint8_t* src, uint8_t* a_rows, int r, int half, float scale) {
+  const int4 q = *reinterpret_cast<const int4*>(src);
+  const int words[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float e[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float v = scale * static_cast<float>(static_cast<int8_t>((words[j] >> (8 * i)) & 0xff));
+      uint32_t u;
+      asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
+      e[i] = __uint_as_float(u);
+    }
+    const int c = 4 * half + j;
+    *reinterpret_cast<float4*>(a_rows + r * 128 + ((c ^ (r & 7)) << 4)) = make_float4(e[0], e[1], e[2], e[3]);
+  }
+}
+
+template <int BN, bool W8>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x,
-                 float* __restrict__ out, int T, int N, int K) {
+                 float* __restrict__ out, const float* __restrict__ scales, int T, int N, int K, int group_size) {
   constexpr int B_BYTES = BN * BK * 4;
   extern __shared__ uint8_t raw_smem[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* a_tiles = base;
   uint8_t* b_tiles = base + STAGES * A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(b_tiles + STAGES * B_BYTES);
+  uint8_t* w8_tiles = b_tiles + STAGES * B_BYTES;  // W8 only
+  uint64_t* bars = reinterpret_cast<uint64_t*>(w8_tiles + (W8 ? STAGES * W8_BYTES : 0));
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
 
@@ -199,8 +232,9 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
         const uint32_t ph = (kb / STAGES) & 1;
         mbar_wait(smem_addr(&empty[s]), ph ^ 1u);
         const uint32_t bar = smem_addr(&full[s]);
-        mbar_expect_tx(bar, A_BYTES + B_BYTES);  // out-of-range rows / columns are zero-filled and still counted
-        tma_load_2d(smem_addr(a_tiles + s * A_BYTES), &map_w, bar, kb * BK, n0);
+        // out-of-range rows / columns are zero-filled and still counted
+        mbar_expect_tx(bar, (W8 ? W8_BYTES : A_BYTES) + B_BYTES);
+        tma_load_2d(smem_addr(W8 ? w8_tiles + s * W8_BYTES : a_tiles + s * A_BYTES), &map_w, bar, kb * BK, n0);
         tma_load_2d(smem_addr(b_tiles + s * B_BYTES), &map_x, bar, kb * BK, t0);
       }
     }
@@ -211,13 +245,25 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
   const uint32_t a_off = static_cast<uint32_t>(wg - 1) * 64 * BK * 4;  // 8 KB: a multiple of the 1024-byte atom
+  // W8: thread t dequantises 16 weights of local row t / 2; the row's scale for K block kb is one float
+  const int dq_row = t >> 1, dq_half = t & 1;
+  const int w_row = n0 + (wg - 1) * 64 + dq_row;
+  const float* srow = (W8 && w_row < N) ? scales + static_cast<size_t>(w_row) * (K / group_size) : nullptr;
+  auto scale_at = [&](int kb) { return srow != nullptr ? __ldg(srow + kb * BK / group_size) : 0.f; };
+  float sc = W8 ? scale_at(0) : 0.f;
   for (int kb = 0; kb < kblocks; ++kb) {
     const int s = kb % STAGES;
+    const float sc_next = (W8 && kb + 1 < kblocks) ? scale_at(kb + 1) : 0.f;
     mbar_wait(smem_addr(&full[s]), (kb / STAGES) & 1);
     // The tensor core truncates fp32 operands to tf32; round them to the nearest tf32 in place first, which halves
-    // the per-operand error.  Each warpgroup rounds its own 64 weight rows and half of the token rows, which
-    // both read, so the two meet at a named barrier before the wgmma (async proxy) reads the tiles.
-    round_tf32(reinterpret_cast<float4*>(a_tiles + s * A_BYTES + a_off), 64 * BK / 4, t);
+    // the per-operand error.  Each warpgroup rounds (or, for int8 weights, dequantises) its own 64 weight rows and
+    // half of the token rows, which both read, so the two meet at a named barrier before the wgmma (async proxy)
+    // reads the tiles.
+    if constexpr (W8)
+      dequant_w8(w8_tiles + s * W8_BYTES + ((wg - 1) * 64 + dq_row) * BK + dq_half * 16, a_tiles + s * A_BYTES + a_off,
+                 dq_row, dq_half, sc);
+    else
+      round_tf32(reinterpret_cast<float4*>(a_tiles + s * A_BYTES + a_off), 64 * BK / 4, t);
     round_tf32(reinterpret_cast<float4*>(b_tiles + s * B_BYTES + (wg - 1) * (B_BYTES / 2)), BN * BK / 8, t);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -231,6 +277,7 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
     // the group of stage kb - 1 has retired: its tiles may be refilled
     asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
     if (kb > 0 && t == 0) mbar_arrive(smem_addr(&empty[(kb - 1) % STAGES]));
+    sc = sc_next;
   }
   asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 
@@ -262,37 +309,50 @@ static EncodeTiledFn encode_tiled() {
   }();
   return fn;
 }
-// 2-D fp32 tensor [rows, cols] (row-major, cols contiguous), box [box_rows x 32 columns], 128-byte swizzle
-static int make_map(CUtensorMap* map, const float* ptr, int rows, int cols, int box_rows) {
+// 2-D tensor [rows, cols] (row-major, cols contiguous) of fp32 (128-byte swizzle) or int8 (no swizzle: the
+// consumers read it back row by row), box [box_rows x 32 columns]
+static int make_map(CUtensorMap* map, const void* ptr, bool int8, int rows, int cols, int box_rows) {
   EncodeTiledFn fn = encode_tiled();
   if (fn == nullptr) return KLLM_E_NODEVICE;
   const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * 4};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * (int8 ? 1 : 4)};
   const cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>(box_rows)};
   const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult r = fn(map, int8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+                        const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        int8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : KLLM_E_INVALID;
 }
 
-template <int BN>
-static int launch(const float* x, const float* w, float* out, int T, int K, int N, cudaStream_t stream) {
+template <int BN, bool W8>
+static int launch(const float* x, const void* w, const float* scales, float* out, int T, int K, int N, int group_size,
+                  cudaStream_t stream) {
   CUtensorMap map_w, map_x;
-  if (int rc = make_map(&map_w, w, N, K, BM)) return rc;
-  if (int rc = make_map(&map_x, x, T, K, BN)) return rc;
-  const size_t smem = 1024 + static_cast<size_t>(STAGES) * (A_BYTES + BN * BK * 4) + 128;
+  if (int rc = make_map(&map_w, w, W8, N, K, BM)) return rc;
+  if (int rc = make_map(&map_x, x, false, T, K, BN)) return rc;
+  const size_t smem = 1024 + static_cast<size_t>(STAGES) * (A_BYTES + BN * BK * 4 + (W8 ? W8_BYTES : 0)) + 128;
   static bool configured = false;
   if (!configured) {
-    const cudaError_t e = cudaFuncSetAttribute(gemm_tf32_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    const cudaError_t e = cudaFuncSetAttribute(gemm_tf32_kernel<BN, W8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                static_cast<int>(smem));
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
   const dim3 grid((N + BM - 1) / BM, (T + BN - 1) / BN);
-  gemm_tf32_kernel<BN><<<grid, THREADS, smem, stream>>>(map_w, map_x, out, T, N, K);
+  gemm_tf32_kernel<BN, W8><<<grid, THREADS, smem, stream>>>(map_w, map_x, out, scales, T, N, K, group_size);
   count_launch();
   return static_cast<int>(cudaGetLastError());
+}
+
+// token-block width: the smallest wgmma N that covers the tokens, 256 at most
+template <bool W8>
+static int dispatch(const float* x, const void* w, const float* scales, float* out, int T, int K, int N, int group_size,
+                    cudaStream_t s) {
+  if (T <= 32) return launch<32, W8>(x, w, scales, out, T, K, N, group_size, s);
+  if (T <= 64) return launch<64, W8>(x, w, scales, out, T, K, N, group_size, s);
+  if (T <= 128) return launch<128, W8>(x, w, scales, out, T, K, N, group_size, s);
+  return launch<256, W8>(x, w, scales, out, T, K, N, group_size, s);
 }
 
 }  // namespace tc
@@ -303,10 +363,18 @@ extern "C" int kllm_gemm_tf32(const float* x, const float* w, float* out, int n_
   if (!x || !w || !out || n_tokens <= 0 || in_dim <= 0 || out_dim <= 0) return KLLM_E_INVALID;
   // TMA needs 16-byte aligned bases and row pitches
   if ((in_dim & 3) || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(w) & 15)) return KLLM_E_UNSUPPORTED;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  using namespace kllm::tc;
-  if (n_tokens <= 32) return launch<32>(x, w, out, n_tokens, in_dim, out_dim, s);
-  if (n_tokens <= 64) return launch<64>(x, w, out, n_tokens, in_dim, out_dim, s);
-  if (n_tokens <= 128) return launch<128>(x, w, out, n_tokens, in_dim, out_dim, s);
-  return launch<256>(x, w, out, n_tokens, in_dim, out_dim, s);
+  return kllm::tc::dispatch<false>(x, w, nullptr, out, n_tokens, in_dim, out_dim, 0, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int kllm_gemm_w8_tf32(const float* x, const int8_t* w, const float* scales, float* out, int n_tokens,
+                                 int in_dim, int out_dim, int group_size, void* stream) {
+  if (!x || !w || !scales || !out || n_tokens <= 0 || in_dim <= 0 || out_dim <= 0 || group_size <= 0)
+    return KLLM_E_INVALID;
+  // TMA needs 16-byte aligned bases and row pitches (in_dim bytes for the int8 rows); one scale per row and
+  // 32-column K block needs whole groups per row and whole K blocks per group
+  if ((in_dim % 16) || (in_dim % group_size) || (group_size % 32) || (reinterpret_cast<uintptr_t>(x) & 15) ||
+      (reinterpret_cast<uintptr_t>(w) & 15))
+    return KLLM_E_UNSUPPORTED;
+  return kllm::tc::dispatch<true>(x, w, scales, out, n_tokens, in_dim, out_dim, group_size,
+                                  static_cast<cudaStream_t>(stream));
 }

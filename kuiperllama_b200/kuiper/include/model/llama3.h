@@ -10,6 +10,10 @@
 //       launch per op) for callers that hand in activations of their own; its named buffers and
 //       KV cache are created on first use.
 // A sequence must stay on one of the two paths (each has its own KV cache).
+//
+// Opt-in batched prompt prefill (set_batched_prefill / KUIPER_BATCHED_PREFILL=1): the first prompt row
+// predict() gets runs every prompt position but the last through the decoder's batched tensor-core prefill
+// (kllm_decoder_prefill_w8 / _tf32, TF32 tolerance), and the later prompt rows return at once.
 #ifndef KLLM_KUIPER_MODEL_LLAMA3_H_
 #define KLLM_KUIPER_MODEL_LLAMA3_H_
 #include <base/cuda_config.h>
@@ -68,6 +72,18 @@ class LLama2Model : public Model {
   const TpConfig& tensor_parallel() const { return tp_; }
   const TpShard& tensor_parallel_shard() const { return shard_; }
 
+  // Batched prompt prefill under predict(): call before init(); without a call init() takes it from
+  // KUIPER_BATCHED_PREFILL=1, so the reference's unchanged demos can opt in.  Off by default: every
+  // prompt position is then one full single-token forward, bit-identical to the reference.  When on,
+  // predict(row pos of the latest embedding() of n >= 3 tokens, pos, is_prompt = true), with the decoder
+  // holding rows [0, pos) of the sequence, fills positions pos .. n - 2 in one batched prefill (the rows
+  // whose logits a prompt throws away; int8 checkpoints through kllm_decoder_prefill_w8, fp32 through
+  // kllm_decoder_prefill_tf32; KV rows within their stated TF32 tolerance, include/kllm_b200.h), and
+  // the prompt calls for those positions then return next = -1 without running.  The last prompt row and
+  // every later position step as before.  Single GPU: init() refuses it under tensor parallelism.
+  void set_batched_prefill(bool on);
+  bool batched_prefill() const { return batched_prefill_; }
+
  protected:
   // qkv_bias: the checkpoint carries a bias vector behind each layer's wq / wk / wv (Qwen2 files)
   LLama2Model(base::TokenizerType tokenizer_type, std::string token_path, std::string model_path,
@@ -107,6 +123,17 @@ class LLama2Model : public Model {
   mutable int32_t decoder_rows_ = 0;
   mutable int32_t layer_rows_ = 0;
   base::Status sync_layer_cache(int32_t pos) const;
+
+  // batched prompt prefill: the switch, and which positions [prefilled_from_, prefilled_to_) of which
+  // embedding() call (embedding_calls_ counts them) the decoder's cache holds from it
+  bool batched_prefill_ = false;
+  bool batched_prefill_explicit_ = false;
+  mutable uint64_t embedding_calls_ = 0;
+  mutable uint64_t prefilled_embedding_ = 0;
+  mutable int32_t prefilled_from_ = 0, prefilled_to_ = 0;
+  // predict() on row `pos` of the latest embedding(): true when the batched prefill has filled (or has just
+  // filled) position pos, so there is nothing left to run
+  base::Status prefill_prompt_rows(int32_t pos, bool* done) const;
 
   // tensor parallel state: who we are, what we own, the exchange and the start-up rendezvous; the host
   // staging buffers of the repacked column shards live until init_mem() has uploaded them

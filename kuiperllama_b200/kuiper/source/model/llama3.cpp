@@ -18,6 +18,7 @@
 #include <kllm_b200.h>
 #include <op/decoder_layers.h>
 
+#include <cstdlib>
 #include <cstring>
 #include <utility>
 
@@ -69,6 +70,11 @@ void LLama2Model::set_tensor_parallel(const TpConfig& config) {
   tp_explicit_ = true;
 }
 
+void LLama2Model::set_batched_prefill(bool on) {
+  batched_prefill_ = on;
+  batched_prefill_explicit_ = true;
+}
+
 const char* LLama2Model::decoder_engine() const { return decoder_ ? kllm_decoder_engine(decoder_) : ""; }
 
 base::Status LLama2Model::init(base::DeviceType device_type) {
@@ -81,6 +87,14 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   device_type_ = device_type;
   if (!tp_explicit_) tp_ = TpConfig::from_env();  // tools/kuiper_tp_launch: one process per GPU
   if (tp_.rank < 0 || tp_.rank >= tp_.world) return error::InvalidArgument("tensor parallel: rank outside the world");
+  if (!batched_prefill_explicit_) {
+    const char* env = std::getenv("KUIPER_BATCHED_PREFILL");
+    batched_prefill_ = env != nullptr && std::string(env) == "1";
+  }
+  if (batched_prefill_ && tp_.on())
+    return error::InvalidArgument(
+        "batched prompt prefill is single-GPU: turn it off (KUIPER_BATCHED_PREFILL / set_batched_prefill) under "
+        "tensor parallelism");
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
     return error::InternalError("No usable CUDA device " + std::to_string(tp_.cuda_device()) + ".");
   cuda_config_ = std::make_shared<kernel::CudaConfig>();
@@ -462,6 +476,10 @@ base::Status LLama2Model::create_decoder() {
     return base::error::InternalError(std::string("kllm_decoder_create failed: ") + kllm_error_string(rc));
   LOG(INFO) << "fused decoder engine: " << kllm_decoder_engine(decoder_) << ", "
             << kllm_decoder_launches_per_step(decoder_) << " launch(es) per token";
+  LOG(INFO) << "prompt prefill: "
+            << (batched_prefill_ ? (is_quant_model_ ? "batched (kllm_decoder_prefill_w8, TF32 tolerance)"
+                                                    : "batched (kllm_decoder_prefill_tf32, TF32 tolerance)")
+                                 : "one forward per position (bit-exact)");
   if (tp_.on()) {
     // every rank has built its engine (and zeroed its exchange area) before anybody's first token
     cudaDeviceSynchronize();
@@ -506,6 +524,7 @@ op::EmbeddingOutput LLama2Model::embedding(const std::vector<int>& tokens) const
   STATUS_CHECK(llama_layers_->embedding_layer_->forward(input_tokens, input_token_num, input_embeddings));
   last_tokens_.assign(tokens.begin(), tokens.end());
   last_embeddings_ = input_embeddings.ptr<float>();
+  ++embedding_calls_;
   return op::EmbeddingOutput(input_tokens, input_embeddings, input_token_num);
 }
 
@@ -524,6 +543,15 @@ base::Status LLama2Model::predict(const tensor::Tensor& input, const tensor::Ten
     const ptrdiff_t row = delta / config_->dim_;
     const bool rows_present = pos <= decoder_rows_ || pos > layer_rows_;  // else only the layer path has them
     if (delta % config_->dim_ == 0 && row < static_cast<ptrdiff_t>(last_tokens_.size()) && rows_present) {
+      if (batched_prefill_ && is_prompt && row == pos) {
+        bool done = false;
+        if (base::Status st = prefill_prompt_rows(pos, &done); !st) return st;
+        if (done) {
+          next = -1;
+          logits_in_decoder_ = true;
+          return base::error::Success();
+        }
+      }
       int32_t nxt = -1;
       const int rc = kllm_decoder_step(decoder_, last_tokens_[row], pos, is_prompt ? 1 : 0, &nxt);
       if (rc != 0) return base::error::InternalError(std::string("kllm_decoder_step: ") + kllm_error_string(rc));
@@ -540,6 +568,34 @@ base::Status LLama2Model::predict(const tensor::Tensor& input, const tensor::Ten
   base::Status st = forward(input, pos_tensor, next);
   if (!st) return st;
   next = post_processing(pos_tensor, is_prompt);
+  return base::error::Success();
+}
+
+// The batched prompt prefill (set_batched_prefill).  A prompt row `pos` of the latest embedding() of n tokens
+// either lies in the range an earlier call of this embedding() prefilled and the decoder still holds (nothing to
+// run), or starts the prompt: the decoder holds rows [0, pos) of the sequence (anything above belongs to an older
+// one), and positions pos .. n - 2 -- whose logits a prompt throws away -- go through one batched prefill.  The
+// last prompt row is predicted with is_prompt = false and steps as usual; any other call falls through to it too.
+base::Status LLama2Model::prefill_prompt_rows(int32_t pos, bool* done) const {
+  *done = false;
+  if (prefilled_embedding_ == embedding_calls_ && pos >= prefilled_from_ && pos < prefilled_to_ &&
+      pos < decoder_rows_) {
+    *done = true;
+    return base::error::Success();
+  }
+  const int32_t n = static_cast<int32_t>(last_tokens_.size());
+  if (n < 3 || pos > n - 2 || pos > decoder_rows_) return base::error::Success();
+  int32_t nxt = -1;
+  const auto entry = is_quant_model_ ? kllm_decoder_prefill_w8 : kllm_decoder_prefill_tf32;
+  const int rc = entry(decoder_, last_tokens_.data() + pos, n - 1 - pos, pos, &nxt);
+  if (rc != 0)
+    return base::error::InternalError(std::string(is_quant_model_ ? "kllm_decoder_prefill_w8: "
+                                                                   : "kllm_decoder_prefill_tf32: ") +
+                                      kllm_error_string(rc));
+  prefilled_embedding_ = embedding_calls_;
+  prefilled_from_ = pos, prefilled_to_ = n - 1;
+  decoder_rows_ = n - 1;
+  *done = true;
   return base::error::Success();
 }
 
