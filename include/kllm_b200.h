@@ -98,6 +98,15 @@ int kllm_argmax_f32(const float* logits, int64_t n, int64_t* out_index, void* st
 /* Convenience with the reference's blocking semantics: returns the index or <0 on error. */
 int64_t kllm_argmax_f32_sync(const float* logits, int64_t n, void* stream);
 
+/* The sampling counterpart of kllm_argmax_f32 (what sampler::ArgmaxSampler calls): the id drawn from
+ * logits[0..n) of position `pos` by the sampling rule of DESIGN.md "Sampling" (temperature, top_k,
+ * Philox4x32-10 Gumbel noise keyed by seed and indexed by (pos, i)).  temperature == 0 is the greedy
+ * argmax; top_k <= 0 or >= n keeps every logit.  The id is a pure function of (logits, temperature,
+ * top_k, seed, pos).  Result to *out_index (device, int64); no synchronisation.  KLLM_E_INVALID for NULL
+ * pointers, n outside [1, 2^31), pos < 0, or a temperature that is negative or not finite. */
+int kllm_sample_f32(const float* logits, int64_t n, float temperature, int32_t top_k, uint64_t seed, int32_t pos,
+                    int64_t* out_index, void* stream);
+
 /* ---- fused per-layer entry points -------------------------------------------------------
  * What LLama2Model::forward (llama3.cpp:147-167) calls instead of 15 launches per layer.
  * All are compositions of the ops above with identical arithmetic.                          */
@@ -273,6 +282,15 @@ int kllm_decoder_prefill_w8(kllm_decoder* dec, const int32_t* tokens_host, int32
 int kllm_decoder_generate(kllm_decoder* dec, int32_t first_token, int32_t start_pos,
                           int32_t n_steps, const int32_t* teacher_host,
                           int32_t* out_tokens_host);
+
+/* Sampling instead of the greedy id, from this call on, for every id the decoder returns: kllm_decoder_step
+ * (non-prompt), _prompt, _prefill_tf32 / _w8 and _generate, including the ids generate feeds back on the
+ * device.  Each id is the rule of kllm_sample_f32 applied to the logits of the position just processed,
+ * with that position as `pos`: the same seed gives the same ids on either engine and on every
+ * tensor-parallel rank.  temperature 0 restores the exact greedy behaviour (a new decoder is greedy).
+ * The parameters live in device memory: no engine or graph is rebuilt.  Synchronises the decoder's
+ * stream.  KLLM_E_INVALID for a temperature that is negative or not finite. */
+int kllm_decoder_set_sampling(kllm_decoder* dec, float temperature, int32_t top_k, uint64_t seed);
 
 /* Blocking copies for tests: logits of the last step [vocab]; the KV cache in the REFERENCE
  * layout [layer][seq_len][kv_dim] (llama3.cpp:469-475) whatever the engine keeps internally. */

@@ -7,11 +7,13 @@
 #include <cuda_runtime.h>
 
 #include <cfloat>
+#include <cmath>
 #include <cstdint>
 
 #include "../../include/kllm_b200.h"
 #include "kllm_device.cuh"
 #include "kllm_host.h"
+#include "sampling.cuh"
 
 namespace kllm {
 
@@ -251,6 +253,16 @@ int launch_rope(int flavour, int dim, int kv_dim, int head_size, float* q, float
   return static_cast<int>(cudaGetLastError());
 }
 
+// kllm_sample_f32: one block draws the id by the rule of sampling.cuh
+__global__ void __launch_bounds__(1024) sample_kernel(const float* __restrict__ logits, int n, SampleParams sp, int pos,
+                                                      long long* out_index) {
+  constexpr int kScratch = sampling::kDrawScratchBase + 2048 * 8;
+  __shared__ __align__(16) unsigned char scratch[kScratch];
+  const int i = sampling::draw_block<1024>(logits, n, sp, pos, nullptr, nullptr, 0, scratch, kScratch,
+                                           [] { __syncthreads(); });
+  if (threadIdx.x == 0) *out_index = i;
+}
+
 }  // namespace kllm
 
 using namespace kllm;
@@ -336,6 +348,17 @@ int kllm_argmax_f32(const float* logits, int64_t n, int64_t* out_index, void* st
   if (!logits || !out_index || n <= 0) return KLLM_E_INVALID;
   argmax_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(
       logits, static_cast<long long>(n), reinterpret_cast<long long*>(out_index));
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+int kllm_sample_f32(const float* logits, int64_t n, float temperature, int32_t top_k, uint64_t seed, int32_t pos,
+                    int64_t* out_index, void* stream) {
+  if (!logits || !out_index || n <= 0 || n > 0x7fffffffLL || pos < 0) return KLLM_E_INVALID;
+  if (!std::isfinite(temperature) || temperature < 0.f) return KLLM_E_INVALID;
+  sample_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(logits, static_cast<int>(n),
+                                                                   SampleParams{temperature, top_k, seed}, pos,
+                                                                   reinterpret_cast<long long*>(out_index));
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }

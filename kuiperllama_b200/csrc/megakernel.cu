@@ -1990,6 +1990,16 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
     // per-CTA (max, lowest index) of the classifier rows this CTA produced: the (up to four) lanes
     // that ran epilogues hold partial bests
     ArgBest wb = best;
+    const SampleParams sp = *P.sampling;
+    if (sampling::perturb_only(sp, P.vocab_size)) {
+      // sampling without top-k: the partial is the argmax of s_i + g_i over the same rows, read back
+      // from the logits the epilogues of this CTA have just stored
+      consumer_sync<CT>();
+      const uint2 key = sampling::seed_key(sp.seed);
+      wb = ArgBest{0.f, -1};
+      for (int i = u0 + tid; i < u1; i += CT)
+        arg_fold(wb, sampling::perturbed(ph.seg[0].out[i], sp.temperature, key, pos, i), i);
+    }
 #pragma unroll
     for (int off = 1; off < 32; off <<= 1) {  // (the mma form runs its epilogues in lanes 0, 4, ..., 28)
       const float ov = __shfl_xor_sync(kFull, wb.v, off);
@@ -2027,7 +2037,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
 // end with the same full logits vector and the same per-CTA partials, hence the same greedy id --
 // the cross-rank argmax needs no further exchange.
 template <int CW>
-__device__ __noinline__ void gather_logits_phase(const Params& P, int tok) {
+__device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int pos) {
   constexpr int CT = CW * 32;
   const Phase& ph = g_ph_cons;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -2039,12 +2049,15 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok) {
   const int u0 = static_cast<int>(static_cast<long long>(cta) * V / G);
   const int u1 = static_cast<int>(static_cast<long long>(cta + 1) * V / G);
   float* logits = ph.seg[0].out;
+  const SampleParams sp = *P.sampling;
+  const bool perturb = sampling::perturb_only(sp, V);  // as the classifier partials (gemv_phase)
+  const uint2 key = sampling::seed_key(sp.seed);
   ArgBest best{0.f, -1};
   for (int i = u0 + tid; i < u1; i += CT) {
     const int r = i / rows, j = i - r * rows;
     const float v = poll_tagged_sys(area + static_cast<size_t>(r) * P.tp_stride + j, tag);
     logits[i] = v;
-    arg_fold(best, v, i);
+    arg_fold(best, perturb ? sampling::perturbed(v, sp.temperature, key, pos, i) : v, i);
   }
 #pragma unroll
   for (int off = 1; off < 32; off <<= 1) {
@@ -2063,6 +2076,23 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok) {
     P.arg_val[cta] = b.v;
     P.arg_idx[cta] = b.i;
   }
+}
+
+// ---- sampled id with top-k -----------------------------------------------------------------------
+// tau needs all V logits, which are complete in L2 once the classifier's grid barrier is passed.  Every
+// CTA draws the id itself from them (no further barrier or hand-off) and gets the same one.  The per-CTA
+// maxima of the raw logits that the classifier (or the gather phase) left in arg_val / arg_idx bound tau
+// from below, so only the few logits near the top become candidates.  The scratch is the input-vector
+// buffer: it is idle from the classifier's last read of its input until the next token stages its first
+// vector.  The barrier after the draw orders every thread's read of the result
+// before any thread writes that buffer again.
+template <int CW>
+__device__ __noinline__ int draw_top_k(const Params& P, int pos) {
+  const int id = sampling::draw_block<CW * 32>(P.logits, P.vocab_size, *P.sampling, pos, P.arg_val, P.arg_idx,
+                                               static_cast<int>(gridDim.x), smem + kCtlBytes, P.xbuf_bytes,
+                                               [] { consumer_sync<CW * 32>(); });
+  consumer_sync<CW * 32>();
+  return id;
 }
 
 // ---- the kernel ---------------------------------------------------------------------------------
@@ -2407,7 +2437,7 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
       if (stamp) stamp[0] = global_ns();
 
       if (ph.kind == kPhaseGather) {
-        if (!(tok < P.skip_cls_tokens)) gather_logits_phase<CW>(P, tok);
+        if (!(tok < P.skip_cls_tokens)) gather_logits_phase<CW>(P, tok, pos);
         if (stamp) stamp[1] = stamp[2] = global_ns();
         if (ph.barrier_after) grid_barrier<CT>(P.barrier, bar_target, G);
         prev_barrier = ph.barrier_after != 0;
@@ -2448,16 +2478,22 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
     }
 
     // ---- greedy id: every CTA folds the per-CTA partials identically (argmax_kernel.cu:49-71
-    // semantics: maximum value, lowest index) -------------------------------------------------------
-    ArgBest b{0.f, -1};
-    for (int c = lane; c < G; c += 32) arg_fold(b, __ldcg(P.arg_val + c), __ldcg(P.arg_idx + c));
+    // semantics: maximum value, lowest index).  Sampling without top-k folds the same way: the
+    // partials are then the perturbed maxima.  With top-k every CTA draws the id itself. ----------------
+    int next;
+    if (!(tok < P.skip_cls_tokens) && sampling::top_k_active(*P.sampling, P.vocab_size)) {
+      next = draw_top_k<CW>(P, pos);
+    } else {
+      ArgBest b{0.f, -1};
+      for (int c = lane; c < G; c += 32) arg_fold(b, __ldcg(P.arg_val + c), __ldcg(P.arg_idx + c));
 #pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      const float ov = __shfl_xor_sync(kFull, b.v, off);
-      const int oi = __shfl_xor_sync(kFull, b.i, off);
-      arg_fold(b, ov, oi);
+      for (int off = 16; off > 0; off >>= 1) {
+        const float ov = __shfl_xor_sync(kFull, b.v, off);
+        const int oi = __shfl_xor_sync(kFull, b.i, off);
+        arg_fold(b, ov, oi);
+      }
+      next = b.i < 0 ? 0 : b.i;
     }
-    const int next = b.i < 0 ? 0 : b.i;
     if (cta == 0 && tid == 0) {
       if (P.out_tokens != nullptr && step < P.max_steps) P.out_tokens[step] = next;
     }
@@ -2580,6 +2616,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     if (hs & 15) return KLLM_E_UNSUPPORTED;
     xbuf = std::max(xbuf, (2 * hs + consumer_warps_ * (hs + 2)) * 4);
   }
+  // the top-k draw's scratch after the classifier (draw_top_k): the histogram and at least 64 candidates
+  xbuf = std::max(xbuf, sampling::kDrawScratchBase + 64 * 8);
   xbuf = (xbuf + 127) & ~127;
   const int xres = tagged_ ? ((dim * 4 + 127) & ~127) : 0;  // the CTA's copy of the residual stream
   const int budget = max_smem - xbuf - xres - 3584;  // static shared memory (3 KB) + slack
@@ -3064,6 +3102,8 @@ int MegaEngine::run(int n_tokens, const int32_t* teacher_dev, unsigned long long
   P.hands_per_token = hands_per_token_;
   P.arg_val = static_cast<float*>(d_arg_val_);
   P.arg_idx = static_cast<int*>(d_arg_idx_);
+  P.sampling = m.sampling;
+  P.logits = m.logits;
   P.prof = prof_dev;
   P.prof_token = prof_token;
   void* args[] = {&P};

@@ -5,6 +5,8 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "sampling.cuh"
+
 namespace kllm {
 namespace mega {
 
@@ -133,6 +135,8 @@ struct Params {
   int hands_per_token;
   float* arg_val;
   int* arg_idx;
+  const SampleParams* sampling;  // read when a token's id is drawn: changing it needs no new engine
+  const float* logits;           // [vocab]: complete once the classifier's grid barrier is passed
   // optional phase timeline of one token: prof[(cta * n_phases + phase) * 4 + k], k = phase
   // entered / input staged / last stage consumed / grid barrier passed (globaltimer ns)
   unsigned long long* prof;
@@ -163,6 +167,7 @@ struct MegaModel {
   const float* sin_cache; const float* cos_cache;
   void* state;
   int32_t* out_tokens;
+  const SampleParams* sampling;
   // tensor parallel (tp_world > 1): exchange areas of every rank (kllm_comm, CUDA IPC)
   int tp_world, tp_rank;
   unsigned long long* tp_data[8];

@@ -263,6 +263,12 @@ class Decoder:
               "kllm_decoder_generate")
         return list(out)
 
+    def set_sampling(self, temperature: float, top_k: int = 0, seed: int = 0):
+        """Draw every later id by the sampling rule (kllm_decoder_set_sampling; sampling.py mirrors it)
+        instead of the greedy argmax; temperature 0 is greedy again."""
+        check(self.lib.kllm_decoder_set_sampling(self.handle, float(temperature), int(top_k), int(seed)),
+              "kllm_decoder_set_sampling")
+
     def logits(self):
         import numpy as np
         buf = np.empty(self.shape.vocab_size, dtype=np.float32)

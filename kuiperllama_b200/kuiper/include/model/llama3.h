@@ -23,6 +23,7 @@
 #include <vector>
 
 #include "model.h"
+#include "sampler/seeded_sampler.h"
 #include "tensor_parallel.h"
 
 struct kllm_decoder;  // include/kllm_b200.h
@@ -84,6 +85,17 @@ class LLama2Model : public Model {
   void set_batched_prefill(bool on);
   bool batched_prefill() const { return batched_prefill_; }
 
+  // Seeded sampling instead of the greedy id (DESIGN.md "Sampling"): call before init(); without a call
+  // init() takes it from KUIPER_TEMPERATURE, KUIPER_TOP_K and KUIPER_SEED, so the reference's unchanged
+  // demos can sample.  Unset or temperature 0 is greedy.  predict() on the fused decoder and forward() +
+  // post_processing on the layer path draw the same id: a pure function of the logits, the settings and
+  // the position.  Under tensor parallelism every rank reads the same settings and draws the same id.
+  void set_sampling(float temperature, int32_t top_k, uint64_t seed);
+  // the settings in force (after init(): the environment's when set_sampling was not called)
+  float sampling_temperature() const { return temperature_; }
+  int32_t sampling_top_k() const { return top_k_; }
+  uint64_t sampling_seed() const { return seed_; }
+
  protected:
   // qkv_bias: the checkpoint carries a bias vector behind each layer's wq / wk / wv (Qwen2 files)
   LLama2Model(base::TokenizerType tokenizer_type, std::string token_path, std::string model_path,
@@ -128,6 +140,11 @@ class LLama2Model : public Model {
   // embedding() call (embedding_calls_ counts them) the decoder's cache holds from it
   bool batched_prefill_ = false;
   bool batched_prefill_explicit_ = false;
+  float temperature_ = 0.f;
+  int32_t top_k_ = 0;
+  uint64_t seed_ = 0;
+  bool sampling_explicit_ = false;
+  sampler::SeededSampler* seeded_ = nullptr;  // sampler_ when sampling, else null
   mutable uint64_t embedding_calls_ = 0;
   mutable uint64_t prefilled_embedding_ = 0;
   mutable int32_t prefilled_from_ = 0, prefilled_to_ = 0;

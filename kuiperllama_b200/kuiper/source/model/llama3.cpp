@@ -18,6 +18,7 @@
 #include <kllm_b200.h>
 #include <op/decoder_layers.h>
 
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <utility>
@@ -75,6 +76,13 @@ void LLama2Model::set_batched_prefill(bool on) {
   batched_prefill_explicit_ = true;
 }
 
+void LLama2Model::set_sampling(float temperature, int32_t top_k, uint64_t seed) {
+  temperature_ = temperature;
+  top_k_ = top_k;
+  seed_ = seed;
+  sampling_explicit_ = true;
+}
+
 const char* LLama2Model::decoder_engine() const { return decoder_ ? kllm_decoder_engine(decoder_) : ""; }
 
 base::Status LLama2Model::init(base::DeviceType device_type) {
@@ -95,6 +103,16 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
     return error::InvalidArgument(
         "batched prompt prefill is single-GPU: turn it off (KUIPER_BATCHED_PREFILL / set_batched_prefill) under "
         "tensor parallelism");
+  if (!sampling_explicit_) {
+    const char* t = std::getenv("KUIPER_TEMPERATURE");
+    const char* k = std::getenv("KUIPER_TOP_K");
+    const char* sd = std::getenv("KUIPER_SEED");
+    temperature_ = t != nullptr ? std::strtof(t, nullptr) : 0.f;
+    top_k_ = k != nullptr ? static_cast<int32_t>(std::strtol(k, nullptr, 10)) : 0;
+    seed_ = sd != nullptr ? std::strtoull(sd, nullptr, 10) : 0;
+  }
+  if (!std::isfinite(temperature_) || temperature_ < 0.f)
+    return error::InvalidArgument("sampling: the temperature must be finite and >= 0 (KUIPER_TEMPERATURE / set_sampling)");
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
     return error::InternalError("No usable CUDA device " + std::to_string(tp_.cuda_device()) + ".");
   cuda_config_ = std::make_shared<kernel::CudaConfig>();
@@ -106,7 +124,13 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   init_mem();
   kernel::sin_cos_cache_calc_cu(config_->head_size_, config_->seq_len_, get_buffer(ModelBufferType::kSinCache),
                                 get_buffer(ModelBufferType::kCosCache), cuda_config_->stream);
-  sampler_ = std::make_unique<sampler::ArgmaxSampler>(device_type_);
+  if (temperature_ > 0.f) {
+    auto seeded = std::make_unique<sampler::SeededSampler>(device_type_, temperature_, top_k_, seed_);
+    seeded_ = seeded.get();
+    sampler_ = std::move(seeded);
+  } else {
+    sampler_ = std::make_unique<sampler::ArgmaxSampler>(device_type_);
+  }
   return create_decoder();
 }
 
@@ -474,6 +498,12 @@ base::Status LLama2Model::create_decoder() {
   const int rc = kllm_decoder_create(&d, cuda_config_->stream, &decoder_);
   if (rc != 0)
     return base::error::InternalError(std::string("kllm_decoder_create failed: ") + kllm_error_string(rc));
+  if (temperature_ > 0.f) {
+    const int src = kllm_decoder_set_sampling(decoder_, temperature_, top_k_, seed_);
+    if (src != 0)
+      return base::error::InternalError(std::string("kllm_decoder_set_sampling failed: ") + kllm_error_string(src));
+    LOG(INFO) << "sampling: temperature " << temperature_ << ", top_k " << top_k_ << ", seed " << seed_;
+  }
   LOG(INFO) << "fused decoder engine: " << kllm_decoder_engine(decoder_) << ", "
             << kllm_decoder_launches_per_step(decoder_) << " launch(es) per token";
   LOG(INFO) << "prompt prefill: "
@@ -692,8 +722,8 @@ void LLama2Model::cls_logits(const tensor::Tensor& input) const {
 }
 
 int32_t LLama2Model::post_processing(const tensor::Tensor& pos, bool is_prompt) const {
-  UNUSED(pos);
   if (is_prompt) return -1;
+  if (seeded_ != nullptr) seeded_->set_position(pos.index<int32_t>(0));
   const tensor::Tensor& logits = Model::get_buffer(ModelBufferType::kForwardOutput);
   return static_cast<int32_t>(sampler_->sample(logits.ptr<float>(), logits.size(), cuda_config_->stream));
 }

@@ -2,19 +2,22 @@
 // drives it with text (embedding -> fill_input -> predict per position).
 //
 //   kuiper_decode <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...]
-//                 [--layers] [--copy-at K] [--logits out.f32]
+//                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED]
 //
-// ids are the prompt; after the prompt the model free-runs greedily until n_steps positions
-// have been processed.  Prints the id chosen at every position (-1 for prompt steps before the
+// ids are the prompt; after the prompt the model free-runs (greedily, or by the model's sampling
+// settings: KUIPER_TEMPERATURE / KUIPER_TOP_K / KUIPER_SEED) until n_steps positions have been processed.  Prints the id chosen at every position (-1 for prompt steps before the
 // last prompt token) on one line.  --layers uses Model::forward (layer-by-layer op registry path)
 // instead of predict's fused decoder.  --copy-at K hands predict() a COPY of the embedding row at
 // position K (so that step cannot be recognised and runs layer by layer in the middle of a sequence
-// the fused decoder started).  --logits writes the last position's logits as raw fp32.
+// the fused decoder started).  --logits writes the last position's logits as raw fp32.  --sampling calls
+// LLama2Model::set_sampling(T, K, SEED) before init() instead of leaving it to the environment.
 #include <base/base.h>
 #include <cuda_runtime_api.h>
 #include <glog/logging.h>
 
+#include <cstdint>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <string>
@@ -26,7 +29,7 @@
 int main(int argc, char** argv) {
   if (argc < 6) {
     std::fprintf(stderr, "usage: %s <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...] "
-                         "[--layers] [--copy-at K] [--logits out.f32]\n", argv[0]);
+                         "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED]\n", argv[0]);
     return 2;
   }
   const std::string checkpoint = argv[1], family = argv[2], prec = argv[3];
@@ -35,8 +38,18 @@ int main(int argc, char** argv) {
   bool layers = false;
   int copy_at = -1;
   std::string logits_path;
+  bool set_sampling = false;
+  float temperature = 0.f;
+  int32_t top_k = 0;
+  uint64_t seed = 0;
   for (int i = 5; i < argc; ++i) {
     if (!std::strcmp(argv[i], "--layers")) layers = true;
+    else if (!std::strcmp(argv[i], "--sampling") && i + 3 < argc) {
+      set_sampling = true;
+      temperature = std::strtof(argv[++i], nullptr);
+      top_k = static_cast<int32_t>(std::strtol(argv[++i], nullptr, 10));
+      seed = std::strtoull(argv[++i], nullptr, 10);
+    }
     else if (!std::strcmp(argv[i], "--copy-at") && i + 1 < argc) copy_at = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--logits") && i + 1 < argc) logits_path = argv[++i];
     else prompt.push_back(std::atoi(argv[i]));
@@ -50,6 +63,7 @@ int main(int argc, char** argv) {
   } else {
     m = std::make_unique<model::LLama2Model>(base::TokenizerType::kEncodeSpe, "<none>", checkpoint, quant);
   }
+  if (set_sampling) m->set_sampling(temperature, top_k, seed);
   base::Status st = m->init(base::DeviceType::kDeviceCUDA);
   if (!st) {
     std::fprintf(stderr, "init failed: %s\n", st.get_err_msg().c_str());
@@ -60,6 +74,11 @@ int main(int argc, char** argv) {
   tensor::Tensor pos_tensor = m->get_buffer(model::ModelBufferType::kInputPos);
   const int32_t prompt_len = static_cast<int32_t>(prompt.size());
   auto prompt_embedding = m->embedding(prompt);
+  // --layers draws with the model's settings too (the layer path's SeededSampler)
+  std::unique_ptr<sampler::SeededSampler> seeded;
+  if (m->sampling_temperature() > 0.f)
+    seeded = std::make_unique<sampler::SeededSampler>(base::DeviceType::kDeviceCUDA, m->sampling_temperature(),
+                                                      m->sampling_top_k(), m->sampling_seed());
   std::vector<float> host_logits;
   int next = -1;
   std::vector<int> chosen;
@@ -79,7 +98,11 @@ int main(int argc, char** argv) {
     }
     STATUS_CHECK(m->forward(input, pos_tensor, next));
     next = -1;
-    if (!is_prompt) {  // greedy argmax, lowest index on ties (argmax_sampler.cpp)
+    if (!is_prompt && seeded) {
+      const tensor::Tensor& lg = m->get_buffer(model::ModelBufferType::kForwardOutput);
+      seeded->set_position(pos_tensor.index<int32_t>(0));
+      next = static_cast<int>(seeded->sample(lg.ptr<float>(), lg.size(), nullptr));
+    } else if (!is_prompt) {  // greedy argmax, lowest index on ties (argmax_sampler.cpp)
       tensor::Tensor lg = m->get_buffer(model::ModelBufferType::kForwardOutput).clone();
       lg.to_cpu();
       const float* p = lg.ptr<float>();

@@ -1,0 +1,80 @@
+#!/usr/bin/env python
+"""Decode throughput with sampling against greedy, on one GPU and one decoder.
+
+    python tools/bench_sampling.py --workload qwen2.5-0.5b --steps 256
+
+One exact-numerics decoder of the workload's model (synthetic weights, bench.py's seed for the workload) runs
+kllm_decoder_generate windows of --steps positions from position 0: greedy, then temperature --temperature with
+top_k 0, then with top_k --top-k, switched by kllm_decoder_set_sampling between windows (the engine is not
+rebuilt).  Each window ends in a host synchronisation, so a host clock around it times it.  Every mode is warmed
+up once, then the modes alternate for --reps repetitions and the medians are reported.  Prints ONE JSON line:
+
+  greedy_tok_s, sampled_tok_s {top_k: tok/s}, overhead {top_k: 1 - sampled / greedy}, engine, card (the GPU's
+  name and power limit, read in the same run)
+
+Needs a CUDA device; there is nothing to time without one.
+"""
+import argparse
+import json
+import statistics
+import sys
+import time
+from pathlib import Path
+
+sys.path.insert(0, str(Path(__file__).resolve().parent))
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+
+from bench_prefill import SEEDS, gpu_card  # noqa: E402
+
+
+def run(workload, steps, reps, seed, temperature, top_k):
+    import torch
+    from kuiperllama_b200 import SHAPES, Decoder, synth_weights
+    shape = SHAPES[workload]
+    if steps > shape.seq_len:
+        raise SystemExit(f"--steps {steps} exceeds the context of {shape.name} ({shape.seq_len})")
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device: the decode paths run on the GPU only")
+    dec = Decoder(shape, synth_weights(shape, "cuda", seed), numerics="exact")
+    modes = [("greedy", 0.0, 0), ("top_k=0", temperature, 0), (f"top_k={top_k}", temperature, top_k)]
+    times = {name: [] for name, _, _ in modes}
+
+    def window(t, k):
+        dec.set_sampling(t, k, seed)
+        t0 = time.perf_counter()
+        dec.generate(1, 0, steps)
+        return time.perf_counter() - t0
+
+    for _, t, k in modes:
+        window(t, k)
+    for _ in range(max(1, reps)):
+        for name, t, k in modes:
+            times[name].append(window(t, k))
+    engine = dec.engine
+    dec.close()
+    rate = {name: steps / statistics.median(v) for name, v in times.items()}
+    g = rate["greedy"]
+    sampled = {name: r for name, r in rate.items() if name != "greedy"}
+    return {"workload": workload, "shape": shape.name, "steps": steps, "reps": max(1, reps),
+            "temperature": temperature, "greedy_tok_s": g, "sampled_tok_s": sampled,
+            "overhead": {name: 1.0 - r / g for name, r in sampled.items()},
+            "engine": engine, "numerics": "exact", "seed": seed, "card": gpu_card(torch.cuda.current_device())}
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--workload", default="tinyllama-1.1b", choices=sorted(SEEDS))
+    ap.add_argument("--steps", type=int, default=256, help="positions per generate window")
+    ap.add_argument("--reps", type=int, default=7, help="timed windows of each mode; medians are reported")
+    ap.add_argument("--temperature", type=float, default=0.8)
+    ap.add_argument("--top-k", type=int, default=40)
+    ap.add_argument("--seed", type=int, default=None, help="default: bench.py's seed for the workload")
+    a = ap.parse_args()
+    if a.steps < 1:
+        raise SystemExit("--steps must be at least 1")
+    seed = SEEDS[a.workload] if a.seed is None else a.seed
+    print(json.dumps(run(a.workload, a.steps, a.reps, seed, a.temperature, a.top_k)))
+
+
+if __name__ == "__main__":
+    main()
