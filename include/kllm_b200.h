@@ -283,6 +283,35 @@ int kllm_decoder_generate(kllm_decoder* dec, int32_t first_token, int32_t start_
                           int32_t n_steps, const int32_t* teacher_host,
                           int32_t* out_tokens_host);
 
+/* The generate loop that stops at a stop id and streams its ids to the host while it runs.
+ *  - Step i feeds token t_i at position start_pos + i and produces id_i; t_0 = first_token, t_i = id_{i-1}
+ *    (kllm_decoder_generate without a teacher).  Ids are drawn by the decoder's sampling settings (greedy by
+ *    default), so a stop applies to the drawn id.
+ *  - The loop ends after the first step whose id is in stop_ids[0 .. n_stop), or after max_steps steps.
+ *  - *n_out is the number of ids produced, counting the stop id; out_tokens_host (capacity max_steps)
+ *    receives them.
+ *  - On return the KV cache holds positions start_pos .. start_pos + *n_out - 1 and kllm_decoder_logits returns
+ *    the logits of the last step that ran: a later call may continue at start_pos + *n_out with
+ *    id_{n_out-1} as its input.
+ *  - Every id reaches on_tokens (if non-null) exactly once, in order, before the call returns: the callbacks'
+ *    concatenation equals out_tokens_host[0 .. *n_out).  The callback runs on the calling thread and must not
+ *    call into the same decoder.
+ *  - With n_stop == 0 and no callback the result equals kllm_decoder_generate(..., n_steps = max_steps,
+ *    teacher = NULL) bit for bit: ids, logits and KV cache.
+ *  - KLLM_E_INVALID, before any launch, for: n_stop outside [0, KLLM_MAX_STOP_IDS]; a stop id outside
+ *    [0, vocab); start_pos + max_steps > seq_len; max_steps <= 0; a null out_tokens_host or n_out; n_stop > 0
+ *    with a null stop_ids.
+ * Persistent engine: one launch; every CTA of every rank computes the same id, so each decides the stop by
+ * itself.  Graph engine: one captured step per launch, and the host waits for each id before it launches the
+ * next step (a host turnaround per token, as with kllm_decoder_step).  Ids reach the host through mapped
+ * pinned memory either way, while the loop is still running. */
+#define KLLM_MAX_STOP_IDS 16
+typedef void (*kllm_token_callback)(void* ctx, const int32_t* ids, int32_t n_ids);
+int kllm_decoder_generate_until(kllm_decoder* dec, int32_t first_token, int32_t start_pos, int32_t max_steps,
+                                const int32_t* stop_ids, int32_t n_stop,
+                                kllm_token_callback on_tokens, void* ctx,
+                                int32_t* out_tokens_host, int32_t* n_out);
+
 /* Sampling instead of the greedy id, from this call on, for every id the decoder returns: kllm_decoder_step
  * (non-prompt), _prompt, _prefill_tf32 / _w8 and _generate, including the ids generate feeds back on the
  * device.  Each id is the rule of kllm_sample_f32 applied to the logits of the position just processed,

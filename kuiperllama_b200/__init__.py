@@ -40,6 +40,9 @@ class GemvJob(ctypes.Structure):
 
 
 ALLREDUCE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_void_p, c_int, c_void_p)
+# kllm_token_callback: (ctx, ids, n_ids), called on the calling thread inside kllm_decoder_generate_until
+TOKEN_CALLBACK = ctypes.CFUNCTYPE(None, c_void_p, POINTER(c_int32), c_int32)
+MAX_STOP_IDS = 16  # KLLM_MAX_STOP_IDS
 
 
 class DecoderDesc(ctypes.Structure):
@@ -101,6 +104,8 @@ _SIGNATURES = {
     "kllm_decoder_prefill_w8": (c_int, [c_void_p, POINTER(c_int32), c_int32, c_int32, POINTER(c_int32)]),
     "kllm_decoder_generate": (c_int, [c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32),
                                       POINTER(c_int32)]),
+    "kllm_decoder_generate_until": (c_int, [c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32), c_int32,
+                                            TOKEN_CALLBACK, c_void_p, POINTER(c_int32), POINTER(c_int32)]),
     "kllm_decoder_set_sampling": (c_int, [c_void_p, c_float, c_int32, c_uint64]),
     "kllm_decoder_logits": (c_int, [c_void_p, c_void_p]),
     "kllm_decoder_logits_device": (c_void_p, [c_void_p]),

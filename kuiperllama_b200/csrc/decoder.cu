@@ -38,6 +38,8 @@ struct StepState {  // device-resident loop state
   int32_t step;     // steps done since generate() started
   int32_t next;     // greedy id produced by the last step
 };
+constexpr int kStreamIds = 32;  // int32 offset of the streamed ids behind the count (kllm_decoder::stream_host)
+static_assert(mega::kMaxStopIds == KLLM_MAX_STOP_IDS, "one stop-set capacity");
 
 __global__ void embed_token_kernel(const StepState* st, const float* __restrict__ table,
                                    float* x, int dim, int vocab) {
@@ -52,11 +54,14 @@ __global__ void embed_token_kernel(const StepState* st, const float* __restrict_
 // The id of the step (greedy, argmax_kernel.cu:49-71 semantics, or drawn by the sampling rule of
 // sampling.cuh with the decoder's device-resident parameters) fused with the loop bookkeeping: record
 // the id, feed it (or the teacher's id) to the next step, pos += 1.
+// With stream_ids (kllm_decoder_generate_until's graph only) the id is also published to mapped host memory:
+// the id, then the count with release semantics at system scope, which the host polls.
 constexpr int kDrawScratchBytes = sampling::kDrawScratchBase + 2048 * 8;
 
 __global__ void __launch_bounds__(1024)
 argmax_advance_kernel(const float* __restrict__ logits, int n, const SampleParams* sp, StepState* st,
-                      int32_t* out_tokens, const int32_t* teacher, int max_steps) {
+                      int32_t* out_tokens, const int32_t* teacher, int max_steps, int32_t* stream_ids,
+                      int32_t* stream_count) {
   __shared__ __align__(16) unsigned char scratch[kDrawScratchBytes];
   const int bi = sampling::draw_block<1024>(logits, n, *sp, st->pos, nullptr, nullptr, 0, scratch, kDrawScratchBytes,
                                             [] { __syncthreads(); });
@@ -65,6 +70,10 @@ argmax_advance_kernel(const float* __restrict__ logits, int n, const SampleParam
     const int step = st->step;
     st->next = next;
     if (out_tokens != nullptr && step < max_steps) out_tokens[step] = next;
+    if (stream_ids != nullptr) {
+      stream_ids[step] = next;
+      asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(stream_count), "r"(step + 1) : "memory");
+    }
     st->token = (teacher != nullptr && step + 1 < max_steps) ? teacher[step + 1] : next;
     st->pos = st->pos + 1;
     st->step = step + 1;
@@ -100,7 +109,13 @@ struct kllm_decoder {
   cudaGraphExec_t exec = nullptr;       // out_tokens recorded, no teacher
   cudaGraph_t graph_tf = nullptr;
   cudaGraphExec_t exec_tf = nullptr;    // teacher forced
+  cudaGraph_t graph_until = nullptr;
+  cudaGraphExec_t exec_until = nullptr;  // out_tokens recorded and streamed (kllm_decoder_generate_until)
   int launches_per_step = 0;
+  // Mapped pinned host memory that kllm_decoder_generate_until streams the ids through: the count at
+  // [0], the ids from [kStreamIds] (a line of their own, apart from the polled count).
+  int32_t* stream_host = nullptr;
+  int32_t* stream_dev = nullptr;  // the same memory as the device addresses it
   // batched wgmma prefill (kllm_decoder_prefill_tf32 / _w8): activations of one block of prompt positions
   float* pf_buf = nullptr;
   PrefillWorkspace pf_ws{};
@@ -129,7 +144,7 @@ int tp_reduce_into_x(kllm_decoder* dc, cudaStream_t s) {
   return kllm_add_f32(dc->x, dc->tp_tmp, dc->x, d.dim, s);
 }
 
-int enqueue_step(kllm_decoder* dc, bool with_teacher, cudaStream_t s) {
+int enqueue_step(kllm_decoder* dc, bool with_teacher, bool streamed, cudaStream_t s) {
   const kllm_decoder_desc& d = dc->d;
   const int dim = d.dim, L = d.layer_num, hid = d.hidden_dim;
   const int q_rows = d.head_num * dc->head_size;  // == dim unless tensor-parallel
@@ -221,16 +236,18 @@ int enqueue_step(kllm_decoder* dc, bool with_teacher, cudaStream_t s) {
     KLLM_TRY(gemv_dispatch(&j, GemvExtra{}, s));
   }
   argmax_advance_kernel<<<1, 1024, 0, s>>>(dc->logits, d.vocab_size, dc->sampling, dc->st, dc->out_tokens,
-                                           with_teacher ? dc->teacher : nullptr, d.seq_len);
+                                           with_teacher ? dc->teacher : nullptr, d.seq_len,
+                                           streamed ? dc->stream_dev + kStreamIds : nullptr,
+                                           streamed ? dc->stream_dev : nullptr);
   count_launch();
   KLLM_TRY(cudaGetLastError());
   dc->launches_per_step = static_cast<int>(launch_counter().load() - before);
   return 0;
 }
 
-int capture(kllm_decoder* dc, bool with_teacher, cudaGraph_t* graph, cudaGraphExec_t* exec) {
+int capture(kllm_decoder* dc, bool with_teacher, bool streamed, cudaGraph_t* graph, cudaGraphExec_t* exec) {
   KLLM_TRY(cudaStreamBeginCapture(dc->stream, cudaStreamCaptureModeRelaxed));
-  const int rc = enqueue_step(dc, with_teacher, dc->stream);
+  const int rc = enqueue_step(dc, with_teacher, streamed, dc->stream);
   cudaGraph_t g = nullptr;
   const cudaError_t end = cudaStreamEndCapture(dc->stream, &g);
   if (rc != 0) {
@@ -321,7 +338,7 @@ int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int3
     KLLM_TRY(gemv_dispatch(&j, GemvExtra{}, dc->stream));
   }
   argmax_advance_kernel<<<1, 1024, 0, dc->stream>>>(dc->logits, d.vocab_size, dc->sampling, dc->st, nullptr, nullptr,
-                                                    d.seq_len);
+                                                    d.seq_len, nullptr, nullptr);
   count_launch();
   KLLM_TRY(cudaGetLastError());
   KLLM_TRY(cudaMemcpyAsync(hs_state, dc->st, sizeof(StepState), cudaMemcpyDeviceToHost, dc->stream));
@@ -412,8 +429,11 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
       cudaMalloc(&dc->out_tokens, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMalloc(&dc->teacher, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMallocHost(&dc->st_host, sizeof(StepState)) != cudaSuccess ||
-      cudaMallocHost(&dc->io_host, sizeof(int32_t) * d.seq_len) != cudaSuccess)
+      cudaMallocHost(&dc->io_host, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
+      cudaHostAlloc(&dc->stream_host, sizeof(int32_t) * (kStreamIds + d.seq_len), cudaHostAllocMapped) != cudaSuccess ||
+      cudaHostGetDevicePointer(&dc->stream_dev, dc->stream_host, 0) != cudaSuccess)
     return fail(static_cast<int>(cudaErrorMemoryAllocation));
+  std::memset(dc->stream_host, 0, sizeof(int32_t) * (kStreamIds + d.seq_len));
   cudaMemsetAsync(dc->st, 0, sizeof(StepState), dc->stream);
   cudaMemsetAsync(dc->sampling, 0, sizeof(SampleParams), dc->stream);
 
@@ -470,8 +490,9 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     return fail(KLLM_E_UNSUPPORTED);
   }
   if (!dc->use_mega) {
-    if ((rc = capture(dc, false, &dc->graph, &dc->exec)) != 0) return fail(rc);
-    if ((rc = capture(dc, true, &dc->graph_tf, &dc->exec_tf)) != 0) return fail(rc);
+    if ((rc = capture(dc, false, false, &dc->graph, &dc->exec)) != 0) return fail(rc);
+    if ((rc = capture(dc, true, false, &dc->graph_tf, &dc->exec_tf)) != 0) return fail(rc);
+    if ((rc = capture(dc, false, true, &dc->graph_until, &dc->exec_until)) != 0) return fail(rc);
   }
   if (cudaStreamSynchronize(dc->stream) != cudaSuccess) return fail(static_cast<int>(cudaGetLastError()));
   *out = dc;
@@ -486,6 +507,8 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->graph) cudaGraphDestroy(dc->graph);
   if (dc->exec_tf) cudaGraphExecDestroy(dc->exec_tf);
   if (dc->graph_tf) cudaGraphDestroy(dc->graph_tf);
+  if (dc->exec_until) cudaGraphExecDestroy(dc->exec_until);
+  if (dc->graph_until) cudaGraphDestroy(dc->graph_until);
   float* bufs[] = {dc->x, dc->q, dc->attn, dc->h, dc->logits, dc->score,
                    dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->k_raw};
   for (float* b : bufs)
@@ -497,6 +520,7 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->pf_buf) cudaFree(dc->pf_buf);
   if (dc->st_host) cudaFreeHost(dc->st_host);
   if (dc->io_host) cudaFreeHost(dc->io_host);
+  if (dc->stream_host) cudaFreeHost(dc->stream_host);
   if (dc->own_stream && dc->stream) cudaStreamDestroy(dc->stream);
   delete dc;
 }
@@ -600,6 +624,71 @@ int kllm_decoder_generate(kllm_decoder* dc, int32_t first_token, int32_t start_p
   }
   KLLM_TRY(cudaStreamSynchronize(dc->stream));
   if (out_tokens_host) std::memcpy(out_tokens_host, dc->io_host, sizeof(int32_t) * n_steps);
+  return 0;
+}
+
+int kllm_decoder_generate_until(kllm_decoder* dc, int32_t first_token, int32_t start_pos, int32_t max_steps,
+                                const int32_t* stop_ids, int32_t n_stop, kllm_token_callback on_tokens, void* ctx,
+                                int32_t* out_tokens_host, int32_t* n_out) {
+  // every refusal comes before the first launch, so a refused call leaves the decoder as it was
+  if (!dc || !out_tokens_host || !n_out || max_steps <= 0 || start_pos < 0) return KLLM_E_INVALID;
+  if (static_cast<int64_t>(start_pos) + max_steps > dc->d.seq_len) return KLLM_E_INVALID;
+  if (n_stop < 0 || n_stop > KLLM_MAX_STOP_IDS || (n_stop > 0 && stop_ids == nullptr)) return KLLM_E_INVALID;
+  for (int i = 0; i < n_stop; ++i)
+    if (stop_ids[i] < 0 || stop_ids[i] >= dc->d.vocab_size) return KLLM_E_INVALID;
+  *n_out = 0;
+  int32_t* count = dc->stream_host;
+  const int32_t* ids = dc->stream_host + kStreamIds;
+  __atomic_store_n(count, 0, __ATOMIC_SEQ_CST);  // before the launch that writes it
+  StepState* hs = dc->st_host;
+  hs->token = first_token;
+  hs->pos = start_pos;
+  hs->step = 0;
+  hs->next = -1;
+  KLLM_TRY(cudaMemcpyAsync(dc->st, hs, sizeof(StepState), cudaMemcpyHostToDevice, dc->stream));
+  int32_t n = 0;
+  if (dc->use_mega) {
+    // One launch that stops on the device; the host hands over whatever ids the count says have arrived
+    // until the stream is done.
+    KLLM_TRY(dc->mega.run_until(max_steps, stop_ids, n_stop, dc->stream_dev + kStreamIds, dc->stream_dev));
+    int32_t delivered = 0;
+    cudaError_t q = cudaErrorNotReady;
+    while (on_tokens != nullptr && q == cudaErrorNotReady) {
+      q = cudaStreamQuery(dc->stream);  // before the count: after a success the count is final
+      const int32_t c = __atomic_load_n(count, __ATOMIC_ACQUIRE);
+      if (c > delivered) {
+        on_tokens(ctx, ids + delivered, c - delivered);
+        delivered = c;
+      }
+    }
+    const cudaError_t e = cudaMemcpyAsync(hs, dc->st, sizeof(StepState), cudaMemcpyDeviceToHost, dc->stream);
+    const cudaError_t s = cudaStreamSynchronize(dc->stream);
+    if (e != cudaSuccess || s != cudaSuccess) return static_cast<int>(e != cudaSuccess ? e : s);
+    n = hs->step;
+    dc->mega.account(n);  // the tags and barriers of the positions that ran, not of max_steps
+    if (on_tokens != nullptr && n > delivered) on_tokens(ctx, ids + delivered, n - delivered);
+  } else {
+    // One captured step per launch, driven from the host: wait for the step's id through the mapped count,
+    // then stop or launch the next step.  No step runs after the stop, on any tensor-parallel rank.
+    for (int i = 0; i < max_steps;) {
+      KLLM_TRY(cudaGraphLaunch(dc->exec_until, dc->stream));
+      count_launch(static_cast<uint64_t>(dc->launches_per_step));
+      while (__atomic_load_n(count, __ATOMIC_ACQUIRE) <= i) {
+        const cudaError_t q = cudaStreamQuery(dc->stream);
+        if (q == cudaSuccess && __atomic_load_n(count, __ATOMIC_ACQUIRE) <= i) return KLLM_E_STATE;
+        if (q != cudaSuccess && q != cudaErrorNotReady) return static_cast<int>(q);
+      }
+      const int32_t id = ids[i++];
+      if (on_tokens != nullptr) on_tokens(ctx, &id, 1);
+      n = i;
+      bool stop = false;
+      for (int j = 0; j < n_stop; ++j) stop |= stop_ids[j] == id;
+      if (stop) break;
+    }
+    KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  }
+  std::memcpy(out_tokens_host, ids, sizeof(int32_t) * n);
+  *n_out = n;
   return 0;
 }
 

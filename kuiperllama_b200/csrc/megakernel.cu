@@ -110,6 +110,33 @@ __device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t parity) {
       "r"(parity), "r"(KLLM_MBAR_HINT_NS)
       : "memory");
 }
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* b, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n .reg .pred p;\n"
+      " mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n"
+      " selp.u32 %0, 1, 0, p;\n}"
+      : "=r"(ok)
+      : "r"(smem_u32(b)), "r"(parity), "r"(KLLM_MBAR_HINT_NS)
+      : "memory");
+  return ok != 0;
+}
+// The producer's wait on a stage's `empty` barrier in a stoppable run: a stopped CTA's consumers never free
+// the slot, so the wait gives up once *stop is set.  Warp-uniform: true (stop, issue nothing) if any lane saw
+// the flag; a copy is issued only when every lane saw the slot free.
+__device__ __forceinline__ bool mbar_wait_or_stop(uint64_t* b, uint32_t parity, const volatile int* stop) {
+  bool stopped = false;
+  while (!mbar_try_wait(b, parity)) {
+    if (*stop) {
+      stopped = true;
+      break;
+    }
+  }
+  return __any_sync(0xffffffffu, stopped);
+}
+__device__ __forceinline__ void st_release_sys(int32_t* p, int32_t v) {
+  asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar,
                                          uint64_t policy) {
   asm volatile(
@@ -252,6 +279,11 @@ __shared__ float g_s_argv[kMaxWarps];
 __shared__ int g_s_argi[kMaxWarps];
 __shared__ float g_s_bcast;
 __shared__ volatile unsigned g_fill_count;  // ring stages the producer has issued so far
+// Stoppable runs (Params::stop_ids): the consumers set g_stop once the token's id is a stop id; the producer
+// then stops issuing and publishes where its ring position ended, 1 + (slot << 1 | parity), in g_prod_end
+// (0: still running).  The consumers drain every fill up to that position before the CTA exits.
+__shared__ volatile int g_stop;
+__shared__ volatile unsigned g_prod_end;
 __shared__ float g_s_team[kMaxWarps / 2][2][3][8];  // team form: the other members' row partials, double buffered per team
 __shared__ Phase g_ph_cons;
 __shared__ Phase g_ph_prod;
@@ -2118,6 +2150,8 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
 
   if (tid == 0) {
     s_fill_count = 0u;
+    g_stop = 0;
+    g_prod_end = 0u;
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], CW);
@@ -2152,15 +2186,21 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
           if (cta >= P.head_num * SP || ppos == 0) continue;
           // rows t < pos of this head: final since the previous token.  Order the async-proxy
           // reads after the grid barrier that closed the previous token.
+          // (A run that stopped never passes the barrier of the token after the stop: give up then.)
+          int stopped = 0;
           if (tok > 0 && lane == 0) {
             const unsigned need = P.barrier_base +
                                   static_cast<unsigned>((tok - 1) * P.bars_per_token + ph.barrier_idx) *
                                       static_cast<unsigned>(G);
             while (static_cast<int>(ld_acquire_u32(P.barrier) - need) < 0) {
+              if (g_stop) {
+                stopped = 1;
+                break;
+              }
             }
             asm volatile("fence.proxy.async;" ::: "memory");
           }
-          __syncwarp();
+          if (__shfl_sync(kFull, stopped, 0)) goto producer_done;
           const int hs = P.head_size;
           const int head = cta / SP, split = cta % SP;
           const int kvh = head / P.kv_mul;
@@ -2175,7 +2215,7 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
               const int t0 = j * T;
               const int nt = min(T, ppos - t0);
               for (int kv = 0; kv < 2; ++kv) {
-                mbar_wait(&empty_bar[pipe.slot], pipe.parity ^ 1u);
+                if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
                 unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
                 if (lane == 0) mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(nt) * hs * 4);
                 __syncwarp();
@@ -2201,7 +2241,7 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
             for (int j = split; j < n_tiles; j += SP) {
               const int t0 = j * T;
               const int nt = min(T, ppos - t0);
-              mbar_wait(&empty_bar[pipe.slot], pipe.parity ^ 1u);
+              if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
               unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
               if (lane == 0) mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(nt) * hs * 4);
               __syncwarp();
@@ -2220,7 +2260,7 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
             for (int j = 0; j < n_tiles; ++j) {
               const int t0 = j * T;
               const int nt = min(T, ppos - t0);
-              mbar_wait(&empty_bar[pipe.slot], pipe.parity ^ 1u);
+              if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
               unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
               if (lane == 0) {
                 mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(nt) * dv * 4);
@@ -2243,7 +2283,7 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
           for (int u = u0; u < u1; u += ups) {
             const int n = min(ups, u1 - u);
             const int nrows = n * rpu;
-            mbar_wait(&empty_bar[pipe.slot], pipe.parity ^ 1u);
+            if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
             unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
             if (lane == 0)
               mbar_expect_tx(&full_bar[pipe.slot],
@@ -2293,7 +2333,7 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
             for (int c = 0; c < ph.chunks_per_row; ++c) {
               const int e0 = c * ph.chunk_elems;
               const int ne = min(ph.chunk_elems, ph.in_dim - e0);
-              mbar_wait(&empty_bar[pipe.slot], pipe.parity ^ 1u);
+              if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
               if (lane == 0) {
                 mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(ne) * wbytes);
                 bulk_g2s(stages + static_cast<size_t>(pipe.slot) * P.stage_bytes,
@@ -2308,6 +2348,9 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
         }
       }
     }
+  producer_done:
+    // every fill up to here is issued: the consumers of a stopped run drain them before the CTA exits
+    if (lane == 0) g_prod_end = 1u + ((static_cast<unsigned>(pipe.slot) << 1) | pipe.parity);
     return;
   }
 
@@ -2349,14 +2392,16 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
         const int u1 = static_cast<int>(static_cast<long long>(cta + 1) * ph.units / G);
         const int rpu = ph.swiglu ? 2 : 1;
         const int row_bytes = ph.in_dim * wbytes;
+        // true: the run stopped (the producer's count will not grow any more), walk no further
         auto throttle = [&]() {
-          while (static_cast<int>(ahead - s_fill_count) >= P.pf_stages) __nanosleep(400);
+          while (static_cast<int>(ahead - s_fill_count) >= P.pf_stages && !g_stop) __nanosleep(400);
+          return __any_sync(kFull, g_stop != 0);
         };
         if (ph.chunks_per_row == 1) {
           const int ups = ph.rows_per_stage / rpu;
           for (int u = u0; u < u1; u += ups) {
             const int nrows = min(ups, u1 - u) * rpu;
-            throttle();
+            if (throttle()) return;
             {
               const int n = nrows / rpu;
               const RowRef rr = lane < nrows ? stage_row(ph, u, n, lane) : RowRef{-1, -1};
@@ -2381,7 +2426,7 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
             for (int c = 0; c < ph.chunks_per_row; ++c) {
               const int e0 = c * ph.chunk_elems;
               const int ne = min(ph.chunk_elems, ph.in_dim - e0);
-              throttle();
+              if (throttle()) return;
               if (lane == 0) bulk_prefetch_l2(src + static_cast<size_t>(e0) * wbytes, static_cast<uint32_t>(ne) * wbytes);
               ++ahead;
             }
@@ -2494,18 +2539,41 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
       }
       next = b.i < 0 ? 0 : b.i;
     }
+    // Every CTA (and every tensor-parallel rank) holds the same `next`, so the stop needs no exchange.
+    bool stop = false;
+#pragma unroll
+    for (int i = 0; i < kMaxStopIds; ++i) stop |= P.stop_ids[i] == next;
     if (cta == 0 && tid == 0) {
       if (P.out_tokens != nullptr && step < P.max_steps) P.out_tokens[step] = next;
+      if (P.stream_ids != nullptr) {  // the id, then (release, system scope) the count the host polls
+        P.stream_ids[step] = next;
+        st_release_sys(P.stream_count, step + 1);
+      }
     }
     token = (P.teacher != nullptr && step + 1 < P.max_steps) ? P.teacher[step + 1] : next;
     if (static_cast<unsigned>(token) >= static_cast<unsigned>(P.vocab_size)) token = 0;
     pos += 1;
     step += 1;
-    if (cta == 0 && tid == 0 && tok == P.n_tokens - 1) {
+    if (cta == 0 && tid == 0 && (tok == P.n_tokens - 1 || stop)) {
       P.state->token = token;
       P.state->pos = pos;
       P.state->step = step;
       P.state->next = next;
+    }
+    if (stop) {
+      // The producer may have issued stages of the next token already, and may be waiting for a slot that
+      // will never be freed.  Tell it to stop, then wait until every fill it issued has landed: the CTA may
+      // not exit with a bulk copy into its shared memory in flight.
+      if (tid == 0) g_stop = 1;
+      unsigned end;
+      while ((end = g_prod_end) == 0u) {
+      }
+      const Pipe last{static_cast<int>((end - 1u) >> 1), (end - 1u) & 1u};
+      while (pipe.slot != last.slot || pipe.parity != last.parity) {
+        mbar_wait(&full_bar[pipe.slot], pipe.parity);
+        pipe.advance(S);
+      }
+      return;
     }
   }
 }
@@ -3040,9 +3108,8 @@ void MegaEngine::destroy() {
   ready_ = false;
 }
 
-int MegaEngine::run(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
-                    int prof_token, int skip_cls_tokens) {
-  if (!ready_) return KLLM_E_STATE;
+Params MegaEngine::params(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev, int prof_token,
+                          int skip_cls_tokens) const {
   Params P{};
   const MegaModel& m = model_;
   P.phases = static_cast<const Phase*>(d_phases_);
@@ -3106,16 +3173,45 @@ int MegaEngine::run(int n_tokens, const int32_t* teacher_dev, unsigned long long
   P.logits = m.logits;
   P.prof = prof_dev;
   P.prof_token = prof_token;
-  void* args[] = {&P};
-  cudaError_t e = cudaLaunchCooperativeKernel(const_cast<void*>(prof_dev != nullptr ? kernel_prof_ : kernel_), dim3(grid_), dim3(threads_), args,
-                                              smem_bytes_, stream_);
+  for (int i = 0; i < mega::kMaxStopIds; ++i) P.stop_ids[i] = -1;  // ids are >= 0: no stop
+  return P;
+}
+
+int MegaEngine::launch(const Params& P) {
+  void* args[] = {const_cast<Params*>(&P)};
+  cudaError_t e = cudaLaunchCooperativeKernel(const_cast<void*>(P.prof != nullptr ? kernel_prof_ : kernel_), dim3(grid_),
+                                              dim3(threads_), args, smem_bytes_, stream_);
   if (e != cudaSuccess) return static_cast<int>(e);
+  count_launch();
+  return 0;
+}
+
+// The tags and barrier counts the next launch waits for continue from where the tokens that ran left them.
+void MegaEngine::account(int n_tokens) {
   tp_seq_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(exch_per_token_);
   hand_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(hands_per_token_);
   barrier_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(n_barriers_per_token_) *
                    static_cast<unsigned>(grid_);
-  count_launch();
+}
+
+int MegaEngine::run(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
+                    int prof_token, int skip_cls_tokens) {
+  if (!ready_) return KLLM_E_STATE;
+  const Params P = params(n_tokens, teacher_dev, prof_dev, prof_token, skip_cls_tokens);
+  if (int rc = launch(P)) return rc;
+  account(n_tokens);
   return 0;
+}
+
+int MegaEngine::run_until(int n_tokens, const int32_t* stop_ids, int n_stop, int32_t* stream_ids,
+                          int32_t* stream_count) {
+  if (!ready_) return KLLM_E_STATE;
+  if (n_stop < 0 || n_stop > mega::kMaxStopIds) return KLLM_E_INVALID;
+  Params P = params(n_tokens, nullptr, nullptr, -1, 0);
+  for (int i = 0; i < n_stop; ++i) P.stop_ids[i] = stop_ids[i];
+  P.stream_ids = stream_ids;
+  P.stream_count = stream_count;
+  return launch(P);
 }
 
 }  // namespace kllm

@@ -19,6 +19,7 @@ enum {
   kPhaseGather = 5 /* tensor parallel, classifier sharded by vocabulary: collect every rank's logits, argmax partials */
 };
 constexpr int kProfStamps = 16;  // uint64 stamps per (CTA, phase) of kllm_decoder_profile
+constexpr int kMaxStopIds = 16;  // == KLLM_MAX_STOP_IDS
 
 struct Seg {
   const void* w;        // fp32 or int8 [rows, in_dim]
@@ -137,6 +138,12 @@ struct Params {
   int* arg_idx;
   const SampleParams* sampling;  // read when a token's id is drawn: changing it needs no new engine
   const float* logits;           // [vocab]: complete once the classifier's grid barrier is passed
+  // Stoppable run (kllm_decoder_generate_until): the run ends after the first token whose id is one of
+  // stop_ids (unused entries are -1, so a run without stop ids compares against nothing), and each id is
+  // also published to stream_ids[step] followed by stream_count = step + 1 (mapped host memory; null: off).
+  int stop_ids[kMaxStopIds];
+  int32_t* stream_ids;
+  int32_t* stream_count;
   // optional phase timeline of one token: prof[(cta * n_phases + phase) * 4 + k], k = phase
   // entered / input staged / last stage consumed / grid barrier passed (globaltimer ns)
   unsigned long long* prof;
@@ -182,6 +189,12 @@ class MegaEngine {
   // Run n_tokens consecutive positions starting from the device-resident state.
   int run(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev = nullptr,
           int prof_token = -1, int skip_cls_tokens = 0);
+  // Up to n_tokens positions, ending after the first id in stop_ids[0 .. n_stop); every id is streamed to
+  // stream_ids / stream_count (device-visible pointers into mapped host memory).  The number of positions
+  // that ran is known only once the launch has finished, so the tag and barrier bases are NOT advanced
+  // here: the caller passes that number (state.step) to account() before the next launch.
+  int run_until(int n_tokens, const int32_t* stop_ids, int n_stop, int32_t* stream_ids, int32_t* stream_count);
+  void account(int n_tokens);
   int grid() const { return grid_; }
   bool ready() const { return ready_; }
   int stages() const { return stages_; }
@@ -196,6 +209,9 @@ class MegaEngine {
   bool int8_fast() const { return int8_fast_ != 0; }
 
  private:
+  mega::Params params(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev, int prof_token,
+                      int skip_cls_tokens) const;
+  int launch(const mega::Params& P);
   MegaModel model_{};
   cudaStream_t stream_ = nullptr;
   void* d_phases_ = nullptr;

@@ -263,6 +263,31 @@ class Decoder:
               "kllm_decoder_generate")
         return list(out)
 
+    def generate_until(self, first_token: int, start_pos: int, max_steps: int, stop_ids=(), on_tokens=None):
+        """Generate from `first_token` at `start_pos` until the first id in `stop_ids` (included in the result) or
+        `max_steps` ids (kllm_decoder_generate_until).  `on_tokens(list_of_ints)` receives every id exactly once,
+        in order, while the loop runs; it must not call into this decoder."""
+        from . import TOKEN_CALLBACK
+        stops = [int(t) for t in stop_ids]
+        sarr = (ctypes.c_int32 * max(len(stops), 1))(*stops)
+        out = (ctypes.c_int32 * max(int(max_steps), 1))()
+        n_out = ctypes.c_int32(0)
+        errors = []
+
+        def relay(_ctx, ids, n):
+            try:
+                on_tokens([ids[i] for i in range(n)])
+            except BaseException as e:  # an exception cannot cross the C frames: re-raised after the call
+                errors.append(e)
+
+        cb = TOKEN_CALLBACK(relay) if on_tokens is not None else TOKEN_CALLBACK()
+        check(self.lib.kllm_decoder_generate_until(self.handle, int(first_token), int(start_pos), int(max_steps),
+                                                   sarr, len(stops), cb, None, out, ctypes.byref(n_out)),
+              "kllm_decoder_generate_until")
+        if errors:
+            raise errors[0]
+        return list(out[:n_out.value])
+
     def set_sampling(self, temperature: float, top_k: int = 0, seed: int = 0):
         """Draw every later id by the sampling rule (kllm_decoder_set_sampling; sampling.py mirrors it)
         instead of the greedy argmax; temperature 0 is greedy again."""

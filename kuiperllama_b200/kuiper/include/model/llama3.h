@@ -18,6 +18,7 @@
 #define KLLM_KUIPER_MODEL_LLAMA3_H_
 #include <base/cuda_config.h>
 
+#include <functional>
 #include <memory>
 #include <string>
 #include <vector>
@@ -96,6 +97,20 @@ class LLama2Model : public Model {
   int32_t sampling_top_k() const { return top_k_; }
   uint64_t sampling_seed() const { return seed_; }
 
+  // A whole generation on the fused decoder, without a host round trip per token:
+  //   1. the prompt from position 0 (the batched prefill for all but its last token when batched_prefill() is
+  //      on, else kllm_decoder_prompt -- also under tensor parallelism);
+  //   2. the id after the prompt; if it is a stop id, that one id is the result;
+  //   3. kllm_decoder_generate_until for the rest, which stops on the device at the first stop id.
+  // `ids` receives at most max_new_tokens ids (fewer where the context ends), counting the stop id.  on_tokens,
+  // if set, receives every id exactly once, in order, while the loop runs.  The stop set is the tokenizer's
+  // generation-ending ids (what is_sentence_ending() accepts) plus set_stop_ids().  Afterwards predict() at
+  // position prompt.size() + ids.size() - 1 with ids.back() continues the same sequence.
+  base::Status generate(const std::vector<int32_t>& prompt, int32_t max_new_tokens, std::vector<int32_t>& ids,
+                        const std::function<void(const int32_t*, int32_t)>& on_tokens = {}) const;
+  // Extra stop ids for generate(), e.g. for tokenizers that stop on nothing.
+  void set_stop_ids(std::vector<int32_t> ids) { extra_stop_ids_ = std::move(ids); }
+
  protected:
   // qkv_bias: the checkpoint carries a bias vector behind each layer's wq / wk / wv (Qwen2 files)
   LLama2Model(base::TokenizerType tokenizer_type, std::string token_path, std::string model_path,
@@ -145,6 +160,7 @@ class LLama2Model : public Model {
   uint64_t seed_ = 0;
   bool sampling_explicit_ = false;
   sampler::SeededSampler* seeded_ = nullptr;  // sampler_ when sampling, else null
+  std::vector<int32_t> extra_stop_ids_;       // set_stop_ids()
   mutable uint64_t embedding_calls_ = 0;
   mutable uint64_t prefilled_embedding_ = 0;
   mutable int32_t prefilled_from_ = 0, prefilled_to_ = 0;

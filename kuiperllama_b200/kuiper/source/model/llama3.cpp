@@ -18,6 +18,7 @@
 #include <kllm_b200.h>
 #include <op/decoder_layers.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -626,6 +627,72 @@ base::Status LLama2Model::prefill_prompt_rows(int32_t pos, bool* done) const {
   prefilled_from_ = pos, prefilled_to_ = n - 1;
   decoder_rows_ = n - 1;
   *done = true;
+  return base::error::Success();
+}
+
+base::Status LLama2Model::generate(const std::vector<int32_t>& prompt, int32_t max_new_tokens,
+                                   std::vector<int32_t>& ids,
+                                   const std::function<void(const int32_t*, int32_t)>& on_tokens) const {
+  ids.clear();
+  if (decoder_ == nullptr) return base::error::InvalidArgument("generate() needs the fused decoder (init() first)");
+  const int32_t n = static_cast<int32_t>(prompt.size());
+  if (n == 0 || n > config_->seq_len_ || max_new_tokens <= 0)
+    return base::error::InvalidArgument("generate(): an empty or too long prompt, or max_new_tokens <= 0");
+  // the stop set: the tokenizer's generation-ending ids, then the caller's
+  std::vector<int32_t> stops;
+  auto add_stop = [&stops](int32_t t) {
+    if (std::find(stops.begin(), stops.end(), t) == stops.end()) stops.push_back(t);
+  };
+  if (encode_layer_ != nullptr)
+    for (int32_t t = 0; t < config_->vocab_size_; ++t)
+      if (encode_layer_->is_sentence_ending(t)) add_stop(t);
+  for (int32_t t : extra_stop_ids_) add_stop(t);
+  if (stops.size() > KLLM_MAX_STOP_IDS)
+    return base::error::InvalidArgument("generate(): more than KLLM_MAX_STOP_IDS stop ids");
+  for (int32_t t : stops)
+    if (t < 0 || t >= config_->vocab_size_) return base::error::InvalidArgument("generate(): a stop id outside the vocabulary");
+
+  // 1. the prompt, from position 0
+  int32_t first = -1;
+  int rc = 0;
+  const char* what = "kllm_decoder_prompt";
+  if (batched_prefill_ && n >= 3) {  // as predict(): the batched prefill for all but the last row, which steps
+    what = is_quant_model_ ? "kllm_decoder_prefill_w8" : "kllm_decoder_prefill_tf32";
+    rc = (is_quant_model_ ? kllm_decoder_prefill_w8 : kllm_decoder_prefill_tf32)(decoder_, prompt.data(), n - 1, 0, &first);
+    if (rc == 0) {
+      what = "kllm_decoder_step";
+      rc = kllm_decoder_step(decoder_, prompt[n - 1], n - 1, 0, &first);
+    }
+  } else {
+    rc = kllm_decoder_prompt(decoder_, prompt.data(), n, 0, &first);
+  }
+  if (rc != 0) return base::error::InternalError(std::string(what) + ": " + kllm_error_string(rc));
+  // the decoder now holds this sequence only: rows of an older one (either path) and an older prefill are void
+  decoder_rows_ = n;
+  layer_rows_ = 0;
+  prefilled_from_ = prefilled_to_ = 0;
+  logits_in_decoder_ = true;
+
+  // 2. the id after the prompt
+  ids.push_back(first);
+  if (on_tokens) on_tokens(&first, 1);
+  const bool stopped = std::find(stops.begin(), stops.end(), first) != stops.end();
+  const int32_t rest = std::min(max_new_tokens - 1, config_->seq_len_ - n);
+  if (stopped || rest <= 0) return base::error::Success();
+
+  // 3. the rest on the device, until a stop id
+  std::vector<int32_t> more(static_cast<size_t>(rest));
+  int32_t n_out = 0;
+  auto relay = [](void* ctx, const int32_t* t, int32_t k) {
+    (*static_cast<const std::function<void(const int32_t*, int32_t)>*>(ctx))(t, k);
+  };
+  rc = kllm_decoder_generate_until(decoder_, first, n, rest, stops.data(), static_cast<int32_t>(stops.size()),
+                                   on_tokens ? +relay : nullptr,
+                                   const_cast<std::function<void(const int32_t*, int32_t)>*>(&on_tokens), more.data(),
+                                   &n_out);
+  if (rc != 0) return base::error::InternalError(std::string("kllm_decoder_generate_until: ") + kllm_error_string(rc));
+  ids.insert(ids.end(), more.begin(), more.begin() + n_out);
+  decoder_rows_ = n + n_out;  // == prompt.size() + ids.size() - 1: predict() continues at that position
   return base::error::Success();
 }
 

@@ -3,6 +3,11 @@
 //
 //   kuiper_decode <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...]
 //                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED]
+//                 [--generate N [--stop ID]... [--then K]]
+//
+// --generate N runs the prompt and LLama2Model::generate() for at most N ids instead (n_steps is then unused),
+// stopping at the tokenizer's stop ids and every --stop ID, and prints the ids generate() returned, followed
+// by the ids of K more predict() steps on the same sequence with --then K.
 //
 // ids are the prompt; after the prompt the model free-runs (greedily, or by the model's sampling
 // settings: KUIPER_TEMPERATURE / KUIPER_TOP_K / KUIPER_SEED) until n_steps positions have been processed.  Prints the id chosen at every position (-1 for prompt steps before the
@@ -29,7 +34,8 @@
 int main(int argc, char** argv) {
   if (argc < 6) {
     std::fprintf(stderr, "usage: %s <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...] "
-                         "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED]\n", argv[0]);
+                         "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] "
+                         "[--generate N [--stop ID]... [--then K]]\n", argv[0]);
     return 2;
   }
   const std::string checkpoint = argv[1], family = argv[2], prec = argv[3];
@@ -42,6 +48,8 @@ int main(int argc, char** argv) {
   float temperature = 0.f;
   int32_t top_k = 0;
   uint64_t seed = 0;
+  int generate = 0, then = 0;
+  std::vector<int32_t> stops;
   for (int i = 5; i < argc; ++i) {
     if (!std::strcmp(argv[i], "--layers")) layers = true;
     else if (!std::strcmp(argv[i], "--sampling") && i + 3 < argc) {
@@ -50,6 +58,9 @@ int main(int argc, char** argv) {
       top_k = static_cast<int32_t>(std::strtol(argv[++i], nullptr, 10));
       seed = std::strtoull(argv[++i], nullptr, 10);
     }
+    else if (!std::strcmp(argv[i], "--generate") && i + 1 < argc) generate = std::atoi(argv[++i]);
+    else if (!std::strcmp(argv[i], "--stop") && i + 1 < argc) stops.push_back(std::atoi(argv[++i]));
+    else if (!std::strcmp(argv[i], "--then") && i + 1 < argc) then = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--copy-at") && i + 1 < argc) copy_at = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--logits") && i + 1 < argc) logits_path = argv[++i];
     else prompt.push_back(std::atoi(argv[i]));
@@ -64,6 +75,7 @@ int main(int argc, char** argv) {
     m = std::make_unique<model::LLama2Model>(base::TokenizerType::kEncodeSpe, "<none>", checkpoint, quant);
   }
   if (set_sampling) m->set_sampling(temperature, top_k, seed);
+  if (!stops.empty()) m->set_stop_ids(stops);
   base::Status st = m->init(base::DeviceType::kDeviceCUDA);
   if (!st) {
     std::fprintf(stderr, "init failed: %s\n", st.get_err_msg().c_str());
@@ -72,6 +84,31 @@ int main(int argc, char** argv) {
   std::fprintf(stderr, "engine: %s%s\n", m->decoder_engine(), layers ? " (unused: --layers)" : "");
 
   tensor::Tensor pos_tensor = m->get_buffer(model::ModelBufferType::kInputPos);
+  if (generate > 0) {
+    // LLama2Model::generate(), then --then more predict() steps on the same sequence
+    std::vector<int32_t> ids, streamed;
+    st = m->generate(std::vector<int32_t>(prompt.begin(), prompt.end()), generate, ids,
+                     [&streamed](const int32_t* t, int32_t k) { streamed.insert(streamed.end(), t, t + k); });
+    if (!st) {
+      std::fprintf(stderr, "generate failed: %s\n", st.get_err_msg().c_str());
+      return 1;
+    }
+    if (streamed != ids) {
+      std::fprintf(stderr, "generate: the streamed ids differ from the returned ones\n");
+      return 1;
+    }
+    int next = ids.back();
+    for (int k = 0; k < then; ++k) {
+      const int32_t pos = static_cast<int32_t>(prompt.size() + ids.size()) - 1;
+      pos_tensor.index<int32_t>(0) = pos;
+      auto emb = m->embedding({next});
+      STATUS_CHECK(m->predict(m->fill_input(pos_tensor, emb, false), pos_tensor, false, next));
+      ids.push_back(next);
+    }
+    for (size_t i = 0; i < ids.size(); ++i) std::printf("%s%d", i ? " " : "", ids[i]);
+    std::printf("\n");
+    return 0;
+  }
   const int32_t prompt_len = static_cast<int32_t>(prompt.size());
   auto prompt_embedding = m->embedding(prompt);
   // --layers draws with the model's settings too (the layer path's SeededSampler)
