@@ -265,7 +265,8 @@ int kllm_decoder_prompt(kllm_decoder* dec, const int32_t* tokens_host, int32_t n
  * tensor cores (TF32 multiply, fp32 accumulate, kllm_gemm_tf32), the weights streamed once per 256
  * positions instead of once per position; classifier only for the last position.  KV-cache rows and
  * logits agree with the position-by-position path to ~1e-3 relative, NOT bit for bit (TF32 keeps 10
- * mantissa bits).  fp32 checkpoints on one GPU; KLLM_E_UNSUPPORTED otherwise (use kllm_decoder_prompt). */
+ * mantissa bits).  fp32 checkpoints on one GPU; KLLM_E_UNSUPPORTED otherwise (use kllm_decoder_prompt).
+ * A token id outside [0, vocab_size) is refused with KLLM_E_INVALID before any launch. */
 int kllm_decoder_prefill_tf32(kllm_decoder* dec, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
                               int32_t* next_host);
 /* The batched prefill for int8 checkpoints: the contract and the tolerance of kllm_decoder_prefill_tf32

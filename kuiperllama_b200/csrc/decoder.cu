@@ -268,7 +268,11 @@ int capture(kllm_decoder* dc, bool with_teacher, bool streamed, cudaGraph_t* gra
 int prefill_args(const kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
                  const int32_t* next_host) {
   if (!dc || !tokens_host || !next_host || n_tokens <= 0 || start_pos < 0) return KLLM_E_INVALID;
-  return start_pos + n_tokens > dc->d.seq_len ? KLLM_E_INVALID : 0;
+  if (start_pos + n_tokens > dc->d.seq_len) return KLLM_E_INVALID;
+  // embed_rows_kernel has no embedding row for an id outside the vocabulary: refuse before any launch
+  for (int32_t i = 0; i < n_tokens; ++i)
+    if (tokens_host[i] < 0 || tokens_host[i] >= dc->d.vocab_size) return KLLM_E_INVALID;
+  return 0;
 }
 
 int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos, int32_t* next_host) {
