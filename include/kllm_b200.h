@@ -106,6 +106,15 @@ int64_t kllm_argmax_f32_sync(const float* logits, int64_t n, void* stream);
  * pointers, n outside [1, 2^31), pos < 0, or a temperature that is negative or not finite. */
 int kllm_sample_f32(const float* logits, int64_t n, float temperature, int32_t top_k, uint64_t seed, int32_t pos,
                     int64_t* out_index, void* stream);
+/* kllm_sample_f32 with nucleus (top-p) sampling after top-k, as in HF's TopPLogitsWarper: a token of the
+ * top-k set is dropped once the probability mass strictly above it reaches top_p; equal logits are kept or
+ * dropped together, and the maximum is always kept.  The mass is an exact integer sum (DESIGN.md
+ * "Sampling", step 3b), so the id stays a pure function of (logits, temperature, top_k, top_p, seed, pos).
+ * top_p == 1 is off: the id is then exactly kllm_sample_f32's.  Flat distributions whose nucleus does not fit
+ * the block's shared memory take a slower path over the whole vector.  KLLM_E_INVALID as kllm_sample_f32,
+ * and for top_p that is NaN, <= 0 or > 1. */
+int kllm_sample_top_p_f32(const float* logits, int64_t n, float temperature, int32_t top_k, float top_p,
+                          uint64_t seed, int32_t pos, int64_t* out_index, void* stream);
 
 /* ---- fused per-layer entry points -------------------------------------------------------
  * What LLama2Model::forward (llama3.cpp:147-167) calls instead of 15 launches per layer.
@@ -321,6 +330,12 @@ int kllm_decoder_generate_until(kllm_decoder* dec, int32_t first_token, int32_t 
  * The parameters live in device memory: no engine or graph is rebuilt.  Synchronises the decoder's
  * stream.  KLLM_E_INVALID for a temperature that is negative or not finite. */
 int kllm_decoder_set_sampling(kllm_decoder* dec, float temperature, int32_t top_k, uint64_t seed);
+/* kllm_decoder_set_sampling with nucleus sampling: each id is then the rule of kllm_sample_top_p_f32, in
+ * every entry that kllm_decoder_set_sampling covers (step, prompt, both batched prefills, generate and
+ * generate_until), on either engine and every tensor-parallel rank.  top_p == 1 is exactly
+ * kllm_decoder_set_sampling, which itself sets top_p back to 1.  KLLM_E_INVALID, with the settings in force
+ * left unchanged, for a temperature that is negative or not finite and for top_p that is NaN, <= 0 or > 1. */
+int kllm_decoder_set_sampling_top_p(kllm_decoder* dec, float temperature, int32_t top_k, float top_p, uint64_t seed);
 
 /* Blocking copies for tests: logits of the last step [vocab]; the KV cache in the REFERENCE
  * layout [layer][seq_len][kv_dim] (llama3.cpp:469-475) whatever the engine keeps internally. */

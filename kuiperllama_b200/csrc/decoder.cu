@@ -698,8 +698,16 @@ int kllm_decoder_generate_until(kllm_decoder* dc, int32_t first_token, int32_t s
 
 int kllm_decoder_set_sampling(kllm_decoder* dc, float temperature, int32_t top_k, uint64_t seed) {
   if (!dc || !std::isfinite(temperature) || temperature < 0.f) return KLLM_E_INVALID;
-  const SampleParams sp{temperature, top_k, seed};
+  const SampleParams sp{temperature, top_k, seed, 1.f};
   // no step of this decoder may still be reading the old parameters, and the next one reads the new
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  KLLM_TRY(cudaMemcpyAsync(dc->sampling, &sp, sizeof(sp), cudaMemcpyHostToDevice, dc->stream));
+  return static_cast<int>(cudaStreamSynchronize(dc->stream));
+}
+
+int kllm_decoder_set_sampling_top_p(kllm_decoder* dc, float temperature, int32_t top_k, float top_p, uint64_t seed) {
+  if (!dc || !std::isfinite(temperature) || temperature < 0.f || !(top_p > 0.f && top_p <= 1.f)) return KLLM_E_INVALID;
+  const SampleParams sp{temperature, top_k, seed, top_p};
   KLLM_TRY(cudaStreamSynchronize(dc->stream));
   KLLM_TRY(cudaMemcpyAsync(dc->sampling, &sp, sizeof(sp), cudaMemcpyHostToDevice, dc->stream));
   return static_cast<int>(cudaStreamSynchronize(dc->stream));

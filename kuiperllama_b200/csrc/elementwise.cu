@@ -363,6 +363,18 @@ int kllm_sample_f32(const float* logits, int64_t n, float temperature, int32_t t
   return static_cast<int>(cudaGetLastError());
 }
 
+int kllm_sample_top_p_f32(const float* logits, int64_t n, float temperature, int32_t top_k, float top_p,
+                          uint64_t seed, int32_t pos, int64_t* out_index, void* stream) {
+  if (!logits || !out_index || n <= 0 || n > 0x7fffffffLL || pos < 0) return KLLM_E_INVALID;
+  if (!std::isfinite(temperature) || temperature < 0.f) return KLLM_E_INVALID;
+  if (!(top_p > 0.f && top_p <= 1.f)) return KLLM_E_INVALID;
+  sample_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(logits, static_cast<int>(n),
+                                                                   SampleParams{temperature, top_k, seed, top_p}, pos,
+                                                                   reinterpret_cast<long long*>(out_index));
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
 int64_t kllm_argmax_f32_sync(const float* logits, int64_t n, void* stream) {
   static thread_local int64_t* d_idx = nullptr;
   if (d_idx == nullptr && cudaMalloc(&d_idx, sizeof(int64_t)) != cudaSuccess) return KLLM_E_NODEVICE;

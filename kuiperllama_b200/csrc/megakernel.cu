@@ -2110,16 +2110,17 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int p
   }
 }
 
-// ---- sampled id with top-k -----------------------------------------------------------------------
+// ---- sampled id with top-k or top-p --------------------------------------------------------------
 // tau needs all V logits, which are complete in L2 once the classifier's grid barrier is passed.  Every
 // CTA draws the id itself from them (no further barrier or hand-off) and gets the same one.  The per-CTA
-// maxima of the raw logits that the classifier (or the gather phase) left in arg_val / arg_idx bound tau
-// from below, so only the few logits near the top become candidates.  The scratch is the input-vector
+// maxima of the raw logits that the classifier (or the gather phase) left in arg_val / arg_idx bound the
+// top-k tau from below, so only the few logits near the top become candidates; top-p alone takes the
+// maximum from them.  The scratch is the input-vector
 // buffer: it is idle from the classifier's last read of its input until the next token stages its first
 // vector.  The barrier after the draw orders every thread's read of the result
 // before any thread writes that buffer again.
 template <int CW>
-__device__ __noinline__ int draw_top_k(const Params& P, int pos) {
+__device__ __noinline__ int draw_truncated(const Params& P, int pos) {
   const int id = sampling::draw_block<CW * 32>(P.logits, P.vocab_size, *P.sampling, pos, P.arg_val, P.arg_idx,
                                                static_cast<int>(gridDim.x), smem + kCtlBytes, P.xbuf_bytes,
                                                [] { consumer_sync<CW * 32>(); });
@@ -2523,11 +2524,11 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
     }
 
     // ---- greedy id: every CTA folds the per-CTA partials identically (argmax_kernel.cu:49-71
-    // semantics: maximum value, lowest index).  Sampling without top-k folds the same way: the
-    // partials are then the perturbed maxima.  With top-k every CTA draws the id itself. ----------------
+    // semantics: maximum value, lowest index).  Sampling without top-k or top-p folds the same way: the
+    // partials are then the perturbed maxima.  With either, every CTA draws the id itself. ---------------
     int next;
-    if (!(tok < P.skip_cls_tokens) && sampling::top_k_active(*P.sampling, P.vocab_size)) {
-      next = draw_top_k<CW>(P, pos);
+    if (!(tok < P.skip_cls_tokens) && sampling::needs_draw(*P.sampling, P.vocab_size)) {
+      next = draw_truncated<CW>(P, pos);
     } else {
       ArgBest b{0.f, -1};
       for (int c = lane; c < G; c += 32) arg_fold(b, __ldcg(P.arg_val + c), __ldcg(P.arg_idx + c));
@@ -2684,7 +2685,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     if (hs & 15) return KLLM_E_UNSUPPORTED;
     xbuf = std::max(xbuf, (2 * hs + consumer_warps_ * (hs + 2)) * 4);
   }
-  // the top-k draw's scratch after the classifier (draw_top_k): the histogram and at least 64 candidates
+  // the top-k / top-p draw's scratch after the classifier (draw_truncated): the histogram and at least 64 candidates
   xbuf = std::max(xbuf, sampling::kDrawScratchBase + 64 * 8);
   xbuf = (xbuf + 127) & ~127;
   const int xres = tagged_ ? ((dim * 4 + 127) & ~127) : 0;  // the CTA's copy of the residual stream

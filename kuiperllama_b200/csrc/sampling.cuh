@@ -2,11 +2,18 @@
 // (kllm_sample_f32, the graph engine's argmax_advance_kernel, the persistent megakernel).  Its numpy
 // mirror is kuiperllama_b200/sampling.py; DESIGN.md "Sampling" gives the reasons.
 //
-// Inputs: logits l[0..V) of position `pos`, temperature T, top_k k, 64-bit seed.
+// Inputs: logits l[0..V) of position `pos`, temperature T, top_k k, top_p, 64-bit seed.
 //   1. T == 0: greedy argmax (maximum, lowest index on ties) -- no noise is computed.
 //   2. s_i = l_i / T, IEEE division.
 //   3. 0 < k < V: tau = the k-th largest s_i; keep every i with s_i >= tau (ties at tau are kept).
 //      k <= 0 or k >= V keeps everything.
+//  3b. 0 < top_p < 1 (nucleus): K = the set kept by step 3, m = max over K of s_i.  Mass
+//      q_i = floor(expf(s_i - m) * 2^32) (fp32 weight, so the maximum's mass is 2^32 and a weight below 2^-32
+//      is mass 0); Z = sum over K of q_i and A_i = sum over K of q_j with s_j > s_i, both exact uint64.
+//      p24 = max(1, rint(top_p * 2^24)).  Keep i iff A_i * 2^24 < p24 * Z (exact, 128-bit): HF's "drop a
+//      token once the mass strictly above it reaches p", with equal s kept or dropped together.  The kept
+//      set is {s_i >= tau_p}; it always holds the maximum.  Integer sums do not depend on their order, so
+//      every block, engine and rank finds the same tau_p.
 //   4. Noise: Philox4x32-10, key (seed & 0xffffffff, seed >> 32).  Logit i takes word i & 3 of the
 //      block at counter (i >> 2, pos, 0, 0); u = ((x >> 8) + 0.5) * 2^-24 rounded toward zero to fp32
 //      (so u stays in (0, 1): the round-to-nearest of (2^24 - 0.5) * 2^-24 would be 1.0 and give an
@@ -19,15 +26,17 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <type_traits>
 
 namespace kllm {
 
 // Device-resident sampling parameters (kllm_decoder_set_sampling).  Engines read them when they run,
-// so changing them rebuilds nothing.  A zeroed struct is greedy.
+// so changing them rebuilds nothing.  A zeroed struct is greedy (and top_p 0 is off, as is 1).
 struct SampleParams {
   float temperature;
   int32_t top_k;
   uint64_t seed;
+  float top_p;
 };
 
 namespace sampling {
@@ -68,10 +77,38 @@ __device__ __forceinline__ bool top_k_active(const SampleParams& sp, int n) {
   return sp.temperature > 0.f && sp.top_k > 0 && sp.top_k < n;
 }
 
-// T > 0 without top-k: the id is a plain argmax of s_i + g_i, so the per-element values can be folded
-// wherever the logits are produced, with the greedy reduction unchanged
+__device__ __forceinline__ bool top_p_active(const SampleParams& sp) {
+  return sp.temperature > 0.f && sp.top_p > 0.f && sp.top_p < 1.f;
+}
+
+// T > 0 without top-k or top-p: the id is a plain argmax of s_i + g_i, so the per-element values can be
+// folded wherever the logits are produced, with the greedy reduction unchanged
 __device__ __forceinline__ bool perturb_only(const SampleParams& sp, int n) {
-  return sp.temperature > 0.f && !top_k_active(sp, n);
+  return sp.temperature > 0.f && !top_k_active(sp, n) && !top_p_active(sp);
+}
+
+// Top-k or top-p: the kept set needs a threshold over the whole vector, so one block draws the id
+__device__ __forceinline__ bool needs_draw(const SampleParams& sp, int n) {
+  return top_k_active(sp, n) || top_p_active(sp);
+}
+
+// Step 3b's mass of score s under the kept maximum m: floor(expf(s - m) * 2^32), at most 2^32
+__device__ __forceinline__ unsigned long long nucleus_mass(float s, float m) {
+  return __float2ull_rz(__fmul_rn(expf(__fsub_rn(s, m)), 0x1p32f));
+}
+
+// ceil(p24 * Z / 2^24): a token is kept iff the mass strictly above it is below this, so tau_p is the
+// largest s whose mass at or above it reaches it (p24 * Z < 2^74: the 128-bit product, then the shift)
+__device__ __forceinline__ unsigned long long nucleus_need(unsigned long long Z, float top_p) {
+  const unsigned long long p24 = max(1ull, static_cast<unsigned long long>(rintf(__fmul_rn(top_p, 0x1p24f))));
+  const unsigned long long lo = p24 * Z, hi = __umul64hi(p24, Z);
+  return ((hi << 40) | (lo >> 24)) + ((lo & 0xffffffull) != 0ull ? 1ull : 0ull);
+}
+
+// The bin of a score in the nucleus's first pass: 8 bins per unit of m - s, from the top; every token
+// with nonzero mass (m - s <= 22.2) lies in the first 178
+__device__ __forceinline__ int nucleus_bin(float s, float m) {
+  return 255 - min(255, static_cast<int>(__fmul_rn(__fsub_rn(m, s), 8.f)));
 }
 
 // (value, index): larger value wins, lowest index on ties -- the fold of the greedy argmax
@@ -93,10 +130,15 @@ __device__ __forceinline__ float key_value(unsigned k) {
 
 // Shared-memory scratch of draw_block; the candidate list (cap pairs) follows it.
 struct DrawScratch {
-  unsigned hist[256];
+  union {
+    unsigned hist[256];              // counts (top-k)
+    unsigned long long mass[256];    // masses (top-p)
+  };
+  unsigned long long sel_above, total;
+  unsigned long long red_q[32];
   float red_v[32];
   int red_i[32];
-  unsigned count, sel_digit, sel_above;
+  unsigned count, sel_digit;
   int result;
   float lbound;
 };
@@ -124,13 +166,55 @@ __device__ __forceinline__ int block_fold(float v, int i, DrawScratch& s, Sync s
   return s.result;
 }
 
-// k-th largest of get(0..m) (1 <= k <= m): radix select over order_key, 8 bits per pass, from the top
-template <int NT, class Get, class Sync>
-__device__ __forceinline__ float kth_largest(Get get, int m, int k, DrawScratch& s, Sync sync) {
+// Histogram scan of the selects: bins from 255 down, the first at which the running weight reaches
+// need(total) -> s.sel_digit, the weight of the bins before it -> s.sel_above, the total -> s.total.
+// Run by warp 0.
+template <class W, class Need>
+__device__ __forceinline__ void scan_bins(const W* hist, Need need, DrawScratch& s) {
+  const int lane = threadIdx.x & 31;
+  W c[8], tot = 0;  // lane l scans bins 255 - 8l down to 248 - 8l
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    c[j] = hist[255 - 8 * lane - j];
+    tot += c[j];
+  }
+  W inc = tot;
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+    const W o = __shfl_up_sync(0xffffffffu, inc, off);
+    if (lane >= off) inc += o;
+  }
+  const W total = __shfl_sync(0xffffffffu, inc, 31);
+  const W rem = need(total);
+  const int hit = __ffs(__ballot_sync(0xffffffffu, inc >= rem)) - 1;
+  if (lane == hit) {
+    W above = inc - tot;
+    bool found = false;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (!found && above + c[j] >= rem) {
+        s.sel_digit = static_cast<unsigned>(255 - 8 * lane - j);
+        s.sel_above = above;
+        found = true;
+      }
+      if (!found) above += c[j];
+    }
+  }
+  if (lane == 0) s.total = total;
+}
+
+// The largest value v of get(0..m) whose weight at or above v reaches `need` (0 < need <= total weight):
+// radix select over order_key, 8 bits per pass, from the top.  W = unsigned counts (weight 1 each) gives
+// the k-th largest; W = unsigned long long gives step 3b's tau_p with the nucleus masses as weights.
+template <int NT, class W, class Get, class Weight, class Sync>
+__device__ __forceinline__ float select_top(Get get, Weight weight, int m, W need, DrawScratch& s, Sync sync) {
+  constexpr bool kCount = std::is_same<W, unsigned>::value;
+  W* hist = reinterpret_cast<W*>(kCount ? static_cast<void*>(s.hist) : static_cast<void*>(s.mass));
   const int tid = threadIdx.x, lane = tid & 31;
-  unsigned prefix = 0u, mask = 0u, rem = static_cast<unsigned>(k);
+  unsigned prefix = 0u, mask = 0u;
+  W rem = need;
   for (int shift = 24; shift >= 0; shift -= 8) {
-    for (int b = tid; b < 256; b += NT) s.hist[b] = 0u;
+    for (int b = tid; b < 256; b += NT) hist[b] = 0;
     sync();
     for (int i0 = 0; i0 < m; i0 += NT) {
       const int i = i0 + tid;
@@ -139,57 +223,70 @@ __device__ __forceinline__ float kth_largest(Get get, int m, int k, DrawScratch&
         const unsigned key = order_key(get(i));
         if ((key & mask) == prefix) bin = static_cast<int>((key >> shift) & 255u);
       }
-      // logits bunch into few bins: one shared atomic per distinct bin of the warp
-      const unsigned peers = __match_any_sync(0xffffffffu, bin);
-      if (bin >= 0 && lane == __ffs(peers) - 1) atomicAdd(&s.hist[bin], static_cast<unsigned>(__popc(peers)));
-    }
-    sync();
-    if (tid < 32) {  // lane l scans bins 255 - 8l down to 248 - 8l
-      unsigned c[8], tot = 0u;
+      if constexpr (kCount) {
+        // logits bunch into few bins: one shared atomic per distinct bin of the warp
+        const unsigned peers = __match_any_sync(0xffffffffu, bin);
+        if (bin >= 0 && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], static_cast<unsigned>(__popc(peers)));
+      } else {
+        W w = bin >= 0 ? weight(i) : W(0);
+        // flat distributions put whole warps into one bin: one atomic for the warp's sum then
+        if (__match_any_sync(0xffffffffu, bin) == 0xffffffffu) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        c[j] = s.hist[255 - 8 * lane - j];
-        tot += c[j];
-      }
-      unsigned inc = tot;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const unsigned o = __shfl_up_sync(0xffffffffu, inc, off);
-        if (lane >= off) inc += o;
-      }
-      const int hit = __ffs(__ballot_sync(0xffffffffu, inc >= rem)) - 1;
-      if (lane == hit) {
-        unsigned above = inc - tot;
-        bool found = false;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (!found && above + c[j] >= rem) {
-            s.sel_digit = static_cast<unsigned>(255 - 8 * lane - j);
-            s.sel_above = above;
-            found = true;
-          }
-          if (!found) above += c[j];
+          for (int off = 16; off > 0; off >>= 1) w += __shfl_xor_sync(0xffffffffu, w, off);
+          if (lane == 0 && bin >= 0 && w != 0) atomicAdd(&hist[bin], w);
+        } else if (w != 0) {
+          atomicAdd(&hist[bin], w);
         }
       }
     }
     sync();
+    if (tid < 32) scan_bins<W>(hist, [rem](W) { return rem; }, s);
+    sync();
     prefix |= s.sel_digit << shift;
     mask |= 0xffu << shift;
-    rem -= s.sel_above;
+    rem -= static_cast<W>(s.sel_above);
   }
   return key_value(prefix);
 }
 
+// k-th largest of get(0..m) (1 <= k <= m)
+template <int NT, class Get, class Sync>
+__device__ __forceinline__ float kth_largest(Get get, int m, int k, DrawScratch& s, Sync sync) {
+  return select_top<NT, unsigned>(get, [](int) { return 1u; }, m, static_cast<unsigned>(k), s, sync);
+}
+
+// Sum of v over the block, returned in every thread
+template <int NT, class Sync>
+__device__ __forceinline__ unsigned long long block_sum(unsigned long long v, DrawScratch& s, Sync sync) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(0xffffffffu, v, off);
+  if (lane == 0) s.red_q[warp] = v;
+  sync();
+  unsigned long long t = 0ull;
+#pragma unroll
+  for (int w = 0; w < NT / 32; ++w) t += s.red_q[w];
+  sync();
+  return t;
+}
+
 // The rule, drawn by one block of NT threads over logits[0..n) (device memory, read through L2).  Returns
 // the id in every thread.  `scratch` (16-byte aligned shared memory, scratch_bytes >= kDrawScratchBase)
-// holds the histogram and a list of top-k candidates.
+// holds the histogram and a list of candidates.
 //
 // Top-k without a full sort: a lower bound L of the k-th largest logit comes from the maxima of disjoint
 // parts of the vector (k of them are k distinct logits >= L): `maxima` / `maxima_idx` (an index < 0
 // marks an empty part) when the caller has them, else the block's per-thread maxima.  Only logits
 // that can still reach tau after the division by T (l >= L less a few ulp) become candidates; tau and
-// the kept argmax are then taken over the candidates in shared memory.  When they do not fit, the
-// same selection runs over the whole vector instead.
+// the kept argmax are then taken over the candidates in shared memory.
+//
+// Top-p with top-k runs step 3b over the top-k candidates.  Top-p alone takes the maximum from the same
+// maxima (else one more pass).  One pass then sums the masses into 256 bins of 1/8 of m - s (Z, and the
+// first bins whose mass reaches the need, which bound tau_p from below) and collects the scores within 8 of
+// m.  When the nucleus reaches below those, or they do not fit, a second pass collects the logits of the
+// bins from the one where the mass reaches the need.  tau_p is the mass-weighted select over the candidates.
+//
+// When the candidates do not fit, the same selections run over the whole vector instead.
 template <int NT, class Sync>
 __device__ __forceinline__ int draw_block(const float* logits, int n, const SampleParams sp, int pos,
                                           const float* maxima, const int* maxima_idx, int n_maxima,
@@ -213,7 +310,8 @@ __device__ __forceinline__ int draw_block(const float* logits, int n, const Samp
     return block_fold<NT>(bv, bi, s, sync);
   }
   const uint2 key = seed_key(sp.seed);
-  if (!top_k_active(sp, n)) {  // one Philox block serves four consecutive logits
+  const bool tk = top_k_active(sp, n), tp = top_p_active(sp);
+  if (!tk && !tp) {  // one Philox block serves four consecutive logits
     for (int j = tid; j < ((n + 3) >> 2); j += NT) {
       const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(j), static_cast<uint32_t>(pos), 0u, 0u), key);
 #pragma unroll
@@ -225,68 +323,164 @@ __device__ __forceinline__ int draw_block(const float* logits, int n, const Samp
     return block_fold<NT>(bv, bi, s, sync);
   }
 
-  // ---- top-k: lower bound L of the k-th largest logit ----
-  const int k = sp.top_k;
-  if (maxima == nullptr) {  // per-thread maxima (cap >= NT)
-    float mx = -INFINITY;
-    for (int i = tid; i < n; i += NT) mx = fmaxf(mx, __ldcg(logits + i));
-    cand_s[tid] = mx;
-    n_maxima = NT;
-  }
-  if (tid == 0) {
-    s.lbound = -INFINITY;
-    s.count = 0u;
-  }
-  sync();
-  auto max_at = [&](int j) {
-    if (maxima == nullptr) return cand_s[j];
-    return maxima_idx[j] < 0 ? -INFINITY : __ldcg(maxima + j);
-  };
-  if (k <= n_maxima) {  // L = the maximum with exactly k - 1 ahead of it (larger, or equal and earlier)
-    for (int t = tid; t < n_maxima; t += NT) {
-      const float v = max_at(t);
-      int ahead = 0;
-      for (int j = 0; j < n_maxima; ++j) {
-        const float w = max_at(j);
-        ahead += (w > v || (w == v && j < t)) ? 1 : 0;
-      }
-      if (ahead == k - 1) s.lbound = v;
-    }
-  }
-  sync();
-  const float L = s.lbound;
-  // l < L can still give l / T == L / T after rounding: admit everything within 2^-20 relative of L
-  const float lo = isfinite(L) ? L - (fabsf(L) * 0x1p-20f + T * 0x1p-126f) : -INFINITY;
-
-  // ---- candidates: kUnroll independent L2 loads in flight per thread, then the warp-aggregated appends ----
+  // f(l, i, valid) over the whole vector, kUnroll independent L2 loads in flight per thread; every lane
+  // calls f the same number of times (f may use warp votes)
   constexpr int kUnroll = 16;
-  for (int i0 = 0; i0 < n; i0 += NT * kUnroll) {
-    float l[kUnroll];
+  auto for_each_logit = [&](auto f) {
+    for (int i0 = 0; i0 < n; i0 += NT * kUnroll) {
+      float l[kUnroll];
 #pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const int i = i0 + u * NT + tid;
-      l[u] = i < n ? __ldcg(logits + i) : -INFINITY;
+      for (int u = 0; u < kUnroll; ++u) {
+        const int i = i0 + u * NT + tid;
+        l[u] = i < n ? __ldcg(logits + i) : -INFINITY;
+      }
+#pragma unroll
+      for (int u = 0; u < kUnroll; ++u) f(l[u], i0 + u * NT + tid, i0 + u * NT + tid < n);
     }
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const int i = i0 + u * NT + tid;
-      const bool c = i < n && l[u] >= lo;
-      const unsigned ball = __ballot_sync(0xffffffffu, c);
-      if (ball == 0u) continue;
-      unsigned base = 0u;
-      if (lane == 0) base = atomicAdd(&s.count, static_cast<unsigned>(__popc(ball)));
-      base = __shfl_sync(0xffffffffu, base, 0);
-      const int slot = static_cast<int>(base) + __popc(ball & ((1u << lane) - 1u));
-      if (c && slot < cap) {
-        cand_s[slot] = __fdiv_rn(l[u], T);
-        cand_i[slot] = i;
+  };
+  // the block's maximum logit, by a pass over the vector
+  auto max_logit = [&]() {
+    float v = 0.f;
+    int vi = -1;
+    for (int i = tid; i < n; i += NT) fold(v, vi, __ldcg(logits + i), i);
+    return __ldcg(logits + block_fold<NT>(v, vi, s, sync));
+  };
+
+  float mx = 0.f;                    // m of step 3b (top-p alone: known before the candidates are taken)
+  unsigned long long need = 0ull;    // nucleus_need(Z) (likewise)
+  float lo = -INFINITY;              // the candidates are logits l >= lo (and more conditions for top-p alone)
+  if (tid == 0) s.count = 0u;        // (published by the barriers of either branch)
+  if (tk) {
+    // ---- top-k: lower bound L of the k-th largest logit ----
+    const int k = sp.top_k;
+    if (maxima == nullptr) {  // per-thread maxima (cap >= NT)
+      float mxl = -INFINITY;
+      for (int i = tid; i < n; i += NT) mxl = fmaxf(mxl, __ldcg(logits + i));
+      cand_s[tid] = mxl;
+      n_maxima = NT;
+    }
+    if (tid == 0) s.lbound = -INFINITY;
+    sync();
+    auto max_at = [&](int j) {
+      if (maxima == nullptr) return cand_s[j];
+      return maxima_idx[j] < 0 ? -INFINITY : __ldcg(maxima + j);
+    };
+    if (k <= n_maxima) {  // L = the maximum with exactly k - 1 ahead of it (larger, or equal and earlier)
+      for (int t = tid; t < n_maxima; t += NT) {
+        const float v = max_at(t);
+        int ahead = 0;
+        for (int j = 0; j < n_maxima; ++j) {
+          const float w = max_at(j);
+          ahead += (w > v || (w == v && j < t)) ? 1 : 0;
+        }
+        if (ahead == k - 1) s.lbound = v;
       }
     }
+    sync();
+    const float L = s.lbound;
+    // l < L can still give l / T == L / T after rounding: admit everything within 2^-20 relative of L
+    lo = isfinite(L) ? L - (fabsf(L) * 0x1p-20f + T * 0x1p-126f) : -INFINITY;
+  } else {
+    // ---- top-p alone: the maximum (from the parts' maxima when the caller has them) ----
+    float lmax;
+    if (maxima != nullptr) {
+      for (int j = tid; j < n_maxima; j += NT)
+        if (maxima_idx[j] >= 0) fold(bv, bi, __ldcg(maxima + j), j);
+      lmax = __ldcg(maxima + block_fold<NT>(bv, bi, s, sync));
+      bv = 0.f;
+      bi = -1;
+    } else {
+      lmax = max_logit();
+    }
+    mx = __fdiv_rn(lmax, T);
+    // raw logits below this have s < m - 23, mass 0 (expf(-23) 2^32 < 1): skipped without the division
+    lo = lmax - (23.f * T + (fabsf(lmax) + 23.f * T) * 0x1p-16f);
   }
-  sync();
-  const int m = static_cast<int>(s.count);
+
+  // ---- candidates (s, i) = (l / T, i): warp-aggregated appends (beyond cap: counted, not stored) ----
+  auto append = [&](bool c, float sv, int i) {
+    const unsigned ball = __ballot_sync(0xffffffffu, c);
+    if (ball == 0u) return;
+    unsigned base = 0u;
+    if (lane == 0) base = atomicAdd(&s.count, static_cast<unsigned>(__popc(ball)));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    const int slot = static_cast<int>(base) + __popc(ball & ((1u << lane) - 1u));
+    if (c && slot < cap) {
+      cand_s[slot] = sv;
+      cand_i[slot] = i;
+    }
+  };
+  // one pass: the logits l >= lo with keep(l) become candidates; returns their count
+  auto collect = [&](auto keep) {
+    for_each_logit([&](float l, int i, bool valid) {
+      const bool c = valid && l >= lo && keep(l);
+      append(c, c ? __fdiv_rn(l, T) : 0.f, i);
+    });
+    sync();
+    return static_cast<int>(s.count);
+  };
+  int m;
+  if (tk) {
+    m = collect([](float) { return true; });
+  } else {
+    // ---- top-p alone, one pass: the masses into 256 bins of 1/8 of m - s (Z, and the first bins whose
+    // mass reaches the need), while the scores within 8 of m become candidates ----
+    constexpr int kNearBin = 255 - 64;
+    for (int b = tid; b < 256; b += NT) s.mass[b] = 0ull;
+    sync();
+    for_each_logit([&](float l, int i, bool valid) {
+      float sv = 0.f;
+      int bin = -1;
+      unsigned long long q = 0ull;
+      if (valid && l >= lo) {
+        sv = __fdiv_rn(l, T);
+        if (__fsub_rn(mx, sv) < 23.f) {
+          q = nucleus_mass(sv, mx);
+          bin = nucleus_bin(sv, mx);
+        }
+      }
+      if (__match_any_sync(0xffffffffu, bin) == 0xffffffffu) {  // a flat stretch: one atomic per warp
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) q += __shfl_xor_sync(0xffffffffu, q, off);
+        if (lane == 0 && q != 0ull) atomicAdd(&s.mass[bin], q);
+      } else if (q != 0ull) {
+        atomicAdd(&s.mass[bin], q);
+      }
+      append(bin >= kNearBin, sv, i);
+    });
+    sync();
+    if (tid < 32) scan_bins<unsigned long long>(s.mass, [&](unsigned long long Z) { return nucleus_need(Z, sp.top_p); }, s);
+    sync();
+    const int top_bin = static_cast<int>(s.sel_digit);
+    need = nucleus_need(s.total, sp.top_p);
+    m = static_cast<int>(s.count);
+    if (top_bin < kNearBin || m > cap) {
+      // the nucleus reaches below the candidates, or they overflowed: a second pass collects the bins
+      // from the one where the mass reaches the need
+      sync();
+      if (tid == 0) s.count = 0u;
+      sync();
+      m = collect([&](float l) { return nucleus_bin(__fdiv_rn(l, T), mx) >= top_bin; });
+    }
+  }
   if (m <= cap) {
-    const float tau = kth_largest<NT>([&](int c) { return cand_s[c]; }, m, k, s, sync);
+    auto cand = [&](int c) { return cand_s[c]; };
+    const float tau_k = tk ? kth_largest<NT>(cand, m, sp.top_k, s, sync) : -INFINITY;
+    float tau = tau_k;
+    if (tp) {
+      if (tk) {  // step 3b over the top-k candidates: their maximum and Z
+        for (int c = tid; c < m; c += NT) fold(bv, bi, cand_s[c], c);
+        mx = cand_s[block_fold<NT>(bv, bi, s, sync)];
+        bv = 0.f;
+        bi = -1;
+        unsigned long long z = 0ull;
+        for (int c = tid; c < m; c += NT)
+          if (cand_s[c] >= tau_k) z += nucleus_mass(cand_s[c], mx);
+        need = nucleus_need(block_sum<NT>(z, s, sync), sp.top_p);
+      }
+      tau = select_top<NT, unsigned long long>(
+          cand, [&](int c) { return cand_s[c] >= tau_k ? nucleus_mass(cand_s[c], mx) : 0ull; }, m, need, s, sync);
+    }
     for (int c = tid; c < m; c += NT) {
       const float sv = cand_s[c];
       if (sv >= tau) {
@@ -295,8 +489,24 @@ __device__ __forceinline__ int draw_block(const float* logits, int n, const Samp
         fold(bv, bi, __fadd_rn(sv, gumbel(pick(r, i & 3))), i);
       }
     }
-  } else {  // too many candidates for the scratch: the same selection over the whole vector
-    const float tau = kth_largest<NT>([&](int i) { return __fdiv_rn(__ldcg(logits + i), T); }, n, k, s, sync);
+  } else {  // too many candidates for the scratch: the same selections over the whole vector
+    auto score = [&](int i) { return __fdiv_rn(__ldcg(logits + i), T); };
+    const float tau_k = tk ? kth_largest<NT>(score, n, sp.top_k, s, sync) : -INFINITY;
+    float tau = tau_k;
+    if (tp) {
+      if (tk) {
+        mx = __fdiv_rn(max_logit(), T);
+        unsigned long long z = 0ull;
+        for (int i = tid; i < n; i += NT) {
+          const float sv = score(i);
+          if (sv >= tau_k) z += nucleus_mass(sv, mx);
+        }
+        need = nucleus_need(block_sum<NT>(z, s, sync), sp.top_p);
+      }
+      tau = select_top<NT, unsigned long long>(
+          score, [&](int i) { const float sv = score(i); return sv >= tau_k ? nucleus_mass(sv, mx) : 0ull; }, n, need,
+          s, sync);
+    }
     for (int i = tid; i < n; i += NT) {
       const float l = __ldcg(logits + i);
       if (__fdiv_rn(l, T) >= tau) fold(bv, bi, perturbed(l, T, key, pos, i), i);

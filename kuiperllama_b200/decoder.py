@@ -288,11 +288,17 @@ class Decoder:
             raise errors[0]
         return list(out[:n_out.value])
 
-    def set_sampling(self, temperature: float, top_k: int = 0, seed: int = 0):
+    def set_sampling(self, temperature: float, top_k: int = 0, seed: int = 0, top_p: float = 1.0):
         """Draw every later id by the sampling rule (kllm_decoder_set_sampling; sampling.py mirrors it)
-        instead of the greedy argmax; temperature 0 is greedy again."""
-        check(self.lib.kllm_decoder_set_sampling(self.handle, float(temperature), int(top_k), int(seed)),
-              "kllm_decoder_set_sampling")
+        instead of the greedy argmax; temperature 0 is greedy again.  top_p < 1 adds nucleus sampling after
+        top-k (kllm_decoder_set_sampling_top_p)."""
+        if top_p == 1.0:
+            check(self.lib.kllm_decoder_set_sampling(self.handle, float(temperature), int(top_k), int(seed)),
+                  "kllm_decoder_set_sampling")
+        else:
+            check(self.lib.kllm_decoder_set_sampling_top_p(self.handle, float(temperature), int(top_k),
+                                                           float(top_p), int(seed)),
+                  "kllm_decoder_set_sampling_top_p")
 
     def logits(self):
         import numpy as np

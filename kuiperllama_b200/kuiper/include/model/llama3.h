@@ -92,10 +92,14 @@ class LLama2Model : public Model {
   // post_processing on the layer path draw the same id: a pure function of the logits, the settings and
   // the position.  Under tensor parallelism every rank reads the same settings and draws the same id.
   void set_sampling(float temperature, int32_t top_k, uint64_t seed);
-  // the settings in force (after init(): the environment's when set_sampling was not called)
+  // Nucleus sampling after top-k (kllm_decoder_set_sampling_top_p): call before init(); without a call init()
+  // takes it from KUIPER_TOP_P.  Unset or 1 is off; init() refuses a value that is NaN, <= 0 or > 1.
+  void set_top_p(float top_p);
+  // the settings in force (after init(): the environment's when set_sampling / set_top_p was not called)
   float sampling_temperature() const { return temperature_; }
   int32_t sampling_top_k() const { return top_k_; }
   uint64_t sampling_seed() const { return seed_; }
+  float sampling_top_p() const { return top_p_; }
 
   // A whole generation on the fused decoder, without a host round trip per token:
   //   1. the prompt from position 0 (the batched prefill for all but its last token when batched_prefill() is
@@ -159,6 +163,8 @@ class LLama2Model : public Model {
   int32_t top_k_ = 0;
   uint64_t seed_ = 0;
   bool sampling_explicit_ = false;
+  float top_p_ = 1.f;
+  bool top_p_explicit_ = false;
   sampler::SeededSampler* seeded_ = nullptr;  // sampler_ when sampling, else null
   std::vector<int32_t> extra_stop_ids_;       // set_stop_ids()
   mutable uint64_t embedding_calls_ = 0;

@@ -1,6 +1,6 @@
-// Seeded temperature / top-k sampling beside the greedy ArgmaxSampler: the id is drawn on the device by the
-// rule of kllm_sample_f32 (DESIGN.md "Sampling"), a pure function of the logits, the settings and the
-// position.  The model sets the position of the logits before each sample() (post_processing).
+// Seeded temperature / top-k / top-p sampling beside the greedy ArgmaxSampler: the id is drawn on the device by
+// the rule of kllm_sample_top_p_f32 (DESIGN.md "Sampling"), a pure function of the logits, the settings and the
+// position.  top_p 1 (the default) is kllm_sample_f32's rule.  The model sets the position of the logits before each sample() (post_processing).
 #ifndef KLLM_KUIPER_SAMPLER_SEEDED_SAMPLER_H_
 #define KLLM_KUIPER_SAMPLER_SEEDED_SAMPLER_H_
 #include <cstdint>
@@ -10,8 +10,8 @@
 namespace sampler {
 class SeededSampler final : public Sampler {
  public:
-  SeededSampler(base::DeviceType device_type, float temperature, int32_t top_k, uint64_t seed)
-      : Sampler(device_type), temperature_(temperature), top_k_(top_k), seed_(seed) {}
+  SeededSampler(base::DeviceType device_type, float temperature, int32_t top_k, uint64_t seed, float top_p = 1.f)
+      : Sampler(device_type), temperature_(temperature), top_k_(top_k), seed_(seed), top_p_(top_p) {}
   void set_position(int32_t pos) { pos_ = pos; }
   size_t sample(const float* logits, size_t size, void* stream) override;
 
@@ -19,6 +19,7 @@ class SeededSampler final : public Sampler {
   float temperature_;
   int32_t top_k_;
   uint64_t seed_;
+  float top_p_;
   int32_t pos_ = 0;
 };
 }  // namespace sampler

@@ -84,6 +84,11 @@ void LLama2Model::set_sampling(float temperature, int32_t top_k, uint64_t seed) 
   sampling_explicit_ = true;
 }
 
+void LLama2Model::set_top_p(float top_p) {
+  top_p_ = top_p;
+  top_p_explicit_ = true;
+}
+
 const char* LLama2Model::decoder_engine() const { return decoder_ ? kllm_decoder_engine(decoder_) : ""; }
 
 base::Status LLama2Model::init(base::DeviceType device_type) {
@@ -114,6 +119,12 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   }
   if (!std::isfinite(temperature_) || temperature_ < 0.f)
     return error::InvalidArgument("sampling: the temperature must be finite and >= 0 (KUIPER_TEMPERATURE / set_sampling)");
+  if (!top_p_explicit_) {
+    const char* p = std::getenv("KUIPER_TOP_P");
+    top_p_ = p != nullptr ? std::strtof(p, nullptr) : 1.f;
+  }
+  if (!(top_p_ > 0.f && top_p_ <= 1.f))
+    return error::InvalidArgument("sampling: top_p must be in (0, 1] (KUIPER_TOP_P / set_top_p)");
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
     return error::InternalError("No usable CUDA device " + std::to_string(tp_.cuda_device()) + ".");
   cuda_config_ = std::make_shared<kernel::CudaConfig>();
@@ -126,7 +137,7 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   kernel::sin_cos_cache_calc_cu(config_->head_size_, config_->seq_len_, get_buffer(ModelBufferType::kSinCache),
                                 get_buffer(ModelBufferType::kCosCache), cuda_config_->stream);
   if (temperature_ > 0.f) {
-    auto seeded = std::make_unique<sampler::SeededSampler>(device_type_, temperature_, top_k_, seed_);
+    auto seeded = std::make_unique<sampler::SeededSampler>(device_type_, temperature_, top_k_, seed_, top_p_);
     seeded_ = seeded.get();
     sampler_ = std::move(seeded);
   } else {
@@ -500,10 +511,12 @@ base::Status LLama2Model::create_decoder() {
   if (rc != 0)
     return base::error::InternalError(std::string("kllm_decoder_create failed: ") + kllm_error_string(rc));
   if (temperature_ > 0.f) {
-    const int src = kllm_decoder_set_sampling(decoder_, temperature_, top_k_, seed_);
+    const int src = kllm_decoder_set_sampling_top_p(decoder_, temperature_, top_k_, top_p_, seed_);
     if (src != 0)
-      return base::error::InternalError(std::string("kllm_decoder_set_sampling failed: ") + kllm_error_string(src));
-    LOG(INFO) << "sampling: temperature " << temperature_ << ", top_k " << top_k_ << ", seed " << seed_;
+      return base::error::InternalError(std::string("kllm_decoder_set_sampling_top_p failed: ") +
+                                        kllm_error_string(src));
+    LOG(INFO) << "sampling: temperature " << temperature_ << ", top_k " << top_k_ << ", top_p " << top_p_
+              << ", seed " << seed_;
   }
   LOG(INFO) << "fused decoder engine: " << kllm_decoder_engine(decoder_) << ", "
             << kllm_decoder_launches_per_step(decoder_) << " launch(es) per token";

@@ -191,8 +191,9 @@ size_t sampler::SeededSampler::sample(const float* logits, size_t size, void* st
   CHECK(device_type_ == base::DeviceType::kDeviceCUDA) << "SeededSampler: CUDA logits only (no CPU backend)";
   static thread_local int64_t* d_idx = nullptr;
   if (d_idx == nullptr) CHECK(cudaMalloc(reinterpret_cast<void**>(&d_idx), sizeof(int64_t)) == cudaSuccess) << "SeededSampler: cudaMalloc";
-  const int rc = kllm_sample_f32(logits, static_cast<int64_t>(size), temperature_, top_k_, seed_, pos_, d_idx, stream);
-  CHECK(rc == 0) << "kllm_sample_f32: " << kllm_error_string(rc);
+  const int rc =
+      kllm_sample_top_p_f32(logits, static_cast<int64_t>(size), temperature_, top_k_, top_p_, seed_, pos_, d_idx, stream);
+  CHECK(rc == 0) << "kllm_sample_top_p_f32: " << kllm_error_string(rc);
   int64_t h = -1;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CHECK(cudaMemcpyAsync(&h, d_idx, sizeof(h), cudaMemcpyDeviceToHost, s) == cudaSuccess &&

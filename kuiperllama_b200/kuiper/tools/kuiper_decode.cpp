@@ -2,7 +2,7 @@
 // drives it with text (embedding -> fill_input -> predict per position).
 //
 //   kuiper_decode <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...]
-//                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED]
+//                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P]
 //                 [--generate N [--stop ID]... [--then K]]
 //
 // --generate N runs the prompt and LLama2Model::generate() for at most N ids instead (n_steps is then unused),
@@ -10,12 +10,13 @@
 // by the ids of K more predict() steps on the same sequence with --then K.
 //
 // ids are the prompt; after the prompt the model free-runs (greedily, or by the model's sampling
-// settings: KUIPER_TEMPERATURE / KUIPER_TOP_K / KUIPER_SEED) until n_steps positions have been processed.  Prints the id chosen at every position (-1 for prompt steps before the
+// settings: KUIPER_TEMPERATURE / KUIPER_TOP_K / KUIPER_TOP_P / KUIPER_SEED) until n_steps positions have been processed.  Prints the id chosen at every position (-1 for prompt steps before the
 // last prompt token) on one line.  --layers uses Model::forward (layer-by-layer op registry path)
 // instead of predict's fused decoder.  --copy-at K hands predict() a COPY of the embedding row at
 // position K (so that step cannot be recognised and runs layer by layer in the middle of a sequence
 // the fused decoder started).  --logits writes the last position's logits as raw fp32.  --sampling calls
-// LLama2Model::set_sampling(T, K, SEED) before init() instead of leaving it to the environment.
+// LLama2Model::set_sampling(T, K, SEED) before init() instead of leaving it to the environment, and --top-p
+// LLama2Model::set_top_p(P) instead of KUIPER_TOP_P.
 #include <base/base.h>
 #include <cuda_runtime_api.h>
 #include <glog/logging.h>
@@ -34,7 +35,7 @@
 int main(int argc, char** argv) {
   if (argc < 6) {
     std::fprintf(stderr, "usage: %s <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...] "
-                         "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] "
+                         "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P] "
                          "[--generate N [--stop ID]... [--then K]]\n", argv[0]);
     return 2;
   }
@@ -48,6 +49,8 @@ int main(int argc, char** argv) {
   float temperature = 0.f;
   int32_t top_k = 0;
   uint64_t seed = 0;
+  bool set_top_p = false;
+  float top_p = 1.f;
   int generate = 0, then = 0;
   std::vector<int32_t> stops;
   for (int i = 5; i < argc; ++i) {
@@ -57,6 +60,10 @@ int main(int argc, char** argv) {
       temperature = std::strtof(argv[++i], nullptr);
       top_k = static_cast<int32_t>(std::strtol(argv[++i], nullptr, 10));
       seed = std::strtoull(argv[++i], nullptr, 10);
+    }
+    else if (!std::strcmp(argv[i], "--top-p") && i + 1 < argc) {
+      set_top_p = true;
+      top_p = std::strtof(argv[++i], nullptr);
     }
     else if (!std::strcmp(argv[i], "--generate") && i + 1 < argc) generate = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--stop") && i + 1 < argc) stops.push_back(std::atoi(argv[++i]));
@@ -75,6 +82,7 @@ int main(int argc, char** argv) {
     m = std::make_unique<model::LLama2Model>(base::TokenizerType::kEncodeSpe, "<none>", checkpoint, quant);
   }
   if (set_sampling) m->set_sampling(temperature, top_k, seed);
+  if (set_top_p) m->set_top_p(top_p);
   if (!stops.empty()) m->set_stop_ids(stops);
   base::Status st = m->init(base::DeviceType::kDeviceCUDA);
   if (!st) {
@@ -115,7 +123,8 @@ int main(int argc, char** argv) {
   std::unique_ptr<sampler::SeededSampler> seeded;
   if (m->sampling_temperature() > 0.f)
     seeded = std::make_unique<sampler::SeededSampler>(base::DeviceType::kDeviceCUDA, m->sampling_temperature(),
-                                                      m->sampling_top_k(), m->sampling_seed());
+                                                      m->sampling_top_k(), m->sampling_seed(),
+                                                      m->sampling_top_p());
   std::vector<float> host_logits;
   int next = -1;
   std::vector<int> chosen;

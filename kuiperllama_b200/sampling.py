@@ -45,31 +45,105 @@ def gumbel(x) -> np.ndarray:
     return -np.log(-np.log(uniform(x)))
 
 
-def scores(logits, temperature: float, top_k: int, seed: int, pos: int):
+NUCLEUS_EPS = 1e-6
+"""np.exp and the device expf may differ in the last ulps of each weight, which moves A and Z by well under
+this much of Z: a nucleus comparison closer than that may go either way on the device."""
+
+
+def top_p_active(temperature: float, top_p: float) -> bool:
+    """Step 3b runs for T > 0 and 0 < top_p < 1 (top_p as the device's fp32)."""
+    p = np.float32(top_p)
+    return temperature > 0 and bool(0 < p < 1)
+
+
+def nucleus_masses(s) -> np.ndarray:
+    """q_i = floor(w_i * 2^32), w_i = exp(s_i - max s) in fp32, of the kept scores s (int64, exact)."""
+    s = np.asarray(s, np.float32)
+    w = np.exp(s - s.max())
+    return np.floor(w.astype(np.float64) * 2.0 ** 32).astype(np.int64)
+
+
+def _nucleus(s, top_p: float):
+    """Over the kept scores s: the distinct values u (ascending), the mass strictly above each (A), Z, p24
+    and J, the index in u of the smallest kept value."""
+    u, inv = np.unique(np.asarray(s, np.float32), return_inverse=True)
+    mass = np.zeros(u.shape[0], np.int64)
+    np.add.at(mass, inv, nucleus_masses(s))
+    above = np.concatenate([np.cumsum(mass[::-1])[::-1][1:], np.zeros(1, np.int64)])
+    z = int(mass.sum())
+    p24 = max(1, int(np.rint(np.float64(np.float32(top_p)) * 2.0 ** 24)))
+    need = -(-p24 * z // 2 ** 24)  # A * 2^24 < p24 * Z  <=>  A < ceil(p24 * Z / 2^24), A an integer
+    j = int(np.argmax(above < need))  # `above` falls as u grows; the largest value has A = 0 < need
+    return u, above, z, p24, j
+
+
+def nucleus_threshold(s, top_p: float) -> np.float32:
+    """tau_p of step 3b over the kept scores s: keep s_i >= tau_p."""
+    u, _, _, _, j = _nucleus(s, top_p)
+    return u[j]
+
+
+def _keep(s, top_k: int, top_p: float, shift: int = 0):
+    """The kept set of steps 3 and 3b (shift moves tau_p by that many distinct values: the margin's what-if)."""
+    n = s.shape[0]
+    keep = np.ones(n, bool)
+    if 0 < top_k < n:
+        keep = s >= np.partition(s, n - top_k)[n - top_k]
+    if top_p_active(1.0, top_p):
+        u, _, _, _, j = _nucleus(s[keep], top_p)
+        keep &= s >= u[min(max(j + shift, 0), u.shape[0] - 1)]
+    return keep
+
+
+def scores(logits, temperature: float, top_k: int, seed: int, pos: int, top_p: float = 1.0, _shift: int = 0):
     """s_i + g_i for the kept i, -inf for the others (temperature > 0)."""
     s = np.asarray(logits, np.float32) / np.float32(temperature)
     n = s.shape[0]
     v = s + gumbel_noise(n, seed, pos)
-    if 0 < top_k < n:
-        tau = np.partition(s, n - top_k)[n - top_k]
-        v = np.where(s >= tau, v, np.float32(-np.inf))
+    if 0 < top_k < n or top_p_active(temperature, top_p):
+        v = np.where(_keep(s, top_k, top_p, _shift), v, np.float32(-np.inf))
     return v
 
 
-def sample(logits, temperature: float, top_k: int, seed: int, pos: int) -> int:
+def sample(logits, temperature: float, top_k: int, seed: int, pos: int, top_p: float = 1.0) -> int:
     """The id the rule draws from `logits` at position `pos` (greedy for temperature 0)."""
     if temperature == 0:
         return int(np.argmax(np.asarray(logits, np.float32)))
-    return int(np.argmax(scores(logits, temperature, top_k, seed, pos)))
+    return int(np.argmax(scores(logits, temperature, top_k, seed, pos, top_p)))
 
 
-def margin(logits, temperature: float, top_k: int, seed: int, pos: int) -> float:
+def nucleus_size(logits, temperature: float, top_k: int, top_p: float) -> int:
+    """How many tokens steps 3 and 3b keep (temperature > 0)."""
+    s = np.asarray(logits, np.float32) / np.float32(temperature)
+    return int(_keep(s, top_k, top_p if top_p_active(temperature, top_p) else 1.0).sum())
+
+
+def nucleus_margin(logits, temperature: float, top_k: int, top_p: float) -> float:
+    """How close step 3b's decisive comparisons (A * 2^24 against p24 * Z at the smallest kept value and the
+    largest dropped one) are, relative to Z * 2^24; inf when top-p is off.  Below NUCLEUS_EPS the device may
+    keep one value more or one less."""
+    if not top_p_active(temperature, top_p):
+        return float("inf")
+    s = np.asarray(logits, np.float32) / np.float32(temperature)
+    n = s.shape[0]
+    kept = s[s >= np.partition(s, n - top_k)[n - top_k]] if 0 < top_k < n else s
+    _, above, z, p24, j = _nucleus(kept, top_p)
+    gaps = [abs(int(above[i]) * 2 ** 24 - p24 * z) for i in (j - 1, j) if i >= 0]
+    return min(gaps) / (z * 2.0 ** 24)
+
+
+def margin(logits, temperature: float, top_k: int, seed: int, pos: int, top_p: float = 1.0) -> float:
     """Relative gap between the two best perturbed scores: below ~1e-5 a last-ulp difference of the
-    device logf may change the id."""
+    device logf may change the id.  With top-p, 0 also when a nucleus comparison is within NUCLEUS_EPS
+    (nucleus_margin) and keeping one value more or one less would change the id."""
     if temperature == 0:
         v = np.asarray(logits, np.float32)
     else:
-        v = scores(logits, temperature, top_k, seed, pos)
+        v = scores(logits, temperature, top_k, seed, pos, top_p)
+        if nucleus_margin(logits, temperature, top_k, top_p) < NUCLEUS_EPS:
+            ids = {int(np.argmax(scores(logits, temperature, top_k, seed, pos, top_p, d))) for d in (-1, 0, 1)}
+            if len(ids) > 1:
+                return 0.0
     top2 = np.partition(v, v.shape[0] - 2)[-2:]
     if not np.isfinite(top2).all():
         return float("inf")

@@ -6,11 +6,15 @@
 One exact-numerics decoder of the workload's model (synthetic weights, bench.py's seed for the workload) runs
 kllm_decoder_generate windows of --steps positions from position 0: greedy, then temperature --temperature with
 top_k 0, then with top_k --top-k, switched by kllm_decoder_set_sampling between windows (the engine is not
-rebuilt).  Each window ends in a host synchronisation, so a host clock around it times it.  Every mode is warmed
-up once, then the modes alternate for --reps repetitions and the medians are reported.  Prints ONE JSON line:
+rebuilt).  With --top-p P two more modes run: top_p P alone, and top_k --top-k with top_p P
+(kllm_decoder_set_sampling_top_p).  Each window ends in a host synchronisation, so a host clock around it times
+it.  Every mode is warmed up once, then the modes alternate for --reps repetitions and the medians are
+reported.  Prints ONE JSON line:
 
-  greedy_tok_s, sampled_tok_s {top_k: tok/s}, overhead {top_k: 1 - sampled / greedy}, engine, card (the GPU's
-  name and power limit, read in the same run)
+  greedy_tok_s, sampled_tok_s {mode: tok/s}, overhead {mode: 1 - sampled / greedy}, engine, card (the GPU's
+  name and power limit, read in the same run); with --top-p also nucleus_size {mode: mean}, the mean number of
+  tokens the rule keeps per position, from a step loop over the same positions after the timed windows (the
+  numpy mirror on the run's own logits): a top-p rate means little without it.
 
 Needs a CUDA device; there is nothing to time without one.
 """
@@ -27,7 +31,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from bench_prefill import SEEDS, gpu_card  # noqa: E402
 
 
-def run(workload, steps, reps, seed, temperature, top_k):
+def run(workload, steps, reps, seed, temperature, top_k, top_p=None):
     import torch
     from kuiperllama_b200 import SHAPES, Decoder, synth_weights
     shape = SHAPES[workload]
@@ -36,29 +40,44 @@ def run(workload, steps, reps, seed, temperature, top_k):
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: the decode paths run on the GPU only")
     dec = Decoder(shape, synth_weights(shape, "cuda", seed), numerics="exact")
-    modes = [("greedy", 0.0, 0), ("top_k=0", temperature, 0), (f"top_k={top_k}", temperature, top_k)]
-    times = {name: [] for name, _, _ in modes}
+    modes = [("greedy", 0.0, 0, 1.0), ("top_k=0", temperature, 0, 1.0), (f"top_k={top_k}", temperature, top_k, 1.0)]
+    if top_p is not None:
+        modes += [(f"top_p={top_p}", temperature, 0, top_p), (f"top_k={top_k},top_p={top_p}", temperature, top_k, top_p)]
+    times = {name: [] for name, _, _, _ in modes}
 
-    def window(t, k):
-        dec.set_sampling(t, k, seed)
+    def window(t, k, p):
+        dec.set_sampling(t, k, seed, top_p=p)
         t0 = time.perf_counter()
         dec.generate(1, 0, steps)
         return time.perf_counter() - t0
 
-    for _, t, k in modes:
-        window(t, k)
+    for _, t, k, p in modes:
+        window(t, k, p)
     for _ in range(max(1, reps)):
-        for name, t, k in modes:
-            times[name].append(window(t, k))
+        for name, t, k, p in modes:
+            times[name].append(window(t, k, p))
+    nucleus = {}
+    if top_p is not None:  # untimed: the same positions stepped one by one, the kept set from each step's logits
+        from kuiperllama_b200 import sampling
+        for name, t, k, p in modes[1:]:
+            dec.set_sampling(t, k, seed, top_p=p)
+            tok, sizes = 1, []
+            for pos in range(steps):
+                tok = dec.step(tok, pos)
+                sizes.append(sampling.nucleus_size(dec.logits(), t, k, p))
+            nucleus[name] = statistics.fmean(sizes)
     engine = dec.engine
     dec.close()
     rate = {name: steps / statistics.median(v) for name, v in times.items()}
     g = rate["greedy"]
     sampled = {name: r for name, r in rate.items() if name != "greedy"}
-    return {"workload": workload, "shape": shape.name, "steps": steps, "reps": max(1, reps),
-            "temperature": temperature, "greedy_tok_s": g, "sampled_tok_s": sampled,
-            "overhead": {name: 1.0 - r / g for name, r in sampled.items()},
-            "engine": engine, "numerics": "exact", "seed": seed, "card": gpu_card(torch.cuda.current_device())}
+    out = {"workload": workload, "shape": shape.name, "steps": steps, "reps": max(1, reps),
+           "temperature": temperature, "greedy_tok_s": g, "sampled_tok_s": sampled,
+           "overhead": {name: 1.0 - r / g for name, r in sampled.items()},
+           "engine": engine, "numerics": "exact", "seed": seed, "card": gpu_card(torch.cuda.current_device())}
+    if top_p is not None:
+        out["nucleus_size"] = nucleus
+    return out
 
 
 def main():
@@ -68,12 +87,15 @@ def main():
     ap.add_argument("--reps", type=int, default=7, help="timed windows of each mode; medians are reported")
     ap.add_argument("--temperature", type=float, default=0.8)
     ap.add_argument("--top-k", type=int, default=40)
+    ap.add_argument("--top-p", type=float, default=None, help="also time top-p alone and top-k with top-p")
     ap.add_argument("--seed", type=int, default=None, help="default: bench.py's seed for the workload")
     a = ap.parse_args()
     if a.steps < 1:
         raise SystemExit("--steps must be at least 1")
+    if a.top_p is not None and not 0 < a.top_p <= 1:
+        raise SystemExit("--top-p must be in (0, 1]")
     seed = SEEDS[a.workload] if a.seed is None else a.seed
-    print(json.dumps(run(a.workload, a.steps, a.reps, seed, a.temperature, a.top_k)))
+    print(json.dumps(run(a.workload, a.steps, a.reps, seed, a.temperature, a.top_k, a.top_p)))
 
 
 if __name__ == "__main__":
