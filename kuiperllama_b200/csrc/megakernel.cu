@@ -515,7 +515,8 @@ __device__ __forceinline__ void accum_w8_any(const uint32_t (&w)[NR], const uint
 // 4 weights and digit: sum_i w_i x_i = s_g * step_g * (65536 D2 + 256 D1 + D0), D_k = sum_i w_i l_k,i
 // exact in int32.  ~6 warp instructions per 128 weight bytes.  The group scale s_g and the int8
 // weights enter exactly as in the reference (dequantised weight = q * s, export.py:60-67); only x is
-// rounded, to 2^-23 of its group maximum -- the same order as fp32 rounding of the products
+// rounded, to within 2^-22 of its group maximum (half a step, 2^-23, plus what the rounded reciprocal
+// `inv` adds: tests/test_decode_model.py pins the bound) -- the order of fp32 rounding of the products
 // themselves.  Logits agree with the exact mode to ~1e-6 relative (tests: <= 1e-4 absolute, same
 // greedy id wherever the top-2 margin exceeds 2e-4), not bit for bit.
 __device__ __forceinline__ uint4 lds_u4(uint32_t a) {

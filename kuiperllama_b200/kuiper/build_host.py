@@ -30,6 +30,25 @@ def binary(variant: str, name: str) -> Path:
     return build_dir(variant) / name
 
 
+def _cache_entry(cache: Path, key: str) -> str | None:
+    for line in cache.read_text(errors="replace").splitlines():
+        if line.startswith(key + ":"):
+            return line.split("=", 1)[1]
+    return None
+
+
+def _made_elsewhere(out: Path) -> bool:
+    """The build directory was configured at another path (the tree was copied or moved with its build products):
+    CMake refuses such a cache, and its Ninja files name the old paths."""
+    cache = out / "CMakeCache.txt"
+    if not cache.exists():
+        return False
+    made_in = _cache_entry(cache, "CMAKE_CACHEFILE_DIR")
+    source = _cache_entry(cache, "CMAKE_HOME_DIRECTORY")
+    return (made_in is None or source is None or Path(made_in).resolve() != out.resolve()
+            or Path(source).resolve() != HERE)
+
+
 def build(variant: str = "llama2", verbose: bool = False) -> Path:
     if variant not in VARIANTS:
         raise ValueError(f"unknown variant {variant!r}")
@@ -37,6 +56,8 @@ def build(variant: str = "llama2", verbose: bool = False) -> Path:
     if cmake is None:
         raise RuntimeError("cmake not found on PATH")
     out = build_dir(variant)
+    if _made_elsewhere(out):
+        shutil.rmtree(out)  # build products only (git-ignored): configure afresh here
     out.mkdir(parents=True, exist_ok=True)
     cfg = [cmake, "-S", str(HERE), "-B", str(out), "-DCMAKE_BUILD_TYPE=Release",
            "-DCMAKE_CXX_COMPILER=/usr/bin/g++", *VARIANTS[variant]]

@@ -1,5 +1,7 @@
-"""fp64 model of what the batched prompt prefill computes (csrc/prefill_gemm.cu, csrc/prefill.cu and the
-last position's classifier in csrc/decoder.cu prefill()), for the tests to hold the kernels against.
+"""fp64 model of what the batched prompt prefill (csrc/prefill_gemm.cu, csrc/prefill.cu and the last position's
+classifier in csrc/decoder.cu prefill()) and the decode step (csrc/megakernel.cu, both numerics modes) compute, for
+the tests to hold the kernels against.  Row p of a causal forward over tokens 0 .. p is what a decode step at
+position p computes, so one forward serves both.
 
 The prefill multiplies on the tensor cores with both operands rounded to TF32 (cvt.rna: 10 explicit
 mantissa bits, nearest, ties away from zero), accumulates in fp32 and stores every activation as fp32.  This
@@ -8,7 +10,14 @@ every point the kernels store fp32.  A TF32 x TF32 product is exact in fp64 (11 
 what is left between a correct kernel and this model is the order and rounding of fp32 accumulation and of
 the fp32 element-wise arithmetic -- and the rare TF32 rounding decision that an fp32 difference of one unit
 flips.  With `tf32=False` no operand is rounded to TF32: that is the plain fp32 model the CPU oracle
-(oracle/kuiper_oracle.c) computes, which is how tests/test_prefill_model.py checks this module.
+(oracle/kuiper_oracle.c) computes, which is how tests/test_prefill_model.py checks this module, and what the
+decode step computes in its exact mode.
+
+The decode step's fast mode (`numerics = fast`) rewrites the input vector of every int8 projection with group size
+64 as 24-bit fixed point per 64-element group before the dot products (quantize_input_inplace, accum_w8_dp4a,
+accum_w8_mma); `fixed_point=True` replaces those inputs with the same fixed-point values (`fixed_point_value`, a
+mirror of the kernel's fp32 arithmetic), so that what remains is again fp32 summation order.  Its attention
+(flash-decoding) reorders the softmax sums only, which the exact softmax here stands for.
 
 The forward is written from the operations, following the model's formulas (rmsnorm, q/k/v with the Qwen
 bias, RoPE with interleaved (llama2) or half-split (qwen2) pairs, causal attention with grouped kv heads,
@@ -61,6 +70,38 @@ def gemm_ref(x, w, tf32=True):
 def gemm_abs_ref(x, w, tf32=True):
     """sum_k |x~[t, k] w~[n, k]|: the scale of the fp32 accumulation error of out[t, n]."""
     return gemm_operand(x, tf32).to(torch.float64).abs() @ gemm_operand(w, tf32).to(torch.float64).abs().t()
+
+
+FP_ONE = 4194304.0  # 2^22: the fixed point's full scale, q = +-2^22 at the group maximum
+
+
+def balanced_digits(q):
+    """q (integers, |q| <= 2^22) -> (a2, a1, a0) with q = 65536 a2 + 256 a1 + a0 and a0, a1 in [-128, 127]: the
+    kernel's balanced base-256 split (quantize_input_inplace).  numpy or torch integer arrays."""
+    a0 = ((q + 128) & 255) - 128
+    q1 = (q - a0) >> 8
+    a1 = ((q1 + 128) & 255) - 128
+    return (q1 - a1) >> 8, a1, a0
+
+
+def fixed_point_parts(x):
+    """The fast mode's fixed point of x [..., M] (M % 64 == 0), in the kernel's fp32 arithmetic, per 64-element
+    group: gmax = max|x|, step = fp32(gmax * 2^-22), inv = fp32(2^22 / gmax) (0 when gmax is 0), q = x * inv
+    rounded to fp32, then to the nearest integer (ties to even, __float2int_rn).  Returns (step [..., M / 64, 1],
+    q [..., M / 64, 64]) as fp32 tensors."""
+    x = torch.as_tensor(x).to(torch.float32)
+    xg = x.reshape(*x.shape[:-1], x.shape[-1] // 64, 64)
+    gmax = xg.abs().amax(dim=-1, keepdim=True)
+    step = gmax * np.float32(1.0 / FP_ONE)
+    inv = torch.where(gmax > 0, np.float32(FP_ONE) / gmax, torch.zeros_like(gmax))
+    return step, torch.round(xg * inv)
+
+
+def fixed_point_value(x):
+    """step * q for every element of x [..., M]: the value the fast mode's int8 dot products see, exact in fp64
+    (not an fp32 value: 24-bit step times 23-bit q)."""
+    step, q = fixed_point_parts(x)
+    return (step.to(torch.float64) * q.to(torch.float64)).reshape(x.shape)
 
 
 def flavour_eps(flavour):
@@ -118,7 +159,8 @@ def _attention(q, k_all, v_all, start_pos, kv_mul, max_bytes=1 << 28):
     return f32(out)
 
 
-def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=True, device=None, logits_at=()):
+def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=True, device=None, logits_at=(),
+                fixed_point=False):
     """The forward of prefill_block over `tokens` at positions start_pos .. start_pos + n - 1, then the last
     position's final RMSNorm and classifier (and those of the rows listed in `logits_at`: what a prefill of
     tokens[:i + 1] would leave, since no row depends on a later one).
@@ -127,6 +169,9 @@ def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=Tr
               the Qwen bias; wcls None = the embedding is the classifier)
     sin, cos  the [seq_len, head_size] tables the kernels read (on the GPU: what kllm_sincos_init wrote)
     kv_in     (k, v) [L, >= start_pos, kv_dim]: the cache rows before start_pos
+    fixed_point  the decode step's fast mode: the input of every int8 projection with group size 64 and an input
+              length divisible by 64 (q/k/v, Wo, W1/W3, W2 and the classifier) becomes fixed_point_value(x).
+              Needs tf32=False.
     Returns dict: k, v [L, n, kv_dim] (the cache rows written, after RoPE for k), logits [vocab] (fp64 of the
     fp32 classifier: no TF32 there, it is the decode path's GEMV), next (first maximum) and logits_at
     {row: logits}."""
@@ -136,6 +181,7 @@ def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=Tr
     n = len(tokens)
     eps = flavour_eps(s.flavour)
     g = s.group_size
+    assert not (fixed_point and tf32), "the fixed point is the decode step's; the prefill's GEMMs are TF32"
     sin, cos = _t(sin, dev), _t(cos, dev)
     pos = torch.arange(start_pos, start_pos + n, device=dev)
     tok = torch.as_tensor(np.asarray(tokens, dtype=np.int64), device=dev)
@@ -146,8 +192,13 @@ def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=Tr
             return dequant_w8(_t(w, dev), _t(weights["s" + name[1:]][l], dev), g, tf32)
         return gemm_operand(_t(w, dev), tf32)
 
+    def operand(x):
+        if fixed_point and g == 64 and x.shape[-1] % 64 == 0:
+            return fixed_point_value(x)
+        return gemm_operand(x.to(torch.float32), tf32).to(torch.float64)
+
     def proj(x, name, l):
-        return f32(gemm_operand(x.to(torch.float32), tf32).to(torch.float64) @ weight(name, l).to(torch.float64).t())
+        return f32(operand(x) @ weight(name, l).to(torch.float64).t())
 
     def bias(y, name, l):
         b = weights.get(name)
@@ -183,6 +234,8 @@ def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=Tr
         wc = dequant_w8(_t(wcls, dev), _t(weights["scls"], dev), g, tf32=False)
     else:
         wc = _t(wcls, dev)
+    if fixed_point and g == 64 and s.dim % 64 == 0:
+        xl = fixed_point_value(xl)
     logits = dict(zip(rows, xl @ wc.to(torch.float64).t()))
     last = logits[n - 1]
     return {"k": torch.stack(ks), "v": torch.stack(vs), "logits": last, "next": int(torch.argmax(last)),

@@ -138,18 +138,20 @@ def test_add_and_swiglu(kllm_lib, ref, oracle, n):
 
 # ---- sin/cos table + rope -----------------------------------------------------------------------
 @pytest.mark.parametrize("flavour,head_size,seq_len", [("llama2", 64, 2048), ("llama2", 48, 256),
-                                                       ("llama2", 128, 512), ("qwen2", 64, 4096)])
+                                                       ("llama2", 128, 512), ("qwen2", 64, 4096),
+                                                       ("llama3", 128, 4096)])
 def test_sincos_table(kllm_lib, ref, ref_qwen, oracle, flavour, head_size, seq_len):
     from kuiperllama_b200 import FLAVOURS
     r = ref if flavour == "llama2" else ref_qwen
     s = torch.zeros(seq_len * head_size, device="cuda"); c = torch.zeros_like(s)
     sr = torch.zeros_like(s); cr = torch.zeros_like(s)
     assert kllm_lib.kllm_sincos_init(head_size, seq_len, FLAVOURS[flavour], ptr(s), ptr(c), None) == 0
-    if r.live:
+    if r.live and flavour != "llama3":
         r.L.kref_sincos(head_size, seq_len, ptr(sr), ptr(cr), None)
     sync()
     key = f"sincos/{flavour}/{head_size}x{seq_len}"
-    r.bits(key + "/sin", s, sr, "sin table"); r.bits(key + "/cos", c, cr, "cos table")
+    if flavour != "llama3":  # no reference build of these kernels is recorded for the Llama-3 flavour: oracle only
+        r.bits(key + "/sin", s, sr, "sin table"); r.bits(key + "/cos", c, cr, "cos table")
     so, co = oracle.sincos(head_size, seq_len, flavour)
     # device powf/sinf/cosf vs libm at arguments up to seq_len: absolute 2e-4 (values in [-1,1])
     assert np.abs(s.cpu().numpy() - so.ravel()).max() < 2e-4
@@ -158,7 +160,7 @@ def test_sincos_table(kllm_lib, ref, ref_qwen, oracle, flavour, head_size, seq_l
 
 @pytest.mark.parametrize("flavour,dim,kv_dim,head_size", [("llama2", 2048, 256, 64), ("llama2", 288, 288, 48),
                                                           ("llama2", 4096, 4096, 128), ("qwen2", 896, 128, 64),
-                                                          ("qwen2", 2048, 2048, 64)])
+                                                          ("qwen2", 2048, 2048, 64), ("llama3", 4096, 1024, 128)])
 def test_rope(kllm_lib, ref, ref_qwen, oracle, flavour, dim, kv_dim, head_size):
     from kuiperllama_b200 import FLAVOURS
     r = ref if flavour == "llama2" else ref_qwen
@@ -174,12 +176,13 @@ def test_rope(kllm_lib, ref, ref_qwen, oracle, flavour, dim, kv_dim, head_size):
         # give it a padded buffer so the overrun stays inside our allocation.
         qr = torch.zeros(dim + head_size, device="cuda"); qr[:dim] = q0
         kr = k0.clone()
-        if r.live:
+        if r.live and flavour != "llama3":
             r.L.kref_rope(dim, kv_dim, head_size, ptr(qr), ptr(kr), pos, ptr(s), ptr(c), seq_len, None)
         sync()
         key = f"rope/{flavour}/{dim}/{kv_dim}/{head_size}/{pos}"
-        r.bits(key + "/q", q, qr[:dim], f"rope q {flavour} pos={pos}")
-        r.bits(key + "/k", k, kr, f"rope k {flavour} pos={pos}")
+        if flavour != "llama3":
+            r.bits(key + "/q", q, qr[:dim], f"rope q {flavour} pos={pos}")
+            r.bits(key + "/k", k, kr, f"rope k {flavour} pos={pos}")
         qo, ko = oracle.rope(flavour, q0.cpu().numpy(), k0.cpu().numpy(), pos,
                              s.cpu().numpy(), c.cpu().numpy(), head_size)
         assert np.abs(q.cpu().numpy() - qo).max() < 1e-5 and np.abs(k.cpu().numpy() - ko).max() < 1e-5
