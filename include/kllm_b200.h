@@ -115,6 +115,15 @@ int kllm_sample_f32(const float* logits, int64_t n, float temperature, int32_t t
  * and for top_p that is NaN, <= 0 or > 1. */
 int kllm_sample_top_p_f32(const float* logits, int64_t n, float temperature, int32_t top_k, float top_p,
                           uint64_t seed, int32_t pos, int64_t* out_index, void* stream);
+/* The repetition penalty of HF's RepetitionPenaltyLogitsProcessor (DESIGN.md "Sampling", step 0b), what a
+ * caller of the per-op path runs before kllm_sample_top_p_f32 or an argmax: out[0..n) = logits[0..n), except
+ * out[i] = logits[i] < 0 ? logits[i] * penalty : logits[i] / penalty (one fp32 IEEE operation) for every i
+ * listed in ids[0..n_ids) (device).  An id listed more than once is penalised once; ids outside [0, n) are
+ * ignored.  `out` must not overlap `logits`.  penalty == 1 copies the logits.  No synchronisation.
+ * KLLM_E_INVALID for NULL pointers (ids may be NULL when n_ids == 0), out == logits, n outside [1, 2^31),
+ * n_ids < 0, or a penalty that is not finite or <= 0. */
+int kllm_repetition_penalty_f32(const float* logits, float* out, int64_t n, const int32_t* ids, int32_t n_ids,
+                                float penalty, void* stream);
 
 /* ---- fused per-layer entry points -------------------------------------------------------
  * What LLama2Model::forward (llama3.cpp:147-167) calls instead of 15 launches per layer.
@@ -336,6 +345,15 @@ int kllm_decoder_set_sampling(kllm_decoder* dec, float temperature, int32_t top_
  * kllm_decoder_set_sampling, which itself sets top_p back to 1.  KLLM_E_INVALID, with the settings in force
  * left unchanged, for a temperature that is negative or not finite and for top_p that is NaN, <= 0 or > 1. */
 int kllm_decoder_set_sampling_top_p(kllm_decoder* dec, float temperature, int32_t top_k, float top_p, uint64_t seed);
+/* Repetition penalty before the draw, from this call on, in every entry that kllm_decoder_set_sampling covers,
+ * on either engine and every tensor-parallel rank, greedy or sampled: each id is drawn from the logits with
+ * kllm_repetition_penalty_f32's step applied to the ids fed at positions [lo, pos] (lo = 0 for last_n == 0,
+ * the whole sequence; else max(0, pos - last_n + 1)), as recorded by the decoder (kllm_decoder_read_history).
+ * penalty < 1 raises those logits instead.  penalty == 1 is off (a new decoder's setting): the ids are then
+ * exactly those without it.  Independent of the sampling settings: neither call changes the other's.
+ * kllm_decoder_logits keeps returning the raw logits.  Synchronises the decoder's stream.  KLLM_E_INVALID,
+ * with the settings in force left unchanged, for a penalty that is not finite or <= 0 and for last_n < 0. */
+int kllm_decoder_set_repetition_penalty(kllm_decoder* dec, float penalty, int32_t last_n);
 
 /* Blocking copies for tests: logits of the last step [vocab]; the KV cache in the REFERENCE
  * layout [layer][seq_len][kv_dim] (llama3.cpp:469-475) whatever the engine keeps internally. */
@@ -345,6 +363,10 @@ int kllm_decoder_logits(kllm_decoder* dec, float* logits_host);
  * contents ordered after the last step on the decoder's stream. */
 const float* kllm_decoder_logits_device(const kllm_decoder* dec);
 int kllm_decoder_read_kv(kllm_decoder* dec, float* key_host, float* value_host);
+/* The decoder's history [seq_len]: the id fed as input at each position by any entry (the id whose K/V rows
+ * are that row of the cache), -1 where none was fed or the id was outside the vocabulary.  Feeding a
+ * position again overwrites its entry. */
+int kllm_decoder_read_history(kllm_decoder* dec, int32_t* ids_host);
 /* Kernel launches one decode step issues (graph nodes; 1 for the persistent engine). */
 int kllm_decoder_launches_per_step(const kllm_decoder* dec);
 /* Classifier rows THIS rank streams per token: vocab_size, or vocab_size / tp_size when the

@@ -87,6 +87,7 @@ _SIGNATURES = {
     "kllm_sample_f32": (c_int, [c_void_p, c_int64, c_float, c_int32, c_uint64, c_int32, c_void_p, c_void_p]),
     "kllm_sample_top_p_f32": (c_int, [c_void_p, c_int64, c_float, c_int32, c_float, c_uint64, c_int32, c_void_p,
                                       c_void_p]),
+    "kllm_repetition_penalty_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int32, c_float, c_void_p]),
     "kllm_gemv_fused": (c_int, [POINTER(GemvJob), c_void_p]),
     "kllm_gemm_tf32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "kllm_gemm_w8_tf32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
@@ -110,6 +111,8 @@ _SIGNATURES = {
                                             TOKEN_CALLBACK, c_void_p, POINTER(c_int32), POINTER(c_int32)]),
     "kllm_decoder_set_sampling": (c_int, [c_void_p, c_float, c_int32, c_uint64]),
     "kllm_decoder_set_sampling_top_p": (c_int, [c_void_p, c_float, c_int32, c_float, c_uint64]),
+    "kllm_decoder_set_repetition_penalty": (c_int, [c_void_p, c_float, c_int32]),
+    "kllm_decoder_read_history": (c_int, [c_void_p, c_void_p]),
     "kllm_decoder_logits": (c_int, [c_void_p, c_void_p]),
     "kllm_decoder_logits_device": (c_void_p, [c_void_p]),
     "kllm_decoder_read_kv": (c_int, [c_void_p, c_void_p, c_void_p]),

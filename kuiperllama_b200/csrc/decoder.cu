@@ -41,10 +41,13 @@ struct StepState {  // device-resident loop state
 constexpr int kStreamIds = 32;  // int32 offset of the streamed ids behind the count (kllm_decoder::stream_host)
 static_assert(mega::kMaxStopIds == KLLM_MAX_STOP_IDS, "one stop-set capacity");
 
+// Also records the fed id in the history (sampling.cuh step 0), -1 for an id outside the vocabulary.
 __global__ void embed_token_kernel(const StepState* st, const float* __restrict__ table,
-                                   float* x, int dim, int vocab) {
+                                   float* x, int dim, int vocab, int32_t* hist) {
   const int32_t token = st->token;
-  if (token < 0 || token >= vocab) return;
+  const bool valid = token >= 0 && token < vocab;
+  if (blockIdx.x == 0 && threadIdx.x == 0) hist[st->pos] = valid ? token : -1;
+  if (!valid) return;
   const float4* s4 = reinterpret_cast<const float4*>(table + static_cast<size_t>(token) * dim);
   float4* d4 = reinterpret_cast<float4*>(x);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < (dim >> 2); i += gridDim.x * blockDim.x)
@@ -56,14 +59,24 @@ __global__ void embed_token_kernel(const StepState* st, const float* __restrict_
 // the id, feed it (or the teacher's id) to the next step, pos += 1.
 // With stream_ids (kllm_decoder_generate_until's graph only) the id is also published to mapped host memory:
 // the id, then the count with release semantics at system scope, which the host polls.
+// With the repetition penalty on (read from device memory, so the captured graphs stay valid), the block first
+// writes the penalised logits to `penalized` and draws from those; the raw logits are left as they are.
 constexpr int kDrawScratchBytes = sampling::kDrawScratchBase + 2048 * 8;
 
 __global__ void __launch_bounds__(1024)
 argmax_advance_kernel(const float* __restrict__ logits, int n, const SampleParams* sp, StepState* st,
                       int32_t* out_tokens, const int32_t* teacher, int max_steps, int32_t* stream_ids,
-                      int32_t* stream_count) {
+                      int32_t* stream_count, const PenaltyParams* pp, const int32_t* hist, float* penalized) {
   __shared__ __align__(16) unsigned char scratch[kDrawScratchBytes];
-  const int bi = sampling::draw_block<1024>(logits, n, *sp, st->pos, nullptr, nullptr, 0, scratch, kDrawScratchBytes,
+  const int pos = st->pos;
+  const float* l = logits;
+  const PenaltyParams pen = *pp;
+  if (sampling::penalty_active(pen)) {
+    sampling::penalize_rows<1024>(logits, penalized, 0, n, hist, sampling::window_lo(pen, pos), pos, pen.penalty,
+                                  [] { __syncthreads(); });
+    l = penalized;
+  }
+  const int bi = sampling::draw_block<1024>(l, n, *sp, pos, nullptr, nullptr, 0, scratch, kDrawScratchBytes,
                                             [] { __syncthreads(); });
   if (threadIdx.x == 0) {
     const int next = bi < 0 ? 0 : bi;
@@ -101,6 +114,9 @@ struct kllm_decoder {
   bool use_mega = false;
   StepState* st = nullptr;
   SampleParams* sampling = nullptr;  // device; zero = greedy (kllm_decoder_set_sampling)
+  PenaltyParams* penalty = nullptr;  // device; zero = off (kllm_decoder_set_repetition_penalty)
+  int32_t* hist = nullptr;           // device [seq_len]: the id fed at each position, -1 for none
+  float* penalized = nullptr;        // device [vocab]: the penalised logits of the last draw
   int32_t* out_tokens = nullptr;  // device [seq_len]
   int32_t* teacher = nullptr;     // device [seq_len]
   StepState* st_host = nullptr;   // pinned
@@ -154,7 +170,7 @@ int enqueue_step(kllm_decoder* dc, bool with_teacher, bool streamed, cudaStream_
   const bool tp = d.tp_size > 1;
   const uint64_t before = launch_counter().load();
 
-  embed_token_kernel<<<4, 256, 0, s>>>(dc->st, d.tok_emb, dc->x, dim, d.vocab_size);
+  embed_token_kernel<<<4, 256, 0, s>>>(dc->st, d.tok_emb, dc->x, dim, d.vocab_size, dc->hist);
   count_launch();
   KLLM_TRY(cudaGetLastError());
 
@@ -238,7 +254,8 @@ int enqueue_step(kllm_decoder* dc, bool with_teacher, bool streamed, cudaStream_
   argmax_advance_kernel<<<1, 1024, 0, s>>>(dc->logits, d.vocab_size, dc->sampling, dc->st, dc->out_tokens,
                                            with_teacher ? dc->teacher : nullptr, d.seq_len,
                                            streamed ? dc->stream_dev + kStreamIds : nullptr,
-                                           streamed ? dc->stream_dev : nullptr);
+                                           streamed ? dc->stream_dev : nullptr, dc->penalty, dc->hist,
+                                           dc->penalized);
   count_launch();
   KLLM_TRY(cudaGetLastError());
   dc->launches_per_step = static_cast<int>(launch_counter().load() - before);
@@ -316,6 +333,9 @@ int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int3
 
   std::memcpy(dc->io_host, tokens_host, sizeof(int32_t) * n_tokens);
   KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_tokens, cudaMemcpyHostToDevice, dc->stream));
+  // the prompt rows' history (prefill_args refused ids outside the vocabulary), in stream order before the draw
+  KLLM_TRY(cudaMemcpyAsync(dc->hist + start_pos, dc->teacher, sizeof(int32_t) * n_tokens, cudaMemcpyDeviceToDevice,
+                           dc->stream));
   int last_rows = 0;
   for (int c0 = 0; c0 < n_tokens; c0 += kBlock) {
     const int T = std::min(kBlock, n_tokens - c0);
@@ -342,7 +362,8 @@ int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int3
     KLLM_TRY(gemv_dispatch(&j, GemvExtra{}, dc->stream));
   }
   argmax_advance_kernel<<<1, 1024, 0, dc->stream>>>(dc->logits, d.vocab_size, dc->sampling, dc->st, nullptr, nullptr,
-                                                    d.seq_len, nullptr, nullptr);
+                                                    d.seq_len, nullptr, nullptr, dc->penalty, dc->hist,
+                                                    dc->penalized);
   count_launch();
   KLLM_TRY(cudaGetLastError());
   KLLM_TRY(cudaMemcpyAsync(hs_state, dc->st, sizeof(StepState), cudaMemcpyDeviceToHost, dc->stream));
@@ -426,10 +447,12 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
       dev_alloc(&dc->kcache, kv_elems) || dev_alloc(&dc->vcache, kv_elems) ||
       dev_alloc(&dc->sin_t, static_cast<size_t>(d.seq_len) * dc->head_size) ||
       dev_alloc(&dc->cos_t, static_cast<size_t>(d.seq_len) * dc->head_size) ||
-      dev_alloc(&dc->tp_tmp, d.dim) || dev_alloc(&dc->k_raw, dc->kv_dim))
+      dev_alloc(&dc->tp_tmp, d.dim) || dev_alloc(&dc->k_raw, dc->kv_dim) || dev_alloc(&dc->penalized, d.vocab_size))
     return fail(static_cast<int>(cudaErrorMemoryAllocation));
   if (cudaMalloc(&dc->st, sizeof(StepState)) != cudaSuccess ||
       cudaMalloc(&dc->sampling, sizeof(SampleParams)) != cudaSuccess ||
+      cudaMalloc(&dc->penalty, sizeof(PenaltyParams)) != cudaSuccess ||
+      cudaMalloc(&dc->hist, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMalloc(&dc->out_tokens, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMalloc(&dc->teacher, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMallocHost(&dc->st_host, sizeof(StepState)) != cudaSuccess ||
@@ -440,6 +463,8 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
   std::memset(dc->stream_host, 0, sizeof(int32_t) * (kStreamIds + d.seq_len));
   cudaMemsetAsync(dc->st, 0, sizeof(StepState), dc->stream);
   cudaMemsetAsync(dc->sampling, 0, sizeof(SampleParams), dc->stream);
+  cudaMemsetAsync(dc->penalty, 0, sizeof(PenaltyParams), dc->stream);
+  cudaMemsetAsync(dc->hist, 0xff, sizeof(int32_t) * d.seq_len, dc->stream);  // -1: no id
 
   int rc = kllm_sincos_init(dc->head_size, d.seq_len, d.flavour, dc->sin_t, dc->cos_t, dc->stream);
   if (rc != 0) return fail(rc);
@@ -483,6 +508,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     mm.logits = dc->logits, mm.score = dc->score, mm.key_cache = dc->kcache, mm.value_cache = dc->vcache;
     mm.sin_cache = dc->sin_t, mm.cos_cache = dc->cos_t, mm.state = dc->st, mm.out_tokens = dc->out_tokens;
     mm.sampling = dc->sampling;
+    mm.hist = dc->hist, mm.penalized = dc->penalized;
     rc = dc->mega.init(mm, dc->stream);
     if (rc == 0) {
       dc->use_mega = true;
@@ -514,11 +540,13 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->exec_until) cudaGraphExecDestroy(dc->exec_until);
   if (dc->graph_until) cudaGraphDestroy(dc->graph_until);
   float* bufs[] = {dc->x, dc->q, dc->attn, dc->h, dc->logits, dc->score,
-                   dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->k_raw};
+                   dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->k_raw, dc->penalized};
   for (float* b : bufs)
     if (b) cudaFree(b);
   if (dc->st) cudaFree(dc->st);
   if (dc->sampling) cudaFree(dc->sampling);
+  if (dc->penalty) cudaFree(dc->penalty);
+  if (dc->hist) cudaFree(dc->hist);
   if (dc->out_tokens) cudaFree(dc->out_tokens);
   if (dc->teacher) cudaFree(dc->teacher);
   if (dc->pf_buf) cudaFree(dc->pf_buf);
@@ -713,6 +741,16 @@ int kllm_decoder_set_sampling_top_p(kllm_decoder* dc, float temperature, int32_t
   return static_cast<int>(cudaStreamSynchronize(dc->stream));
 }
 
+int kllm_decoder_set_repetition_penalty(kllm_decoder* dc, float penalty, int32_t last_n) {
+  if (!dc || !std::isfinite(penalty) || !(penalty > 0.f) || last_n < 0) return KLLM_E_INVALID;
+  const PenaltyParams pp{penalty, last_n};
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  KLLM_TRY(cudaMemcpyAsync(dc->penalty, &pp, sizeof(pp), cudaMemcpyHostToDevice, dc->stream));
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  if (dc->use_mega) dc->mega.set_penalty(pp);  // the megakernel takes it in its launch parameters
+  return 0;
+}
+
 int kllm_decoder_profile(kllm_decoder* dc, int32_t first_token, int32_t start_pos, int32_t n_steps,
                          int32_t profiled_step, uint64_t* stamps_host, int32_t capacity,
                          int32_t* grid_out, int32_t* phases_out) {
@@ -776,6 +814,13 @@ int kllm_decoder_read_kv(kllm_decoder* dc, float* key_host, float* value_host) {
     }
   return 0;
 }
+
+int kllm_decoder_read_history(kllm_decoder* dc, int32_t* ids_host) {
+  if (!dc || !ids_host) return KLLM_E_INVALID;
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  return static_cast<int>(cudaMemcpy(ids_host, dc->hist, sizeof(int32_t) * dc->d.seq_len, cudaMemcpyDeviceToHost));
+}
+
 int kllm_decoder_launches_per_step(const kllm_decoder* dc) { return dc ? dc->launches_per_step : 0; }
 int kllm_decoder_classifier_rows(const kllm_decoder* dc) {
   if (!dc) return 0;

@@ -6,6 +6,7 @@
 // reference kernels bit for bit (DESIGN.md "Bit-exactness").
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
@@ -263,6 +264,19 @@ __global__ void __launch_bounds__(1024) sample_kernel(const float* __restrict__ 
   if (threadIdx.x == 0) *out_index = i;
 }
 
+// kllm_repetition_penalty_f32: the raw logits, then step 0b of sampling.cuh over the ids.  The second kernel
+// reads the raw logit, so an id listed twice writes the same value twice.
+__global__ void copy_f32_kernel(const float* __restrict__ in, float* __restrict__ out, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = in[i];
+}
+__global__ void penalize_ids_kernel(const float* __restrict__ logits, float* __restrict__ out, int n,
+                                    const int32_t* __restrict__ ids, int n_ids, float penalty) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n_ids) return;
+  const int id = ids[j];
+  if (id >= 0 && id < n) out[id] = sampling::penalize(logits[id], penalty);
+}
+
 }  // namespace kllm
 
 using namespace kllm;
@@ -372,6 +386,22 @@ int kllm_sample_top_p_f32(const float* logits, int64_t n, float temperature, int
                                                                    SampleParams{temperature, top_k, seed, top_p}, pos,
                                                                    reinterpret_cast<long long*>(out_index));
   count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+int kllm_repetition_penalty_f32(const float* logits, float* out, int64_t n, const int32_t* ids, int32_t n_ids,
+                                float penalty, void* stream) {
+  if (!logits || !out || out == logits || n <= 0 || n > 0x7fffffffLL || n_ids < 0 || (n_ids > 0 && !ids))
+    return KLLM_E_INVALID;
+  if (!std::isfinite(penalty) || !(penalty > 0.f)) return KLLM_E_INVALID;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int m = static_cast<int>(n);
+  copy_f32_kernel<<<std::min(1024, (m + 255) / 256), 256, 0, s>>>(logits, out, m);
+  count_launch();
+  if (n_ids > 0) {  // after the copy, in stream order
+    penalize_ids_kernel<<<static_cast<unsigned>((static_cast<int64_t>(n_ids) + 255) / 256), 256, 0, s>>>(logits, out, m, ids, n_ids, penalty);
+    count_launch();
+  }
   return static_cast<int>(cudaGetLastError());
 }
 

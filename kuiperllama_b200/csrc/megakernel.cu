@@ -1659,6 +1659,39 @@ __device__ KLLM_STAGE_CALL void stage_handoff(const unsigned long long* src, uns
   stage_handoff_inline<UP>(src, tag, n4, t, NT, xs4);
 }
 
+// ---- repetition penalty over this CTA's classifier rows ---------------------------------------------
+// Step 0b of the rule for the rows [u0, u1) this CTA produced (their raw logits, stored by its own
+// threads): the penalised rows go to P.penalized, and the CTA's partial -- greedy, or perturbed as in the
+// perturb_only path -- is folded over them.  draw_truncated reads P.penalized, and the partials stay a
+// lower bound of its top-k threshold because they are maxima of the penalised vector.  Each consumer
+// thread t reads only the history entries j = t (mod CT), the ones it wrote itself in this launch (the
+// token loop) or that an earlier launch wrote, so no hand-off is needed (DESIGN.md 5.7).
+template <int CW>
+__device__ __noinline__ ArgBest penalized_partial(const Params& P, const float* logits, int u0, int u1, int pos) {
+  constexpr int CT = CW * 32;
+  const SampleParams sp = *P.sampling;
+  const PenaltyParams pp = P.penalty;
+  consumer_sync<CT>();  // the raw rows of every warp of the CTA are stored
+  sampling::penalize_rows<CT>(logits, P.penalized, u0, u1, P.hist, sampling::window_lo(pp, pos), pos, pp.penalty,
+                              [] { consumer_sync<CT>(); });
+  const bool perturb = sampling::perturb_only(sp, P.vocab_size);
+  const uint2 key = sampling::seed_key(sp.seed);
+  ArgBest b{0.f, -1};
+  for (int i = u0 + static_cast<int>(threadIdx.x); i < u1; i += CT) {
+    const float v = __ldcg(P.penalized + i);
+    arg_fold(b, perturb ? sampling::perturbed(v, sp.temperature, key, pos, i) : v, i);
+  }
+  return b;
+}
+
+// The history entry of position `pos`, fed `token`: stored by consumer thread pos % CT of every CTA, the
+// one thread that reads it in penalized_partial (-1: an id outside the vocabulary holds none)
+template <int CT>
+__device__ __forceinline__ void record_fed(const Params& P, int pos, int token) {
+  if (static_cast<int>(threadIdx.x) == pos % CT)
+    P.hist[pos] = static_cast<unsigned>(token) < static_cast<unsigned>(P.vocab_size) ? token : -1;
+}
+
 // ---- one GEMV phase of one CTA's consumer warps --------------------------------------------------
 // Stages the phase's input vector (tagged residual exchange / tagged hand-off / plain vector) into
 // shared memory, RMS-normalises it when the phase asks for it, consumes this CTA's ring stages
@@ -2024,7 +2057,9 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
     // that ran epilogues hold partial bests
     ArgBest wb = best;
     const SampleParams sp = *P.sampling;
-    if (sampling::perturb_only(sp, P.vocab_size)) {
+    if (sampling::penalty_active(P.penalty)) {
+      wb = penalized_partial<CW>(P, ph.seg[0].out, u0, u1, pos);
+    } else if (sampling::perturb_only(sp, P.vocab_size)) {
       // sampling without top-k: the partial is the argmax of s_i + g_i over the same rows, read back
       // from the logits the epilogues of this CTA have just stored
       consumer_sync<CT>();
@@ -2084,14 +2119,16 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int p
   float* logits = ph.seg[0].out;
   const SampleParams sp = *P.sampling;
   const bool perturb = sampling::perturb_only(sp, V);  // as the classifier partials (gemv_phase)
+  const bool penalized = sampling::penalty_active(P.penalty);  // then the partial is folded afterwards
   const uint2 key = sampling::seed_key(sp.seed);
   ArgBest best{0.f, -1};
   for (int i = u0 + tid; i < u1; i += CT) {
     const int r = i / rows, j = i - r * rows;
     const float v = poll_tagged_sys(area + static_cast<size_t>(r) * P.tp_stride + j, tag);
     logits[i] = v;
-    arg_fold(best, perturb ? sampling::perturbed(v, sp.temperature, key, pos, i) : v, i);
+    if (!penalized) arg_fold(best, perturb ? sampling::perturbed(v, sp.temperature, key, pos, i) : v, i);
   }
+  if (penalized) best = penalized_partial<CW>(P, logits, u0, u1, pos);
 #pragma unroll
   for (int off = 1; off < 32; off <<= 1) {
     const float ov = __shfl_xor_sync(kFull, best.v, off);
@@ -2119,10 +2156,12 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int p
 // maximum from them.  The scratch is the input-vector
 // buffer: it is idle from the classifier's last read of its input until the next token stages its first
 // vector.  The barrier after the draw orders every thread's read of the result
-// before any thread writes that buffer again.
+// before any thread writes that buffer again.  With the repetition penalty on, the draw reads the penalised
+// vector, which is complete behind the same barrier (penalized_partial).
 template <int CW>
 __device__ __noinline__ int draw_truncated(const Params& P, int pos) {
-  const int id = sampling::draw_block<CW * 32>(P.logits, P.vocab_size, *P.sampling, pos, P.arg_val, P.arg_idx,
+  const float* l = sampling::penalty_active(P.penalty) ? P.penalized : P.logits;
+  const int id = sampling::draw_block<CW * 32>(l, P.vocab_size, *P.sampling, pos, P.arg_val, P.arg_idx,
                                                static_cast<int>(gridDim.x), smem + kCtlBytes, P.xbuf_bytes,
                                                [] { consumer_sync<CW * 32>(); });
   consumer_sync<CW * 32>();
@@ -2442,8 +2481,9 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
   // =============================== consumer warps ===============================================
   unsigned bar_target = P.barrier_base;
   int token = P.state->token;
-  if (static_cast<unsigned>(token) >= static_cast<unsigned>(P.vocab_size)) token = 0;
   int pos = P.state->pos;
+  record_fed<CT>(P, pos, token);
+  if (static_cast<unsigned>(token) >= static_cast<unsigned>(P.vocab_size)) token = 0;
   int step = P.state->step;
   float4* xres4 = reinterpret_cast<float4*>(xres);
   constexpr int kPhaseWords = static_cast<int>(sizeof(Phase) / 4);
@@ -2553,6 +2593,7 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
       }
     }
     token = (P.teacher != nullptr && step + 1 < P.max_steps) ? P.teacher[step + 1] : next;
+    if (!stop && tok + 1 < P.n_tokens) record_fed<CT>(P, pos + 1, token);  // the next token of this launch
     if (static_cast<unsigned>(token) >= static_cast<unsigned>(P.vocab_size)) token = 0;
     pos += 1;
     step += 1;
@@ -3173,6 +3214,9 @@ Params MegaEngine::params(int n_tokens, const int32_t* teacher_dev, unsigned lon
   P.arg_idx = static_cast<int*>(d_arg_idx_);
   P.sampling = m.sampling;
   P.logits = m.logits;
+  P.penalty = penalty_;
+  P.hist = m.hist;
+  P.penalized = m.penalized;
   P.prof = prof_dev;
   P.prof_token = prof_token;
   for (int i = 0; i < mega::kMaxStopIds; ++i) P.stop_ids[i] = -1;  // ids are >= 0: no stop

@@ -138,6 +138,12 @@ struct Params {
   int* arg_idx;
   const SampleParams* sampling;  // read when a token's id is drawn: changing it needs no new engine
   const float* logits;           // [vocab]: complete once the classifier's grid barrier is passed
+  // Repetition penalty (sampling.cuh step 0b): the settings of this launch (a copy of the decoder's, which change
+  // only between launches), hist[seq_len] the id fed at each position, penalized[vocab] the penalised logits,
+  // complete behind the same barrier as `logits` when the penalty is on.
+  PenaltyParams penalty;
+  int32_t* hist;
+  float* penalized;
   // Stoppable run (kllm_decoder_generate_until): the run ends after the first token whose id is one of
   // stop_ids (unused entries are -1, so a run without stop ids compares against nothing), and each id is
   // also published to stream_ids[step] followed by stream_count = step + 1 (mapped host memory; null: off).
@@ -175,6 +181,8 @@ struct MegaModel {
   void* state;
   int32_t* out_tokens;
   const SampleParams* sampling;
+  int32_t* hist;
+  float* penalized;
   // tensor parallel (tp_world > 1): exchange areas of every rank (kllm_comm, CUDA IPC)
   int tp_world, tp_rank;
   unsigned long long* tp_data[8];
@@ -195,6 +203,8 @@ class MegaEngine {
   // here: the caller passes that number (state.step) to account() before the next launch.
   int run_until(int n_tokens, const int32_t* stop_ids, int n_stop, int32_t* stream_ids, int32_t* stream_count);
   void account(int n_tokens);
+  // the repetition penalty of later launches (kllm_decoder_set_repetition_penalty, after its stream synchronise)
+  void set_penalty(const PenaltyParams& pp) { penalty_ = pp; }
   int grid() const { return grid_; }
   bool ready() const { return ready_; }
   int stages() const { return stages_; }
@@ -213,6 +223,7 @@ class MegaEngine {
                       int skip_cls_tokens) const;
   int launch(const mega::Params& P);
   MegaModel model_{};
+  PenaltyParams penalty_{};
   cudaStream_t stream_ = nullptr;
   void* d_phases_ = nullptr;
   void* d_barrier_ = nullptr;

@@ -2,7 +2,16 @@
 // (kllm_sample_f32, the graph engine's argmax_advance_kernel, the persistent megakernel).  Its numpy
 // mirror is kuiperllama_b200/sampling.py; DESIGN.md "Sampling" gives the reasons.
 //
-// Inputs: logits l[0..V) of position `pos`, temperature T, top_k k, top_p, 64-bit seed.
+// Inputs: logits l[0..V) of position `pos`, temperature T, top_k k, top_p, 64-bit seed, repetition penalty
+// theta with window last_n, and the history H(pos) of fed ids.
+//   0. History: H(pos) = the ids fed as input at positions j in [lo, pos], lo = 0 for last_n == 0 (the whole
+//      sequence) else max(0, pos - last_n + 1).  "Fed at j" is the id whose embedding entered the model at
+//      position j (its K/V rows are row j of the cache), by whichever entry fed it; a position never fed, or
+//      fed an id outside [0, V), holds none.  Feeding a position again overwrites it.
+//  0b. Repetition penalty (HF's RepetitionPenaltyLogitsProcessor): for i in H(pos),
+//      l'_i = l_i < 0 ? l_i * theta : l_i / theta (one fp32 IEEE multiply or divide); every other l'_i = l_i.
+//      An id that occurs more than once is penalised once.  theta == 1 is off, and then the history is not
+//      read.  Steps 1 to 5 run on l'.
 //   1. T == 0: greedy argmax (maximum, lowest index on ties) -- no noise is computed.
 //   2. s_i = l_i / T, IEEE division.
 //   3. 0 < k < V: tau = the k-th largest s_i; keep every i with s_i >= tau (ties at tau are kept).
@@ -39,7 +48,46 @@ struct SampleParams {
   float top_p;
 };
 
+// Device-resident repetition penalty (kllm_decoder_set_repetition_penalty), apart from SampleParams so that
+// setting either leaves the other alone.  A zeroed struct is off, as is penalty 1.
+struct PenaltyParams {
+  float penalty;
+  int32_t last_n;
+};
+
 namespace sampling {
+
+__host__ __device__ __forceinline__ bool penalty_active(const PenaltyParams& pp) {
+  return pp.penalty > 0.f && pp.penalty != 1.f;
+}
+
+// Step 0's lower end of the window at `pos`
+__host__ __device__ __forceinline__ int window_lo(const PenaltyParams& pp, int pos) {
+  return pp.last_n == 0 ? 0 : max(0, pos - pp.last_n + 1);
+}
+
+// Step 0b on one logit of the history
+__device__ __forceinline__ float penalize(float l, float theta) {
+  return l < 0.f ? __fmul_rn(l, theta) : __fdiv_rn(l, theta);
+}
+
+// Step 0b of logits[lo_row, hi_row) into out[lo_row, hi_row) by the NT threads of one block (or one CTA's
+// consumer threads): copy the raw rows, then penalise every id of hist[lo, pos] that falls in the range.
+// Thread t reads the history entries j = t (mod NT) only.  A duplicate id writes the same value again, so no
+// deduplication is needed.  `sync` orders the copy before the penalised writes and those before the caller's
+// reads (a CTA barrier orders global memory between its threads).
+template <int NT, class Sync>
+__device__ __forceinline__ void penalize_rows(const float* logits, float* out, int lo_row, int hi_row,
+                                              const int32_t* hist, int lo, int pos, float theta, Sync sync) {
+  const int tid = threadIdx.x;
+  for (int i = lo_row + tid; i < hi_row; i += NT) out[i] = __ldcg(logits + i);
+  sync();
+  for (int j = lo + ((tid - lo % NT) + NT) % NT; j <= pos; j += NT) {
+    const int id = hist[j];
+    if (id >= lo_row && id < hi_row) out[id] = penalize(__ldcg(logits + id), theta);
+  }
+  sync();
+}
 
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
   constexpr uint32_t kM0 = 0xD2511F53u, kM1 = 0xCD9E8D57u, kW0 = 0x9E3779B9u, kW1 = 0xBB67AE85u;

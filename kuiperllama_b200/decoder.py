@@ -300,6 +300,21 @@ class Decoder:
                                                            float(top_p), int(seed)),
                   "kllm_decoder_set_sampling_top_p")
 
+    def set_repetition_penalty(self, penalty: float, last_n: int = 0):
+        """Penalise, before every later draw, the logits of the ids fed at the last `last_n` positions (0: the whole
+        sequence), as HF's RepetitionPenaltyLogitsProcessor does (kllm_decoder_set_repetition_penalty;
+        sampling.penalize mirrors it).  penalty 1 is off; the sampling settings are left alone."""
+        check(self.lib.kllm_decoder_set_repetition_penalty(self.handle, float(penalty), int(last_n)),
+              "kllm_decoder_set_repetition_penalty")
+
+    def history(self):
+        """The id fed at each position [seq_len], -1 where none was (kllm_decoder_read_history)."""
+        import numpy as np
+        buf = np.empty(self.shape.seq_len, dtype=np.int32)
+        check(self.lib.kllm_decoder_read_history(self.handle, buf.ctypes.data_as(ctypes.c_void_p)),
+              "kllm_decoder_read_history")
+        return buf
+
     def logits(self):
         import numpy as np
         buf = np.empty(self.shape.vocab_size, dtype=np.float32)

@@ -95,11 +95,19 @@ class LLama2Model : public Model {
   // Nucleus sampling after top-k (kllm_decoder_set_sampling_top_p): call before init(); without a call init()
   // takes it from KUIPER_TOP_P.  Unset or 1 is off; init() refuses a value that is NaN, <= 0 or > 1.
   void set_top_p(float top_p);
+  // HF's repetition penalty before every draw (kllm_decoder_set_repetition_penalty, DESIGN.md 5.7), over the ids fed
+  // at the last `last_n` positions (0: the whole sequence): call before init(); without a call init() takes it from
+  // KUIPER_REPETITION_PENALTY and KUIPER_REPEAT_LAST_N.  Unset or 1 is off; init() refuses a penalty that is not
+  // finite or <= 0 and last_n < 0.  The fused paths take the ids from the decoder's history; predict() of a tensor
+  // that is not a row of the last embedding() cannot know its id and is refused while the penalty is on.
+  void set_repetition_penalty(float penalty, int32_t last_n = 0);
   // the settings in force (after init(): the environment's when set_sampling / set_top_p was not called)
   float sampling_temperature() const { return temperature_; }
   int32_t sampling_top_k() const { return top_k_; }
   uint64_t sampling_seed() const { return seed_; }
   float sampling_top_p() const { return top_p_; }
+  float sampling_repetition_penalty() const { return penalty_; }
+  int32_t sampling_repeat_last_n() const { return repeat_last_n_; }
 
   // A whole generation on the fused decoder, without a host round trip per token:
   //   1. the prompt from position 0 (the batched prefill for all but its last token when batched_prefill() is
@@ -165,6 +173,9 @@ class LLama2Model : public Model {
   bool sampling_explicit_ = false;
   float top_p_ = 1.f;
   bool top_p_explicit_ = false;
+  float penalty_ = 1.f;
+  int32_t repeat_last_n_ = 0;
+  bool penalty_explicit_ = false;
   sampler::SeededSampler* seeded_ = nullptr;  // sampler_ when sampling, else null
   std::vector<int32_t> extra_stop_ids_;       // set_stop_ids()
   mutable uint64_t embedding_calls_ = 0;

@@ -89,6 +89,12 @@ void LLama2Model::set_top_p(float top_p) {
   top_p_explicit_ = true;
 }
 
+void LLama2Model::set_repetition_penalty(float penalty, int32_t last_n) {
+  penalty_ = penalty;
+  repeat_last_n_ = last_n;
+  penalty_explicit_ = true;
+}
+
 const char* LLama2Model::decoder_engine() const { return decoder_ ? kllm_decoder_engine(decoder_) : ""; }
 
 base::Status LLama2Model::init(base::DeviceType device_type) {
@@ -125,6 +131,16 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   }
   if (!(top_p_ > 0.f && top_p_ <= 1.f))
     return error::InvalidArgument("sampling: top_p must be in (0, 1] (KUIPER_TOP_P / set_top_p)");
+  if (!penalty_explicit_) {
+    const char* rp = std::getenv("KUIPER_REPETITION_PENALTY");
+    const char* n = std::getenv("KUIPER_REPEAT_LAST_N");
+    penalty_ = rp != nullptr ? std::strtof(rp, nullptr) : 1.f;
+    repeat_last_n_ = n != nullptr ? static_cast<int32_t>(std::strtol(n, nullptr, 10)) : 0;
+  }
+  if (!std::isfinite(penalty_) || !(penalty_ > 0.f) || repeat_last_n_ < 0)
+    return error::InvalidArgument(
+        "sampling: repetition_penalty must be finite and > 0, and its last_n >= 0 (KUIPER_REPETITION_PENALTY / "
+        "KUIPER_REPEAT_LAST_N / set_repetition_penalty)");
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
     return error::InternalError("No usable CUDA device " + std::to_string(tp_.cuda_device()) + ".");
   cuda_config_ = std::make_shared<kernel::CudaConfig>();
@@ -137,7 +153,7 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   kernel::sin_cos_cache_calc_cu(config_->head_size_, config_->seq_len_, get_buffer(ModelBufferType::kSinCache),
                                 get_buffer(ModelBufferType::kCosCache), cuda_config_->stream);
   if (temperature_ > 0.f) {
-    auto seeded = std::make_unique<sampler::SeededSampler>(device_type_, temperature_, top_k_, seed_, top_p_);
+    auto seeded = std::make_unique<sampler::SeededSampler>(device_type_, temperature_, top_k_, seed_, top_p_, penalty_);
     seeded_ = seeded.get();
     sampler_ = std::move(seeded);
   } else {
@@ -518,6 +534,13 @@ base::Status LLama2Model::create_decoder() {
     LOG(INFO) << "sampling: temperature " << temperature_ << ", top_k " << top_k_ << ", top_p " << top_p_
               << ", seed " << seed_;
   }
+  if (penalty_ != 1.f) {
+    const int prc = kllm_decoder_set_repetition_penalty(decoder_, penalty_, repeat_last_n_);
+    if (prc != 0)
+      return base::error::InternalError(std::string("kllm_decoder_set_repetition_penalty failed: ") +
+                                        kllm_error_string(prc));
+    LOG(INFO) << "sampling: repetition_penalty " << penalty_ << ", last_n " << repeat_last_n_;
+  }
   LOG(INFO) << "fused decoder engine: " << kllm_decoder_engine(decoder_) << ", "
             << kllm_decoder_launches_per_step(decoder_) << " launch(es) per token";
   LOG(INFO) << "prompt prefill: "
@@ -605,6 +628,10 @@ base::Status LLama2Model::predict(const tensor::Tensor& input, const tensor::Ten
       return base::error::Success();
     }
   }
+  if (penalty_ != 1.f)
+    return base::error::InvalidArgument(
+        "repetition_penalty: predict() needs a row of the last embedding() call, whose token id the penalty's "
+        "history records (the layer path cannot know the id of another tensor)");
   if (tp_.on())
     return base::error::InvalidArgument(
         "tensor parallel: predict() needs a row of the last embedding() call (the fused decoder is the only "

@@ -191,6 +191,31 @@ size_t sampler::SeededSampler::sample(const float* logits, size_t size, void* st
   CHECK(device_type_ == base::DeviceType::kDeviceCUDA) << "SeededSampler: CUDA logits only (no CPU backend)";
   static thread_local int64_t* d_idx = nullptr;
   if (d_idx == nullptr) CHECK(cudaMalloc(reinterpret_cast<void**>(&d_idx), sizeof(int64_t)) == cudaSuccess) << "SeededSampler: cudaMalloc";
+  if (penalty_ != 1.f) {  // step 0b on a copy of the logits, then the draw from that copy
+    static thread_local float* d_pen = nullptr;
+    static thread_local size_t pen_cap = 0;
+    static thread_local int32_t* d_ids = nullptr;
+    static thread_local size_t ids_cap = 0;
+    if (pen_cap < size) {
+      if (d_pen != nullptr) cudaFree(d_pen);
+      CHECK(cudaMalloc(reinterpret_cast<void**>(&d_pen), size * sizeof(float)) == cudaSuccess) << "SeededSampler: cudaMalloc";
+      pen_cap = size;
+    }
+    if (ids_cap < history_.size()) {
+      if (d_ids != nullptr) cudaFree(d_ids);
+      CHECK(cudaMalloc(reinterpret_cast<void**>(&d_ids), history_.size() * sizeof(int32_t)) == cudaSuccess)
+          << "SeededSampler: cudaMalloc";
+      ids_cap = history_.size();
+    }
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (!history_.empty())
+      CHECK(cudaMemcpyAsync(d_ids, history_.data(), history_.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s) ==
+            cudaSuccess) << "SeededSampler: copy of the history";
+    const int prc = kllm_repetition_penalty_f32(logits, d_pen, static_cast<int64_t>(size), d_ids,
+                                                static_cast<int32_t>(history_.size()), penalty_, stream);
+    CHECK(prc == 0) << "kllm_repetition_penalty_f32: " << kllm_error_string(prc);
+    logits = d_pen;
+  }
   const int rc =
       kllm_sample_top_p_f32(logits, static_cast<int64_t>(size), temperature_, top_k_, top_p_, seed_, pos_, d_idx, stream);
   CHECK(rc == 0) << "kllm_sample_top_p_f32: " << kllm_error_string(rc);

@@ -3,7 +3,7 @@
 //
 //   kuiper_decode <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...]
 //                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P]
-//                 [--generate N [--stop ID]... [--then K]]
+//                 [--repetition-penalty P N] [--generate N [--stop ID]... [--then K]]
 //
 // --generate N runs the prompt and LLama2Model::generate() for at most N ids instead (n_steps is then unused),
 // stopping at the tokenizer's stop ids and every --stop ID, and prints the ids generate() returned, followed
@@ -16,11 +16,14 @@
 // position K (so that step cannot be recognised and runs layer by layer in the middle of a sequence
 // the fused decoder started).  --logits writes the last position's logits as raw fp32.  --sampling calls
 // LLama2Model::set_sampling(T, K, SEED) before init() instead of leaving it to the environment, and --top-p
-// LLama2Model::set_top_p(P) instead of KUIPER_TOP_P.
+// LLama2Model::set_top_p(P) instead of KUIPER_TOP_P.  --repetition-penalty P N calls
+// LLama2Model::set_repetition_penalty(P, N) instead of KUIPER_REPETITION_PENALTY / KUIPER_REPEAT_LAST_N; --layers
+// applies the penalty itself, over the ids this tool fed, to the seeded draw and to its greedy argmax.
 #include <base/base.h>
 #include <cuda_runtime_api.h>
 #include <glog/logging.h>
 
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -36,7 +39,7 @@ int main(int argc, char** argv) {
   if (argc < 6) {
     std::fprintf(stderr, "usage: %s <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...] "
                          "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P] "
-                         "[--generate N [--stop ID]... [--then K]]\n", argv[0]);
+                         "[--repetition-penalty P N] [--generate N [--stop ID]... [--then K]]\n", argv[0]);
     return 2;
   }
   const std::string checkpoint = argv[1], family = argv[2], prec = argv[3];
@@ -51,6 +54,9 @@ int main(int argc, char** argv) {
   uint64_t seed = 0;
   bool set_top_p = false;
   float top_p = 1.f;
+  bool set_penalty = false;
+  float penalty = 1.f;
+  int32_t last_n = 0;
   int generate = 0, then = 0;
   std::vector<int32_t> stops;
   for (int i = 5; i < argc; ++i) {
@@ -64,6 +70,11 @@ int main(int argc, char** argv) {
     else if (!std::strcmp(argv[i], "--top-p") && i + 1 < argc) {
       set_top_p = true;
       top_p = std::strtof(argv[++i], nullptr);
+    }
+    else if (!std::strcmp(argv[i], "--repetition-penalty") && i + 2 < argc) {
+      set_penalty = true;
+      penalty = std::strtof(argv[++i], nullptr);
+      last_n = static_cast<int32_t>(std::strtol(argv[++i], nullptr, 10));
     }
     else if (!std::strcmp(argv[i], "--generate") && i + 1 < argc) generate = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--stop") && i + 1 < argc) stops.push_back(std::atoi(argv[++i]));
@@ -83,6 +94,7 @@ int main(int argc, char** argv) {
   }
   if (set_sampling) m->set_sampling(temperature, top_k, seed);
   if (set_top_p) m->set_top_p(top_p);
+  if (set_penalty) m->set_repetition_penalty(penalty, last_n);
   if (!stops.empty()) m->set_stop_ids(stops);
   base::Status st = m->init(base::DeviceType::kDeviceCUDA);
   if (!st) {
@@ -124,10 +136,19 @@ int main(int argc, char** argv) {
   if (m->sampling_temperature() > 0.f)
     seeded = std::make_unique<sampler::SeededSampler>(base::DeviceType::kDeviceCUDA, m->sampling_temperature(),
                                                       m->sampling_top_k(), m->sampling_seed(),
-                                                      m->sampling_top_p());
+                                                      m->sampling_top_p(), m->sampling_repetition_penalty());
   std::vector<float> host_logits;
   int next = -1;
   std::vector<int> chosen;
+  // --layers: the id fed at each position, and the penalty's window of them at `pos` (DESIGN.md 5.7)
+  const float theta = m->sampling_repetition_penalty();
+  const size_t vocab = m->get_buffer(model::ModelBufferType::kForwardOutput).size();
+  std::vector<int32_t> fed(static_cast<size_t>(n_steps), -1);
+  auto window = [&](int32_t pos) {
+    const int32_t n = m->sampling_repeat_last_n();
+    const int32_t lo = n == 0 ? 0 : std::max(0, pos - n + 1);
+    return std::vector<int32_t>(fed.begin() + lo, fed.begin() + pos + 1);
+  };
   auto run = [&](const tensor::Tensor& input, bool is_prompt) {
     if (!layers) {
       if (pos_tensor.index<int32_t>(0) == copy_at) {
@@ -147,11 +168,19 @@ int main(int argc, char** argv) {
     if (!is_prompt && seeded) {
       const tensor::Tensor& lg = m->get_buffer(model::ModelBufferType::kForwardOutput);
       seeded->set_position(pos_tensor.index<int32_t>(0));
+      seeded->set_history(window(pos_tensor.index<int32_t>(0)));
       next = static_cast<int>(seeded->sample(lg.ptr<float>(), lg.size(), nullptr));
     } else if (!is_prompt) {  // greedy argmax, lowest index on ties (argmax_sampler.cpp)
       tensor::Tensor lg = m->get_buffer(model::ModelBufferType::kForwardOutput).clone();
       lg.to_cpu();
-      const float* p = lg.ptr<float>();
+      float* p = lg.ptr<float>();
+      if (theta != 1.f) {  // step 0b on the host: one fp32 multiply or divide per distinct id of the window
+        std::vector<int32_t> ids = window(pos_tensor.index<int32_t>(0));
+        std::sort(ids.begin(), ids.end());
+        ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
+        for (int32_t id : ids)
+          if (id >= 0 && static_cast<size_t>(id) < lg.size()) p[id] = p[id] < 0.f ? p[id] * theta : p[id] / theta;
+      }
       size_t best = 0;
       for (size_t i = 1; i < lg.size(); ++i)
         if (p[i] > p[best]) best = i;
@@ -160,6 +189,8 @@ int main(int argc, char** argv) {
   };
   for (int32_t pos = 0; pos < n_steps; ++pos) {
     pos_tensor.index<int32_t>(0) = pos;
+    const int32_t id = pos < prompt_len ? prompt[pos] : next;
+    fed[pos] = id >= 0 && static_cast<size_t>(id) < vocab ? id : -1;
     if (pos < prompt_len - 1) {
       run(m->fill_input(pos_tensor, prompt_embedding, true), true);
     } else if (pos == prompt_len - 1) {

@@ -45,6 +45,26 @@ def gumbel(x) -> np.ndarray:
     return -np.log(-np.log(uniform(x)))
 
 
+def history_window(history, pos: int, last_n: int = 0) -> np.ndarray:
+    """Step 0's H(pos): the entries of `history` (the id fed at each position, < 0 for none) at positions
+    [lo, pos], lo = 0 for last_n == 0 else max(0, pos - last_n + 1)."""
+    lo = 0 if last_n == 0 else max(0, pos - last_n + 1)
+    return np.asarray(history, np.int64)[lo:pos + 1]
+
+
+def penalize(logits, ids, penalty: float) -> np.ndarray:
+    """Step 0b: l_i * theta for negative l_i, else l_i / theta, for every i in `ids` (ids < 0 or >= len(logits)
+    ignored, duplicates penalised once), theta = fp32(penalty); the other logits unchanged."""
+    out = np.array(logits, np.float32, copy=True)
+    ids = np.asarray(ids, np.int64)
+    ids = np.unique(ids[(ids >= 0) & (ids < out.shape[0])])
+    theta = np.float32(penalty)
+    l = out[ids]
+    with np.errstate(over="ignore"):  # both branches are evaluated; an overflow to inf is the fp32 result
+        out[ids] = np.where(l < 0, l * theta, l / theta)
+    return out
+
+
 NUCLEUS_EPS = 1e-6
 """np.exp and the device expf may differ in the last ulps of each weight, which moves A and Z by well under
 this much of Z: a nucleus comparison closer than that may go either way on the device."""
