@@ -8,19 +8,17 @@
 // and a dedicated producer warp streams that CTA's share of EVERY weight matrix, in schedule
 // order, through a ring of shared-memory stages with TMA bulk copies (cp.async.bulk ->
 // UBLKCP) signalled on mbarriers.  Weights never depend on activations, so the producer runs
-// ahead across every dependency of the token; a second producer warp can walk the same schedule a
-// few stages further ahead and only pull the bytes into L2 (cp.async.bulk.prefetch.L2;
-// KLLM_PREFETCH_STAGES, off by default -- it measured slower on an H100).
+// ahead across every dependency of the token.
 //
 // Schedule per layer:  QKV(+bias) | attention(+RoPE) | Wo | W1,W3->SiLU*gate | W2 ; then
 // classifier + greedy argmax.  RoPE moves into the attention phase so GEMV rows can be split
 // evenly over all SMs.
 //
-// Consumers (CW warps, 8 by default for fp32 and int8 weights): the rows of a ring stage are handed out as TASKS of
+// Consumers (CW = 8 warps for fp32 and int8 weights): the rows of a ring stage are handed out as TASKS of
 // up to four rows to one warp each, round-robin.  A task's rows share every load of the input vector, their
 // dot-product chains interleave (ILP instead of occupancy), their totals are folded with "packed" shuffle trees
 // (kllm_device.cuh) that do the additions of cub's tree only, and one lane per row runs the epilogues side by
-// side.  (int8, toleranced mode, opt-in: a team of warps shares a stage -- mma.sync s8 or dp4a; gemv_phase.)
+// side.
 //
 // No local memory: the ring takes the whole unified L1, so a stack access is a round trip to L2.  The kernel
 // parameters are __grid_constant__ (never copied to the stack), register buffers are always written in full
@@ -63,14 +61,6 @@ namespace mega {
 #ifndef KLLM_MBAR_HINT_NS
 #define KLLM_MBAR_HINT_NS 20000u
 #endif
-// 1: warps without a row in an attention tile skip its wait and block at a hardware barrier instead of
-// spinning on the mbarrier.  Off by default.
-#ifndef KLLM_ATTN_GATE
-#define KLLM_ATTN_GATE 0
-#endif
-#ifndef KLLM_TASK_ROWS
-#define KLLM_TASK_ROWS 4
-#endif
 #ifndef KLLM_PHASE_CALL
 #define KLLM_PHASE_CALL __forceinline__
 #endif
@@ -78,7 +68,9 @@ namespace mega {
 #define KLLM_STAGE_CALL __noinline__  // once per phase, and their poll buffers would otherwise push the row loops' state out
 #endif
 constexpr int kMaxStages = 16;
-constexpr int kMaxWarps = 16;
+// CW of every instantiation.  More consumer warps cap the registers of a thread below what the row loops
+// need and ptxas spills on sm_90a (int8, 14 warps: 240 tok/s against 261 with 8 on an H100 SXM at 700 W).
+constexpr int kConsumerWarps = 8;
 constexpr int kSoftmaxThreads = 256;  // mha_kernel.cu:112-127 launches 256 threads per head
 constexpr int kNormThreads = 128;     // rmsnorm_kernel.cu:58-77 launches 128 threads
 constexpr long long kSpinLimit = 120000000000LL;  // ~1 minute of SM clocks: a lost peer becomes a trap
@@ -149,10 +141,6 @@ __device__ __forceinline__ uint64_t policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
   return p;
-}
-// Non-blocking "pull this span into L2": no shared memory, no completion to wait for.
-__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ uint64_t policy_evict_last() {
   uint64_t p;
@@ -269,25 +257,21 @@ struct Pipe {
 
 // Static shared memory (namespace scope, so the phase functions address it with immediates instead of
 // pointers held in registers).  The ring leaves only a few KB of L1, so everything the inner loops
-// touch lives in shared memory or registers: the schedule entries the consumers, the ring producer
-// and the L2 prefetcher are working on (usually three different phases), the barriers and the
-// reduction scratch.
+// touch lives in shared memory or registers: the schedule entries the consumers and the ring producer
+// are working on (usually two different phases), the barriers and the reduction scratch.
 __shared__ uint64_t g_full_bar[kMaxStages];
 __shared__ uint64_t g_empty_bar[kMaxStages];
-__shared__ float g_s_warp[kMaxWarps];
-__shared__ float g_s_argv[kMaxWarps];
-__shared__ int g_s_argi[kMaxWarps];
+__shared__ float g_s_warp[kConsumerWarps];
+__shared__ float g_s_argv[kConsumerWarps];
+__shared__ int g_s_argi[kConsumerWarps];
 __shared__ float g_s_bcast;
-__shared__ volatile unsigned g_fill_count;  // ring stages the producer has issued so far
 // Stoppable runs (Params::stop_ids): the consumers set g_stop once the token's id is a stop id; the producer
 // then stops issuing and publishes where its ring position ended, 1 + (slot << 1 | parity), in g_prod_end
 // (0: still running).  The consumers drain every fill up to that position before the CTA exits.
 __shared__ volatile int g_stop;
 __shared__ volatile unsigned g_prod_end;
-__shared__ float g_s_team[kMaxWarps / 2][2][3][8];  // team form: the other members' row partials, double buffered per team
 __shared__ Phase g_ph_cons;
 __shared__ Phase g_ph_prod;
-__shared__ Phase g_ph_pf;
 constexpr int kCtlBytes = 0;
 extern __shared__ __align__(128) unsigned char smem[];
 // per-thread state the phase functions hand back to the kernel loop
@@ -542,7 +526,7 @@ __device__ __forceinline__ float small_int_to_float(int d) {
 // plane is the 16-byte chunk q of its region.
 template <int NR>
 __device__ __forceinline__ void accum_w8_dp4a(const uint32_t (&w)[NR], const uint32_t (&sc)[NR], uint32_t x, int M,
-                                              int lane, float (&acc)[NR], int it_begin = 0, int it_end = 1 << 30) {
+                                              int lane, float (&acc)[NR]) {
   // lane owns 16 consecutive elements per step of 512: group = 8 * step + lane / 4, quarter = lane % 4
   const uint32_t odd = (lane >> 2) & 1u;
   const uint32_t gq = x + (lane >> 2) * 256 + (lane & 3) * 16;
@@ -554,9 +538,9 @@ __device__ __forceinline__ void accum_w8_dp4a(const uint32_t (&w)[NR], const uin
     wp[r] = w[r] + lane * 16;
     sp[r] = sc[r] + (lane >> 2) * 4;
   }
-  const int steps = min((M + 511) >> 9, it_end);
+  const int steps = (M + 511) >> 9;
 #pragma unroll 2
-  for (int it = it_begin; it < steps; ++it) {
+  for (int it = 0; it < steps; ++it) {
     if (it * 512 + lane * 16 < M) {  // M % 512 != 0: the last step covers part of the lanes (M % 64 == 0)
       const uint4 a0 = lds_u4(l0 + it * 2048), a1 = lds_u4(l1 + it * 2048), a2 = lds_u4(l2 + it * 2048);
       const float xstep = lds_f32(xsp + it * 2048);
@@ -572,58 +556,6 @@ __device__ __forceinline__ void accum_w8_dp4a(const uint32_t (&w)[NR], const uin
       }
     }
   }
-}
-
-// ---- int8 weights x fixed-point activations on the tensor cores (TOLERANCED, same numbers as above) ----------
-// The dp4a rows above spend 12 IDP.4A per 16 weights on the integer dot-product unit, so where a ring stage holds several rows that share the input
-// vector -- every matrix with 4096-byte rows -- the 64-element groups go through mma.sync m16n8k32 (s8 x s8 ->
-// s32, SASS IMMA.16832.S8.S8) instead:
-//     A (16 x 32, row major)  rows 0..7 = the (up to 8) weight rows of the stage, rows 8..15 mirror them
-//     B (32 x 8, column major) columns 0, 1, 2 = the three digit planes of x, columns 3..7 = 0
-//     D (16 x 8, s32)          D[r][k] = sum_i w[r][i] * l_k[i]  -- the exact integers D_k of the dp4a form
-// two mma per group (K = 2 x 32); the lane that holds D[r][0..1] fetches D[r][2] from its neighbour and adds
-// s_g * step_g * (65536 D2 + 256 D1 + D0) to the row's running sum.  A PAIR of warps takes a whole stage (the
-// ring holds only six stages: one warp per stage would leave most consumer warps idle): the even warp the first
-// half of the groups, the odd warp the second half; the halves meet through shared memory.  Rows are
-// staged `row_stride` bytes apart = row length + 16, which spreads the eight rows of a fragment load over all
-// 32 banks (row r, k-quad t -> bank 4 r + t); the scale rows likewise.
-// Result: lane 4 r holds the total of row r (rows >= nrows repeat row nrows - 1).
-__device__ __forceinline__ void mma_s8(int (&c)[4], uint32_t a0, uint32_t a2, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
-      : "r"(a0), "r"(a0), "r"(a2), "r"(a2), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ float accum_w8_mma(uint32_t w_base, uint32_t row_stride, uint32_t sc_base, uint32_t sc_stride,
-                                              int nrows, uint32_t x, int g_begin, int g_end, int lane) {
-  const int gid = lane >> 2, tig = lane & 3;
-  const int r = min(gid, nrows - 1);
-  const uint32_t wrow = w_base + static_cast<uint32_t>(r) * row_stride + static_cast<uint32_t>(tig) * 4u;
-  const uint32_t srow = sc_base + static_cast<uint32_t>(r) * sc_stride;
-  const uint32_t plane = static_cast<uint32_t>(min(gid, 2));
-  const bool bcol = gid < 3;
-  float acc = 0.f;
-#pragma unroll 2
-  for (int g = g_begin; g < g_end; ++g) {
-    const uint32_t odd = static_cast<uint32_t>(g) & 1u;
-    const uint32_t xg = x + static_cast<uint32_t>(g) * 256u;
-    const uint32_t pb = xg + ((plane + odd) & 3u) * 64u + static_cast<uint32_t>(tig) * 4u;
-    uint32_t b0 = lds_u32(pb), b1 = lds_u32(pb + 16), b2 = lds_u32(pb + 32), b3 = lds_u32(pb + 48);
-    if (!bcol) b0 = b1 = b2 = b3 = 0u;
-    const uint32_t wa = wrow + static_cast<uint32_t>(g) * 64u;
-    const uint32_t a0 = lds_u32(wa), a1 = lds_u32(wa + 16), a2 = lds_u32(wa + 32), a3 = lds_u32(wa + 48);
-    const float xstep = lds_f32(xg + ((3u + odd) & 3u) * 64u);
-    const float ws = lds_f32(srow + static_cast<uint32_t>(g) * 4u);
-    int c[4] = {0, 0, 0, 0};
-    mma_s8(c, a0, a1, b0, b1);  // elements 0..31 of the group
-    mma_s8(c, a2, a3, b2, b3);  // elements 32..63
-    // c[0] = D[row gid][column 2 tig], c[1] = D[row gid][column 2 tig + 1]: |D| <= 64 * 128 * 128 = 2^20
-    const int d2 = __shfl_down_sync(kFull, c[0], 1);  // for the tig == 0 lanes: column 2 lives in tig 1
-    const float f = __fmaf_rn(small_int_to_float(d2), 65536.0f,
-                              __fmaf_rn(small_int_to_float(c[1]), 256.0f, small_int_to_float(c[0])));
-    acc = __fmaf_rn(f, __fmul_rn(xstep, ws), acc);
-  }
-  return acc;
 }
 
 // The phase's input vector (fp32, M floats at xs, M % 64 == 0) -> digit planes + step per group, in
@@ -855,7 +787,6 @@ __device__ __forceinline__ float attention_inputs(const Params& P, const Phase& 
 //       block and "thread i walks column i" is conflict-free.
 // Rows t < pos were written by earlier tokens, so -- like weights -- the producer warp streams
 // them through the ring ahead of time; only row pos is handled here from registers.
-constexpr bool kAttnGate = KLLM_ATTN_GATE != 0;
 __device__ __forceinline__ int attn_tiles(int pos, int T) { return (pos + T - 1) / T; }
 // tiles j = s, s + SP, ... < n
 __device__ __forceinline__ int own_tiles(int n, int s, int SP) { return n > s ? (n - s + SP - 1) / SP : 0; }
@@ -957,15 +888,9 @@ __device__ KLLM_PHASE_CALL Pipe attention_fused_phase(const Params& P, int head,
   for (int j = 0; j < n_tiles; ++j) {
     const int t0 = j * T;
     const int nt = min(T, pos - t0);
-    // warps without a row in this tile do not wait for it (a spinning warp costs its neighbours
-    // issue slots and shared-memory queue entries): they arrive at once and block at the hardware
-    // barrier below, which also keeps them from lapping the ring
-    const bool works = !kAttnGate || ((tid & ~31) < nt);
-    if (works) {
-      const long long w0 = stamp ? clock64() : 0;
-      mbar_wait(&full_bar[pipe.slot], pipe.parity);
-      if (stamp) c_wait += clock64() - w0;
-    }
+    const long long w0 = stamp ? clock64() : 0;
+    mbar_wait(&full_bar[pipe.slot], pipe.parity);
+    if (stamp) c_wait += clock64() - w0;
     const float4* tile = reinterpret_cast<const float4*>(stages + static_cast<size_t>(pipe.slot) * P.stage_bytes);
     if (tid < nt) {
       float score = 0.0f;
@@ -983,7 +908,6 @@ __device__ KLLM_PHASE_CALL Pipe attention_fused_phase(const Params& P, int head,
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[pipe.slot]);
     pipe.advance(S);
-    if (kAttnGate) consumer_sync<CT>();
   }
   if (tid == 0) {  // t == pos from the freshly rotated key
     const float4* k4 = reinterpret_cast<const float4*>(k_s);
@@ -1059,15 +983,9 @@ __device__ KLLM_PHASE_CALL Pipe attention_fused_phase(const Params& P, int head,
   for (int j = 0; j < n_tiles_v; ++j) {
     const int t0 = j * Tv;
     const int nt = min(Tv, pos - t0);
-    // warps without a row in this tile do not wait for it (a spinning warp costs its neighbours
-    // issue slots and shared-memory queue entries): they arrive at once and block at the hardware
-    // barrier below, which also keeps them from lapping the ring
-    const bool works = !kAttnGate || ((tid & ~31) < hs);
-    if (works) {
-      const long long w0 = stamp ? clock64() : 0;
-      mbar_wait(&full_bar[pipe.slot], pipe.parity);
-      if (stamp) c_wait += clock64() - w0;
-    }
+    const long long w0 = stamp ? clock64() : 0;
+    mbar_wait(&full_bar[pipe.slot], pipe.parity);
+    if (stamp) c_wait += clock64() - w0;
     if (tid < hs) {
       const float* vt = reinterpret_cast<const float*>(stages + static_cast<size_t>(pipe.slot) * P.stage_bytes) + tid;
       value = score_in_smem ? pv_chain_smem(smem_u32(score_head + t0), smem_u32(vt), hs * 4, nt, value)
@@ -1076,7 +994,6 @@ __device__ KLLM_PHASE_CALL Pipe attention_fused_phase(const Params& P, int head,
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[pipe.slot]);
     pipe.advance(S);
-    if (kAttnGate) consumer_sync<CT>();
   }
   if (tid < hs) {
     value = __fmaf_rn(score_head[pos], v_pos, value);
@@ -1130,15 +1047,9 @@ __device__ KLLM_PHASE_CALL Pipe attention_scores_phase(const Params& P, int head
   for (int j = split; j < n_tiles; j += SP) {
     const int t0 = j * T;
     const int nt = min(T, pos - t0);
-    // warps without a row in this tile do not wait for it (a spinning warp costs its neighbours
-    // issue slots and shared-memory queue entries): they arrive at once and block at the hardware
-    // barrier below, which also keeps them from lapping the ring
-    const bool works = !kAttnGate || ((tid & ~31) < nt);
-    if (works) {
-      const long long w0 = stamp ? clock64() : 0;
-      mbar_wait(&full_bar[pipe.slot], pipe.parity);
-      if (stamp) c_wait += clock64() - w0;
-    }
+    const long long w0 = stamp ? clock64() : 0;
+    mbar_wait(&full_bar[pipe.slot], pipe.parity);
+    if (stamp) c_wait += clock64() - w0;
     const float4* tile = reinterpret_cast<const float4*>(stages + static_cast<size_t>(pipe.slot) * P.stage_bytes);
     if (tid < nt) {
       float score = 0.0f;
@@ -1156,7 +1067,6 @@ __device__ KLLM_PHASE_CALL Pipe attention_scores_phase(const Params& P, int head
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[pipe.slot]);
     pipe.advance(S);
-    if (kAttnGate) consumer_sync<CT>();
   }
   if (split == 0 && tid == 0) {  // t == pos from the freshly rotated key
     const float4* k4 = reinterpret_cast<const float4*>(k_s);
@@ -1284,15 +1194,9 @@ __device__ KLLM_PHASE_CALL Pipe attention_pv_phase(const Params& P, int head, in
   for (int j = 0; j < n_tiles; ++j) {
     const int t0 = j * T;
     const int nt = min(T, pos - t0);
-    // warps without a row in this tile do not wait for it (a spinning warp costs its neighbours
-    // issue slots and shared-memory queue entries): they arrive at once and block at the hardware
-    // barrier below, which also keeps them from lapping the ring
-    const bool works = !kAttnGate || ((tid & ~31) < dv);
-    if (works) {
-      const long long w0 = stamp ? clock64() : 0;
-      mbar_wait(&full_bar[pipe.slot], pipe.parity);
-      if (stamp) c_wait += clock64() - w0;
-    }
+    const long long w0 = stamp ? clock64() : 0;
+    mbar_wait(&full_bar[pipe.slot], pipe.parity);
+    if (stamp) c_wait += clock64() - w0;
     if (tid < dv) {
       const float* vt = reinterpret_cast<const float*>(stages + static_cast<size_t>(pipe.slot) * P.stage_bytes) + tid;
       value = score_in_smem ? pv_chain_smem(smem_u32(score_head + t0), smem_u32(vt), dv * 4, nt, value)
@@ -1301,7 +1205,6 @@ __device__ KLLM_PHASE_CALL Pipe attention_pv_phase(const Params& P, int head, in
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[pipe.slot]);
     pipe.advance(S);
-    if (kAttnGate) consumer_sync<CT>();
   }
   if (tid < dv) {
     value = __fmaf_rn(score_head[pos], v_pos, value);
@@ -1734,19 +1637,18 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
   bool ssq_ready = false;
   // The RMSNorm weight of the phase does not depend on anything: fetch this thread's packs from L2
   // BEFORE polling the input, so their latency (~0.4 us) hides behind the poll instead of following it.
-  // Fat-warp builds only (the thin int8 build has no registers to park them in); vectors too long for
-  // kNormPre packs per thread are read after the poll as before.  Slots past the end re-read the last
-  // pack so that the buffer is always written (stays in registers).
-  constexpr int kNormPre = CW <= 6 ? 3 : (CW <= 8 ? 2 : 0);
-  const bool norm_pre = kNormPre > 0 && has_norm && n4 <= kNormPre * CT;
-  float4 nw_pre[kNormPre > 0 ? kNormPre : 1];
-  if (kNormPre > 0 && norm_pre) {
+  // Vectors too long for kNormPre packs per thread are read after the poll as before.  Slots past the end
+  // re-read the last pack so that the buffer is always written (stays in registers).
+  constexpr int kNormPre = 2;
+  const bool norm_pre = has_norm && n4 <= kNormPre * CT;
+  float4 nw_pre[kNormPre];
+  if (norm_pre) {
     const float4* nw4 = reinterpret_cast<const float4*>(ph.norm_w);
 #pragma unroll
     for (int k = 0; k < kNormPre; ++k) nw_pre[k] = __ldg(nw4 + min(tid + k * CT, n4 - 1));
   } else {
 #pragma unroll
-    for (int k = 0; k < (kNormPre > 0 ? kNormPre : 1); ++k) nw_pre[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int k = 0; k < kNormPre; ++k) nw_pre[k] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   if (ph.tp_in) {
     // x = x_old + (p_0 + ... + p_{W-1}); no grid barrier, no all-reduce kernel
@@ -1755,13 +1657,8 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
         P.tp_data[P.tp_rank] + static_cast<size_t>(tag & 1u) * P.tp_world * P.tp_stride;
     switch (P.tp_world) {
       case 1:
-        // Many thin warps (int8 build, 96 registers): all threads poll two packs each -- the poll
-        // buffers of a deeper batch would spill, and a spill is an L2 round trip here; the sum of
-        // squares is then taken from shared memory.  Few fat warps: the 128 rmsnorm threads poll four
-        // packs each and fold the sum of squares into the same pass.
-        if (CW >= 12) {
-          stage_exchange<1, 2, false>(area, P.tp_stride, tag, n4, tid, CT, xs4w, xres4);
-        } else if (has_norm) {
+        // The 128 rmsnorm threads poll four packs each and fold the sum of squares into the same pass.
+        if (has_norm) {
           if (tid < kNormThreads)
             ssq = stage_exchange<1, 4, true>(area, P.tp_stride, tag, n4, tid, kNormThreads, xs4w, xres4);
           ssq_ready = true;
@@ -1774,10 +1671,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
       default: stage_exchange<8, 1, false>(area, P.tp_stride, tag, n4, tid, CT, xs4w, xres4); break;
     }
   } else if (ph.tag_in != nullptr) {
-    if (CW >= 12)
-      stage_handoff<2>(ph.tag_in, hand_tag(ph.hand_in), n4, tid, CT, xs4w);
-    else
-      stage_handoff<4>(ph.tag_in, hand_tag(ph.hand_in), n4, tid, CT, xs4w);
+    stage_handoff<4>(ph.tag_in, hand_tag(ph.hand_in), n4, tid, CT, xs4w);
   } else {
     const float4* xg4 = reinterpret_cast<const float4*>(ph.x_from_emb ? emb_row : ph.x);
     for (int i = tid; i < n4; i += CT) xs4w[i] = __ldcg(xg4 + i);
@@ -1817,7 +1711,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
         v.w = __fmul_rn(__fmul_rn(sc, v.w), nw.w);
         xs4w[i] = v;
       };
-      if (kNormPre > 0 && norm_pre) {
+      if (norm_pre) {
 #pragma unroll
         for (int k = 0; k < kNormPre; ++k)
           if (tid + k * CT < n4) scale_pack(tid + k * CT, nw_pre[k]);
@@ -1892,15 +1786,10 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
     // A stage holds n units; they are handed out as tasks of up to 4 rows (plain: 4 units, SwiGLU:
     // 2 units = w1 + w3 rows of two outputs), task after task round-robin over the consumer warps.
     const int ups = ph.rows_per_stage / rpu;
-    // Rows per task (compile-time knob KLLM_TASK_ROWS: 1, 2 or 4).  A CTA owns only 14-83 rows of a
-    // phase and every consumer warp has to pass (wait + arrive) every ring stage in order, so a warp
-    // sitting on a fat task while its neighbours have none holds up the refill of the whole ring.
-    // The host picks the rows per task of each phase (MegaEngine::init, pick_task_rows): short phases
-    // whose rows are already in the ring when they start are as slow as their slowest warp, so they
-    // want many small tasks; long ones want fat tasks that share the loads of the input vector.
-    constexpr int kTaskRows = KLLM_TASK_ROWS;  // upper bound (compile time: which dot_rows<> forms exist)
-    const int task_rows = min(kTaskRows, max(1, ph.task_rows));
-    const int upt = ph.swiglu ? (task_rows >= 2 ? task_rows / 2 : 1) : task_rows;  // units per task
+    // Units per task: 4 rows, or 2 SwiGLU units.  The value reaches the loop through an opaque move: with the
+    // constant in sight nvcc specialises the loop and the fp32 kernel needs 152 registers instead of 148.
+    int upt;
+    asm("mov.u32 %0, %1;" : "=r"(upt) : "r"(ph.swiglu ? 2 : 4));
     int task = 0;                      // tasks of this phase so far (same count in every warp)
     for (int u = u0; u < u1; u += ups) {
       const int n = min(ups, u1 - u);
@@ -1909,65 +1798,8 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
       const long long c1 = stamp ? clock64() : 0;
       cyc_wait += c1 - c0;
       const unsigned char* sbase = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
-      if constexpr (INT8) {
-        if (ph.team && int8_fast) {
-          // TEAM form.  With one task per warp the (six) stages of the ring are consumed side by side and
-          // released together: the producer cannot refill while the consumers compute, and a phase takes the
-          // sum of both (measured: int8 rows at half the HBM rate).  Here kTeam warps share ONE stage -- each
-          // takes a slice of the columns of all its rows -- so stages are finished and released one after the
-          // other and the refill of the first overlaps the arithmetic on the next.  Member 0 adds the members'
-          // row partials (in member order, through shared memory) and runs the epilogues.
-          constexpr int kTeam = (CW % 4 == 0) ? 4 : 2, kTeams = CW / kTeam;
-          const int team = warp / kTeam, member = warp % kTeam;
-          if (task % kTeams == team) {
-            const int j = lane >> 2;  // lane 4 j ends with the total of stage row j
-            const bool owner = member == 0 && (lane & 3) == 0 && j < n;
-            float bias_v = 0.f, res_v = 0.f;
-            if (owner) prefetch_addend(u + j, bias_v, res_v);
-            const int nrows = n * rpu;
-            float tot = 0.f;
-            if (ph.mma) {  // <= 8 rows on the tensor cores; the member's share of the 64-element groups
-              const uint32_t pad = static_cast<uint32_t>(ph.row_pad);
-              const int groups = M >> 6;
-              tot = accum_w8_mma(smem_u32(sbase), static_cast<uint32_t>(row_bytes) + pad,
-                                 smem_u32(sbase) + static_cast<uint32_t>(ph.scale_off),
-                                 static_cast<uint32_t>(ph.scale_row_bytes) + pad, nrows, smem_u32(xs),
-                                 groups * member / kTeam, groups * (member + 1) / kTeam, lane);
-            } else {  // one or two long rows on dp4a; the member's share of the 512-element steps
-              const int steps = (M + 511) >> 9;
-              const uint32_t wa = smem_u32(sbase), sa = wa + static_cast<uint32_t>(ph.scale_off);
-              const uint32_t w2[2] = {wa, wa + (nrows > 1 ? static_cast<uint32_t>(row_bytes) : 0u)};
-              const uint32_t s2[2] = {sa, sa + (nrows > 1 ? static_cast<uint32_t>(ph.scale_row_bytes) : 0u)};
-              float a2[2] = {0.f, 0.f};
-              accum_w8_dp4a<2>(w2, s2, smem_u32(xs), M, lane, a2, steps * member / kTeam, steps * (member + 1) / kTeam);
-#pragma unroll
-              for (int off = 16; off > 0; off >>= 1) {
-                a2[0] += __shfl_xor_sync(kFull, a2[0], off);
-                a2[1] += __shfl_xor_sync(kFull, a2[1], off);
-              }
-              tot = j == 0 ? a2[0] : a2[1];
-            }
-            float* scratch = &g_s_team[team][(task / kTeams) & 1][0][0];
-            if (member != 0 && (lane & 3) == 0) scratch[(member - 1) * 8 + j] = tot;
-            asm volatile("bar.sync %0, %1;" ::"r"(2 + team), "n"(kTeam * 32) : "memory");  // the warps of the team
-            if (member == 0) {
-#pragma unroll
-              for (int mm = 1; mm < kTeam; ++mm) tot = __fadd_rn(tot, scratch[(mm - 1) * 8 + j]);
-              // SwiGLU stage order: w1 rows of the n units, then their w3 rows
-              const float tot_w3 = __shfl_sync(kFull, tot, min(j + n, 7) * 4);
-              if (owner) epilogue(u + j, tot, tot_w3, bias_v, res_v);
-            }
-          }
-          ++task;
-          __syncwarp();
-          if (stamp) cyc_rows += clock64() - c1;
-          if (lane == 0) mbar_arrive(&empty_bar[pipe.slot]);
-          pipe.advance(S);
-          continue;
-        }
-      }
       for (int i0 = 0; i0 < n; i0 += upt, ++task) {
-        if (task % CW != warp) continue;  // CW is 6, 8 or 16: a real modulo (a mask would idle warps 2 and 3 of 6)
+        if (task % CW != warp) continue;
         const int nu = min(upt, n - i0);
         const long long t_a = stamp ? clock64() : 0;
         float bias_v = 0.f, res_v = 0.f;
@@ -1980,7 +1812,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
         const uint32_t xa = smem_u32(xs);
         if (ph.swiglu) {
           // stage order: w1 rows of the n units, then their w3 rows
-          if (kTaskRows == 4 && nu == 2) {
+          if (nu == 2) {
             const Rows4 rp{{wa + i0 * rb, wa + (n + i0) * rb, wa + (i0 + 1) * rb, wa + (n + i0 + 1) * rb}};
             const Rows4 sp{{sa + i0 * srb, sa + (n + i0) * srb, sa + (i0 + 1) * srb, sa + (n + i0 + 1) * srb}};
             const float4 d = dot_rows<4, INT8>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
@@ -1992,7 +1824,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
             const float4 d = dot_rows<2, INT8>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
             e0 = d.x, e1 = d.y;
           }
-        } else if (kTaskRows == 4 && nu == 4) {
+        } else if (nu == 4) {
           const Rows4 rp{{wa + i0 * rb, wa + (i0 + 1) * rb, wa + (i0 + 2) * rb, wa + (i0 + 3) * rb}};
           const Rows4 sp{{sa + i0 * srb, sa + (i0 + 1) * srb, sa + (i0 + 2) * srb, sa + (i0 + 3) * srb}};
           const float4 d = dot_rows<4, INT8>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
@@ -2069,7 +1901,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
         arg_fold(wb, sampling::perturbed(ph.seg[0].out[i], sp.temperature, key, pos, i), i);
     }
 #pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {  // (the mma form runs its epilogues in lanes 0, 4, ..., 28)
+    for (int off = 1; off < 32; off <<= 1) {
       const float ov = __shfl_xor_sync(kFull, wb.v, off);
       const int oi = __shfl_xor_sync(kFull, wb.i, off);
       arg_fold(wb, ov, oi);
@@ -2170,14 +2002,12 @@ __device__ __noinline__ int draw_truncated(const Params& P, int pos) {
 
 // ---- the kernel ---------------------------------------------------------------------------------
 template <int CW, bool INT8, bool PROF>
-__global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __grid_constant__ Params P) {
+__global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __grid_constant__ Params P) {
   constexpr int CT = CW * 32;  // consumer threads
   uint64_t* full_bar = g_full_bar;
   uint64_t* empty_bar = g_empty_bar;
   Phase& s_phase_cons = g_ph_cons;
   Phase& s_phase_prod = g_ph_prod;
-  Phase& s_phase_pf = g_ph_pf;
-  volatile unsigned& s_fill_count = g_fill_count;
 
   float* xres = reinterpret_cast<float*>(smem + kCtlBytes + P.xbuf_bytes);  // residual stream (tagged modes)
   unsigned char* stages = smem + kCtlBytes + P.xbuf_bytes + P.xres_bytes;
@@ -2190,7 +2020,6 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
   const int G = gridDim.x;
 
   if (tid == 0) {
-    s_fill_count = 0u;
     g_stop = 0;
     g_prod_end = 0u;
     for (int s = 0; s < S; ++s) {
@@ -2208,7 +2037,6 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
   if (is_producer) {
     const uint64_t policy = policy_evict_first();  // weights: streamed once per token
     const uint64_t policy_kv = policy_evict_last();  // KV tiles: re-read every token, keep in L2
-    unsigned filled = 0u;
     int ppos = P.state->pos;
     for (int tok = 0; tok < P.n_tokens; ++tok, ++ppos) {
       const int n_run = tok < P.skip_cls_tokens ? P.n_phases - P.n_cls_phases : P.n_phases;  // prompt token: no classifier
@@ -2270,7 +2098,6 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
                            &full_bar[pipe.slot], policy_kv);
                 }
                 pipe.advance(S);
-                if (lane == 0) s_fill_count = ++filled; else ++filled;
               }
             }
             continue;
@@ -2291,7 +2118,6 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
                          kbase + (static_cast<size_t>(lane) * P.seq_len + t0) * 4,
                          static_cast<uint32_t>(nt) * 16, &full_bar[pipe.slot], policy_kv);
               pipe.advance(S);
-              if (lane == 0) s_fill_count = ++filled; else ++filled;
             }
           }
           if (ph.kind != kPhaseAttention) {  // this CTA's slice of V: [seq_len][dv] contiguous
@@ -2310,7 +2136,6 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
               }
               __syncwarp();
               pipe.advance(S);
-              if (lane == 0) s_fill_count = ++filled; else ++filled;
             }
           }
           continue;
@@ -2330,41 +2155,22 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
               mbar_expect_tx(&full_bar[pipe.slot],
                              static_cast<uint32_t>(nrows) * (row_bytes + ph.scale_row_bytes));
             __syncwarp();
-            if (ph.row_pad) {
-              // padded rows (mma form, nrows <= 8): one copy per weight row (lanes 0..7) and per scale row (16..23)
-              const int j = lane & 15;
-              if (j < nrows && (lane & 8) == 0) {
-                const RowRef rr = stage_row(ph, u, n, j);
-                const long long e = static_cast<long long>(rr.row) * ph.in_dim;
-                if (lane < 16) {
-                  bulk_g2s(dst + static_cast<size_t>(j) * (row_bytes + ph.row_pad),
-                           static_cast<const unsigned char*>(ph.seg[rr.seg].w) + e * wbytes, static_cast<uint32_t>(row_bytes),
-                           &full_bar[pipe.slot], policy);
-                } else {
-                  const long long g0 = ph.group_shift >= 0 ? (e >> ph.group_shift) : (e / ph.group_size);
-                  bulk_g2s(dst + ph.scale_off + static_cast<size_t>(j) * (ph.scale_row_bytes + ph.row_pad),
-                           ph.seg[rr.seg].scales + g0, static_cast<uint32_t>(ph.scale_row_bytes), &full_bar[pipe.slot],
-                           policy);
-                }
-              }
-            } else {  // one bulk copy per run of consecutive rows of one matrix (nrows <= 32: lane = row)
-              const RowRef rr = lane < nrows ? stage_row(ph, u, n, lane) : RowRef{-1, -1};
-              const int len = run_length(rr, lane, nrows);
-              if (len > 0) {
-                const long long e = static_cast<long long>(rr.row) * ph.in_dim;
-                const unsigned char* src = static_cast<const unsigned char*>(ph.seg[rr.seg].w) + e * wbytes;
-                bulk_g2s(dst + static_cast<size_t>(lane) * row_bytes, src, static_cast<uint32_t>(len) * row_bytes,
+            // one bulk copy per run of consecutive rows of one matrix (nrows <= 32: lane = row)
+            const RowRef rr = lane < nrows ? stage_row(ph, u, n, lane) : RowRef{-1, -1};
+            const int len = run_length(rr, lane, nrows);
+            if (len > 0) {
+              const long long e = static_cast<long long>(rr.row) * ph.in_dim;
+              const unsigned char* src = static_cast<const unsigned char*>(ph.seg[rr.seg].w) + e * wbytes;
+              bulk_g2s(dst + static_cast<size_t>(lane) * row_bytes, src, static_cast<uint32_t>(len) * row_bytes,
+                       &full_bar[pipe.slot], policy);
+              if (ph.scale_row_bytes) {
+                const long long g0 = ph.group_shift >= 0 ? (e >> ph.group_shift) : (e / ph.group_size);
+                bulk_g2s(dst + ph.scale_off + static_cast<size_t>(lane) * ph.scale_row_bytes,
+                         ph.seg[rr.seg].scales + g0, static_cast<uint32_t>(len) * ph.scale_row_bytes,
                          &full_bar[pipe.slot], policy);
-                if (ph.scale_row_bytes) {
-                  const long long g0 = ph.group_shift >= 0 ? (e >> ph.group_shift) : (e / ph.group_size);
-                  bulk_g2s(dst + ph.scale_off + static_cast<size_t>(lane) * ph.scale_row_bytes,
-                           ph.seg[rr.seg].scales + g0, static_cast<uint32_t>(len) * ph.scale_row_bytes,
-                           &full_bar[pipe.slot], policy);
-                }
               }
             }
             pipe.advance(S);
-            if (lane == 0) s_fill_count = ++filled; else ++filled;
           }
         } else {
           for (int u = u0; u < u1; ++u) {
@@ -2383,7 +2189,6 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
               }
               __syncwarp();
               pipe.advance(S);
-              if (lane == 0) s_fill_count = ++filled; else ++filled;
             }
           }
         }
@@ -2392,89 +2197,6 @@ __global__ void __launch_bounds__(CW * 32 + 64, 1) decode_megakernel(const __gri
   producer_done:
     // every fill up to here is issued: the consumers of a stopped run drain them before the CTA exits
     if (lane == 0) g_prod_end = 1u + ((static_cast<unsigned>(pipe.slot) << 1) | pipe.parity);
-    return;
-  }
-
-  // =============================== L2 prefetch warp ==============================================
-  // The ring (num_stages x stage_bytes per SM, ~4 us of HBM time chip-wide) is shallower than the
-  // dead time around a grid barrier or an attention phase, so HBM would idle there.  This warp
-  // walks the same weight schedule as the producer, pf_stages ring-stages AHEAD of it, and only
-  // pulls the bytes into L2 (cp.async.bulk.prefetch.L2): the outstanding window keeps HBM
-  // streaming while the SMs wait for each other, and the ring then refills from L2.
-  if (warp == CW + 1) {
-    if (P.pf_stages <= 0) return;
-    unsigned ahead = 0u;  // stages walked by this warp (same counting as the producer's `filled`)
-    int ppos = P.state->pos;
-    for (int tok = 0; tok < P.n_tokens; ++tok, ++ppos) {
-      const int n_run = tok < P.skip_cls_tokens ? P.n_phases - P.n_cls_phases : P.n_phases;
-      for (int pi = 0; pi < n_run; ++pi) {
-        {
-          const uint32_t* src = reinterpret_cast<const uint32_t*>(P.phases + pi);
-          uint32_t* dst = reinterpret_cast<uint32_t*>(&s_phase_pf);
-          __syncwarp();
-          for (int i = lane; i < static_cast<int>(sizeof(Phase) / 4); i += 32) dst[i] = __ldg(src + i);
-          __syncwarp();
-        }
-        const Phase& ph = s_phase_pf;
-        if (ph.kind == kPhaseGather) continue;
-        if (ph.kind != kPhaseGemv) {
-          // KV tiles are L2-resident already (evict_last): count the producer's ring stages only
-          if (cta < P.head_num * P.attn_split && ppos > 0) {
-            if (ph.kind == kPhaseAttnFlash)
-              ahead += 2u * static_cast<unsigned>(own_tiles(attn_tiles(ppos, P.attn_tile), cta % P.attn_split, P.attn_split));
-            else if (ph.kind != kPhaseAttnPV)
-              ahead += static_cast<unsigned>(own_tiles(attn_tiles(ppos, P.attn_tile), cta % P.attn_split, P.attn_split));
-            if (ph.kind == kPhaseAttnPV || ph.kind == kPhaseAttnFused)
-              ahead += static_cast<unsigned>(attn_tiles(ppos, P.attn_tile_v));
-          }
-          continue;
-        }
-        const int u0 = static_cast<int>(static_cast<long long>(cta) * ph.units / G);
-        const int u1 = static_cast<int>(static_cast<long long>(cta + 1) * ph.units / G);
-        const int rpu = ph.swiglu ? 2 : 1;
-        const int row_bytes = ph.in_dim * wbytes;
-        // true: the run stopped (the producer's count will not grow any more), walk no further
-        auto throttle = [&]() {
-          while (static_cast<int>(ahead - s_fill_count) >= P.pf_stages && !g_stop) __nanosleep(400);
-          return __any_sync(kFull, g_stop != 0);
-        };
-        if (ph.chunks_per_row == 1) {
-          const int ups = ph.rows_per_stage / rpu;
-          for (int u = u0; u < u1; u += ups) {
-            const int nrows = min(ups, u1 - u) * rpu;
-            if (throttle()) return;
-            {
-              const int n = nrows / rpu;
-              const RowRef rr = lane < nrows ? stage_row(ph, u, n, lane) : RowRef{-1, -1};
-              const int len = run_length(rr, lane, nrows);
-              if (len > 0) {
-                const long long e = static_cast<long long>(rr.row) * ph.in_dim;
-                bulk_prefetch_l2(static_cast<const unsigned char*>(ph.seg[rr.seg].w) + e * wbytes,
-                                 static_cast<uint32_t>(len) * row_bytes);
-                if (ph.scale_row_bytes) {
-                  const long long g0 = ph.group_shift >= 0 ? (e >> ph.group_shift) : (e / ph.group_size);
-                  bulk_prefetch_l2(ph.seg[rr.seg].scales + g0, static_cast<uint32_t>(len) * ph.scale_row_bytes);
-                }
-              }
-            }
-            ++ahead;
-          }
-        } else {
-          for (int u = u0; u < u1; ++u) {
-            const RowRef rr = resolve_row(ph, u, 0);
-            const unsigned char* src = static_cast<const unsigned char*>(ph.seg[rr.seg].w) +
-                                       static_cast<long long>(rr.row) * row_bytes;
-            for (int c = 0; c < ph.chunks_per_row; ++c) {
-              const int e0 = c * ph.chunk_elems;
-              const int ne = min(ph.chunk_elems, ph.in_dim - e0);
-              if (throttle()) return;
-              if (lane == 0) bulk_prefetch_l2(src + static_cast<size_t>(e0) * wbytes, static_cast<uint32_t>(ne) * wbytes);
-              ++ahead;
-            }
-          }
-        }
-      }
-    }
     return;
   }
 
@@ -2630,17 +2352,11 @@ using mega::Phase;
 namespace {
 // PROF: the instantiation kllm_decoder_profile launches (its stamps cost registers in the row loops)
 template <bool PROF>
-const void* kernel_for(int consumer_warps, bool int8) {
-  if (int8) {
-    if (consumer_warps == 16) return reinterpret_cast<const void*>(mega::decode_megakernel<16, true, PROF>);
-    if (consumer_warps == 14) return reinterpret_cast<const void*>(mega::decode_megakernel<14, true, PROF>);
-    if (consumer_warps == 12) return reinterpret_cast<const void*>(mega::decode_megakernel<12, true, PROF>);
-    if (consumer_warps == 6) return reinterpret_cast<const void*>(mega::decode_megakernel<6, true, PROF>);
-    return reinterpret_cast<const void*>(mega::decode_megakernel<8, true, PROF>);
-  }
-  if (consumer_warps == 6) return reinterpret_cast<const void*>(mega::decode_megakernel<6, false, PROF>);
-  return reinterpret_cast<const void*>(mega::decode_megakernel<8, false, PROF>);
+const void* kernel_for(bool int8) {
+  if (int8) return reinterpret_cast<const void*>(mega::decode_megakernel<mega::kConsumerWarps, true, PROF>);
+  return reinterpret_cast<const void*>(mega::decode_megakernel<mega::kConsumerWarps, false, PROF>);
 }
+constexpr int kThreads = mega::kConsumerWarps * 32 + 32;  // the consumer warps and the ring producer
 }  // namespace
 
 int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
@@ -2673,16 +2389,6 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     for (int d : dims)
       if (d % m.group_size != 0 || ((d / m.group_size) * 4) % 16 != 0) return KLLM_E_UNSUPPORTED;
   }
-  // consumer warps (+ the ring producer and the L2 prefetcher): 8 for fp32 and int8 rows.  With 12 or 14 int8
-  // consumers the CTA is capped at 128 registers a thread and ptxas spills on sm_90a (16 consumers: 96).
-  // Measured on an H100 SXM (700 W), Llama-2-7B int8, fast mode, bench.py --steps 128: 8 warps 261 / 262 tok/s
-  // vs 14 warps 240 / 240 (two runs each).
-  consumer_warps_ = 8;
-  if (const char* e = getenv("KLLM_CONSUMER_WARPS")) {
-    const int v = atoi(e);
-    if (int8 && (v == 6 || v == 8 || v == 12 || v == 14 || v == 16)) consumer_warps_ = v;  // fast mode: CT >= 192 quantises M <= 16384 in <= 6 rounds
-    if (!int8 && (v == 6 || v == 8)) consumer_warps_ = v;
-  }
   // int8 arithmetic: "exact" reproduces the reference's fma(x * scale, float(w), acc) per element bit for
   // bit; "fast" (KLLM_INT8_MODE=fast) is the dp4a fixed-point mode (toleranced, ~3.5x fewer instructions)
   // The same switch frees the attention's summation order (flash-decoding, attention_flash_phase).
@@ -2691,9 +2397,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   for (const char* name : {"KLLM_INT8_MODE", "KLLM_MODE"})
     if (const char* e = getenv(name)) fast_ = std::string(e) == "fast" ? 1 : 0;
   int8_fast_ = (int8 && fast_) ? 1 : 0;
-  kernel_ = kernel_for<false>(consumer_warps_, int8);
-  kernel_prof_ = kernel_for<true>(consumer_warps_, int8);
-  threads_ = consumer_warps_ * 32 + 64;
+  kernel_ = kernel_for<false>(int8);
+  kernel_prof_ = kernel_for<true>(int8);
 
   // Tagged exchange instead of "write x, grid barrier, read x" after o_proj and down_proj:
   // mandatory under tensor parallelism (it IS the all-reduce), optional on one GPU.
@@ -2720,18 +2425,18 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   int stage_bytes = int8 ? 27 * 1024 : 32 * 1024;
   if (const char* e = getenv("KLLM_STAGE_BYTES")) stage_bytes = atoi(e);
   stage_bytes = (stage_bytes + 127) & ~127;
-  attn_tile_ = std::min(stage_bytes / (hs * 4), consumer_warps_ * 32) & ~31;  // one timestep per consumer thread
+  attn_tile_ = std::min(stage_bytes / (hs * 4), mega::kConsumerWarps * 32) & ~31;  // one timestep per consumer thread
   if (attn_tile_ < 32) return KLLM_E_UNSUPPORTED;
   attn_parts_ = 1;
   if (fast_) {  // flash attention: a lane quartet per timestep, warp partials (m, l, o[hs]) in the input buffer
     if (hs & 15) return KLLM_E_UNSUPPORTED;
-    xbuf = std::max(xbuf, (2 * hs + consumer_warps_ * (hs + 2)) * 4);
+    xbuf = std::max(xbuf, (2 * hs + mega::kConsumerWarps * (hs + 2)) * 4);
   }
   // the top-k / top-p draw's scratch after the classifier (draw_truncated): the histogram and at least 64 candidates
   xbuf = std::max(xbuf, sampling::kDrawScratchBase + 64 * 8);
   xbuf = (xbuf + 127) & ~127;
   const int xres = tagged_ ? ((dim * 4 + 127) & ~127) : 0;  // the CTA's copy of the residual stream
-  const int budget = max_smem - xbuf - xres - 3584;  // static shared memory (3 KB) + slack
+  const int budget = max_smem - xbuf - xres - 3584;  // static shared memory (1.1 KB) + slack
   int stages = budget / stage_bytes;
   if (stages > mega::kMaxStages) stages = mega::kMaxStages;
   if (const char* e = getenv("KLLM_STAGES")) stages = std::min(stages, atoi(e));
@@ -2769,43 +2474,6 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
 
   // ---- phase table ---------------------------------------------------------------------------------
   std::vector<Phase> ph;
-  // Rows per consumer task (1, 2 or 4) of a phase: 4 everywhere by default -- the four rows of a task share
-  // every load of the input vector, which is meant to outweigh the better balance of small tasks.  KLLM_TASK_ROWS_RT=1|2|4 forces a size, =auto picks per phase with the cost model
-  // below (rounds x (rows + x_cost), tasks never crossing a ring stage).
-  int forced_task_rows = 4;
-  if (const char* e = getenv("KLLM_TASK_ROWS_RT")) {
-    const int v = atoi(e);
-    if (v == 1 || v == 2 || v == 4) forced_task_rows = v;
-    if (std::string(e) == "auto") forced_task_rows = 0;
-  }
-  // KLLM_INT8_MMA=1: int8 fast rows in the team form -- mma.sync m16n8k32 s8 for stages of 3-8 rows, dp4a with the
-  // columns split over the team for 1-2 long rows.  Correct (the parity suite passes with it); at one byte per
-  // weight the shared-memory reads of the fragments cost about what the dp4a arithmetic costs.  Off by default.
-  bool int8_mma = false;
-  if (const char* e = getenv("KLLM_INT8_MMA")) int8_mma = atoi(e) != 0;
-  auto pick_task_rows = [&](Phase& p) {
-    const int rpu = p.swiglu ? 2 : 1;
-    p.task_rows = 4;
-    if (p.chunks_per_row != 1) return;
-    if (forced_task_rows) {
-      p.task_rows = std::max(forced_task_rows, rpu);
-      return;
-    }
-    const int rows_cta = ((p.units + grid_ - 1) / grid_) * rpu;
-    const int rps = std::max(rpu, p.rows_per_stage);
-    const double x_cost = int8 ? 0.5 : 1.0;
-    double best_cost = 1e30;
-    for (int nr : {4, 2, 1}) {
-      if (nr < rpu) continue;  // SwiGLU units are row pairs
-      int tasks = 0;
-      for (int left = rows_cta; left > 0; left -= rps) tasks += (std::min(rps, left) + nr - 1) / nr;
-      // tasks never cross a ring stage, so at most stages x (tasks per stage) of them exist at a time
-      const int concurrent = std::max(1, std::min(consumer_warps_, stages * ((rps + nr - 1) / nr)));
-      const int rounds = (tasks + concurrent - 1) / concurrent;
-      const double cost = rounds * (std::min(nr, rps) + x_cost);
-      if (cost < best_cost - 1e-9) best_cost = cost, p.task_rows = nr;
-    }
-  };
   auto plan = [&](Phase& p) -> int {
     const int row_bytes = p.in_dim * wb;
     p.group_size = m.group_size;
@@ -2817,31 +2485,11 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     }
     p.scale_row_bytes = int8 ? (p.in_dim / m.group_size) * 4 : 0;
     const int rpu = p.swiglu ? 2 : 1;
-    // int8 fast mode: stages that hold >= 3 rows go through the tensor cores (accum_w8_mma): <= 8 rows per
-    // stage, rows and scale rows staged 16 bytes apart more than their length
-    p.mma = 0, p.row_pad = 0, p.team = 0;
-    if (int8_fast_ && int8_mma && m.group_size == 64 && p.in_dim % 64 == 0) {
-      const int padded = row_bytes + 16 + p.scale_row_bytes + 16;
-      int rows = std::min(8, stage_bytes / padded);
-      rows -= rows % rpu;
-      while (rows >= 3 && ((rows * (row_bytes + 16) + 127) & ~127) + rows * (p.scale_row_bytes + 16) > stage_bytes) rows -= rpu;
-      if (rows >= 3) {
-        p.mma = 1, p.row_pad = 16, p.team = 1;
-        p.rows_per_stage = rows;
-        p.chunks_per_row = 1;
-        p.chunk_elems = p.in_dim;
-        p.scale_off = (rows * (row_bytes + 16) + 127) & ~127;
-        pick_task_rows(p);
-        return 0;
-      }
-    }
     const int per_row = row_bytes + p.scale_row_bytes;
     if (per_row * rpu <= stage_bytes) {
       int rows = stage_bytes / per_row;
       rows -= rows % rpu;
       rows = std::min(rows, 32);  // one bulk copy per producer lane
-      // int8 fast mode, one or two long rows per stage (hidden_dim columns): a team of warps on dp4a
-      if (int8_fast_ && int8_mma && m.group_size == 64 && p.in_dim % 64 == 0 && rows <= 2) p.team = 1;
       p.rows_per_stage = rows;
       p.chunks_per_row = 1;
       p.chunk_elems = p.in_dim;
@@ -2864,7 +2512,6 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
       p.rows_per_stage = 1;
       p.scale_off = 0;
     }
-    pick_task_rows(p);
     return 0;
   };
 
@@ -3125,7 +2772,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   e = cudaFuncSetAttribute(kernel_prof_, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes_));
   if (e != cudaSuccess) return static_cast<int>(e);
   int occ = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel_, threads_, smem_bytes_);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel_, kThreads, smem_bytes_);
   if (e != cudaSuccess) return static_cast<int>(e);
   if (occ < 1) return KLLM_E_UNSUPPORTED;
   barrier_base_ = 0;
@@ -3171,11 +2818,6 @@ Params MegaEngine::params(int n_tokens, const int32_t* teacher_dev, unsigned lon
   P.attn_vsplit = attn_vsplit_;
   P.attn_parts = attn_parts_;
   P.scores = d_scores_;
-  // Off by default: on an H100 (50 MB L2) every run-ahead distance measured slower than none.  H100 SXM at a
-  // 400 W power limit, bench.py --steps 128 --reps 3, tok/s for KLLM_PREFETCH_STAGES = 0 / 4 / 8-9 (256 KB per
-  // SM) / 16 / 24: TinyLlama-1.1B fp32 585 / 566 / 544 / 399 / 379, Llama-2-7B int8 267 / 258 / 244 / 196 / 184.
-  P.pf_stages = 0;
-  if (const char* e = getenv("KLLM_PREFETCH_STAGES")) P.pf_stages = std::max(0, atoi(e));
   P.group_size = m.group_size;
   P.dim = m.dim;
   P.vocab_size = m.vocab_size;
@@ -3226,7 +2868,7 @@ Params MegaEngine::params(int n_tokens, const int32_t* teacher_dev, unsigned lon
 int MegaEngine::launch(const Params& P) {
   void* args[] = {const_cast<Params*>(&P)};
   cudaError_t e = cudaLaunchCooperativeKernel(const_cast<void*>(P.prof != nullptr ? kernel_prof_ : kernel_), dim3(grid_),
-                                              dim3(threads_), args, smem_bytes_, stream_);
+                                              dim3(kThreads), args, smem_bytes_, stream_);
   if (e != cudaSuccess) return static_cast<int>(e);
   count_launch();
   return 0;

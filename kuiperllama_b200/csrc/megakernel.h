@@ -48,10 +48,6 @@ struct Phase {
   int residual_from_emb;  // residual source is the embedding row (layer 0)
   int group_size, group_shift;
   int rows_per_stage;     // whole rows per ring stage (chunks_per_row == 1)
-  int task_rows;          // rows handed to one consumer warp at a time (1, 2 or 4; picked per phase at init)
-  int mma;                // int8 fast mode: the rows of a stage go through mma.sync m16n8k32 s8
-  int team;               // int8 fast mode: a TEAM of consumer warps shares each ring stage, splitting the columns
-  int row_pad;            // ... and are staged row_pad bytes apart more than their length (bank-conflict-free fragments)
   int chunks_per_row;     // > 1: a row spans this many stages (fp32 rows longer than a stage)
   int chunk_elems;
   int scale_off;          // byte offset of the scales region inside a stage (int8)
@@ -104,9 +100,8 @@ struct Params {
   int xres_bytes;  // shared-memory copy of the residual stream behind the input vector (tagged modes; else 0)
   int attn_tile;    // timesteps per K ring stage
   int attn_tile_v;  // timesteps per V ring stage (rows of head_size / attn_split floats)
-  int attn_split;   // CTAs per query head: K tiles round-robin, P.V output dims split (bit-exact chains)
   unsigned long long* scores;  // [head][seq_len] tagged scaled scores: scores phase -> P.V phase
-  int pf_stages;  // L2 prefetch run-ahead of the ring producer, in ring stages (0 = off)
+  int attn_split;   // CTAs per query head: K tiles round-robin, P.V output dims split (bit-exact chains)
   int group_size;
   int dim, vocab_size, head_num, head_size, kv_dim, kv_mul, seq_len, flavour;
   const float* tok_emb;
@@ -215,7 +210,6 @@ class MegaEngine {
   int attn_vsplit() const { return attn_vsplit_; }  // slices of the V cache layout
   bool fast() const { return fast_ != 0; }
   int cls_rows() const { return cls_rows_; }  // classifier rows this rank streams per token
-  int consumer_warps() const { return consumer_warps_; }
   bool int8_fast() const { return int8_fast_ != 0; }
 
  private:
@@ -236,14 +230,13 @@ class MegaEngine {
   int exch_per_token_ = 0, hands_per_token_ = 0;
   unsigned tp_seq_base_ = 0, hand_base_ = 0;
   int grid_ = 0, stages_ = 0, stage_bytes_ = 0, xbuf_bytes_ = 0, xres_bytes_ = 0, n_phases_ = 0, attn_tile_ = 0;
-  int consumer_warps_ = 8, threads_ = 0;
   int attn_split_ = 1, attn_tile_v_ = 0;
   unsigned long long* d_scores_ = nullptr;  // tagged scores of the split attention
   int int8_fast_ = 0;
   int fast_ = 0;  // numerics: 0 = bit-exact with the reference, 1 = toleranced (free summation order)
   int attn_vsplit_ = 1, attn_parts_ = 1;
   int cls_rows_ = 0, n_cls_phases_ = 1;
-  const void* kernel_ = nullptr;       // decode_megakernel<consumer warps, int8, false>
+  const void* kernel_ = nullptr;       // decode_megakernel<8 consumer warps, int8, false>
   const void* kernel_prof_ = nullptr;  // ... <.., true>: records the phase timeline stamps
   int n_barriers_per_token_ = 0;
   size_t smem_bytes_ = 0;

@@ -14,8 +14,8 @@ flips.  With `tf32=False` no operand is rounded to TF32: that is the plain fp32 
 decode step computes in its exact mode.
 
 The decode step's fast mode (`numerics = fast`) rewrites the input vector of every int8 projection with group size
-64 as 24-bit fixed point per 64-element group before the dot products (quantize_input_inplace, accum_w8_dp4a,
-accum_w8_mma); `fixed_point=True` replaces those inputs with the same fixed-point values (`fixed_point_value`, a
+64 as 24-bit fixed point per 64-element group before the dot products (quantize_input_inplace,
+accum_w8_dp4a); `fixed_point=True` replaces those inputs with the same fixed-point values (`fixed_point_value`, a
 mirror of the kernel's fp32 arithmetic), so that what remains is again fp32 summation order.  Its attention
 (flash-decoding) reorders the softmax sums only, which the exact softmax here stands for.
 

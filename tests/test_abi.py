@@ -78,6 +78,9 @@ def test_megakernel_keeps_its_state_out_of_local_memory(kllm_lib):
         usage[m.group(1)] = (int(m.group(2)), int(m.group(3)))
     defaults = {"_ZN4kllm4mega17decode_megakernelILi8ELb0ELb0EEEvNS0_6ParamsE": 168,
                 "_ZN4kllm4mega17decode_megakernelILi8ELb1ELb0EEEvNS0_6ParamsE": 168}
+    # one consumer-warp count: {fp32, int8} x {plain, profiling}
+    assert sorted(k for k in usage if "decode_megakernel" in k) == sorted(
+        f"_ZN4kllm4mega17decode_megakernelILi8ELb{int8}ELb{prof}EEEvNS0_6ParamsE" for int8 in (0, 1) for prof in (0, 1))
     for name, reg_cap in defaults.items():
         assert name in usage, sorted(k for k in usage if "megakernel" in k)
         regs, stack = usage[name]

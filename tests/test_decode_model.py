@@ -2,8 +2,8 @@
 tests/test_decode_model_gpu.py holds the kernels to.
 
 1. The fixed point (quantize_input_inplace in csrc/megakernel.cu, mirrored by fixed_point_parts): known answers,
-   the balanced base-256 digit split over every q in [-2^22, 2^22] and the integer range the dp4a and mma sums
-   stay in, and the worst rounding error: 2^-22 of the group maximum, not 2^-23, because the kernel multiplies by
+   the balanced base-256 digit split over every q in [-2^22, 2^22] and the integer range the dp4a sums stay
+   in, and the worst rounding error: 2^-22 of the group maximum, not 2^-23, because the kernel multiplies by
    a rounded reciprocal.
 2. Negative controls at the GPU test's constants: a quantiser that keeps two digit planes and two broken flash
    attentions move the model by 10x the bound or more, while +-1 unit of fp32 noise at every store (what a correct

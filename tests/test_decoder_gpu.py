@@ -446,47 +446,6 @@ def test_fast_numerics_within_north_star_tolerance(kllm_lib, monkeypatch, key, s
     exact.close(); fast.close()
 
 
-@pytest.mark.parametrize("key,steps,warps", [("small-int8", 64, None), ("small-tp-int8", 64, "12"),
-                                             ("llama2-7b-int8", 48, None), ("llama2-7b-int8", 48, "12")])
-def test_int8_tensor_core_team_form_within_tolerance(kllm_lib, monkeypatch, key, steps, warps):
-    """KLLM_INT8_MMA=1 (opt-in): int8 fast rows in the team form -- stages of 3-8 rows through mma.sync m16n8k32
-    s8 (weight rows x the three digit planes of x), one or two long rows on dp4a with the columns split over the
-    team; pairs of warps (14 consumer warps) or teams of four (12).  Same fixed-point arithmetic as the default
-    dp4a rows, different float summation order: TOLERANCED against the exact mode like the default fast mode."""
-    from kuiperllama_b200 import SHAPES, Decoder, synth_weights
-    monkeypatch.setenv("KLLM_ENGINE", "persistent")
-    if key == "llama2-7b-int8":
-        case = _full_size_case(key, 1236)
-        shape, w = case["shape"], case["w"]
-    else:
-        shape = SHAPES[key]
-        w = synth_weights(shape, "cuda", 31)
-    exact = Decoder(shape, w)
-    monkeypatch.setenv("KLLM_INT8_MMA", "1")
-    if warps:
-        monkeypatch.setenv("KLLM_CONSUMER_WARPS", warps)
-    team = Decoder(shape, w, numerics="fast")
-    monkeypatch.delenv("KLLM_INT8_MMA")
-    monkeypatch.delenv("KLLM_CONSUMER_WARPS", raising=False)
-    plain = Decoder(shape, w, numerics="fast")
-    tok, worst, differs = 1, 0.0, False
-    for pos in range(steps):
-        a = exact.step(tok, pos)
-        b = team.step(tok, pos)
-        plain.step(tok, pos)
-        la, lb = exact.logits(), team.logits()
-        worst = max(worst, float(np.abs(la - lb).max()))
-        differs = differs or not np.array_equal(lb, plain.logits())
-        top2 = np.sort(la)[-2:]
-        if top2[1] - top2[0] > 2 * TOL:
-            assert a == b, pos
-        tok = a
-    assert worst <= TOL, worst
-    assert differs, "the team form produced the plain dp4a rows' bits: it did not run"
-    for d in (exact, team, plain):
-        d.close()
-
-
 def test_fast_numerics_by_environment(kllm_lib, monkeypatch):
     """KLLM_MODE=fast overrides the descriptor's numerics at create time (and KLLM_MODE=exact a
     descriptor that asks for fast)."""

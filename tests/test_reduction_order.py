@@ -79,59 +79,3 @@ def test_quad_packed_equals_cub_tree(seed):
         acc = [v[e::4].copy() for e in range(4)]  # acc[e][lane] = thread 4 lane + e
         assert quad_packed(acc).tobytes() == cub_block128(v).tobytes()
 
-
-# ---- the fragment bookkeeping of the int8 tensor-core form (csrc/megakernel.cu, accum_w8_mma) -----------------
-# mma.sync.m16n8k32.row.col.s32.s8.s8.s32 (PTX ISA, "Matrix fragments for mma.m16n8k32"): with g = lane / 4 and
-# t = lane % 4, a0 = A[g][4t..4t+3], a1 = A[g+8][4t..], a2 = A[g][16+4t..], a3 = A[g+8][16+4t..];
-# b0 = B[4t..4t+3][g], b1 = B[16+4t..][g]; c0 = D[g][2t], c1 = D[g][2t+1], c2 = D[g+8][2t], c3 = D[g+8][2t+1].
-# accum_w8_mma puts the (up to 8) weight rows of a ring stage in rows 0..7 (mirrored into 8..15), the three
-# digit planes of the quantised input in columns 0..2 of B, runs two mma per 64-element group and lets lane
-# 4 r read D0, D1 from its own c0, c1 and D2 from c0 of lane 4 r + 1.  Simulated here lane by lane.
-def _mma_m16n8k32(a_frag, b_frag, c_frag):
-    """One warp-wide mma from per-lane fragments: a_frag[lane][4][4], b_frag[lane][2][4], c_frag[lane][4]."""
-    A = np.zeros((16, 32), np.int64)
-    B = np.zeros((32, 8), np.int64)
-    for lane in range(32):
-        g, t = lane // 4, lane % 4
-        A[g, 4 * t:4 * t + 4] = a_frag[lane][0]
-        A[g + 8, 4 * t:4 * t + 4] = a_frag[lane][1]
-        A[g, 16 + 4 * t:16 + 4 * t + 4] = a_frag[lane][2]
-        A[g + 8, 16 + 4 * t:16 + 4 * t + 4] = a_frag[lane][3]
-        B[4 * t:4 * t + 4, g] = b_frag[lane][0]
-        B[16 + 4 * t:16 + 4 * t + 4, g] = b_frag[lane][1]
-    D = A @ B
-    out = np.zeros((32, 4), np.int64)
-    for lane in range(32):
-        g, t = lane // 4, lane % 4
-        out[lane] = c_frag[lane] + np.array([D[g, 2 * t], D[g, 2 * t + 1], D[g + 8, 2 * t], D[g + 8, 2 * t + 1]])
-    return out
-
-
-@pytest.mark.parametrize("nrows", [1, 3, 6, 8])
-def test_int8_mma_fragments_give_the_three_digit_sums(nrows):
-    rng = np.random.default_rng(nrows)
-    w = rng.integers(-128, 128, (nrows, 64))          # the stage's weight rows, one 64-element group
-    planes = rng.integers(-128, 128, (3, 64))         # balanced base-256 digits of the quantised input
-    c = np.zeros((32, 4), np.int64)
-    for half in range(2):                             # elements 0..31, then 32..63 (two mma per group)
-        a_frag, b_frag = [], []
-        for lane in range(32):
-            g, t = lane // 4, lane % 4
-            r = min(g, nrows - 1)                      # lanes past the last row repeat it
-            lo = w[r, half * 32 + 4 * t: half * 32 + 4 * t + 4]
-            hi = w[r, half * 32 + 16 + 4 * t: half * 32 + 16 + 4 * t + 4]
-            a_frag.append([lo, lo, hi, hi])            # rows 8..15 mirror rows 0..7
-            if g < 3:
-                b_frag.append([planes[g, half * 32 + 4 * t: half * 32 + 4 * t + 4],
-                               planes[g, half * 32 + 16 + 4 * t: half * 32 + 16 + 4 * t + 4]])
-            else:
-                b_frag.append([np.zeros(4, np.int64), np.zeros(4, np.int64)])
-        c = _mma_m16n8k32(a_frag, b_frag, c)
-    want = w @ planes.T                                # [row][digit plane]
-    assert np.abs(want).max() < 2 ** 22               # small_int_to_float is exact below 2^22
-    for r in range(nrows):
-        lane = 4 * r
-        d0, d1 = c[lane][0], c[lane][1]
-        d2 = c[lane + 1][0]                            # __shfl_down_sync(c0, 1): column 2 lives in t = 1
-        assert (d0, d1, d2) == tuple(want[r])
-        assert c[lane + 1][1] == 0 and not c[lane + 2][:2].any()  # columns 3..7 of B are zero
