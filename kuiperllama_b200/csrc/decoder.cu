@@ -109,7 +109,6 @@ struct kllm_decoder {
   float *x = nullptr, *q = nullptr, *attn = nullptr, *h = nullptr, *logits = nullptr;
   float *score = nullptr, *kcache = nullptr, *vcache = nullptr, *sin_t = nullptr, *cos_t = nullptr;
   float* tp_tmp = nullptr;
-  float* k_raw = nullptr;  // persistent engine: un-rotated key row of the current position
   MegaEngine mega;
   bool use_mega = false;
   StepState* st = nullptr;
@@ -447,7 +446,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
       dev_alloc(&dc->kcache, kv_elems) || dev_alloc(&dc->vcache, kv_elems) ||
       dev_alloc(&dc->sin_t, static_cast<size_t>(d.seq_len) * dc->head_size) ||
       dev_alloc(&dc->cos_t, static_cast<size_t>(d.seq_len) * dc->head_size) ||
-      dev_alloc(&dc->tp_tmp, d.dim) || dev_alloc(&dc->k_raw, dc->kv_dim) || dev_alloc(&dc->penalized, d.vocab_size))
+      dev_alloc(&dc->tp_tmp, d.dim) || dev_alloc(&dc->penalized, d.vocab_size))
     return fail(static_cast<int>(cudaErrorMemoryAllocation));
   if (cudaMalloc(&dc->st, sizeof(StepState)) != cudaSuccess ||
       cudaMalloc(&dc->sampling, sizeof(SampleParams)) != cudaSuccess ||
@@ -504,7 +503,6 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     mm.bq = dc->bq.empty() ? nullptr : dc->bq.data();
     mm.bk = dc->bk.empty() ? nullptr : dc->bk.data();
     mm.bv = dc->bv.empty() ? nullptr : dc->bv.data();
-    mm.x = dc->x, mm.q = dc->q, mm.k_raw = dc->k_raw, mm.attn_out = dc->attn, mm.h = dc->h;
     mm.logits = dc->logits, mm.score = dc->score, mm.key_cache = dc->kcache, mm.value_cache = dc->vcache;
     mm.sin_cache = dc->sin_t, mm.cos_cache = dc->cos_t, mm.state = dc->st, mm.out_tokens = dc->out_tokens;
     mm.sampling = dc->sampling;
@@ -540,7 +538,7 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->exec_until) cudaGraphExecDestroy(dc->exec_until);
   if (dc->graph_until) cudaGraphDestroy(dc->graph_until);
   float* bufs[] = {dc->x, dc->q, dc->attn, dc->h, dc->logits, dc->score,
-                   dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->k_raw, dc->penalized};
+                   dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->penalized};
   for (float* b : bufs)
     if (b) cudaFree(b);
   if (dc->st) cudaFree(dc->st);

@@ -44,8 +44,6 @@ struct Phase {
   int swiglu;             // units are (w1 row, w3 row) pairs -> SiLU*gate epilogue
   int argmax;             // track (max, index) of the produced rows (classifier)
   int cls;                // classifier work: skipped for prompt positions (llama3.cpp:733-745 discards their logits)
-  int x_from_emb;         // input vector is the embedding row of the current token
-  int residual_from_emb;  // residual source is the embedding row (layer 0)
   int group_size, group_shift;
   int rows_per_stage;     // whole rows per ring stage (chunks_per_row == 1)
   int chunks_per_row;     // > 1: a row spans this many stages (fp32 rows longer than a stage)
@@ -54,9 +52,9 @@ struct Phase {
   int scale_row_bytes;
   int layer;              // attention: layer index
   float norm_eps;
-  const float* x;         // input vector (global memory)
-  const float* norm_w;    // optional RMSNorm weight applied to x
-  const float* residual;  // optional residual vector
+  const float* norm_w;    // optional RMSNorm weight applied to the input vector
+  // The input vector is the residual stream (tp_in), the previous phase's output (tag_in) or, when
+  // neither is set (the QKV phase of layer 0), the embedding row of the current token.
   // Tagged exchange (replaces the grid barrier AND, under tensor parallelism, the all-reduce):
   //   tp_out: each produced row is published as {value, tag} -- one 64-bit store -- into every
   //           rank's exchange area instead of seg[0].out; no residual add, no barrier after.
@@ -68,8 +66,6 @@ struct Phase {
   int tp_in, tp_out;
   int exch;      // index (within the token) of the exchange tp_in consumes
   int exch_out;  // ... of the exchange tp_out publishes (a phase may do both: the sharded classifier)
-  int barrier_after;      // 1: a grid barrier closes the phase
-  int barrier_idx;        // barriers of this token passed once this phase is closed
   // Local tagged hand-offs (same words, one rank): the phase's input vector is polled from tag_in
   // (GEMV) or tq/tk/tv (attention: this head's query, its kv head's raw key and value rows);
   // outputs go to seg[].tag_out (GEMV) or ta (attention).  hand_in / hand_out number the
@@ -92,12 +88,11 @@ struct Params {
   const Phase* phases;
   int n_phases, n_tokens;
   int attn_vsplit;      // V cache layout [L][kv_head][attn_vsplit][seq_len][head_size / attn_vsplit]
-  int attn_parts;       // flash attention: threads per timestep in the scores pass
-  int int8_fast;        // int8 weights: 1 = fixed-point activations on dp4a (toleranced), 0 = the reference's per-element order
+  int int8_fast;       // int8 weights: 1 = fixed-point activations on dp4a (toleranced), 0 = the reference's per-element order
   int n_cls_phases;     // trailing phases that make up the classifier (1, or 2 with the vocabulary-sharded form)
   int skip_cls_tokens;  // the first skip_cls_tokens positions of this launch are prompt tokens: no classifier pass
   int num_stages, stage_bytes, xbuf_bytes;
-  int xres_bytes;  // shared-memory copy of the residual stream behind the input vector (tagged modes; else 0)
+  int xres_bytes;  // shared-memory copy of the residual stream behind the input vector
   int attn_tile;    // timesteps per K ring stage
   int attn_tile_v;  // timesteps per V ring stage (rows of head_size / attn_split floats)
   unsigned long long* scores;  // [head][seq_len] tagged scaled scores: scores phase -> P.V phase
@@ -105,9 +100,6 @@ struct Params {
   int group_size;
   int dim, vocab_size, head_num, head_size, kv_dim, kv_mul, seq_len, flavour;
   const float* tok_emb;
-  const float* q;
-  const float* k_raw;
-  float* attn_out;
   float* score;
   // KV cache in the persistent engine's own layout (see megakernel.cu "KV layout"):
   //   K [L][kv_head][head_size/4][seq_len][4]    V [L][kv_head][attn_split][seq_len][head_size/attn_split]
@@ -120,8 +112,8 @@ struct Params {
   const int32_t* teacher;
   int max_steps;
   unsigned* barrier;
+  // one grid barrier per token: token tok of this launch passes it when *barrier reaches barrier_base + (tok + 1) * grid
   unsigned barrier_base;
-  int bars_per_token;
   // tagged exchange areas: tp_data[r] = rank r's area [2 slots][tp_world][tp_stride] of 64-bit
   // {tag:32 | fp32 bits:32}; tp_data[tp_rank] is local memory, the others NVLink peer mappings
   unsigned long long* tp_data[8];
@@ -170,7 +162,7 @@ struct MegaModel {
   const float* scls;
   const float* const* bq; const float* const* bk; const float* const* bv;
   // activations / state owned by the decoder
-  float* x; float* q; float* k_raw; float* attn_out; float* h; float* logits; float* score;
+  float* logits; float* score;
   float* key_cache; float* value_cache;
   const float* sin_cache; const float* cos_cache;
   void* state;
@@ -201,16 +193,9 @@ class MegaEngine {
   // the repetition penalty of later launches (kllm_decoder_set_repetition_penalty, after its stream synchronise)
   void set_penalty(const PenaltyParams& pp) { penalty_ = pp; }
   int grid() const { return grid_; }
-  bool ready() const { return ready_; }
-  int stages() const { return stages_; }
-  int stage_bytes() const { return stage_bytes_; }
   int phases() const { return n_phases_; }
-  int attn_tile() const { return attn_tile_; }
-  int attn_split() const { return attn_split_; }    // CTAs per query head
   int attn_vsplit() const { return attn_vsplit_; }  // slices of the V cache layout
-  bool fast() const { return fast_ != 0; }
   int cls_rows() const { return cls_rows_; }  // classifier rows this rank streams per token
-  bool int8_fast() const { return int8_fast_ != 0; }
 
  private:
   mega::Params params(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev, int prof_token,
@@ -225,8 +210,6 @@ class MegaEngine {
   void* d_arg_idx_ = nullptr;
   unsigned long long* d_tagged_ = nullptr;  // single-GPU exchange area (tp_world == 1)
   unsigned long long* d_handoff_ = nullptr;  // local tagged hand-off vectors (q | k | v | attn | h)
-  bool tagged_ = false;
-  int tagged_mode_ = 0;  // 0: grid barriers everywhere; 1: tagged residual exchange; 2: + tagged hand-offs
   int exch_per_token_ = 0, hands_per_token_ = 0;
   unsigned tp_seq_base_ = 0, hand_base_ = 0;
   int grid_ = 0, stages_ = 0, stage_bytes_ = 0, xbuf_bytes_ = 0, xres_bytes_ = 0, n_phases_ = 0, attn_tile_ = 0;
@@ -234,11 +217,10 @@ class MegaEngine {
   unsigned long long* d_scores_ = nullptr;  // tagged scores of the split attention
   int int8_fast_ = 0;
   int fast_ = 0;  // numerics: 0 = bit-exact with the reference, 1 = toleranced (free summation order)
-  int attn_vsplit_ = 1, attn_parts_ = 1;
+  int attn_vsplit_ = 1;
   int cls_rows_ = 0, n_cls_phases_ = 1;
   const void* kernel_ = nullptr;       // decode_megakernel<8 consumer warps, int8, false>
   const void* kernel_prof_ = nullptr;  // ... <.., true>: records the phase timeline stamps
-  int n_barriers_per_token_ = 0;
   size_t smem_bytes_ = 0;
   unsigned barrier_base_ = 0;
   bool ready_ = false;

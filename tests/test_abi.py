@@ -45,6 +45,15 @@ def test_product_sources_never_touch_the_oracle():
             "liboracle" not in text, f"{p} references the oracle"
 
 
+def test_library_reads_only_the_documented_environment(kllm_lib):
+    """Every KLLM_ environment variable the library reads: the engine, the numerics mode, and the ring-stage
+    size and attention split that the decode-model tests use to reach ring geometries.  An option that nothing
+    sets is a code path that nothing tests, so a new name has to be added here on purpose."""
+    data = LIB_PATH.read_bytes()
+    names = {m.decode() for m in re.findall(rb"(?<![A-Za-z0-9_])KLLM_[A-Z0-9_]+(?=\x00)", data)}
+    assert names == {"KLLM_ENGINE", "KLLM_MODE", "KLLM_STAGE_BYTES", "KLLM_ATTN_SPLIT"}
+
+
 def test_missing_library_fails_loudly(tmp_path):
     with pytest.raises(KllmError):
         load_library(tmp_path / "libkllm_b200.so")

@@ -163,7 +163,7 @@ CASES = [("hs16", "loud", {}), ("small", "synth", {}), ("small", "loud", {}), ("
          ("small-int8", "synth", {}), ("small-int8", "outliers", {}), ("small-tp-int8", "synth", {}),
          ("llama2-7b-int8-2l", "outliers", {}),
          ("qwen2.5-reduced", "synth", {}), ("tinyllama-1.1b", "synth", {})]
-KNOBS = ("KLLM_ENGINE", "KLLM_MODE", "KLLM_INT8_MODE", "KLLM_ATTN_SPLIT", "KLLM_STAGE_BYTES")
+KNOBS = ("KLLM_ENGINE", "KLLM_MODE", "KLLM_ATTN_SPLIT", "KLLM_STAGE_BYTES")
 
 
 def case_id(c):

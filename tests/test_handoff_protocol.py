@@ -1,5 +1,5 @@
 """A schedule-fuzzing model of the persistent megakernel's barrier-free hand-over protocol
-(kuiperllama_b200/csrc/megakernel.cu, KLLM_MEGA_TAGGED=2; DESIGN.md section 5.2).
+(kuiperllama_b200/csrc/megakernel.cu; DESIGN.md section 5.2).
 
 The kernel replaces grid barriers by tagged 64-bit words: a producer publishes {tag, value} with one
 store, a consumer polls until the tag is the one it expects.  Which buffers may be single-slot, which
