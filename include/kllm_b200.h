@@ -124,6 +124,16 @@ int kllm_sample_top_p_f32(const float* logits, int64_t n, float temperature, int
  * n_ids < 0, or a penalty that is not finite or <= 0. */
 int kllm_repetition_penalty_f32(const float* logits, float* out, int64_t n, const int32_t* ids, int32_t n_ids,
                                 float penalty, void* stream);
+/* Log-probabilities of logits[0..n) (device) by the rule of DESIGN.md 5.8: out_lp[j] = log softmax(logits)[ids[j]]
+ * for j < n_ids, NaN for an id outside [0, n); out_top_ids / out_top_lp[0..top_n) = the top_n largest logits in
+ * descending order, lowest index on ties, with their log-probabilities (index -1, lp -inf past the n-th).  All
+ * outputs device memory; ids may be NULL when n_ids == 0, the top arrays when top_n == 0.  One block of one
+ * launch; no synchronisation.  The ids are exact; each lp is within the bound of DESIGN.md 5.8 of the fp64
+ * log_softmax of the same fp32 logits.  KLLM_E_INVALID for NULL pointers, n outside [1, 2^31), n_ids < 0 or
+ * top_n outside [0, KLLM_MAX_TOP_LOGPROBS]. */
+#define KLLM_MAX_TOP_LOGPROBS 20
+int kllm_logprobs_f32(const float* logits, int64_t n, const int32_t* ids, int32_t n_ids, int32_t top_n, float* out_lp,
+                      int32_t* out_top_ids, float* out_top_lp, void* stream);
 
 /* ---- fused per-layer entry points -------------------------------------------------------
  * What LLama2Model::forward (llama3.cpp:147-167) calls instead of 15 launches per layer.
@@ -354,6 +364,35 @@ int kllm_decoder_set_sampling_top_p(kllm_decoder* dec, float temperature, int32_
  * kllm_decoder_logits keeps returning the raw logits.  Synchronises the decoder's stream.  KLLM_E_INVALID,
  * with the settings in force left unchanged, for a penalty that is not finite or <= 0 and for last_n < 0. */
 int kllm_decoder_set_repetition_penalty(kllm_decoder* dec, float penalty, int32_t last_n);
+/* Log-probabilities of the returned ids, from this call on (DESIGN.md 5.8): whenever a position's classifier runs,
+ * the decoder records, at that position, the id it returns with its log-probability and, for top_n > 0, the
+ * top_n largest logits with theirs.  Log-probabilities are taken over the RAW logits (kllm_decoder_logits),
+ * before the repetition penalty, temperature, top-k and top-p, so they mean the same whatever the sampling
+ * settings.  Entries are written by kllm_decoder_step (non-prompt), the last position of _prompt /
+ * _prefill_tf32 / _prefill_w8, every position of _generate (with or without a teacher: the entry holds the
+ * drawn id) and the positions of _generate_until that ran; prompt positions whose classifier is skipped write
+ * nothing, and processing a position again overwrites its entry.  top_n -1 is off (a new decoder's setting),
+ * 0 records the id's log-probability only, 1..KLLM_MAX_TOP_LOGPROBS also the top_n.  Ids, logits, KV cache and
+ * history are bit-identical with and without it.  Clears the record (every id -1) and synchronises the stream.
+ * KLLM_E_INVALID, with the setting in force left unchanged, for top_n outside [-1, KLLM_MAX_TOP_LOGPROBS]. */
+int kllm_decoder_set_logprobs(kllm_decoder* dec, int32_t top_n);
+/* The record of positions [start_pos, start_pos + n): ids_host / lp_host [n], and, when non-NULL,
+ * top_ids_host / top_lp_host [n][top_n] with the top_n in force (nothing is written to them when it is <= 0).
+ * An id of -1 marks a position without an entry.  Blocking.  KLLM_E_INVALID for a range outside [0, seq_len)
+ * or NULL ids_host / lp_host. */
+int kllm_decoder_read_logprobs(kllm_decoder* dec, int32_t start_pos, int32_t n, int32_t* ids_host, float* lp_host,
+                               int32_t* top_ids_host, float* top_lp_host);
+/* Teacher-forced scoring: feeds tokens_host[0 .. n_tokens - 2] at positions start_pos .. start_pos + n_tokens - 2,
+ * running the classifier at every one, and writes lp_host[i] = log p(tokens_host[i + 1] | the tokens up to
+ * position start_pos + i), n_tokens - 1 values, by the rule of kllm_decoder_set_logprobs.  The record of those
+ * positions then holds the TARGET id tokens_host[i + 1] and its log-probability (with the top_n in force when
+ * logprobs are on).  Afterwards the KV cache and the history hold those positions, so tokens_host[n_tokens - 1]
+ * fed at start_pos + n_tokens - 1 continues the sequence.  Sampling and penalty settings do not change the
+ * result.  Persistent engine: one launch.  KLLM_E_INVALID, before any launch, for n_tokens < 2, a token outside
+ * [0, vocab_size), start_pos < 0, start_pos + n_tokens > seq_len (the position that continues the sequence must
+ * exist) or NULL pointers. */
+int kllm_decoder_score(kllm_decoder* dec, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
+                       float* lp_host);
 
 /* Blocking copies for tests: logits of the last step [vocab]; the KV cache in the REFERENCE
  * layout [layer][seq_len][kv_dim] (llama3.cpp:469-475) whatever the engine keeps internally. */

@@ -43,6 +43,7 @@ ALLREDUCE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_void_p, c_int, c_void_p)
 # kllm_token_callback: (ctx, ids, n_ids), called on the calling thread inside kllm_decoder_generate_until
 TOKEN_CALLBACK = ctypes.CFUNCTYPE(None, c_void_p, POINTER(c_int32), c_int32)
 MAX_STOP_IDS = 16  # KLLM_MAX_STOP_IDS
+MAX_TOP_LOGPROBS = 20  # KLLM_MAX_TOP_LOGPROBS
 
 
 class DecoderDesc(ctypes.Structure):
@@ -88,6 +89,8 @@ _SIGNATURES = {
     "kllm_sample_top_p_f32": (c_int, [c_void_p, c_int64, c_float, c_int32, c_float, c_uint64, c_int32, c_void_p,
                                       c_void_p]),
     "kllm_repetition_penalty_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int32, c_float, c_void_p]),
+    "kllm_logprobs_f32": (c_int, [c_void_p, c_int64, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
+                                  c_void_p]),
     "kllm_gemv_fused": (c_int, [POINTER(GemvJob), c_void_p]),
     "kllm_gemm_tf32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "kllm_gemm_w8_tf32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
@@ -113,6 +116,9 @@ _SIGNATURES = {
     "kllm_decoder_set_sampling_top_p": (c_int, [c_void_p, c_float, c_int32, c_float, c_uint64]),
     "kllm_decoder_set_repetition_penalty": (c_int, [c_void_p, c_float, c_int32]),
     "kllm_decoder_read_history": (c_int, [c_void_p, c_void_p]),
+    "kllm_decoder_set_logprobs": (c_int, [c_void_p, c_int32]),
+    "kllm_decoder_read_logprobs": (c_int, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "kllm_decoder_score": (c_int, [c_void_p, POINTER(c_int32), c_int32, c_int32, c_void_p]),
     "kllm_decoder_logits": (c_int, [c_void_p, c_void_p]),
     "kllm_decoder_logits_device": (c_void_p, [c_void_p]),
     "kllm_decoder_read_kv": (c_int, [c_void_p, c_void_p, c_void_p]),

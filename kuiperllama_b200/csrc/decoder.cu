@@ -61,14 +61,19 @@ __global__ void embed_token_kernel(const StepState* st, const float* __restrict_
 // the id, then the count with release semantics at system scope, which the host polls.
 // With the repetition penalty on (read from device memory, so the captured graphs stay valid), the block first
 // writes the penalised logits to `penalized` and draws from those; the raw logits are left as they are.
+// With logprobs on (also read from device memory), the block then writes the record entry of the position from the
+// raw logits (sampling.cuh, DESIGN.md 5.8): of the drawn id, or of targets[step + 1] when scoring.
 constexpr int kDrawScratchBytes = sampling::kDrawScratchBase + 2048 * 8;
+static_assert(kDrawScratchBytes >= sampling::logprob_scratch_bytes(1024), "one scratch for the draw and the logprobs");
 
 __global__ void __launch_bounds__(1024)
 argmax_advance_kernel(const float* __restrict__ logits, int n, const SampleParams* sp, StepState* st,
                       int32_t* out_tokens, const int32_t* teacher, int max_steps, int32_t* stream_ids,
-                      int32_t* stream_count, const PenaltyParams* pp, const int32_t* hist, float* penalized) {
+                      int32_t* stream_count, const PenaltyParams* pp, const int32_t* hist, float* penalized,
+                      const sampling::LogprobParams* lpp, sampling::LogprobRecord rec, const int32_t* targets) {
   __shared__ __align__(16) unsigned char scratch[kDrawScratchBytes];
   const int pos = st->pos;
+  const int step0 = st->step;  // read by every thread before thread 0 advances the state
   const float* l = logits;
   const PenaltyParams pen = *pp;
   if (sampling::penalty_active(pen)) {
@@ -78,6 +83,14 @@ argmax_advance_kernel(const float* __restrict__ logits, int n, const SampleParam
   }
   const int bi = sampling::draw_block<1024>(l, n, *sp, pos, nullptr, nullptr, 0, scratch, kDrawScratchBytes,
                                             [] { __syncthreads(); });
+  const sampling::LogprobParams lp = *lpp;
+  if (lp.top_n >= 0 && step0 >= lp.from_step) {
+    sampling::logprobs_block<1024>(logits, n, lp.top_n, scratch, kDrawScratchBytes, [] { __syncthreads(); });
+    const int id = lp.target ? targets[step0 + 1] : (bi < 0 ? 0 : bi);
+    const size_t row = static_cast<size_t>(pos) * sampling::kMaxTopLogprobs;
+    sampling::write_entry(logits, n, id, lp.top_n, *reinterpret_cast<const sampling::LogprobScratch*>(scratch),
+                          rec.id + pos, rec.lp + pos, rec.top_ids + row, rec.top_lp + row);
+  }
   if (threadIdx.x == 0) {
     const int next = bi < 0 ? 0 : bi;
     const int step = st->step;
@@ -119,6 +132,12 @@ struct kllm_decoder {
   int32_t* out_tokens = nullptr;  // device [seq_len]
   int32_t* teacher = nullptr;     // device [seq_len]
   StepState* st_host = nullptr;   // pinned
+  // log-probabilities (kllm_decoder_set_logprobs): the setting, its device copy that argmax_advance_kernel reads
+  // (two pinned staging slots: an entry may queue the target mode and its reset), and the record
+  int lp_top_n = -1;
+  sampling::LogprobParams* lp_params = nullptr;
+  sampling::LogprobParams* lp_host = nullptr;
+  sampling::LogprobRecord rec{};
   int32_t* io_host = nullptr;     // pinned scratch
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;       // out_tokens recorded, no teacher
@@ -157,6 +176,19 @@ int tp_reduce_into_x(kllm_decoder* dc, cudaStream_t s) {
   if (d.comm != nullptr) return kllm_comm_allreduce_residual(d.comm, dc->tp_tmp, dc->x, dc->x, d.dim, s);
   KLLM_TRY(d.allreduce(d.allreduce_ctx, dc->tp_tmp, d.dim, s));
   return kllm_add_f32(dc->x, dc->tp_tmp, dc->x, d.dim, s);
+}
+
+// The logprob setting argmax_advance_kernel reads for the next launches of this entry, in stream order: entries
+// before step `from_step` are prompt positions; `target` is kllm_decoder_score's mode.  While logprobs are off the
+// device copy already says off (kllm_decoder_set_logprobs and kllm_decoder_score's reset, which runs on every exit,
+// keep it so), so nothing is queued unless scoring.  The copies come from pinned staging slots, which are free again
+// because every entry ends in a stream synchronise; `slot` 1 is the reset of kllm_decoder_score, queued while the
+// copy from slot 0 may not have run yet.
+int lp_arm(kllm_decoder* dc, int target, int from_step, int slot = 0) {
+  if (dc->lp_top_n < 0 && !target && slot == 0) return 0;
+  sampling::LogprobParams* h = dc->lp_host + slot;
+  *h = sampling::LogprobParams{target ? std::max(dc->lp_top_n, 0) : dc->lp_top_n, target, from_step};
+  return static_cast<int>(cudaMemcpyAsync(dc->lp_params, h, sizeof(*h), cudaMemcpyHostToDevice, dc->stream));
 }
 
 int enqueue_step(kllm_decoder* dc, bool with_teacher, bool streamed, cudaStream_t s) {
@@ -254,7 +286,7 @@ int enqueue_step(kllm_decoder* dc, bool with_teacher, bool streamed, cudaStream_
                                            with_teacher ? dc->teacher : nullptr, d.seq_len,
                                            streamed ? dc->stream_dev + kStreamIds : nullptr,
                                            streamed ? dc->stream_dev : nullptr, dc->penalty, dc->hist,
-                                           dc->penalized);
+                                           dc->penalized, dc->lp_params, dc->rec, dc->teacher);
   count_launch();
   KLLM_TRY(cudaGetLastError());
   dc->launches_per_step = static_cast<int>(launch_counter().load() - before);
@@ -349,6 +381,7 @@ int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int3
   hs_state->step = 0;
   hs_state->next = -1;
   KLLM_TRY(cudaMemcpyAsync(dc->st, hs_state, sizeof(StepState), cudaMemcpyHostToDevice, dc->stream));
+  KLLM_TRY(lp_arm(dc, 0, 0));
   {
     kllm_gemv_job j{};
     j.x = dc->pf_ws.x + static_cast<size_t>(last_rows - 1) * d.dim;
@@ -362,7 +395,7 @@ int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int3
   }
   argmax_advance_kernel<<<1, 1024, 0, dc->stream>>>(dc->logits, d.vocab_size, dc->sampling, dc->st, nullptr, nullptr,
                                                     d.seq_len, nullptr, nullptr, dc->penalty, dc->hist,
-                                                    dc->penalized);
+                                                    dc->penalized, dc->lp_params, dc->rec, dc->teacher);
   count_launch();
   KLLM_TRY(cudaGetLastError());
   KLLM_TRY(cudaMemcpyAsync(hs_state, dc->st, sizeof(StepState), cudaMemcpyDeviceToHost, dc->stream));
@@ -455,6 +488,12 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
       cudaMalloc(&dc->out_tokens, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMalloc(&dc->teacher, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMallocHost(&dc->st_host, sizeof(StepState)) != cudaSuccess ||
+      cudaMalloc(&dc->lp_params, sizeof(sampling::LogprobParams)) != cudaSuccess ||
+      cudaMallocHost(&dc->lp_host, 2 * sizeof(sampling::LogprobParams)) != cudaSuccess ||
+      cudaMalloc(&dc->rec.id, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
+      cudaMalloc(&dc->rec.lp, sizeof(float) * d.seq_len) != cudaSuccess ||
+      cudaMalloc(&dc->rec.top_ids, sizeof(int32_t) * d.seq_len * sampling::kMaxTopLogprobs) != cudaSuccess ||
+      cudaMalloc(&dc->rec.top_lp, sizeof(float) * d.seq_len * sampling::kMaxTopLogprobs) != cudaSuccess ||
       cudaMallocHost(&dc->io_host, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaHostAlloc(&dc->stream_host, sizeof(int32_t) * (kStreamIds + d.seq_len), cudaHostAllocMapped) != cudaSuccess ||
       cudaHostGetDevicePointer(&dc->stream_dev, dc->stream_host, 0) != cudaSuccess)
@@ -464,6 +503,12 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
   cudaMemsetAsync(dc->sampling, 0, sizeof(SampleParams), dc->stream);
   cudaMemsetAsync(dc->penalty, 0, sizeof(PenaltyParams), dc->stream);
   cudaMemsetAsync(dc->hist, 0xff, sizeof(int32_t) * d.seq_len, dc->stream);  // -1: no id
+  dc->lp_host[0] = sampling::LogprobParams{-1, 0, 0};  // off
+  cudaMemcpyAsync(dc->lp_params, dc->lp_host, sizeof(sampling::LogprobParams), cudaMemcpyHostToDevice, dc->stream);
+  cudaMemsetAsync(dc->rec.id, 0xff, sizeof(int32_t) * d.seq_len, dc->stream);
+  cudaMemsetAsync(dc->rec.lp, 0, sizeof(float) * d.seq_len, dc->stream);
+  cudaMemsetAsync(dc->rec.top_ids, 0xff, sizeof(int32_t) * d.seq_len * sampling::kMaxTopLogprobs, dc->stream);
+  cudaMemsetAsync(dc->rec.top_lp, 0, sizeof(float) * d.seq_len * sampling::kMaxTopLogprobs, dc->stream);
 
   int rc = kllm_sincos_init(dc->head_size, d.seq_len, d.flavour, dc->sin_t, dc->cos_t, dc->stream);
   if (rc != 0) return fail(rc);
@@ -507,6 +552,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     mm.sin_cache = dc->sin_t, mm.cos_cache = dc->cos_t, mm.state = dc->st, mm.out_tokens = dc->out_tokens;
     mm.sampling = dc->sampling;
     mm.hist = dc->hist, mm.penalized = dc->penalized;
+    mm.lp_rec = dc->rec;
     rc = dc->mega.init(mm, dc->stream);
     if (rc == 0) {
       dc->use_mega = true;
@@ -549,6 +595,12 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->teacher) cudaFree(dc->teacher);
   if (dc->pf_buf) cudaFree(dc->pf_buf);
   if (dc->st_host) cudaFreeHost(dc->st_host);
+  if (dc->lp_params) cudaFree(dc->lp_params);
+  if (dc->lp_host) cudaFreeHost(dc->lp_host);
+  if (dc->rec.id) cudaFree(dc->rec.id);
+  if (dc->rec.lp) cudaFree(dc->rec.lp);
+  if (dc->rec.top_ids) cudaFree(dc->rec.top_ids);
+  if (dc->rec.top_lp) cudaFree(dc->rec.top_lp);
   if (dc->io_host) cudaFreeHost(dc->io_host);
   if (dc->stream_host) cudaFreeHost(dc->stream_host);
   if (dc->own_stream && dc->stream) cudaStreamDestroy(dc->stream);
@@ -565,6 +617,7 @@ int kllm_decoder_step(kllm_decoder* dc, int32_t token_host, int32_t pos, int is_
   hs->step = 0;
   hs->next = -1;
   KLLM_TRY(cudaMemcpyAsync(dc->st, hs, sizeof(StepState), cudaMemcpyHostToDevice, dc->stream));
+  KLLM_TRY(lp_arm(dc, 0, is_prompt ? 1 : 0));
   if (dc->use_mega) {
     // a prompt position needs no logits (llama3.cpp:738-739 returns -1): the classifier is skipped
     KLLM_TRY(dc->mega.run(1, nullptr, nullptr, -1, is_prompt ? 1 : 0));
@@ -591,6 +644,7 @@ int kllm_decoder_prompt(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_
   std::memcpy(dc->io_host, tokens_host, sizeof(int32_t) * n_tokens);
   KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_tokens, cudaMemcpyHostToDevice,
                            dc->stream));
+  KLLM_TRY(lp_arm(dc, 0, n_tokens - 1));  // the last position only, as on the persistent engine
   if (dc->use_mega) {
     // ONE launch for the whole prompt; only the last position runs the classifier
     KLLM_TRY(dc->mega.run(n_tokens, dc->teacher, nullptr, -1, n_tokens - 1));
@@ -641,6 +695,7 @@ int kllm_decoder_generate(kllm_decoder* dc, int32_t first_token, int32_t start_p
     KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_steps,
                              cudaMemcpyHostToDevice, dc->stream));
   }
+  KLLM_TRY(lp_arm(dc, 0, 0));
   if (dc->use_mega) {
     KLLM_TRY(dc->mega.run(n_steps, teacher_host ? dc->teacher : nullptr));
   } else {
@@ -676,6 +731,7 @@ int kllm_decoder_generate_until(kllm_decoder* dc, int32_t first_token, int32_t s
   hs->step = 0;
   hs->next = -1;
   KLLM_TRY(cudaMemcpyAsync(dc->st, hs, sizeof(StepState), cudaMemcpyHostToDevice, dc->stream));
+  KLLM_TRY(lp_arm(dc, 0, 0));
   int32_t n = 0;
   if (dc->use_mega) {
     // One launch that stops on the device; the host hands over whatever ids the count says have arrived
@@ -746,6 +802,87 @@ int kllm_decoder_set_repetition_penalty(kllm_decoder* dc, float penalty, int32_t
   KLLM_TRY(cudaMemcpyAsync(dc->penalty, &pp, sizeof(pp), cudaMemcpyHostToDevice, dc->stream));
   KLLM_TRY(cudaStreamSynchronize(dc->stream));
   if (dc->use_mega) dc->mega.set_penalty(pp);  // the megakernel takes it in its launch parameters
+  return 0;
+}
+
+int kllm_decoder_set_logprobs(kllm_decoder* dc, int32_t top_n) {
+  if (!dc || top_n < -1 || top_n > KLLM_MAX_TOP_LOGPROBS) return KLLM_E_INVALID;
+  static_assert(sampling::kMaxTopLogprobs == KLLM_MAX_TOP_LOGPROBS, "one top-N capacity");
+  // no step of this decoder may still be writing the record or reading the old setting
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  dc->lp_top_n = top_n;
+  dc->lp_host[0] = sampling::LogprobParams{top_n, 0, 0};
+  const size_t S = dc->d.seq_len, T = S * sampling::kMaxTopLogprobs;
+  KLLM_TRY(cudaMemcpyAsync(dc->lp_params, dc->lp_host, sizeof(sampling::LogprobParams), cudaMemcpyHostToDevice,
+                           dc->stream));
+  KLLM_TRY(cudaMemsetAsync(dc->rec.id, 0xff, sizeof(int32_t) * S, dc->stream));
+  KLLM_TRY(cudaMemsetAsync(dc->rec.lp, 0, sizeof(float) * S, dc->stream));
+  KLLM_TRY(cudaMemsetAsync(dc->rec.top_ids, 0xff, sizeof(int32_t) * T, dc->stream));
+  KLLM_TRY(cudaMemsetAsync(dc->rec.top_lp, 0, sizeof(float) * T, dc->stream));
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  if (dc->use_mega) dc->mega.set_logprobs(top_n);  // the megakernel takes it in its launch parameters
+  return 0;
+}
+
+int kllm_decoder_read_logprobs(kllm_decoder* dc, int32_t start_pos, int32_t n, int32_t* ids_host, float* lp_host,
+                               int32_t* top_ids_host, float* top_lp_host) {
+  if (!dc || !ids_host || !lp_host || start_pos < 0 || n < 0) return KLLM_E_INVALID;
+  if (static_cast<int64_t>(start_pos) + n > dc->d.seq_len) return KLLM_E_INVALID;
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  if (n == 0) return 0;
+  KLLM_TRY(cudaMemcpy(ids_host, dc->rec.id + start_pos, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
+  KLLM_TRY(cudaMemcpy(lp_host, dc->rec.lp + start_pos, sizeof(float) * n, cudaMemcpyDeviceToHost));
+  const int N = dc->lp_top_n;
+  if (N <= 0 || (!top_ids_host && !top_lp_host)) return 0;
+  constexpr int K = sampling::kMaxTopLogprobs;
+  const size_t row0 = static_cast<size_t>(start_pos) * K, rows = static_cast<size_t>(n) * K;
+  std::vector<int32_t> ti(rows);
+  std::vector<float> tl(rows);
+  KLLM_TRY(cudaMemcpy(ti.data(), dc->rec.top_ids + row0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost));
+  KLLM_TRY(cudaMemcpy(tl.data(), dc->rec.top_lp + row0, sizeof(float) * rows, cudaMemcpyDeviceToHost));
+  for (int32_t i = 0; i < n; ++i)
+    for (int r = 0; r < N; ++r) {
+      if (top_ids_host) top_ids_host[static_cast<size_t>(i) * N + r] = ti[static_cast<size_t>(i) * K + r];
+      if (top_lp_host) top_lp_host[static_cast<size_t>(i) * N + r] = tl[static_cast<size_t>(i) * K + r];
+    }
+  return 0;
+}
+
+int kllm_decoder_score(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
+                       float* lp_host) {
+  // every refusal comes before the first launch
+  if (!dc || !tokens_host || !lp_host || n_tokens < 2 || start_pos < 0) return KLLM_E_INVALID;
+  if (static_cast<int64_t>(start_pos) + n_tokens > dc->d.seq_len) return KLLM_E_INVALID;
+  for (int32_t i = 0; i < n_tokens; ++i)
+    if (tokens_host[i] < 0 || tokens_host[i] >= dc->d.vocab_size) return KLLM_E_INVALID;
+  const int steps = n_tokens - 1;
+  StepState* hs = dc->st_host;
+  hs->token = tokens_host[0];
+  hs->pos = start_pos;
+  hs->step = 0;
+  hs->next = -1;
+  KLLM_TRY(cudaMemcpyAsync(dc->st, hs, sizeof(StepState), cudaMemcpyHostToDevice, dc->stream));
+  // the targets: the teacher holds all n tokens, one more than the positions run, so step i's target is [i + 1]
+  std::memcpy(dc->io_host, tokens_host, sizeof(int32_t) * n_tokens);
+  KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_tokens, cudaMemcpyHostToDevice, dc->stream));
+  if (dc->use_mega) {
+    KLLM_TRY(dc->mega.run(steps, dc->teacher, nullptr, -1, 0, 1));
+  } else {
+    int rc = lp_arm(dc, 1, 0);
+    int launched = 0;
+    for (; rc == 0 && launched < steps; ++launched) rc = static_cast<int>(cudaGraphLaunch(dc->exec_tf, dc->stream));
+    count_launch(static_cast<uint64_t>(dc->launches_per_step) * launched);
+    // back to the setting in force on every exit, so that no later entry records in target mode
+    const int reset = lp_arm(dc, 0, 0, 1);
+    if (rc != 0 || reset != 0) {
+      cudaStreamSynchronize(dc->stream);  // the staging slots are free again before the next entry
+      return rc != 0 ? rc : reset;
+    }
+  }
+  KLLM_TRY(cudaMemcpyAsync(dc->io_host, dc->rec.lp + start_pos, sizeof(float) * steps, cudaMemcpyDeviceToHost,
+                           dc->stream));
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  std::memcpy(lp_host, dc->io_host, sizeof(float) * steps);
   return 0;
 }
 

@@ -277,6 +277,26 @@ __global__ void penalize_ids_kernel(const float* __restrict__ logits, float* __r
   if (id >= 0 && id < n) out[id] = sampling::penalize(logits[id], penalty);
 }
 
+// kllm_logprobs_f32: the logprob rule of sampling.cuh over one block (the graph engine's partition), then lp of
+// every listed id
+__global__ void __launch_bounds__(1024) logprobs_kernel(const float* __restrict__ logits, int n,
+                                                        const int32_t* __restrict__ ids, int n_ids, int top_n,
+                                                        float* out_lp, int32_t* out_top_ids, float* out_top_lp) {
+  constexpr int kScratch = sampling::logprob_scratch_bytes(1024);
+  __shared__ __align__(16) unsigned char scratch[kScratch];
+  sampling::logprobs_block<1024>(logits, n, top_n, scratch, kScratch, [] { __syncthreads(); });
+  const sampling::LogprobScratch& ls = *reinterpret_cast<const sampling::LogprobScratch*>(scratch);
+  if (static_cast<int>(threadIdx.x) < top_n) {
+    const int i = ls.top_i[threadIdx.x];
+    out_top_ids[threadIdx.x] = i;
+    out_top_lp[threadIdx.x] = i < 0 ? -INFINITY : sampling::logprob(ls.top_v[threadIdx.x], ls.m, ls.lse_off);
+  }
+  for (int j = threadIdx.x; j < n_ids; j += 1024) {
+    const int id = ids[j];
+    out_lp[j] = (id >= 0 && id < n) ? sampling::logprob(logits[id], ls.m, ls.lse_off) : __int_as_float(0x7fffffff);
+  }
+}
+
 }  // namespace kllm
 
 using namespace kllm;
@@ -402,6 +422,16 @@ int kllm_repetition_penalty_f32(const float* logits, float* out, int64_t n, cons
     penalize_ids_kernel<<<static_cast<unsigned>((static_cast<int64_t>(n_ids) + 255) / 256), 256, 0, s>>>(logits, out, m, ids, n_ids, penalty);
     count_launch();
   }
+  return static_cast<int>(cudaGetLastError());
+}
+
+int kllm_logprobs_f32(const float* logits, int64_t n, const int32_t* ids, int32_t n_ids, int32_t top_n, float* out_lp,
+                      int32_t* out_top_ids, float* out_top_lp, void* stream) {
+  if (!logits || n <= 0 || n > 0x7fffffffLL || n_ids < 0 || (n_ids > 0 && (!ids || !out_lp))) return KLLM_E_INVALID;
+  if (top_n < 0 || top_n > KLLM_MAX_TOP_LOGPROBS || (top_n > 0 && (!out_top_ids || !out_top_lp))) return KLLM_E_INVALID;
+  logprobs_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(logits, static_cast<int>(n), ids, n_ids, top_n,
+                                                                     out_lp, out_top_ids, out_top_lp);
+  count_launch();
   return static_cast<int>(cudaGetLastError());
 }
 

@@ -1524,6 +1524,61 @@ __device__ KLLM_STAGE_CALL void stage_handoff(const unsigned long long* src, uns
   stage_handoff_inline<UP>(src, tag, n4, t, NT, xs4);
 }
 
+// ---- log-probabilities: this CTA's part (DESIGN.md 5.8) ---------------------------------------------
+// L1 of sampling.cuh over the rows [u0, u1) this CTA produced (or gathered) -- (m_c, S_c) to lp_part[cta] -- and,
+// for lp_top_n > 0, their top-N to lp_cand_v / lp_cand_i[cta] (index -1 pads a part of fewer rows).  The input
+// vector buffer is idle once every warp is done with its rows (the draw after the barrier relies on the same), so
+// it is the scratch.  CTA 0 reads the results behind the token's grid barrier (logprob_record, from
+// draw_truncated).
+template <int CW>
+__device__ __noinline__ void logprob_partial(const Params& P, const float* logits, int u0, int u1) {
+  constexpr int CT = CW * 32;
+  auto sync = [] { consumer_sync<CT>(); };
+  sync();  // the rows of every warp are stored, and no warp reads the input vector any more
+  sampling::LogprobScratch& ls = *reinterpret_cast<sampling::LogprobScratch*>(smem);
+  const float2 p = sampling::block_part<CT>([&](int i) { return __ldcg(logits + i); }, u0, u1, ls, sync);
+  if (threadIdx.x == 0) P.lp_part[blockIdx.x] = p;
+  const int N = P.lp_top_n;
+  if (N > 0) {
+    const size_t off = static_cast<size_t>(blockIdx.x) * sampling::kMaxTopLogprobs;
+    sampling::top_n_block<CT>([&](int k) { return sampling::Cand{__ldcg(logits + u0 + k), u0 + k}; }, u1 - u0, N,
+                              smem + sampling::kLogprobScratchBase, P.xbuf_bytes - sampling::kLogprobScratchBase,
+                              P.lp_cand_v + off, P.lp_cand_i + off, sync);
+  }
+}
+
+// ---- log-probabilities: the record entry (CTA 0, behind the token's grid barrier) --------------------
+// L2 over the G parts in CTA order, the top-N of the G x N candidates, then the entry of position `pos` for `id`.
+// The input vector buffer is the scratch, as in draw_truncated; the closing barrier orders every read of it before
+// the next token stages its first vector.
+template <int CW>
+__device__ __noinline__ void logprob_record(const Params& P, int pos, int id) {
+  constexpr int CT = CW * 32;
+  auto sync = [] { consumer_sync<CT>(); };
+  sampling::LogprobScratch& ls = *reinterpret_cast<sampling::LogprobScratch*>(smem);
+  const int G = gridDim.x, N = P.lp_top_n;
+  sync();  // the draw's scratch (the same buffer) is read
+  if (threadIdx.x < 32) {
+    const float2 f = sampling::warp_fold_parts([&](int c) { return __ldcg(P.lp_part + c); }, G);
+    if (threadIdx.x == 0) {
+      ls.m = f.x;
+      ls.lse_off = f.y;
+    }
+  }
+  if (N > 0) {
+    sampling::top_n_block<CT>([&](int k) { return sampling::Cand{__ldcg(P.lp_cand_v + (k / N) * sampling::kMaxTopLogprobs + k % N),
+                                                                 __ldcg(P.lp_cand_i + (k / N) * sampling::kMaxTopLogprobs + k % N)}; },
+                              G * N, N, smem + sampling::kLogprobScratchBase, P.xbuf_bytes - sampling::kLogprobScratchBase,
+                              ls.top_v, ls.top_i, sync);
+  } else {
+    sync();
+  }
+  const size_t row = static_cast<size_t>(pos) * sampling::kMaxTopLogprobs;
+  sampling::write_entry(P.logits, P.vocab_size, id, N, ls, P.lp_rec.id + pos, P.lp_rec.lp + pos,
+                        P.lp_rec.top_ids + row, P.lp_rec.top_lp + row);
+  sync();
+}
+
 // ---- repetition penalty over this CTA's classifier rows ---------------------------------------------
 // Step 0b of the rule for the rows [u0, u1) this CTA produced (their raw logits, stored by its own
 // threads): the penalised rows go to P.penalized, and the CTA's partial -- greedy, or perturbed as in the
@@ -1549,6 +1604,26 @@ __device__ __noinline__ ArgBest penalized_partial(const Params& P, const float* 
   return b;
 }
 
+// ---- the classifier rows of this CTA in logprob_megakernel --------------------------------------------
+// The log-probability partials of the raw rows [u0, u1) (logprob_partial), then the CTA's partial of the draw:
+// penalized_partial's with the penalty on, else the greedy or perturbed fold over the raw rows.
+template <int CW>
+__device__ __noinline__ ArgBest classifier_partial(const Params& P, const float* logits, int u0, int u1, int pos) {
+  constexpr int CT = CW * 32;
+  if (P.lp_top_n >= 0) logprob_partial<CW>(P, logits, u0, u1);
+  if (sampling::penalty_active(P.penalty)) return penalized_partial<CW>(P, logits, u0, u1, pos);
+  consumer_sync<CT>();  // the raw rows of every warp of the CTA are stored
+  const SampleParams sp = *P.sampling;
+  const bool perturb = sampling::perturb_only(sp, P.vocab_size);
+  const uint2 key = sampling::seed_key(sp.seed);
+  ArgBest b{0.f, -1};
+  for (int i = u0 + static_cast<int>(threadIdx.x); i < u1; i += CT) {
+    const float v = __ldcg(logits + i);
+    arg_fold(b, perturb ? sampling::perturbed(v, sp.temperature, key, pos, i) : v, i);
+  }
+  return b;
+}
+
 // The history entry of position `pos`, fed `token`: stored by consumer thread pos % CT of every CTA, the
 // one thread that reads it in penalized_partial (-1: an id outside the vocabulary holds none)
 template <int CT>
@@ -1561,7 +1636,7 @@ __device__ __forceinline__ void record_fed(const Params& P, int pos, int token) 
 // Stages the phase's input vector (tagged residual exchange / tagged hand-off / embedding row) into
 // shared memory, RMS-normalises it when the phase asks for it, consumes this CTA's ring stages
 // task by task, runs the epilogues and, for the classifier, leaves the CTA's (max, index).
-template <int CW, bool INT8, bool PROF>
+template <int CW, bool INT8, bool PROF, bool LP>
 __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int tok, int pos, const float* emb_row,
                                             unsigned long long* stamp) {
   constexpr int CT = CW * 32;
@@ -1844,8 +1919,9 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
     // that ran epilogues hold partial bests
     ArgBest wb = best;
     const SampleParams sp = *P.sampling;
-    if (sampling::penalty_active(P.penalty)) {
-      wb = penalized_partial<CW>(P, ph.seg[0].out, u0, u1, pos);
+    if (sampling::penalty_active(P.penalty) || (LP && P.lp_top_n >= 0)) {
+      if constexpr (LP) wb = classifier_partial<CW>(P, ph.seg[0].out, u0, u1, pos);
+      else wb = penalized_partial<CW>(P, ph.seg[0].out, u0, u1, pos);
     } else if (sampling::perturb_only(sp, P.vocab_size)) {
       // sampling without top-k: the partial is the argmax of s_i + g_i over the same rows, read back
       // from the logits the epilogues of this CTA have just stored
@@ -1891,7 +1967,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
 // words of the local area between them: poll, store the logit, keep (max, lowest index).  All ranks
 // end with the same full logits vector and the same per-CTA partials, hence the same greedy id --
 // the cross-rank argmax needs no further exchange.
-template <int CW>
+template <int CW, bool LP>
 __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int pos) {
   constexpr int CT = CW * 32;
   const Phase& ph = g_ph_cons;
@@ -1906,7 +1982,8 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int p
   float* logits = ph.seg[0].out;
   const SampleParams sp = *P.sampling;
   const bool perturb = sampling::perturb_only(sp, V);  // as the classifier partials (gemv_phase)
-  const bool penalized = sampling::penalty_active(P.penalty);  // then the partial is folded afterwards
+  // with the penalty or the log-probabilities on, the partial is folded afterwards (classifier_partial)
+  const bool penalized = sampling::penalty_active(P.penalty) || (LP && P.lp_top_n >= 0);
   const uint2 key = sampling::seed_key(sp.seed);
   ArgBest best{0.f, -1};
   for (int i = u0 + tid; i < u1; i += CT) {
@@ -1915,7 +1992,10 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int p
     logits[i] = v;
     if (!penalized) arg_fold(best, perturb ? sampling::perturbed(v, sp.temperature, key, pos, i) : v, i);
   }
-  if (penalized) best = penalized_partial<CW>(P, logits, u0, u1, pos);
+  if (penalized) {
+    if constexpr (LP) best = classifier_partial<CW>(P, logits, u0, u1, pos);
+    else best = penalized_partial<CW>(P, logits, u0, u1, pos);
+  }
 #pragma unroll
   for (int off = 1; off < 32; off <<= 1) {
     const float ov = __shfl_xor_sync(kFull, best.v, off);
@@ -1944,7 +2024,7 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int p
 // buffer: it is idle from the classifier's last read of its input until the next token stages its first
 // vector.  The barrier after the draw orders every thread's read of the result
 // before any thread writes that buffer again.  With the repetition penalty on, the draw reads the penalised
-// vector, which is complete behind the same barrier (penalized_partial).
+// vector, which is complete behind the same barrier (classifier_partial).
 template <int CW>
 __device__ __noinline__ int draw_truncated(const Params& P, int pos) {
   const float* l = sampling::penalty_active(P.penalty) ? P.penalized : P.logits;
@@ -1955,9 +2035,35 @@ __device__ __noinline__ int draw_truncated(const Params& P, int pos) {
   return id;
 }
 
+// The id of a token in logprob_megakernel, and the position's record entry: the draw (top-k / top-p) or the
+// kernel's fold of the per-CTA partials, then CTA 0 writes the entry -- of the target teacher[step + 1] when
+// scoring.
+template <int CW>
+__device__ __noinline__ int draw_with_logprobs(const Params& P, int pos, int step) {
+  int id;
+  if (sampling::needs_draw(*P.sampling, P.vocab_size)) {
+    id = draw_truncated<CW>(P, pos);
+  } else {  // the kernel's fold of the per-CTA partials
+    const int lane = threadIdx.x & 31;
+    ArgBest b{0.f, -1};
+    for (int c = lane; c < static_cast<int>(gridDim.x); c += 32) arg_fold(b, __ldcg(P.arg_val + c), __ldcg(P.arg_idx + c));
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const float ov = __shfl_xor_sync(kFull, b.v, off);
+      const int oi = __shfl_xor_sync(kFull, b.i, off);
+      arg_fold(b, ov, oi);
+    }
+    id = b.i < 0 ? 0 : b.i;
+  }
+  if (P.lp_top_n >= 0 && blockIdx.x == 0) logprob_record<CW>(P, pos, P.lp_target ? P.teacher[step + 1] : id);
+  return id;
+}
+
 // ---- the kernel ---------------------------------------------------------------------------------
-template <int CW, bool INT8, bool PROF>
-__global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __grid_constant__ Params P) {
+// LP: the logprob_megakernel instantiation, launched while log-probabilities are on.  decode_megakernel (LP false)
+// compiles to the code it has without the feature: the off path adds nothing to it, not even a test.
+template <int CW, bool INT8, bool PROF, bool LP>
+__device__ __forceinline__ void megakernel_body(const Params& P) {
   constexpr int CT = CW * 32;  // consumer threads
   uint64_t* full_bar = g_full_bar;
   uint64_t* empty_bar = g_empty_bar;
@@ -2196,7 +2302,7 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __gri
       if (stamp) stamp[0] = global_ns();
 
       if (ph.kind == kPhaseGather) {
-        if (!(tok < P.skip_cls_tokens)) gather_logits_phase<CW>(P, tok, pos);
+        if (!(tok < P.skip_cls_tokens)) gather_logits_phase<CW, LP>(P, tok, pos);
         if (stamp) stamp[1] = stamp[2] = global_ns();
       } else if (ph.kind != kPhaseGemv) {
         const int SP = P.attn_split;
@@ -2216,7 +2322,7 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __gri
         // A prompt token (llama3.cpp:733-745: predict(..., is_prompt = true) discards the logits and
         // returns -1) skips the classifier -- its weights are not even streamed -- but keeps the grid
         // barrier that closes the token.
-        const Carry out = gemv_phase<CW, INT8, PROF>(P, Carry{pipe, best.v, best.i}, tok, pos, emb_row, stamp);
+        const Carry out = gemv_phase<CW, INT8, PROF, LP>(P, Carry{pipe, best.v, best.i}, tok, pos, emb_row, stamp);
         pipe = out.pipe;
         best.v = out.best_v, best.i = out.best_i;
       }
@@ -2231,7 +2337,9 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __gri
     // semantics: maximum value, lowest index).  Sampling without top-k or top-p folds the same way: the
     // partials are then the perturbed maxima.  With either, every CTA draws the id itself. ---------------
     int next;
-    if (!(tok < P.skip_cls_tokens) && sampling::needs_draw(*P.sampling, P.vocab_size)) {
+    if (LP && !(tok < P.skip_cls_tokens)) {
+      next = draw_with_logprobs<CW>(P, pos, step);
+    } else if (!(tok < P.skip_cls_tokens) && sampling::needs_draw(*P.sampling, P.vocab_size)) {
       next = draw_truncated<CW>(P, pos);
     } else {
       ArgBest b{0.f, -1};
@@ -2284,6 +2392,16 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __gri
   }
 }
 
+template <int CW, bool INT8, bool PROF>
+__global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __grid_constant__ Params P) {
+  megakernel_body<CW, INT8, PROF, false>(P);
+}
+
+template <int CW, bool INT8>
+__global__ void __launch_bounds__(CW * 32 + 32, 1) logprob_megakernel(const __grid_constant__ Params P) {
+  megakernel_body<CW, INT8, false, true>(P);
+}
+
 }  // namespace mega
 
 // ================================== host side ======================================================
@@ -2296,6 +2414,10 @@ template <bool PROF>
 const void* kernel_for(bool int8) {
   if (int8) return reinterpret_cast<const void*>(mega::decode_megakernel<mega::kConsumerWarps, true, PROF>);
   return reinterpret_cast<const void*>(mega::decode_megakernel<mega::kConsumerWarps, false, PROF>);
+}
+const void* logprob_kernel_for(bool int8) {
+  if (int8) return reinterpret_cast<const void*>(mega::logprob_megakernel<mega::kConsumerWarps, true>);
+  return reinterpret_cast<const void*>(mega::logprob_megakernel<mega::kConsumerWarps, false>);
 }
 constexpr int kThreads = mega::kConsumerWarps * 32 + 32;  // the consumer warps and the ring producer
 }  // namespace
@@ -2339,6 +2461,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   int8_fast_ = (int8 && fast_) ? 1 : 0;
   kernel_ = kernel_for<false>(int8);
   kernel_prof_ = kernel_for<true>(int8);
+  kernel_lp_ = logprob_kernel_for(int8);
 
   // The residual exchange after o_proj and down_proj is tagged (under tensor parallelism it IS the
   // all-reduce), and so are the hand-offs q|k|v -> attention -> Wo and SwiGLU -> W2: the one grid
@@ -2366,6 +2489,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   }
   // the top-k / top-p draw's scratch after the classifier (draw_truncated): the histogram and at least 64 candidates
   xbuf = std::max(xbuf, sampling::kDrawScratchBase + 64 * 8);
+  // ... and the log-probabilities' (logprob_partial, logprob_record): the top-N select keeps one maximum per thread
+  xbuf = std::max(xbuf, sampling::logprob_scratch_bytes(mega::kConsumerWarps * 32));
   xbuf = (xbuf + 127) & ~127;
   const int xres = (dim * 4 + 127) & ~127;  // the CTA's copy of the residual stream
   const int budget = max_smem - xbuf - xres - 3584;  // static shared memory (1.1 KB) + slack
@@ -2620,7 +2745,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   if (cudaMalloc(&d_barrier_, 128) != cudaSuccess) return static_cast<int>(cudaErrorMemoryAllocation);
   cudaMemsetAsync(d_barrier_, 0, 128, stream);
   if (cudaMalloc(&d_arg_val_, sizeof(float) * grid_) != cudaSuccess ||
-      cudaMalloc(&d_arg_idx_, sizeof(int) * grid_) != cudaSuccess)
+      cudaMalloc(&d_arg_idx_, sizeof(int) * grid_) != cudaSuccess ||
+      cudaMalloc(&d_lp_, static_cast<size_t>(grid_) * (sizeof(float2) + 8 * sampling::kMaxTopLogprobs)) != cudaSuccess)
     return static_cast<int>(cudaErrorMemoryAllocation);
   cudaStreamSynchronize(stream);  // ph (host vector) must outlive the async copy
 
@@ -2629,6 +2755,12 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   if (e != cudaSuccess) return static_cast<int>(e);
   e = cudaFuncSetAttribute(kernel_prof_, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes_));
   if (e != cudaSuccess) return static_cast<int>(e);
+  e = cudaFuncSetAttribute(kernel_lp_, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes_));
+  if (e != cudaSuccess) return static_cast<int>(e);
+  int occ_lp = 0;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_lp, kernel_lp_, kThreads, smem_bytes_);
+  if (e != cudaSuccess) return static_cast<int>(e);
+  if (occ_lp < 1) return KLLM_E_UNSUPPORTED;
   int occ = 0;
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel_, kThreads, smem_bytes_);
   if (e != cudaSuccess) return static_cast<int>(e);
@@ -2643,6 +2775,8 @@ void MegaEngine::destroy() {
   if (d_barrier_) cudaFree(d_barrier_);
   if (d_arg_val_) cudaFree(d_arg_val_);
   if (d_arg_idx_) cudaFree(d_arg_idx_);
+  if (d_lp_) cudaFree(d_lp_);
+  d_lp_ = nullptr;
   if (d_tagged_) cudaFree(d_tagged_);
   if (d_handoff_) cudaFree(d_handoff_);
   if (d_scores_) cudaFree(d_scores_);
@@ -2715,12 +2849,20 @@ Params MegaEngine::params(int n_tokens, const int32_t* teacher_dev, unsigned lon
   P.prof = prof_dev;
   P.prof_token = prof_token;
   for (int i = 0; i < mega::kMaxStopIds; ++i) P.stop_ids[i] = -1;  // ids are >= 0: no stop
+  P.lp_top_n = lp_top_n_;
+  P.lp_target = 0;
+  P.lp_part = static_cast<float2*>(d_lp_);
+  P.lp_cand_v = reinterpret_cast<float*>(P.lp_part + grid_);
+  P.lp_cand_i = reinterpret_cast<int*>(P.lp_cand_v + static_cast<size_t>(grid_) * sampling::kMaxTopLogprobs);
+  P.lp_rec = m.lp_rec;
   return P;
 }
 
 int MegaEngine::launch(const Params& P) {
   void* args[] = {const_cast<Params*>(&P)};
-  cudaError_t e = cudaLaunchCooperativeKernel(const_cast<void*>(P.prof != nullptr ? kernel_prof_ : kernel_), dim3(grid_),
+  // the profiling instantiation records no log-probabilities; logprob_megakernel runs while they are on
+  const void* k = P.prof != nullptr ? kernel_prof_ : P.lp_top_n >= 0 ? kernel_lp_ : kernel_;
+  cudaError_t e = cudaLaunchCooperativeKernel(const_cast<void*>(k), dim3(grid_),
                                               dim3(kThreads), args, smem_bytes_, stream_);
   if (e != cudaSuccess) return static_cast<int>(e);
   count_launch();
@@ -2735,9 +2877,13 @@ void MegaEngine::account(int n_tokens) {
 }
 
 int MegaEngine::run(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
-                    int prof_token, int skip_cls_tokens) {
+                    int prof_token, int skip_cls_tokens, int lp_target) {
   if (!ready_) return KLLM_E_STATE;
-  const Params P = params(n_tokens, teacher_dev, prof_dev, prof_token, skip_cls_tokens);
+  Params P = params(n_tokens, teacher_dev, prof_dev, prof_token, skip_cls_tokens);
+  if (lp_target) {
+    P.lp_target = 1;
+    P.lp_top_n = std::max(lp_top_n_, 0);
+  }
   if (int rc = launch(P)) return rc;
   account(n_tokens);
   return 0;

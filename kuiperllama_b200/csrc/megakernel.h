@@ -141,6 +141,14 @@ struct Params {
   // entered / input staged / last stage consumed / grid barrier passed (globaltimer ns)
   unsigned long long* prof;
   int prof_token;
+  // Log-probabilities (sampling.cuh, DESIGN.md 5.8).  lp_top_n -1 is off; else each CTA leaves its part's (m_c, S_c)
+  // in lp_part and, for lp_top_n > 0, its top-N in lp_cand_v / lp_cand_i [grid][kMaxTopLogprobs]; CTA 0 folds them
+  // behind the token's grid barrier into the record.  lp_target 1: the entry's id is teacher[step + 1].
+  int lp_top_n, lp_target;
+  float2* lp_part;
+  float* lp_cand_v;
+  int* lp_cand_i;
+  sampling::LogprobRecord lp_rec;
 };
 
 }  // namespace mega
@@ -170,6 +178,7 @@ struct MegaModel {
   const SampleParams* sampling;
   int32_t* hist;
   float* penalized;
+  sampling::LogprobRecord lp_rec;
   // tensor parallel (tp_world > 1): exchange areas of every rank (kllm_comm, CUDA IPC)
   int tp_world, tp_rank;
   unsigned long long* tp_data[8];
@@ -182,8 +191,9 @@ class MegaEngine {
   int init(const MegaModel& m, cudaStream_t stream);
   void destroy();
   // Run n_tokens consecutive positions starting from the device-resident state.
+  // lp_target: kllm_decoder_score's run, whose record entries hold teacher[step + 1] (written even with logprobs off)
   int run(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev = nullptr,
-          int prof_token = -1, int skip_cls_tokens = 0);
+          int prof_token = -1, int skip_cls_tokens = 0, int lp_target = 0);
   // Up to n_tokens positions, ending after the first id in stop_ids[0 .. n_stop); every id is streamed to
   // stream_ids / stream_count (device-visible pointers into mapped host memory).  The number of positions
   // that ran is known only once the launch has finished, so the tag and barrier bases are NOT advanced
@@ -192,6 +202,8 @@ class MegaEngine {
   void account(int n_tokens);
   // the repetition penalty of later launches (kllm_decoder_set_repetition_penalty, after its stream synchronise)
   void set_penalty(const PenaltyParams& pp) { penalty_ = pp; }
+  // the logprob setting of later launches (kllm_decoder_set_logprobs, after its stream synchronise)
+  void set_logprobs(int top_n) { lp_top_n_ = top_n; }
   int grid() const { return grid_; }
   int phases() const { return n_phases_; }
   int attn_vsplit() const { return attn_vsplit_; }  // slices of the V cache layout
@@ -203,6 +215,8 @@ class MegaEngine {
   int launch(const mega::Params& P);
   MegaModel model_{};
   PenaltyParams penalty_{};
+  int lp_top_n_ = -1;
+  void* d_lp_ = nullptr;  // lp_part [grid] float2, then lp_cand_v / lp_cand_i [grid][kMaxTopLogprobs]
   cudaStream_t stream_ = nullptr;
   void* d_phases_ = nullptr;
   void* d_barrier_ = nullptr;
@@ -221,6 +235,7 @@ class MegaEngine {
   int cls_rows_ = 0, n_cls_phases_ = 1;
   const void* kernel_ = nullptr;       // decode_megakernel<8 consumer warps, int8, false>
   const void* kernel_prof_ = nullptr;  // ... <.., true>: records the phase timeline stamps
+  const void* kernel_lp_ = nullptr;    // logprob_megakernel<8 consumer warps, int8>: log-probabilities on
   size_t smem_bytes_ = 0;
   unsigned barrier_base_ = 0;
   bool ready_ = false;

@@ -563,5 +563,247 @@ __device__ __forceinline__ int draw_block(const float* logits, int n, const Samp
   return block_fold<NT>(bv, bi, s, sync);
 }
 
+// ---- log-probabilities (DESIGN.md 5.8) ------------------------------------------------------------------
+// Over the RAW logits l[0..V) of position pos (what kllm_decoder_logits returns: before step 0b, temperature,
+// top-k and top-p), for a partition of [0, V) into parts:
+//  L1. For each part c: m_c = max of its l_i; S_c = sum of expf(l_i - m_c) over its l_i, in fp32.
+//  L2. m = max over the parts of m_c; S = sum over c of S_c * expf(m_c - m), folded in part-index order;
+//      lse_off = logf(S).
+//  L3. lp_i = (l_i - m) - lse_off, two IEEE fp32 subtractions.
+//  Top-N: the N largest l_i in descending order, lowest index on ties (the greedy fold's order), each with its
+//  lp_i.  A selection has no rounding, so the ids are exact whatever the partition.
+// The same partition gives the same bits (every run, CTA and tensor-parallel rank); different partitions agree
+// within the bound of DESIGN.md 5.8.  Parts: a CTA's classifier rows (or its range of the tensor-parallel gather)
+// in the persistent engine, a warp's contiguous range in the one-block kernels.  Mirror: sampling.logprobs.
+constexpr int kMaxTopLogprobs = 20;  // == KLLM_MAX_TOP_LOGPROBS
+
+// Device-resident logprob setting of the graph engine (the persistent engine takes it in its launch parameters)
+struct LogprobParams {
+  int32_t top_n;      // -1: off; 0: the id's lp; 1..kMaxTopLogprobs: also the top-N
+  int32_t target;     // 1: the entry's id is teacher[step + 1] (kllm_decoder_score); 0: the drawn id
+  int32_t from_step;  // the steps before this one are prompt positions: they write no entry
+};
+
+// The decoder's record, indexed by position: id[pos], lp[pos], top_ids / top_lp [pos][kMaxTopLogprobs]
+struct LogprobRecord {
+  int32_t* id;
+  float* lp;
+  int32_t* top_ids;
+  float* top_lp;
+};
+
+struct Cand {
+  float v;
+  int i;  // < 0: no entry
+};
+
+// L3
+__device__ __forceinline__ float logprob(float l, float m, float lse_off) { return __fsub_rn(__fsub_rn(l, m), lse_off); }
+
+// Sum over a warp by a fixed butterfly: every lane ends with the same bits
+__device__ __forceinline__ float warp_sum_fixed(float v) {
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, off));
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, off));
+  return v;
+}
+
+// Shared memory of the logprob routines, in front of top_n_block's scratch
+struct LogprobScratch {
+  float part_m[32], part_s[32];  // per-warp partials
+  float m, lse_off;
+  float top_v[kMaxTopLogprobs];
+  int top_i[kMaxTopLogprobs];
+};
+constexpr int kLogprobScratchBase = static_cast<int>((sizeof(LogprobScratch) + 15) & ~size_t{15});
+// scratch bytes the logprob routines of a block of NT threads need (top_n_block keeps NT maxima)
+__host__ __device__ constexpr int logprob_scratch_bytes(int NT) { return kLogprobScratchBase + kDrawScratchBase + NT * 8; }
+
+// L1 of the part get(lo..hi) by one warp, in every lane: lane j takes i = lo + j (mod 32) in increasing order,
+// then the fixed butterfly
+template <class Get>
+__device__ __forceinline__ float2 warp_part(Get get, int lo, int hi) {
+  const int lane = threadIdx.x & 31;
+  float mx = -INFINITY;
+  for (int i = lo + lane; i < hi; i += 32) mx = fmaxf(mx, get(i));
+  mx = warp_max(mx);
+  float s = 0.f;
+  for (int i = lo + lane; i < hi; i += 32) s = __fadd_rn(s, expf(__fsub_rn(get(i), mx)));
+  return make_float2(mx, warp_sum_fixed(s));
+}
+
+// L1 of the part get(lo..hi) by a block of NT threads, returned in thread 0: thread t takes i = lo + t (mod NT) in
+// increasing order, the fixed butterfly per warp, then the warp sums in warp order
+template <int NT, class Get, class Sync>
+__device__ __forceinline__ float2 block_part(Get get, int lo, int hi, LogprobScratch& ls, Sync sync) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  float mx = -INFINITY;
+  for (int i = lo + tid; i < hi; i += NT) mx = fmaxf(mx, get(i));
+  mx = warp_max(mx);
+  if (lane == 0) ls.part_m[warp] = mx;
+  sync();
+  mx = -INFINITY;
+#pragma unroll
+  for (int w = 0; w < NT / 32; ++w) mx = fmaxf(mx, ls.part_m[w]);
+  float s = 0.f;
+  if (mx > -INFINITY)
+    for (int i = lo + tid; i < hi; i += NT) s = __fadd_rn(s, expf(__fsub_rn(get(i), mx)));
+  s = warp_sum_fixed(s);
+  if (lane == 0) ls.part_s[warp] = s;
+  sync();
+  s = 0.f;
+  if (tid == 0)
+    for (int w = 0; w < NT / 32; ++w) s = __fadd_rn(s, ls.part_s[w]);
+  return make_float2(mx, s);
+}
+
+// L2 over parts part(0..n_parts) -> (m, lse_off) in every lane of the calling warp.  Lane 0 folds in part order.
+template <class Part>
+__device__ __forceinline__ float2 warp_fold_parts(Part part, int n_parts) {
+  const int lane = threadIdx.x & 31;
+  float mx = -INFINITY;
+  for (int c = lane; c < n_parts; c += 32) mx = fmaxf(mx, part(c).x);
+  mx = warp_max(mx);
+  float s = 0.f;
+  if (lane == 0)
+    for (int c = 0; c < n_parts; ++c) {
+      const float2 p = part(c);
+      if (p.y > 0.f) s = __fadd_rn(s, __fmul_rn(p.y, expf(__fsub_rn(p.x, mx))));
+    }
+  return make_float2(mx, logf(__shfl_sync(0xffffffffu, s, 0)));
+}
+
+// Top-N of get(0..m) (get(k) -> Cand; entries with i < 0 are skipped) by one warp, written to out_v / out_i[0..N)
+// by lane 0; index -1 (lp -inf) pads a list with fewer than N entries.  Round r takes the best entry that ranks
+// after round r - 1's.
+template <class Get>
+__device__ __forceinline__ void warp_top_n(Get get, int m, int N, float* out_v, int* out_i) {
+  const int lane = threadIdx.x & 31;
+  float pv = 0.f;
+  int pi = -1;
+  bool more = true;
+  for (int r = 0; r < N; ++r) {
+    float bv = 0.f;
+    int bi = -1;
+    if (more)
+      for (int k = lane; k < m; k += 32) {
+        const Cand c = get(k);
+        if (c.i >= 0 && (r == 0 || c.v < pv || (c.v == pv && c.i > pi))) fold(bv, bi, c.v, c.i);
+      }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) fold(bv, bi, __shfl_xor_sync(0xffffffffu, bv, off), __shfl_xor_sync(0xffffffffu, bi, off));
+    if (lane == 0) {
+      out_v[r] = bi < 0 ? -INFINITY : bv;
+      out_i[r] = bi;
+    }
+    more = bi >= 0;
+    pv = bv;
+    pi = bi;
+  }
+}
+
+// Top-N of get(0..m) by a block of NT threads into out_v / out_i[0..N) (visible to the block on return).
+// scratch: logprob_scratch_bytes(NT) - kLogprobScratchBase bytes or more.  A lower bound tau of the N-th largest
+// value is the N-th largest of the NT per-thread maxima (N distinct entries reach it), so only the entries >= tau
+// become candidates; when they do not fit the scratch, the warp's rounds run over the whole list instead.
+template <int NT, class Get, class Sync>
+__device__ __forceinline__ void top_n_block(Get get, int m, int N, unsigned char* scratch, int scratch_bytes,
+                                            float* out_v, int* out_i, Sync sync) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  DrawScratch& s = *reinterpret_cast<DrawScratch*>(scratch);
+  const int cap = (scratch_bytes - kDrawScratchBase) / 8;
+  float* cv = reinterpret_cast<float*>(scratch + kDrawScratchBase);
+  int* ci = reinterpret_cast<int*>(cv + cap);
+  float bv = 0.f;
+  int bi = -1;
+  for (int k = tid; k < m; k += NT) {
+    const Cand c = get(k);
+    fold(bv, bi, c.v, c.i);
+  }
+  cv[tid] = bi < 0 ? -INFINITY : bv;
+  const int n_max = static_cast<int>(block_sum<NT>(bi >= 0 ? 1ull : 0ull, s, sync));  // (its barriers publish cv)
+  const float tau = N <= n_max ? kth_largest<NT>([&](int j) { return cv[j]; }, NT, N, s, sync) : -INFINITY;
+  if (tid == 0) s.count = 0u;
+  sync();
+  for (int k0 = 0; k0 < m; k0 += NT) {
+    const int k = k0 + tid;
+    Cand c{0.f, -1};
+    if (k < m) c = get(k);
+    const bool take = c.i >= 0 && c.v >= tau;
+    const unsigned ball = __ballot_sync(0xffffffffu, take);
+    if (ball == 0u) continue;
+    unsigned base = 0u;
+    if (lane == 0) base = atomicAdd(&s.count, static_cast<unsigned>(__popc(ball)));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    const int slot = static_cast<int>(base) + __popc(ball & ((1u << lane) - 1u));
+    if (take && slot < cap) {
+      cv[slot] = c.v;
+      ci[slot] = c.i;
+    }
+  }
+  sync();
+  const int nc = static_cast<int>(s.count);
+  if (tid < 32) {
+    if (nc <= cap)
+      warp_top_n([&](int k) { return Cand{cv[k], ci[k]}; }, nc, N, out_v, out_i);
+    else
+      warp_top_n(get, m, N, out_v, out_i);
+  }
+  sync();
+}
+
+// The record entry of one position (or the per-op outputs) by a block of NT threads, once m and lse_off are in
+// ls and the top-N in ls.top_v / top_i: lp of `id` (logit read from l), then the top-N with their lp.  id outside
+// [0, n): lp NaN.
+__device__ __forceinline__ void write_entry(const float* l, int n, int id, int N, const LogprobScratch& ls,
+                                            int32_t* out_id, float* out_lp, int32_t* top_ids, float* top_lp) {
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    if (out_id != nullptr) *out_id = id;
+    *out_lp = (id >= 0 && id < n) ? logprob(__ldcg(l + id), ls.m, ls.lse_off) : __int_as_float(0x7fffffff);
+  }
+  if (tid < N) {
+    const int i = ls.top_i[tid];
+    top_ids[tid] = i;
+    top_lp[tid] = i < 0 ? -INFINITY : logprob(ls.top_v[tid], ls.m, ls.lse_off);
+  }
+}
+
+// The logprob rule over l[0..n) by one block of NT threads (the graph engine's argmax_advance_kernel and
+// kllm_logprobs_f32): parts are the warps' contiguous ranges [w n / W, (w + 1) n / W).  Leaves m, lse_off and the
+// top-N in ls (visible to the block on return).  scratch: logprob_scratch_bytes(NT) bytes, ls at its front.
+template <int NT, class Sync>
+__device__ __forceinline__ void logprobs_block(const float* l, int n, int N, unsigned char* scratch, int scratch_bytes,
+                                               Sync sync) {
+  constexpr int W = NT / 32;
+  LogprobScratch& ls = *reinterpret_cast<LogprobScratch*>(scratch);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  sync();  // the scratch may still be read by a draw that just ended
+  auto get = [&](int i) { return __ldcg(l + i); };
+  const float2 p = warp_part(get, static_cast<int>(static_cast<long long>(warp) * n / W),
+                             static_cast<int>(static_cast<long long>(warp + 1) * n / W));
+  if (lane == 0) {
+    ls.part_m[warp] = p.x;
+    ls.part_s[warp] = p.y;
+  }
+  sync();
+  if (warp == 0) {
+    const float2 f = warp_fold_parts([&](int c) { return make_float2(ls.part_m[c], ls.part_s[c]); }, W);
+    if (lane == 0) {
+      ls.m = f.x;
+      ls.lse_off = f.y;
+    }
+  }
+  if (N > 0)
+    top_n_block<NT>([&](int k) { return Cand{__ldcg(l + k), k}; }, n, N, scratch + kLogprobScratchBase,
+                    scratch_bytes - kLogprobScratchBase, ls.top_v, ls.top_i, sync);
+  else
+    sync();
+}
+
 }  // namespace sampling
 }  // namespace kllm

@@ -186,6 +186,7 @@ class Decoder:
             d.comm = comm.handle
             self.comm = comm  # keep alive
         self.desc = d
+        self._top_n = -1  # kllm_decoder_set_logprobs's setting (a new decoder's is off)
         # local head geometry (head counts in `shape` are per-rank under tensor parallelism)
         self.head_size = d.dim // (s.head_num * max(tp_size, 1))
         self.local_kv_dim = s.kv_head_num * self.head_size
@@ -306,6 +307,40 @@ class Decoder:
         sampling.penalize mirrors it).  penalty 1 is off; the sampling settings are left alone."""
         check(self.lib.kllm_decoder_set_repetition_penalty(self.handle, float(penalty), int(last_n)),
               "kllm_decoder_set_repetition_penalty")
+
+    def set_logprobs(self, top_n: int):
+        """Record, at every position whose classifier runs, the returned id's log-probability over the raw logits and,
+        for top_n > 0, the top_n alternatives (kllm_decoder_set_logprobs; sampling.logprobs mirrors the rule).  -1 is
+        off.  Clears the record."""
+        check(self.lib.kllm_decoder_set_logprobs(self.handle, int(top_n)), "kllm_decoder_set_logprobs")
+        self._top_n = int(top_n)
+
+    def logprobs(self, start_pos: int, n: int):
+        """The record of positions [start_pos, start_pos + n) (kllm_decoder_read_logprobs): numpy (ids [n], lp [n],
+        top_ids [n, top_n], top_lp [n, top_n]); an id of -1 marks a position without an entry."""
+        import numpy as np
+        k = max(self._top_n, 0)
+        ids = np.empty(n, np.int32)
+        lp = np.empty(n, np.float32)
+        top_ids = np.empty((n, k), np.int32)
+        top_lp = np.empty((n, k), np.float32)
+        vp = ctypes.c_void_p
+        check(self.lib.kllm_decoder_read_logprobs(self.handle, int(start_pos), int(n), ids.ctypes.data_as(vp),
+                                                  lp.ctypes.data_as(vp), top_ids.ctypes.data_as(vp) if k else None,
+                                                  top_lp.ctypes.data_as(vp) if k else None),
+              "kllm_decoder_read_logprobs")
+        return ids, lp, top_ids, top_lp
+
+    def score(self, tokens, start_pos: int = 0):
+        """Teacher-forced log-likelihood (kllm_decoder_score): lp[i] = log p(tokens[i + 1] | tokens[:i + 1]) with
+        tokens[0] at start_pos, n - 1 values as numpy fp32.  The cache then holds those positions."""
+        import numpy as np
+        n = len(tokens)
+        arr = (ctypes.c_int32 * max(n, 1))(*[int(t) for t in tokens])
+        lp = np.empty(max(n - 1, 1), np.float32)
+        check(self.lib.kllm_decoder_score(self.handle, arr, n, int(start_pos), lp.ctypes.data_as(ctypes.c_void_p)),
+              "kllm_decoder_score")
+        return lp[:n - 1]
 
     def history(self):
         """The id fed at each position [seq_len], -1 where none was (kllm_decoder_read_history)."""

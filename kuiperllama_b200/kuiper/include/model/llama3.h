@@ -120,6 +120,19 @@ class LLama2Model : public Model {
   // position prompt.size() + ids.size() - 1 with ids.back() continues the same sequence.
   base::Status generate(const std::vector<int32_t>& prompt, int32_t max_new_tokens, std::vector<int32_t>& ids,
                         const std::function<void(const int32_t*, int32_t)>& on_tokens = {}) const;
+  // Log-probabilities of the returned ids (kllm_decoder_set_logprobs, DESIGN.md 5.8): call before init(), which
+  // refuses a value outside [-1, KLLM_MAX_TOP_LOGPROBS].  -1 (the default) is off; 0 records each returned id's
+  // log-probability over the raw logits, 1..20 also its top_n alternatives.  Entries are written by the fused
+  // paths (predict() on the fused decoder, generate()), at every position whose classifier runs.
+  void set_logprobs(int32_t top_n);
+  int32_t logprobs_top_n() const { return logprobs_top_n_; }
+  // The record of positions [first_pos, first_pos + n) (kllm_decoder_read_logprobs): ids (-1: no entry), lp, and
+  // top_ids / top_lp [n][logprobs_top_n()] (empty when it is <= 0).
+  base::Status logprobs(int32_t first_pos, int32_t n, std::vector<int32_t>& ids, std::vector<float>& lp,
+                        std::vector<int32_t>& top_ids, std::vector<float>& top_lp) const;
+  // Teacher-forced scoring from position 0 (kllm_decoder_score): lp[i] = log p(tokens[i + 1] | tokens[0..i]),
+  // tokens.size() - 1 values.  Afterwards the decoder holds positions 0 .. tokens.size() - 2.
+  base::Status score(const std::vector<int32_t>& tokens, std::vector<float>& lp) const;
   // Extra stop ids for generate(), e.g. for tokenizers that stop on nothing.
   void set_stop_ids(std::vector<int32_t> ids) { extra_stop_ids_ = std::move(ids); }
 
@@ -176,6 +189,7 @@ class LLama2Model : public Model {
   float penalty_ = 1.f;
   int32_t repeat_last_n_ = 0;
   bool penalty_explicit_ = false;
+  int32_t logprobs_top_n_ = -1;
   sampler::SeededSampler* seeded_ = nullptr;  // sampler_ when sampling, else null
   std::vector<int32_t> extra_stop_ids_;       // set_stop_ids()
   mutable uint64_t embedding_calls_ = 0;

@@ -95,6 +95,38 @@ void LLama2Model::set_repetition_penalty(float penalty, int32_t last_n) {
   penalty_explicit_ = true;
 }
 
+void LLama2Model::set_logprobs(int32_t top_n) { logprobs_top_n_ = top_n; }
+
+base::Status LLama2Model::logprobs(int32_t first_pos, int32_t n, std::vector<int32_t>& ids, std::vector<float>& lp,
+                                   std::vector<int32_t>& top_ids, std::vector<float>& top_lp) const {
+  if (decoder_ == nullptr) return base::error::InternalError("logprobs(): the fused decoder is not initialised");
+  if (first_pos < 0 || n < 0) return base::error::InvalidArgument("logprobs(): a range outside the context");
+  const size_t k = logprobs_top_n_ > 0 ? static_cast<size_t>(logprobs_top_n_) : 0;
+  ids.assign(n, -1);
+  lp.assign(n, 0.f);
+  top_ids.assign(k * n, -1);
+  top_lp.assign(k * n, 0.f);
+  const int rc = kllm_decoder_read_logprobs(decoder_, first_pos, n, ids.data(), lp.data(), k ? top_ids.data() : nullptr,
+                                            k ? top_lp.data() : nullptr);
+  if (rc != 0) return base::error::InvalidArgument(std::string("kllm_decoder_read_logprobs failed: ") + kllm_error_string(rc));
+  return base::error::Success();
+}
+
+base::Status LLama2Model::score(const std::vector<int32_t>& tokens, std::vector<float>& lp) const {
+  if (decoder_ == nullptr) return base::error::InternalError("score(): the fused decoder is not initialised");
+  const int32_t n = static_cast<int32_t>(tokens.size());
+  if (n < 2) return base::error::InvalidArgument("score(): needs at least two tokens");
+  lp.assign(n - 1, 0.f);
+  const int rc = kllm_decoder_score(decoder_, tokens.data(), n, 0, lp.data());
+  if (rc != 0) return base::error::InvalidArgument(std::string("kllm_decoder_score failed: ") + kllm_error_string(rc));
+  // the decoder now holds this sequence only (as after generate()): predict() continues at position n - 1
+  decoder_rows_ = n - 1;
+  layer_rows_ = 0;
+  prefilled_from_ = prefilled_to_ = 0;
+  logits_in_decoder_ = true;
+  return base::error::Success();
+}
+
 const char* LLama2Model::decoder_engine() const { return decoder_ ? kllm_decoder_engine(decoder_) : ""; }
 
 base::Status LLama2Model::init(base::DeviceType device_type) {
@@ -141,6 +173,8 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
     return error::InvalidArgument(
         "sampling: repetition_penalty must be finite and > 0, and its last_n >= 0 (KUIPER_REPETITION_PENALTY / "
         "KUIPER_REPEAT_LAST_N / set_repetition_penalty)");
+  if (logprobs_top_n_ < -1 || logprobs_top_n_ > KLLM_MAX_TOP_LOGPROBS)
+    return error::InvalidArgument("logprobs: top_n must be in [-1, 20] (set_logprobs)");
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
     return error::InternalError("No usable CUDA device " + std::to_string(tp_.cuda_device()) + ".");
   cuda_config_ = std::make_shared<kernel::CudaConfig>();
@@ -540,6 +574,12 @@ base::Status LLama2Model::create_decoder() {
       return base::error::InternalError(std::string("kllm_decoder_set_repetition_penalty failed: ") +
                                         kllm_error_string(prc));
     LOG(INFO) << "sampling: repetition_penalty " << penalty_ << ", last_n " << repeat_last_n_;
+  }
+  if (logprobs_top_n_ >= 0) {
+    const int lrc = kllm_decoder_set_logprobs(decoder_, logprobs_top_n_);
+    if (lrc != 0)
+      return base::error::InternalError(std::string("kllm_decoder_set_logprobs failed: ") + kllm_error_string(lrc));
+    LOG(INFO) << "logprobs: top_n " << logprobs_top_n_;
   }
   LOG(INFO) << "fused decoder engine: " << kllm_decoder_engine(decoder_) << ", "
             << kllm_decoder_launches_per_step(decoder_) << " launch(es) per token";

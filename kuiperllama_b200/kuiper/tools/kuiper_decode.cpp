@@ -3,7 +3,7 @@
 //
 //   kuiper_decode <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...]
 //                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P]
-//                 [--repetition-penalty P N] [--generate N [--stop ID]... [--then K]]
+//                 [--repetition-penalty P N] [--generate N [--stop ID]... [--then K]] [--logprobs N] [--score]
 //
 // --generate N runs the prompt and LLama2Model::generate() for at most N ids instead (n_steps is then unused),
 // stopping at the tokenizer's stop ids and every --stop ID, and prints the ids generate() returned, followed
@@ -19,11 +19,17 @@
 // LLama2Model::set_top_p(P) instead of KUIPER_TOP_P.  --repetition-penalty P N calls
 // LLama2Model::set_repetition_penalty(P, N) instead of KUIPER_REPETITION_PENALTY / KUIPER_REPEAT_LAST_N; --layers
 // applies the penalty itself, over the ids this tool fed, to the seeded draw and to its greedy argmax.
+// --logprobs N calls LLama2Model::set_logprobs(N) and, after the ids, prints one line per position that has a record
+// entry: "lp <pos> <id> <lp>" followed by N pairs "<top id> <top lp>" (%.9g: the fp32 values round-trip).
+// --score scores the given ids with LLama2Model::score() instead of decoding (n_steps is then unused): one line of
+// the n - 1 log-probabilities, then "perplexity <exp(-mean)>".  The layer path has neither: --layers with either is
+// refused.
 #include <base/base.h>
 #include <cuda_runtime_api.h>
 #include <glog/logging.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -59,6 +65,8 @@ int main(int argc, char** argv) {
   int32_t last_n = 0;
   int generate = 0, then = 0;
   std::vector<int32_t> stops;
+  int32_t logprobs = -1;
+  bool set_logprobs = false, score = false;
   for (int i = 5; i < argc; ++i) {
     if (!std::strcmp(argv[i], "--layers")) layers = true;
     else if (!std::strcmp(argv[i], "--sampling") && i + 3 < argc) {
@@ -80,10 +88,19 @@ int main(int argc, char** argv) {
     else if (!std::strcmp(argv[i], "--stop") && i + 1 < argc) stops.push_back(std::atoi(argv[++i]));
     else if (!std::strcmp(argv[i], "--then") && i + 1 < argc) then = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--copy-at") && i + 1 < argc) copy_at = std::atoi(argv[++i]);
+    else if (!std::strcmp(argv[i], "--logprobs") && i + 1 < argc) {
+      set_logprobs = true;
+      logprobs = std::atoi(argv[++i]);
+    }
+    else if (!std::strcmp(argv[i], "--score")) score = true;
     else if (!std::strcmp(argv[i], "--logits") && i + 1 < argc) logits_path = argv[++i];
     else prompt.push_back(std::atoi(argv[i]));
   }
   if (prompt.empty() || n_steps <= 0) return 2;
+  if (layers && (set_logprobs || score)) {
+    std::fprintf(stderr, "--layers has no log-probabilities: --logprobs and --score need the fused decoder\n");
+    return 2;
+  }
   const bool quant = prec == "int8";
 
   std::unique_ptr<model::LLama2Model> m;
@@ -96,12 +113,48 @@ int main(int argc, char** argv) {
   if (set_top_p) m->set_top_p(top_p);
   if (set_penalty) m->set_repetition_penalty(penalty, last_n);
   if (!stops.empty()) m->set_stop_ids(stops);
+  if (set_logprobs) m->set_logprobs(logprobs);  // init() refuses a value outside [-1, 20]
   base::Status st = m->init(base::DeviceType::kDeviceCUDA);
   if (!st) {
     std::fprintf(stderr, "init failed: %s\n", st.get_err_msg().c_str());
     return 1;
   }
   std::fprintf(stderr, "engine: %s%s\n", m->decoder_engine(), layers ? " (unused: --layers)" : "");
+
+  // the record entries of positions [0, n): one line each where there is one
+  auto print_logprobs = [&](int32_t n) {
+    if (logprobs < 0) return true;
+    std::vector<int32_t> ids, top_ids;
+    std::vector<float> lp, top_lp;
+    base::Status s = m->logprobs(0, n, ids, lp, top_ids, top_lp);
+    if (!s) {
+      std::fprintf(stderr, "logprobs failed: %s\n", s.get_err_msg().c_str());
+      return false;
+    }
+    const int32_t k = std::max(logprobs, 0);
+    for (int32_t p = 0; p < n; ++p) {
+      if (ids[p] < 0) continue;
+      std::printf("lp %d %d %.9g", p, ids[p], lp[p]);
+      for (int32_t r = 0; r < k; ++r) std::printf(" %d %.9g", top_ids[p * k + r], top_lp[p * k + r]);
+      std::printf("\n");
+    }
+    return true;
+  };
+  if (score) {
+    std::vector<float> lp;
+    st = m->score(std::vector<int32_t>(prompt.begin(), prompt.end()), lp);
+    if (!st) {
+      std::fprintf(stderr, "score failed: %s\n", st.get_err_msg().c_str());
+      return 1;
+    }
+    double sum = 0.0;
+    for (size_t i = 0; i < lp.size(); ++i) {
+      std::printf("%s%.9g", i ? " " : "", lp[i]);
+      sum += lp[i];
+    }
+    std::printf("\nperplexity %.9g\n", std::exp(-sum / static_cast<double>(lp.size())));
+    return print_logprobs(static_cast<int32_t>(prompt.size())) ? 0 : 1;
+  }
 
   tensor::Tensor pos_tensor = m->get_buffer(model::ModelBufferType::kInputPos);
   if (generate > 0) {
@@ -127,7 +180,7 @@ int main(int argc, char** argv) {
     }
     for (size_t i = 0; i < ids.size(); ++i) std::printf("%s%d", i ? " " : "", ids[i]);
     std::printf("\n");
-    return 0;
+    return print_logprobs(static_cast<int32_t>(prompt.size() + ids.size())) ? 0 : 1;
   }
   const int32_t prompt_len = static_cast<int32_t>(prompt.size());
   auto prompt_embedding = m->embedding(prompt);
@@ -206,6 +259,7 @@ int main(int argc, char** argv) {
   }
   for (size_t i = 0; i < chosen.size(); ++i) std::printf("%s%d", i ? " " : "", chosen[i]);
   std::printf("\n");
+  if (!print_logprobs(n_steps)) return 1;
   if (!logits_path.empty() && m->tensor_parallel().rank == 0) {  // under kuiper_tp_launch every rank holds the same logits
     tensor::Tensor lg = m->get_buffer(model::ModelBufferType::kForwardOutput).clone();
     lg.to_cpu();

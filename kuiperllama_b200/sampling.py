@@ -152,6 +152,80 @@ def nucleus_margin(logits, temperature: float, top_k: int, top_p: float) -> floa
     return min(gaps) / (z * 2.0 ** 24)
 
 
+MAX_TOP_LOGPROBS = 20
+
+
+def top_n(logits, n: int) -> np.ndarray:
+    """The n largest logits' ids in descending order, lowest index on ties (-1 pads past the vector's length)."""
+    v = np.asarray(logits, np.float32)
+    order = np.lexsort((np.arange(v.shape[0]), -v.astype(np.float64)))[:n]
+    return np.concatenate([order, -np.ones(max(0, n - v.shape[0]), np.int64)]).astype(np.int64)
+
+
+def warp_parts(n: int, w: int = 32):
+    """The partition of the one-block kernels: w contiguous ranges [j n / w, (j + 1) n / w)."""
+    return [(j * n // w, (j + 1) * n // w) for j in range(w)]
+
+
+def logprobs(logits, ids, top_n_: int = 0, parts=None):
+    """The logprob rule of csrc/sampling.cuh (DESIGN.md 5.8) over raw fp32 logits: (lp of each of `ids`, top-N ids,
+    top-N lp).  parts=None: exact fp64 log_softmax.  Otherwise L1-L3 emulated in fp32 over the given partition
+    (a list of (lo, hi) ranges), each part summed in increasing index order."""
+    l = np.asarray(logits, np.float32)
+    ids = np.asarray(ids, np.int64)
+    top = top_n(l, top_n_)
+    if parts is None:
+        l64 = l.astype(np.float64)
+        m = l64.max()
+        lse = m + np.log(np.exp(l64 - m).sum())
+        lp = lambda i: l64[i] - lse  # noqa: E731
+    else:
+        f = np.float32
+        ms, ss = [], []
+        for lo, hi in parts:
+            if hi <= lo:
+                ms.append(f(-np.inf)), ss.append(f(0))
+                continue
+            seg = l[lo:hi]
+            mc = seg.max()
+            # np.add.accumulate adds in order, one fp32 rounding per term (np.sum would add pairwise)
+            ms.append(mc), ss.append(np.add.accumulate(np.exp(seg - mc).astype(np.float32), dtype=np.float32)[-1])
+        m = max(ms)
+        S = f(0)
+        for mc, sc in zip(ms, ss):
+            if sc > 0:
+                S = f(S + f(sc * np.exp(f(mc - m))))
+        lse_off = np.log(S).astype(np.float32)
+        lp = lambda i: ((l[i] - m).astype(np.float32) - lse_off).astype(np.float32)  # noqa: E731
+    lp_ids = np.array([lp(i) if 0 <= i < l.shape[0] else np.nan for i in ids], np.float64)
+    lp_top = np.array([lp(i) if i >= 0 else -np.inf for i in top], np.float64)
+    return lp_ids, top, lp_top
+
+
+def logprob_bound(lp, chain: int, V: int) -> np.ndarray:
+    """|lp - lp_fp64| <= (k + 10) u + 5 u log V + 2 u |lp|, u = 2^-24, for a computation of S whose longest chain of
+    dependent fp32 additions is k (DESIGN.md 5.8 derives it)."""
+    u = 2.0 ** -24
+    return (chain + 10) * u + 5 * u * np.log(V) + 2 * u * np.abs(np.asarray(lp, np.float64))
+
+
+def chain_of_parts(parts) -> int:
+    """k of the emulation: a part summed in order, then the parts folded in order."""
+    return max(hi - lo for lo, hi in parts) + len(parts)
+
+
+def chain_persistent(V: int, grid: int, threads: int = 256) -> int:
+    """k of the persistent engine: a thread's strided rows, the warp butterfly, the warps in order, the CTAs in order."""
+    rows = -(-V // grid)
+    return -(-rows // threads) + 5 + threads // 32 + grid
+
+
+def chain_one_block(V: int) -> int:
+    """k of the one-block kernels (graph engine, kllm_logprobs_f32): a lane's strided share of its warp's range, the
+    butterfly, the 32 warps in order."""
+    return -(-(-(-V // 32)) // 32) + 5 + 32
+
+
 def margin(logits, temperature: float, top_k: int, seed: int, pos: int, top_p: float = 1.0) -> float:
     """Relative gap between the two best perturbed scores: below ~1e-5 a last-ulp difference of the
     device logf may change the id.  With top-p, 0 also when a nucleus comparison is within NUCLEUS_EPS
