@@ -124,6 +124,20 @@ int kllm_sample_top_p_f32(const float* logits, int64_t n, float temperature, int
  * n_ids < 0, or a penalty that is not finite or <= 0. */
 int kllm_repetition_penalty_f32(const float* logits, float* out, int64_t n, const int32_t* ids, int32_t n_ids,
                                 float penalty, void* stream);
+/* The whole of step 0 (DESIGN.md 5.9) over explicit id lists: out[0..n) = logits[0..n) (device) with, in order,
+ * the logit bias of the map bias_ids_host[k] -> bias_host[k], k < n_bias (HOST arrays: the map is validated here;
+ * n_bias == 0 skips the step), the repetition penalty over rep_ids[0..n_rep) (device, as
+ * kllm_repetition_penalty_f32), then l_i - frequency * c_i and l_i - presence for every i with c_i > 0
+ * occurrences in count_ids[0..n_count) (device).  Ids outside [0, n) in rep_ids / count_ids are ignored.  With
+ * n_bias == 0 and frequency == presence == 0 it equals kllm_repetition_penalty_f32 bit for bit.  Enqueued on
+ * `stream` with a stream-ordered scratch [n] (two with a bias); staging the bias table synchronises the stream.
+ * KLLM_E_INVALID for NULL pointers where the count is > 0, out == logits, n outside [1, 2^31), a negative count
+ * or n_count >= 2^30, a penalty that is not finite or <= 0, an alpha that is not finite, and a bias id outside
+ * [0, n), a repeated bias id or a bias that is not finite. */
+int kllm_logit_penalties_f32(const float* logits, float* out, int64_t n, const int32_t* bias_ids_host,
+                             const float* bias_host, int32_t n_bias, float penalty, const int32_t* rep_ids,
+                             int32_t n_rep, float frequency, float presence, const int32_t* count_ids,
+                             int32_t n_count, void* stream);
 /* Log-probabilities of logits[0..n) (device) by the rule of DESIGN.md 5.8: out_lp[j] = log softmax(logits)[ids[j]]
  * for j < n_ids, NaN for an id outside [0, n); out_top_ids / out_top_lp[0..top_n) = the top_n largest logits in
  * descending order, lowest index on ties, with their log-probabilities (index -1, lp -inf past the n-th).  All
@@ -364,6 +378,23 @@ int kllm_decoder_set_sampling_top_p(kllm_decoder* dec, float temperature, int32_
  * kllm_decoder_logits keeps returning the raw logits.  Synchronises the decoder's stream.  KLLM_E_INVALID,
  * with the settings in force left unchanged, for a penalty that is not finite or <= 0 and for last_n < 0. */
 int kllm_decoder_set_repetition_penalty(kllm_decoder* dec, float penalty, int32_t last_n);
+/* Frequency and presence penalties before the draw (DESIGN.md 5.9, OpenAI's frequency_penalty /
+ * presence_penalty), from this call on, in every entry that kllm_decoder_set_sampling covers, on either engine and
+ * every tensor-parallel rank: with c_i the number of times id i was fed at positions [from_pos, pos] (the
+ * decoder's history), every i with c_i > 0 gets l_i - frequency * c_i, then l_i - presence, after the repetition
+ * penalty.  from_pos is absolute: the prompt's length counts only the generated ids (the draw after the prompt
+ * counts none), 0 the prompt too.  frequency == presence == 0 is off (a new decoder's setting).  Negative values
+ * raise the counted ids.  Independent of the other setters.  kllm_decoder_logits keeps returning the raw logits
+ * and kllm_decoder_score ignores it.  Synchronises the decoder's stream.  KLLM_E_INVALID, with the settings in
+ * force left unchanged, for a value that is not finite and for from_pos < 0. */
+int kllm_decoder_set_frequency_presence(kllm_decoder* dec, float frequency, float presence, int32_t from_pos);
+/* Logit bias before the draw (DESIGN.md 5.9, OpenAI's logit_bias), from this call on, in the same entries:
+ * l_i + bias of i, before the penalties, for every id of the map ids_host[k] -> bias_host[k], k < n (host
+ * arrays).  Each call replaces the whole map; n == 0 clears it (a new decoder's setting).  A large negative bias
+ * bans an id, a large positive one forces it.  Independent of the other setters.  Synchronises the decoder's
+ * stream.  KLLM_E_INVALID, with the map in force left unchanged, for NULL arrays with n > 0, n < 0, an id
+ * outside [0, vocab_size), a repeated id, or a bias that is not finite. */
+int kllm_decoder_set_logit_bias(kllm_decoder* dec, const int32_t* ids_host, const float* bias_host, int32_t n);
 /* Log-probabilities of the returned ids, from this call on (DESIGN.md 5.8): whenever a position's classifier runs,
  * the decoder records, at that position, the id it returns with its log-probability and, for top_n > 0, the
  * top_n largest logits with theirs.  Log-probabilities are taken over the RAW logits (kllm_decoder_logits),

@@ -89,6 +89,8 @@ _SIGNATURES = {
     "kllm_sample_top_p_f32": (c_int, [c_void_p, c_int64, c_float, c_int32, c_float, c_uint64, c_int32, c_void_p,
                                       c_void_p]),
     "kllm_repetition_penalty_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int32, c_float, c_void_p]),
+    "kllm_logit_penalties_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int32, c_float, c_void_p,
+                                         c_int32, c_float, c_float, c_void_p, c_int32, c_void_p]),
     "kllm_logprobs_f32": (c_int, [c_void_p, c_int64, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
                                   c_void_p]),
     "kllm_gemv_fused": (c_int, [POINTER(GemvJob), c_void_p]),
@@ -115,6 +117,8 @@ _SIGNATURES = {
     "kllm_decoder_set_sampling": (c_int, [c_void_p, c_float, c_int32, c_uint64]),
     "kllm_decoder_set_sampling_top_p": (c_int, [c_void_p, c_float, c_int32, c_float, c_uint64]),
     "kllm_decoder_set_repetition_penalty": (c_int, [c_void_p, c_float, c_int32]),
+    "kllm_decoder_set_frequency_presence": (c_int, [c_void_p, c_float, c_float, c_int32]),
+    "kllm_decoder_set_logit_bias": (c_int, [c_void_p, c_void_p, c_void_p, c_int32]),
     "kllm_decoder_read_history": (c_int, [c_void_p, c_void_p]),
     "kllm_decoder_set_logprobs": (c_int, [c_void_p, c_int32]),
     "kllm_decoder_read_logprobs": (c_int, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),

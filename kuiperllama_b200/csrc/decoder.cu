@@ -59,8 +59,9 @@ __global__ void embed_token_kernel(const StepState* st, const float* __restrict_
 // the id, feed it (or the teacher's id) to the next step, pos += 1.
 // With stream_ids (kllm_decoder_generate_until's graph only) the id is also published to mapped host memory:
 // the id, then the count with release semantics at system scope, which the host polls.
-// With the repetition penalty on (read from device memory, so the captured graphs stay valid), the block first
-// writes the penalised logits to `penalized` and draws from those; the raw logits are left as they are.
+// With step 0 on -- the repetition, frequency or presence penalty or a logit bias, read from device memory, so
+// the captured graphs stay valid -- the block first writes the adjusted logits to `penalized` and draws from
+// those; the raw logits are left as they are.
 // With logprobs on (also read from device memory), the block then writes the record entry of the position from the
 // raw logits (sampling.cuh, DESIGN.md 5.8): of the drawn id, or of targets[step + 1] when scoring.
 constexpr int kDrawScratchBytes = sampling::kDrawScratchBase + 2048 * 8;
@@ -76,9 +77,8 @@ argmax_advance_kernel(const float* __restrict__ logits, int n, const SampleParam
   const int step0 = st->step;  // read by every thread before thread 0 advances the state
   const float* l = logits;
   const PenaltyParams pen = *pp;
-  if (sampling::penalty_active(pen)) {
-    sampling::penalize_rows<1024>(logits, penalized, 0, n, hist, sampling::window_lo(pen, pos), pos, pen.penalty,
-                                  [] { __syncthreads(); });
+  if (sampling::step0_active(pen)) {
+    sampling::step0_history<1024>(logits, penalized, 0, n, pen, hist, pos, [] { __syncthreads(); });
     l = penalized;
   }
   const int bi = sampling::draw_block<1024>(l, n, *sp, pos, nullptr, nullptr, 0, scratch, kDrawScratchBytes,
@@ -126,9 +126,12 @@ struct kllm_decoder {
   bool use_mega = false;
   StepState* st = nullptr;
   SampleParams* sampling = nullptr;  // device; zero = greedy (kllm_decoder_set_sampling)
-  PenaltyParams* penalty = nullptr;  // device; zero = off (kllm_decoder_set_repetition_penalty)
+  PenaltyParams* penalty = nullptr;  // device; zero = off (the step 0 setters)
+  PenaltyParams pen{};               // the settings in force, of which `penalty` is the device copy
   int32_t* hist = nullptr;           // device [seq_len]: the id fed at each position, -1 for none
   float* penalized = nullptr;        // device [vocab]: the penalised logits of the last draw
+  float* bias = nullptr;             // device [vocab]: the dense logit bias table (kllm_decoder_set_logit_bias)
+  int32_t* marks = nullptr;          // device [vocab]: step 0's mark words, zero between tokens
   int32_t* out_tokens = nullptr;  // device [seq_len]
   int32_t* teacher = nullptr;     // device [seq_len]
   StepState* st_host = nullptr;   // pinned
@@ -479,12 +482,14 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
       dev_alloc(&dc->kcache, kv_elems) || dev_alloc(&dc->vcache, kv_elems) ||
       dev_alloc(&dc->sin_t, static_cast<size_t>(d.seq_len) * dc->head_size) ||
       dev_alloc(&dc->cos_t, static_cast<size_t>(d.seq_len) * dc->head_size) ||
-      dev_alloc(&dc->tp_tmp, d.dim) || dev_alloc(&dc->penalized, d.vocab_size))
+      dev_alloc(&dc->tp_tmp, d.dim) || dev_alloc(&dc->penalized, d.vocab_size) ||
+      dev_alloc(&dc->bias, d.vocab_size))
     return fail(static_cast<int>(cudaErrorMemoryAllocation));
   if (cudaMalloc(&dc->st, sizeof(StepState)) != cudaSuccess ||
       cudaMalloc(&dc->sampling, sizeof(SampleParams)) != cudaSuccess ||
       cudaMalloc(&dc->penalty, sizeof(PenaltyParams)) != cudaSuccess ||
       cudaMalloc(&dc->hist, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
+      cudaMalloc(&dc->marks, sizeof(int32_t) * d.vocab_size) != cudaSuccess ||
       cudaMalloc(&dc->out_tokens, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMalloc(&dc->teacher, sizeof(int32_t) * d.seq_len) != cudaSuccess ||
       cudaMallocHost(&dc->st_host, sizeof(StepState)) != cudaSuccess ||
@@ -503,6 +508,8 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
   cudaMemsetAsync(dc->sampling, 0, sizeof(SampleParams), dc->stream);
   cudaMemsetAsync(dc->penalty, 0, sizeof(PenaltyParams), dc->stream);
   cudaMemsetAsync(dc->hist, 0xff, sizeof(int32_t) * d.seq_len, dc->stream);  // -1: no id
+  cudaMemsetAsync(dc->marks, 0, sizeof(int32_t) * d.vocab_size, dc->stream);
+  dc->pen.marks = dc->marks;  // off until a setter turns a sub-step on
   dc->lp_host[0] = sampling::LogprobParams{-1, 0, 0};  // off
   cudaMemcpyAsync(dc->lp_params, dc->lp_host, sizeof(sampling::LogprobParams), cudaMemcpyHostToDevice, dc->stream);
   cudaMemsetAsync(dc->rec.id, 0xff, sizeof(int32_t) * d.seq_len, dc->stream);
@@ -584,13 +591,14 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->exec_until) cudaGraphExecDestroy(dc->exec_until);
   if (dc->graph_until) cudaGraphDestroy(dc->graph_until);
   float* bufs[] = {dc->x, dc->q, dc->attn, dc->h, dc->logits, dc->score,
-                   dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->penalized};
+                   dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->penalized, dc->bias};
   for (float* b : bufs)
     if (b) cudaFree(b);
   if (dc->st) cudaFree(dc->st);
   if (dc->sampling) cudaFree(dc->sampling);
   if (dc->penalty) cudaFree(dc->penalty);
   if (dc->hist) cudaFree(dc->hist);
+  if (dc->marks) cudaFree(dc->marks);
   if (dc->out_tokens) cudaFree(dc->out_tokens);
   if (dc->teacher) cudaFree(dc->teacher);
   if (dc->pf_buf) cudaFree(dc->pf_buf);
@@ -795,14 +803,55 @@ int kllm_decoder_set_sampling_top_p(kllm_decoder* dc, float temperature, int32_t
   return static_cast<int>(cudaStreamSynchronize(dc->stream));
 }
 
-int kllm_decoder_set_repetition_penalty(kllm_decoder* dc, float penalty, int32_t last_n) {
-  if (!dc || !std::isfinite(penalty) || !(penalty > 0.f) || last_n < 0) return KLLM_E_INVALID;
-  const PenaltyParams pp{penalty, last_n};
-  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+namespace {
+// The step 0 settings `pp` in force from the next entry on; the caller has synchronised the stream
+int put_penalty(kllm_decoder* dc, PenaltyParams pp) {
+  sampling::step0_finish(pp);
   KLLM_TRY(cudaMemcpyAsync(dc->penalty, &pp, sizeof(pp), cudaMemcpyHostToDevice, dc->stream));
   KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  dc->pen = pp;
   if (dc->use_mega) dc->mega.set_penalty(pp);  // the megakernel takes it in its launch parameters
   return 0;
+}
+}  // namespace
+
+int kllm_decoder_set_repetition_penalty(kllm_decoder* dc, float penalty, int32_t last_n) {
+  if (!dc || !std::isfinite(penalty) || !(penalty > 0.f) || last_n < 0) return KLLM_E_INVALID;
+  PenaltyParams pp = dc->pen;
+  pp.penalty = penalty, pp.last_n = last_n;
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  return put_penalty(dc, pp);
+}
+
+int kllm_decoder_set_frequency_presence(kllm_decoder* dc, float frequency, float presence, int32_t from_pos) {
+  if (!dc || !std::isfinite(frequency) || !std::isfinite(presence) || from_pos < 0) return KLLM_E_INVALID;
+  PenaltyParams pp = dc->pen;
+  pp.frequency = frequency == 0.f ? 0.f : frequency;  // -0.0 is off, as 0
+  pp.presence = presence == 0.f ? 0.f : presence;
+  pp.from_pos = from_pos;
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  return put_penalty(dc, pp);
+}
+
+int kllm_decoder_set_logit_bias(kllm_decoder* dc, const int32_t* ids_host, const float* bias_host, int32_t n) {
+  if (!dc || n < 0 || (n > 0 && (!ids_host || !bias_host))) return KLLM_E_INVALID;
+  const int V = dc->d.vocab_size;
+  std::vector<float> table;
+  if (n > 0) {
+    std::vector<char> seen(V, 0);
+    table.assign(V, 0.f);
+    for (int32_t k = 0; k < n; ++k) {
+      const int32_t id = ids_host[k];
+      if (id < 0 || id >= V || seen[id] || !std::isfinite(bias_host[k])) return KLLM_E_INVALID;
+      seen[id] = 1;
+      table[id] = 0.f + bias_host[k];  // HF's table: 0 + b, so a -0.0 bias adds +0.0
+    }
+  }
+  PenaltyParams pp = dc->pen;
+  pp.bias = n > 0 ? dc->bias : nullptr;
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  if (n > 0) KLLM_TRY(cudaMemcpy(dc->bias, table.data(), sizeof(float) * V, cudaMemcpyHostToDevice));
+  return put_penalty(dc, pp);
 }
 
 int kllm_decoder_set_logprobs(kllm_decoder* dc, int32_t top_n) {

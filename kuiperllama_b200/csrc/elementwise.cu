@@ -10,6 +10,7 @@
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
+#include <vector>
 
 #include "../../include/kllm_b200.h"
 #include "kllm_device.cuh"
@@ -277,6 +278,16 @@ __global__ void penalize_ids_kernel(const float* __restrict__ logits, float* __r
   if (id >= 0 && id < n) out[id] = sampling::penalize(logits[id], penalty);
 }
 
+// kllm_logit_penalties_f32: step 0 of sampling.cuh over explicit id lists, block b over its own range of rows
+__global__ void __launch_bounds__(256) logit_penalties_kernel(const float* __restrict__ logits, float* out, int n,
+                                                              PenaltyParams pp, const int32_t* rep_ids, int n_rep,
+                                                              const int32_t* count_ids, int n_count) {
+  const int lo = static_cast<int>(static_cast<int64_t>(blockIdx.x) * n / gridDim.x);
+  const int hi = static_cast<int>(static_cast<int64_t>(blockIdx.x + 1) * n / gridDim.x);
+  sampling::step0_rows<256>(logits, out, lo, hi, pp, sampling::IdRange{rep_ids, 0, n_rep},
+                            sampling::IdRange{count_ids, 0, n_count}, [] { __syncthreads(); });
+}
+
 // kllm_logprobs_f32: the logprob rule of sampling.cuh over one block (the graph engine's partition), then lp of
 // every listed id
 __global__ void __launch_bounds__(1024) logprobs_kernel(const float* __restrict__ logits, int n,
@@ -423,6 +434,54 @@ int kllm_repetition_penalty_f32(const float* logits, float* out, int64_t n, cons
     count_launch();
   }
   return static_cast<int>(cudaGetLastError());
+}
+
+int kllm_logit_penalties_f32(const float* logits, float* out, int64_t n, const int32_t* bias_ids_host,
+                             const float* bias_host, int32_t n_bias, float penalty, const int32_t* rep_ids,
+                             int32_t n_rep, float frequency, float presence, const int32_t* count_ids,
+                             int32_t n_count, void* stream) {
+  if (!logits || !out || out == logits || n <= 0 || n > 0x7fffffffLL || n_bias < 0 || n_rep < 0 || n_count < 0 ||
+      n_count >= sampling::kInHistory || (n_bias > 0 && (!bias_ids_host || !bias_host)) || (n_rep > 0 && !rep_ids) ||
+      (n_count > 0 && !count_ids))
+    return KLLM_E_INVALID;
+  if (!std::isfinite(penalty) || !(penalty > 0.f) || !std::isfinite(frequency) || !std::isfinite(presence))
+    return KLLM_E_INVALID;
+  const int m = static_cast<int>(n);
+  std::vector<float> table;
+  if (n_bias > 0) {
+    std::vector<char> seen(m, 0);
+    table.assign(m, 0.f);
+    for (int32_t k = 0; k < n_bias; ++k) {
+      const int32_t id = bias_ids_host[k];
+      if (id < 0 || id >= m || seen[id] || !std::isfinite(bias_host[k])) return KLLM_E_INVALID;
+      seen[id] = 1;
+      table[id] = 0.f + bias_host[k];  // HF's table: 0 + b
+    }
+  }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // scratch: the mark words [n] (zeroed), then the dense bias table [n]
+  int32_t* marks = nullptr;
+  const size_t bytes = sizeof(int32_t) * m + (n_bias > 0 ? sizeof(float) * m : 0);
+  if (cudaMallocAsync(reinterpret_cast<void**>(&marks), bytes, s) != cudaSuccess) return KLLM_E_NODEVICE;
+  float* bias = n_bias > 0 ? reinterpret_cast<float*>(marks + m) : nullptr;
+  int rc = static_cast<int>(cudaMemsetAsync(marks, 0, sizeof(int32_t) * m, s));
+  // from pageable memory: returns once the table is staged, so `table` may go out of scope
+  if (rc == 0 && bias) rc = static_cast<int>(cudaMemcpyAsync(bias, table.data(), sizeof(float) * m,
+                                                             cudaMemcpyHostToDevice, s));
+  if (rc == 0) {
+    PenaltyParams pp{};
+    pp.penalty = penalty, pp.frequency = frequency == 0.f ? 0.f : frequency;
+    pp.presence = presence == 0.f ? 0.f : presence;
+    pp.bias = bias, pp.marks = marks;
+    const int rep_n = sampling::penalty_active(pp) ? n_rep : 0;
+    const int cnt_n = sampling::counts_active(pp) ? n_count : 0;
+    logit_penalties_kernel<<<std::max(1, std::min(64, (m + 4095) / 4096)), 256, 0, s>>>(logits, out, m, pp, rep_ids,
+                                                                                        rep_n, count_ids, cnt_n);
+    count_launch();
+    rc = static_cast<int>(cudaGetLastError());
+  }
+  const int frc = static_cast<int>(cudaFreeAsync(marks, s));
+  return rc != 0 ? rc : frc;
 }
 
 int kllm_logprobs_f32(const float* logits, int64_t n, const int32_t* ids, int32_t n_ids, int32_t top_n, float* out_lp,

@@ -1579,10 +1579,10 @@ __device__ __noinline__ void logprob_record(const Params& P, int pos, int id) {
   sync();
 }
 
-// ---- repetition penalty over this CTA's classifier rows ---------------------------------------------
-// Step 0b of the rule for the rows [u0, u1) this CTA produced (their raw logits, stored by its own
-// threads): the penalised rows go to P.penalized, and the CTA's partial -- greedy, or perturbed as in the
-// perturb_only path -- is folded over them.  draw_truncated reads P.penalized, and the partials stay a
+// ---- step 0 (bias and penalties) over this CTA's classifier rows ---------------------------------------
+// Step 0 of the rule for the rows [u0, u1) this CTA produced (their raw logits, stored by its own
+// threads): the adjusted rows go to P.penalized, and the CTA's partial -- greedy, or perturbed as in the
+// perturb_only path -- is folded over them.  The rows' mark words in P.penalty.marks are this CTA's alone.  draw_truncated reads P.penalized, and the partials stay a
 // lower bound of its top-k threshold because they are maxima of the penalised vector.  Each consumer
 // thread t reads only the history entries j = t (mod CT), the ones it wrote itself in this launch (the
 // token loop) or that an earlier launch wrote, so no hand-off is needed (DESIGN.md 5.7).
@@ -1590,10 +1590,8 @@ template <int CW>
 __device__ __noinline__ ArgBest penalized_partial(const Params& P, const float* logits, int u0, int u1, int pos) {
   constexpr int CT = CW * 32;
   const SampleParams sp = *P.sampling;
-  const PenaltyParams pp = P.penalty;
   consumer_sync<CT>();  // the raw rows of every warp of the CTA are stored
-  sampling::penalize_rows<CT>(logits, P.penalized, u0, u1, P.hist, sampling::window_lo(pp, pos), pos, pp.penalty,
-                              [] { consumer_sync<CT>(); });
+  sampling::step0_history<CT>(logits, P.penalized, u0, u1, P.penalty, P.hist, pos, [] { consumer_sync<CT>(); });
   const bool perturb = sampling::perturb_only(sp, P.vocab_size);
   const uint2 key = sampling::seed_key(sp.seed);
   ArgBest b{0.f, -1};
@@ -1606,12 +1604,12 @@ __device__ __noinline__ ArgBest penalized_partial(const Params& P, const float* 
 
 // ---- the classifier rows of this CTA in logprob_megakernel --------------------------------------------
 // The log-probability partials of the raw rows [u0, u1) (logprob_partial), then the CTA's partial of the draw:
-// penalized_partial's with the penalty on, else the greedy or perturbed fold over the raw rows.
+// penalized_partial's with step 0 on, else the greedy or perturbed fold over the raw rows.
 template <int CW>
 __device__ __noinline__ ArgBest classifier_partial(const Params& P, const float* logits, int u0, int u1, int pos) {
   constexpr int CT = CW * 32;
   if (P.lp_top_n >= 0) logprob_partial<CW>(P, logits, u0, u1);
-  if (sampling::penalty_active(P.penalty)) return penalized_partial<CW>(P, logits, u0, u1, pos);
+  if (sampling::step0_active(P.penalty)) return penalized_partial<CW>(P, logits, u0, u1, pos);
   consumer_sync<CT>();  // the raw rows of every warp of the CTA are stored
   const SampleParams sp = *P.sampling;
   const bool perturb = sampling::perturb_only(sp, P.vocab_size);
@@ -1919,7 +1917,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
     // that ran epilogues hold partial bests
     ArgBest wb = best;
     const SampleParams sp = *P.sampling;
-    if (sampling::penalty_active(P.penalty) || (LP && P.lp_top_n >= 0)) {
+    if (sampling::step0_active(P.penalty) || (LP && P.lp_top_n >= 0)) {
       if constexpr (LP) wb = classifier_partial<CW>(P, ph.seg[0].out, u0, u1, pos);
       else wb = penalized_partial<CW>(P, ph.seg[0].out, u0, u1, pos);
     } else if (sampling::perturb_only(sp, P.vocab_size)) {
@@ -1982,8 +1980,8 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int p
   float* logits = ph.seg[0].out;
   const SampleParams sp = *P.sampling;
   const bool perturb = sampling::perturb_only(sp, V);  // as the classifier partials (gemv_phase)
-  // with the penalty or the log-probabilities on, the partial is folded afterwards (classifier_partial)
-  const bool penalized = sampling::penalty_active(P.penalty) || (LP && P.lp_top_n >= 0);
+  // with step 0 or the log-probabilities on, the partial is folded afterwards (classifier_partial)
+  const bool penalized = sampling::step0_active(P.penalty) || (LP && P.lp_top_n >= 0);
   const uint2 key = sampling::seed_key(sp.seed);
   ArgBest best{0.f, -1};
   for (int i = u0 + tid; i < u1; i += CT) {
@@ -2023,11 +2021,11 @@ __device__ __noinline__ void gather_logits_phase(const Params& P, int tok, int p
 // maximum from them.  The scratch is the input-vector
 // buffer: it is idle from the classifier's last read of its input until the next token stages its first
 // vector.  The barrier after the draw orders every thread's read of the result
-// before any thread writes that buffer again.  With the repetition penalty on, the draw reads the penalised
-// vector, which is complete behind the same barrier (classifier_partial).
+// before any thread writes that buffer again.  With step 0 on, the draw reads the adjusted vector, which is
+// complete behind the same barrier (classifier_partial).
 template <int CW>
 __device__ __noinline__ int draw_truncated(const Params& P, int pos) {
-  const float* l = sampling::penalty_active(P.penalty) ? P.penalized : P.logits;
+  const float* l = sampling::step0_active(P.penalty) ? P.penalized : P.logits;
   const int id = sampling::draw_block<CW * 32>(l, P.vocab_size, *P.sampling, pos, P.arg_val, P.arg_idx,
                                                static_cast<int>(gridDim.x), smem, P.xbuf_bytes,
                                                [] { consumer_sync<CW * 32>(); });

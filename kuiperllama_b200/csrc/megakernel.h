@@ -125,9 +125,10 @@ struct Params {
   int* arg_idx;
   const SampleParams* sampling;  // read when a token's id is drawn: changing it needs no new engine
   const float* logits;           // [vocab]: complete once the classifier's grid barrier is passed
-  // Repetition penalty (sampling.cuh step 0b): the settings of this launch (a copy of the decoder's, which change
-  // only between launches), hist[seq_len] the id fed at each position, penalized[vocab] the penalised logits,
-  // complete behind the same barrier as `logits` when the penalty is on.
+  // Step 0 of the rule (sampling.cuh: logit bias, repetition, frequency and presence penalties): the settings of
+  // this launch (a copy of the decoder's, which change only between launches, with its bias table and mark words),
+  // hist[seq_len] the id fed at each position, penalized[vocab] the adjusted logits, complete behind the same
+  // barrier as `logits` when step 0 is on.
   PenaltyParams penalty;
   int32_t* hist;
   float* penalized;
@@ -200,7 +201,7 @@ class MegaEngine {
   // here: the caller passes that number (state.step) to account() before the next launch.
   int run_until(int n_tokens, const int32_t* stop_ids, int n_stop, int32_t* stream_ids, int32_t* stream_count);
   void account(int n_tokens);
-  // the repetition penalty of later launches (kllm_decoder_set_repetition_penalty, after its stream synchronise)
+  // the step 0 settings of later launches (the decoder's setters, after their stream synchronise)
   void set_penalty(const PenaltyParams& pp) { penalty_ = pp; }
   // the logprob setting of later launches (kllm_decoder_set_logprobs, after its stream synchronise)
   void set_logprobs(int top_n) { lp_top_n_ = top_n; }

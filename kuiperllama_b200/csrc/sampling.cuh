@@ -10,8 +10,17 @@
 //      fed an id outside [0, V), holds none.  Feeding a position again overwrites it.
 //  0b. Repetition penalty (HF's RepetitionPenaltyLogitsProcessor): for i in H(pos),
 //      l'_i = l_i < 0 ? l_i * theta : l_i / theta (one fp32 IEEE multiply or divide); every other l'_i = l_i.
-//      An id that occurs more than once is penalised once.  theta == 1 is off, and then the history is not
-//      read.  Steps 1 to 5 run on l'.
+//      An id that occurs more than once is penalised once.  theta == 1 is off.
+//   Step 0 runs as four sub-steps, in HF's order (sequence bias before the repetition penalty) and, within the
+//   penalties, vLLM's (repetition, frequency, presence), each one fp32 IEEE operation:
+//  0a. Logit bias: l_i + b_i for every i, b the dense [V] table of an {id: bias} map (unset entries 0, each
+//      entry 0 + bias as HF builds it).  Skipped when no bias is set, which keeps the sign of a -0.0 logit.
+//  0b. The repetition penalty above, over H(pos).
+//  0c. Frequency: C(pos) = the multiset of ids fed at positions [from_pos, pos] (empty for from_pos > pos), c_i
+//      the multiplicity of i in it.  For c_i > 0: l_i - alpha_f * (float)c_i.  Skipped for alpha_f == 0.
+//  0d. Presence: for c_i > 0, l_i - alpha_p.  Skipped for alpha_p == 0.
+//   With every sub-step off the history is not read.  Counts are exact integers, so every block, CTA, engine
+//   and rank computes the same l'.  Steps 1 to 5 run on l'.
 //   1. T == 0: greedy argmax (maximum, lowest index on ties) -- no noise is computed.
 //   2. s_i = l_i / T, IEEE division.
 //   3. 0 < k < V: tau = the k-th largest s_i; keep every i with s_i >= tau (ties at tau are kept).
@@ -48,11 +57,19 @@ struct SampleParams {
   float top_p;
 };
 
-// Device-resident repetition penalty (kllm_decoder_set_repetition_penalty), apart from SampleParams so that
-// setting either leaves the other alone.  A zeroed struct is off, as is penalty 1.
+// Device-resident step 0 (kllm_decoder_set_repetition_penalty, kllm_decoder_set_frequency_presence,
+// kllm_decoder_set_logit_bias), apart from SampleParams so that setting either leaves the other alone.  A
+// zeroed struct is off.  `active` is set by the host (step0_finish) when any sub-step is on, so that the
+// engines test one word.  `marks` [V] is zero between tokens (step0_rows).
 struct PenaltyParams {
-  float penalty;
-  int32_t last_n;
+  int32_t active;
+  float penalty;      // 0b; 1 (or 0 in a zeroed struct) is off
+  int32_t last_n;     // 0b's window
+  float frequency;    // 0c; 0 is off
+  float presence;     // 0d; 0 is off
+  int32_t from_pos;   // 0c / 0d count the ids fed at [from_pos, pos]
+  const float* bias;  // 0a's dense [V] table; null is off
+  int32_t* marks;
 };
 
 namespace sampling {
@@ -60,6 +77,17 @@ namespace sampling {
 __host__ __device__ __forceinline__ bool penalty_active(const PenaltyParams& pp) {
   return pp.penalty > 0.f && pp.penalty != 1.f;
 }
+
+__host__ __device__ __forceinline__ bool counts_active(const PenaltyParams& pp) {
+  return pp.frequency != 0.f || pp.presence != 0.f;
+}
+
+// The host's last word on a PenaltyParams it changed
+__host__ __forceinline__ void step0_finish(PenaltyParams& pp) {
+  pp.active = penalty_active(pp) || counts_active(pp) || pp.bias != nullptr;
+}
+
+__host__ __device__ __forceinline__ bool step0_active(const PenaltyParams& pp) { return pp.active != 0; }
 
 // Step 0's lower end of the window at `pos`
 __host__ __device__ __forceinline__ int window_lo(const PenaltyParams& pp, int pos) {
@@ -71,22 +99,81 @@ __device__ __forceinline__ float penalize(float l, float theta) {
   return l < 0.f ? __fmul_rn(l, theta) : __fdiv_rn(l, theta);
 }
 
-// Step 0b of logits[lo_row, hi_row) into out[lo_row, hi_row) by the NT threads of one block (or one CTA's
-// consumer threads): copy the raw rows, then penalise every id of hist[lo, pos] that falls in the range.
-// Thread t reads the history entries j = t (mod NT) only.  A duplicate id writes the same value again, so no
-// deduplication is needed.  `sync` orders the copy before the penalised writes and those before the caller's
-// reads (a CTA barrier orders global memory between its threads).
-template <int NT, class Sync>
-__device__ __forceinline__ void penalize_rows(const float* logits, float* out, int lo_row, int hi_row,
-                                              const int32_t* hist, int lo, int pos, float theta, Sync sync) {
-  const int tid = threadIdx.x;
-  for (int i = lo_row + tid; i < hi_row; i += NT) out[i] = __ldcg(logits + i);
-  sync();
-  for (int j = lo + ((tid - lo % NT) + NT) % NT; j <= pos; j += NT) {
-    const int id = hist[j];
-    if (id >= lo_row && id < hi_row) out[id] = penalize(__ldcg(logits + id), theta);
+// A mark word of step0_rows: bit 30 is membership in H(pos), bits 0..29 the count c_i (positions < 2^30)
+constexpr int32_t kInHistory = 1 << 30;
+
+// The whole of step 0 on the raw logit l of id i with mark word `mark`
+__device__ __forceinline__ float step0_value(float l, const PenaltyParams& pp, int i, int32_t mark) {
+  if (pp.bias != nullptr) l = __fadd_rn(l, __ldg(pp.bias + i));
+  if (mark & kInHistory) l = penalize(l, pp.penalty);
+  if (mark & (kInHistory - 1)) {
+    if (pp.frequency != 0.f) l = __fsub_rn(l, __fmul_rn(pp.frequency, __int2float_rn(mark & (kInHistory - 1))));
+    if (pp.presence != 0.f) l = __fsub_rn(l, pp.presence);
   }
+  return l;
+}
+
+// ids[lo, hi): step 0's windows are two such ranges of the history
+struct IdRange {
+  const int32_t* ids;
+  int lo, hi;
+};
+
+// fn(id) for the entries j of r with j = t (mod NT), t this thread
+template <int NT, class F>
+__device__ __forceinline__ void for_each_id(const IdRange& r, F fn) {
+  const int tid = threadIdx.x;
+  for (int j = r.lo + ((tid - r.lo % NT) + NT) % NT; j < r.hi; j += NT) fn(__ldcg(r.ids + j));
+}
+
+// Step 0 of logits[lo_row, hi_row) into out[lo_row, hi_row) by the NT threads of one block (or one CTA's
+// consumer threads), `rep` the ids of H(pos) and `cnt` those of C(pos):
+//   1. the copy pass writes l_i (+ b_i);
+//   2. every id of either window in the row range is marked in pp.marks with integer atomics: + 1 per
+//      occurrence in `cnt`, | kInHistory for one in `rep`;
+//   3. every thread that meets an id writes step0_value of its raw logit and its mark word, so a duplicate
+//      writes the same value again and no deduplication is needed;
+//   4. the marks of the ids met are reset to 0.
+// Thread t reads the window entries j = t (mod NT) only.  Rows outside [lo_row, hi_row) are not touched, so
+// blocks over disjoint ranges do not race.  `sync` orders each pass before the next (a CTA barrier orders
+// global memory between its threads) and the writes before the caller's reads; the reset needs no barrier of
+// its own, as the next token's marks come behind the caller's.
+template <int NT, class Sync>
+__device__ __forceinline__ void step0_rows(const float* logits, float* out, int lo_row, int hi_row,
+                                           const PenaltyParams& pp, const IdRange& rep, const IdRange& cnt,
+                                           Sync sync) {
+  const int tid = threadIdx.x;
+  for (int i = lo_row + tid; i < hi_row; i += NT) {
+    const float l = __ldcg(logits + i);
+    out[i] = pp.bias != nullptr ? __fadd_rn(l, __ldg(pp.bias + i)) : l;
+  }
+  if (rep.lo >= rep.hi && cnt.lo >= cnt.hi) {  // the bias alone
+    sync();
+    return;
+  }
+  int32_t* marks = pp.marks;
+  const auto mine = [lo_row, hi_row](int id) { return id >= lo_row && id < hi_row; };
+  for_each_id<NT>(cnt, [&](int id) { if (mine(id)) atomicAdd(marks + id, 1); });
+  for_each_id<NT>(rep, [&](int id) { if (mine(id)) atomicOr(marks + id, kInHistory); });
   sync();
+  const auto write = [&](int id) {
+    if (mine(id)) out[id] = step0_value(__ldcg(logits + id), pp, id, __ldcg(marks + id));
+  };
+  for_each_id<NT>(cnt, write);
+  for_each_id<NT>(rep, write);
+  sync();
+  const auto reset = [&](int id) { if (mine(id)) marks[id] = 0; };
+  for_each_id<NT>(cnt, reset);
+  for_each_id<NT>(rep, reset);
+}
+
+// Step 0 at `pos` over the decoder's history hist[seq_len] (the id fed at each position)
+template <int NT, class Sync>
+__device__ __forceinline__ void step0_history(const float* logits, float* out, int lo_row, int hi_row,
+                                              const PenaltyParams& pp, const int32_t* hist, int pos, Sync sync) {
+  const IdRange rep{hist, penalty_active(pp) ? window_lo(pp, pos) : 0, penalty_active(pp) ? pos + 1 : 0};
+  const IdRange cnt{hist, counts_active(pp) ? max(0, pp.from_pos) : 0, counts_active(pp) ? pos + 1 : 0};
+  step0_rows<NT>(logits, out, lo_row, hi_row, pp, rep, cnt, sync);
 }
 
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {

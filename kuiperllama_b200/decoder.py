@@ -308,6 +308,23 @@ class Decoder:
         check(self.lib.kllm_decoder_set_repetition_penalty(self.handle, float(penalty), int(last_n)),
               "kllm_decoder_set_repetition_penalty")
 
+    def set_frequency_presence(self, frequency: float, presence: float, from_pos: int = 0):
+        """Subtract, before every later draw, frequency * c_i and then presence from the logit of every id fed
+        c_i > 0 times at positions [from_pos, pos] (OpenAI's frequency_penalty / presence_penalty; from_pos = the
+        prompt's length counts the generated ids only).  0, 0 is off; the other settings are left alone
+        (kllm_decoder_set_frequency_presence; sampling.frequency_presence mirrors it)."""
+        check(self.lib.kllm_decoder_set_frequency_presence(self.handle, float(frequency), float(presence),
+                                                           int(from_pos)), "kllm_decoder_set_frequency_presence")
+
+    def set_logit_bias(self, mapping=None):
+        """Add mapping[id] to the logit of each id before every later draw (OpenAI's logit_bias), replacing the
+        map in force; None or {} clears it (kllm_decoder_set_logit_bias; sampling.apply_bias mirrors it)."""
+        mapping = mapping or {}
+        ids = (ctypes.c_int32 * max(1, len(mapping)))(*[int(i) for i in mapping])
+        vals = (ctypes.c_float * max(1, len(mapping)))(*[float(b) for b in mapping.values()])
+        check(self.lib.kllm_decoder_set_logit_bias(self.handle, ids, vals, len(mapping)),
+              "kllm_decoder_set_logit_bias")
+
     def set_logprobs(self, top_n: int):
         """Record, at every position whose classifier runs, the returned id's log-probability over the raw logits and,
         for top_n > 0, the top_n alternatives (kllm_decoder_set_logprobs; sampling.logprobs mirrors the rule).  -1 is

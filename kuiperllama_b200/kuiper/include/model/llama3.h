@@ -101,6 +101,15 @@ class LLama2Model : public Model {
   // finite or <= 0 and last_n < 0.  The fused paths take the ids from the decoder's history; predict() of a tensor
   // that is not a row of the last embedding() cannot know its id and is refused while the penalty is on.
   void set_repetition_penalty(float penalty, int32_t last_n = 0);
+  // Frequency and presence penalties before every draw (kllm_decoder_set_frequency_presence, DESIGN.md 5.9): each id
+  // fed c > 0 times at positions [from_pos, pos] loses frequency * c, then presence.  Call before init(); without a
+  // call init() takes them from KUIPER_FREQUENCY_PENALTY and KUIPER_PRESENCE_PENALTY (from_pos 0).  Unset or 0 is
+  // off; init() refuses a value that is not finite and from_pos < 0.  Like the repetition penalty, predict() of a
+  // tensor that is not a row of the last embedding() is refused while they are on.
+  void set_frequency_presence(float frequency, float presence, int32_t from_pos = 0);
+  // Logit bias before every draw (kllm_decoder_set_logit_bias): id -> bias, added before the penalties.  Call before
+  // init(), which refuses an id outside the vocabulary, a repeated id and a bias that is not finite.  Empty is off.
+  void set_logit_bias(std::vector<std::pair<int32_t, float>> bias);
   // the settings in force (after init(): the environment's when set_sampling / set_top_p was not called)
   float sampling_temperature() const { return temperature_; }
   int32_t sampling_top_k() const { return top_k_; }
@@ -108,6 +117,12 @@ class LLama2Model : public Model {
   float sampling_top_p() const { return top_p_; }
   float sampling_repetition_penalty() const { return penalty_; }
   int32_t sampling_repeat_last_n() const { return repeat_last_n_; }
+  float sampling_frequency_penalty() const { return frequency_; }
+  float sampling_presence_penalty() const { return presence_; }
+  int32_t sampling_count_from() const { return count_from_; }
+  const std::vector<std::pair<int32_t, float>>& sampling_logit_bias() const { return logit_bias_; }
+  // any of step 0's settings other than the repetition penalty is on
+  bool sampling_step0_extras() const { return frequency_ != 0.f || presence_ != 0.f || !logit_bias_.empty(); }
 
   // A whole generation on the fused decoder, without a host round trip per token:
   //   1. the prompt from position 0 (the batched prefill for all but its last token when batched_prefill() is
@@ -189,6 +204,10 @@ class LLama2Model : public Model {
   float penalty_ = 1.f;
   int32_t repeat_last_n_ = 0;
   bool penalty_explicit_ = false;
+  float frequency_ = 0.f, presence_ = 0.f;
+  int32_t count_from_ = 0;
+  bool frequency_presence_explicit_ = false;
+  std::vector<std::pair<int32_t, float>> logit_bias_;
   int32_t logprobs_top_n_ = -1;
   sampler::SeededSampler* seeded_ = nullptr;  // sampler_ when sampling, else null
   std::vector<int32_t> extra_stop_ids_;       // set_stop_ids()

@@ -95,6 +95,15 @@ void LLama2Model::set_repetition_penalty(float penalty, int32_t last_n) {
   penalty_explicit_ = true;
 }
 
+void LLama2Model::set_frequency_presence(float frequency, float presence, int32_t from_pos) {
+  frequency_ = frequency;
+  presence_ = presence;
+  count_from_ = from_pos;
+  frequency_presence_explicit_ = true;
+}
+
+void LLama2Model::set_logit_bias(std::vector<std::pair<int32_t, float>> bias) { logit_bias_ = std::move(bias); }
+
 void LLama2Model::set_logprobs(int32_t top_n) { logprobs_top_n_ = top_n; }
 
 base::Status LLama2Model::logprobs(int32_t first_pos, int32_t n, std::vector<int32_t>& ids, std::vector<float>& lp,
@@ -173,6 +182,28 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
     return error::InvalidArgument(
         "sampling: repetition_penalty must be finite and > 0, and its last_n >= 0 (KUIPER_REPETITION_PENALTY / "
         "KUIPER_REPEAT_LAST_N / set_repetition_penalty)");
+  if (!frequency_presence_explicit_) {
+    const char* f = std::getenv("KUIPER_FREQUENCY_PENALTY");
+    const char* p = std::getenv("KUIPER_PRESENCE_PENALTY");
+    frequency_ = f != nullptr ? std::strtof(f, nullptr) : 0.f;
+    presence_ = p != nullptr ? std::strtof(p, nullptr) : 0.f;
+    count_from_ = 0;
+  }
+  if (!std::isfinite(frequency_) || !std::isfinite(presence_) || count_from_ < 0)
+    return error::InvalidArgument(
+        "sampling: frequency and presence penalties must be finite, and from_pos >= 0 (KUIPER_FREQUENCY_PENALTY / "
+        "KUIPER_PRESENCE_PENALTY / set_frequency_presence)");
+  {
+    std::vector<int32_t> ids;
+    for (const auto& [id, b] : logit_bias_) {
+      if (id < 0 || !std::isfinite(b))
+        return error::InvalidArgument("sampling: a logit bias needs ids >= 0 and finite values (set_logit_bias)");
+      ids.push_back(id);
+    }
+    std::sort(ids.begin(), ids.end());
+    if (std::adjacent_find(ids.begin(), ids.end()) != ids.end())
+      return error::InvalidArgument("sampling: a logit bias lists an id twice (set_logit_bias)");
+  }
   if (logprobs_top_n_ < -1 || logprobs_top_n_ > KLLM_MAX_TOP_LOGPROBS)
     return error::InvalidArgument("logprobs: top_n must be in [-1, 20] (set_logprobs)");
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
@@ -188,6 +219,7 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
                                 get_buffer(ModelBufferType::kCosCache), cuda_config_->stream);
   if (temperature_ > 0.f) {
     auto seeded = std::make_unique<sampler::SeededSampler>(device_type_, temperature_, top_k_, seed_, top_p_, penalty_);
+    seeded->set_penalties(frequency_, presence_, logit_bias_);
     seeded_ = seeded.get();
     sampler_ = std::move(seeded);
   } else {
@@ -575,6 +607,24 @@ base::Status LLama2Model::create_decoder() {
                                         kllm_error_string(prc));
     LOG(INFO) << "sampling: repetition_penalty " << penalty_ << ", last_n " << repeat_last_n_;
   }
+  if (frequency_ != 0.f || presence_ != 0.f) {
+    const int frc = kllm_decoder_set_frequency_presence(decoder_, frequency_, presence_, count_from_);
+    if (frc != 0)
+      return base::error::InternalError(std::string("kllm_decoder_set_frequency_presence failed: ") +
+                                        kllm_error_string(frc));
+    LOG(INFO) << "sampling: frequency_penalty " << frequency_ << ", presence_penalty " << presence_ << ", from_pos "
+              << count_from_;
+  }
+  if (!logit_bias_.empty()) {
+    std::vector<int32_t> ids;
+    std::vector<float> vals;
+    for (const auto& [id, b] : logit_bias_) ids.push_back(id), vals.push_back(b);
+    const int brc = kllm_decoder_set_logit_bias(decoder_, ids.data(), vals.data(), static_cast<int32_t>(ids.size()));
+    if (brc != 0)
+      return base::error::InvalidArgument(std::string("sampling: kllm_decoder_set_logit_bias refused the map (an id "
+                                                      "outside the vocabulary?): ") + kllm_error_string(brc));
+    LOG(INFO) << "sampling: logit_bias of " << ids.size() << " id(s)";
+  }
   if (logprobs_top_n_ >= 0) {
     const int lrc = kllm_decoder_set_logprobs(decoder_, logprobs_top_n_);
     if (lrc != 0)
@@ -668,6 +718,10 @@ base::Status LLama2Model::predict(const tensor::Tensor& input, const tensor::Ten
       return base::error::Success();
     }
   }
+  if (sampling_step0_extras())
+    return base::error::InvalidArgument(
+        "frequency / presence penalty or logit bias: predict() needs a row of the last embedding() call (the layer "
+        "path applies them in tools only, from the ids the tool fed)");
   if (penalty_ != 1.f)
     return base::error::InvalidArgument(
         "repetition_penalty: predict() needs a row of the last embedding() call, whose token id the penalty's "

@@ -191,7 +191,8 @@ size_t sampler::SeededSampler::sample(const float* logits, size_t size, void* st
   CHECK(device_type_ == base::DeviceType::kDeviceCUDA) << "SeededSampler: CUDA logits only (no CPU backend)";
   static thread_local int64_t* d_idx = nullptr;
   if (d_idx == nullptr) CHECK(cudaMalloc(reinterpret_cast<void**>(&d_idx), sizeof(int64_t)) == cudaSuccess) << "SeededSampler: cudaMalloc";
-  if (penalty_ != 1.f) {  // step 0b on a copy of the logits, then the draw from that copy
+  const bool extras = frequency_ != 0.f || presence_ != 0.f || !bias_ids_.empty();
+  if (penalty_ != 1.f || extras) {  // step 0 on a copy of the logits, then the draw from that copy
     static thread_local float* d_pen = nullptr;
     static thread_local size_t pen_cap = 0;
     static thread_local int32_t* d_ids = nullptr;
@@ -201,19 +202,32 @@ size_t sampler::SeededSampler::sample(const float* logits, size_t size, void* st
       CHECK(cudaMalloc(reinterpret_cast<void**>(&d_pen), size * sizeof(float)) == cudaSuccess) << "SeededSampler: cudaMalloc";
       pen_cap = size;
     }
-    if (ids_cap < history_.size()) {
+    // the history, then (with extras) the counted ids behind it
+    const size_t n_ids = history_.size() + (extras ? counted_.size() : 0);
+    if (ids_cap < n_ids) {
       if (d_ids != nullptr) cudaFree(d_ids);
-      CHECK(cudaMalloc(reinterpret_cast<void**>(&d_ids), history_.size() * sizeof(int32_t)) == cudaSuccess)
+      CHECK(cudaMalloc(reinterpret_cast<void**>(&d_ids), n_ids * sizeof(int32_t)) == cudaSuccess)
           << "SeededSampler: cudaMalloc";
-      ids_cap = history_.size();
+      ids_cap = n_ids;
     }
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (!history_.empty())
       CHECK(cudaMemcpyAsync(d_ids, history_.data(), history_.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s) ==
             cudaSuccess) << "SeededSampler: copy of the history";
-    const int prc = kllm_repetition_penalty_f32(logits, d_pen, static_cast<int64_t>(size), d_ids,
-                                                static_cast<int32_t>(history_.size()), penalty_, stream);
-    CHECK(prc == 0) << "kllm_repetition_penalty_f32: " << kllm_error_string(prc);
+    if (extras) {
+      if (!counted_.empty())
+        CHECK(cudaMemcpyAsync(d_ids + history_.size(), counted_.data(), counted_.size() * sizeof(int32_t),
+                              cudaMemcpyHostToDevice, s) == cudaSuccess) << "SeededSampler: copy of the counted ids";
+      const int prc = kllm_logit_penalties_f32(
+          logits, d_pen, static_cast<int64_t>(size), bias_ids_.data(), bias_.data(), static_cast<int32_t>(bias_.size()),
+          penalty_, d_ids, static_cast<int32_t>(history_.size()), frequency_, presence_, d_ids + history_.size(),
+          static_cast<int32_t>(counted_.size()), stream);
+      CHECK(prc == 0) << "kllm_logit_penalties_f32: " << kllm_error_string(prc);
+    } else {
+      const int prc = kllm_repetition_penalty_f32(logits, d_pen, static_cast<int64_t>(size), d_ids,
+                                                  static_cast<int32_t>(history_.size()), penalty_, stream);
+      CHECK(prc == 0) << "kllm_repetition_penalty_f32: " << kllm_error_string(prc);
+    }
     logits = d_pen;
   }
   const int rc =

@@ -3,7 +3,8 @@
 //
 //   kuiper_decode <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...]
 //                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P]
-//                 [--repetition-penalty P N] [--generate N [--stop ID]... [--then K]] [--logprobs N] [--score]
+//                 [--repetition-penalty P N] [--frequency-presence F P [FROM]] [--logit-bias ID:B,...]
+//                 [--generate N [--stop ID]... [--then K]] [--logprobs N] [--score]
 //
 // --generate N runs the prompt and LLama2Model::generate() for at most N ids instead (n_steps is then unused),
 // stopping at the tokenizer's stop ids and every --stop ID, and prints the ids generate() returned, followed
@@ -19,6 +20,10 @@
 // LLama2Model::set_top_p(P) instead of KUIPER_TOP_P.  --repetition-penalty P N calls
 // LLama2Model::set_repetition_penalty(P, N) instead of KUIPER_REPETITION_PENALTY / KUIPER_REPEAT_LAST_N; --layers
 // applies the penalty itself, over the ids this tool fed, to the seeded draw and to its greedy argmax.
+// --frequency-presence F P [FROM] calls LLama2Model::set_frequency_presence(F, P, FROM) (FROM, 0 when absent, is
+// taken when the next argument is an integer: give the prompt ids first) and --logit-bias ID:B,...
+// LLama2Model::set_logit_bias; with either on, --layers draws through SeededSampler (kllm_logit_penalties_f32 over
+// the ids this tool fed), greedily at temperature 0.
 // --logprobs N calls LLama2Model::set_logprobs(N) and, after the ids, prints one line per position that has a record
 // entry: "lp <pos> <id> <lp>" followed by N pairs "<top id> <top lp>" (%.9g: the fp32 values round-trip).
 // --score scores the given ids with LLama2Model::score() instead of decoding (n_steps is then unused): one line of
@@ -45,7 +50,8 @@ int main(int argc, char** argv) {
   if (argc < 6) {
     std::fprintf(stderr, "usage: %s <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...] "
                          "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P] "
-                         "[--repetition-penalty P N] [--generate N [--stop ID]... [--then K]]\n", argv[0]);
+                         "[--repetition-penalty P N] [--frequency-presence F P [FROM]] [--logit-bias ID:B,...] "
+                         "[--generate N [--stop ID]... [--then K]]\n", argv[0]);
     return 2;
   }
   const std::string checkpoint = argv[1], family = argv[2], prec = argv[3];
@@ -63,6 +69,10 @@ int main(int argc, char** argv) {
   bool set_penalty = false;
   float penalty = 1.f;
   int32_t last_n = 0;
+  bool set_fp = false;
+  float frequency = 0.f, presence = 0.f;
+  int32_t count_from = 0;
+  std::vector<std::pair<int32_t, float>> logit_bias;
   int generate = 0, then = 0;
   std::vector<int32_t> stops;
   int32_t logprobs = -1;
@@ -83,6 +93,26 @@ int main(int argc, char** argv) {
       set_penalty = true;
       penalty = std::strtof(argv[++i], nullptr);
       last_n = static_cast<int32_t>(std::strtol(argv[++i], nullptr, 10));
+    }
+    else if (!std::strcmp(argv[i], "--frequency-presence") && i + 2 < argc) {
+      set_fp = true;
+      frequency = std::strtof(argv[++i], nullptr);
+      presence = std::strtof(argv[++i], nullptr);
+      char* end = nullptr;
+      if (i + 1 < argc) {
+        const long from = std::strtol(argv[i + 1], &end, 10);
+        if (end != argv[i + 1] && *end == '\0') {
+          count_from = static_cast<int32_t>(from);
+          ++i;
+        }
+      }
+    }
+    else if (!std::strcmp(argv[i], "--logit-bias") && i + 1 < argc) {
+      for (char* tok = std::strtok(argv[++i], ","); tok != nullptr; tok = std::strtok(nullptr, ",")) {
+        char* colon = std::strchr(tok, ':');
+        if (colon == nullptr) return 2;
+        logit_bias.emplace_back(static_cast<int32_t>(std::strtol(tok, nullptr, 10)), std::strtof(colon + 1, nullptr));
+      }
     }
     else if (!std::strcmp(argv[i], "--generate") && i + 1 < argc) generate = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--stop") && i + 1 < argc) stops.push_back(std::atoi(argv[++i]));
@@ -112,6 +142,8 @@ int main(int argc, char** argv) {
   if (set_sampling) m->set_sampling(temperature, top_k, seed);
   if (set_top_p) m->set_top_p(top_p);
   if (set_penalty) m->set_repetition_penalty(penalty, last_n);
+  if (set_fp) m->set_frequency_presence(frequency, presence, count_from);
+  if (!logit_bias.empty()) m->set_logit_bias(logit_bias);
   if (!stops.empty()) m->set_stop_ids(stops);
   if (set_logprobs) m->set_logprobs(logprobs);  // init() refuses a value outside [-1, 20]
   base::Status st = m->init(base::DeviceType::kDeviceCUDA);
@@ -186,10 +218,12 @@ int main(int argc, char** argv) {
   auto prompt_embedding = m->embedding(prompt);
   // --layers draws with the model's settings too (the layer path's SeededSampler)
   std::unique_ptr<sampler::SeededSampler> seeded;
-  if (m->sampling_temperature() > 0.f)
+  if (m->sampling_temperature() > 0.f || m->sampling_step0_extras()) {
     seeded = std::make_unique<sampler::SeededSampler>(base::DeviceType::kDeviceCUDA, m->sampling_temperature(),
                                                       m->sampling_top_k(), m->sampling_seed(),
                                                       m->sampling_top_p(), m->sampling_repetition_penalty());
+    seeded->set_penalties(m->sampling_frequency_penalty(), m->sampling_presence_penalty(), m->sampling_logit_bias());
+  }
   std::vector<float> host_logits;
   int next = -1;
   std::vector<int> chosen;
@@ -222,6 +256,9 @@ int main(int argc, char** argv) {
       const tensor::Tensor& lg = m->get_buffer(model::ModelBufferType::kForwardOutput);
       seeded->set_position(pos_tensor.index<int32_t>(0));
       seeded->set_history(window(pos_tensor.index<int32_t>(0)));
+      // step 0's count window [from_pos, pos] of the ids fed (DESIGN.md 5.9)
+      const int32_t at = pos_tensor.index<int32_t>(0), from = std::min(m->sampling_count_from(), at + 1);
+      seeded->set_counted(std::vector<int32_t>(fed.begin() + from, fed.begin() + at + 1));
       next = static_cast<int>(seeded->sample(lg.ptr<float>(), lg.size(), nullptr));
     } else if (!is_prompt) {  // greedy argmax, lowest index on ties (argmax_sampler.cpp)
       tensor::Tensor lg = m->get_buffer(model::ModelBufferType::kForwardOutput).clone();

@@ -65,6 +65,60 @@ def penalize(logits, ids, penalty: float) -> np.ndarray:
     return out
 
 
+def bias_table(mapping, n: int):
+    """Step 0a's dense table [n] fp32 of an {id: bias} map (unset entries 0), or None for an empty map: then the
+    step is skipped, which keeps the sign of a -0.0 logit.  Each entry is 0 + b, as HF builds its bias (a -0.0
+    bias is +0.0)."""
+    if not mapping:
+        return None
+    table = np.zeros(n, np.float32)
+    for i, b in mapping.items():
+        table[int(i)] += np.float32(b)
+    return table
+
+
+def apply_bias(logits, table) -> np.ndarray:
+    """Step 0a: l_i + b_i for every i (one fp32 addition), or the logits unchanged when `table` is None."""
+    out = np.array(logits, np.float32, copy=True)
+    return out if table is None else out + np.asarray(table, np.float32)
+
+
+def count_window(history, pos: int, from_pos: int) -> np.ndarray:
+    """Steps 0c/0d's C(pos): the entries of `history` at positions [from_pos, pos] (empty for from_pos > pos)."""
+    return np.asarray(history, np.int64)[max(0, from_pos):pos + 1]
+
+
+def frequency_presence(logits, ids, frequency: float, presence: float) -> np.ndarray:
+    """Steps 0c and 0d: for every i with c_i > 0 occurrences in `ids` (ids < 0 or >= len(logits) ignored),
+    l_i - fp32(frequency) * fp32(c_i), then - fp32(presence), each one fp32 operation; a zero alpha skips its
+    line.  The other logits unchanged."""
+    out = np.array(logits, np.float32, copy=True)
+    ids = np.asarray(ids, np.int64)
+    ids = ids[(ids >= 0) & (ids < out.shape[0])]
+    if ids.size == 0:
+        return out
+    counted, c = np.unique(ids, return_counts=True)
+    f, p = np.float32(frequency), np.float32(presence)
+    l = out[counted]
+    with np.errstate(over="ignore"):
+        if f != 0:
+            l = l - f * c.astype(np.float32)
+        if p != 0:
+            l = l - p
+    out[counted] = l
+    return out
+
+
+def penalties(logits, *, bias=None, rep_ids=(), penalty: float = 1.0, count_ids=(), frequency: float = 0.0,
+              presence: float = 0.0) -> np.ndarray:
+    """The whole of step 0 in its order: 0a bias (`bias` a dense table or None), 0b the repetition penalty over
+    `rep_ids`, 0c frequency and 0d presence over the multiset `count_ids`."""
+    out = apply_bias(logits, bias)
+    if np.float32(penalty) != 1:
+        out = penalize(out, rep_ids, penalty)
+    return frequency_presence(out, count_ids, frequency, presence)
+
+
 NUCLEUS_EPS = 1e-6
 """np.exp and the device expf may differ in the last ulps of each weight, which moves A and Z by well under
 this much of Z: a nucleus comparison closer than that may go either way on the device."""

@@ -20,11 +20,16 @@ synchronisation, so a host clock around it times it.  Every mode is warmed up on
   numpy mirror on the run's own logits): a top-p rate means little without it.  With --repetition-penalty,
   the modes with the penalty are named "<mode>+rp", and penalty_overhead {mode: 1 - rate with / rate without}.
 
+--frequency F, --presence P (kllm_decoder_set_frequency_presence, counting from --start-pos: the ids generated in
+the window) and --logit-bias N (N random ids with biases in [-2, 2], kllm_decoder_set_logit_bias) join the settings
+of the "+rp" modes in the same way; they run without a repetition penalty unless --repetition-penalty is given.
+
 Needs a CUDA device; there is nothing to time without one.
 """
 import argparse
 import json
 import math
+import random
 import statistics
 import sys
 import time
@@ -36,7 +41,8 @@ sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from bench_prefill import SEEDS, gpu_card  # noqa: E402
 
 
-def run(workload, steps, reps, seed, temperature, top_k, top_p=None, penalty=None, last_n=0, start_pos=0):
+def run(workload, steps, reps, seed, temperature, top_k, top_p=None, penalty=None, last_n=0, start_pos=0,
+        frequency=0.0, presence=0.0, n_bias=0):
     import torch
     from kuiperllama_b200 import SHAPES, Decoder, synth_weights
     shape = SHAPES[workload]
@@ -48,26 +54,36 @@ def run(workload, steps, reps, seed, temperature, top_k, top_p=None, penalty=Non
     modes = [("greedy", 0.0, 0, 1.0), ("top_k=0", temperature, 0, 1.0), (f"top_k={top_k}", temperature, top_k, 1.0)]
     if top_p is not None:
         modes += [(f"top_p={top_p}", temperature, 0, top_p), (f"top_k={top_k},top_p={top_p}", temperature, top_k, top_p)]
-    runs = [(name, t, k, p, 1.0) for name, t, k, p in modes]
-    if penalty is not None:  # each mode with the penalty right after the same mode without it
-        runs = [r for name, t, k, p in modes for r in ((name, t, k, p, 1.0), (name + "+rp", t, k, p, penalty))]
+    runs = [(name, t, k, p, False) for name, t, k, p in modes]
+    extras = frequency != 0 or presence != 0 or n_bias > 0
+    rng = random.Random(seed)
+    bias = {}
+    while len(bias) < n_bias:
+        bias[rng.randrange(shape.vocab_size)] = rng.uniform(-2, 2)
+    if penalty is not None or extras:  # each mode with the settings right after the same mode without them
+        runs = [r for name, t, k, p in modes for r in ((name, t, k, p, False), (name + "+rp", t, k, p, True))]
     times = {r[0]: [] for r in runs}
     if start_pos > 0:  # the cache and the history of the positions before the windows
         dec.generate(1, 0, start_pos)
 
-    def window(t, k, p, rp):
+    def window(t, k, p, on):
         dec.set_sampling(t, k, seed, top_p=p)
-        dec.set_repetition_penalty(rp, last_n)
+        dec.set_repetition_penalty(penalty if on and penalty is not None else 1.0, last_n)
+        if extras:
+            dec.set_frequency_presence(frequency if on else 0.0, presence if on else 0.0, start_pos)
+            dec.set_logit_bias(bias if on else None)
         t0 = time.perf_counter()
         dec.generate(1, start_pos, steps)
         return time.perf_counter() - t0
 
-    for _, t, k, p, rp in runs:
-        window(t, k, p, rp)
+    for _, t, k, p, on in runs:
+        window(t, k, p, on)
     for _ in range(max(1, reps)):
-        for name, t, k, p, rp in runs:
-            times[name].append(window(t, k, p, rp))
+        for name, t, k, p, on in runs:
+            times[name].append(window(t, k, p, on))
     dec.set_repetition_penalty(1.0)
+    dec.set_frequency_presence(0.0, 0.0)
+    dec.set_logit_bias(None)
     nucleus = {}
     if top_p is not None:  # untimed: the same positions stepped one by one, the kept set from each step's logits
         from kuiperllama_b200 import sampling
@@ -87,8 +103,9 @@ def run(workload, steps, reps, seed, temperature, top_k, top_p=None, penalty=Non
            "temperature": temperature, "greedy_tok_s": g, "sampled_tok_s": sampled,
            "overhead": {name: 1.0 - r / g for name, r in sampled.items()},
            "engine": engine, "numerics": "exact", "seed": seed, "card": gpu_card(torch.cuda.current_device())}
-    if penalty is not None:
-        out.update(repetition_penalty=penalty, repeat_last_n=last_n, start_pos=start_pos,
+    if penalty is not None or extras:
+        out.update(repetition_penalty=penalty, repeat_last_n=last_n, start_pos=start_pos, frequency=frequency,
+                   presence=presence, logit_bias_ids=n_bias,
                    penalty_overhead={name: 1.0 - rate[name + "+rp"] / rate[name] for name, _, _, _ in modes})
     if top_p is not None:
         out["nucleus_size"] = nucleus
@@ -106,6 +123,9 @@ def main():
     ap.add_argument("--repetition-penalty", type=float, default=None,
                     help="also time every mode with this repetition penalty")
     ap.add_argument("--repeat-last-n", type=int, default=0, help="the penalty's window (0: the whole sequence)")
+    ap.add_argument("--frequency", type=float, default=0.0, help="frequency penalty of the +rp modes")
+    ap.add_argument("--presence", type=float, default=0.0, help="presence penalty of the +rp modes")
+    ap.add_argument("--logit-bias", type=int, default=0, help="number of biased ids in the +rp modes")
     ap.add_argument("--start-pos", type=int, default=0, help="first position of the timed windows")
     ap.add_argument("--seed", type=int, default=None, help="default: bench.py's seed for the workload")
     a = ap.parse_args()
@@ -119,7 +139,7 @@ def main():
         raise SystemExit("--repeat-last-n and --start-pos must be >= 0")
     seed = SEEDS[a.workload] if a.seed is None else a.seed
     print(json.dumps(run(a.workload, a.steps, a.reps, seed, a.temperature, a.top_k, a.top_p, a.repetition_penalty,
-                         a.repeat_last_n, a.start_pos)))
+                         a.repeat_last_n, a.start_pos, a.frequency, a.presence, a.logit_bias)))
 
 
 if __name__ == "__main__":
