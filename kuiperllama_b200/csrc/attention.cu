@@ -156,6 +156,13 @@ int launch_mha(PosArg pos, int head_num, int layer_index, int seq_len, int kv_di
     return KLLM_E_UNSUPPORTED;
   const long long layer_offset = static_cast<long long>(layer_index) * seq_len * kv_dim;
   const size_t smem = sizeof(float) * (head_size + 2 * kVTile * head_size);
+  // head_size 188 is the largest whose q row and two value tiles fit the default 48 KB; larger
+  // heads (up to 256: 66 KB) opt in, as launch_gemv does.  The tiling does not touch the arithmetic.
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(mha_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         static_cast<int>(smem));
+    if (e != cudaSuccess) return static_cast<int>(e);
+  }
   mha_decode_kernel<<<head_num, kMhaThreads, smem, stream>>>(pos, seq_len, query, score, mha_out,
                                                             key_cache, value_cache, kv_dim,
                                                             kv_mul, head_size, layer_offset);

@@ -8,6 +8,9 @@ tests/test_decode_model_gpu.py holds the kernels to.
 2. Negative controls at the GPU test's constants: a quantiser that keeps two digit planes and two broken flash
    attentions move the model by 10x the bound or more, while +-1 unit of fp32 noise at every store (what a correct
    kernel with another summation order does) stays within half of it.
+3. Negative controls for tests/test_graph_engine_model_gpu.py: int8 scale groups restarted at each row or taken
+   one group too far move layer 0 by 10x KV_TAU_FIRST or more, and attention capped at head_size 128 moves the
+   later layers and the logits by 10x KV_TAU and LOGIT_TAU or more.
 """
 import math
 from dataclasses import replace
@@ -18,9 +21,9 @@ import torch
 
 import prefill_model
 from prefill_model import FP_ONE, balanced_digits, fixed_point_parts, fixed_point_value, prefill_ref
-from test_decode_model_gpu import KV_TAU, KV_TAU_FIRST, LOGIT_TAU, loud_weights, outlier_weights
+from decode_model_util import KV_TAU, KV_TAU_FIRST, LOGIT_TAU, loud_weights, outlier_weights
 
-from kuiperllama_b200 import SHAPES, synth_weights
+from kuiperllama_b200 import SHAPES, ModelShape, synth_weights
 
 
 def f32_bits(*u):
@@ -274,3 +277,89 @@ def test_one_unit_of_fp32_noise_stays_within_half_the_bound(monkeypatch, case):
     print(f"{case}: +-1 ulp moves K / V by {per_layer[0] / KV_TAU_FIRST:.3g} KV_TAU_FIRST in layer 0, "
           f"{[round(r / KV_TAU, 3) for r in per_layer[1:]]} KV_TAU after, logits by {logits / LOGIT_TAU:.3g} LOGIT_TAU")
     assert per_layer[0] <= KV_TAU_FIRST / 2 and max(per_layer[1:]) <= KV_TAU / 2 and logits <= LOGIT_TAU / 2
+
+
+# ---- negative controls for the graph engine's shapes and other group sizes ------------------------------------------
+def dequant_groups_per_row(q, scales, group_size, tf32=True):
+    """Groups restarted at each row: element c of row r takes scale r * (K / group) + c / group (integer division),
+    what a kernel indexing the scales per row computes, in place of one index over the flattened tensor."""
+    q = torch.as_tensor(q)
+    n, k = q.shape
+    s = torch.as_tensor(scales).to(torch.float32).reshape(-1)
+    idx = torch.arange(n)[:, None] * (k // group_size) + torch.arange(k)[None, :] // group_size
+    w = s[idx] * q.to(torch.float32)
+    return prefill_model.tf32_rna(w) if tf32 else w
+
+
+def dequant_next_group(q, scales, group_size, tf32=True):
+    """The scale index one group too far (the last group keeps its own scale)."""
+    q = torch.as_tensor(q)
+    n, k = q.shape
+    s = torch.as_tensor(scales).to(torch.float32).reshape(-1)
+    idx = (torch.arange(n * k) // group_size + 1).clamp(max=s.numel() - 1).reshape(n, k)
+    w = s[idx] * q.to(torch.float32)
+    return prefill_model.tf32_rna(w) if tf32 else w
+
+
+MODEL_ATTENTION = prefill_model._attention
+
+
+def attention_capped_at_128(q, k_all, v_all, start_pos, kv_mul, max_bytes=1 << 28):
+    """Attention over the first 128 dimensions of each head only, the output zero beyond them: a kernel whose
+    output chains and score loops stop at 128."""
+    out = torch.zeros_like(q)
+    out[..., :128] = MODEL_ATTENTION(q[..., :128].contiguous(), k_all[..., :128].contiguous(),
+                                     v_all[..., :128].contiguous(), start_pos, kv_mul, max_bytes)
+    return out
+
+
+CONTROL_SHAPES = {
+    # the graph-only int8 shapes of test_graph_engine_model_gpu.py at 32 positions
+    "rowspan": ModelShape("int8-g64-rowspan", 96, 160, 2, 3, 1, 512, 32, group_size=64),
+    "g32": ModelShape("int8-g32-hs48", 288, 768, 2, 6, 2, 1024, 32, group_size=32),
+    "hs192": ModelShape("hs192", 576, 1536, 2, 3, 1, 1024, 32),
+    "hs128": ModelShape("hs128", 256, 688, 2, 2, 1, 512, 32),
+}
+
+
+def control_model(key, seq=32):
+    shape = CONTROL_SHAPES[key]
+    w = (synth_weights if shape.group_size else loud_weights)(shape, "cpu", 77)
+    return shape, w, sincos(shape), tokens(shape, seq), list(range(0, seq, 4)) + [seq - 1]
+
+
+@pytest.mark.parametrize("key,patch,fn", [("g32", "dequant_w8", dequant_groups_per_row),
+                                          ("hs128", "_attention", attention_capped_at_128)])
+def test_controls_equal_the_model_where_nothing_differs(key, patch, fn):
+    """Groups per row are the flattened groups when the row length is a multiple of the group, and a cap at 128
+    does nothing at head_size 128: the controls below break only what they name."""
+    shape, w, (sin, cos), toks, ends = control_model(key)
+    ref = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends)
+    with pytest.MonkeyPatch.context() as mp:
+        mp.setattr(prefill_model, patch, fn)
+        same = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends)
+    assert max(kv_rel(same, ref)) == 0.0 and logit_rel(same, ref) == 0.0
+
+
+@pytest.mark.parametrize("broken,key", [("groups-per-row", "rowspan"), ("next-group", "g32"),
+                                        ("next-group", "rowspan"), ("head-size-capped", "hs192")])
+def test_broken_graph_engine_shapes_move_the_model_by_ten_bounds(monkeypatch, broken, key):
+    """Scale groups restarted at each row or taken one group too far move layer 0's K / V rows (before any
+    attention) by >= 10 KV_TAU_FIRST; attention capped at head_size 128 moves the later layers' rows by >= 10
+    KV_TAU and the logits by >= 10 LOGIT_TAU, leaving layer 0 as it was."""
+    shape, w, (sin, cos), toks, ends = control_model(key)
+    ref = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends)
+    if broken == "head-size-capped":
+        monkeypatch.setattr(prefill_model, "_attention", attention_capped_at_128)
+    else:
+        fn = dequant_groups_per_row if broken == "groups-per-row" else dequant_next_group
+        monkeypatch.setattr(prefill_model, "dequant_w8", fn)
+    bad = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends)
+    per_layer, logits = kv_rel(bad, ref), logit_rel(bad, ref)
+    print(f"{broken} on {key}: K / V move {per_layer[0] / KV_TAU_FIRST:.3g} KV_TAU_FIRST in layer 0, "
+          f"{[round(r / KV_TAU, 1) for r in per_layer[1:]]} KV_TAU after, logits {logits / LOGIT_TAU:.3g} LOGIT_TAU")
+    if broken == "head-size-capped":
+        assert per_layer[0] == 0.0
+        assert max(per_layer[1:]) >= 10 * KV_TAU and logits >= 10 * LOGIT_TAU
+    else:
+        assert per_layer[0] >= 10 * KV_TAU_FIRST

@@ -34,144 +34,22 @@ own, tight enough that a quantiser with two digit planes misses it by 20x (tests
 The fixed point's cost, the fast mode against the plain model: K / V within 6.4e-6 of the row rms and logits within
 7.0e-6 of their rms (llama2-7b-int8-2l outliers); 1e-6 to 3e-6 on the synth weights.
 """
-import math
-from dataclasses import replace
-
 import numpy as np
 import pytest
-import torch
 
-from gpu_util import ptr, sync
-from prefill_model import prefill_ref
-
-from kuiperllama_b200 import FLAVOURS, SHAPES, Decoder, ModelShape, synth_weights
-from kuiperllama_b200.decoder import quantize_q80
+from decode_model_util import (CASES, GEOMETRIES, KV_TAU, LOGIT_TAU, cached_model, case_id, clear_cache, edge_ends,
+                               flash_geometry, make_decoder, run, sms, split_cap, taus)
 
 pytestmark = pytest.mark.gpu
 
-# Worst measured error / rms beside each constant: exact mode, fast mode (both within 2x: one constant)
-KV_TAU_FIRST = 1e-5  # layer 0 of every case: 2.47e-6, 2.43e-6
-KV_TAU = 6e-5  # layers 1 and 2: 2.51e-5, 1.37e-5
-LOGIT_TAU = 8e-5  # 3.22e-5, 2.08e-5
-# TinyLlama-1.1B, 22 layers (synth weights: smaller errors than the loud 2 to 3 layer cases)
-KV_TAU_DEEP = 2e-5  # layers 1 .. 21: 6.32e-6, 5.23e-6
-LOGIT_TAU_DEEP = 2e-5  # 5.39e-6, 4.59e-6
+# The constants, with the worst values above beside them, live in tests/decode_model_util.py: the graph engine's
+# test holds its cases to the same ones.
 
 
-def report(*parts):
-    print("[decode-model]", *parts, flush=True)
-
-
-# ---- weights --------------------------------------------------------------------------------------------------
-def loud_weights(shape, device, seed):
-    """synth_weights with wq and wk scaled so that q.k / sqrt(hs) has std ~5 (q and k elements of std sqrt(5) for
-    unit-rms inputs) and Wo at std 1/sqrt(dim)."""
-    w = synth_weights(shape, device, seed)
-    c = math.sqrt(5.0 / (0.02 ** 2 * shape.dim))
-    w["wq"] *= c
-    w["wk"] *= c
-    g = torch.Generator(device=device).manual_seed(seed + 1)
-    w["wo"] = torch.empty_like(w["wo"]).normal_(0.0, 1.0 / math.sqrt(shape.dim), generator=g)
-    return w
-
-
-OUTLIER_CHANNELS = (5, -7)  # in the first and the last 64-group
-ZERO_GROUP = slice(64, 128)  # the second 64-group
-
-
-def outlier_weights(shape, device, seed):
-    """int8 weights with massive activations and all-zero groups, built in fp32 and quantised as export.py does:
-    two embedding channels at 300x the others (they dominate the residual stream of every layer), attn_norm zero on
-    one 64-group (an all-zero group reaches the quantiser in the QKV phase) and W1 zero on 64 rows (the SwiGLU
-    output, W2's input, is zero on that group), and weight bytes of -128 (the file format allows them; export.py
-    never writes them) in every matrix."""
-    w = synth_weights(replace(shape, group_size=0), device, seed)
-    for c in OUTLIER_CHANNELS:
-        w["tok_emb"][:, c] *= 300.0
-    w["attn_norm"][:, ZERO_GROUP] = 0.0
-    w["w1"][:, ZERO_GROUP, :] = 0.0
-    g = torch.Generator(device=device).manual_seed(seed + 2)
-    for name in ("wq", "wk", "wv", "wo", "w1", "w2", "w3", "wcls"):
-        mats = [w[name]] if name == "wcls" else list(w[name])
-        qs = [quantize_q80(t, shape.group_size) for t in mats]
-        q = torch.stack([a for a, _ in qs])
-        sc = torch.stack([b for _, b in qs])
-        flat = q.view(-1)
-        idx = torch.randint(0, flat.numel(), (64,), device=device, generator=g)
-        flat[idx] = -128
-        if name == "wcls":
-            q, sc = q[0], sc[0]
-        w[name], w["s" + name[1:]] = q.contiguous(), sc.contiguous()
-    return w
-
-
-WEIGHTS = {"synth": lambda shape, device, seed: synth_weights(shape, device, seed),
-           "loud": loud_weights, "outliers": outlier_weights}
-
-
-# ---- the engine's flash geometry (MegaEngine::init) ----------------------------------------------------------------
-def flash_geometry(shape, env, sms):
-    """(tile T, split SP) the fast mode runs with under `env`: T = min(stage_bytes / (hs * 4), 8 warps * 32) & ~31,
-    SP = the largest power of two <= 8 with heads * SP <= grid and SP * (hs + 2) <= seq_len unless KLLM_ATTN_SPLIT
-    asks for a smaller one (a larger one is ignored)."""
-    int8 = shape.group_size != 0
-    hs = shape.head_size
-    stage = int(env.get("KLLM_STAGE_BYTES", 27 * 1024 if int8 else 32 * 1024))
-    stage = (stage + 127) & ~127
-    T = min(stage // (hs * 4), 8 * 32) & ~31
-    grid = min(sms, shape.dim, shape.hidden_dim)
-    cap = 1
-    while cap * 2 <= 8 and shape.head_num * cap * 2 <= grid and cap * 2 * (hs + 2) <= shape.seq_len:
-        cap *= 2
-    sp = int(env.get("KLLM_ATTN_SPLIT", cap))
-    return T, sp if sp <= cap else cap
-
-
-def split_cap(shape, sms):
-    return flash_geometry(shape, {"KLLM_ATTN_SPLIT": "8"}, sms)[1]
-
-
-def edge_ends(T, SP, seq_len):
-    """Segment ends: the first blocks of 8 timesteps, the first tile's edge, the first CTA's second tile, the end."""
-    e = {0, 1, 7, 8, 9, T - 1, T, T + 1, SP * T - 1, SP * T, SP * T + 1, seq_len - 1}
-    return sorted(p for p in e if 0 <= p < seq_len)
-
-
-# ---- cases -------------------------------------------------------------------------------------------------------
-GEOMETRIES = {
-    # dim 64, 4 / 2 heads: head_size 16, T = 256, 8 CTAs per head
-    "hs16": ModelShape("decode-hs16", 64, 172, 2, 4, 2, 512, 2080),
-    "small": replace(SHAPES["small"], seq_len=2080),  # head_size 32, GQA 3, T = 256
-    "small-hs48": replace(SHAPES["small-hs48"], seq_len=1312),  # T = 160
-    "hs128": ModelShape("decode-hs128", 512, 1376, 2, 4, 2, 2048, 1056),  # T = 64
-    "small-qwen": replace(SHAPES["small-qwen"], seq_len=1056),  # bias, half-split pairs, eps 1e-6, T = 128
-    # Llama-3-8B attention geometry and vocabulary at two layers: half-split pairs, theta 5e5
-    "llama3-reduced": ModelShape("llama3-reduced", 4096, 14336, 2, 32, 8, 128256, 544, flavour="llama3"),
-    "small-int8": replace(SHAPES["small-int8"], seq_len=800),  # T = 96
-    "small-tp-int8": replace(SHAPES["small-tp-int8"], seq_len=800),
-    # Llama-2-7B int8 at two layers: T = 32, 4 CTAs per head
-    "llama2-7b-int8-2l": replace(SHAPES["llama2-7b-int8"], layer_num=2, seq_len=544),
-    "qwen2.5-reduced": ModelShape("qwen2.5-reduced", 896, 4864, 2, 14, 2, 4096, 16384, True, flavour="qwen2"),
-    "tinyllama-1.1b": replace(SHAPES["tinyllama-1.1b"], seq_len=1024),
-}
+# ---- cases (GEOMETRIES and CASES: tests/decode_model_util.py) -------------------------------------------------------
 # (geometry, flash tile T); T = 256 = one timestep per consumer thread only on `small`, where two such stages fit
 SWEEP_TILES = [("small", T) for T in (32, 64, 128, 192, 256)] + [("hs128", T) for T in (32, 64, 128, 160, 192)]
 SWEEP_SPLITS = [1, 2, 4, 8]
-# (geometry, weights, environment of the fast mode)
-CASES = [("hs16", "loud", {}), ("small", "synth", {}), ("small", "loud", {}), ("small-hs48", "loud", {}),
-         ("hs128", "loud", {}), ("small-qwen", "loud", {}), ("llama3-reduced", "loud", {}),
-         ("small-int8", "synth", {}), ("small-int8", "outliers", {}), ("small-tp-int8", "synth", {}),
-         ("llama2-7b-int8-2l", "outliers", {}),
-         ("qwen2.5-reduced", "synth", {}), ("tinyllama-1.1b", "synth", {})]
-KNOBS = ("KLLM_ENGINE", "KLLM_MODE", "KLLM_ATTN_SPLIT", "KLLM_STAGE_BYTES")
-
-
-def case_id(c):
-    return "-".join([c[0], c[1]] + [f"{k[5:].lower()}{v}" for k, v in c[2].items()])
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def all_ends(key):
@@ -189,116 +67,15 @@ def sweep_env(shape, T, sp):
     return {"KLLM_STAGE_BYTES": str(T * shape.head_size * 4), "KLLM_ATTN_SPLIT": str(sp)}
 
 
-_CACHE = {}
-
-
 @pytest.fixture(scope="module", autouse=True)
 def _free():
     yield
-    _CACHE.clear()
-    torch.cuda.empty_cache()
-
-
-def device_sincos(lib, shape):
-    sin = torch.empty(shape.seq_len, shape.head_size, device="cuda")
-    cos = torch.empty_like(sin)
-    assert lib.kllm_sincos_init(shape.head_size, shape.seq_len, FLAVOURS[shape.flavour], ptr(sin), ptr(cos),
-                                None) == 0
-    sync()
-    return sin, cos
-
-
-def sequence(vocab, n, seed):
-    toks = np.random.default_rng(seed).integers(0, vocab, n)
-    toks[:3] = (1, 0, vocab - 1)
-    return [int(t) for t in toks]
+    clear_cache()
 
 
 def model(lib, key, weights):
     """(shape, weights, tokens, plain model, fixed-point model or None); one geometry held at a time."""
-    if (key, weights) not in _CACHE:
-        _CACHE.clear()
-        torch.cuda.empty_cache()
-        shape = GEOMETRIES[key]
-        w = WEIGHTS[weights](shape, "cuda", 77)
-        toks = sequence(shape.vocab_size, shape.seq_len, 5)
-        sin, cos = device_sincos(lib, shape)
-        ends = all_ends(key)
-        plain = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends)
-        fixed = None
-        if shape.group_size:
-            fixed = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends, fixed_point=True)
-        _CACHE[(key, weights)] = (shape, w, toks, plain, fixed)
-    return _CACHE[(key, weights)]
-
-
-def make_decoder(monkeypatch, shape, w, numerics, env):
-    for name in KNOBS:
-        monkeypatch.delenv(name, raising=False)
-    monkeypatch.setenv("KLLM_ENGINE", "persistent")
-    for name, value in env.items():
-        monkeypatch.setenv(name, value)
-    dec = Decoder(shape, w, numerics=numerics)
-    assert dec.engine == "persistent"
-    return dec
-
-
-def kv_ratios(got, ref, tau, tau_first=KV_TAU_FIRST):
-    """Per-layer worst |got - ref| / (tau * rms(row)) over every position, for K and V; layer 0 against
-    tau_first."""
-    out = {}
-    for name, g, r in (("K", got[0], ref["k"]), ("V", got[1], ref["v"])):
-        g = torch.from_numpy(g).cuda().double()
-        rms = r.pow(2).mean(-1, keepdim=True).sqrt()
-        t = torch.full((r.shape[0], 1, 1), tau, dtype=torch.float64, device=r.device)
-        t[0] = tau_first
-        out[name] = [float(x) for x in ((g - r).abs() / (t * rms)).amax(dim=(1, 2))]
-    return out
-
-
-def logit_ratio(got, ref_logits, tau):
-    return float((torch.from_numpy(got).cuda().double() - ref_logits).abs().max()) / (
-        tau * float(ref_logits.pow(2).mean().sqrt()))
-
-
-def fmt(per_layer):
-    return {k: [float(f"{x:.3g}") for x in v] for k, v in per_layer.items()}
-
-
-def run(what, dec, shape, toks, ref, ends, kv_tau, logit_tau, plain=None):
-    """Teacher-force toks over every position in segments ending at `ends`; check the logits at each end and
-    every K / V row at the end.  Returns the cache."""
-    start, worst_logit, worst_end, worst_plain = 0, 0.0, 0, 0.0
-    for end in ends:
-        ids = dec.generate(0, start, end + 1 - start, teacher=toks[start:end + 1])
-        got = dec.logits()
-        lref = ref["logits_at"][end]
-        r = logit_ratio(got, lref, logit_tau)
-        if r > worst_logit:
-            worst_logit, worst_end = r, end
-        top2 = torch.topk(lref, 2).values
-        bound = logit_tau * float(lref.pow(2).mean().sqrt())
-        if float(top2[0] - top2[1]) > 2 * bound:
-            assert ids[-1] == int(torch.argmax(lref)), (what, end)
-        if plain is not None:
-            worst_plain = max(worst_plain, logit_ratio(got, plain["logits_at"][end], 1.0))
-        start = end + 1
-    assert start == shape.seq_len
-    kv = dec.kv_cache()
-    per_layer = kv_ratios(kv, ref, kv_tau)
-    report(what, f"segments {ends}")
-    report(what, f"logits err / bound {worst_logit:.3g}; K / V err / bound per layer {fmt(per_layer)}")
-    if plain is not None:
-        report(what, f"fixed point's cost, against the plain model: logits err / rms {worst_plain:.3g}; "
-                     f"K / V err / rms per layer {fmt(kv_ratios(kv, plain, 1.0, 1.0))}")
-    assert worst_logit <= 1.0, (what, worst_end, worst_logit)
-    for name, v in per_layer.items():
-        assert max(v) <= 1.0, (what, name, v)
-    return kv
-
-
-def taus(key):
-    return (KV_TAU_DEEP, LOGIT_TAU_DEEP) if key == "tinyllama-1.1b" else (KV_TAU, LOGIT_TAU)
+    return cached_model(lib, (key, weights), GEOMETRIES[key], weights, all_ends(key))
 
 
 @pytest.mark.parametrize("key,weights,env", CASES, ids=[case_id(c) for c in CASES])
@@ -313,7 +90,7 @@ def test_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env):
         dec = make_decoder(monkeypatch, shape, w, numerics, env if numerics == "fast" else {})
         ref = fixed if numerics == "fast" and fixed is not None else plain
         caches[numerics] = run(f"{what} {numerics}", dec, shape, toks, ref, ends, kv_tau, logit_tau,
-                               plain=plain if ref is fixed else None)
+                               plain=plain if ref is fixed else None)[0]
         dec.close()
     (ke, ve), (kf, vf) = caches["exact"], caches["fast"]
     same = [np.array_equal(a[l].view(np.uint32), b[l].view(np.uint32)) for a, b in ((ke, kf), (ve, vf))
@@ -341,7 +118,7 @@ def test_fast_decode_tiles_and_splits(kllm_lib, monkeypatch, key, T):
         assert flash_geometry(shape, env, sms()) == (T, sp)
         dec = make_decoder(monkeypatch, shape, w, "fast", env)
         caches[sp] = run(f"{key} loud fast T={T} SP={sp}", dec, shape, toks, plain,
-                         edge_ends(T, sp, shape.seq_len), KV_TAU, LOGIT_TAU)
+                         edge_ends(T, sp, shape.seq_len), KV_TAU, LOGIT_TAU)[0]
         dec.close()
     # the split took effect: layer 1's rows (after one layer of split attention) differ between SP = 1 and 4
     assert not np.array_equal(caches[1][0][1].view(np.uint32), caches[4][0][1].view(np.uint32)), (key, T)

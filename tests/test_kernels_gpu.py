@@ -5,6 +5,7 @@
   (b) the CPU oracle: within fp32 reassociation tolerance (written at each assert).
 Shapes follow the reference's tests (test_cu_*.cpp) plus the model shapes of BASELINE.json."""
 import ctypes
+import math
 
 import numpy as np
 import pytest
@@ -89,6 +90,57 @@ def test_matmul_w8_bit_exact(kllm_lib, ref, oracle, M, K):
         assert_bit_equal(out, oc, "gemv_w8 vs oracle cuda-order model")
         st = oracle.matmul_w8(x.cpu().numpy(), q.cpu().numpy(), s.cpu().numpy(), 64)
         assert np.abs(out.cpu().numpy() - st).max() < 1e-4
+
+
+U = 2.0 ** -24  # fp32 unit roundoff
+
+
+def w8_terms(x, q, s, group):
+    """x_i * s_g * q_i in fp64, [K, M], with g = e // group over the flattened matrix (export.py's groups: they
+    run across row ends when M % group != 0)."""
+    K, M = q.shape
+    e = torch.arange(K * M, device=q.device).reshape(K, M)
+    return x.double()[None, :] * s.double()[e // group] * q.double()
+
+
+def rows_around(threshold, step):
+    """Row counts just below and at a threshold, multiples of `step` (whole groups)."""
+    below = ((threshold - 1) // step) * step
+    return [below, -(-threshold // step) * step]
+
+
+# (group, in_dim): in_dim 1000 leaves a 104-element last chunk of 128 and, for every group but 8, groups that span
+# row ends; 1056 = 11 * 96 keeps the division path's groups inside rows; 14336 (> 12288 floats) opts in to more
+# than 48 KB of shared memory
+W8_GROUPS = [(8, 1000), (32, 1000), (64, 1000), (96, 1000), (96, 1056), (128, 1000), (256, 1000), (256, 14336)]
+
+
+@pytest.mark.parametrize("group,M", W8_GROUPS, ids=[f"g{g}-in{m}" for g, m in W8_GROUPS])
+def test_gemv_w8_groups_against_fp64(kllm_lib, group, M):
+    """kllm_gemv_w8 at other group sizes (shift path for powers of two, division path for 96) against the fp64
+    sum.  Bound from the kernel's order: fp32(x * s) is one rounding, each of the 128 virtual threads is a
+    ceil(M / 128)-long FFMA chain, and the block reduction a 7-level tree, so |out - sum| <= (ceil(M / 128) + 8) u
+    sum |x s q|.  Row counts on both sides of the 2- and 4-rows-per-warp switches (2 and 4 rows per warp of one
+    wave of 8-warp CTAs).  Worst measured error / bound 0.034 (group 64, in_dim 1000; NVIDIA H100 80GB HBM3)."""
+    from kuiperllama_b200.decoder import quantize_q80
+    wave = torch.cuda.get_device_properties(0).multi_processor_count * 8
+    step = group // math.gcd(group, M)  # K * M % group == 0: whole groups in the tensor
+    counts = [step * 3] + rows_around(2 * wave, step) + rows_around(4 * wave, step)
+    assert len(set(counts)) == 5
+    x = rnd(M, 50 + M)
+    worst = 0.0
+    for K in counts:
+        w = rnd((K, M), 51 + K, 0.02)
+        q, s = quantize_q80(w, group)
+        out = torch.zeros(K, device="cuda")
+        assert kllm_lib.kllm_gemv_w8(ptr(x), ptr(q), ptr(s), ptr(out), M, K, group, None) == 0
+        sync()
+        t = w8_terms(x, q, s, group)
+        err = (out.double() - t.sum(1)).abs()
+        ratio = float((err / ((math.ceil(M / 128) + 8) * U * t.abs().sum(1))).max())
+        worst = max(worst, ratio)
+        assert ratio <= 1.0, (group, M, K, ratio)
+    print(f"gemv_w8 g={group} in={M}: worst error / bound {worst:.3g}")
 
 
 # ---- rmsnorm ----------------------------------------------------------------------------------
@@ -214,6 +266,78 @@ def test_mha_decode(kllm_lib, ref, oracle, heads, kv_heads, head_size, seq_len, 
             oc, _ = oracle.mha(pos, heads, layer, seq_len, kv_dim, kv_mul, head_size, q.cpu().numpy(),
                                kc.cpu().numpy(), vc.cpu().numpy())
             assert np.abs(out.cpu().numpy() - oc).max() < 1e-5
+
+
+def mha_fp64(q, kc, vc, pos, layer, heads, kv_heads, head_size):
+    """Softmax attention of each query head over cache rows 0 .. pos of `layer`, in fp64.  Returns (out,
+    probabilities, sum_t p_t |v_t|, the largest sum_i |k_ti q_i| / sqrt(hs), the largest max_t s_t - s_t)."""
+    kv_mul = heads // kv_heads
+    k = kc[layer, :pos + 1].double().reshape(pos + 1, kv_heads, head_size).repeat_interleave(kv_mul, 1)
+    v = vc[layer, :pos + 1].double().reshape(pos + 1, kv_heads, head_size).repeat_interleave(kv_mul, 1)
+    qd = q.double().reshape(heads, head_size)
+    s = torch.einsum("thd,hd->ht", k, qd) / math.sqrt(head_size)
+    a = torch.einsum("thd,hd->ht", k.abs(), qd.abs()) / math.sqrt(head_size)
+    p = torch.softmax(s, -1)
+    out = torch.einsum("ht,thd->hd", p, v)
+    mag = torch.einsum("ht,thd->hd", p, v.abs())
+    spread = (s.amax(-1, keepdim=True) - s).amax(-1, keepdim=True)
+    return out, p, mag, a.amax(-1, keepdim=True), spread
+
+
+MHA_HEADS = [16, 32, 160, 188, 192, 256]
+
+
+@pytest.mark.parametrize("head_size", MHA_HEADS)
+def test_mha_decode_head_sizes_against_fp64(kllm_lib, head_size):
+    """kllm_mha_decode_f32 at GQA 3 (6 query heads over 2 kv heads) for every head size up to the 256 it accepts:
+    192 and 256 need more than 48 KB of shared memory for the q row and two value tiles.  Bound, first order in
+    u = 2^-24, from the kernel's order: a score is an hs-long FFMA chain times 1.f / sqrtf(hs) (two roundings),
+    rounded, so off by delta <= (hs + 3) u A with A = sum_i |k_i q_i| / sqrt(hs); the computed maximum only shifts
+    every exponent alike, which the normalisation cancels; the argument s_t - max is rounded (u times the spread)
+    and expf is within 2 ulp (4 u); a probability is then within 2 (delta + u spread + 4 u) of its share, plus the
+    sum (a ceil((pos + 1) / 256)-long strided chain and an 8-level tree) and the division; each output is a
+    (pos + 1)-long FFMA chain.  So |out - ref| <= u (pos + 1 + 2 (hs + 3) A + 2 spread + ceil((pos + 1) / 256) + 20)
+    sum_t p_t |v_t|.  q at std 3 makes the softmax peaked (scores of std ~3).  Worst measured error / bound 0.030
+    (head_size 16; 0.002 to 0.005 from 160 up; NVIDIA H100 80GB HBM3)."""
+    heads, kv_heads, seq_len, L, layer = 6, 2, 520, 2, 1
+    kv_dim = kv_heads * head_size
+    kc = rnd((L, seq_len, kv_dim), 60 + head_size)
+    vc = rnd((L, seq_len, kv_dim), 61 + head_size)
+    sc = torch.zeros(heads * seq_len, device="cuda")
+    worst = 0.0
+    for pos in (0, 1, 31, 32, 33, 255, 256, seq_len - 1):
+        q = rnd(heads * head_size, 62 + pos, 3.0)
+        out = torch.full((heads * head_size,), float("nan"), device="cuda")
+        assert kllm_lib.kllm_mha_decode_f32(pos, heads, layer, seq_len, kv_dim, 3, head_size, ptr(out), ptr(q),
+                                            ptr(sc), ptr(kc), ptr(vc), None) == 0
+        sync()
+        ref, p, mag, a, spread = mha_fp64(q, kc, vc, pos, layer, heads, kv_heads, head_size)
+        soft = 2 * (head_size + 3) * a + 2 * spread + math.ceil((pos + 1) / 256) + 20
+        terms = pos + 1 + soft
+        ratio = float(((out.double().reshape(heads, head_size) - ref).abs() / (U * terms * mag)).max())
+        worst = max(worst, ratio)
+        assert ratio <= 1.0, (head_size, pos, ratio)
+        # the probabilities the kernel leaves in the score buffer: the same first-order terms, output chain aside
+        pk = sc.view(heads, seq_len)[:, :pos + 1].double()
+        pb = U * soft * p
+        assert bool(((pk - p).abs() <= pb).all()), (head_size, pos)
+    print(f"mha hs={head_size}: worst error / bound {worst:.3g}")
+
+
+def test_mha_decode_refuses_head_size_above_256(kllm_lib):
+    """head_size 260: the kernel's output chains are threads < head_size of a 256-thread CTA.  The launch and a
+    decoder built with that head size both refuse it."""
+    from kuiperllama_b200 import Decoder, KllmError, ModelShape, synth_weights
+    hs, heads, seq_len = 260, 2, 8
+    kc = torch.zeros((1, seq_len, heads * hs), device="cuda")
+    q = torch.zeros(heads * hs, device="cuda")
+    out = torch.zeros_like(q)
+    sc = torch.zeros(heads * seq_len, device="cuda")
+    assert kllm_lib.kllm_mha_decode_f32(0, heads, 0, seq_len, heads * hs, 1, hs, ptr(out), ptr(q), ptr(sc),
+                                        ptr(kc), ptr(kc), None) == -2  # KLLM_E_UNSUPPORTED
+    shape = ModelShape("hs260", heads * hs, 1024, 1, heads, heads, 256, seq_len)
+    with pytest.raises(KllmError, match=r"kllm_decoder_create failed: -2\b"):
+        Decoder(shape, synth_weights(shape, "cuda", 1))
 
 
 # ---- embedding / argmax -----------------------------------------------------------------------------

@@ -5,6 +5,8 @@
 2. With TF32 rounding off, prefill_ref is the plain fp32 model: over the golden checkpoints it must give the
    CPU oracle's K / V cache rows and last logits (oracle/kuiper_oracle.c stepping one position at a time)
    within 1e-5.  fp64 against fp32 arithmetic in other orders differs by a few 1e-7 here (|logits| <= 1.4).
+   The same over synthetic int8 checkpoints at groups of 32, 96 and 128, and of 64 over rows of 96 and 160
+   elements (groups that span row ends).
 3. A prompt modelled in chunks (start_pos > 0 with the earlier rows as kv_in) equals one call.
 """
 import numpy as np
@@ -13,6 +15,8 @@ import torch
 
 from conftest import GOLDEN
 from prefill_model import dequant_w8, gemm_ref, prefill_ref, tf32_rna
+
+from kuiperllama_b200 import ModelShape, synth_weights
 
 
 def bits(*u):
@@ -106,6 +110,40 @@ def test_prefill_ref_without_tf32_matches_the_cpu_oracle(oracle, name, quant, fl
     n = len(toks)
     assert np.abs(r["k"].numpy() - k_o[:, :n]).max() < 1e-5
     assert np.abs(r["v"].numpy() - v_o[:, :n]).max() < 1e-5
+    assert np.abs(r["logits"].numpy() - logits).max() < 1e-5
+    assert r["next"] == nxt
+
+
+# int8 checkpoints at group sizes other than the goldens' 64, written with write_checkpoint
+INT8_GROUPS = [
+    ModelShape("int8-g32", 128, 384, 2, 4, 2, 256, 24, group_size=32),
+    ModelShape("int8-g96", 192, 384, 2, 4, 2, 256, 24, group_size=96),  # 96: not a power of two
+    ModelShape("int8-g128", 256, 512, 2, 4, 2, 256, 24, group_size=128),
+    # 96 % 64 and 160 % 64 != 0: groups run across row ends (over the flattened tensor, as export.py writes them)
+    ModelShape("int8-g64-rowspan", 96, 160, 2, 3, 1, 512, 24, group_size=64),
+]
+
+
+@pytest.mark.parametrize("shape", INT8_GROUPS, ids=[s.name for s in INT8_GROUPS])
+def test_prefill_ref_at_other_group_sizes_matches_the_cpu_oracle(oracle, tmp_path, shape):
+    """dequant_w8's scale index against the oracle's (scales[idx / group_size] over each tensor), stepping every
+    position of a synthetic checkpoint."""
+    from kuiperllama_b200.checkpoint import write_checkpoint
+    w = synth_weights(shape, "cpu", 77)
+    path = tmp_path / f"{shape.name}.bin"
+    write_checkpoint(str(path), shape, w)
+    toks = [int(t) for t in np.random.default_rng(5).integers(0, shape.vocab_size, shape.seq_len)]
+    om = oracle.open_model(path, True, "llama2")
+    try:
+        for t, tok in enumerate(toks):
+            nxt, logits = om.step(tok, t)
+        k_o, v_o = (a.copy() for a in om.kv_cache())
+    finally:
+        om.close()
+    sin, cos = oracle.sincos(shape.head_size, shape.seq_len, "llama2")
+    r = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False)
+    assert np.abs(r["k"].numpy() - k_o).max() < 1e-5
+    assert np.abs(r["v"].numpy() - v_o).max() < 1e-5
     assert np.abs(r["logits"].numpy() - logits).max() < 1e-5
     assert r["next"] == nxt
 
