@@ -62,7 +62,7 @@ class DecoderDesc(ctypes.Structure):
         ("bq", POINTER(c_void_p)), ("bk", POINTER(c_void_p)), ("bv", POINTER(c_void_p)),
         ("tp_size", c_int32), ("tp_rank", c_int32),
         ("allreduce", ALLREDUCE_FN), ("allreduce_ctx", c_void_p), ("comm", c_void_p),
-        ("numerics", c_int32),
+        ("numerics", c_int32), ("kv_cache", c_int32),
     ]
 
 

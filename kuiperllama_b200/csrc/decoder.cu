@@ -352,6 +352,7 @@ int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int3
   m.kv_head_num = d.kv_head_num, m.vocab_size = d.vocab_size, m.seq_len = d.seq_len, m.head_size = hs;
   m.flavour = d.flavour, m.mega_layout = dc->use_mega ? 1 : 0, m.eps = flavour_eps(d.flavour);
   m.attn_split = dc->use_mega ? dc->mega.attn_vsplit() : 1;
+  m.kv_bf16 = d.kv_cache == KLLM_KV_BF16 ? 1 : 0;
   m.tok_emb = d.tok_emb, m.attn_norm = dc->attn_norm.data(), m.ffn_norm = dc->ffn_norm.data();
   m.wq = dc->wq.data(), m.wk = dc->wk.data(), m.wv = dc->wv.data(), m.wo = dc->wo.data();
   m.w1 = dc->w1.data(), m.w2 = dc->w2.data(), m.w3 = dc->w3.data();
@@ -427,6 +428,13 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
   // head_size from the FULL model: dim / (head_num * tp)
   if (d.dim % (d.head_num * tp) != 0 || d.head_num % d.kv_head_num != 0) return KLLM_E_INVALID;
   if ((d.dim & 3) != 0 || (d.hidden_dim & 3) != 0) return KLLM_E_UNSUPPORTED;
+  if (d.kv_cache != KLLM_KV_F32 && d.kv_cache != KLLM_KV_BF16) return KLLM_E_INVALID;
+  // a bf16 cache exists on the persistent engine's flash form only; the rest of the refusals come from its init
+  const bool kv_bf16 = d.kv_cache == KLLM_KV_BF16;
+  const char* want = getenv("KLLM_ENGINE");
+  const bool force_graph = want != nullptr && strcmp(want, "graph") == 0;
+  const bool force_mega = want != nullptr && strcmp(want, "persistent") == 0;
+  if (kv_bf16 && (tp > 1 || force_graph)) return KLLM_E_UNSUPPORTED;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return KLLM_E_NODEVICE;
 
@@ -475,11 +483,12 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     return static_cast<int>(cudaMemsetAsync(*p, 0, n * sizeof(float), dc->stream));
   };
   const size_t kv_elems = static_cast<size_t>(L) * d.seq_len * dc->kv_dim;
+  const size_t kv_floats = kv_bf16 ? (kv_elems + 1) / 2 : kv_elems;  // bf16: half the bytes behind the same pointers
   const int q_rows = d.head_num * dc->head_size;
   if (dev_alloc(&dc->x, d.dim) || dev_alloc(&dc->q, q_rows) || dev_alloc(&dc->attn, q_rows) ||
       dev_alloc(&dc->h, d.hidden_dim) || dev_alloc(&dc->logits, d.vocab_size) ||
       dev_alloc(&dc->score, static_cast<size_t>(d.head_num) * d.seq_len) ||
-      dev_alloc(&dc->kcache, kv_elems) || dev_alloc(&dc->vcache, kv_elems) ||
+      dev_alloc(&dc->kcache, kv_floats) || dev_alloc(&dc->vcache, kv_floats) ||
       dev_alloc(&dc->sin_t, static_cast<size_t>(d.seq_len) * dc->head_size) ||
       dev_alloc(&dc->cos_t, static_cast<size_t>(d.seq_len) * dc->head_size) ||
       dev_alloc(&dc->tp_tmp, d.dim) || dev_alloc(&dc->penalized, d.vocab_size) ||
@@ -522,10 +531,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
   // Engine: the persistent megakernel (one cooperative launch per run) when the shape fits its
   // shared-memory ring, else the CUDA-graph chain of fused launches.  KLLM_ENGINE=graph|persistent
   // forces one (persistent fails loudly if unsupported).  Both are CUDA; neither is a fallback to
-  // anything off-device.
-  const char* want = getenv("KLLM_ENGINE");
-  const bool force_graph = want != nullptr && strcmp(want, "graph") == 0;
-  const bool force_mega = want != nullptr && strcmp(want, "persistent") == 0;
+  // anything off-device.  A bf16 cache never falls back to the graph engine.
   // tensor parallel: the persistent engine needs the peer-memory transport (its exchange IS
   // the all-reduce); with NCCL or a caller-supplied callback the graph engine is used
   unsigned long long* tp_areas[8] = {};
@@ -539,6 +545,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     MegaModel mm{};
     mm.tp_world = tp, mm.tp_rank = tp_rank, mm.tp_stride = tp_stride;
     mm.numerics = d.numerics;
+    mm.kv_cache = d.kv_cache;
     for (int r = 0; r < 8; ++r) mm.tp_data[r] = tp_areas[r];
     mm.dim = d.dim, mm.hidden_dim = d.hidden_dim, mm.layer_num = L, mm.head_num = d.head_num;
     mm.kv_head_num = d.kv_head_num, mm.vocab_size = d.vocab_size, mm.seq_len = d.seq_len;
@@ -564,10 +571,10 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     if (rc == 0) {
       dc->use_mega = true;
       dc->launches_per_step = 1;
-    } else if (rc != KLLM_E_UNSUPPORTED || force_mega) {
+    } else if (rc != KLLM_E_UNSUPPORTED || force_mega || kv_bf16) {
       return fail(rc);
     }
-  } else if (force_mega) {
+  } else if (force_mega || kv_bf16) {
     return fail(KLLM_E_UNSUPPORTED);
   }
   if (!dc->use_mega) {
@@ -939,7 +946,7 @@ int kllm_decoder_profile(kllm_decoder* dc, int32_t first_token, int32_t start_po
                          int32_t profiled_step, uint64_t* stamps_host, int32_t capacity,
                          int32_t* grid_out, int32_t* phases_out) {
   if (!dc || !stamps_host || !grid_out || !phases_out || n_steps <= 0) return KLLM_E_INVALID;
-  if (!dc->use_mega) return KLLM_E_UNSUPPORTED;
+  if (!dc->use_mega || dc->d.kv_cache == KLLM_KV_BF16) return KLLM_E_UNSUPPORTED;  // no bf16-cache timeline kernel
   if (start_pos < 0 || start_pos + n_steps > dc->d.seq_len) return KLLM_E_INVALID;
   const int grid = dc->mega.grid(), phases = dc->mega.phases();
   const size_t n = static_cast<size_t>(grid) * phases * mega::kProfStamps;
@@ -979,11 +986,35 @@ int kllm_decoder_read_kv(kllm_decoder* dc, float* key_host, float* value_host) {
     KLLM_TRY(cudaMemcpy(key_host, dc->kcache, n * sizeof(float), cudaMemcpyDeviceToHost));
     return static_cast<int>(cudaMemcpy(value_host, dc->vcache, n * sizeof(float), cudaMemcpyDeviceToHost));
   }
+  const size_t nh = kvd / hs;
+  if (dc->d.kv_cache == KLLM_KV_BF16) {
+    // bf16: K [L][kvh][hs/8][S][8], V [L][kvh][S][hs] -> reference [L][S][kv_dim], each element widened exactly
+    std::vector<uint16_t> kraw(n), vraw(n);
+    KLLM_TRY(cudaMemcpy(kraw.data(), dc->kcache, n * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+    KLLM_TRY(cudaMemcpy(vraw.data(), dc->vcache, n * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+    auto widen = [](uint16_t b) {
+      const uint32_t u = static_cast<uint32_t>(b) << 16;
+      float f;
+      std::memcpy(&f, &u, sizeof(f));
+      return f;
+    };
+    for (size_t l = 0; l < L; ++l)
+      for (size_t g = 0; g < nh; ++g) {
+        const uint16_t* kb = kraw.data() + (l * nh + g) * S * hs;
+        const uint16_t* vb = vraw.data() + (l * nh + g) * S * hs;
+        for (size_t t = 0; t < S; ++t)
+          for (size_t i = 0; i < hs; ++i) {
+            const size_t dst = (l * S + t) * kvd + g * hs + i;
+            key_host[dst] = widen(kb[((i >> 3) * S + t) * 8 + (i & 7)]);
+            value_host[dst] = widen(vb[t * hs + i]);
+          }
+      }
+    return 0;
+  }
   // persistent engine: K [L][kvh][hs/4][S][4], V [L][kvh][SP][S][hs/SP] -> reference [L][S][kv_dim]
   std::vector<float> kraw(n), vraw(n);
   KLLM_TRY(cudaMemcpy(kraw.data(), dc->kcache, n * sizeof(float), cudaMemcpyDeviceToHost));
   KLLM_TRY(cudaMemcpy(vraw.data(), dc->vcache, n * sizeof(float), cudaMemcpyDeviceToHost));
-  const size_t nh = kvd / hs;
   const size_t SP = static_cast<size_t>(dc->mega.attn_vsplit()), dv = hs / SP;
   for (size_t l = 0; l < L; ++l)
     for (size_t g = 0; g < nh; ++g) {

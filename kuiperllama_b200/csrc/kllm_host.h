@@ -43,6 +43,7 @@ struct PrefillModel {
   int dim, hidden_dim, layer_num, head_num, kv_head_num, vocab_size, seq_len, head_size, flavour;
   int mega_layout;  // 1: the persistent engine's head-major K / V cache layout (megakernel.cu)
   int attn_split;   // ... whose V rows are cut into attn_split slices of head_size / attn_split dims
+  int kv_bf16;      // 1: that layout in bf16 (K [kvh][hs/8][seq][8], V [kvh][seq][hs]); the caches hold bf16
   float eps;
   const float* tok_emb;
   const float* const* attn_norm;

@@ -37,6 +37,7 @@
 // dot product, reduction tree, softmax sum and value chain reproduces the reference CUDA
 // kernels' floating-point order, so logits stay bit-identical to the reference's CUDA path.
 #include <cooperative_groups.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
 #include <cfloat>
@@ -344,6 +345,15 @@ __device__ __forceinline__ float lds_f32(uint32_t a) {
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
   return v;
 }
+// bf16 KV cache: an element widened exactly to fp32 (the bf16 bits are the float's upper half)
+__device__ __forceinline__ float lds_bf16(uint32_t a) {
+  unsigned short v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(a));
+  return __uint_as_float(static_cast<uint32_t>(v) << 16);
+}
+// the two bf16 elements of a 32-bit word (held as a float's bits): element 2i in the low half, 2i + 1 in the high
+__device__ __forceinline__ float bf16_lo(float w) { return __uint_as_float(__float_as_uint(w) << 16); }
+__device__ __forceinline__ float bf16_hi(float w) { return __uint_as_float(__float_as_uint(w) & 0xffff0000u); }
 
 // fp32: virtual thread (lane + 32 j) owns packs base + 32 j + lane (matmul_kernel.cu:27-35).  The
 // NR rows of a task share each load of x; per batch (two 32-pack columns) 2 x loads and 2 NR weight
@@ -711,10 +721,11 @@ __device__ __forceinline__ AttnIn poll_attention_inputs(const unsigned long long
 }
 
 // RoPE on q (this head) and -- with_k -- on the new key row (rope_kernel.cu as compiled, elementwise.cu); the
-// rotated key goes to k_s and, by one CTA per kv head, into the cache row of `pos`.  Returns this thread's
-// element of the value row (with_v, tid < hs), else 0.
+// rotated key goes to k_s and, by one CTA per kv head, into the cache row of `pos` (rounded to bf16 with
+// KV16, the bf16 KV cache).  Returns this thread's element of the value row (with_v, tid < hs), else 0.
+template <bool KV16 = false>
 __device__ __forceinline__ float attention_inputs(const Params& P, const Phase& ph, int head, int kvh, int pos, unsigned tag_in,
-                                                  bool with_k, bool with_v, float* q_s, float* k_s, float* kcache) {
+                                                  bool with_k, bool with_v, float* q_s, float* k_s, size_t head_block) {
   const int tid = threadIdx.x;
   const int hs = P.head_size, seq_len = P.seq_len;
   const bool need_q = tid < hs / 2, need_k = need_q && with_k, need_v = with_v && tid < hs;
@@ -743,8 +754,15 @@ __device__ __forceinline__ float attention_inputs(const Params& P, const Phase& 
       k_s[i0] = r0;
       k_s[i1] = r1;
       if (head % P.kv_mul == 0) {  // one writer per kv head stores the rotated key
-        kcache[(static_cast<size_t>(i0 >> 2) * seq_len + pos) * 4 + (i0 & 3)] = r0;
-        kcache[(static_cast<size_t>(i1 >> 2) * seq_len + pos) * 4 + (i1 & 3)] = r1;
+        if constexpr (KV16) {
+          __nv_bfloat16* kcache = reinterpret_cast<__nv_bfloat16*>(P.key_cache) + head_block;
+          kcache[(static_cast<size_t>(i0 >> 3) * seq_len + pos) * 8 + (i0 & 7)] = __float2bfloat16_rn(r0);
+          kcache[(static_cast<size_t>(i1 >> 3) * seq_len + pos) * 8 + (i1 & 7)] = __float2bfloat16_rn(r1);
+        } else {
+          float* kcache = P.key_cache + head_block;
+          kcache[(static_cast<size_t>(i0 >> 2) * seq_len + pos) * 4 + (i0 & 3)] = r0;
+          kcache[(static_cast<size_t>(i1 >> 2) * seq_len + pos) * 4 + (i1 & 3)] = r1;
+        }
       }
     }
   }
@@ -767,6 +785,8 @@ __device__ __forceinline__ float attention_inputs(const Params& P, const Phase& 
 //       is a conflict-free 128-bit shared-memory access (consecutive t -> consecutive 16 B);
 //   V [L][kv_head][SP][seq_len][dv]           -- a tile of T timesteps of one slice is one contiguous
 //       block and "thread i walks column i" is conflict-free.
+//   bf16 KV cache (flash form, SP layout 1): K [L][kv_head][head_size/8][seq_len][8] and V [L][kv_head][seq_len]
+//       [head_size] in bf16 -- still 16-byte chunks and contiguous V rows, half the bytes.
 // Rows t < pos were written by earlier tokens, so -- like weights -- the producer warp streams
 // them through the ring ahead of time; only row pos is handled here from registers.
 __device__ __forceinline__ int attn_tiles(int pos, int T) { return (pos + T - 1) / T; }
@@ -849,7 +869,6 @@ __device__ KLLM_PHASE_CALL Pipe attention_fused_phase(const Params& P, int head,
   float* k_s = ws + hs;  // [hs] rotated key of the current position
   const int kvh = head / P.kv_mul;
   const size_t head_block = (static_cast<size_t>(ph.layer) * (P.kv_dim / hs) + kvh) * seq_len * hs;
-  float* kcache = P.key_cache + head_block;
   // scores / probabilities: shared memory when the context fits the workspace (the ring leaves
   // almost no L1), else the global [head][seq_len] buffer the reference uses
   const int smem_cap = (P.xbuf_bytes >> 2) - 2 * hs;
@@ -857,7 +876,7 @@ __device__ KLLM_PHASE_CALL Pipe attention_fused_phase(const Params& P, int head,
   float* score_head = score_in_smem ? (ws + 2 * hs) : (P.score + static_cast<size_t>(head) * seq_len);
 
   // q, the new key row (rotated) and the value row of the current position (QKV phase of this token)
-  const float v_pos = attention_inputs(P, ph, head, kvh, pos, tag_in, true, true, q_s, k_s, kcache);
+  const float v_pos = attention_inputs(P, ph, head, kvh, pos, tag_in, true, true, q_s, k_s, head_block);
   consumer_sync<CT>();
   const long long c_rope = stamp ? clock64() : 0;
 
@@ -1010,10 +1029,9 @@ __device__ KLLM_PHASE_CALL Pipe attention_scores_phase(const Params& P, int head
   float* k_s = ws + hs;  // [hs] rotated key of the current position
   const int kvh = head / P.kv_mul;
   const size_t head_block = (static_cast<size_t>(ph.layer) * (P.kv_dim / hs) + kvh) * seq_len * hs;
-  float* kcache = P.key_cache + head_block;
   unsigned long long* sc_out = P.scores + static_cast<size_t>(head) * seq_len;
   // q and -- in the CTA that scores it -- the new key row, rotated (the value row is the P.V phase's business)
-  attention_inputs(P, ph, head, kvh, pos, tag_in, split == 0, false, q_s, k_s, kcache);
+  attention_inputs(P, ph, head, kvh, pos, tag_in, split == 0, false, q_s, k_s, head_block);
   consumer_sync<CT>();
   const long long c_rope = stamp ? clock64() : 0;
 
@@ -1200,11 +1218,14 @@ __device__ KLLM_PHASE_CALL Pipe attention_pv_phase(const Params& P, int head, in
 //            the quarters, three more give the block's maximum and sum -> running (m, l) of the warp;
 //   P.V      lane owns output dims lane, lane + 32, ...: o[d] = o[d] alpha + sum_tt p_tt v[tt][d] with p_tt
 //            shuffled from lane tt (conflict-free 32-bit reads of the V tile [T][hs]).
+// bf16 KV cache (KV16): the same mapping over tiles of half the bytes -- a 16-byte K chunk is 8 dims of a
+// timestep (K tile [hs/8][T][8], so a quarter of the head is hs/32 chunks) and the V tile is [T][hs] bf16;
+// every element is widened exactly to fp32 and the arithmetic is unchanged.
 // At the end the CW warp partials (m, l, o[hs]) are merged through shared memory, CTA 0 of the head folds
 // in the current position's row from registers and merges the partials of the other CTAs that had
 // tiles (tagged words in the scores area: [head][s][hs + 2]); at short contexts (pos <= T) that is
 // nobody, and the phase costs what the fused one does.
-template <int CW>
+template <int CW, bool KV16>
 __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head, int split, int pos, Pipe pipe,
                                                        unsigned tag_in, unsigned tag_out, unsigned long long* stamp) {
   const Phase& ph = g_ph_cons;
@@ -1226,9 +1247,8 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
   float* red = ws + 2 * hs;       // [CW][hs + 2] warp partials: m, l, o[hs]
   const int kvh = head / P.kv_mul;
   const size_t head_block = (static_cast<size_t>(ph.layer) * (P.kv_dim / hs) + kvh) * seq_len * hs;
-  float* kcache = P.key_cache + head_block;
   // q, and in CTA 0 of the head the new key row (rotated) and the value row of the current position
-  const float v_pos = attention_inputs(P, ph, head, kvh, pos, tag_in, split == 0, split == 0, q_s, k_s, kcache);
+  const float v_pos = attention_inputs<KV16>(P, ph, head, kvh, pos, tag_in, split == 0, split == 0, q_s, k_s, head_block);
   consumer_sync<CT>();
   const long long c_rope = stamp ? clock64() : 0;
 
@@ -1257,7 +1277,21 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
       const int tl = b * 8 + tt;  // this lane's timestep within the tile
       const bool valid = tl < nt;
       float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-      if (valid) {
+      if (KV16 && valid) {  // chunk c = dims 8c .. 8c + 7 of the timestep, 8 bf16 (host: head_size % 32 == 0)
+#pragma unroll 2
+        for (int c = cg * (cpg >> 1); c < (cg + 1) * (cpg >> 1); ++c) {
+          const float4 kw = lds_f4(ktile + static_cast<uint32_t>(c * T + tl) * 16u);
+          const float4 qa = q4[2 * c], qb = q4[2 * c + 1];
+          a0 = __fmaf_rn(bf16_lo(kw.x), qa.x, a0);
+          a1 = __fmaf_rn(bf16_hi(kw.x), qa.y, a1);
+          a2 = __fmaf_rn(bf16_lo(kw.y), qa.z, a2);
+          a3 = __fmaf_rn(bf16_hi(kw.y), qa.w, a3);
+          a0 = __fmaf_rn(bf16_lo(kw.z), qb.x, a0);
+          a1 = __fmaf_rn(bf16_hi(kw.z), qb.y, a1);
+          a2 = __fmaf_rn(bf16_lo(kw.w), qb.z, a2);
+          a3 = __fmaf_rn(bf16_hi(kw.w), qb.w, a3);
+        }
+      } else if (valid) {
 #pragma unroll 4
         for (int c = cg * cpg; c < (cg + 1) * cpg; ++c) {
           const float4 kv = lds_f4(ktile + static_cast<uint32_t>(c * T + tl) * 16u);
@@ -1290,13 +1324,19 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
       // P.V of the block
       const int nv = min(8, nt - b * 8);
       float acc[4] = {0.f, 0.f, 0.f, 0.f};
-      const uint32_t vrow = vtile + static_cast<uint32_t>(b * 8 * hs + lane) * 4u;
+      // element (timestep, dim) of the V tile [T][hs] at byte (timestep * hs + dim) << esh: the 32 lanes read
+      // 32 consecutive elements, conflict-free in either width
+      constexpr uint32_t esh = KV16 ? 1u : 2u;
+      const uint32_t vrow = vtile + (static_cast<uint32_t>(b * 8 * hs + lane) << esh);
       for (int k = 0; k < nv; ++k) {
         const float pk = __shfl_sync(kFull, pr, k);
-        const uint32_t va = vrow + static_cast<uint32_t>(k * hs) * 4u;
+        const uint32_t va = vrow + (static_cast<uint32_t>(k * hs) << esh);
 #pragma unroll
         for (int i = 0; i < 4; ++i)
-          if (lane + 32 * i < hs) acc[i] = __fmaf_rn(pk, lds_f32(va + 128u * i), acc[i]);
+          if (lane + 32 * i < hs) {
+            const uint32_t a = va + ((32u * i) << esh);
+            acc[i] = __fmaf_rn(pk, KV16 ? lds_bf16(a) : lds_f32(a), acc[i]);
+          }
       }
 #pragma unroll
       for (int i = 0; i < 4; ++i) o[i] = __fmaf_rn(o[i], alpha, acc[i]);
@@ -1634,7 +1674,7 @@ __device__ __forceinline__ void record_fed(const Params& P, int pos, int token) 
 // Stages the phase's input vector (tagged residual exchange / tagged hand-off / embedding row) into
 // shared memory, RMS-normalises it when the phase asks for it, consumes this CTA's ring stages
 // task by task, runs the epilogues and, for the classifier, leaves the CTA's (max, index).
-template <int CW, bool INT8, bool PROF, bool LP>
+template <int CW, bool INT8, bool PROF, bool LP, bool KV16>
 __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int tok, int pos, const float* emb_row,
                                             unsigned long long* stamp) {
   constexpr int CT = CW * 32;
@@ -1798,10 +1838,14 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
     if (sg.bias != nullptr) v = __fadd_rn(v, bias_v);       // matmul.cpp:74-77: out + bias
     if (sg.tag_out != nullptr) st_tagged_gpu(sg.tag_out + rr.row, v, hand_tag(ph.hand_out));
     if (sg.out == nullptr) {
-    } else if (sg.head_major) {  // value cache [kv_head][SP][seq_len][dv]
+    } else if (sg.head_major) {  // value cache [kv_head][SP][seq_len][dv], bf16 elements with KV16
       const int hs = P.head_size, dv = hs / P.attn_vsplit;
       const int kvh = rr.row / hs, d = rr.row % hs;
-      sg.out[((static_cast<size_t>(kvh) * P.attn_vsplit + d / dv) * P.seq_len + pos) * dv + d % dv] = v;
+      const size_t at = ((static_cast<size_t>(kvh) * P.attn_vsplit + d / dv) * P.seq_len + pos) * dv + d % dv;
+      if constexpr (KV16)
+        reinterpret_cast<__nv_bfloat16*>(sg.out)[at] = __float2bfloat16_rn(v);
+      else
+        sg.out[at] = v;
     } else {
       sg.out[static_cast<long long>(pos) * sg.pos_stride + rr.row] = v;
     }
@@ -2060,7 +2104,8 @@ __device__ __noinline__ int draw_with_logprobs(const Params& P, int pos, int ste
 // ---- the kernel ---------------------------------------------------------------------------------
 // LP: the logprob_megakernel instantiation, launched while log-probabilities are on.  decode_megakernel (LP false)
 // compiles to the code it has without the feature: the off path adds nothing to it, not even a test.
-template <int CW, bool INT8, bool PROF, bool LP>
+// KV16: the bf16 KV cache (kv16_megakernel), fast numerics' flash form only; the same holds for it.
+template <int CW, bool INT8, bool PROF, bool LP, bool KV16>
 __device__ __forceinline__ void megakernel_body(const Params& P) {
   constexpr int CT = CW * 32;  // consumer threads
   uint64_t* full_bar = g_full_bar;
@@ -2133,9 +2178,11 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
           const size_t head_block =
               (static_cast<size_t>(ph.layer) * (P.kv_dim / hs) + kvh) * P.seq_len * hs;
           if (ph.kind == kPhaseAttnFlash) {  // tiles j = split, split + SP, ...: K tile, then V tile
-            const int T = P.attn_tile;
-            const float* kbase = P.key_cache + head_block;
-            const float* vbase = P.value_cache + head_block;
+            // K: hs * esz / 16 chunk columns of 16 bytes (4 fp32 or 8 bf16 dims) per timestep; V: rows of hs * esz
+            constexpr int esz = KV16 ? 2 : 4;
+            const int T = P.attn_tile, row_bytes = hs * esz;
+            const unsigned char* kbase = reinterpret_cast<const unsigned char*>(P.key_cache) + head_block * esz;
+            const unsigned char* vbase = reinterpret_cast<const unsigned char*>(P.value_cache) + head_block * esz;
             const int n_tiles = attn_tiles(ppos, T);
             for (int j = split; j < n_tiles; j += SP) {
               const int t0 = j * T;
@@ -2143,15 +2190,15 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
               for (int kv = 0; kv < 2; ++kv) {
                 if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
                 unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
-                if (lane == 0) mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(nt) * hs * 4);
+                if (lane == 0) mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(nt) * row_bytes);
                 __syncwarp();
                 if (kv == 0) {
-                  if (lane < (hs >> 2))
+                  if (lane < (row_bytes >> 4))
                     bulk_g2s(dst + static_cast<size_t>(lane) * T * 16,
-                             kbase + (static_cast<size_t>(lane) * P.seq_len + t0) * 4,
+                             kbase + (static_cast<size_t>(lane) * P.seq_len + t0) * 16,
                              static_cast<uint32_t>(nt) * 16, &full_bar[pipe.slot], policy_kv);
                 } else if (lane == 0) {
-                  bulk_g2s(dst, vbase + static_cast<size_t>(t0) * hs, static_cast<uint32_t>(nt) * hs * 4,
+                  bulk_g2s(dst, vbase + static_cast<size_t>(t0) * row_bytes, static_cast<uint32_t>(nt) * row_bytes,
                            &full_bar[pipe.slot], policy_kv);
                 }
                 pipe.advance(S);
@@ -2306,7 +2353,7 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
         const int SP = P.attn_split;
         if (cta < P.head_num * SP) {
           if (ph.kind == kPhaseAttnFlash)
-            pipe = attention_flash_phase<CW>(P, cta / SP, cta % SP, pos, pipe, hand_tag(ph.hand_in), hand_tag(ph.hand_out), stamp);
+            pipe = attention_flash_phase<CW, KV16>(P, cta / SP, cta % SP, pos, pipe, hand_tag(ph.hand_in), hand_tag(ph.hand_out), stamp);
           else if (ph.kind == kPhaseAttnFused)
             pipe = attention_fused_phase<CW>(P, cta, pos, pipe, hand_tag(ph.hand_in), hand_tag(ph.hand_out), stamp);
           else if (ph.kind == kPhaseAttention)
@@ -2320,7 +2367,7 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
         // A prompt token (llama3.cpp:733-745: predict(..., is_prompt = true) discards the logits and
         // returns -1) skips the classifier -- its weights are not even streamed -- but keeps the grid
         // barrier that closes the token.
-        const Carry out = gemv_phase<CW, INT8, PROF, LP>(P, Carry{pipe, best.v, best.i}, tok, pos, emb_row, stamp);
+        const Carry out = gemv_phase<CW, INT8, PROF, LP, KV16>(P, Carry{pipe, best.v, best.i}, tok, pos, emb_row, stamp);
         pipe = out.pipe;
         best.v = out.best_v, best.i = out.best_i;
       }
@@ -2392,12 +2439,18 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
 
 template <int CW, bool INT8, bool PROF>
 __global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __grid_constant__ Params P) {
-  megakernel_body<CW, INT8, PROF, false>(P);
+  megakernel_body<CW, INT8, PROF, false, false>(P);
 }
 
 template <int CW, bool INT8>
 __global__ void __launch_bounds__(CW * 32 + 32, 1) logprob_megakernel(const __grid_constant__ Params P) {
-  megakernel_body<CW, INT8, false, true>(P);
+  megakernel_body<CW, INT8, false, true, false>(P);
+}
+
+// The bf16 KV cache's instantiations, with (LP) and without log-probabilities; no profiling one.
+template <int CW, bool INT8, bool LP>
+__global__ void __launch_bounds__(CW * 32 + 32, 1) kv16_megakernel(const __grid_constant__ Params P) {
+  megakernel_body<CW, INT8, false, LP, true>(P);
 }
 
 }  // namespace mega
@@ -2412,6 +2465,11 @@ template <bool PROF>
 const void* kernel_for(bool int8) {
   if (int8) return reinterpret_cast<const void*>(mega::decode_megakernel<mega::kConsumerWarps, true, PROF>);
   return reinterpret_cast<const void*>(mega::decode_megakernel<mega::kConsumerWarps, false, PROF>);
+}
+template <bool LP>
+const void* kv16_kernel_for(bool int8) {
+  if (int8) return reinterpret_cast<const void*>(mega::kv16_megakernel<mega::kConsumerWarps, true, LP>);
+  return reinterpret_cast<const void*>(mega::kv16_megakernel<mega::kConsumerWarps, false, LP>);
 }
 const void* logprob_kernel_for(bool int8) {
   if (int8) return reinterpret_cast<const void*>(mega::logprob_megakernel<mega::kConsumerWarps, true>);
@@ -2457,9 +2515,14 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   fast_ = m.numerics == 1 ? 1 : 0;
   if (const char* e = getenv("KLLM_MODE")) fast_ = std::string(e) == "fast" ? 1 : 0;
   int8_fast_ = (int8 && fast_) ? 1 : 0;
-  kernel_ = kernel_for<false>(int8);
-  kernel_prof_ = kernel_for<true>(int8);
-  kernel_lp_ = logprob_kernel_for(int8);
+  // bf16 KV cache: a toleranced variant of the flash attention only, over 16-byte chunks of 8 dims with a
+  // quarter of the head per lane (head_size % 32 == 0); refused rather than run in any other form
+  if (m.kv_cache != KLLM_KV_F32 && m.kv_cache != KLLM_KV_BF16) return KLLM_E_INVALID;
+  kv_bf16_ = m.kv_cache == KLLM_KV_BF16 ? 1 : 0;
+  if (kv_bf16_ && (!fast_ || m.tp_world > 1 || hs % 32 != 0)) return KLLM_E_UNSUPPORTED;
+  kernel_ = kv_bf16_ ? kv16_kernel_for<false>(int8) : kernel_for<false>(int8);
+  kernel_prof_ = kv_bf16_ ? nullptr : kernel_for<true>(int8);  // no profiling instantiation for the bf16 cache
+  kernel_lp_ = kv_bf16_ ? kv16_kernel_for<true>(int8) : logprob_kernel_for(int8);
 
   // The residual exchange after o_proj and down_proj is tagged (under tensor parallelism it IS the
   // all-reduce), and so are the hand-offs q|k|v -> attention -> Wo and SwiGLU -> W2: the one grid
@@ -2479,7 +2542,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   int stage_bytes = int8 ? 27 * 1024 : 32 * 1024;
   if (const char* e = getenv("KLLM_STAGE_BYTES")) stage_bytes = atoi(e);
   stage_bytes = (stage_bytes + 127) & ~127;
-  attn_tile_ = std::min(stage_bytes / (hs * 4), mega::kConsumerWarps * 32) & ~31;  // one timestep per consumer thread
+  const int kv_esz = kv_bf16_ ? 2 : 4;  // bytes per cached element
+  attn_tile_ = std::min(stage_bytes / (hs * kv_esz), mega::kConsumerWarps * 32) & ~31;  // one timestep per consumer thread
   if (attn_tile_ < 32) return KLLM_E_UNSUPPORTED;
   if (fast_) {  // flash attention: a lane quartet per timestep, warp partials (m, l, o[hs]) in the input buffer
     if (hs & 15) return KLLM_E_UNSUPPORTED;
@@ -2520,7 +2584,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     if (v >= 1 && v <= split_cap && (v & (v - 1)) == 0) attn_split_ = v;
   }
   attn_vsplit_ = fast_ ? 1 : attn_split_;
-  attn_tile_v_ = (stage_bytes / ((hs / attn_vsplit_) * 4)) & ~31;
+  attn_tile_v_ = (stage_bytes / ((hs / attn_vsplit_) * kv_esz)) & ~31;
   if (attn_tile_v_ < 32) return KLLM_E_UNSUPPORTED;
   xbuf_bytes_ = xbuf;
   xres_bytes_ = xres;
@@ -2610,8 +2674,9 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
       p.norm_eps = eps;
       p.seg[0] = {m.wq[l], int8 ? m.sq[l] : nullptr, m.bq ? m.bq[l] : nullptr, nullptr, 0, q_rows, 0, t_q};
       p.seg[1] = {m.wk[l], int8 ? m.sk[l] : nullptr, m.bk ? m.bk[l] : nullptr, nullptr, 0, kvd, 0, t_k};
-      p.seg[2] = {m.wv[l], int8 ? m.sv[l] : nullptr, m.bv ? m.bv[l] : nullptr,
-                  m.value_cache + layer_off, 0, kvd, 1, t_v};
+      float* vrows = kv_bf16_ ? reinterpret_cast<float*>(reinterpret_cast<__nv_bfloat16*>(m.value_cache) + layer_off)
+                              : m.value_cache + layer_off;  // kv16_megakernel's epilogue stores bf16 elements
+      p.seg[2] = {m.wv[l], int8 ? m.sv[l] : nullptr, m.bv ? m.bv[l] : nullptr, vrows, 0, kvd, 1, t_v};
       p.units = q_rows + 2 * kvd;
       if (int rc = plan(p)) return rc;
       p.hand_out = hands;
@@ -2751,8 +2816,10 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   cudaError_t e = cudaFuncSetAttribute(kernel_, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        static_cast<int>(smem_bytes_));
   if (e != cudaSuccess) return static_cast<int>(e);
-  e = cudaFuncSetAttribute(kernel_prof_, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes_));
-  if (e != cudaSuccess) return static_cast<int>(e);
+  if (kernel_prof_ != nullptr) {
+    e = cudaFuncSetAttribute(kernel_prof_, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes_));
+    if (e != cudaSuccess) return static_cast<int>(e);
+  }
   e = cudaFuncSetAttribute(kernel_lp_, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes_));
   if (e != cudaSuccess) return static_cast<int>(e);
   int occ_lp = 0;
@@ -2860,6 +2927,7 @@ int MegaEngine::launch(const Params& P) {
   void* args[] = {const_cast<Params*>(&P)};
   // the profiling instantiation records no log-probabilities; logprob_megakernel runs while they are on
   const void* k = P.prof != nullptr ? kernel_prof_ : P.lp_top_n >= 0 ? kernel_lp_ : kernel_;
+  if (k == nullptr) return KLLM_E_UNSUPPORTED;
   cudaError_t e = cudaLaunchCooperativeKernel(const_cast<void*>(k), dim3(grid_),
                                               dim3(kThreads), args, smem_bytes_, stream_);
   if (e != cudaSuccess) return static_cast<int>(e);

@@ -103,6 +103,8 @@ struct Params {
   float* score;
   // KV cache in the persistent engine's own layout (see megakernel.cu "KV layout"):
   //   K [L][kv_head][head_size/4][seq_len][4]    V [L][kv_head][attn_split][seq_len][head_size/attn_split]
+  // kv16_megakernel (KLLM_KV_BF16, flash form only): both caches hold bf16 elements behind these pointers,
+  //   K [L][kv_head][head_size/8][seq_len][8]    V [L][kv_head][seq_len][head_size]
   float* key_cache;
   const float* value_cache;
   const float* sin_cache;
@@ -185,6 +187,7 @@ struct MegaModel {
   unsigned long long* tp_data[8];
   int tp_stride;
   int numerics;  // kllm_decoder_desc::numerics
+  int kv_cache;  // kllm_decoder_desc::kv_cache: KLLM_KV_BF16 needs the fast numerics (flash attention)
 };
 
 class MegaEngine {
@@ -233,9 +236,10 @@ class MegaEngine {
   int int8_fast_ = 0;
   int fast_ = 0;  // numerics: 0 = bit-exact with the reference, 1 = toleranced (free summation order)
   int attn_vsplit_ = 1;
+  int kv_bf16_ = 0;  // bf16 KV cache: the kernels are kv16_megakernel's
   int cls_rows_ = 0, n_cls_phases_ = 1;
   const void* kernel_ = nullptr;       // decode_megakernel<8 consumer warps, int8, false>
-  const void* kernel_prof_ = nullptr;  // ... <.., true>: records the phase timeline stamps
+  const void* kernel_prof_ = nullptr;  // ... <.., true>: records the phase timeline stamps (none with kv_bf16_)
   const void* kernel_lp_ = nullptr;    // logprob_megakernel<8 consumer warps, int8>: log-probabilities on
   size_t smem_bytes_ = 0;
   unsigned barrier_base_ = 0;

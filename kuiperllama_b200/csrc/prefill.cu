@@ -12,6 +12,7 @@
 // Because of TF32 (10 mantissa bits per operand) the cache rows and the final logits agree with the
 // position-by-position path to ~1e-3 relative, not bit for bit; tests/test_prefill_gpu.py states the
 // bound.  fp32 and int8 checkpoints (the int8 GEMM dequantises its weight tiles to TF32), single GPU.
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
 #include <cfloat>
@@ -86,8 +87,11 @@ __global__ void swiglu_rows_kernel(float* __restrict__ h1, const float* __restri
 struct CacheLayout {
   int mega;  // 1: persistent engine K [kvh][hs/4][seq][4], V [kvh][split][seq][hs/split]; 0: [seq][kv_dim]
   int seq_len, kv_dim, head_size, split;
+  int bf16;  // with mega: bf16 elements, K [kvh][hs/8][seq][8] (16-byte chunks of 8 dims), V split 1
 };
 __device__ __forceinline__ size_t k_index(const CacheLayout& c, int pos, int kvh, int i) {
+  if (c.mega && c.bf16)
+    return (static_cast<size_t>(kvh) * (c.head_size >> 3) + (i >> 3)) * c.seq_len * 8 + static_cast<size_t>(pos) * 8 + (i & 7);
   if (c.mega) return (static_cast<size_t>(kvh) * (c.head_size >> 2) + (i >> 2)) * c.seq_len * 4 + static_cast<size_t>(pos) * 4 + (i & 3);
   return static_cast<size_t>(pos) * c.kv_dim + kvh * c.head_size + i;
 }
@@ -98,12 +102,19 @@ __device__ __forceinline__ size_t v_index(const CacheLayout& c, int pos, int kvh
   }
   return static_cast<size_t>(pos) * c.kv_dim + kvh * c.head_size + i;
 }
+// A cache element of type E (float, or __nv_bfloat16 for the bf16 KV cache: rounded to nearest even on the way
+// in, widened exactly on the way out)
+__device__ __forceinline__ void put(float* p, float v) { *p = v; }
+__device__ __forceinline__ void put(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+__device__ __forceinline__ float get(const float* p) { return *p; }
+__device__ __forceinline__ float get(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
 // RoPE (rope_kernel.cu) on the T query rows in place, and on the T key rows while they are scattered,
-// with the value rows, into the layer's cache.  grid = T, one thread per rotation pair.
+// with the value rows, into the layer's cache (of element type E).  grid = T, one thread per rotation pair.
+template <typename E>
 __global__ void rope_scatter_kernel(float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                                     const float* __restrict__ sin_t, const float* __restrict__ cos_t,
-                                    float* __restrict__ kcache, float* __restrict__ vcache, CacheLayout c, int heads,
+                                    E* __restrict__ kcache, E* __restrict__ vcache, CacheLayout c, int heads,
                                     int kv_heads, int flavour, int start_pos) {
   const int t = blockIdx.x, pos = start_pos + t, hs = c.head_size, half = hs >> 1;
   float* qrow = q + static_cast<size_t>(t) * heads * hs;
@@ -127,18 +138,19 @@ __global__ void rope_scatter_kernel(float* __restrict__ q, const float* __restri
     } else {
       const int kvh = h - heads;
       const float a = krow[kvh * hs + i0], b = krow[kvh * hs + i1];
-      kcache[k_index(c, pos, kvh, i0)] = __fmaf_rn(fcr, a, -__fmul_rn(fci, b));
-      kcache[k_index(c, pos, kvh, i1)] = __fmaf_rn(fci, a, __fmul_rn(fcr, b));
+      put(kcache + k_index(c, pos, kvh, i0), __fmaf_rn(fcr, a, -__fmul_rn(fci, b)));
+      put(kcache + k_index(c, pos, kvh, i1), __fmaf_rn(fci, a, __fmul_rn(fcr, b)));
     }
   }
   for (int p = threadIdx.x; p < kv_heads * hs; p += blockDim.x)
-    vcache[v_index(c, pos, p / hs, p % hs)] = vrow[p];
+    put(vcache + v_index(c, pos, p / hs, p % hs), vrow[p]);
 }
 
 // Causal attention of query (t, head) over cache positions 0 .. start_pos + t (mha_kernel.cu:47-110
-// arithmetic, fp32).  grid = (heads, T); scores in dynamic shared memory.
-__global__ void attn_rows_kernel(const float* __restrict__ q, const float* __restrict__ kcache,
-                                 const float* __restrict__ vcache, float* __restrict__ out, CacheLayout c, int heads,
+// arithmetic, fp32, over cache elements of type E).  grid = (heads, T); scores in dynamic shared memory.
+template <typename E>
+__global__ void attn_rows_kernel(const float* __restrict__ q, const E* __restrict__ kcache,
+                                 const E* __restrict__ vcache, float* __restrict__ out, CacheLayout c, int heads,
                                  int kv_mul, int start_pos) {
   extern __shared__ float sc[];
   __shared__ float scratch[32];
@@ -148,7 +160,7 @@ __global__ void attn_rows_kernel(const float* __restrict__ q, const float* __res
   float mx = -FLT_MAX;
   for (int j = threadIdx.x; j <= pos; j += blockDim.x) {
     float s = 0.f;
-    for (int i = 0; i < hs; ++i) s = __fmaf_rn(kcache[k_index(c, j, kvh, i)], qh[i], s);
+    for (int i = 0; i < hs; ++i) s = __fmaf_rn(get(kcache + k_index(c, j, kvh, i)), qh[i], s);
     s *= scale;
     sc[j] = s;
     mx = fmaxf(mx, s);
@@ -164,7 +176,7 @@ __global__ void attn_rows_kernel(const float* __restrict__ q, const float* __res
   __syncthreads();
   for (int i = threadIdx.x; i < hs; i += blockDim.x) {
     float acc = 0.f;
-    for (int j = 0; j <= pos; ++j) acc = __fmaf_rn(sc[j] / sum, vcache[v_index(c, j, kvh, i)], acc);
+    for (int j = 0; j <= pos; ++j) acc = __fmaf_rn(sc[j] / sum, get(vcache + v_index(c, j, kvh, i)), acc);
     out[(static_cast<size_t>(t) * heads + head) * hs + i] = acc;
   }
 }
@@ -196,7 +208,7 @@ int prefill_block(const PrefillModel& m, PrefillWorkspace& ws, const int32_t* to
   const int ew_grid = 528;  // 4 x 132 SMs for the grid-stride elementwise kernels
   embed_rows_kernel<<<T, 256, 0, s>>>(tokens_dev, m.tok_emb, ws.x, dim, m.vocab_size);
   PF_TRY(count());
-  const CacheLayout cl{m.mega_layout, m.seq_len, kvd, hs, m.attn_split > 0 ? m.attn_split : 1};
+  const CacheLayout cl{m.mega_layout, m.seq_len, kvd, hs, m.attn_split > 0 ? m.attn_split : 1, m.kv_bf16};
   for (int l = 0; l < m.layer_num; ++l) {
     const size_t layer_off = static_cast<size_t>(l) * m.seq_len * kvd;
     rmsnorm_rows_kernel<<<T, 256, 0, s>>>(ws.x, m.attn_norm[l], ws.xn, dim, m.eps);
@@ -211,12 +223,21 @@ int prefill_block(const PrefillModel& m, PrefillWorkspace& ws, const int32_t* to
       count_launch(2);
       PF_TRY(count());
     }
-    rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, m.key_cache + layer_off,
-                                          m.value_cache + layer_off, cl, heads, kvh, m.flavour, start_pos);
-    PF_TRY(count());
     const size_t sc_bytes = static_cast<size_t>(start_pos + T) * sizeof(float);
-    attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, m.key_cache + layer_off, m.value_cache + layer_off,
-                                                           ws.att, cl, heads, heads / kvh, start_pos);
+    if (m.kv_bf16) {
+      __nv_bfloat16* kc = reinterpret_cast<__nv_bfloat16*>(m.key_cache) + layer_off;
+      __nv_bfloat16* vc = reinterpret_cast<__nv_bfloat16*>(m.value_cache) + layer_off;
+      rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc, vc, cl, heads, kvh,
+                                            m.flavour, start_pos);
+      PF_TRY(count());
+      attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, kc, vc, ws.att, cl, heads, heads / kvh, start_pos);
+    } else {
+      rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, m.key_cache + layer_off,
+                                            m.value_cache + layer_off, cl, heads, kvh, m.flavour, start_pos);
+      PF_TRY(count());
+      attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, m.key_cache + layer_off, m.value_cache + layer_off,
+                                                             ws.att, cl, heads, heads / kvh, start_pos);
+    }
     PF_TRY(count());
     PF_TRY(gemm(ws.att, m.wo[l], scales(m.so, l), ws.tmp, q_rows, dim));
     add_rows_kernel<<<ew_grid, 256, 0, s>>>(ws.x, ws.tmp, static_cast<size_t>(T) * dim);
@@ -237,9 +258,11 @@ int prefill_block(const PrefillModel& m, PrefillWorkspace& ws, const int32_t* to
 int prefill_attention_smem_opt_in(size_t bytes) {
   static size_t configured = 0;
   if (bytes <= 48 * 1024 || bytes <= configured) return 0;
-  const cudaError_t e =
-      cudaFuncSetAttribute(attn_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
-  if (e != cudaSuccess) return static_cast<int>(e);
+  for (const void* k : {reinterpret_cast<const void*>(attn_rows_kernel<float>),
+                        reinterpret_cast<const void*>(attn_rows_kernel<__nv_bfloat16>)}) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e != cudaSuccess) return static_cast<int>(e);
+  }
   configured = bytes;
   return 0;
 }

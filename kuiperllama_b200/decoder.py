@@ -143,7 +143,8 @@ class Decoder:
     """Owns a ``kllm_decoder`` built over torch-held device weights."""
 
     def __init__(self, shape: ModelShape, weights: dict, stream=None, tp_size=1, tp_rank=0,
-                 allreduce=None, allreduce_ctx=None, full_dim=None, comm=None, numerics="exact"):
+                 allreduce=None, allreduce_ctx=None, full_dim=None, comm=None, numerics="exact",
+                 kv_cache="fp32"):
         self.lib = load_library()
         self.shape = shape
         self.weights = weights  # keep the tensors alive
@@ -179,6 +180,9 @@ class Decoder:
         d.tp_size, d.tp_rank = tp_size, tp_rank
         # "exact": bit-identical to the reference; "fast": toleranced (kllm_b200.h, kllm_decoder_desc::numerics)
         d.numerics = {"exact": 0, "fast": 1}[numerics]
+        # "fp32": the cache of every other mode; "bf16": rows rounded to bf16 as they are cached, fast numerics on
+        # the persistent engine only (kllm_b200.h, kllm_decoder_desc::kv_cache)
+        d.kv_cache = {"fp32": 0, "bf16": 1}[kv_cache]
         if allreduce is not None:
             d.allreduce = allreduce
             d.allreduce_ctx = allreduce_ctx

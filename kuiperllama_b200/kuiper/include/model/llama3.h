@@ -86,6 +86,14 @@ class LLama2Model : public Model {
   void set_batched_prefill(bool on);
   bool batched_prefill() const { return batched_prefill_; }
 
+  // bf16 KV cache in the fused decoder (kllm_decoder_desc::kv_cache = KLLM_KV_BF16): call before init();
+  // without a call init() takes it from KUIPER_KV_CACHE=bf16.  Off by default.  Half the cache memory and
+  // half the attention's cache reads, toleranced: it needs the fast numerics (KUIPER_NUMERICS=fast) on
+  // one GPU, and init() fails rather than run without it.  The layer path (forward()) keeps fp32 rows;
+  // the rows it takes over from the decoder are the widened bf16 values.
+  void set_bf16_kv_cache(bool on);
+  bool bf16_kv_cache() const { return bf16_kv_cache_; }
+
   // Seeded sampling instead of the greedy id (DESIGN.md "Sampling"): call before init(); without a call
   // init() takes it from KUIPER_TEMPERATURE, KUIPER_TOP_K and KUIPER_SEED, so the reference's unchanged
   // demos can sample.  Unset or temperature 0 is greedy.  predict() on the fused decoder and forward() +
@@ -195,6 +203,8 @@ class LLama2Model : public Model {
   // embedding() call (embedding_calls_ counts them) the decoder's cache holds from it
   bool batched_prefill_ = false;
   bool batched_prefill_explicit_ = false;
+  bool bf16_kv_cache_ = false;
+  bool bf16_kv_cache_explicit_ = false;
   float temperature_ = 0.f;
   int32_t top_k_ = 0;
   uint64_t seed_ = 0;

@@ -77,6 +77,11 @@ void LLama2Model::set_batched_prefill(bool on) {
   batched_prefill_explicit_ = true;
 }
 
+void LLama2Model::set_bf16_kv_cache(bool on) {
+  bf16_kv_cache_ = on;
+  bf16_kv_cache_explicit_ = true;
+}
+
 void LLama2Model::set_sampling(float temperature, int32_t top_k, uint64_t seed) {
   temperature_ = temperature;
   top_k_ = top_k;
@@ -156,6 +161,10 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
     return error::InvalidArgument(
         "batched prompt prefill is single-GPU: turn it off (KUIPER_BATCHED_PREFILL / set_batched_prefill) under "
         "tensor parallelism");
+  if (!bf16_kv_cache_explicit_) {
+    const char* env = std::getenv("KUIPER_KV_CACHE");
+    bf16_kv_cache_ = env != nullptr && std::string(env) == "bf16";
+  }
   if (!sampling_explicit_) {
     const char* t = std::getenv("KUIPER_TEMPERATURE");
     const char* k = std::getenv("KUIPER_TOP_K");
@@ -589,9 +598,13 @@ base::Status LLama2Model::create_decoder() {
     d.comm = comm_;
   }
   if (const char* mode = std::getenv("KUIPER_NUMERICS"); mode && std::string(mode) == "fast") d.numerics = KLLM_NUMERICS_FAST;
+  if (bf16_kv_cache_) d.kv_cache = KLLM_KV_BF16;
   const int rc = kllm_decoder_create(&d, cuda_config_->stream, &decoder_);
   if (rc != 0)
-    return base::error::InternalError(std::string("kllm_decoder_create failed: ") + kllm_error_string(rc));
+    return base::error::InternalError(
+        std::string("kllm_decoder_create failed: ") + kllm_error_string(rc) +
+        (bf16_kv_cache_ ? " (the bf16 KV cache needs KUIPER_NUMERICS=fast, one GPU and head_size % 32 == 0)" : ""));
+  if (bf16_kv_cache_) LOG(INFO) << "KV cache: bf16 (rounded to nearest even as rows are cached)";
   if (temperature_ > 0.f) {
     const int src = kllm_decoder_set_sampling_top_p(decoder_, temperature_, top_k_, top_p_, seed_);
     if (src != 0)

@@ -4,7 +4,7 @@
 //   kuiper_decode <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...]
 //                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P]
 //                 [--repetition-penalty P N] [--frequency-presence F P [FROM]] [--logit-bias ID:B,...]
-//                 [--generate N [--stop ID]... [--then K]] [--logprobs N] [--score]
+//                 [--generate N [--stop ID]... [--then K]] [--logprobs N] [--score] [--kv-cache fp32|bf16]
 //
 // --generate N runs the prompt and LLama2Model::generate() for at most N ids instead (n_steps is then unused),
 // stopping at the tokenizer's stop ids and every --stop ID, and prints the ids generate() returned, followed
@@ -28,7 +28,8 @@
 // entry: "lp <pos> <id> <lp>" followed by N pairs "<top id> <top lp>" (%.9g: the fp32 values round-trip).
 // --score scores the given ids with LLama2Model::score() instead of decoding (n_steps is then unused): one line of
 // the n - 1 log-probabilities, then "perplexity <exp(-mean)>".  The layer path has neither: --layers with either is
-// refused.
+// refused.  --kv-cache bf16 calls LLama2Model::set_bf16_kv_cache(true) instead of leaving it to KUIPER_KV_CACHE (the
+// fused decoder's bf16 KV cache needs KUIPER_NUMERICS=fast); --kv-cache fp32 turns it off.
 #include <base/base.h>
 #include <cuda_runtime_api.h>
 #include <glog/logging.h>
@@ -51,7 +52,7 @@ int main(int argc, char** argv) {
     std::fprintf(stderr, "usage: %s <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...] "
                          "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P] "
                          "[--repetition-penalty P N] [--frequency-presence F P [FROM]] [--logit-bias ID:B,...] "
-                         "[--generate N [--stop ID]... [--then K]]\n", argv[0]);
+                         "[--generate N [--stop ID]... [--then K]] [--kv-cache fp32|bf16]\n", argv[0]);
     return 2;
   }
   const std::string checkpoint = argv[1], family = argv[2], prec = argv[3];
@@ -77,6 +78,7 @@ int main(int argc, char** argv) {
   std::vector<int32_t> stops;
   int32_t logprobs = -1;
   bool set_logprobs = false, score = false;
+  int kv_cache = -1;  // -1: KUIPER_KV_CACHE decides, 0: fp32, 1: bf16
   for (int i = 5; i < argc; ++i) {
     if (!std::strcmp(argv[i], "--layers")) layers = true;
     else if (!std::strcmp(argv[i], "--sampling") && i + 3 < argc) {
@@ -123,6 +125,11 @@ int main(int argc, char** argv) {
       logprobs = std::atoi(argv[++i]);
     }
     else if (!std::strcmp(argv[i], "--score")) score = true;
+    else if (!std::strcmp(argv[i], "--kv-cache") && i + 1 < argc) {
+      const std::string v = argv[++i];
+      if (v != "fp32" && v != "bf16") return 2;
+      kv_cache = v == "bf16" ? 1 : 0;
+    }
     else if (!std::strcmp(argv[i], "--logits") && i + 1 < argc) logits_path = argv[++i];
     else prompt.push_back(std::atoi(argv[i]));
   }
@@ -146,6 +153,7 @@ int main(int argc, char** argv) {
   if (!logit_bias.empty()) m->set_logit_bias(logit_bias);
   if (!stops.empty()) m->set_stop_ids(stops);
   if (set_logprobs) m->set_logprobs(logprobs);  // init() refuses a value outside [-1, 20]
+  if (kv_cache >= 0) m->set_bf16_kv_cache(kv_cache == 1);
   base::Status st = m->init(base::DeviceType::kDeviceCUDA);
   if (!st) {
     std::fprintf(stderr, "init failed: %s\n", st.get_err_msg().c_str());
