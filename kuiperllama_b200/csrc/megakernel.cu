@@ -2142,9 +2142,23 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
     const uint64_t policy = policy_evict_first();  // weights: streamed once per token
     const uint64_t policy_kv = policy_evict_last();  // KV tiles: re-read every token, keep in L2
     int ppos = P.state->pos;
+    // PROF: the cycles each fill of the profiled token waited for a free slot, and the fills, per phase (stamps 11
+    // and 12, tools/phase_timeline.py).  A slot is free once the consumers have read it, so this is the time the
+    // ring was full: of copies still in flight, or of stages the consumers had not yet read.
+    unsigned long long* pstamp = nullptr;
+    auto fill_waited = [&](long long c0) {
+      if (pstamp && lane == 0) {
+        atomicAdd(pstamp + 11, static_cast<unsigned long long>(clock64() - c0));
+        atomicAdd(pstamp + 12, 1ull);
+      }
+    };
     for (int tok = 0; tok < P.n_tokens; ++tok, ++ppos) {
       const int n_run = tok < P.skip_cls_tokens ? P.n_phases - P.n_cls_phases : P.n_phases;  // prompt token: no classifier
       for (int pi = 0; pi < n_run; ++pi) {
+        if constexpr (PROF)
+          pstamp = (P.prof != nullptr && tok == P.prof_token)
+                       ? P.prof + (static_cast<size_t>(cta) * P.n_phases + pi) * kProfStamps
+                       : nullptr;
         {
           const uint32_t* src = reinterpret_cast<const uint32_t*>(P.phases + pi);
           uint32_t* dst = reinterpret_cast<uint32_t*>(&s_phase_prod);
@@ -2188,7 +2202,9 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
               const int t0 = j * T;
               const int nt = min(T, ppos - t0);
               for (int kv = 0; kv < 2; ++kv) {
+                const long long pw0 = PROF ? clock64() : 0;
                 if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
+                if constexpr (PROF) fill_waited(pw0);
                 unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
                 if (lane == 0) mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(nt) * row_bytes);
                 __syncwarp();
@@ -2213,7 +2229,9 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
             for (int j = split; j < n_tiles; j += SP) {
               const int t0 = j * T;
               const int nt = min(T, ppos - t0);
+              const long long pw0 = PROF ? clock64() : 0;
               if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
+              if constexpr (PROF) fill_waited(pw0);
               unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
               if (lane == 0) mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(nt) * hs * 4);
               __syncwarp();
@@ -2231,7 +2249,9 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
             for (int j = 0; j < n_tiles; ++j) {
               const int t0 = j * T;
               const int nt = min(T, ppos - t0);
+              const long long pw0 = PROF ? clock64() : 0;
               if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
+              if constexpr (PROF) fill_waited(pw0);
               unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
               if (lane == 0) {
                 mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(nt) * dv * 4);
@@ -2253,7 +2273,9 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
           for (int u = u0; u < u1; u += ups) {
             const int n = min(ups, u1 - u);
             const int nrows = n * rpu;
+            const long long pw0 = PROF ? clock64() : 0;
             if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
+            if constexpr (PROF) fill_waited(pw0);
             unsigned char* dst = stages + static_cast<size_t>(pipe.slot) * P.stage_bytes;
             if (lane == 0)
               mbar_expect_tx(&full_bar[pipe.slot],
@@ -2284,7 +2306,9 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
             for (int c = 0; c < ph.chunks_per_row; ++c) {
               const int e0 = c * ph.chunk_elems;
               const int ne = min(ph.chunk_elems, ph.in_dim - e0);
+              const long long pw0 = PROF ? clock64() : 0;
               if (mbar_wait_or_stop(&empty_bar[pipe.slot], pipe.parity ^ 1u, &g_stop)) goto producer_done;
+              if constexpr (PROF) fill_waited(pw0);
               if (lane == 0) {
                 mbar_expect_tx(&full_bar[pipe.slot], static_cast<uint32_t>(ne) * wbytes);
                 bulk_g2s(stages + static_cast<size_t>(pipe.slot) * P.stage_bytes,
@@ -2539,7 +2563,15 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   // fp32: 32 KB (4 rows of dim 2048, 2 of 4096).  int8: 27 KB = 6 rows of dim 4096 (+ scales) or
   // 2 rows of hidden 11008, which leaves six stages next to the 44 KB input vector and the 16 KB
   // residual stream of Llama-2-7B.
-  int stage_bytes = int8 ? 27 * 1024 : 32 * 1024;
+  // fp32 in the fast numerics (fp32 cache), when a 16 KB stage still holds two input rows of dim (dim <= 2048): 12 ×
+  // 16 KB.  The same ring in twice the slots is released at half the grain: a stage of 2 rows of dim 2048 is one
+  // task of one warp, so all 8 warps drain the ring at once instead of 6, and TinyLlama's W2 (22.5 KB rows, 2 chunks
+  // of 12 and 10 KB) fills it as well as one row filled 32 KB.  H100 80GB HBM3, 700 W: TinyLlama-1.1B 670 tok/s
+  // against 627 with 32 KB (20 KB: 649, 24 KB: 645), Qwen2.5-0.5B 1058 against 1032.  At dim 4096 a 16 KB stage is
+  // ONE row, a task no longer shares its x loads, and Llama-2-7B fell from 108 to 80 tok/s.  The flash tiles shrink
+  // with the stage (head_size 64: 64 timesteps).
+  const bool small_stages = fast_ && !kv_bf16_ && 2 * dim * 4 <= 16 * 1024;
+  int stage_bytes = int8 ? 27 * 1024 : small_stages ? 16 * 1024 : 32 * 1024;
   if (const char* e = getenv("KLLM_STAGE_BYTES")) stage_bytes = atoi(e);
   stage_bytes = (stage_bytes + 127) & ~127;
   const int kv_esz = kv_bf16_ ? 2 : 4;  // bytes per cached element

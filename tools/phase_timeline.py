@@ -18,6 +18,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="tinyllama-1.1b")
     ap.add_argument("--pos", type=int, default=256)
+    ap.add_argument("--ghz", type=float, default=1.98, help="SM clock for cycles -> us (nvidia-smi clocks.max.sm)")
     a = ap.parse_args()
     from kuiperllama_b200 import SHAPES, Decoder, check, synth_weights
     shape = SHAPES[a.workload]
@@ -36,6 +37,8 @@ def main():
     st = raw[:, :, :4]
     cyc = raw[:, :, 4:10]  # SM cycles of warp 0: addend prefetch, dots, reductions, epilogues, ring waits, stage rows
     polled = raw[:, :, 10]
+    pblk = raw[:, :, 11]  # cycles the ring producer waited for a free slot (ring full: copies in flight or unread stages)
+    pfills = raw[:, :, 12]
     t0 = st[:, 0, 0].min()
     st = (st - t0) / 1e3  # us
     polled = np.where(polled > 0, (polled - t0) / 1e3, st[:, :, 1])
@@ -49,14 +52,15 @@ def main():
     bar = (st[:, :, 3] - st[:, :, 2])            # waiting at the grid barrier
     dur = st[:, :, 3].max(axis=0) - st[:, :, 0].min(axis=0)
     poll = polled - st[:, :, 0]                  # of stage_x: until the input vector is complete
-    ghz = 1.98  # cycles -> us at the H100 SXM's boost clock (clocks.max.sm); the split is what matters
+    ghz = a.ghz  # cycles -> us; the split is what matters
     print(f"{'phase':>10} {'count':>5} {'phase_us':>9} {'stage_x':>8} {'(poll)':>7} {'work_med':>9} {'work_max':>9} {'barrier_min':>11} "
-          f"{'barrier_med':>11} | warp 0 of the median CTA, us: {'ringwait':>8} {'dots':>6} {'reduce':>6} {'epilog':>6} {'addend':>6}")
+          f"{'barrier_med':>11} {'prod_blk':>8} {'fills':>5} | warp 0 of the median CTA, us: {'ringwait':>8} {'dots':>6} {'reduce':>6} {'epilog':>6} {'addend':>6}")
 
     def row(nm, idx, ctas=slice(None)):
         c = np.median(cyc[ctas][:, idx], axis=0).mean(axis=0) / ghz / 1e3 if len(idx) > 1 else np.median(cyc[ctas][:, idx], axis=0)[0] / ghz / 1e3
         print(f"{nm:>10} {len(idx):5d} {dur[idx].mean():9.2f} {np.median(stage[:, idx]):8.2f} {np.median(poll[:, idx]):7.2f} {np.median(work[:, idx]):9.2f} "
-              f"{work[:, idx].max(axis=0).mean():9.2f} {bar[:, idx].min(axis=0).mean():11.2f} {np.median(bar[:, idx]):11.2f} | "
+              f"{work[:, idx].max(axis=0).mean():9.2f} {bar[:, idx].min(axis=0).mean():11.2f} {np.median(bar[:, idx]):11.2f} "
+              f"{np.median(pblk[ctas][:, idx].mean(axis=1)) / ghz / 1e3:8.2f} {np.median(pfills[ctas][:, idx].mean(axis=1)):5.1f} | "
               f"{'':32s}{c[4]:8.2f} {c[1]:6.2f} {c[2]:6.2f} {c[3]:6.2f} {c[0]:6.2f}")
     fast = os.environ.get("KLLM_MODE") == "fast"
     sp = int(os.environ.get("KLLM_ATTN_SPLIT_SHOWN", "0")) or (4 if (NPL == 6 or fast) else 1)
@@ -75,6 +79,13 @@ def main():
     print(f"# attention (scores + softmax + P.V) on the first {heads} attention CTAs: median {np.median(attn):.2f} us, slowest head per layer (mean) "
           f"{attn.max(axis=0).mean():.2f} us")
     print(f"# sum of phase durations: {dur.sum():.1f} us; barrier_min = time the LAST arriving CTA spends in the barrier")
+    tok_us = st[:, -1, 3].max()
+    blk_us = pblk.sum(axis=1) / ghz / 1e3
+    ring_us = cyc[:, :, 4].sum(axis=1) / ghz / 1e3
+    print(f"# ring producer waiting for a free slot (ring full): median CTA {np.median(blk_us):.1f} us = "
+          f"{100 * np.median(blk_us) / tok_us:.1f} % of the token, max CTA {blk_us.max():.1f} us; "
+          f"consumer warp 0 waiting on a stage (ringwait): median CTA {np.median(ring_us):.1f} us = "
+          f"{100 * np.median(ring_us) / tok_us:.1f} %")
     # ---- critical path: absolute times of one layer's all-to-all points, averaged over the layers -----------
     # last_done(X) = when the slowest CTA finished producing X; polled(Y) = when the median CTA held all of
     # Y's input vector; hand-off latency = polled(next) - last_done(prev); the phase body = last_done - polled.
