@@ -2887,8 +2887,8 @@ void MegaEngine::destroy() {
   ready_ = false;
 }
 
-Params MegaEngine::params(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev, int prof_token,
-                          int skip_cls_tokens) const {
+Params MegaEngine::params(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev,
+                          unsigned long long* prof_dev, int prof_token, int skip_cls_tokens) const {
   Params P{};
   const MegaModel& m = model_;
   P.phases = static_cast<const Phase*>(d_phases_);
@@ -2921,7 +2921,7 @@ Params MegaEngine::params(int n_tokens, const int32_t* teacher_dev, unsigned lon
   P.value_cache = m.value_cache;
   P.sin_cache = m.sin_cache;
   P.cos_cache = m.cos_cache;
-  P.state = static_cast<mega::State*>(m.state);
+  P.state = m.state;
   P.out_tokens = m.out_tokens;
   P.teacher = teacher_dev;
   P.max_steps = m.seq_len;
@@ -2940,13 +2940,13 @@ Params MegaEngine::params(int n_tokens, const int32_t* teacher_dev, unsigned lon
   P.arg_idx = static_cast<int*>(d_arg_idx_);
   P.sampling = m.sampling;
   P.logits = m.logits;
-  P.penalty = penalty_;
+  P.penalty = cfg.penalty;
   P.hist = m.hist;
   P.penalized = m.penalized;
   P.prof = prof_dev;
   P.prof_token = prof_token;
   for (int i = 0; i < mega::kMaxStopIds; ++i) P.stop_ids[i] = -1;  // ids are >= 0: no stop
-  P.lp_top_n = lp_top_n_;
+  P.lp_top_n = cfg.lp_top_n;
   P.lp_target = 0;
   P.lp_part = static_cast<float2*>(d_lp_);
   P.lp_cand_v = reinterpret_cast<float*>(P.lp_part + grid_);
@@ -2974,24 +2974,21 @@ void MegaEngine::account(int n_tokens) {
   barrier_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(grid_);  // one grid barrier per token
 }
 
-int MegaEngine::run(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
+int MegaEngine::run(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
                     int prof_token, int skip_cls_tokens, int lp_target) {
   if (!ready_) return KLLM_E_STATE;
-  Params P = params(n_tokens, teacher_dev, prof_dev, prof_token, skip_cls_tokens);
-  if (lp_target) {
-    P.lp_target = 1;
-    P.lp_top_n = std::max(lp_top_n_, 0);
-  }
+  Params P = params(cfg, n_tokens, teacher_dev, prof_dev, prof_token, skip_cls_tokens);
+  P.lp_target = lp_target;
   if (int rc = launch(P)) return rc;
   account(n_tokens);
   return 0;
 }
 
-int MegaEngine::run_until(int n_tokens, const int32_t* stop_ids, int n_stop, int32_t* stream_ids,
-                          int32_t* stream_count) {
+int MegaEngine::run_until(const DrawSettings& cfg, int n_tokens, const int32_t* stop_ids, int n_stop,
+                          int32_t* stream_ids, int32_t* stream_count) {
   if (!ready_) return KLLM_E_STATE;
   if (n_stop < 0 || n_stop > mega::kMaxStopIds) return KLLM_E_INVALID;
-  Params P = params(n_tokens, nullptr, nullptr, -1, 0);
+  Params P = params(cfg, n_tokens, nullptr, nullptr, -1, 0);
   for (int i = 0; i < n_stop; ++i) P.stop_ids[i] = stop_ids[i];
   P.stream_ids = stream_ids;
   P.stream_count = stream_count;

@@ -80,8 +80,18 @@ struct Phase {
   Seg seg[3];
 };
 
-struct State {  // == StepState in decoder.cu
-  int32_t token, pos, step, next;
+// The device-resident step state of both engines: the loop state, then the mode of the entry that uploaded it.
+// The persistent engine reads and writes the first four fields only; it takes the mode in its launch parameters.
+struct State {
+  int32_t token;  // input token of the current step
+  int32_t pos;    // position of the current step
+  int32_t step;   // steps done since the entry started
+  int32_t next;   // id produced by the last step
+  // the graph engine's per-entry switches (argmax_advance_kernel), written by the host only
+  int32_t teacher;    // feed teacher[step + 1] instead of the id
+  int32_t streamed;   // publish the id, then the count, to mapped host memory (kllm_decoder_generate_until)
+  int32_t lp_from;    // the first step that writes a record entry: the steps before it are prompt positions
+  int32_t lp_target;  // kllm_decoder_score: the entry's id is teacher[step + 1], recorded with top_n max(top_n, 0)
 };
 
 struct Params {
@@ -176,9 +186,9 @@ struct MegaModel {
   float* logits; float* score;
   float* key_cache; float* value_cache;
   const float* sin_cache; const float* cos_cache;
-  void* state;
+  mega::State* state;
   int32_t* out_tokens;
-  const SampleParams* sampling;
+  const SampleParams* sampling;  // the sampling part of the decoder's device DrawSettings
   int32_t* hist;
   float* penalized;
   sampling::LogprobRecord lp_rec;
@@ -194,32 +204,29 @@ class MegaEngine {
  public:
   int init(const MegaModel& m, cudaStream_t stream);
   void destroy();
-  // Run n_tokens consecutive positions starting from the device-resident state.
-  // lp_target: kllm_decoder_score's run, whose record entries hold teacher[step + 1] (written even with logprobs off)
-  int run(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev = nullptr,
+  // Run n_tokens consecutive positions starting from the device-resident state, under the decoder's settings
+  // `cfg` (its step 0 and logprob setting ride in the launch parameters; the sampling parameters are read through
+  // MegaModel::sampling).  lp_target: kllm_decoder_score's run, whose record entries hold teacher[step + 1]
+  // (cfg.lp_top_n >= 0, so that they are written even with logprobs off)
+  int run(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev = nullptr,
           int prof_token = -1, int skip_cls_tokens = 0, int lp_target = 0);
   // Up to n_tokens positions, ending after the first id in stop_ids[0 .. n_stop); every id is streamed to
   // stream_ids / stream_count (device-visible pointers into mapped host memory).  The number of positions
   // that ran is known only once the launch has finished, so the tag and barrier bases are NOT advanced
   // here: the caller passes that number (state.step) to account() before the next launch.
-  int run_until(int n_tokens, const int32_t* stop_ids, int n_stop, int32_t* stream_ids, int32_t* stream_count);
+  int run_until(const DrawSettings& cfg, int n_tokens, const int32_t* stop_ids, int n_stop, int32_t* stream_ids,
+                int32_t* stream_count);
   void account(int n_tokens);
-  // the step 0 settings of later launches (the decoder's setters, after their stream synchronise)
-  void set_penalty(const PenaltyParams& pp) { penalty_ = pp; }
-  // the logprob setting of later launches (kllm_decoder_set_logprobs, after its stream synchronise)
-  void set_logprobs(int top_n) { lp_top_n_ = top_n; }
   int grid() const { return grid_; }
   int phases() const { return n_phases_; }
   int attn_vsplit() const { return attn_vsplit_; }  // slices of the V cache layout
   int cls_rows() const { return cls_rows_; }  // classifier rows this rank streams per token
 
  private:
-  mega::Params params(int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev, int prof_token,
-                      int skip_cls_tokens) const;
+  mega::Params params(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
+                      int prof_token, int skip_cls_tokens) const;
   int launch(const mega::Params& P);
   MegaModel model_{};
-  PenaltyParams penalty_{};
-  int lp_top_n_ = -1;
   void* d_lp_ = nullptr;  // lp_part [grid] float2, then lp_cand_v / lp_cand_i [grid][kMaxTopLogprobs]
   cudaStream_t stream_ = nullptr;
   void* d_phases_ = nullptr;

@@ -48,8 +48,7 @@
 
 namespace kllm {
 
-// Device-resident sampling parameters (kllm_decoder_set_sampling).  Engines read them when they run,
-// so changing them rebuilds nothing.  A zeroed struct is greedy (and top_p 0 is off, as is 1).
+// Sampling parameters (kllm_decoder_set_sampling_top_p).  A zeroed struct is greedy (and top_p 0 is off, as is 1).
 struct SampleParams {
   float temperature;
   int32_t top_k;
@@ -57,9 +56,8 @@ struct SampleParams {
   float top_p;
 };
 
-// Device-resident step 0 (kllm_decoder_set_repetition_penalty, kllm_decoder_set_frequency_presence,
-// kllm_decoder_set_logit_bias), apart from SampleParams so that setting either leaves the other alone.  A
-// zeroed struct is off.  `active` is set by the host (step0_finish) when any sub-step is on, so that the
+// Step 0 (kllm_decoder_set_repetition_penalty, kllm_decoder_set_frequency_presence, kllm_decoder_set_logit_bias).
+// A zeroed struct is off.  `active` is set by the host (step0_finish) when any sub-step is on, so that the
 // engines test one word.  `marks` [V] is zero between tokens (step0_rows).
 struct PenaltyParams {
   int32_t active;
@@ -70,6 +68,14 @@ struct PenaltyParams {
   int32_t from_pos;   // 0c / 0d count the ids fed at [from_pos, pos]
   const float* bias;  // 0a's dense [V] table; null is off
   int32_t* marks;
+};
+
+// Everything a decoder's ids are drawn and recorded under: its setters change a copy and put it in force between
+// two stream synchronises, on the host and in one device copy that the engines read (decoder.cu put_settings).
+struct DrawSettings {
+  SampleParams sample;
+  PenaltyParams penalty;
+  int32_t lp_top_n;  // log-probabilities: -1 off; 0 the id's lp; 1..kMaxTopLogprobs also the top-N (DESIGN.md 5.8)
 };
 
 namespace sampling {
@@ -663,13 +669,6 @@ __device__ __forceinline__ int draw_block(const float* logits, int n, const Samp
 // within the bound of DESIGN.md 5.8.  Parts: a CTA's classifier rows (or its range of the tensor-parallel gather)
 // in the persistent engine, a warp's contiguous range in the one-block kernels.  Mirror: sampling.logprobs.
 constexpr int kMaxTopLogprobs = 20;  // == KLLM_MAX_TOP_LOGPROBS
-
-// Device-resident logprob setting of the graph engine (the persistent engine takes it in its launch parameters)
-struct LogprobParams {
-  int32_t top_n;      // -1: off; 0: the id's lp; 1..kMaxTopLogprobs: also the top-N
-  int32_t target;     // 1: the entry's id is teacher[step + 1] (kllm_decoder_score); 0: the drawn id
-  int32_t from_step;  // the steps before this one are prompt positions: they write no entry
-};
 
 // The decoder's record, indexed by position: id[pos], lp[pos], top_ids / top_lp [pos][kMaxTopLogprobs]
 struct LogprobRecord {

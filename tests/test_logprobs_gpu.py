@@ -199,6 +199,13 @@ def test_entries_only_where_the_classifier_ran(engine):
     drawn = dec.generate(nxt, 5, 10, teacher=teacher)
     ids = dec.logprobs(5, 10)[0]
     assert (ids == drawn).all()
+    # scoring's target mode ends with the score: a generate over the same positions records the ids it drew
+    tokens = [int(t) for t in np.random.default_rng(3).integers(0, 4096, 11)]
+    dec.score(tokens, 5)
+    assert (dec.logprobs(5, 10)[0] == tokens[1:]).all()
+    drawn = dec.generate(nxt, 5, 10)
+    ids = dec.logprobs(5, 10)[0]
+    assert (ids == drawn).all() and (ids != tokens[1:]).any()
 
 
 def test_prefill_records_the_last_position(engine):
