@@ -118,19 +118,8 @@ class LLama2Model : public Model {
   // Logit bias before every draw (kllm_decoder_set_logit_bias): id -> bias, added before the penalties.  Call before
   // init(), which refuses an id outside the vocabulary, a repeated id and a bias that is not finite.  Empty is off.
   void set_logit_bias(std::vector<std::pair<int32_t, float>> bias);
-  // the settings in force (after init(): the environment's when set_sampling / set_top_p was not called)
-  float sampling_temperature() const { return temperature_; }
-  int32_t sampling_top_k() const { return top_k_; }
-  uint64_t sampling_seed() const { return seed_; }
-  float sampling_top_p() const { return top_p_; }
-  float sampling_repetition_penalty() const { return penalty_; }
-  int32_t sampling_repeat_last_n() const { return repeat_last_n_; }
-  float sampling_frequency_penalty() const { return frequency_; }
-  float sampling_presence_penalty() const { return presence_; }
-  int32_t sampling_count_from() const { return count_from_; }
-  const std::vector<std::pair<int32_t, float>>& sampling_logit_bias() const { return logit_bias_; }
-  // any of step 0's settings other than the repetition penalty is on
-  bool sampling_step0_extras() const { return frequency_ != 0.f || presence_ != 0.f || !logit_bias_.empty(); }
+  // the draw settings in force (after init(): the environment's for each group no setter above was called for)
+  const sampler::DrawConfig& draw_config() const { return draw_; }
 
   // A whole generation on the fused decoder, without a host round trip per token:
   //   1. the prompt from position 0 (the batched prefill for all but its last token when batched_prefill() is
@@ -148,7 +137,7 @@ class LLama2Model : public Model {
   // log-probability over the raw logits, 1..20 also its top_n alternatives.  Entries are written by the fused
   // paths (predict() on the fused decoder, generate()), at every position whose classifier runs.
   void set_logprobs(int32_t top_n);
-  int32_t logprobs_top_n() const { return logprobs_top_n_; }
+  int32_t logprobs_top_n() const { return draw_.logprobs_top_n; }
   // The record of positions [first_pos, first_pos + n) (kllm_decoder_read_logprobs): ids (-1: no entry), lp, and
   // top_ids / top_lp [n][logprobs_top_n()] (empty when it is <= 0).
   base::Status logprobs(int32_t first_pos, int32_t n, std::vector<int32_t>& ids, std::vector<float>& lp,
@@ -205,20 +194,8 @@ class LLama2Model : public Model {
   bool batched_prefill_explicit_ = false;
   bool bf16_kv_cache_ = false;
   bool bf16_kv_cache_explicit_ = false;
-  float temperature_ = 0.f;
-  int32_t top_k_ = 0;
-  uint64_t seed_ = 0;
-  bool sampling_explicit_ = false;
-  float top_p_ = 1.f;
-  bool top_p_explicit_ = false;
-  float penalty_ = 1.f;
-  int32_t repeat_last_n_ = 0;
-  bool penalty_explicit_ = false;
-  float frequency_ = 0.f, presence_ = 0.f;
-  int32_t count_from_ = 0;
-  bool frequency_presence_explicit_ = false;
-  std::vector<std::pair<int32_t, float>> logit_bias_;
-  int32_t logprobs_top_n_ = -1;
+  sampler::DrawConfig draw_;
+  sampler::DrawGroups draw_set_;              // the groups a setter gave: init() keeps them over the environment
   sampler::SeededSampler* seeded_ = nullptr;  // sampler_ when sampling, else null
   std::vector<int32_t> extra_stop_ids_;       // set_stop_ids()
   mutable uint64_t embedding_calls_ = 0;

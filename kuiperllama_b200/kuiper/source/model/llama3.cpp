@@ -17,9 +17,9 @@
 #include <cuda_runtime_api.h>
 #include <kllm_b200.h>
 #include <op/decoder_layers.h>
+#include <sampler/draw_config.h>
 
 #include <algorithm>
-#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <utility>
@@ -83,39 +83,29 @@ void LLama2Model::set_bf16_kv_cache(bool on) {
 }
 
 void LLama2Model::set_sampling(float temperature, int32_t top_k, uint64_t seed) {
-  temperature_ = temperature;
-  top_k_ = top_k;
-  seed_ = seed;
-  sampling_explicit_ = true;
+  draw_.temperature = temperature, draw_.top_k = top_k, draw_.seed = seed, draw_set_.sampling = true;
 }
 
-void LLama2Model::set_top_p(float top_p) {
-  top_p_ = top_p;
-  top_p_explicit_ = true;
-}
+void LLama2Model::set_top_p(float top_p) { draw_.top_p = top_p, draw_set_.top_p = true; }
 
 void LLama2Model::set_repetition_penalty(float penalty, int32_t last_n) {
-  penalty_ = penalty;
-  repeat_last_n_ = last_n;
-  penalty_explicit_ = true;
+  draw_.penalty = penalty, draw_.last_n = last_n, draw_set_.penalty = true;
 }
 
 void LLama2Model::set_frequency_presence(float frequency, float presence, int32_t from_pos) {
-  frequency_ = frequency;
-  presence_ = presence;
-  count_from_ = from_pos;
-  frequency_presence_explicit_ = true;
+  draw_.frequency = frequency, draw_.presence = presence, draw_.from_pos = from_pos;
+  draw_set_.frequency_presence = true;
 }
 
-void LLama2Model::set_logit_bias(std::vector<std::pair<int32_t, float>> bias) { logit_bias_ = std::move(bias); }
+void LLama2Model::set_logit_bias(std::vector<std::pair<int32_t, float>> bias) { draw_.logit_bias = std::move(bias); }
 
-void LLama2Model::set_logprobs(int32_t top_n) { logprobs_top_n_ = top_n; }
+void LLama2Model::set_logprobs(int32_t top_n) { draw_.logprobs_top_n = top_n; }
 
 base::Status LLama2Model::logprobs(int32_t first_pos, int32_t n, std::vector<int32_t>& ids, std::vector<float>& lp,
                                    std::vector<int32_t>& top_ids, std::vector<float>& top_lp) const {
   if (decoder_ == nullptr) return base::error::InternalError("logprobs(): the fused decoder is not initialised");
   if (first_pos < 0 || n < 0) return base::error::InvalidArgument("logprobs(): a range outside the context");
-  const size_t k = logprobs_top_n_ > 0 ? static_cast<size_t>(logprobs_top_n_) : 0;
+  const size_t k = draw_.logprobs_top_n > 0 ? static_cast<size_t>(draw_.logprobs_top_n) : 0;
   ids.assign(n, -1);
   lp.assign(n, 0.f);
   top_ids.assign(k * n, -1);
@@ -165,56 +155,8 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
     const char* env = std::getenv("KUIPER_KV_CACHE");
     bf16_kv_cache_ = env != nullptr && std::string(env) == "bf16";
   }
-  if (!sampling_explicit_) {
-    const char* t = std::getenv("KUIPER_TEMPERATURE");
-    const char* k = std::getenv("KUIPER_TOP_K");
-    const char* sd = std::getenv("KUIPER_SEED");
-    temperature_ = t != nullptr ? std::strtof(t, nullptr) : 0.f;
-    top_k_ = k != nullptr ? static_cast<int32_t>(std::strtol(k, nullptr, 10)) : 0;
-    seed_ = sd != nullptr ? std::strtoull(sd, nullptr, 10) : 0;
-  }
-  if (!std::isfinite(temperature_) || temperature_ < 0.f)
-    return error::InvalidArgument("sampling: the temperature must be finite and >= 0 (KUIPER_TEMPERATURE / set_sampling)");
-  if (!top_p_explicit_) {
-    const char* p = std::getenv("KUIPER_TOP_P");
-    top_p_ = p != nullptr ? std::strtof(p, nullptr) : 1.f;
-  }
-  if (!(top_p_ > 0.f && top_p_ <= 1.f))
-    return error::InvalidArgument("sampling: top_p must be in (0, 1] (KUIPER_TOP_P / set_top_p)");
-  if (!penalty_explicit_) {
-    const char* rp = std::getenv("KUIPER_REPETITION_PENALTY");
-    const char* n = std::getenv("KUIPER_REPEAT_LAST_N");
-    penalty_ = rp != nullptr ? std::strtof(rp, nullptr) : 1.f;
-    repeat_last_n_ = n != nullptr ? static_cast<int32_t>(std::strtol(n, nullptr, 10)) : 0;
-  }
-  if (!std::isfinite(penalty_) || !(penalty_ > 0.f) || repeat_last_n_ < 0)
-    return error::InvalidArgument(
-        "sampling: repetition_penalty must be finite and > 0, and its last_n >= 0 (KUIPER_REPETITION_PENALTY / "
-        "KUIPER_REPEAT_LAST_N / set_repetition_penalty)");
-  if (!frequency_presence_explicit_) {
-    const char* f = std::getenv("KUIPER_FREQUENCY_PENALTY");
-    const char* p = std::getenv("KUIPER_PRESENCE_PENALTY");
-    frequency_ = f != nullptr ? std::strtof(f, nullptr) : 0.f;
-    presence_ = p != nullptr ? std::strtof(p, nullptr) : 0.f;
-    count_from_ = 0;
-  }
-  if (!std::isfinite(frequency_) || !std::isfinite(presence_) || count_from_ < 0)
-    return error::InvalidArgument(
-        "sampling: frequency and presence penalties must be finite, and from_pos >= 0 (KUIPER_FREQUENCY_PENALTY / "
-        "KUIPER_PRESENCE_PENALTY / set_frequency_presence)");
-  {
-    std::vector<int32_t> ids;
-    for (const auto& [id, b] : logit_bias_) {
-      if (id < 0 || !std::isfinite(b))
-        return error::InvalidArgument("sampling: a logit bias needs ids >= 0 and finite values (set_logit_bias)");
-      ids.push_back(id);
-    }
-    std::sort(ids.begin(), ids.end());
-    if (std::adjacent_find(ids.begin(), ids.end()) != ids.end())
-      return error::InvalidArgument("sampling: a logit bias lists an id twice (set_logit_bias)");
-  }
-  if (logprobs_top_n_ < -1 || logprobs_top_n_ > KLLM_MAX_TOP_LOGPROBS)
-    return error::InvalidArgument("logprobs: top_n must be in [-1, 20] (set_logprobs)");
+  sampler::fill_from_env(draw_, draw_set_);
+  if (Status st = sampler::validate(draw_); !st) return st;
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
     return error::InternalError("No usable CUDA device " + std::to_string(tp_.cuda_device()) + ".");
   cuda_config_ = std::make_shared<kernel::CudaConfig>();
@@ -226,9 +168,8 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   init_mem();
   kernel::sin_cos_cache_calc_cu(config_->head_size_, config_->seq_len_, get_buffer(ModelBufferType::kSinCache),
                                 get_buffer(ModelBufferType::kCosCache), cuda_config_->stream);
-  if (temperature_ > 0.f) {
-    auto seeded = std::make_unique<sampler::SeededSampler>(device_type_, temperature_, top_k_, seed_, top_p_, penalty_);
-    seeded->set_penalties(frequency_, presence_, logit_bias_);
+  if (draw_.temperature > 0.f) {
+    auto seeded = std::make_unique<sampler::SeededSampler>(device_type_, draw_);
     seeded_ = seeded.get();
     sampler_ = std::move(seeded);
   } else {
@@ -605,45 +546,7 @@ base::Status LLama2Model::create_decoder() {
         std::string("kllm_decoder_create failed: ") + kllm_error_string(rc) +
         (bf16_kv_cache_ ? " (the bf16 KV cache needs KUIPER_NUMERICS=fast, one GPU and head_size % 32 == 0)" : ""));
   if (bf16_kv_cache_) LOG(INFO) << "KV cache: bf16 (rounded to nearest even as rows are cached)";
-  if (temperature_ > 0.f) {
-    const int src = kllm_decoder_set_sampling_top_p(decoder_, temperature_, top_k_, top_p_, seed_);
-    if (src != 0)
-      return base::error::InternalError(std::string("kllm_decoder_set_sampling_top_p failed: ") +
-                                        kllm_error_string(src));
-    LOG(INFO) << "sampling: temperature " << temperature_ << ", top_k " << top_k_ << ", top_p " << top_p_
-              << ", seed " << seed_;
-  }
-  if (penalty_ != 1.f) {
-    const int prc = kllm_decoder_set_repetition_penalty(decoder_, penalty_, repeat_last_n_);
-    if (prc != 0)
-      return base::error::InternalError(std::string("kllm_decoder_set_repetition_penalty failed: ") +
-                                        kllm_error_string(prc));
-    LOG(INFO) << "sampling: repetition_penalty " << penalty_ << ", last_n " << repeat_last_n_;
-  }
-  if (frequency_ != 0.f || presence_ != 0.f) {
-    const int frc = kllm_decoder_set_frequency_presence(decoder_, frequency_, presence_, count_from_);
-    if (frc != 0)
-      return base::error::InternalError(std::string("kllm_decoder_set_frequency_presence failed: ") +
-                                        kllm_error_string(frc));
-    LOG(INFO) << "sampling: frequency_penalty " << frequency_ << ", presence_penalty " << presence_ << ", from_pos "
-              << count_from_;
-  }
-  if (!logit_bias_.empty()) {
-    std::vector<int32_t> ids;
-    std::vector<float> vals;
-    for (const auto& [id, b] : logit_bias_) ids.push_back(id), vals.push_back(b);
-    const int brc = kllm_decoder_set_logit_bias(decoder_, ids.data(), vals.data(), static_cast<int32_t>(ids.size()));
-    if (brc != 0)
-      return base::error::InvalidArgument(std::string("sampling: kllm_decoder_set_logit_bias refused the map (an id "
-                                                      "outside the vocabulary?): ") + kllm_error_string(brc));
-    LOG(INFO) << "sampling: logit_bias of " << ids.size() << " id(s)";
-  }
-  if (logprobs_top_n_ >= 0) {
-    const int lrc = kllm_decoder_set_logprobs(decoder_, logprobs_top_n_);
-    if (lrc != 0)
-      return base::error::InternalError(std::string("kllm_decoder_set_logprobs failed: ") + kllm_error_string(lrc));
-    LOG(INFO) << "logprobs: top_n " << logprobs_top_n_;
-  }
+  if (base::Status st = sampler::apply_to_decoder(draw_, decoder_); !st) return st;
   LOG(INFO) << "fused decoder engine: " << kllm_decoder_engine(decoder_) << ", "
             << kllm_decoder_launches_per_step(decoder_) << " launch(es) per token";
   LOG(INFO) << "prompt prefill: "
@@ -731,11 +634,11 @@ base::Status LLama2Model::predict(const tensor::Tensor& input, const tensor::Ten
       return base::error::Success();
     }
   }
-  if (sampling_step0_extras())
+  if (draw_.step0_extras())
     return base::error::InvalidArgument(
         "frequency / presence penalty or logit bias: predict() needs a row of the last embedding() call (the layer "
         "path applies them in tools only, from the ids the tool fed)");
-  if (penalty_ != 1.f)
+  if (draw_.step0())
     return base::error::InvalidArgument(
         "repetition_penalty: predict() needs a row of the last embedding() call, whose token id the penalty's "
         "history records (the layer path cannot know the id of another tensor)");

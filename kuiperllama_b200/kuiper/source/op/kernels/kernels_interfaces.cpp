@@ -191,8 +191,7 @@ size_t sampler::SeededSampler::sample(const float* logits, size_t size, void* st
   CHECK(device_type_ == base::DeviceType::kDeviceCUDA) << "SeededSampler: CUDA logits only (no CPU backend)";
   static thread_local int64_t* d_idx = nullptr;
   if (d_idx == nullptr) CHECK(cudaMalloc(reinterpret_cast<void**>(&d_idx), sizeof(int64_t)) == cudaSuccess) << "SeededSampler: cudaMalloc";
-  const bool extras = frequency_ != 0.f || presence_ != 0.f || !bias_ids_.empty();
-  if (penalty_ != 1.f || extras) {  // step 0 on a copy of the logits, then the draw from that copy
+  if (cfg_.step0()) {  // step 0 on a copy of the logits, then the draw from that copy
     static thread_local float* d_pen = nullptr;
     static thread_local size_t pen_cap = 0;
     static thread_local int32_t* d_ids = nullptr;
@@ -202,36 +201,38 @@ size_t sampler::SeededSampler::sample(const float* logits, size_t size, void* st
       CHECK(cudaMalloc(reinterpret_cast<void**>(&d_pen), size * sizeof(float)) == cudaSuccess) << "SeededSampler: cudaMalloc";
       pen_cap = size;
     }
-    // the history, then (with extras) the counted ids behind it
-    const size_t n_ids = history_.size() + (extras ? counted_.size() : 0);
-    if (ids_cap < n_ids) {
+    if (ids_cap < fed_.size()) {
       if (d_ids != nullptr) cudaFree(d_ids);
-      CHECK(cudaMalloc(reinterpret_cast<void**>(&d_ids), n_ids * sizeof(int32_t)) == cudaSuccess)
+      CHECK(cudaMalloc(reinterpret_cast<void**>(&d_ids), fed_.size() * sizeof(int32_t)) == cudaSuccess)
           << "SeededSampler: cudaMalloc";
-      ids_cap = n_ids;
+      ids_cap = fed_.size();
     }
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (!history_.empty())
-      CHECK(cudaMemcpyAsync(d_ids, history_.data(), history_.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s) ==
-            cudaSuccess) << "SeededSampler: copy of the history";
-    if (extras) {
-      if (!counted_.empty())
-        CHECK(cudaMemcpyAsync(d_ids + history_.size(), counted_.data(), counted_.size() * sizeof(int32_t),
-                              cudaMemcpyHostToDevice, s) == cudaSuccess) << "SeededSampler: copy of the counted ids";
+    if (!fed_.empty())
+      CHECK(cudaMemcpyAsync(d_ids, fed_.data(), fed_.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s) ==
+            cudaSuccess) << "SeededSampler: copy of the fed ids";
+    // the windows of sampling.cuh (window_lo, step0_history): H(pos) = fed[rep_lo, pos], C(pos) = fed[cnt_lo, pos]
+    const int32_t n_fed = static_cast<int32_t>(fed_.size());
+    const int32_t rep_lo = std::min(n_fed, cfg_.last_n == 0 ? 0 : std::max(0, pos_ - cfg_.last_n + 1));
+    const int32_t cnt_lo = std::min(n_fed, cfg_.from_pos);
+    if (cfg_.step0_extras()) {
+      std::vector<int32_t> bias_ids;
+      std::vector<float> bias;
+      for (const auto& [id, b] : cfg_.logit_bias) bias_ids.push_back(id), bias.push_back(b);
       const int prc = kllm_logit_penalties_f32(
-          logits, d_pen, static_cast<int64_t>(size), bias_ids_.data(), bias_.data(), static_cast<int32_t>(bias_.size()),
-          penalty_, d_ids, static_cast<int32_t>(history_.size()), frequency_, presence_, d_ids + history_.size(),
-          static_cast<int32_t>(counted_.size()), stream);
+          logits, d_pen, static_cast<int64_t>(size), bias_ids.data(), bias.data(), static_cast<int32_t>(bias.size()),
+          cfg_.penalty, d_ids + rep_lo, n_fed - rep_lo, cfg_.frequency, cfg_.presence, d_ids + cnt_lo, n_fed - cnt_lo,
+          stream);
       CHECK(prc == 0) << "kllm_logit_penalties_f32: " << kllm_error_string(prc);
     } else {
-      const int prc = kllm_repetition_penalty_f32(logits, d_pen, static_cast<int64_t>(size), d_ids,
-                                                  static_cast<int32_t>(history_.size()), penalty_, stream);
+      const int prc = kllm_repetition_penalty_f32(logits, d_pen, static_cast<int64_t>(size), d_ids + rep_lo,
+                                                  n_fed - rep_lo, cfg_.penalty, stream);
       CHECK(prc == 0) << "kllm_repetition_penalty_f32: " << kllm_error_string(prc);
     }
     logits = d_pen;
   }
-  const int rc =
-      kllm_sample_top_p_f32(logits, static_cast<int64_t>(size), temperature_, top_k_, top_p_, seed_, pos_, d_idx, stream);
+  const int rc = kllm_sample_top_p_f32(logits, static_cast<int64_t>(size), cfg_.temperature, cfg_.top_k, cfg_.top_p,
+                                       cfg_.seed, pos_, d_idx, stream);
   CHECK(rc == 0) << "kllm_sample_top_p_f32: " << kllm_error_string(rc);
   int64_t h = -1;
   cudaStream_t s = static_cast<cudaStream_t>(stream);

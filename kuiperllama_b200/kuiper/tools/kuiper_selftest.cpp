@@ -13,6 +13,7 @@
 #include <tensor/tensor.h>
 
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <functional>
 #include <memory>
@@ -34,6 +35,12 @@ struct ModelInspector {
   static const char* payload(const LLama2Model& m) { return static_cast<const char*>(m.raw_model_data_->weight_data); }
   static size_t file_size(const LLama2Model& m) { return m.raw_model_data_->file_size; }
   static int32_t group_size(const LLama2Model& m) { return m.group_size_; }
+  // the draw settings init() goes on to validate
+  static sampler::DrawConfig draw_from_env(const LLama2Model& m) {
+    sampler::DrawConfig cfg = m.draw_;
+    sampler::fill_from_env(cfg, m.draw_set_);
+    return cfg;
+  }
 };
 }  // namespace model
 
@@ -181,6 +188,33 @@ int main(int argc, char** argv) {
     EXPECT(mm.get_scale_num() == 4);
     // export.py --version 3: the fp32 group scales sit right behind the int8 block
     EXPECT(static_cast<const void*>(mm.get_scales().ptr<float>()) == static_cast<const void*>(blob.data() + 4 * 64));
+  });
+
+  run("draw settings: each group from its setter, else from its KUIPER_* variables, else the default", [&] {
+    const char* vars[][2] = {{"KUIPER_TEMPERATURE", "0.5"}, {"KUIPER_TOP_K", "7"}, {"KUIPER_SEED", "9"},
+                             {"KUIPER_TOP_P", "0.5"}, {"KUIPER_REPETITION_PENALTY", "1.5"}, {"KUIPER_REPEAT_LAST_N", "4"},
+                             {"KUIPER_FREQUENCY_PENALTY", "0.25"}, {"KUIPER_PRESENCE_PENALTY", "0.75"}};
+    // the defaults, the values of `vars` and the values the setters below are given
+    const sampler::DrawConfig unset, env{0.5f, 7, 9, 0.5f, 1.5f, 4, 0.25f, 0.75f, 0},
+        set{0.875f, 3, 11, 0.625f, 1.25f, 2, 0.125f, 0.375f, 5};
+    auto group = [](const sampler::DrawConfig& c, int g) {  // the fields of group g
+      return std::vector<std::vector<double>>{{c.temperature, double(c.top_k), double(c.seed)}, {c.top_p},
+                                              {c.penalty, double(c.last_n)},
+                                              {c.frequency, c.presence, double(c.from_pos)}}[g];
+    };
+    // init()'s settings with or without the variables, after the setters of the groups in `mask`
+    auto expect = [&](bool env_on, unsigned mask) {
+      for (const auto& v : vars) env_on ? setenv(v[0], v[1], 1) : unsetenv(v[0]);
+      model::LLama2Model m(TokenizerType::kEncodeSpe, "<none>", "<none>", false);
+      if (mask & 1) m.set_sampling(set.temperature, set.top_k, set.seed);
+      if (mask & 2) m.set_top_p(set.top_p);
+      if (mask & 4) m.set_repetition_penalty(set.penalty, set.last_n);
+      if (mask & 8) m.set_frequency_presence(set.frequency, set.presence, set.from_pos);
+      const sampler::DrawConfig c = model::ModelInspector::draw_from_env(m);
+      for (int g = 0; g < 4; ++g) EXPECT(group(c, g) == group(mask >> g & 1 ? set : env_on ? env : unset, g));
+    };
+    for (unsigned mask : {0u, 1u, 2u, 4u, 8u, 15u}) expect(true, mask);  // the environment only, one setter each, all
+    expect(false, 15), expect(false, 0);                                   // the setters only; neither
   });
 
   if (argc > 1) {

@@ -4,7 +4,8 @@ after the host suite, whose build it uses.)
 
 kuiper_decode prints the same ids as the C-ABI decoder with the same settings on the fused path (predict() on
 embedding rows) and on the layer path (--layers: SeededSampler's kllm_logit_penalties_f32 over the ids the tool fed),
-greedy and sampled, and through LLama2Model::generate().  Invalid settings are refused by init()."""
+greedy and sampled, and through LLama2Model::generate().  A bias id outside the vocabulary is refused once the decoder
+exists (the other invalid settings: test_z_host_cpp_draw_settings.py)."""
 import os
 import subprocess
 
@@ -84,13 +85,10 @@ def test_cpp_environment_and_generate(kllm_lib, tmp_path, key, variant, family, 
     assert ids_of(r) == probe[:N]
 
 
-@pytest.mark.parametrize("args", [["--frequency-presence", "nan", "0"], ["--frequency-presence", "0", "inf"],
-                                  ["--frequency-presence", "0.5", "0", "-1"], ["--logit-bias", "3:1,3:2"],
-                                  ["--logit-bias", "3:nan"], ["--logit-bias", "100000000:1"]])
-def test_cpp_refuses_invalid_settings(kllm_lib, tmp_path, args):
+def test_cpp_refuses_a_bias_id_outside_the_vocabulary(kllm_lib, tmp_path):
     _, _, path = checkpoint(tmp_path, "small", "cpu")
-    r = subprocess.run([str(ensure_built("llama2")), str(path), "llama", "fp32", "8", "1", "5", *args],
-                       capture_output=True, text=True, timeout=300)
+    r = subprocess.run([str(ensure_built("llama2")), str(path), "llama", "fp32", "8", "1", "5", "--logit-bias",
+                        "100000000:1"], capture_output=True, text=True, timeout=300)
     assert r.returncode != 0 and "init failed" in r.stderr, (r.returncode, r.stderr)
 
 

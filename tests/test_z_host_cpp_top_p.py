@@ -51,15 +51,3 @@ def test_cpp_top_p_identical_to_cabi(kllm_lib, tmp_path, key, variant, family, p
         assert r.returncode == 0, r.stderr
         assert [int(x) for x in r.stdout.split()][len(prompt) - 1:] == want, ("--top-p", extra)
     assert "top_p" in r.stderr  # init() logs the setting
-
-
-@pytest.mark.parametrize("value", ["0", "-0.5", "1.5", "nan"])
-def test_cpp_refuses_invalid_top_p(kllm_lib, tmp_path, value):
-    from kuiperllama_b200 import SHAPES, synth_weights
-    from kuiperllama_b200.checkpoint import write_checkpoint
-    shape = SHAPES["small"]
-    path = tmp_path / "small.bin"
-    write_checkpoint(str(path), shape, synth_weights(shape, "cpu", 77))
-    env = dict(os.environ, KUIPER_TEMPERATURE="0.8", KUIPER_TOP_P=value)
-    r = run_decode("llama2", path, "llama", "fp32", 8, [1, 5], env=env)
-    assert r.returncode != 0 and "top_p" in r.stderr, (r.returncode, r.stderr)
