@@ -465,6 +465,12 @@ int kllm_decoder_classifier_rows(const kllm_decoder* dec);
  * ring; "graph": CUDA-graph chain of fused launches (shapes the ring does not handle, tensor
  * parallel).  Environment KLLM_ENGINE=graph|persistent forces a choice at create time. */
 const char* kllm_decoder_engine(const kllm_decoder* dec);
+/* Persistent engine only (KLLM_E_UNSUPPORTED on the graph engine): the attention geometry create chose.
+ * tile: timesteps per K ring stage (the flash form's K and V tile); split: CTAs per query head (the
+ * exact form splits the V dims into head_size / split slices, the flash form the timesteps);
+ * tile_v: timesteps per V ring stage; stage_bytes: bytes per ring stage. */
+int kllm_decoder_attention_geometry(const kllm_decoder* dec, int* tile, int* split, int* tile_v,
+                                    int* stage_bytes);
 /* Persistent engine only: run n_steps positions and record, for step `profiled_step`, sixteen
  * stamps per CTA per schedule phase into stamps_host[grid][phases][16] (capacity in uint64
  * elements).  Globaltimer ns: [0] phase entered, [1] input vector staged (+normalised), [2] last

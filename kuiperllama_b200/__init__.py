@@ -129,6 +129,8 @@ _SIGNATURES = {
     "kllm_decoder_launches_per_step": (c_int, [c_void_p]),
     "kllm_decoder_classifier_rows": (c_int, [c_void_p]),
     "kllm_decoder_engine": (c_char_p, [c_void_p]),
+    "kllm_decoder_attention_geometry": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int),
+                                                POINTER(c_int)]),
     "kllm_decoder_profile": (c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32,
                                      POINTER(c_int32), POINTER(c_int32)]),
 }

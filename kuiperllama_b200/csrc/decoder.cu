@@ -948,5 +948,14 @@ const char* kllm_decoder_engine(const kllm_decoder* dc) {
   if (!dc) return "";
   return dc->use_mega ? "persistent" : "graph";
 }
+int kllm_decoder_attention_geometry(const kllm_decoder* dc, int* tile, int* split, int* tile_v, int* stage_bytes) {
+  if (!dc || !tile || !split || !tile_v || !stage_bytes) return KLLM_E_INVALID;
+  if (!dc->use_mega) return KLLM_E_UNSUPPORTED;
+  *tile = dc->mega.attn_tile();
+  *split = dc->mega.attn_split();
+  *tile_v = dc->mega.attn_tile_v();
+  *stage_bytes = dc->mega.stage_bytes();
+  return 0;
+}
 
 }  // extern "C"

@@ -220,6 +220,10 @@ class MegaEngine {
   int grid() const { return grid_; }
   int phases() const { return n_phases_; }
   int attn_vsplit() const { return attn_vsplit_; }  // slices of the V cache layout
+  int attn_tile() const { return attn_tile_; }      // timesteps per K (flash: K and V) ring stage
+  int attn_split() const { return attn_split_; }    // CTAs per query head
+  int attn_tile_v() const { return attn_tile_v_; }  // timesteps per V ring stage
+  int stage_bytes() const { return stage_bytes_; }
   int cls_rows() const { return cls_rows_; }  // classifier rows this rank streams per token
 
  private:

@@ -224,6 +224,15 @@ class Decoder:
     def engine(self) -> str:
         return self.lib.kllm_decoder_engine(self.handle).decode()
 
+    @property
+    def attention_geometry(self):
+        """(tile, split, tile_v, stage_bytes) of the persistent engine's attention
+        (kllm_decoder_attention_geometry); KllmError on the graph engine."""
+        out = [ctypes.c_int(0) for _ in range(4)]
+        check(self.lib.kllm_decoder_attention_geometry(self.handle, *[ctypes.byref(v) for v in out]),
+              "kllm_decoder_attention_geometry")
+        return tuple(v.value for v in out)
+
     def step(self, token: int, pos: int, is_prompt: bool = False) -> int:
         """Reference-facing call with host buffers (predict + post_processing)."""
         nxt = ctypes.c_int32(-1)

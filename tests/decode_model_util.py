@@ -21,17 +21,17 @@ from kuiperllama_b200 import FLAVOURS, SHAPES, Decoder, ModelShape, synth_weight
 from kuiperllama_b200.decoder import quantize_q80
 
 KV_TAU_FIRST = 1e-5  # layer 0 of every case: 2.47e-6, 2.43e-6
-KV_TAU = 6e-5  # layers 1 and 2: 2.51e-5, 1.37e-5
-LOGIT_TAU = 8e-5  # 3.22e-5, 2.08e-5
+KV_TAU = 6e-5  # layers 1 and 2: 2.51e-5, 1.39e-5
+LOGIT_TAU = 8e-5  # 2.57e-5, 2.08e-5
 # TinyLlama-1.1B, 22 layers (synth weights: smaller errors than the loud 2 to 3 layer cases)
-KV_TAU_DEEP = 2e-5  # layers 1 .. 21: 6.32e-6, 5.23e-6
-LOGIT_TAU_DEEP = 2e-5  # 5.39e-6, 4.59e-6
+KV_TAU_DEEP = 2e-5  # layers 1 .. 21: 6.32e-6, 5.24e-6
+LOGIT_TAU_DEEP = 2e-5  # 5.88e-6, 4.94e-6
 
 KNOBS = ("KLLM_ENGINE", "KLLM_MODE", "KLLM_ATTN_SPLIT", "KLLM_STAGE_BYTES")
 
 
-def report(*parts):
-    print("[decode-model]", *parts, flush=True)
+def report(*parts, tag="[decode-model]"):
+    print(tag, *parts, flush=True)
 
 
 # ---- weights --------------------------------------------------------------------------------------------------
@@ -81,22 +81,42 @@ WEIGHTS = {"synth": lambda shape, device, seed: synth_weights(shape, device, see
            "loud": loud_weights, "outliers": outlier_weights}
 
 
-# ---- the persistent engine's flash geometry (MegaEngine::init) ---------------------------------------------------
-def flash_geometry(shape, env, sms):
-    """(tile T, split SP) the fast mode runs with under `env`: T = min(stage_bytes / (hs * 4), 8 warps * 32) & ~31,
-    SP = the largest power of two <= 8 with heads * SP <= grid and SP * (hs + 2) <= seq_len unless KLLM_ATTN_SPLIT
-    asks for a smaller one (a larger one is ignored)."""
+# ---- the persistent engine's attention geometry (MegaEngine::init) -----------------------------------------------
+def engine_geometry(shape, numerics, env, sms, kv_cache="fp32"):
+    """(tile T, split SP, V tile, stage bytes) the persistent engine chooses, which Decoder.attention_geometry
+    reports; every persistent case asserts the two agree, so that a change to the rules fails loudly instead of
+    moving the segment ends off the tiles' edges.
+    Stage: KLLM_STAGE_BYTES, else 27 KB for int8, 16 KB for fp32 in the fast mode with an fp32 cache when two input
+    rows of dim fit (dim <= 2048), else 32 KB; rounded up to 128 bytes.  T = min(stage / (hs * elem), 256) & ~31.
+    Split: the largest power of two <= 8 with heads * SP <= grid and, in the fast mode, SP * (hs + 2) <= seq_len, in
+    the exact mode hs / SP a multiple of 4 (the exact mode splits only head sizes >= 128 unless asked); a
+    KLLM_ATTN_SPLIT power of two up to that cap replaces it.  V tile: stage / ((hs / SP) * elem) & ~31 in the exact
+    mode (V slices of hs / SP dims), stage / (hs * elem) & ~31 in the fast mode."""
     int8 = shape.group_size != 0
+    fast = numerics == "fast"
+    bf16 = kv_cache == "bf16"
     hs = shape.head_size
-    stage = int(env.get("KLLM_STAGE_BYTES", 27 * 1024 if int8 else 32 * 1024))
+    small_stages = fast and not bf16 and 2 * shape.dim * 4 <= 16 * 1024
+    stage = int(env.get("KLLM_STAGE_BYTES", 27 * 1024 if int8 else 16 * 1024 if small_stages else 32 * 1024))
     stage = (stage + 127) & ~127
-    T = min(stage // (hs * 4), 8 * 32) & ~31
+    esz = 2 if bf16 else 4
+    T = min(stage // (hs * esz), 8 * 32) & ~31
     grid = min(sms, shape.dim, shape.hidden_dim)
     cap = 1
-    while cap * 2 <= 8 and shape.head_num * cap * 2 <= grid and cap * 2 * (hs + 2) <= shape.seq_len:
+    while cap * 2 <= 8 and shape.head_num * cap * 2 <= grid and (
+            cap * 2 * (hs + 2) <= shape.seq_len if fast else (hs // (cap * 2)) % 4 == 0 and hs % (cap * 2) == 0):
         cap *= 2
-    sp = int(env.get("KLLM_ATTN_SPLIT", cap))
-    return T, sp if sp <= cap else cap
+    sp = cap if fast or hs >= 128 else 1
+    asked = int(env.get("KLLM_ATTN_SPLIT", 0))
+    if 1 <= asked <= cap and (asked & (asked - 1)) == 0:
+        sp = asked
+    T_v = (stage // ((hs // (1 if fast else sp)) * esz)) & ~31
+    return T, sp, T_v, stage
+
+
+def flash_geometry(shape, env, sms):
+    """(tile T, split SP) of the fast mode with an fp32 cache under `env` (engine_geometry)."""
+    return engine_geometry(shape, "fast", env, sms)[:2]
 
 
 def split_cap(shape, sms):
@@ -114,21 +134,23 @@ def sms():
 
 
 # ---- the persistent engine's cases (test_decode_model_gpu.py), which the graph engine repeats ---------------
+# The flash tile T of the fast mode's default 16 KB stages (fp32 up to dim 2048; engine_geometry) and 27 KB (int8)
 GEOMETRIES = {
     # dim 64, 4 / 2 heads: head_size 16, T = 256, 8 CTAs per head
     "hs16": ModelShape("decode-hs16", 64, 172, 2, 4, 2, 512, 2080),
-    "small": replace(SHAPES["small"], seq_len=2080),  # head_size 32, GQA 3, T = 256
-    "small-hs48": replace(SHAPES["small-hs48"], seq_len=1312),  # T = 160
-    "hs128": ModelShape("decode-hs128", 512, 1376, 2, 4, 2, 2048, 1056),  # T = 64
-    "small-qwen": replace(SHAPES["small-qwen"], seq_len=1056),  # bias, half-split pairs, eps 1e-6, T = 128
-    # Llama-3-8B attention geometry and vocabulary at two layers: half-split pairs, theta 5e5
+    "small": replace(SHAPES["small"], seq_len=2080),  # head_size 32, GQA 3, T = 128
+    "small-hs48": replace(SHAPES["small-hs48"], seq_len=1312),  # T = 64
+    "hs128": ModelShape("decode-hs128", 512, 1376, 2, 4, 2, 2048, 1056),  # T = 32
+    "small-qwen": replace(SHAPES["small-qwen"], seq_len=1056),  # bias, half-split pairs, eps 1e-6, T = 64
+    # Llama-3-8B attention geometry and vocabulary at two layers: half-split pairs, theta 5e5; 32 KB stages, T = 64
     "llama3-reduced": ModelShape("llama3-reduced", 4096, 14336, 2, 32, 8, 128256, 544, flavour="llama3"),
     "small-int8": replace(SHAPES["small-int8"], seq_len=800),  # T = 96
     "small-tp-int8": replace(SHAPES["small-tp-int8"], seq_len=800),
     # Llama-2-7B int8 at two layers: T = 32, 4 CTAs per head
     "llama2-7b-int8-2l": replace(SHAPES["llama2-7b-int8"], layer_num=2, seq_len=544),
-    "qwen2.5-reduced": ModelShape("qwen2.5-reduced", 896, 4864, 2, 14, 2, 4096, 16384, True, flavour="qwen2"),
-    "tinyllama-1.1b": replace(SHAPES["tinyllama-1.1b"], seq_len=1024),
+    "qwen2.5-reduced": ModelShape("qwen2.5-reduced", 896, 4864, 2, 14, 2, 4096, 16384, True,
+                                  flavour="qwen2"),  # T = 64
+    "tinyllama-1.1b": replace(SHAPES["tinyllama-1.1b"], seq_len=1024),  # T = 64
 }
 # (geometry, weights, environment of the fast mode)
 CASES = [("hs16", "loud", {}), ("small", "synth", {}), ("small", "loud", {}), ("small-hs48", "loud", {}),
@@ -187,17 +209,21 @@ def cached_model(lib, key, shape, weights, ends):
 
 
 # ---- decoders and checks -------------------------------------------------------------------------------------------
-def make_decoder(monkeypatch, shape, w, numerics, env, engine="persistent"):
-    """A decoder with every engine knob cleared, then `env` set; `engine` None leaves the choice to the library."""
+def make_decoder(monkeypatch, shape, w, numerics, env, engine="persistent", kv_cache="fp32"):
+    """A decoder with every engine knob cleared, then `env` set; `engine` None leaves the choice to the library.
+    On the persistent engine, the attention geometry it reports must be engine_geometry's."""
     for name in KNOBS:
         monkeypatch.delenv(name, raising=False)
     if engine is not None:
         monkeypatch.setenv("KLLM_ENGINE", engine)
     for name, value in env.items():
         monkeypatch.setenv(name, value)
-    dec = Decoder(shape, w, numerics=numerics)
+    dec = Decoder(shape, w, numerics=numerics, kv_cache=kv_cache)
     if engine is not None:
         assert dec.engine == engine
+    if dec.engine == "persistent":
+        want = engine_geometry(shape, numerics, env, sms(), kv_cache)
+        assert dec.attention_geometry == want, (shape.name, numerics, env, kv_cache, dec.attention_geometry, want)
     return dec
 
 
@@ -223,7 +249,8 @@ def fmt(per_layer):
     return {k: [float(f"{x:.3g}") for x in v] for k, v in per_layer.items()}
 
 
-def run(what, dec, shape, toks, ref, ends, kv_tau, logit_tau, plain=None, kv_tau_first=KV_TAU_FIRST):
+def run(what, dec, shape, toks, ref, ends, kv_tau, logit_tau, plain=None, kv_tau_first=KV_TAU_FIRST,
+        tag="[decode-model]"):
     """Teacher-force toks over every position in segments ending at `ends`; check the logits at each end and
     every K / V row at the end.  Returns (the cache, {end: logits})."""
     start, worst_logit, worst_end, worst_plain = 0, 0.0, 0, 0.0
@@ -246,11 +273,11 @@ def run(what, dec, shape, toks, ref, ends, kv_tau, logit_tau, plain=None, kv_tau
     assert start == shape.seq_len
     kv = dec.kv_cache()
     per_layer = kv_ratios(kv, ref, kv_tau, kv_tau_first)
-    report(what, f"segments {ends}")
-    report(what, f"logits err / bound {worst_logit:.3g}; K / V err / bound per layer {fmt(per_layer)}")
+    report(what, f"segments {ends}", tag=tag)
+    report(what, f"logits err / bound {worst_logit:.3g}; K / V err / bound per layer {fmt(per_layer)}", tag=tag)
     if plain is not None:
         report(what, f"fixed point's cost, against the plain model: logits err / rms {worst_plain:.3g}; "
-                     f"K / V err / rms per layer {fmt(kv_ratios(kv, plain, 1.0, 1.0))}")
+                     f"K / V err / rms per layer {fmt(kv_ratios(kv, plain, 1.0, 1.0))}", tag=tag)
     assert worst_logit <= 1.0, (what, worst_end, worst_logit)
     for name, v in per_layer.items():
         assert max(v) <= 1.0, (what, name, v)
@@ -259,3 +286,15 @@ def run(what, dec, shape, toks, ref, ends, kv_tau, logit_tau, plain=None, kv_tau
 
 def same_bits(a, b):
     return np.array_equal(np.ascontiguousarray(a).view(np.uint32), np.ascontiguousarray(b).view(np.uint32))
+
+
+def compare_engines(what, shape, ends, a, b):
+    """Two (cache, {end: logits}) results bit for bit; names the first differing layer and position."""
+    (ka, la), (kb, lb) = a, b
+    for end in ends:
+        assert same_bits(la[end], lb[end]), (what, "logits", end)
+    for name, x, y in (("K", ka[0], kb[0]), ("V", ka[1], kb[1])):
+        for l in range(shape.layer_num):
+            if not same_bits(x[l], y[l]):
+                rows = np.nonzero((x[l].view(np.uint32) != y[l].view(np.uint32)).any(-1))[0]
+                raise AssertionError(f"{what}: {name} layer {l} differs first at position {rows[0]}")

@@ -5,7 +5,9 @@ fp32 model; the fast mode is the same model with the input of every int8 project
 point (`fixed_point=True`, a mirror of quantize_input_inplace), and flash-decoding attention, which only reorders
 the softmax sums.  Each case teacher-forces one seeded sequence over every position 0 .. seq_len - 1 in segments
 that end on the flash tiles' edges, compares the logits at every segment end, and then the K / V cache rows of
-every layer at every position.  Bounds take the form of test_prefill_tf32_model_gpu.py: each K / V element within
+every layer at every position.  The edges come from decode_model_util.engine_geometry, and every decoder asserts
+that the geometry the engine reports (Decoder.attention_geometry) is that one, so the ends cannot drift off the
+engine's tiles unnoticed.  Bounds take the form of test_prefill_tf32_model_gpu.py: each K / V element within
 KV_TAU * rms(row), the logits within LOGIT_TAU * rms(logits), and the greedy id equal to the model's argmax
 wherever the model's top-2 margin exceeds twice the logit bound.  The fast mode is also measured against the plain
 model: that distance is what the fixed point costs.
@@ -27,10 +29,10 @@ H100 80GB HBM3 at a 700 W power limit.  The fast mode's worst stays within 2x of
 so both modes share each constant.  Layer 0's rows come before any attention, so they have a constant of their
 own, tight enough that a quantiser with two digit planes misses it by 20x (tests/test_decode_model.py).
     KV_TAU_FIRST    1e-5  layer 0, every case:  exact 2.47e-6, fast 2.43e-6 (llama2-7b-int8-2l outliers)
-    KV_TAU          6e-5  later layers:         exact 2.51e-5 (small-hs48 loud), fast 1.37e-5 (small loud, T 128, SP 2)
-    LOGIT_TAU       8e-5                        exact 3.22e-5 (small-hs48 loud), fast 2.08e-5 (small loud)
-    KV_TAU_DEEP     2e-5  TinyLlama, 22 layers: exact 6.32e-6, fast 5.23e-6
-    LOGIT_TAU_DEEP  2e-5                        exact 5.39e-6, fast 4.59e-6
+    KV_TAU          6e-5  later layers:         exact 2.51e-5 (small-hs48 loud), fast 1.39e-5 (small loud, T 192, SP 2)
+    LOGIT_TAU       8e-5                        exact 2.57e-5 (small-hs48 loud), fast 2.08e-5 (small loud, T 256, SP 8)
+    KV_TAU_DEEP     2e-5  TinyLlama, 22 layers: exact 6.32e-6, fast 5.24e-6
+    LOGIT_TAU_DEEP  2e-5                        exact 5.88e-6, fast 4.94e-6
 The fixed point's cost, the fast mode against the plain model: K / V within 6.4e-6 of the row rms and logits within
 7.0e-6 of their rms (llama2-7b-int8-2l outliers); 1e-6 to 3e-6 on the synth weights.
 """
@@ -115,8 +117,8 @@ def test_fast_decode_tiles_and_splits(kllm_lib, monkeypatch, key, T):
     for sp in SWEEP_SPLITS:
         assert sp <= split_cap(shape, sms()), (key, sp)
         env = sweep_env(shape, T, sp)
-        assert flash_geometry(shape, env, sms()) == (T, sp)
         dec = make_decoder(monkeypatch, shape, w, "fast", env)
+        assert dec.attention_geometry[:2] == (T, sp), (key, dec.attention_geometry)
         caches[sp] = run(f"{key} loud fast T={T} SP={sp}", dec, shape, toks, plain,
                          edge_ends(T, sp, shape.seq_len), KV_TAU, LOGIT_TAU)[0]
         dec.close()

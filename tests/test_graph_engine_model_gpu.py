@@ -43,8 +43,8 @@ import pytest
 import torch
 
 from conftest import GOLDEN
-from decode_model_util import (CASES, GEOMETRIES, KV_TAU, LOGIT_TAU, cached_model, case_id,
-                               clear_cache, device_sincos, edge_ends, flash_geometry, make_decoder, report, run,
+from decode_model_util import (CASES, GEOMETRIES, KV_TAU, LOGIT_TAU, cached_model, case_id, clear_cache,
+                               compare_engines, device_sincos, edge_ends, flash_geometry, make_decoder, report, run,
                                same_bits, sequence, sms, taus)
 from prefill_model import prefill_ref
 
@@ -57,18 +57,6 @@ pytestmark = pytest.mark.gpu
 def _free():
     yield
     clear_cache()
-
-
-def compare_engines(what, shape, ends, a, b):
-    """Two (cache, {end: logits}) results bit for bit; names the first differing layer and position."""
-    (ka, la), (kb, lb) = a, b
-    for end in ends:
-        assert same_bits(la[end], lb[end]), (what, "logits", end)
-    for name, x, y in (("K", ka[0], kb[0]), ("V", ka[1], kb[1])):
-        for l in range(shape.layer_num):
-            if not same_bits(x[l], y[l]):
-                rows = np.nonzero((x[l].view(np.uint32) != y[l].view(np.uint32)).any(-1))[0]
-                raise AssertionError(f"{what}: {name} layer {l} differs first at position {rows[0]}")
 
 
 # ---- 1. the persistent cases on the graph engine --------------------------------------------------------------------

@@ -284,7 +284,7 @@ def mha_fp64(q, kc, vc, pos, layer, heads, kv_heads, head_size):
     return out, p, mag, a.amax(-1, keepdim=True), spread
 
 
-MHA_HEADS = [16, 32, 160, 188, 192, 256]
+MHA_HEADS = [8, 16, 20, 32, 80, 96, 100, 112, 124, 160, 188, 192, 256]
 
 
 @pytest.mark.parametrize("head_size", MHA_HEADS)

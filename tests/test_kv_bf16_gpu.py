@@ -26,7 +26,8 @@ import numpy as np
 import pytest
 import torch
 
-from decode_model_util import CASES, GEOMETRIES, KNOBS, WEIGHTS, case_id, device_sincos, sequence, sms, taus
+from decode_model_util import (CASES, GEOMETRIES, KNOBS, WEIGHTS, case_id, device_sincos, engine_geometry, sequence, sms,
+                               taus)
 from kv_bf16_model import bf16_rne, prefill_ref_bf16
 from prefill_model import prefill_ref
 
@@ -58,16 +59,9 @@ def make(monkeypatch, shape, w, env=None, kv_cache="bf16", numerics="fast"):
 
 
 def bf16_geometry(shape, env):
-    """(T, SP) of the flash form with a bf16 cache: T = min(stage / (hs * 2), 256) & ~31; the split as fp32's."""
-    int8 = shape.group_size != 0
-    stage = (int(env.get("KLLM_STAGE_BYTES", 27 * 1024 if int8 else 32 * 1024)) + 127) & ~127
-    T = min(stage // (shape.head_size * 2), 256) & ~31
-    grid = min(sms(), shape.dim, shape.hidden_dim)
-    cap = 1
-    while cap * 2 <= 8 and shape.head_num * cap * 2 <= grid and cap * 2 * (shape.head_size + 2) <= shape.seq_len:
-        cap *= 2
-    sp = int(env.get("KLLM_ATTN_SPLIT", cap))
-    return T, min(sp, cap)
+    """(T, SP) of the flash form with a bf16 cache: T = min(stage / (hs * 2), 256) & ~31; the split as fp32's
+    (decode_model_util.engine_geometry)."""
+    return engine_geometry(shape, "fast", env, sms(), "bf16")[:2]
 
 
 def ends_for(T, SP, seq_len):
@@ -84,10 +78,15 @@ def ulp_bf16(x):
 @pytest.mark.parametrize("key,weights,env", BF16_CASES, ids=[case_id(c) for c in BF16_CASES])
 def test_bf16_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env):
     shape = GEOMETRIES[key]
-    kv_tau, logit_tau = taus(key)
+    decode_against_the_bf16_model(kllm_lib, monkeypatch, case_id((key, weights, env)), shape,
+                                  WEIGHTS[weights](shape, "cuda", 77), env, *taus(key))
+
+
+def decode_against_the_bf16_model(kllm_lib, monkeypatch, what, shape, w, env, kv_tau, logit_tau, tag="[kv-bf16]"):
+    """One bf16-cache decoder teacher-forced over every position in segments ending on the edges of the tiles it
+    reports (which must be bf16_geometry's), held to the bounds of the module docstring."""
     T, SP = bf16_geometry(shape, env)
     ends = ends_for(T, SP, shape.seq_len)
-    w = WEIGHTS[weights](shape, "cuda", 77)
     toks = sequence(shape.vocab_size, shape.seq_len, 5)
     sin, cos = device_sincos(kllm_lib, shape)
     fixed = shape.group_size == 64
@@ -96,6 +95,7 @@ def test_bf16_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env)
     plain = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends, fixed_point=fixed)
     dec = make(monkeypatch, shape, w, env)
     assert dec.engine == "persistent"
+    assert dec.attention_geometry == engine_geometry(shape, "fast", env, sms(), "bf16"), (what, dec.attention_geometry)
     start, logits = 0, {}
     for end in ends:
         dec.generate(0, start, end + 1 - start, teacher=toks[start:end + 1])
@@ -113,7 +113,7 @@ def test_bf16_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env)
         bound = ulp_bf16(want) + kv_tau * rms
         r = float(((got.double() - want).abs() / bound).max())
         worst_kv = max(worst_kv, r)
-        assert r <= 1.0, (key, name, r)
+        assert r <= 1.0, (what, name, r)
     # (2) the logits against the model fed the GPU's own cache rows, (3) against the fp32-cache model
     worst_own, worst_plain, rule_dist = 0.0, 0.0, 0.0
     for end in ends:
@@ -123,11 +123,11 @@ def test_bf16_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env)
         rule_dist = max(rule_dist, float((model["logits_at"][end] - plain["logits_at"][end]).abs().max()) / rms)
         worst_plain = max(worst_plain, float((logits[end] - plain["logits_at"][end]).abs().max()) / rms)
     plain_bound = BF16_GAIN * rule_dist + logit_tau
-    report(f"{case_id((key, weights, env))} T={T} SP={SP}: K/V err / (ulp + tau rms) {worst_kv:.3g}; logits err / "
-           f"fast bound vs model on GPU rows {worst_own:.3g}; vs fp32-cache model err / rms {worst_plain:.3g} "
-           f"(bound {plain_bound:.3g}, bf16 model's own distance {rule_dist:.3g})")
-    assert worst_own <= 1.0, (key, worst_own)
-    assert worst_plain <= plain_bound, (key, worst_plain, plain_bound)
+    print(tag, f"{what} T={T} SP={SP}: K/V err / (ulp + tau rms) {worst_kv:.3g}; logits err / "
+          f"fast bound vs model on GPU rows {worst_own:.3g}; vs fp32-cache model err / rms {worst_plain:.3g} "
+          f"(bound {plain_bound:.3g}, bf16 model's own distance {rule_dist:.3g})", flush=True)
+    assert worst_own <= 1.0, (what, worst_own)
+    assert worst_plain <= plain_bound, (what, worst_plain, plain_bound)
     dec.close()
 
 
