@@ -10,6 +10,9 @@
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
+#include <map>
+#include <mutex>
+#include <utility>
 #include <vector>
 
 #include "../../include/kllm_b200.h"
@@ -22,6 +25,21 @@ namespace kllm {
 std::atomic<uint64_t>& launch_counter() {
   static std::atomic<uint64_t> c{0};
   return c;
+}
+
+int smem_opt_in(const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, size_t> granted;  // (device, kernel) -> the attribute's value
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return KLLM_E_NODEVICE;
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& have = granted[{dev, kernel}];
+  if (bytes <= have) return 0;
+  const cudaError_t e =
+      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+  if (e != cudaSuccess) return static_cast<int>(e);
+  have = bytes;
+  return 0;
 }
 
 // ---- rmsnorm: rmsnorm_kernel.cu:4-50 (one 128-thread block there; one warp carrying the

@@ -13,6 +13,12 @@ namespace kllm {
 std::atomic<uint64_t>& launch_counter();
 inline void count_launch(uint64_t n = 1) { launch_counter().fetch_add(n, std::memory_order_relaxed); }
 
+// Opt `kernel` in to `bytes` of dynamic shared memory on the current device.  The attribute belongs to the kernel
+// function, one value per device for the whole process, and every live decoder launches the same instantiations at
+// its own size: so the value only ever rises, to the largest size any caller has asked for (a later decoder's smaller
+// request must not refuse an earlier one's launches).  Each launch still passes its own size.  Thread-safe.
+int smem_opt_in(const void* kernel, size_t bytes);
+
 // A position that is either a host value or read from device memory at kernel run time; the
 // decoder's CUDA graph uses the device form so ONE captured graph serves every position.
 struct PosArg {

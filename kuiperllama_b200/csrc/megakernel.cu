@@ -2672,17 +2672,12 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     return static_cast<int>(cudaErrorMemoryAllocation);
   cudaStreamSynchronize(stream);  // ph (host vector) must outlive the async copy
 
-  cudaError_t e = cudaFuncSetAttribute(kernel_, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(smem_bytes_));
-  if (e != cudaSuccess) return static_cast<int>(e);
-  if (kernel_prof_ != nullptr) {
-    e = cudaFuncSetAttribute(kernel_prof_, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes_));
-    if (e != cudaSuccess) return static_cast<int>(e);
-  }
-  e = cudaFuncSetAttribute(kernel_lp_, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes_));
-  if (e != cudaSuccess) return static_cast<int>(e);
+  // process-wide and only ever raised: another decoder's engine launches the same instantiations at its own size
+  for (const void* k : {kernel_, kernel_prof_, kernel_lp_})
+    if (k != nullptr)
+      if (int rc = smem_opt_in(k, smem_bytes_)) return rc;
   int occ_lp = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_lp, kernel_lp_, kThreads, smem_bytes_);
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_lp, kernel_lp_, kThreads, smem_bytes_);
   if (e != cudaSuccess) return static_cast<int>(e);
   if (occ_lp < 1) return KLLM_E_UNSUPPORTED;
   int occ = 0;

@@ -256,14 +256,10 @@ int prefill_block(const PrefillModel& m, PrefillWorkspace& ws, const int32_t* to
 }
 
 int prefill_attention_smem_opt_in(size_t bytes) {
-  static size_t configured = 0;
-  if (bytes <= 48 * 1024 || bytes <= configured) return 0;
+  if (bytes <= 48 * 1024) return 0;
   for (const void* k : {reinterpret_cast<const void*>(attn_rows_kernel<float>),
-                        reinterpret_cast<const void*>(attn_rows_kernel<__nv_bfloat16>)}) {
-    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
-    if (e != cudaSuccess) return static_cast<int>(e);
-  }
-  configured = bytes;
+                        reinterpret_cast<const void*>(attn_rows_kernel<__nv_bfloat16>)})
+    if (int rc = smem_opt_in(k, bytes)) return rc;
   return 0;
 }
 
