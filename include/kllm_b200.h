@@ -57,6 +57,11 @@ int kllm_gemv_f32(const float* x, const float* w, float* out, int in_dim, int ou
 int kllm_gemv_w8(const float* x, const int8_t* w, const float* scales, float* out, int in_dim,
                  int out_dim, int group_size, void* stream);
 
+/* kllm_gemv_f32 over bf16 weights (the decoder's KLLM_WEIGHTS_BF16): w[out_dim, in_dim] holds bf16 bit patterns,
+ * each widened exactly to fp32 before the same fp32 arithmetic, so out is bit-identical to kllm_gemv_f32 over the
+ * widened matrix.  Any in_dim; rows need not be aligned. */
+int kllm_gemv_bf16(const float* x, const uint16_t* w, float* out, int in_dim, int out_dim, void* stream);
+
 /* RMSNormKernel -> rmsnorm_kernel_cu, cuda/rmsnorm_kernel.cu:52-78 (eps is the flavour
  * constant there; here it is an argument). In-place (out == x) is allowed. */
 int kllm_rmsnorm_f32(const float* x, const float* w, float* out, int n, float eps, void* stream);
@@ -201,6 +206,12 @@ int kllm_gemm_tf32(const float* x, const float* w, float* out, int n_tokens, int
  * x, w are 16-byte aligned. */
 int kllm_gemm_w8_tf32(const float* x, const int8_t* w, const float* scales, float* out, int n_tokens, int in_dim,
                       int out_dim, int group_size, void* stream);
+/* The same GEMM for bf16 weights (the decoder's KLLM_WEIGHTS_BF16): w[out_dim, in_dim] holds bf16 bit patterns.  The
+ * weight tile is loaded as bf16 and widened into the fp32 tile; a bf16 value is exact in tf32, so out is bit-identical
+ * to kllm_gemm_tf32 over the widened matrix.  KLLM_E_INVALID for NULL pointers or non-positive sizes;
+ * KLLM_E_UNSUPPORTED unless in_dim % 8 == 0 and x, w are 16-byte aligned. */
+int kllm_gemm_bf16_tf32(const float* x, const uint16_t* w, float* out, int n_tokens, int in_dim, int out_dim,
+                        void* stream);
 
 /* ---- tensor-parallel exchange --------------------------------------------------------------
  * Not in the reference (single GPU: llama3.cpp:118 pins device 0); SURVEY.md section 8e.  One
@@ -287,11 +298,26 @@ typedef struct {
    * engine (KLLM_ENGINE=graph, or a shape only it takes), tp_size > 1, or head_size % 32 != 0.
    * kllm_decoder_profile returns KLLM_E_UNSUPPORTED on a bf16 decoder. */
   int32_t kv_cache;
+  /* Storage of the weight matrices (DESIGN.md 5.11).  KLLM_WEIGHTS_F32 (0, the default of a zeroed struct): as
+   * group_size says.  KLLM_WEIGHTS_BF16 (1): wq wk wv wo w1 w2 w3 and wcls are device arrays of bf16 (uint16 bit
+   * patterns), each the caller's fp32 tensor rounded to nearest even (torch.Tensor.to(torch.bfloat16)); half the
+   * bytes every decode step streams.  tok_emb, the norms and the Qwen2 biases stay fp32; with a shared classifier
+   * wcls is a separate bf16 copy of the embedding (the row gather keeps reading the fp32 tok_emb).  All arithmetic
+   * stays fp32: a bf16 value widens exactly, so every entry's ids, logits and KV cache are bit for bit those of the
+   * same decoder with KLLM_WEIGHTS_F32 over the rounded weights widened back to fp32, in either numerics at the same
+   * ring geometry (KLLM_STAGE_BYTES / KLLM_ATTN_SPLIT: bf16 rows pick their own default stage), and with either
+   * kv_cache.  Shapes the persistent engine does not take (dim, hidden_dim or the query rows not multiples of 8) run
+   * on the graph engine.  kllm_decoder_create returns KLLM_E_INVALID for any other value or for bf16 with
+   * group_size > 0, and KLLM_E_UNSUPPORTED, creating nothing, for tp_size > 1.  kllm_decoder_prefill_w8 and
+   * kllm_decoder_profile return KLLM_E_UNSUPPORTED on a bf16-weight decoder. */
+  int32_t weights;
 } kllm_decoder_desc;
 #define KLLM_NUMERICS_EXACT 0
 #define KLLM_NUMERICS_FAST 1
 #define KLLM_KV_F32 0
 #define KLLM_KV_BF16 1
+#define KLLM_WEIGHTS_F32 0
+#define KLLM_WEIGHTS_BF16 1
 
 typedef struct kllm_decoder kllm_decoder;
 
@@ -322,7 +348,10 @@ int kllm_decoder_prompt(kllm_decoder* dec, const int32_t* tokens_host, int32_t n
  * tensor cores (TF32 multiply, fp32 accumulate, kllm_gemm_tf32), the weights streamed once per 256
  * positions instead of once per position; classifier only for the last position.  KV-cache rows and
  * logits agree with the position-by-position path to ~1e-3 relative, NOT bit for bit (TF32 keeps 10
- * mantissa bits).  fp32 checkpoints on one GPU; KLLM_E_UNSUPPORTED otherwise (use kllm_decoder_prompt).
+ * mantissa bits).  fp32 checkpoints on one GPU, their weights held in fp32 or, KLLM_WEIGHTS_BF16, in bf16
+ * (kllm_gemm_bf16_tf32: bit for bit the fp32-weight decoder's result over the widened weights; dim, hidden_dim and
+ * head_num * head_size must then be multiples of 8); KLLM_E_UNSUPPORTED otherwise (use kllm_decoder_prompt),
+ * checked before any launch, so a refused call leaves the cache, the history and the logits as they were.
  * A token id outside [0, vocab_size) is refused with KLLM_E_INVALID before any launch. */
 int kllm_decoder_prefill_tf32(kllm_decoder* dec, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
                               int32_t* next_host);

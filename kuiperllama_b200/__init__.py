@@ -62,7 +62,7 @@ class DecoderDesc(ctypes.Structure):
         ("bq", POINTER(c_void_p)), ("bk", POINTER(c_void_p)), ("bv", POINTER(c_void_p)),
         ("tp_size", c_int32), ("tp_rank", c_int32),
         ("allreduce", ALLREDUCE_FN), ("allreduce_ctx", c_void_p), ("comm", c_void_p),
-        ("numerics", c_int32), ("kv_cache", c_int32),
+        ("numerics", c_int32), ("kv_cache", c_int32), ("weights", c_int32),
     ]
 
 
@@ -74,6 +74,7 @@ _SIGNATURES = {
     "kllm_launch_count": (c_uint64, []),
     "kllm_gemv_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "kllm_gemv_w8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "kllm_gemv_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "kllm_rmsnorm_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p]),
     "kllm_add_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "kllm_swiglu_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
@@ -96,6 +97,7 @@ _SIGNATURES = {
     "kllm_gemv_fused": (c_int, [POINTER(GemvJob), c_void_p]),
     "kllm_gemm_tf32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "kllm_gemm_w8_tf32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "kllm_gemm_bf16_tf32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "kllm_comm_unique_id": (c_int, [c_void_p]),
     "kllm_comm_create": (c_int, [c_int, c_int, c_int, c_int, c_void_p, POINTER(c_void_p)]),
     "kllm_comm_ipc_handle": (c_int, [c_void_p, c_void_p]),

@@ -219,6 +219,8 @@ int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
   const PosArg pos{&dc->st->pos, 0};
   const bool tp = d.tp_size > 1;
   const uint64_t before = launch_counter().load();
+  GemvExtra wx;  // the jobs' weight form
+  wx.bf16 = d.weights == KLLM_WEIGHTS_BF16 ? 1 : 0;
 
   embed_token_kernel<<<4, 256, 0, s>>>(dc->st, d.tok_emb, dc->x, dim, d.vocab_size, dc->hist);
   count_launch();
@@ -241,7 +243,7 @@ int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
                   dc->kcache + layer_off, kvd};
       j.seg[2] = {dc->wv[l], d.group_size ? dc->sv[l] : nullptr, dc->bv.empty() ? nullptr : dc->bv[l],
                   dc->vcache + layer_off, kvd};
-      GemvExtra ex;
+      GemvExtra ex = wx;
       ex.pos = pos;
       ex.pos_stride[1] = kvd;
       ex.pos_stride[2] = kvd;
@@ -260,7 +262,7 @@ int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
       j.n_seg = 1;
       j.seg[0] = {dc->wo[l], d.group_size ? dc->so[l] : nullptr, nullptr, tp ? dc->tp_tmp : dc->x, dim};
       j.residual = tp ? nullptr : dc->x;  // feed_forward's first add (llama3.cpp:683-684)
-      KLLM_TRY(gemv_dispatch(&j, GemvExtra{}, s));
+      KLLM_TRY(gemv_dispatch(&j, wx, s));
       if (tp) KLLM_TRY(tp_reduce_into_x(dc, s));
     }
     // feed_forward (llama3.cpp:686-720)
@@ -275,7 +277,7 @@ int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
       j.seg[0] = {dc->w1[l], d.group_size ? dc->s1[l] : nullptr, nullptr, dc->h, hid};
       j.seg[1] = {dc->w3[l], d.group_size ? dc->s3[l] : nullptr, nullptr, nullptr, hid};
       j.swiglu_pair = 1;
-      KLLM_TRY(gemv_dispatch(&j, GemvExtra{}, s));
+      KLLM_TRY(gemv_dispatch(&j, wx, s));
     }
     {
       kllm_gemv_job j{};
@@ -285,7 +287,7 @@ int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
       j.n_seg = 1;
       j.seg[0] = {dc->w2[l], d.group_size ? dc->s2[l] : nullptr, nullptr, tp ? dc->tp_tmp : dc->x, dim};
       j.residual = tp ? nullptr : dc->x;
-      KLLM_TRY(gemv_dispatch(&j, GemvExtra{}, s));
+      KLLM_TRY(gemv_dispatch(&j, wx, s));
       if (tp) KLLM_TRY(tp_reduce_into_x(dc, s));
     }
   }
@@ -299,7 +301,7 @@ int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
     j.group_size = d.group_size;
     j.n_seg = 1;
     j.seg[0] = {d.wcls, d.group_size ? d.scls : nullptr, nullptr, dc->logits, d.vocab_size};
-    KLLM_TRY(gemv_dispatch(&j, GemvExtra{}, s));
+    KLLM_TRY(gemv_dispatch(&j, wx, s));
   }
   argmax_advance_kernel<<<1, 1024, 0, s>>>(dc->logits, d.vocab_size, dc->d_cfg, dc->st, dc->out_tokens, dc->teacher,
                                            d.seq_len, dc->stream_dev + kStreamIds, dc->stream_dev, dc->hist,
@@ -371,6 +373,7 @@ int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int3
   m.wq = dc->wq.data(), m.wk = dc->wk.data(), m.wv = dc->wv.data(), m.wo = dc->wo.data();
   m.w1 = dc->w1.data(), m.w2 = dc->w2.data(), m.w3 = dc->w3.data();
   m.group_size = d.group_size;
+  m.bf16 = d.weights == KLLM_WEIGHTS_BF16 ? 1 : 0;
   if (d.group_size > 0) {
     m.sq = dc->sq.data(), m.sk = dc->sk.data(), m.sv = dc->sv.data(), m.so = dc->so.data();
     m.s1 = dc->s1.data(), m.s2 = dc->s2.data(), m.s3 = dc->s3.data();
@@ -403,7 +406,9 @@ int prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int3
     j.group_size = d.group_size;
     j.n_seg = 1;
     j.seg[0] = {d.wcls, d.group_size ? d.scls : nullptr, nullptr, dc->logits, d.vocab_size};
-    KLLM_TRY(gemv_dispatch(&j, GemvExtra{}, dc->stream));
+    GemvExtra wx;
+    wx.bf16 = d.weights == KLLM_WEIGHTS_BF16 ? 1 : 0;
+    KLLM_TRY(gemv_dispatch(&j, wx, dc->stream));
   }
   argmax_advance_kernel<<<1, 1024, 0, dc->stream>>>(dc->logits, d.vocab_size, dc->d_cfg, dc->st, nullptr, nullptr,
                                                     d.seq_len, nullptr, nullptr, dc->hist, dc->penalized, dc->rec);
@@ -436,6 +441,11 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
   if (d.dim % (d.head_num * tp) != 0 || d.head_num % d.kv_head_num != 0) return KLLM_E_INVALID;
   if ((d.dim & 3) != 0 || (d.hidden_dim & 3) != 0) return KLLM_E_UNSUPPORTED;
   if (d.kv_cache != KLLM_KV_F32 && d.kv_cache != KLLM_KV_BF16) return KLLM_E_INVALID;
+  // bf16 weights: fp32 checkpoints' matrices rounded by the caller; one GPU
+  if (d.weights != KLLM_WEIGHTS_F32 && d.weights != KLLM_WEIGHTS_BF16) return KLLM_E_INVALID;
+  const bool w16 = d.weights == KLLM_WEIGHTS_BF16;
+  if (w16 && d.group_size > 0) return KLLM_E_INVALID;
+  if (w16 && tp > 1) return KLLM_E_UNSUPPORTED;
   // a bf16 cache exists on the persistent engine's flash form only; the rest of the refusals come from its init
   const bool kv_bf16 = d.kv_cache == KLLM_KV_BF16;
   const char* want = getenv("KLLM_ENGINE");
@@ -547,6 +557,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     mm.tp_world = tp, mm.tp_rank = tp_rank, mm.tp_stride = tp_stride;
     mm.numerics = d.numerics;
     mm.kv_cache = d.kv_cache;
+    mm.weights = d.weights;
     for (int r = 0; r < 8; ++r) mm.tp_data[r] = tp_areas[r];
     mm.dim = d.dim, mm.hidden_dim = d.hidden_dim, mm.layer_num = L, mm.head_num = d.head_num;
     mm.kv_head_num = d.kv_head_num, mm.vocab_size = d.vocab_size, mm.seq_len = d.seq_len;
@@ -646,7 +657,12 @@ int kllm_decoder_prompt(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_
 int kllm_decoder_prefill_tf32(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
                               int32_t* next_host) {
   KLLM_TRY(prefill_args(dc, tokens_host, n_tokens, start_pos, next_host));
-  if (dc->d.group_size != 0 || dc->d.tp_size > 1) return KLLM_E_UNSUPPORTED;  // fp32 checkpoints, one GPU
+  const kllm_decoder_desc& d = dc->d;
+  if (d.group_size != 0 || d.tp_size > 1) return KLLM_E_UNSUPPORTED;  // fp32 checkpoints, one GPU
+  // what kllm_gemm_bf16_tf32 takes (in_dim % 8 == 0), for every projection's in_dim; checked before any launch, so
+  // a refused call leaves the cache and the history as they were
+  const int q_rows = d.head_num * dc->head_size;
+  if (d.weights == KLLM_WEIGHTS_BF16 && ((d.dim & 7) || (d.hidden_dim & 7) || (q_rows & 7))) return KLLM_E_UNSUPPORTED;
   return prefill(dc, tokens_host, n_tokens, start_pos, next_host);
 }
 
@@ -851,7 +867,8 @@ int kllm_decoder_profile(kllm_decoder* dc, int32_t first_token, int32_t start_po
                          int32_t profiled_step, uint64_t* stamps_host, int32_t capacity,
                          int32_t* grid_out, int32_t* phases_out) {
   if (!dc || !stamps_host || !grid_out || !phases_out || n_steps <= 0) return KLLM_E_INVALID;
-  if (!dc->use_mega || dc->d.kv_cache == KLLM_KV_BF16) return KLLM_E_UNSUPPORTED;  // no bf16-cache timeline kernel
+  // no timeline kernel for the bf16 cache or bf16 weights
+  if (!dc->use_mega || dc->d.kv_cache == KLLM_KV_BF16 || dc->d.weights == KLLM_WEIGHTS_BF16) return KLLM_E_UNSUPPORTED;
   if (start_pos < 0 || start_pos + n_steps > dc->d.seq_len) return KLLM_E_INVALID;
   const int grid = dc->mega.grid(), phases = dc->mega.phases();
   const size_t n = static_cast<size_t>(grid) * phases * mega::kProfStamps;

@@ -9,7 +9,7 @@
 // and each lane carries the partial sums of four of those 128 "virtual threads", so the
 // floating-point result is bit-identical while a warp streams 2 KiB of contiguous weights per
 // step with 128-bit loads and several rows in flight.  HBM-bound: 4 B (fp32) or 1.0625 B
-// (int8 + scales) per multiply-add; tensor cores are deliberately not used (batch 1,
+// (int8 + scales) or 2 B (bf16) per multiply-add; tensor cores are deliberately not used (batch 1,
 // 0.5 flop/B, and tf32/bf16 would break the 1e-4 / identical-token contract).
 #include <cuda_runtime.h>
 
@@ -40,7 +40,7 @@ struct GemvParams {
   int in_dim;
   int group_size;
   int group_shift;  // log2(group_size) or -1
-  int vec_ok;       // fp32: every weight row is 16-byte aligned (in_dim % 4 == 0, aligned bases)
+  int vec_ok;       // fp32 / bf16: every weight row is 16- / 8-byte aligned (in_dim % 4 == 0, aligned bases)
   int n_seg;
   int units;  // output rows (or w1/w3 row pairs when swiglu)
   PosArg pos;
@@ -78,7 +78,8 @@ __device__ __forceinline__ float rms_scale_ref(const float* xs, int n, float eps
   return rsqrtf(__fadd_rn(__fdiv_rn(sum, static_cast<float>(n)), eps));
 }
 
-template <int R, bool kInt8, bool kSwiglu>
+// kBf16: bf16 weights widened exactly to fp32 on load; every operation is the fp32 path's.
+template <int R, bool kInt8, bool kSwiglu, bool kBf16 = false>
 __global__ void __launch_bounds__(kGemvThreads) gemv_kernel(const GemvParams p) {
   extern __shared__ __align__(16) float xs[];
   const int lane = threadIdx.x & 31;
@@ -141,15 +142,55 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_kernel(const GemvParams p) 
       const long long e = static_cast<long long>(row) * M;
       ebase[r] = e;
       srow[r] = p.seg[seg].scales;
-      wrow[r] = kInt8 ? static_cast<const void*>(static_cast<const int8_t*>(p.seg[seg].w) + e)
-                      : static_cast<const void*>(static_cast<const float*>(p.seg[seg].w) + e);
+      wrow[r] = kInt8    ? static_cast<const void*>(static_cast<const int8_t*>(p.seg[seg].w) + e)
+                : kBf16 ? static_cast<const void*>(static_cast<const unsigned short*>(p.seg[seg].w) + e)
+                        : static_cast<const void*>(static_cast<const float*>(p.seg[seg].w) + e);
     }
 
     float acc[R][4];
 #pragma unroll
     for (int r = 0; r < R; ++r) acc[r][0] = acc[r][1] = acc[r][2] = acc[r][3] = 0.f;
 
-    if constexpr (!kInt8) {
+    if constexpr (kBf16) {
+      // the fp32 path below with 8-byte packs of four bf16 weights (scalar loads for unaligned rows)
+      auto pack = [&](int r, int idx) {
+        if (p.vec_ok) return ldg_stream_bf16x4(static_cast<const uint2*>(wrow[r]) + idx);
+        const unsigned short* wp = static_cast<const unsigned short*>(wrow[r]) + 4 * idx;
+        return make_float4(widen_bf16(__ldg(wp)), widen_bf16(__ldg(wp + 1)), widen_bf16(__ldg(wp + 2)),
+                           widen_bf16(__ldg(wp + 3)));
+      };
+      const int full = p.vec_ok ? (pack_num & ~127) : 0;
+      for (int base = 0; base < full; base += 128) {
+        float4 wv[R][4];
+#pragma unroll
+        for (int r = 0; r < R; ++r)
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            wv[r][j] = ldg_stream_bf16x4(static_cast<const uint2*>(wrow[r]) + base + 32 * j + lane);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float4 xv = xs4[base + 32 * j + lane];
+#pragma unroll
+          for (int r = 0; r < R; ++r) acc[r][j] = __fadd_rn(dot4_ref(xv, wv[r][j]), acc[r][j]);
+        }
+      }
+      for (int base = full; base < pack_num; base += 128) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int idx = base + 32 * j + lane;
+          if (idx < pack_num) {
+            const float4 xv = xs4[idx];
+#pragma unroll
+            for (int r = 0; r < R; ++r) acc[r][j] = __fadd_rn(dot4_ref(xv, pack(r, idx)), acc[r][j]);
+          }
+        }
+      }
+      for (int i = (pack_num << 2) + lane; i < M; i += 128) {
+#pragma unroll
+        for (int r = 0; r < R; ++r)
+          acc[r][0] = __fmaf_rn(xs[i], widen_bf16(__ldg(static_cast<const unsigned short*>(wrow[r]) + i)), acc[r][0]);
+      }
+    } else if constexpr (!kInt8) {
       // virtual thread (lane + 32 j) <- packs base + 32 j + lane, base += 128
       const int full = p.vec_ok ? (pack_num & ~127) : 0;
       for (int base = 0; base < full; base += 128) {
@@ -267,11 +308,11 @@ static int sm_count() {
   return g_sm_count;
 }
 
-template <int R, bool kInt8, bool kSwiglu>
+template <int R, bool kInt8, bool kSwiglu, bool kBf16 = false>
 static int launch_gemv(const GemvParams& p, cudaStream_t stream) {
   constexpr int kUnits = R / (kSwiglu ? 2 : 1);
   const size_t smem = static_cast<size_t>(p.in_dim) * sizeof(float);
-  auto kern = gemv_kernel<R, kInt8, kSwiglu>;
+  auto kern = gemv_kernel<R, kInt8, kSwiglu, kBf16>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(smem));
@@ -292,6 +333,8 @@ int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t
   if (job == nullptr || job->x == nullptr || job->in_dim <= 0) return KLLM_E_INVALID;
   if (job->n_seg < 1 || job->n_seg > 3) return KLLM_E_INVALID;
   const bool int8 = job->group_size > 0;
+  const bool bf16 = extra.bf16 != 0;
+  if (bf16 && int8) return KLLM_E_INVALID;
   if (job->swiglu_pair && (job->n_seg != 2 || job->seg[0].rows != job->seg[1].rows ||
                            job->residual != nullptr))
     return KLLM_E_INVALID;
@@ -321,7 +364,7 @@ int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t
     if (g.w == nullptr || g.rows <= 0) return KLLM_E_INVALID;
     if (int8 && g.scales == nullptr) return KLLM_E_INVALID;
     if (g.out == nullptr && !(job->swiglu_pair && s == 1)) return KLLM_E_INVALID;
-    if ((reinterpret_cast<uintptr_t>(g.w) & (int8 ? 3 : 15)) != 0) {
+    if ((reinterpret_cast<uintptr_t>(g.w) & (int8 ? 3 : bf16 ? 7 : 15)) != 0) {
       if (int8) return KLLM_E_UNSUPPORTED;
       p.vec_ok = 0;
     }
@@ -333,6 +376,14 @@ int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t
   // Rows per warp: enough independent 128-bit loads in flight per lane (R*4) while still
   // giving every SM work for the small matrices (kv projections: 256 rows).
   const int warps_1wave = sm_count() * kGemvWarps;
+  if (bf16) {
+    if (job->swiglu_pair)
+      return p.units >= warps_1wave * 2 ? launch_gemv<4, false, true, true>(p, stream)
+                                        : launch_gemv<2, false, true, true>(p, stream);
+    if (p.units >= warps_1wave * 4) return launch_gemv<4, false, false, true>(p, stream);
+    if (p.units >= warps_1wave * 2) return launch_gemv<2, false, false, true>(p, stream);
+    return launch_gemv<1, false, false, true>(p, stream);
+  }
   if (job->swiglu_pair) {
     if (int8) return p.units >= warps_1wave * 2 ? launch_gemv<4, true, true>(p, stream)
                                                 : launch_gemv<2, true, true>(p, stream);
@@ -368,6 +419,20 @@ int kllm_gemv_f32(const float* x, const float* w, float* out, int in_dim, int ou
   job.seg[0].out = out;
   job.seg[0].rows = out_dim;
   return kllm_gemv_fused(&job, stream);
+}
+
+int kllm_gemv_bf16(const float* x, const uint16_t* w, float* out, int in_dim, int out_dim, void* stream) {
+  if (!x || !w || !out || in_dim <= 0 || out_dim <= 0) return KLLM_E_INVALID;
+  kllm_gemv_job job{};
+  job.x = x;
+  job.in_dim = in_dim;
+  job.n_seg = 1;
+  job.seg[0].w = w;
+  job.seg[0].out = out;
+  job.seg[0].rows = out_dim;
+  kllm::GemvExtra ex;
+  ex.bf16 = 1;
+  return kllm::gemv_dispatch(&job, ex, static_cast<cudaStream_t>(stream));
 }
 
 int kllm_gemv_w8(const float* x, const int8_t* w, const float* scales, float* out, int in_dim,

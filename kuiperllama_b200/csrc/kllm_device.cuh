@@ -28,6 +28,20 @@ __device__ __forceinline__ uint32_t ldg_stream_u32(const uint32_t* p) {
   return v;
 }
 
+// bf16 weights (KLLM_WEIGHTS_BF16): four consecutive elements held in two 32-bit words, element 2i in the low half,
+// widened exactly to fp32 (a bf16 value is the upper half of the float with the same value).
+__device__ __forceinline__ float4 widen_bf16x4(uint32_t lo, uint32_t hi) {
+  return make_float4(__uint_as_float(lo << 16), __uint_as_float(lo & 0xffff0000u), __uint_as_float(hi << 16),
+                     __uint_as_float(hi & 0xffff0000u));
+}
+__device__ __forceinline__ float widen_bf16(unsigned short v) { return __uint_as_float(static_cast<uint32_t>(v) << 16); }
+// 64-bit streaming load of four bf16 weights, widened
+__device__ __forceinline__ float4 ldg_stream_bf16x4(const uint2* p) {
+  uint32_t a, b;
+  asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(a), "=r"(b) : "l"(p));
+  return widen_bf16x4(a, b);
+}
+
 // matmul_kernel.cu:30-34 as compiled: part = fma(x.w,w.w, fma(x.z,w.z, fma(x.x,w.x, x.y*w.y))).
 __device__ __forceinline__ float dot4_ref(const float4& x, const float4& w) {
   float p = __fmul_rn(x.y, w.y);

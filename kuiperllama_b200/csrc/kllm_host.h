@@ -28,9 +28,11 @@ struct PosArg {
 };
 
 // Output rows of segment s land at seg[s].out + pos * pos_stride[s] (KV-cache rows).
+// bf16: the segments' weights are bf16 (kllm_gemv_bf16, the decoder's KLLM_WEIGHTS_BF16), group_size 0.
 struct GemvExtra {
   PosArg pos{nullptr, 0};
   long long pos_stride[3] = {0, 0, 0};
+  int bf16 = 0;
 };
 
 int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t stream);
@@ -57,6 +59,7 @@ struct PrefillModel {
   const void* const* wq; const void* const* wk; const void* const* wv; const void* const* wo;
   const void* const* w1; const void* const* w2; const void* const* w3;
   int group_size;  // 0: fp32 weights (kllm_gemm_tf32); > 0: int8 weights + scales (kllm_gemm_w8_tf32)
+  int bf16;        // 1 (group_size 0): bf16 weights (kllm_gemm_bf16_tf32)
   const float* const* sq; const float* const* sk; const float* const* sv; const float* const* so;
   const float* const* s1; const float* const* s2; const float* const* s3;
   const float* const* bq; const float* const* bk; const float* const* bv;

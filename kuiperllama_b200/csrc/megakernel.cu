@@ -398,6 +398,52 @@ __device__ __forceinline__ void accum_f32(const uint32_t (&w)[NR], uint32_t x, i
   }
 }
 
+// bf16 weights (w16_megakernel): accum_f32's mapping and order over rows of half the bytes.  A pack of four bf16
+// weights is one 8-byte load (a warp reads 256 consecutive bytes: no bank conflicts), widened exactly to fp32, so
+// every dot4 and addition is the fp32 kernel's over the widened weights.
+__device__ __forceinline__ float4 lds_bf16x4(uint32_t a) {
+  uint32_t lo, hi;
+  asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(lo), "=r"(hi) : "r"(a));
+  return widen_bf16x4(lo, hi);
+}
+template <int NR>
+__device__ __forceinline__ void accum_bf16(const uint32_t (&w)[NR], uint32_t x, int n_packs, int lane,
+                                           float (&acc)[NR][4]) {
+  const int full = n_packs & ~127;
+  uint32_t xp = x + lane * 16;
+  uint32_t wp[NR];
+#pragma unroll
+  for (int r = 0; r < NR; ++r) wp[r] = w[r] + lane * 8;
+#pragma unroll 2
+  for (int base = 0; base < full; base += 128) {
+    float4 xv[4];
+    float4 wv[NR][4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) xv[j] = lds_f4(xp + 512 * j);
+#pragma unroll
+    for (int r = 0; r < NR; ++r)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) wv[r][j] = lds_bf16x4(wp[r] + 256 * j);
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int r = 0; r < NR; ++r) acc[r][j] = __fadd_rn(dot4_ref(xv[j], wv[r][j]), acc[r][j]);
+    xp += 2048;
+#pragma unroll
+    for (int r = 0; r < NR; ++r) wp[r] += 1024;
+  }
+  if (full < n_packs) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (full + 32 * j + lane < n_packs) {
+        const float4 xv = lds_f4(xp + 512 * j);
+#pragma unroll
+        for (int r = 0; r < NR; ++r) acc[r][j] = __fadd_rn(dot4_ref(xv, lds_bf16x4(wp[r] + 256 * j)), acc[r][j]);
+      }
+    }
+  }
+}
+
 // int8, group size 64 (export.py --version 3): virtual thread (4 lane + e) owns elements
 // 128 k + 4 lane + e (matmul_kernel.cu:70-74), so the lane's four bytes of chunk k sit in group
 // 2 k + (lane >> 4) of the row: the scale address just steps by two floats.  Per element the
@@ -625,7 +671,7 @@ __device__ __noinline__ void quantize_input_inplace(float* xs, int M, int tid) {
 struct Rows4 {
   uint32_t a[4];
 };
-template <int NR, bool INT8>
+template <int NR, bool INT8, bool W16>
 __device__ __forceinline__ float4 dot_rows(Rows4 rows, Rows4 scales, uint32_t x, int M, int group_size,
                                            int group_shift, int lane, bool fast = false) {
   float acc[NR][4];
@@ -662,7 +708,10 @@ __device__ __forceinline__ float4 dot_rows(Rows4 rows, Rows4 scales, uint32_t x,
 #pragma unroll
     for (int r = 0; r < NR; ++r) d[r] = block128_sum_quad_packed(acc[r]);
   } else {
-    accum_f32<NR>(w, x, M >> 2, lane, acc);
+    if constexpr (W16)
+      accum_bf16<NR>(w, x, M >> 2, lane, acc);
+    else
+      accum_f32<NR>(w, x, M >> 2, lane, acc);
 #pragma unroll
     for (int r = 0; r < NR; ++r) d[r] = block128_sum_vt_packed(acc[r], lane);
   }
@@ -1587,11 +1636,11 @@ __device__ __forceinline__ void record_fed(const Params& P, int pos, int token) 
 // Stages the phase's input vector (tagged residual exchange / tagged hand-off / embedding row) into
 // shared memory, RMS-normalises it when the phase asks for it, consumes this CTA's ring stages
 // task by task, runs the epilogues and, for the classifier, leaves the CTA's (max, index).
-template <int CW, bool INT8, bool PROF, bool LP, bool KV16>
+template <int CW, bool INT8, bool PROF, bool LP, bool KV16, bool W16>
 __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int tok, int pos, const float* emb_row,
                                             unsigned long long* stamp) {
   constexpr int CT = CW * 32;
-  constexpr int wbytes = INT8 ? 1 : 4;
+  constexpr int wbytes = INT8 ? 1 : W16 ? 2 : 4;
   const Phase& ph = g_ph_cons;
   uint64_t* full_bar = g_full_bar;
   uint64_t* empty_bar = g_empty_bar;
@@ -1798,33 +1847,33 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
           if (nu == 2) {
             const Rows4 rp{{wa + i0 * rb, wa + (n + i0) * rb, wa + (i0 + 1) * rb, wa + (n + i0 + 1) * rb}};
             const Rows4 sp{{sa + i0 * srb, sa + (n + i0) * srb, sa + (i0 + 1) * srb, sa + (n + i0 + 1) * srb}};
-            const float4 d = dot_rows<4, INT8>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
+            const float4 d = dot_rows<4, INT8, W16>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
             e0 = lane == 0 ? d.x : d.z;
             e1 = lane == 0 ? d.y : d.w;
           } else {
             const Rows4 rp{{wa + i0 * rb, wa + (n + i0) * rb, 0u, 0u}};
             const Rows4 sp{{sa + i0 * srb, sa + (n + i0) * srb, 0u, 0u}};
-            const float4 d = dot_rows<2, INT8>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
+            const float4 d = dot_rows<2, INT8, W16>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
             e0 = d.x, e1 = d.y;
           }
         } else if (nu == 4) {
           const Rows4 rp{{wa + i0 * rb, wa + (i0 + 1) * rb, wa + (i0 + 2) * rb, wa + (i0 + 3) * rb}};
           const Rows4 sp{{sa + i0 * srb, sa + (i0 + 1) * srb, sa + (i0 + 2) * srb, sa + (i0 + 3) * srb}};
-          const float4 d = dot_rows<4, INT8>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
+          const float4 d = dot_rows<4, INT8, W16>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
           e0 = lane == 0 ? d.x : lane == 1 ? d.y : lane == 2 ? d.z : d.w;
         } else {
           int r0 = 0;
           if (nu >= 2) {
             const Rows4 rp{{wa + i0 * rb, wa + (i0 + 1) * rb, 0u, 0u}};
             const Rows4 sp{{sa + i0 * srb, sa + (i0 + 1) * srb, 0u, 0u}};
-            const float4 d = dot_rows<2, INT8>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
+            const float4 d = dot_rows<2, INT8, W16>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
             e0 = lane == 0 ? d.x : d.y;
             r0 = 2;
           }
           if (r0 < nu) {  // nu is 1 or 3: one more row
             const Rows4 rp{{wa + (i0 + r0) * rb, 0u, 0u, 0u}};
             const Rows4 sp{{sa + (i0 + r0) * srb, 0u, 0u, 0u}};
-            const float4 d = dot_rows<1, INT8>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
+            const float4 d = dot_rows<1, INT8, W16>(rp, sp, xa, M, ph.group_size, ph.group_shift, lane, int8_fast);
             if (lane == r0) e0 = d.x;
           }
         }
@@ -1840,7 +1889,7 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
       pipe.advance(S);
     }
   } else {
-    // rows longer than a stage (fp32 only): the owning warp carries its partial sums across
+    // rows longer than a stage (fp32 and bf16): the owning warp carries its partial sums across
     // consecutive stages; chunk boundaries are multiples of 128 packs so every virtual
     // thread still sees its packs in increasing order.
     for (int u = u0; u < u1; ++u) {
@@ -1854,7 +1903,10 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
         mbar_wait(&full_bar[pipe.slot], pipe.parity);
         if (mine) {
           const uint32_t w[1] = {smem_u32(stages + static_cast<size_t>(pipe.slot) * P.stage_bytes)};
-          accum_f32<1>(w, smem_u32(xs) + static_cast<uint32_t>(e0) * 4u, ne >> 2, lane, acc);
+          if constexpr (W16)
+            accum_bf16<1>(w, smem_u32(xs) + static_cast<uint32_t>(e0) * 4u, ne >> 2, lane, acc);
+          else
+            accum_f32<1>(w, smem_u32(xs) + static_cast<uint32_t>(e0) * 4u, ne >> 2, lane, acc);
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[pipe.slot]);
@@ -1957,7 +2009,8 @@ __device__ __noinline__ int draw_with_logprobs(const Params& P, int pos, int ste
 // LP: the logprob_megakernel instantiation, launched while log-probabilities are on.  decode_megakernel (LP false)
 // compiles to the code it has without the feature: the off path adds nothing to it, not even a test.
 // KV16: the bf16 KV cache (kv16_megakernel), fast numerics' flash form only; the same holds for it.
-template <int CW, bool INT8, bool PROF, bool LP, bool KV16>
+// W16: bf16 weight rows (w16_megakernel), never with INT8; the same holds for it.
+template <int CW, bool INT8, bool PROF, bool LP, bool KV16, bool W16 = false>
 __device__ __forceinline__ void megakernel_body(const Params& P) {
   constexpr int CT = CW * 32;  // consumer threads
   uint64_t* full_bar = g_full_bar;
@@ -1987,7 +2040,7 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
   __syncthreads();
 
   Pipe pipe{0, 0u};
-  constexpr int wbytes = INT8 ? 1 : 4;
+  constexpr int wbytes = INT8 ? 1 : W16 ? 2 : 4;
 
   // =============================== producer warp ===============================================
   if (is_producer) {
@@ -2228,7 +2281,7 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
         // A prompt token (llama3.cpp:733-745: predict(..., is_prompt = true) discards the logits and
         // returns -1) skips the classifier -- its weights are not even streamed -- but keeps the grid
         // barrier that closes the token.
-        const Carry out = gemv_phase<CW, INT8, PROF, LP, KV16>(P, Carry{pipe, best.v, best.i}, tok, pos, emb_row, stamp);
+        const Carry out = gemv_phase<CW, INT8, PROF, LP, KV16, W16>(P, Carry{pipe, best.v, best.i}, tok, pos, emb_row, stamp);
         pipe = out.pipe;
         best.v = out.best_v, best.i = out.best_i;
       }
@@ -2304,6 +2357,13 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) kv16_megakernel(const __grid_
   megakernel_body<CW, INT8, false, LP, true>(P);
 }
 
+// bf16 weights (KLLM_WEIGHTS_BF16): with (LP) and without log-probabilities, over an fp32 or (KV16) a bf16 cache; no
+// profiling one.
+template <int CW, bool LP, bool KV16>
+__global__ void __launch_bounds__(CW * 32 + 32, 1) w16_megakernel(const __grid_constant__ Params P) {
+  megakernel_body<CW, false, false, LP, KV16, true>(P);
+}
+
 }  // namespace mega
 
 // ================================== host side ======================================================
@@ -2322,11 +2382,25 @@ const void* kv16_kernel_for(bool int8) {
   if (int8) return reinterpret_cast<const void*>(mega::kv16_megakernel<mega::kConsumerWarps, true, LP>);
   return reinterpret_cast<const void*>(mega::kv16_megakernel<mega::kConsumerWarps, false, LP>);
 }
+template <bool LP>
+const void* w16_kernel_for(bool kv16) {
+  if (kv16) return reinterpret_cast<const void*>(mega::w16_megakernel<mega::kConsumerWarps, LP, true>);
+  return reinterpret_cast<const void*>(mega::w16_megakernel<mega::kConsumerWarps, LP, false>);
+}
 const void* logprob_kernel_for(bool int8) {
   if (int8) return reinterpret_cast<const void*>(mega::logprob_megakernel<mega::kConsumerWarps, true>);
   return reinterpret_cast<const void*>(mega::logprob_megakernel<mega::kConsumerWarps, false>);
 }
 constexpr int kThreads = mega::kConsumerWarps * 32 + 32;  // the consumer warps and the ring producer
+// Ring stage of bf16 weights, per numerics mode as fp32's.  H100 80GB HBM3, 700 W, tok/s at positions 1 / 512 / 2047
+// (tools/bench_weights.py, DESIGN.md 5.11), 16 / 24 / 32 KB:
+//   exact: TinyLlama-1.1B at 2047 607 / 710 / 745, Qwen2.5-0.5B at 2047 703 / 799 / 848 -- the exact attention's
+//          tiles shrink with the stage; Llama-2-7B within 2-6 % of each other.  32 KB.
+//   fast:  24 KB is at or above 32 KB at every measured point of the three models (TinyLlama-1.1B +1-2 %,
+//          Qwen2.5-0.5B +2-7 %, Llama-2-7B +1 %); 16 KB is best on Llama-2-7B (+4-5 % over 24 KB) but loses 2-6 % on
+//          TinyLlama-1.1B.  24 KB.
+constexpr int kW16StageBytes = 32 * 1024;
+constexpr int kW16FastStageBytes = 24 * 1024;
 }  // namespace
 
 int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
@@ -2343,7 +2417,11 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   const int dim = m.dim, hid = m.hidden_dim, hs = m.head_size, kvd = m.kv_dim;
   const int q_rows = m.head_num * hs;
   const bool int8 = m.group_size > 0;
-  const int wb = int8 ? 1 : 4;
+  // bf16 weights: 2-byte rows through the same ring (the decoder refuses them with int8)
+  if (m.weights != KLLM_WEIGHTS_F32 && m.weights != KLLM_WEIGHTS_BF16) return KLLM_E_INVALID;
+  const bool w16 = m.weights == KLLM_WEIGHTS_BF16;
+  if (w16 && int8) return KLLM_E_INVALID;
+  const int wb = int8 ? 1 : w16 ? 2 : 4;
   // One CTA per SM, but never more CTAs than the shortest row-parallel phase has rows: the
   // slot-reuse argument of the tagged hand-offs wants every CTA to own rows in every producing
   // phase (a CTA without rows gates nothing and could be overtaken).  Small test shapes only.
@@ -2353,6 +2431,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   // head_size <= 128: the K-tile producer issues one bulk copy per lane for hs/4 <= 32 chunk columns
   if ((dim & 3) || (hid & 3) || (q_rows & 3) || (hs & 3) || hs > 128) return KLLM_E_UNSUPPORTED;
   if (int8 && ((dim & 15) || (hid & 15) || (q_rows & 15) || (m.group_size & 3))) return KLLM_E_UNSUPPORTED;
+  if (w16 && ((dim & 7) || (hid & 7) || (q_rows & 7))) return KLLM_E_UNSUPPORTED;  // bf16 rows: 16-byte multiples
   if ((hs * 4) % 16 != 0) return KLLM_E_UNSUPPORTED;
   if (int8) {
     const int dims[3] = {dim, hid, q_rows};
@@ -2371,9 +2450,15 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   if (m.kv_cache != KLLM_KV_F32 && m.kv_cache != KLLM_KV_BF16) return KLLM_E_INVALID;
   kv_bf16_ = m.kv_cache == KLLM_KV_BF16 ? 1 : 0;
   if (kv_bf16_ && (!fast_ || m.tp_world > 1 || hs % 32 != 0)) return KLLM_E_UNSUPPORTED;
-  kernel_ = kv_bf16_ ? kv16_kernel_for<false>(int8) : kernel_for<false>(int8);
-  kernel_prof_ = kv_bf16_ ? nullptr : kernel_for<true>(int8);  // no profiling instantiation for the bf16 cache
-  kernel_lp_ = kv_bf16_ ? kv16_kernel_for<true>(int8) : logprob_kernel_for(int8);
+  if (w16) {  // no profiling instantiation for bf16 weights
+    kernel_ = w16_kernel_for<false>(kv_bf16_);
+    kernel_prof_ = nullptr;
+    kernel_lp_ = w16_kernel_for<true>(kv_bf16_);
+  } else {
+    kernel_ = kv_bf16_ ? kv16_kernel_for<false>(int8) : kernel_for<false>(int8);
+    kernel_prof_ = kv_bf16_ ? nullptr : kernel_for<true>(int8);  // no profiling instantiation for the bf16 cache
+    kernel_lp_ = kv_bf16_ ? kv16_kernel_for<true>(int8) : logprob_kernel_for(int8);
+  }
 
   // The residual exchange after o_proj and down_proj is tagged (under tensor parallelism it IS the
   // all-reduce), and so are the hand-offs q|k|v -> attention -> Wo and SwiGLU -> W2: the one grid
@@ -2397,8 +2482,9 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   // against 627 with 32 KB (20 KB: 649, 24 KB: 645), Qwen2.5-0.5B 1058 against 1032.  At dim 4096 a 16 KB stage is
   // ONE row, a task no longer shares its x loads, and Llama-2-7B fell from 108 to 80 tok/s.  The flash tiles shrink
   // with the stage (head_size 64: 64 timesteps).
-  const bool small_stages = fast_ && !kv_bf16_ && 2 * dim * 4 <= 16 * 1024;
-  int stage_bytes = int8 ? 27 * 1024 : small_stages ? 16 * 1024 : 32 * 1024;
+  const bool small_stages = fast_ && !kv_bf16_ && !w16 && 2 * dim * 4 <= 16 * 1024;
+  int stage_bytes = int8 ? 27 * 1024 : w16 ? (fast_ ? kW16FastStageBytes : kW16StageBytes) : small_stages ? 16 * 1024
+                                                                                                 : 32 * 1024;
   if (const char* e = getenv("KLLM_STAGE_BYTES")) stage_bytes = atoi(e);
   stage_bytes = (stage_bytes + 127) & ~127;
   const int kv_esz = kv_bf16_ ? 2 : 4;  // bytes per cached element
@@ -2480,7 +2566,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
       }
     } else {
       if (int8 || p.swiglu) return KLLM_E_UNSUPPORTED;
-      const int chunk_max = (stage_bytes / 4) & ~511;  // multiple of 128 packs
+      const int chunk_max = (stage_bytes / wb) & ~511;  // elements: a multiple of 128 packs
       p.chunks_per_row = (p.in_dim + chunk_max - 1) / chunk_max;
       int ce = (p.in_dim + p.chunks_per_row - 1) / p.chunks_per_row;
       ce = (ce + 511) & ~511;

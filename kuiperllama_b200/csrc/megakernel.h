@@ -198,6 +198,7 @@ struct MegaModel {
   int tp_stride;
   int numerics;  // kllm_decoder_desc::numerics
   int kv_cache;  // kllm_decoder_desc::kv_cache: KLLM_KV_BF16 needs the fast numerics (flash attention)
+  int weights;   // kllm_decoder_desc::weights: KLLM_WEIGHTS_BF16 = bf16 matrices (w16_megakernel), group_size 0
 };
 
 class MegaEngine {
@@ -250,7 +251,8 @@ class MegaEngine {
   int kv_bf16_ = 0;  // bf16 KV cache: the kernels are kv16_megakernel's
   int cls_rows_ = 0, n_cls_phases_ = 1;
   const void* kernel_ = nullptr;       // decode_megakernel<8 consumer warps, int8, false>
-  const void* kernel_prof_ = nullptr;  // ... <.., true>: records the phase timeline stamps (none with kv_bf16_)
+  const void* kernel_prof_ = nullptr;  // ... <.., true>: records the phase timeline stamps (none with kv_bf16_ or
+                                       // bf16 weights)
   const void* kernel_lp_ = nullptr;    // logprob_megakernel<8 consumer warps, int8>: log-probabilities on
   size_t smem_bytes_ = 0;
   unsigned barrier_base_ = 0;

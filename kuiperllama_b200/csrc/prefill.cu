@@ -198,6 +198,7 @@ int prefill_block(const PrefillModel& m, PrefillWorkspace& ws, const int32_t* to
   auto gemm = [&](const float* x, const void* w, const float* scales, float* out, int K, int N) {
     if (m.group_size > 0)
       return kllm_gemm_w8_tf32(x, static_cast<const int8_t*>(w), scales, out, T, K, N, m.group_size, s);
+    if (m.bf16) return kllm_gemm_bf16_tf32(x, static_cast<const uint16_t*>(w), out, T, K, N, s);
     return kllm_gemm_tf32(x, static_cast<const float*>(w), out, T, K, N, s);
   };
   auto scales = [&](const float* const* per_layer, int l) { return m.group_size > 0 ? per_layer[l] : nullptr; };

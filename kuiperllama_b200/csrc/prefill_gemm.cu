@@ -27,6 +27,10 @@
 // K block (group_size % 32 == 0, in_dim % group_size == 0) and is read with an ordinary non-coherent load
 // one K block ahead: scale rows can be 4 bytes, which TMA cannot copy.  A stage is dequantised while the
 // wgmma group of the stage before it is still running.
+//
+// bf16 weights (template parameter W16, kllm_gemm_bf16_tf32): the same staging with a [128 x 32 bf16] tile of
+// 64-byte rows, widened into the fp32 A tile.  A bf16 value widens exactly and is already a tf32 value, so the A
+// tile holds what kllm_gemm_tf32 holds after its rounding of the widened weights: the results are bit-identical.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -44,6 +48,12 @@ constexpr int WG_K = 8;     // tf32: 32 bytes of K per wgmma
 constexpr int STAGES = 4;
 constexpr int A_BYTES = BM * BK * 4;  // 16 KB
 constexpr int W8_BYTES = BM * BK;     // 4 KB: the int8 weight tile as loaded, rows of 32 bytes
+constexpr int W16_BYTES = BM * BK * 2;  // 8 KB: the bf16 weight tile as loaded, rows of 64 bytes
+// bytes of the weight staging area per stage
+template <bool W8, bool W16>
+__host__ __device__ constexpr int staging_bytes() {
+  return W8 ? W8_BYTES : W16 ? W16_BYTES : 0;
+}
 constexpr int THREADS = 384;
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) {
@@ -197,7 +207,25 @@ __device__ __forceinline__ void dequant_w8(const uint8_t* src, uint8_t* a_rows, 
   }
 }
 
-template <int BN, bool W8>
+// Thread (r, half) of a consumer warpgroup widens the 16 bf16 weights of columns 16 half .. + 15 of its local row r
+// into the swizzled A tile, as dequant_w8 does.
+__device__ __forceinline__ void widen_w16(const uint8_t* src, uint8_t* a_rows, int r, int half) {
+  const int4 q0 = *reinterpret_cast<const int4*>(src);
+  const int4 q1 = *reinterpret_cast<const int4*>(src + 16);
+  const uint32_t words[8] = {static_cast<uint32_t>(q0.x), static_cast<uint32_t>(q0.y), static_cast<uint32_t>(q0.z),
+                             static_cast<uint32_t>(q0.w), static_cast<uint32_t>(q1.x), static_cast<uint32_t>(q1.y),
+                             static_cast<uint32_t>(q1.z), static_cast<uint32_t>(q1.w)};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const uint32_t lo = words[2 * j], hi = words[2 * j + 1];
+    const int c = 4 * half + j;
+    *reinterpret_cast<float4*>(a_rows + r * 128 + ((c ^ (r & 7)) << 4)) =
+        make_float4(__uint_as_float(lo << 16), __uint_as_float(lo & 0xffff0000u), __uint_as_float(hi << 16),
+                    __uint_as_float(hi & 0xffff0000u));
+  }
+}
+
+template <int BN, bool W8, bool W16 = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x,
                  float* __restrict__ out, const float* __restrict__ scales, int T, int N, int K, int group_size) {
@@ -206,8 +234,9 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* a_tiles = base;
   uint8_t* b_tiles = base + STAGES * A_BYTES;
-  uint8_t* w8_tiles = b_tiles + STAGES * B_BYTES;  // W8 only
-  uint64_t* bars = reinterpret_cast<uint64_t*>(w8_tiles + (W8 ? STAGES * W8_BYTES : 0));
+  uint8_t* w8_tiles = b_tiles + STAGES * B_BYTES;  // W8 / W16 only: the weight staging area
+  constexpr int WS_BYTES = staging_bytes<W8, W16>();
+  uint64_t* bars = reinterpret_cast<uint64_t*>(w8_tiles + STAGES * WS_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
 
@@ -233,8 +262,8 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
         mbar_wait(smem_addr(&empty[s]), ph ^ 1u);
         const uint32_t bar = smem_addr(&full[s]);
         // out-of-range rows / columns are zero-filled and still counted
-        mbar_expect_tx(bar, (W8 ? W8_BYTES : A_BYTES) + B_BYTES);
-        tma_load_2d(smem_addr(W8 ? w8_tiles + s * W8_BYTES : a_tiles + s * A_BYTES), &map_w, bar, kb * BK, n0);
+        mbar_expect_tx(bar, (WS_BYTES ? WS_BYTES : A_BYTES) + B_BYTES);
+        tma_load_2d(smem_addr(WS_BYTES ? w8_tiles + s * WS_BYTES : a_tiles + s * A_BYTES), &map_w, bar, kb * BK, n0);
         tma_load_2d(smem_addr(b_tiles + s * B_BYTES), &map_x, bar, kb * BK, t0);
       }
     }
@@ -262,6 +291,9 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
     if constexpr (W8)
       dequant_w8(w8_tiles + s * W8_BYTES + ((wg - 1) * 64 + dq_row) * BK + dq_half * 16, a_tiles + s * A_BYTES + a_off,
                  dq_row, dq_half, sc);
+    else if constexpr (W16)
+      widen_w16(w8_tiles + s * W16_BYTES + ((wg - 1) * 64 + dq_row) * BK * 2 + dq_half * 32,
+                a_tiles + s * A_BYTES + a_off, dq_row, dq_half);
     else
       round_tf32(reinterpret_cast<float4*>(a_tiles + s * A_BYTES + a_off), 64 * BK / 4, t);
     round_tf32(reinterpret_cast<float4*>(b_tiles + s * B_BYTES + (wg - 1) * (B_BYTES / 2)), BN * BK / 8, t);
@@ -309,50 +341,53 @@ static EncodeTiledFn encode_tiled() {
   }();
   return fn;
 }
-// 2-D tensor [rows, cols] (row-major, cols contiguous) of fp32 (128-byte swizzle) or int8 (no swizzle: the
-// consumers read it back row by row), box [box_rows x 32 columns]
-static int make_map(CUtensorMap* map, const void* ptr, bool int8, int rows, int cols, int box_rows) {
+// 2-D tensor [rows, cols] (row-major, cols contiguous) of fp32 (elem 4, 128-byte swizzle), or of int8 or bf16
+// (elem 1 or 2, no swizzle: the consumers read it back row by row), box [box_rows x 32 columns]
+static int make_map(CUtensorMap* map, const void* ptr, int elem, int rows, int cols, int box_rows) {
   EncodeTiledFn fn = encode_tiled();
   if (fn == nullptr) return KLLM_E_NODEVICE;
   const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * (int8 ? 1 : 4)};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * elem};
   const cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>(box_rows)};
   const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(map, int8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+  const CUtensorMapDataType type = elem == 1   ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                   : elem == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT16
+                                               : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const CUresult r = fn(map, type, 2,
                         const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        int8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
+                        elem != 4 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : KLLM_E_INVALID;
 }
 
-template <int BN, bool W8>
+template <int BN, bool W8, bool W16 = false>
 static int launch(const float* x, const void* w, const float* scales, float* out, int T, int K, int N, int group_size,
                   cudaStream_t stream) {
   CUtensorMap map_w, map_x;
-  if (int rc = make_map(&map_w, w, W8, N, K, BM)) return rc;
-  if (int rc = make_map(&map_x, x, false, T, K, BN)) return rc;
-  const size_t smem = 1024 + static_cast<size_t>(STAGES) * (A_BYTES + BN * BK * 4 + (W8 ? W8_BYTES : 0)) + 128;
+  if (int rc = make_map(&map_w, w, W8 ? 1 : W16 ? 2 : 4, N, K, BM)) return rc;
+  if (int rc = make_map(&map_x, x, 4, T, K, BN)) return rc;
+  const size_t smem = 1024 + static_cast<size_t>(STAGES) * (A_BYTES + BN * BK * 4 + staging_bytes<W8, W16>()) + 128;
   static bool configured = false;
   if (!configured) {
-    const cudaError_t e = cudaFuncSetAttribute(gemm_tf32_kernel<BN, W8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               static_cast<int>(smem));
+    const cudaError_t e = cudaFuncSetAttribute(gemm_tf32_kernel<BN, W8, W16>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
   const dim3 grid((N + BM - 1) / BM, (T + BN - 1) / BN);
-  gemm_tf32_kernel<BN, W8><<<grid, THREADS, smem, stream>>>(map_w, map_x, out, scales, T, N, K, group_size);
+  gemm_tf32_kernel<BN, W8, W16><<<grid, THREADS, smem, stream>>>(map_w, map_x, out, scales, T, N, K, group_size);
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }
 
 // token-block width: the smallest wgmma N that covers the tokens, 256 at most
-template <bool W8>
+template <bool W8, bool W16 = false>
 static int dispatch(const float* x, const void* w, const float* scales, float* out, int T, int K, int N, int group_size,
                     cudaStream_t s) {
-  if (T <= 32) return launch<32, W8>(x, w, scales, out, T, K, N, group_size, s);
-  if (T <= 64) return launch<64, W8>(x, w, scales, out, T, K, N, group_size, s);
-  if (T <= 128) return launch<128, W8>(x, w, scales, out, T, K, N, group_size, s);
-  return launch<256, W8>(x, w, scales, out, T, K, N, group_size, s);
+  if (T <= 32) return launch<32, W8, W16>(x, w, scales, out, T, K, N, group_size, s);
+  if (T <= 64) return launch<64, W8, W16>(x, w, scales, out, T, K, N, group_size, s);
+  if (T <= 128) return launch<128, W8, W16>(x, w, scales, out, T, K, N, group_size, s);
+  return launch<256, W8, W16>(x, w, scales, out, T, K, N, group_size, s);
 }
 
 }  // namespace tc
@@ -377,4 +412,14 @@ extern "C" int kllm_gemm_w8_tf32(const float* x, const int8_t* w, const float* s
     return KLLM_E_UNSUPPORTED;
   return kllm::tc::dispatch<true>(x, w, scales, out, n_tokens, in_dim, out_dim, group_size,
                                   static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int kllm_gemm_bf16_tf32(const float* x, const uint16_t* w, float* out, int n_tokens, int in_dim, int out_dim,
+                                   void* stream) {
+  if (!x || !w || !out || n_tokens <= 0 || in_dim <= 0 || out_dim <= 0) return KLLM_E_INVALID;
+  // TMA needs 16-byte aligned bases and row pitches (2 in_dim bytes for the bf16 rows)
+  if ((in_dim & 7) || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(w) & 15))
+    return KLLM_E_UNSUPPORTED;
+  return kllm::tc::dispatch<false, true>(x, w, nullptr, out, n_tokens, in_dim, out_dim, 0,
+                                         static_cast<cudaStream_t>(stream));
 }

@@ -40,12 +40,18 @@ class ModelShape:
     def kv_mul(self) -> int:
         return self.head_num // self.kv_head_num
 
-    def weight_bytes_per_token(self) -> int:
+    def weight_bytes_per_token(self, weights: str = "fp32") -> int:
         """ALGORITHMIC bytes one decode step must read (SURVEY.md section 8d): every matmul
-        weight once (+ int8 scales), the 2L+1 norm vectors, qkv biases and one embedding row."""
+        weight once (+ int8 scales), the 2L+1 norm vectors, qkv biases and one embedding row.
+        weights="bf16": the matrices of an fp32 checkpoint held in bf16 (Decoder(weight_format="bf16")), 2 bytes each."""
         d, h, L, kv, V = self.dim, self.hidden_dim, self.layer_num, self.kv_dim, self.vocab_size
         numel = L * (2 * d * d + 2 * kv * d + 3 * h * d) + V * d
-        wbytes = numel * 4 if self.group_size == 0 else numel + (numel // self.group_size) * 4
+        if weights not in ("fp32", "bf16") or (weights == "bf16" and self.group_size):
+            raise ValueError(f"weights={weights!r} for {self.name}")
+        if self.group_size:
+            wbytes = numel + (numel // self.group_size) * 4
+        else:
+            wbytes = numel * (2 if weights == "bf16" else 4)
         extra = (2 * L + 1) * d * 4 + d * 4
         if self.flavour == "qwen2" and self.group_size == 0:
             extra += L * (d + 2 * kv) * 4
@@ -134,6 +140,34 @@ def synth_weights(shape: ModelShape, device="cuda", seed: int = 1234, norm_jitte
     return w
 
 
+MATRICES = ("wq", "wk", "wv", "wo", "w1", "w2", "w3")
+
+
+def bf16_weights(weights: dict) -> dict:
+    """The weight dict Decoder(weight_format="bf16") takes, from an fp32 one (synth_weights or a checkpoint's): the matrices
+    and the classifier rounded to bf16, round to nearest even (torch's conversion); with a shared classifier
+    ("wcls" None) a separate bf16 copy of the embedding.  tok_emb, the norms and the Qwen2 biases stay fp32."""
+    import torch
+    if "sq" in weights:
+        raise KllmError("bf16 weights are for fp32 checkpoints, not int8 ones")
+    out = dict(weights)
+    for n in MATRICES:
+        out[n] = weights[n].to(torch.bfloat16).contiguous()
+    wcls = weights.get("wcls")
+    out["wcls"] = (wcls if wcls is not None else weights["tok_emb"]).to(torch.bfloat16).contiguous()
+    return out
+
+
+def widen_weights(weights16: dict) -> dict:
+    """bf16_weights' result widened back to fp32 (exact): the fp32 decoder over these weights is what a bf16-weight
+    decoder reproduces bit for bit.  The classifier is always given explicitly (never None)."""
+    import torch
+    out = dict(weights16)
+    for n in MATRICES + ("wcls",):
+        out[n] = weights16[n].to(torch.float32).contiguous()
+    return out
+
+
 def _ptr_array(tensors):
     arr = (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
     return arr
@@ -144,7 +178,7 @@ class Decoder:
 
     def __init__(self, shape: ModelShape, weights: dict, stream=None, tp_size=1, tp_rank=0,
                  allreduce=None, allreduce_ctx=None, full_dim=None, comm=None, numerics="exact",
-                 kv_cache="fp32"):
+                 kv_cache="fp32", weight_format="fp32"):
         self.lib = load_library()
         self.shape = shape
         self.weights = weights  # keep the tensors alive
@@ -183,6 +217,15 @@ class Decoder:
         # "fp32": the cache of every other mode; "bf16": rows rounded to bf16 as they are cached, fast numerics on
         # the persistent engine only (kllm_b200.h, kllm_decoder_desc::kv_cache)
         d.kv_cache = {"fp32": 0, "bf16": 1}[kv_cache]
+        # "bf16": the matrices and wcls are bf16 tensors (bf16_weights), the arithmetic fp32 (kllm_decoder_desc::weights)
+        d.weights = {"fp32": 0, "bf16": 1}[weight_format]
+        want = "torch.bfloat16" if weight_format == "bf16" else None
+        for n in MATRICES + ("wcls",):
+            t = weights.get(n)
+            if t is not None and (str(t.dtype) == "torch.bfloat16") != (want is not None):
+                raise KllmError(f"weight_format={weight_format!r} with {n} of {t.dtype} (decoder.bf16_weights)")
+        if weight_format == "bf16" and weights.get("wcls") is None:
+            raise KllmError("weight_format='bf16' needs its own bf16 wcls (decoder.bf16_weights)")
         if allreduce is not None:
             d.allreduce = allreduce
             d.allreduce_ctx = allreduce_ctx

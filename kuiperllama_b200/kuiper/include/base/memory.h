@@ -11,6 +11,7 @@
 //                         pointer the caller keeps alive (use_external) -- checkpoint views
 #ifndef KLLM_KUIPER_BASE_MEMORY_H_
 #define KLLM_KUIPER_BASE_MEMORY_H_
+#include <cstring>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -47,6 +48,15 @@ class DeviceAllocator {
 // Here large copies go through two pinned buffers: while the copy engine drains one, the host fills
 // the other from the mapping (page-cache reads overlap the DMA).  One instance per process; copies of
 // less than kMinBytes, and everything after a failed pinned allocation, take the plain path.
+// fp32 -> bf16 bits, round to nearest even (torch.Tensor.to(torch.bfloat16)): finite values past the largest bf16
+// become inf, NaN stays a quiet NaN of the same sign.
+inline uint16_t fp32_to_bf16_rne(float f) {
+  uint32_t u;
+  std::memcpy(&u, &f, 4);
+  if ((u & 0x7fffffffu) > 0x7f800000u) return static_cast<uint16_t>((u >> 16) | 0x40u);
+  return static_cast<uint16_t>((u + 0x7fffu + ((u >> 16) & 1u)) >> 16);
+}
+
 class PinnedUploader {
  public:
   static constexpr size_t kChunkBytes = size_t(32) << 20;
@@ -55,6 +65,9 @@ class PinnedUploader {
   ~PinnedUploader();
   // enqueue host -> device on `stream`; returns false if the pinned path is unavailable
   bool upload(void* dst_device, const void* src_host, size_t bytes, void* stream);
+  // the same for n fp32 values that land on the device as bf16 (fp32_to_bf16_rne), rounded chunk by chunk while
+  // they are staged: only the 2-byte values cross the bus
+  bool upload_bf16(void* dst_device, const float* src_host, size_t n, void* stream);
   size_t bytes_uploaded() const { return uploaded_; }
 
  private:

@@ -43,8 +43,9 @@ struct LLama2Layers {
   LayerList w1_layers_, w2_layers_, w3_layers_;              // SwiGLU FFN: gate, down, up
   LayerPtr rope_layer_, mha_layer_, add_layer_, swiglu_layer_;  // weight-free, shared by all layers
 
-  // bind the stream and upload every weight
-  void to_cuda(std::shared_ptr<kernel::CudaConfig> config);
+  // bind the stream and upload every weight; matrices = false leaves the projection and classifier matrices on the
+  // host (bf16 weights: LLama2Model uploads its own bf16 copies of them)
+  void to_cuda(std::shared_ptr<kernel::CudaConfig> config, bool matrices = true);
 };
 
 class LLama2Model : public Model {
@@ -93,6 +94,16 @@ class LLama2Model : public Model {
   // the rows it takes over from the decoder are the widened bf16 values.
   void set_bf16_kv_cache(bool on);
   bool bf16_kv_cache() const { return bf16_kv_cache_; }
+
+  // bf16 weights in the fused decoder (kllm_decoder_desc::weights = KLLM_WEIGHTS_BF16): call before init(); without
+  // a call init() takes it from KUIPER_WEIGHTS=bf16|fp32 (fp32 by default).  The matrices wq wk wv wo w1 w2 w3 and the
+  // classifier (a bf16 copy of the embedding when shared) are rounded to bf16, nearest even, while they are staged
+  // for the upload: only the bf16 copies reach the device, half the upload and half their device memory.  Every
+  // result equals the fp32 model's over the rounded weights.  fp32 checkpoints on one GPU only: init() fails for an
+  // int8 checkpoint or under tensor parallelism; forward() (the layer path, which has no bf16 kernels) returns an
+  // error in this mode.
+  void set_bf16_weights(bool on);
+  bool bf16_weights() const { return bf16_weights_; }
 
   // Seeded sampling instead of the greedy id (DESIGN.md "Sampling"): call before init(); without a call
   // init() takes it from KUIPER_TEMPERATURE, KUIPER_TOP_K and KUIPER_SEED, so the reference's unchanged
@@ -194,6 +205,11 @@ class LLama2Model : public Model {
   bool batched_prefill_explicit_ = false;
   bool bf16_kv_cache_ = false;
   bool bf16_kv_cache_explicit_ = false;
+  bool bf16_weights_ = false;
+  bool bf16_weights_explicit_ = false;
+  // bf16 weights: the device copies of the matrices, in create_decoder's order (wq.. per layer, then wcls)
+  std::vector<std::shared_ptr<base::Buffer>> bf16_matrices_;
+  base::Status upload_bf16_matrices();
   sampler::DrawConfig draw_;
   sampler::DrawGroups draw_set_;              // the groups a setter gave: init() keeps them over the environment
   sampler::SeededSampler* seeded_ = nullptr;  // sampler_ when sampling, else null

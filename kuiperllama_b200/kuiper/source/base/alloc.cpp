@@ -93,6 +93,28 @@ bool PinnedUploader::upload(void* dst_device, const void* src_host, size_t bytes
   uploaded_ += bytes;
   return true;
 }
+bool PinnedUploader::upload_bf16(void* dst_device, const float* src_host, size_t n, void* stream) {
+  std::lock_guard<std::mutex> lock(mu_);
+  if (!ensure()) return false;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  char* dst = static_cast<char*>(dst_device);
+  const size_t per_chunk = kChunkBytes / sizeof(uint16_t);
+  for (size_t off = 0; off < n; off += per_chunk) {
+    const size_t k = std::min(per_chunk, n - off);
+    const int b = next_;
+    next_ ^= 1;
+    if (busy_[b]) cudaEventSynchronize(static_cast<cudaEvent_t>(done_[b]));
+    uint16_t* staged = static_cast<uint16_t*>(pinned_[b]);
+    for (size_t i = 0; i < k; ++i) staged[i] = fp32_to_bf16_rne(src_host[off + i]);
+    if (cudaMemcpyAsync(dst + off * sizeof(uint16_t), staged, k * sizeof(uint16_t), cudaMemcpyHostToDevice, s) !=
+        cudaSuccess)
+      return false;
+    cudaEventRecord(static_cast<cudaEvent_t>(done_[b]), s);
+    busy_[b] = true;
+  }
+  uploaded_ += n * sizeof(uint16_t);
+  return true;
+}
 PinnedUploader::~PinnedUploader() {
   for (int i = 0; i < 2; ++i) {
     if (done_[i]) cudaEventDestroy(static_cast<cudaEvent_t>(done_[i]));

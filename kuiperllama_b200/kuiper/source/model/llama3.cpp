@@ -33,18 +33,29 @@ std::shared_ptr<op::LayerParam> as_param(const std::shared_ptr<op::Layer>& l) {
 }
 }  // namespace
 
-void LLama2Layers::to_cuda(std::shared_ptr<kernel::CudaConfig> config) {
+void LLama2Layers::to_cuda(std::shared_ptr<kernel::CudaConfig> config, bool matrices) {
   auto move = [&](const std::shared_ptr<op::Layer>& l) {
     if (l) {
       l->set_cuda_config(config);
       l->to_cuda();
     }
   };
+  auto bind = [&](const std::shared_ptr<op::Layer>& l) {
+    if (!l) return;
+    l->set_cuda_config(config);
+    auto m = std::dynamic_pointer_cast<op::MatmulLayer>(l);
+    if (m && m->has_bias()) m->get_bias(0).to_cuda(config->stream);
+  };
   move(add_layer_), move(rope_layer_), move(swiglu_layer_), move(mha_layer_);
-  move(cls_layer_), move(embedding_layer_);
-  for (auto* group : {&wq_layers_, &wk_layers_, &wv_layers_, &wo_layers_, &w1_layers_, &w2_layers_, &w3_layers_,
-                      &rmsnorm_layers_})
-    for (auto& l : *group) move(l);
+  move(embedding_layer_);
+  for (auto& l : rmsnorm_layers_) move(l);
+  if (matrices) {
+    move(cls_layer_);
+  } else {  // bf16 weights: the biases (Qwen2) still go up with their layer, but the matrices stay on the host
+    bind(cls_layer_);
+  }
+  for (auto* group : {&wq_layers_, &wk_layers_, &wv_layers_, &wo_layers_, &w1_layers_, &w2_layers_, &w3_layers_})
+    for (auto& l : *group) matrices ? move(l) : bind(l);
 }
 
 LLama2Model::LLama2Model(base::TokenizerType tokenizer_type, std::string token_path, std::string model_path,
@@ -80,6 +91,11 @@ void LLama2Model::set_batched_prefill(bool on) {
 void LLama2Model::set_bf16_kv_cache(bool on) {
   bf16_kv_cache_ = on;
   bf16_kv_cache_explicit_ = true;
+}
+
+void LLama2Model::set_bf16_weights(bool on) {
+  bf16_weights_ = on;
+  bf16_weights_explicit_ = true;
 }
 
 void LLama2Model::set_sampling(float temperature, int32_t top_k, uint64_t seed) {
@@ -155,6 +171,18 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
     const char* env = std::getenv("KUIPER_KV_CACHE");
     bf16_kv_cache_ = env != nullptr && std::string(env) == "bf16";
   }
+  if (!bf16_weights_explicit_) {
+    const char* env = std::getenv("KUIPER_WEIGHTS");
+    if (env != nullptr && std::string(env) != "bf16" && std::string(env) != "fp32")
+      return error::InvalidArgument("KUIPER_WEIGHTS must be bf16 or fp32, not '" + std::string(env) + "'");
+    bf16_weights_ = env != nullptr && std::string(env) == "bf16";
+  }
+  if (bf16_weights_ && is_quant_model_)
+    return error::InvalidArgument(
+        "bf16 weights (KUIPER_WEIGHTS / set_bf16_weights) are for fp32 checkpoints: an int8 checkpoint runs as it is");
+  if (bf16_weights_ && tp_.on())
+    return error::InvalidArgument(
+        "bf16 weights (KUIPER_WEIGHTS / set_bf16_weights) run on one GPU: turn them off under tensor parallelism");
   sampler::fill_from_env(draw_, draw_set_);
   if (Status st = sampler::validate(draw_); !st) return st;
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
@@ -398,7 +426,9 @@ base::Status LLama2Model::create_layers() {
 void LLama2Model::init_mem() {
   CHECK(device_type_ == base::DeviceType::kDeviceCUDA);
   CHECK_NE(cuda_config_, nullptr);
-  llama_layers_->to_cuda(cuda_config_);  // weights: mmap (or the packed column shards) -> device
+  // weights: mmap (or the packed column shards) -> device; with bf16 weights the matrices go up as bf16 copies
+  llama_layers_->to_cuda(cuda_config_, !bf16_weights_);
+  if (bf16_weights_) CHECK(upload_bf16_matrices()) << "bf16 weights: the upload failed";
   cudaStreamSynchronize(cuda_config_->stream);
   tp_staging_.clear();
   // the host mapping is no longer needed for the weights that now live on the device
@@ -415,6 +445,28 @@ void LLama2Model::init_mem() {
   CHECK(insert_buffer(ModelBufferType::kCosCache, tensor::Tensor(f32, table, true, gpu)));
   // Everything else (activations of the layer-by-layer path, its KV cache, the logits mirror) is
   // created on first use by ensure_lazy_buffer(): the fused decoder keeps its own.
+}
+
+// Each matrix (viewing the mapped checkpoint on the host) rounded to bf16 while it is staged into the pinned
+// uploader: the fp32 matrix never reaches the device.
+base::Status LLama2Model::upload_bf16_matrices() {
+  auto gpu = base::CUDADeviceAllocatorFactory::get_instance();
+  auto up = [&](const std::shared_ptr<op::Layer>& l) {
+    const tensor::Tensor& w = as_param(l)->get_weight(0);
+    const size_t n = w.size();
+    auto dev = std::make_shared<base::Buffer>(n * sizeof(uint16_t), gpu);
+    if (dev->ptr() == nullptr) return false;
+    if (!base::PinnedUploader::instance().upload_bf16(dev->ptr(), w.ptr<float>(), n, cuda_config_->stream)) return false;
+    bf16_matrices_.push_back(std::move(dev));
+    return true;
+  };
+  for (auto* group : {&llama_layers_->wq_layers_, &llama_layers_->wk_layers_, &llama_layers_->wv_layers_,
+                      &llama_layers_->wo_layers_, &llama_layers_->w1_layers_, &llama_layers_->w2_layers_,
+                      &llama_layers_->w3_layers_})
+    for (auto& l : *group)
+      if (!up(l)) return base::error::InternalError("bf16 weights: a matrix upload failed");
+  if (!up(llama_layers_->cls_layer_)) return base::error::InternalError("bf16 weights: the classifier upload failed");
+  return base::error::Success();
 }
 
 void LLama2Model::ensure_lazy_buffer(ModelBufferType idx) const {
@@ -499,10 +551,17 @@ base::Status LLama2Model::create_decoder() {
     attn_norm.push_back(as_param(llama_layers_->rmsnorm_layers_[l])->get_weight(0).ptr<float>());
     ffn_norm.push_back(as_param(llama_layers_->rmsnorm_layers_[l + L])->get_weight(0).ptr<float>());
   }
-  const auto wq = weight_ptrs(llama_layers_->wq_layers_), wk = weight_ptrs(llama_layers_->wk_layers_),
-             wv = weight_ptrs(llama_layers_->wv_layers_), wo = weight_ptrs(llama_layers_->wo_layers_),
-             w1 = weight_ptrs(llama_layers_->w1_layers_), w2 = weight_ptrs(llama_layers_->w2_layers_),
-             w3 = weight_ptrs(llama_layers_->w3_layers_);
+  auto wq = weight_ptrs(llama_layers_->wq_layers_), wk = weight_ptrs(llama_layers_->wk_layers_),
+       wv = weight_ptrs(llama_layers_->wv_layers_), wo = weight_ptrs(llama_layers_->wo_layers_),
+       w1 = weight_ptrs(llama_layers_->w1_layers_), w2 = weight_ptrs(llama_layers_->w2_layers_),
+       w3 = weight_ptrs(llama_layers_->w3_layers_);
+  const void* wcls = as_param(llama_layers_->cls_layer_)->get_weight(0).ptr<int8_t>();
+  if (bf16_weights_) {  // the device copies, in upload_bf16_matrices' order
+    size_t k = 0;
+    for (auto* v : {&wq, &wk, &wv, &wo, &w1, &w2, &w3})
+      for (auto& p : *v) p = bf16_matrices_.at(k++)->ptr();
+    wcls = bf16_matrices_.at(k)->ptr();
+  }
   std::vector<const float*> sq, sk, sv, so, s1, s2, s3, bq, bk, bv;
 
   kllm_decoder_desc d{};
@@ -515,7 +574,7 @@ base::Status LLama2Model::create_decoder() {
   d.final_norm = as_param(llama_layers_->rmsnorm_layers_[2 * L])->get_weight(0).ptr<float>();
   d.wq = wq.data(), d.wk = wk.data(), d.wv = wv.data(), d.wo = wo.data();
   d.w1 = w1.data(), d.w2 = w2.data(), d.w3 = w3.data();
-  d.wcls = as_param(llama_layers_->cls_layer_)->get_weight(0).ptr<int8_t>();
+  d.wcls = wcls;
   if (is_quant_model_) {
     sq = scale_ptrs(llama_layers_->wq_layers_), sk = scale_ptrs(llama_layers_->wk_layers_);
     sv = scale_ptrs(llama_layers_->wv_layers_), so = scale_ptrs(llama_layers_->wo_layers_);
@@ -540,12 +599,14 @@ base::Status LLama2Model::create_decoder() {
   }
   if (const char* mode = std::getenv("KUIPER_NUMERICS"); mode && std::string(mode) == "fast") d.numerics = KLLM_NUMERICS_FAST;
   if (bf16_kv_cache_) d.kv_cache = KLLM_KV_BF16;
+  if (bf16_weights_) d.weights = KLLM_WEIGHTS_BF16;
   const int rc = kllm_decoder_create(&d, cuda_config_->stream, &decoder_);
   if (rc != 0)
     return base::error::InternalError(
         std::string("kllm_decoder_create failed: ") + kllm_error_string(rc) +
         (bf16_kv_cache_ ? " (the bf16 KV cache needs KUIPER_NUMERICS=fast, one GPU and head_size % 32 == 0)" : ""));
   if (bf16_kv_cache_) LOG(INFO) << "KV cache: bf16 (rounded to nearest even as rows are cached)";
+  if (bf16_weights_) LOG(INFO) << "weights: bf16 matrices (rounded to nearest even as they were uploaded)";
   if (base::Status st = sampler::apply_to_decoder(draw_, decoder_); !st) return st;
   LOG(INFO) << "fused decoder engine: " << kllm_decoder_engine(decoder_) << ", "
             << kllm_decoder_launches_per_step(decoder_) << " launch(es) per token";
@@ -772,6 +833,9 @@ base::Status LLama2Model::forward(const tensor::Tensor& input, const tensor::Ten
   if (tp_.on())
     return base::error::FunctionNotImplement("forward() is the single-GPU layer-by-layer path; a tensor-parallel "
                                              "model steps through predict()");
+  if (bf16_weights_)
+    return base::error::FunctionNotImplement("forward() is the fp32 layer-by-layer path, which has no bf16 kernels: "
+                                             "a model with bf16 weights steps through predict()");
   const int32_t pos = pos_tensor.index<int32_t>(0);
   if (base::Status st = sync_layer_cache(pos); !st) return st;
   for (int32_t l = 0; l < config_->layer_num_; ++l) {

@@ -5,6 +5,7 @@
 //                 [--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P]
 //                 [--repetition-penalty P N] [--frequency-presence F P [FROM]] [--logit-bias ID:B,...]
 //                 [--generate N [--stop ID]... [--then K]] [--logprobs N] [--score] [--kv-cache fp32|bf16]
+//                 [--weights fp32|bf16]
 //
 // --generate N runs the prompt and LLama2Model::generate() for at most N ids instead (n_steps is then unused),
 // stopping at the tokenizer's stop ids and every --stop ID, and prints the ids generate() returned, followed
@@ -27,7 +28,9 @@
 // --score scores the given ids with LLama2Model::score() instead of decoding (n_steps is then unused): one line of
 // the n - 1 log-probabilities, then "perplexity <exp(-mean)>".  The layer path has neither: --layers with either is
 // refused.  --kv-cache bf16 calls LLama2Model::set_bf16_kv_cache(true) instead of leaving it to KUIPER_KV_CACHE (the
-// fused decoder's bf16 KV cache needs KUIPER_NUMERICS=fast); --kv-cache fp32 turns it off.
+// fused decoder's bf16 KV cache needs KUIPER_NUMERICS=fast); --kv-cache fp32 turns it off.  --weights bf16 / fp32 calls
+// LLama2Model::set_bf16_weights instead of leaving it to KUIPER_WEIGHTS.  After init() the tool reports on stderr the
+// device memory init() took ("device bytes after init: N", from cudaMemGetInfo).
 #include <base/base.h>
 #include <cuda_runtime_api.h>
 #include <glog/logging.h>
@@ -51,7 +54,7 @@ int main(int argc, char** argv) {
     std::fprintf(stderr, "usage: %s <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...] "
                          "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P] "
                          "[--repetition-penalty P N] [--frequency-presence F P [FROM]] [--logit-bias ID:B,...] "
-                         "[--generate N [--stop ID]... [--then K]] [--kv-cache fp32|bf16]\n", argv[0]);
+                         "[--generate N [--stop ID]... [--then K]] [--kv-cache fp32|bf16] [--weights fp32|bf16]\n", argv[0]);
     return 2;
   }
   const std::string checkpoint = argv[1], family = argv[2], prec = argv[3];
@@ -116,6 +119,11 @@ int main(int argc, char** argv) {
       if (v != "fp32" && v != "bf16") return 2;
       m->set_bf16_kv_cache(v == "bf16");
     }
+    else if (!std::strcmp(argv[i], "--weights") && i + 1 < argc) {
+      const std::string v = argv[++i];
+      if (v != "fp32" && v != "bf16") return 2;
+      m->set_bf16_weights(v == "bf16");
+    }
     else if (!std::strcmp(argv[i], "--logits") && i + 1 < argc) logits_path = argv[++i];
     else prompt.push_back(std::atoi(argv[i]));
   }
@@ -126,7 +134,11 @@ int main(int argc, char** argv) {
     return 2;
   }
   if (!stops.empty()) m->set_stop_ids(stops);
+  size_t free_before = 0, free_after = 0, total = 0;
+  const bool meminfo = cudaMemGetInfo(&free_before, &total) == cudaSuccess;
   base::Status st = m->init(base::DeviceType::kDeviceCUDA);
+  if (st && meminfo && cudaMemGetInfo(&free_after, &total) == cudaSuccess)
+    std::fprintf(stderr, "device bytes after init: %zu\n", free_before - free_after);
   if (!st) {
     std::fprintf(stderr, "init failed: %s\n", st.get_err_msg().c_str());
     return 1;

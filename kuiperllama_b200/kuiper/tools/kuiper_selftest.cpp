@@ -6,6 +6,7 @@
 //   kuiper_selftest [checkpoint.bin [llama|qwen fp32|int8]]      exit code 0 = all passed
 #include <base/base.h>
 #include <base/buffer.h>
+#include <base/memory.h>
 #include <glog/logging.h>
 #include <op/add.h>
 #include <op/matmul.h>
@@ -62,8 +63,24 @@ void run(const char* name, const std::function<void()>& fn) {
 }
 }  // namespace
 
+// kuiper_selftest --bf16-round in.f32 out.u16: the host's fp32 -> bf16 rounding (base::fp32_to_bf16_rne, what the
+// bf16-weight upload applies) over a raw fp32 file, written as raw bf16 bits.
+static int bf16_round(const char* in_path, const char* out_path) {
+  FILE* in = std::fopen(in_path, "rb");
+  FILE* out = std::fopen(out_path, "wb");
+  if (in == nullptr || out == nullptr) return 2;
+  float f;
+  while (std::fread(&f, sizeof(f), 1, in) == 1) {
+    const uint16_t b = base::fp32_to_bf16_rne(f);
+    if (std::fwrite(&b, sizeof(b), 1, out) != 1) return 2;
+  }
+  std::fclose(in);
+  return std::fclose(out) == 0 ? 0 : 2;
+}
+
 int main(int argc, char** argv) {
   using namespace base;
+  if (argc == 4 && !std::strcmp(argv[1], "--bf16-round")) return bf16_round(argv[2], argv[3]);
   auto cpu = CPUDeviceAllocatorFactory::get_instance();
 
   run("buffer.allocate", [&] {  // test_buffer.cpp:7-12

@@ -204,15 +204,18 @@ class Comm:
 
 
 def make_tp_decoder(shape: ModelShape, full_weights: dict, comm: Comm, stream=None, numerics="exact",
-                    kv_cache="fp32") -> Decoder:
+                    kv_cache="fp32", weight_format="fp32") -> Decoder:
     """Decoder for this rank's shard of `full_weights` (every rank passes the same full dict,
     e.g. synth_weights with the same seed; the shard is cut here and the rest can be freed).
-    A bf16 KV cache runs on one GPU only (kllm_decoder_desc::kv_cache)."""
+    A bf16 KV cache and bf16 weights run on one GPU only (kllm_decoder_desc::kv_cache, ::weights)."""
     tp, rank = comm.world, comm.rank
     if tp == 1:
-        return Decoder(shape, full_weights, stream=stream, numerics=numerics, kv_cache=kv_cache)
+        return Decoder(shape, full_weights, stream=stream, numerics=numerics, kv_cache=kv_cache,
+                       weight_format=weight_format)
     if kv_cache != "fp32":
         raise ValueError(f"kv_cache={kv_cache!r} is not supported under tensor parallelism (tp_size {tp})")
+    if weight_format != "fp32":
+        raise ValueError(f"weight_format={weight_format!r} is not supported under tensor parallelism (tp_size {tp})")
     shard = shard_weights(shape, full_weights, tp, rank)
     return Decoder(local_shape(shape, tp, rank), shard, stream=stream, tp_size=tp, tp_rank=rank,
                    comm=comm, full_dim=shape.dim, numerics=numerics)
