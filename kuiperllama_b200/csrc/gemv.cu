@@ -332,9 +332,8 @@ static int launch_gemv(const GemvParams& p, cudaStream_t stream) {
 int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t stream) {
   if (job == nullptr || job->x == nullptr || job->in_dim <= 0) return KLLM_E_INVALID;
   if (job->n_seg < 1 || job->n_seg > 3) return KLLM_E_INVALID;
-  const bool int8 = job->group_size > 0;
-  const bool bf16 = extra.bf16 != 0;
-  if (bf16 && int8) return KLLM_E_INVALID;
+  const bool int8 = extra.format == WeightFormat::kInt8;
+  const bool bf16 = extra.format == WeightFormat::kBf16;
   if (job->swiglu_pair && (job->n_seg != 2 || job->seg[0].rows != job->seg[1].rows ||
                            job->residual != nullptr))
     return KLLM_E_INVALID;
@@ -349,12 +348,7 @@ int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t
   p.residual = job->residual;
   p.in_dim = job->in_dim;
   p.group_size = job->group_size;
-  p.group_shift = -1;
-  if (int8 && (job->group_size & (job->group_size - 1)) == 0) {
-    int s = 0;
-    while ((1 << s) < job->group_size) ++s;
-    p.group_shift = s;
-  }
+  p.group_shift = int8 ? group_shift_of(job->group_size) : -1;
   p.n_seg = job->n_seg;
   p.pos = extra.pos;
   p.vec_ok = (job->in_dim & 3) == 0;
@@ -405,7 +399,9 @@ int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t
 extern "C" {
 
 int kllm_gemv_fused(const kllm_gemv_job* job, void* stream) {
-  return kllm::gemv_dispatch(job, kllm::GemvExtra{}, static_cast<cudaStream_t>(stream));
+  kllm::GemvExtra ex;
+  if (job != nullptr && job->group_size > 0) ex.format = kllm::WeightFormat::kInt8;
+  return kllm::gemv_dispatch(job, ex, static_cast<cudaStream_t>(stream));
 }
 
 int kllm_gemv_f32(const float* x, const float* w, float* out, int in_dim, int out_dim,
@@ -431,7 +427,7 @@ int kllm_gemv_bf16(const float* x, const uint16_t* w, float* out, int in_dim, in
   job.seg[0].out = out;
   job.seg[0].rows = out_dim;
   kllm::GemvExtra ex;
-  ex.bf16 = 1;
+  ex.format = kllm::WeightFormat::kBf16;
   return kllm::gemv_dispatch(&job, ex, static_cast<cudaStream_t>(stream));
 }
 

@@ -2371,25 +2371,29 @@ using mega::Params;
 using mega::Phase;
 
 namespace {
-// PROF: the instantiation kllm_decoder_profile launches (its stamps cost registers in the row loops)
-template <bool PROF>
-const void* kernel_for(bool int8) {
-  if (int8) return reinterpret_cast<const void*>(mega::decode_megakernel<mega::kConsumerWarps, true, PROF>);
-  return reinterpret_cast<const void*>(mega::decode_megakernel<mega::kConsumerWarps, false, PROF>);
+template <typename K>
+const void* fn(K* kernel) {
+  return reinterpret_cast<const void*>(kernel);
 }
-template <bool LP>
-const void* kv16_kernel_for(bool int8) {
-  if (int8) return reinterpret_cast<const void*>(mega::kv16_megakernel<mega::kConsumerWarps, true, LP>);
-  return reinterpret_cast<const void*>(mega::kv16_megakernel<mega::kConsumerWarps, false, LP>);
-}
-template <bool LP>
-const void* w16_kernel_for(bool kv16) {
-  if (kv16) return reinterpret_cast<const void*>(mega::w16_megakernel<mega::kConsumerWarps, LP, true>);
-  return reinterpret_cast<const void*>(mega::w16_megakernel<mega::kConsumerWarps, LP, false>);
-}
-const void* logprob_kernel_for(bool int8) {
-  if (int8) return reinterpret_cast<const void*>(mega::logprob_megakernel<mega::kConsumerWarps, true>);
-  return reinterpret_cast<const void*>(mega::logprob_megakernel<mega::kConsumerWarps, false>);
+// The instantiations that run a model of weight format `f` over an fp32 or (kv16) a bf16 cache: the plain one, the
+// profiling one kllm_decoder_profile launches (its stamps cost registers in the row loops; none for a bf16 cache
+// or bf16 weights) and the log-probability one.
+struct Kernels {
+  const void *plain, *prof, *lp;
+};
+Kernels kernels_for(WeightFormat f, bool kv16) {
+  using namespace mega;
+  constexpr int CW = kConsumerWarps;
+  if (f == WeightFormat::kBf16)
+    return kv16 ? Kernels{fn(w16_megakernel<CW, false, true>), nullptr, fn(w16_megakernel<CW, true, true>)}
+                : Kernels{fn(w16_megakernel<CW, false, false>), nullptr, fn(w16_megakernel<CW, true, false>)};
+  if (f == WeightFormat::kInt8)
+    return kv16 ? Kernels{fn(kv16_megakernel<CW, true, false>), nullptr, fn(kv16_megakernel<CW, true, true>)}
+                : Kernels{fn(decode_megakernel<CW, true, false>), fn(decode_megakernel<CW, true, true>),
+                          fn(logprob_megakernel<CW, true>)};
+  return kv16 ? Kernels{fn(kv16_megakernel<CW, false, false>), nullptr, fn(kv16_megakernel<CW, false, true>)}
+              : Kernels{fn(decode_megakernel<CW, false, false>), fn(decode_megakernel<CW, false, true>),
+                        fn(logprob_megakernel<CW, false>)};
 }
 constexpr int kThreads = mega::kConsumerWarps * 32 + 32;  // the consumer warps and the ring producer
 // Ring stage of bf16 weights, per numerics mode as fp32's.  H100 80GB HBM3, 700 W, tok/s at positions 1 / 512 / 2047
@@ -2403,7 +2407,8 @@ constexpr int kW16StageBytes = 32 * 1024;
 constexpr int kW16FastStageBytes = 24 * 1024;
 }  // namespace
 
-int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
+int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t stream) {
+  dm_ = &dm;
   model_ = m;
   stream_ = stream;
   int dev = 0;
@@ -2414,29 +2419,25 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   if (!coop) return KLLM_E_UNSUPPORTED;
 
-  const int dim = m.dim, hid = m.hidden_dim, hs = m.head_size, kvd = m.kv_dim;
-  const int q_rows = m.head_num * hs;
-  const bool int8 = m.group_size > 0;
-  // bf16 weights: 2-byte rows through the same ring (the decoder refuses them with int8)
-  if (m.weights != KLLM_WEIGHTS_F32 && m.weights != KLLM_WEIGHTS_BF16) return KLLM_E_INVALID;
-  const bool w16 = m.weights == KLLM_WEIGHTS_BF16;
-  if (w16 && int8) return KLLM_E_INVALID;
-  const int wb = int8 ? 1 : w16 ? 2 : 4;
+  const int dim = dm.dim, hid = dm.hidden_dim, hs = dm.head_size, kvd = dm.kv_dim, q_rows = dm.q_rows;
+  const bool int8 = dm.format == WeightFormat::kInt8;
+  const bool w16 = dm.format == WeightFormat::kBf16;  // 2-byte rows through the same ring
+  const int wb = weight_bytes(dm.format);
   // One CTA per SM, but never more CTAs than the shortest row-parallel phase has rows: the
   // slot-reuse argument of the tagged hand-offs wants every CTA to own rows in every producing
   // phase (a CTA without rows gates nothing and could be overtaken).  Small test shapes only.
   grid_ = std::min(sms, std::min(dim, hid));
-  if (grid_ < m.head_num) return KLLM_E_UNSUPPORTED;  // attention: one CTA per (local) query head
+  if (grid_ < dm.head_num) return KLLM_E_UNSUPPORTED;  // attention: one CTA per (local) query head
   // shapes the ring handles: 16-byte rows, 128-byte aligned kv rows (L1-cached reads stay exact);
   // head_size <= 128: the K-tile producer issues one bulk copy per lane for hs/4 <= 32 chunk columns
   if ((dim & 3) || (hid & 3) || (q_rows & 3) || (hs & 3) || hs > 128) return KLLM_E_UNSUPPORTED;
-  if (int8 && ((dim & 15) || (hid & 15) || (q_rows & 15) || (m.group_size & 3))) return KLLM_E_UNSUPPORTED;
+  if (int8 && ((dim & 15) || (hid & 15) || (q_rows & 15) || (dm.group_size & 3))) return KLLM_E_UNSUPPORTED;
   if (w16 && ((dim & 7) || (hid & 7) || (q_rows & 7))) return KLLM_E_UNSUPPORTED;  // bf16 rows: 16-byte multiples
   if ((hs * 4) % 16 != 0) return KLLM_E_UNSUPPORTED;
   if (int8) {
     const int dims[3] = {dim, hid, q_rows};
     for (int d : dims)
-      if (d % m.group_size != 0 || ((d / m.group_size) * 4) % 16 != 0) return KLLM_E_UNSUPPORTED;
+      if (d % dm.group_size != 0 || ((d / dm.group_size) * 4) % 16 != 0) return KLLM_E_UNSUPPORTED;
   }
   // int8 arithmetic: "exact" reproduces the reference's fma(x * scale, float(w), acc) per element bit for
   // bit; "fast" is the dp4a fixed-point mode (toleranced, ~3.5x fewer instructions)
@@ -2450,15 +2451,8 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   if (m.kv_cache != KLLM_KV_F32 && m.kv_cache != KLLM_KV_BF16) return KLLM_E_INVALID;
   kv_bf16_ = m.kv_cache == KLLM_KV_BF16 ? 1 : 0;
   if (kv_bf16_ && (!fast_ || m.tp_world > 1 || hs % 32 != 0)) return KLLM_E_UNSUPPORTED;
-  if (w16) {  // no profiling instantiation for bf16 weights
-    kernel_ = w16_kernel_for<false>(kv_bf16_);
-    kernel_prof_ = nullptr;
-    kernel_lp_ = w16_kernel_for<true>(kv_bf16_);
-  } else {
-    kernel_ = kv_bf16_ ? kv16_kernel_for<false>(int8) : kernel_for<false>(int8);
-    kernel_prof_ = kv_bf16_ ? nullptr : kernel_for<true>(int8);  // no profiling instantiation for the bf16 cache
-    kernel_lp_ = kv_bf16_ ? kv16_kernel_for<true>(int8) : logprob_kernel_for(int8);
-  }
+  const Kernels ks = kernels_for(dm.format, kv_bf16_);
+  kernel_ = ks.plain, kernel_prof_ = ks.prof, kernel_lp_ = ks.lp;
 
   // The residual exchange after o_proj and down_proj is tagged (under tensor parallelism it IS the
   // all-reduce), and so are the hand-offs q|k|v -> attention -> Wo and SwiGLU -> W2: the one grid
@@ -2508,9 +2502,9 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   stages_ = stages;
   // attention split: SP CTAs per query head (power of two, <= 8), each owning head_size / SP output dims
   // (a multiple of 4 floats so that V slice rows stay 16-byte units for the bulk copies)
-  if (m.seq_len & 3) return KLLM_E_UNSUPPORTED;
+  if (dm.seq_len & 3) return KLLM_E_UNSUPPORTED;
   attn_split_ = 1;
-  while (attn_split_ * 2 <= 8 && m.head_num * attn_split_ * 2 <= grid_ && (hs / (attn_split_ * 2)) % 4 == 0 &&
+  while (attn_split_ * 2 <= 8 && dm.head_num * attn_split_ * 2 <= grid_ && (hs / (attn_split_ * 2)) % 4 == 0 &&
          hs % (attn_split_ * 2) == 0)
     attn_split_ *= 2;
   const int attn_split_max = attn_split_;
@@ -2520,7 +2514,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   int split_cap = attn_split_max;
   if (fast_) {  // flash: split by timestep, any power of two whose partial triples fit the scores area
     attn_split_ = 1;
-    while (attn_split_ * 2 <= 8 && m.head_num * attn_split_ * 2 <= grid_ && attn_split_ * 2 * (hs + 2) <= m.seq_len)
+    while (attn_split_ * 2 <= 8 && dm.head_num * attn_split_ * 2 <= grid_ && attn_split_ * 2 * (hs + 2) <= dm.seq_len)
       attn_split_ *= 2;
     split_cap = attn_split_;
   }
@@ -2539,14 +2533,9 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   std::vector<Phase> ph;
   auto plan = [&](Phase& p) -> int {
     const int row_bytes = p.in_dim * wb;
-    p.group_size = m.group_size;
-    p.group_shift = -1;
-    if (int8 && (m.group_size & (m.group_size - 1)) == 0) {
-      int s = 0;
-      while ((1 << s) < m.group_size) ++s;
-      p.group_shift = s;
-    }
-    p.scale_row_bytes = int8 ? (p.in_dim / m.group_size) * 4 : 0;
+    p.group_size = dm.group_size;
+    p.group_shift = dm.group_shift;
+    if (int8) p.scale_row_bytes = (p.in_dim / dm.group_size) * 4;
     const int rpu = p.swiglu ? 2 : 1;
     const int per_row = row_bytes + p.scale_row_bytes;
     if (per_row * rpu <= stage_bytes) {
@@ -2586,7 +2575,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
   unsigned long long *t_q = d_handoff_, *t_k = t_q + q_rows, *t_v = t_k + kvd, *t_attn = t_v + kvd,
                      *t_h = t_attn + q_rows;
   {
-    const size_t words = static_cast<size_t>(m.head_num) * m.seq_len;
+    const size_t words = static_cast<size_t>(dm.head_num) * dm.seq_len;
     if (cudaMalloc(&d_scores_, sizeof(unsigned long long) * words) != cudaSuccess)
       return static_cast<int>(cudaErrorMemoryAllocation);
     cudaMemsetAsync(d_scores_, 0, sizeof(unsigned long long) * words, stream);
@@ -2606,22 +2595,26 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     p.exch = exch - 1;
   };
 
-  const float eps = flavour_eps(m.flavour);
-  for (int l = 0; l < m.layer_num; ++l) {
-    const size_t layer_off = static_cast<size_t>(l) * m.seq_len * kvd;
+  // a GEMV segment of `rows` rows of the matrix `w`
+  auto seg = [](const Matrix& w, float* out, int rows, int head_major = 0, unsigned long long* tag_out = nullptr) {
+    return mega::Seg{w.w, w.scales, w.bias, out, 0, rows, head_major, tag_out};
+  };
+  for (int l = 0; l < dm.layer_num; ++l) {
+    const LayerWeights& lw = dm.layers[l];
+    const size_t layer_off = static_cast<size_t>(l) * dm.seq_len * kvd;
     {  // attention_rms + q | k | v (+bias).  q and the raw k are handed off only; v also goes into the cache.
       Phase p{};
       p.kind = mega::kPhaseGemv;
       p.in_dim = dim;
       p.n_seg = 3;
       input_is_x(p);
-      p.norm_w = m.attn_norm[l];
-      p.norm_eps = eps;
-      p.seg[0] = {m.wq[l], int8 ? m.sq[l] : nullptr, m.bq ? m.bq[l] : nullptr, nullptr, 0, q_rows, 0, t_q};
-      p.seg[1] = {m.wk[l], int8 ? m.sk[l] : nullptr, m.bk ? m.bk[l] : nullptr, nullptr, 0, kvd, 0, t_k};
+      p.norm_w = lw.attn_norm;
+      p.norm_eps = dm.eps;
+      p.seg[0] = seg(lw.q, nullptr, q_rows, 0, t_q);
+      p.seg[1] = seg(lw.k, nullptr, kvd, 0, t_k);
       float* vrows = kv_bf16_ ? reinterpret_cast<float*>(reinterpret_cast<__nv_bfloat16*>(m.value_cache) + layer_off)
                               : m.value_cache + layer_off;  // kv16_megakernel's epilogue stores bf16 elements
-      p.seg[2] = {m.wv[l], int8 ? m.sv[l] : nullptr, m.bv ? m.bv[l] : nullptr, vrows, 0, kvd, 1, t_v};
+      p.seg[2] = seg(lw.v, vrows, kvd, 1, t_v);
       p.units = q_rows + 2 * kvd;
       if (int rc = plan(p)) return rc;
       p.hand_out = hands;
@@ -2665,7 +2658,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
       p.n_seg = 1;
       p.tag_in = t_attn;
       p.hand_in = hands++;
-      p.seg[0] = {m.wo[l], int8 ? m.so[l] : nullptr, nullptr, nullptr, 0, dim, 0};
+      p.seg[0] = seg(lw.o, nullptr, dim);
       p.units = dim;
       if (int rc = plan(p)) return rc;
       p.tp_out = 1;
@@ -2679,10 +2672,10 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
       p.n_seg = 2;
       p.swiglu = 1;
       input_is_x(p);
-      p.norm_w = m.ffn_norm[l];
-      p.norm_eps = eps;
-      p.seg[0] = {m.w1[l], int8 ? m.s1[l] : nullptr, nullptr, nullptr, 0, hid, 0, t_h};
-      p.seg[1] = {m.w3[l], int8 ? m.s3[l] : nullptr, nullptr, nullptr, 0, hid, 0};
+      p.norm_w = lw.ffn_norm;
+      p.norm_eps = dm.eps;
+      p.seg[0] = seg(lw.w1, nullptr, hid, 0, t_h);
+      p.seg[1] = seg(lw.w3, nullptr, hid);
       p.units = hid;
       if (int rc = plan(p)) return rc;
       p.hand_out = hands;
@@ -2695,7 +2688,7 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
       p.n_seg = 1;
       p.tag_in = t_h;
       p.hand_in = hands++;
-      p.seg[0] = {m.w2[l], int8 ? m.s2[l] : nullptr, nullptr, nullptr, 0, dim, 0};
+      p.seg[0] = seg(lw.w2, nullptr, dim);
       p.units = dim;
       if (int rc = plan(p)) return rc;
       p.tp_out = 1;
@@ -2709,19 +2702,18 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
     p.in_dim = dim;
     p.n_seg = 1;
     input_is_x(p);
-    p.norm_w = m.final_norm;
-    p.norm_eps = eps;
+    p.norm_w = dm.final_norm;
+    p.norm_eps = dm.eps;
     p.cls = 1;
     // Tensor parallel: shard the classifier by vocabulary when the exchange area can carry a rank's
     // rows (kllm_comm_create(max_count >= vocab / world)); every rank still holds the whole matrix and
     // reads only its rows.  Otherwise it stays replicated.
-    const bool shard = W > 1 && m.vocab_size % W == 0 && m.tp_stride >= m.vocab_size / W;
-    cls_rows_ = shard ? m.vocab_size / W : m.vocab_size;
+    const int V = dm.vocab_size;
+    const bool shard = W > 1 && V % W == 0 && m.tp_stride >= V / W;
+    cls_rows_ = shard ? V / W : V;
     n_cls_phases_ = shard ? 2 : 1;
     if (shard) {
-      const size_t row0 = static_cast<size_t>(m.tp_rank) * cls_rows_;
-      p.seg[0] = {static_cast<const unsigned char*>(m.wcls) + row0 * dim * wb,
-                  int8 ? m.scls + row0 * (dim / m.group_size) : nullptr, nullptr, nullptr, 0, cls_rows_, 0};
+      p.seg[0] = seg(dm.rows_from(dm.cls, static_cast<size_t>(m.tp_rank) * cls_rows_, dim), nullptr, cls_rows_);
       p.units = cls_rows_;
       if (int rc = plan(p)) return rc;
       p.tp_out = 1;  // rows go to every rank's exchange area as tagged words
@@ -2731,14 +2723,14 @@ int MegaEngine::init(const MegaModel& m, cudaStream_t stream) {
       g.kind = mega::kPhaseGather;
       g.cls = 1;
       g.argmax = 1;
-      g.units = m.vocab_size;
+      g.units = V;
       g.in_dim = cls_rows_;
       g.exch = p.exch_out;
       g.seg[0].out = m.logits;
       ph.push_back(g);
     } else {
-      p.seg[0] = {m.wcls, int8 ? m.scls : nullptr, nullptr, m.logits, 0, m.vocab_size, 0};
-      p.units = m.vocab_size;
+      p.seg[0] = seg(dm.cls, m.logits, V);
+      p.units = V;
       p.argmax = 1;
       if (int rc = plan(p)) return rc;
       ph.push_back(p);
@@ -2798,6 +2790,7 @@ void MegaEngine::destroy() {
 Params MegaEngine::params(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev,
                           unsigned long long* prof_dev, int prof_token, int skip_cls_tokens) const {
   Params P{};
+  const DecoderModel& dm = *dm_;
   const MegaModel& m = model_;
   P.phases = static_cast<const Phase*>(d_phases_);
   P.n_phases = n_phases_;
@@ -2814,16 +2807,16 @@ Params MegaEngine::params(const DrawSettings& cfg, int n_tokens, const int32_t* 
   P.attn_split = attn_split_;
   P.attn_vsplit = attn_vsplit_;
   P.scores = d_scores_;
-  P.group_size = m.group_size;
-  P.dim = m.dim;
-  P.vocab_size = m.vocab_size;
-  P.head_num = m.head_num;
-  P.head_size = m.head_size;
-  P.kv_dim = m.kv_dim;
-  P.kv_mul = m.kv_mul;
-  P.seq_len = m.seq_len;
-  P.flavour = m.flavour;
-  P.tok_emb = m.tok_emb;
+  P.group_size = dm.group_size;
+  P.dim = dm.dim;
+  P.vocab_size = dm.vocab_size;
+  P.head_num = dm.head_num;
+  P.head_size = dm.head_size;
+  P.kv_dim = dm.kv_dim;
+  P.kv_mul = dm.kv_mul;
+  P.seq_len = dm.seq_len;
+  P.flavour = dm.flavour;
+  P.tok_emb = dm.tok_emb;
   P.score = m.score;
   P.key_cache = m.key_cache;
   P.value_cache = m.value_cache;
@@ -2832,12 +2825,12 @@ Params MegaEngine::params(const DrawSettings& cfg, int n_tokens, const int32_t* 
   P.state = m.state;
   P.out_tokens = m.out_tokens;
   P.teacher = teacher_dev;
-  P.max_steps = m.seq_len;
+  P.max_steps = dm.seq_len;
   P.barrier = static_cast<unsigned*>(d_barrier_);
   P.barrier_base = barrier_base_;
   P.tp_world = m.tp_world > 1 ? m.tp_world : 1;
   P.tp_rank = m.tp_world > 1 ? m.tp_rank : 0;
-  P.tp_stride = m.tp_world > 1 ? m.tp_stride : m.dim;
+  P.tp_stride = m.tp_world > 1 ? m.tp_stride : dm.dim;
   for (int r = 0; r < 8; ++r) P.tp_data[r] = m.tp_world > 1 ? m.tp_data[r] : nullptr;
   if (m.tp_world <= 1) P.tp_data[0] = d_tagged_;
   P.exch_per_token = exch_per_token_;

@@ -5,6 +5,7 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "decoder_model.h"
 #include "sampling.cuh"
 
 namespace kllm {
@@ -166,23 +167,8 @@ struct Params {
 
 }  // namespace mega
 
-// Everything the engine needs to know about the model; all pointers are device pointers, the
-// per-layer arrays are host arrays of device pointers (owned by the decoder).
+// What the engine needs besides the model (DecoderModel): all pointers are device pointers, the buffers the decoder owns.
 struct MegaModel {
-  int dim, hidden_dim, layer_num, head_num, kv_head_num, vocab_size, seq_len;
-  int head_size, kv_dim, kv_mul, flavour, group_size;
-  const float* tok_emb;
-  const float* const* attn_norm;
-  const float* const* ffn_norm;
-  const float* final_norm;
-  const void* const* wq; const void* const* wk; const void* const* wv; const void* const* wo;
-  const void* const* w1; const void* const* w2; const void* const* w3;
-  const void* wcls;
-  const float* const* sq; const float* const* sk; const float* const* sv; const float* const* so;
-  const float* const* s1; const float* const* s2; const float* const* s3;
-  const float* scls;
-  const float* const* bq; const float* const* bk; const float* const* bv;
-  // activations / state owned by the decoder
   float* logits; float* score;
   float* key_cache; float* value_cache;
   const float* sin_cache; const float* cos_cache;
@@ -198,12 +184,12 @@ struct MegaModel {
   int tp_stride;
   int numerics;  // kllm_decoder_desc::numerics
   int kv_cache;  // kllm_decoder_desc::kv_cache: KLLM_KV_BF16 needs the fast numerics (flash attention)
-  int weights;   // kllm_decoder_desc::weights: KLLM_WEIGHTS_BF16 = bf16 matrices (w16_megakernel), group_size 0
 };
 
 class MegaEngine {
  public:
-  int init(const MegaModel& m, cudaStream_t stream);
+  // `dm` is read again by every launch: it outlives the engine
+  int init(const DecoderModel& dm, const MegaModel& m, cudaStream_t stream);
   void destroy();
   // Run n_tokens consecutive positions starting from the device-resident state, under the decoder's settings
   // `cfg` (its step 0 and logprob setting ride in the launch parameters; the sampling parameters are read through
@@ -231,6 +217,7 @@ class MegaEngine {
   mega::Params params(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
                       int prof_token, int skip_cls_tokens) const;
   int launch(const mega::Params& P);
+  const DecoderModel* dm_ = nullptr;
   MegaModel model_{};
   void* d_lp_ = nullptr;  // lp_part [grid] float2, then lp_cand_v / lp_cand_i [grid][kMaxTopLogprobs]
   cudaStream_t stream_ = nullptr;
@@ -248,12 +235,12 @@ class MegaEngine {
   int int8_fast_ = 0;
   int fast_ = 0;  // numerics: 0 = bit-exact with the reference, 1 = toleranced (free summation order)
   int attn_vsplit_ = 1;
-  int kv_bf16_ = 0;  // bf16 KV cache: the kernels are kv16_megakernel's
+  int kv_bf16_ = 0;  // bf16 KV cache
   int cls_rows_ = 0, n_cls_phases_ = 1;
-  const void* kernel_ = nullptr;       // decode_megakernel<8 consumer warps, int8, false>
-  const void* kernel_prof_ = nullptr;  // ... <.., true>: records the phase timeline stamps (none with kv_bf16_ or
-                                       // bf16 weights)
-  const void* kernel_lp_ = nullptr;    // logprob_megakernel<8 consumer warps, int8>: log-probabilities on
+  // the instantiations of the weight format and KV cache (megakernel.cu, kernels_for)
+  const void* kernel_ = nullptr;       // plain
+  const void* kernel_prof_ = nullptr;  // records the phase timeline stamps; none with a bf16 cache or bf16 weights
+  const void* kernel_lp_ = nullptr;    // log-probabilities on
   size_t smem_bytes_ = 0;
   unsigned barrier_base_ = 0;
   bool ready_ = false;

@@ -19,6 +19,7 @@
 #include <cstdint>
 
 #include "../../include/kllm_b200.h"
+#include "cache_layout.h"
 #include "kllm_device.cuh"
 #include "kllm_host.h"
 
@@ -84,24 +85,6 @@ __global__ void swiglu_rows_kernel(float* __restrict__ h1, const float* __restri
     h1[i] = swiglu_ref(h1[i], h3[i]);
 }
 
-struct CacheLayout {
-  int mega;  // 1: persistent engine K [kvh][hs/4][seq][4], V [kvh][split][seq][hs/split]; 0: [seq][kv_dim]
-  int seq_len, kv_dim, head_size, split;
-  int bf16;  // with mega: bf16 elements, K [kvh][hs/8][seq][8] (16-byte chunks of 8 dims), V split 1
-};
-__device__ __forceinline__ size_t k_index(const CacheLayout& c, int pos, int kvh, int i) {
-  if (c.mega && c.bf16)
-    return (static_cast<size_t>(kvh) * (c.head_size >> 3) + (i >> 3)) * c.seq_len * 8 + static_cast<size_t>(pos) * 8 + (i & 7);
-  if (c.mega) return (static_cast<size_t>(kvh) * (c.head_size >> 2) + (i >> 2)) * c.seq_len * 4 + static_cast<size_t>(pos) * 4 + (i & 3);
-  return static_cast<size_t>(pos) * c.kv_dim + kvh * c.head_size + i;
-}
-__device__ __forceinline__ size_t v_index(const CacheLayout& c, int pos, int kvh, int i) {
-  if (c.mega) {
-    const int dv = c.head_size / c.split;
-    return ((static_cast<size_t>(kvh) * c.split + i / dv) * c.seq_len + pos) * dv + i % dv;
-  }
-  return static_cast<size_t>(pos) * c.kv_dim + kvh * c.head_size + i;
-}
 // A cache element of type E (float, or __nv_bfloat16 for the bf16 KV cache: rounded to nearest even on the way
 // in, widened exactly on the way out)
 __device__ __forceinline__ void put(float* p, float v) { *p = v; }
@@ -191,65 +174,65 @@ using namespace prefill;
     if (rc_ != 0) return rc_;              \
   } while (0)
 
-int prefill_block(const PrefillModel& m, PrefillWorkspace& ws, const int32_t* tokens_dev, int T, int start_pos,
-                  cudaStream_t s) {
-  const int dim = m.dim, hid = m.hidden_dim, hs = m.head_size, heads = m.head_num, kvh = m.kv_head_num;
-  const int q_rows = heads * hs, kvd = kvh * hs;
-  auto gemm = [&](const float* x, const void* w, const float* scales, float* out, int K, int N) {
-    if (m.group_size > 0)
-      return kllm_gemm_w8_tf32(x, static_cast<const int8_t*>(w), scales, out, T, K, N, m.group_size, s);
-    if (m.bf16) return kllm_gemm_bf16_tf32(x, static_cast<const uint16_t*>(w), out, T, K, N, s);
-    return kllm_gemm_tf32(x, static_cast<const float*>(w), out, T, K, N, s);
-  };
-  auto scales = [&](const float* const* per_layer, int l) { return m.group_size > 0 ? per_layer[l] : nullptr; };
+int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspace& ws, const int32_t* tokens_dev, int T,
+                  int start_pos, cudaStream_t s) {
+  const int dim = dm.dim, hid = dm.hidden_dim, heads = dm.head_num, kvh = dm.kv_head_num;
+  const int q_rows = dm.q_rows, kvd = dm.kv_dim;
   auto count = [&]() {
     count_launch();
     return static_cast<int>(cudaGetLastError());
   };
+  // out[T, N] = x[T, K] . w^T (+ bias)
+  auto gemm = [&](const float* x, const Matrix& w, float* out, int K, int N) {
+    int rc;
+    if (dm.format == WeightFormat::kInt8)
+      rc = kllm_gemm_w8_tf32(x, static_cast<const int8_t*>(w.w), w.scales, out, T, K, N, dm.group_size, s);
+    else if (dm.format == WeightFormat::kBf16)
+      rc = kllm_gemm_bf16_tf32(x, static_cast<const uint16_t*>(w.w), out, T, K, N, s);
+    else
+      rc = kllm_gemm_tf32(x, static_cast<const float*>(w.w), out, T, K, N, s);
+    if (rc != 0 || w.bias == nullptr) return rc;
+    add_bias_rows_kernel<<<T, 256, 0, s>>>(out, w.bias, N);
+    return count();
+  };
   const int ew_grid = 528;  // 4 x 132 SMs for the grid-stride elementwise kernels
-  embed_rows_kernel<<<T, 256, 0, s>>>(tokens_dev, m.tok_emb, ws.x, dim, m.vocab_size);
+  embed_rows_kernel<<<T, 256, 0, s>>>(tokens_dev, dm.tok_emb, ws.x, dim, dm.vocab_size);
   PF_TRY(count());
-  const CacheLayout cl{m.mega_layout, m.seq_len, kvd, hs, m.attn_split > 0 ? m.attn_split : 1, m.kv_bf16};
-  for (int l = 0; l < m.layer_num; ++l) {
-    const size_t layer_off = static_cast<size_t>(l) * m.seq_len * kvd;
-    rmsnorm_rows_kernel<<<T, 256, 0, s>>>(ws.x, m.attn_norm[l], ws.xn, dim, m.eps);
+  const CacheLayout& cl = m.cache;
+  for (int l = 0; l < dm.layer_num; ++l) {
+    const LayerWeights& lw = dm.layers[l];
+    const size_t layer_off = static_cast<size_t>(l) * dm.seq_len * kvd;
+    rmsnorm_rows_kernel<<<T, 256, 0, s>>>(ws.x, lw.attn_norm, ws.xn, dim, dm.eps);
     PF_TRY(count());
-    PF_TRY(gemm(ws.xn, m.wq[l], scales(m.sq, l), ws.q, dim, q_rows));
-    PF_TRY(gemm(ws.xn, m.wk[l], scales(m.sk, l), ws.k, dim, kvd));
-    PF_TRY(gemm(ws.xn, m.wv[l], scales(m.sv, l), ws.v, dim, kvd));
-    if (m.bq != nullptr) {
-      add_bias_rows_kernel<<<T, 256, 0, s>>>(ws.q, m.bq[l], q_rows);
-      add_bias_rows_kernel<<<T, 256, 0, s>>>(ws.k, m.bk[l], kvd);
-      add_bias_rows_kernel<<<T, 256, 0, s>>>(ws.v, m.bv[l], kvd);
-      count_launch(2);
-      PF_TRY(count());
-    }
+    PF_TRY(gemm(ws.xn, lw.q, ws.q, dim, q_rows));
+    PF_TRY(gemm(ws.xn, lw.k, ws.k, dim, kvd));
+    PF_TRY(gemm(ws.xn, lw.v, ws.v, dim, kvd));
     const size_t sc_bytes = static_cast<size_t>(start_pos + T) * sizeof(float);
-    if (m.kv_bf16) {
+    if (cl.bf16) {
       __nv_bfloat16* kc = reinterpret_cast<__nv_bfloat16*>(m.key_cache) + layer_off;
       __nv_bfloat16* vc = reinterpret_cast<__nv_bfloat16*>(m.value_cache) + layer_off;
       rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc, vc, cl, heads, kvh,
-                                            m.flavour, start_pos);
+                                            dm.flavour, start_pos);
       PF_TRY(count());
-      attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, kc, vc, ws.att, cl, heads, heads / kvh, start_pos);
+      attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, kc, vc, ws.att, cl, heads, dm.kv_mul, start_pos);
     } else {
       rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, m.key_cache + layer_off,
-                                            m.value_cache + layer_off, cl, heads, kvh, m.flavour, start_pos);
+                                            m.value_cache + layer_off, cl, heads, kvh, dm.flavour, start_pos);
       PF_TRY(count());
       attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, m.key_cache + layer_off, m.value_cache + layer_off,
-                                                             ws.att, cl, heads, heads / kvh, start_pos);
+                                                             ws.att, cl, heads, dm.kv_mul, start_pos);
     }
     PF_TRY(count());
-    PF_TRY(gemm(ws.att, m.wo[l], scales(m.so, l), ws.tmp, q_rows, dim));
+    PF_TRY(gemm(ws.att, lw.o, ws.tmp, q_rows, dim));
     add_rows_kernel<<<ew_grid, 256, 0, s>>>(ws.x, ws.tmp, static_cast<size_t>(T) * dim);
     PF_TRY(count());
-    rmsnorm_rows_kernel<<<T, 256, 0, s>>>(ws.x, m.ffn_norm[l], ws.xn, dim, m.eps);
+    rmsnorm_rows_kernel<<<T, 256, 0, s>>>(ws.x, lw.ffn_norm, ws.xn, dim, dm.eps);
     PF_TRY(count());
-    PF_TRY(gemm(ws.xn, m.w1[l], scales(m.s1, l), ws.h1, dim, hid));
-    PF_TRY(gemm(ws.xn, m.w3[l], scales(m.s3, l), ws.h3, dim, hid));
+    PF_TRY(gemm(ws.xn, lw.w1, ws.h1, dim, hid));
+    PF_TRY(gemm(ws.xn, lw.w3, ws.h3, dim, hid));
     swiglu_rows_kernel<<<ew_grid, 256, 0, s>>>(ws.h1, ws.h3, static_cast<size_t>(T) * hid);
     PF_TRY(count());
-    PF_TRY(gemm(ws.h1, m.w2[l], scales(m.s2, l), ws.tmp, hid, dim));
+    PF_TRY(gemm(ws.h1, lw.w2, ws.tmp, hid, dim));
     add_rows_kernel<<<ew_grid, 256, 0, s>>>(ws.x, ws.tmp, static_cast<size_t>(T) * dim);
     PF_TRY(count());
   }
