@@ -296,7 +296,16 @@ typedef struct {
    * values.  kllm_decoder_create returns KLLM_E_INVALID for any other value and KLLM_E_UNSUPPORTED, creating
    * nothing, when KLLM_KV_BF16 cannot be honoured: exact numerics (after the KLLM_MODE override), the graph
    * engine (KLLM_ENGINE=graph, or a shape only it takes), tp_size > 1, or head_size % 32 != 0.
-   * kllm_decoder_profile returns KLLM_E_UNSUPPORTED on a bf16 decoder. */
+   * kllm_decoder_profile returns KLLM_E_UNSUPPORTED on a bf16 decoder.
+   * KLLM_KV_FP8 (2, DESIGN.md 5.12): both caches hold fp8 e4m3 codes (__nv_fp8_e4m3, torch.float8_e4m3fn) with a
+   * static scale per (layer, KV head) from kv_scales (required) -- a quarter of the fp32 cache's memory and reads.  An element x
+   * of a K row (after RoPE) or a V row at layer l, KV head h is cached as code = e4m3(fp32(x * inv)), round to nearest
+   * even and saturated to +-448, with inv = 1.0f / s (one fp32 division per scale, at create); the code stands for
+   * value(code) * s.  The positions are as for KLLM_KV_BF16: a decode step reads rows < pos from the cache and row pos
+   * unrounded from registers, the batched prefill reads every row from the cache.  All arithmetic stays fp32 (the
+   * kernels may fold s into the score scale and the merged output).  kllm_decoder_read_kv returns fp32(value * s).
+   * The refusals are KLLM_KV_BF16's, with head_size % 64 != 0 in place of % 32; fp32, int8 and bf16 weights all
+   * take it. */
   int32_t kv_cache;
   /* Storage of the weight matrices (DESIGN.md 5.11).  KLLM_WEIGHTS_F32 (0, the default of a zeroed struct): as
    * group_size says.  KLLM_WEIGHTS_BF16 (1): wq wk wv wo w1 w2 w3 and wcls are device arrays of bf16 (uint16 bit
@@ -311,11 +320,19 @@ typedef struct {
    * group_size > 0, and KLLM_E_UNSUPPORTED, creating nothing, for tp_size > 1.  kllm_decoder_prefill_w8 and
    * kllm_decoder_profile return KLLM_E_UNSUPPORTED on a bf16-weight decoder. */
   int32_t weights;
+  /* The fp8 KV cache's scales (kv_cache KLLM_KV_FP8), a host array [2][layer_num][kv_head_num]: first the K scales
+   * s_k[l][h], then the V scales s_v[l][h] (kv_head_num as given here, this rank's).  Copied at create.  Required
+   * with KLLM_KV_FP8 and NULL (the default of a zeroed struct) with every other cache: kllm_decoder_create returns
+   * KLLM_E_INVALID for KLLM_KV_FP8 without scales (a description written before the fp8 cache existed, whose value 2
+   * was refused, stays refused), for scales with another cache, and for a scale that is not finite and > 0.  Unit
+   * scales are an array of ones; the Python and C++ front ends pass one when no scales are given. */
+  const float* kv_scales;
 } kllm_decoder_desc;
 #define KLLM_NUMERICS_EXACT 0
 #define KLLM_NUMERICS_FAST 1
 #define KLLM_KV_F32 0
 #define KLLM_KV_BF16 1
+#define KLLM_KV_FP8 2
 #define KLLM_WEIGHTS_F32 0
 #define KLLM_WEIGHTS_BF16 1
 
@@ -471,7 +488,7 @@ int kllm_decoder_score(kllm_decoder* dec, const int32_t* tokens_host, int32_t n_
 
 /* Blocking copies for tests: logits of the last step [vocab]; the KV cache in the REFERENCE
  * layout [layer][seq_len][kv_dim] (llama3.cpp:469-475) whatever the engine keeps internally (a bf16
- * cache, KLLM_KV_BF16: its values widened exactly to fp32). */
+ * cache, KLLM_KV_BF16: its values widened exactly to fp32; an fp8 cache, KLLM_KV_FP8: fp32(value(code) * scale)). */
 int kllm_decoder_logits(kllm_decoder* dec, float* logits_host);
 /* Device pointer to the same logits [vocab] (what the reference keeps in
  * ModelBufferType::kForwardOutput, llama3.cpp:498-506); valid until the decoder is destroyed,

@@ -63,6 +63,7 @@ class DecoderDesc(ctypes.Structure):
         ("tp_size", c_int32), ("tp_rank", c_int32),
         ("allreduce", ALLREDUCE_FN), ("allreduce_ctx", c_void_p), ("comm", c_void_p),
         ("numerics", c_int32), ("kv_cache", c_int32), ("weights", c_int32),
+        ("kv_scales", POINTER(ctypes.c_float)),
     ]
 
 

@@ -5,18 +5,26 @@
 
 #include <cstddef>
 
+#include "../../include/kllm_b200.h"
+
 namespace kllm {
 namespace prefill {  // the prefill's kernels take a CacheLayout by value
 
 struct CacheLayout {
   int mega;  // 1: persistent engine K [kvh][hs/4][seq][4], V [kvh][split][seq][hs/split]; 0: [seq][kv_dim]
   int seq_len, kv_dim, head_size, split;
-  int bf16;  // with mega: bf16 elements, K [kvh][hs/8][seq][8] (16-byte chunks of 8 dims), V split 1
+  // the element, a kllm_decoder_desc::kv_cache value.  With mega, K keeps 16-byte chunks: KLLM_KV_BF16 K
+  // [kvh][hs/8][seq][8] bf16, KLLM_KV_FP8 K [kvh][hs/16][seq][16] e4m3 codes; both with V split 1
+  int elem;
 };
+__host__ __device__ __forceinline__ int kv_elem_bytes(int elem) {
+  return elem == KLLM_KV_FP8 ? 1 : elem == KLLM_KV_BF16 ? 2 : 4;
+}
 __host__ __device__ __forceinline__ size_t k_index(const CacheLayout& c, int pos, int kvh, int i) {
-  if (c.mega && c.bf16)
-    return (static_cast<size_t>(kvh) * (c.head_size >> 3) + (i >> 3)) * c.seq_len * 8 + static_cast<size_t>(pos) * 8 + (i & 7);
-  if (c.mega) return (static_cast<size_t>(kvh) * (c.head_size >> 2) + (i >> 2)) * c.seq_len * 4 + static_cast<size_t>(pos) * 4 + (i & 3);
+  if (c.mega) {  // w elements of a 16-byte chunk
+    const int w = 16 / kv_elem_bytes(c.elem);
+    return (static_cast<size_t>(kvh) * (c.head_size / w) + i / w) * c.seq_len * w + static_cast<size_t>(pos) * w + i % w;
+  }
   return static_cast<size_t>(pos) * c.kv_dim + kvh * c.head_size + i;
 }
 __host__ __device__ __forceinline__ size_t v_index(const CacheLayout& c, int pos, int kvh, int i) {

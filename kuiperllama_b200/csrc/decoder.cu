@@ -101,6 +101,19 @@ argmax_advance_kernel(const float* __restrict__ logits, int n, const DrawSetting
   }
 }
 
+// value(code) of an e4m3 code (sign, 4 exponent bits of bias 7, 3 mantissa bits; no infinities, S.1111.111 is NaN)
+float e4m3_value_host(uint8_t code) {
+  const int e = (code >> 3) & 15, f = code & 7;
+  float v;
+  if (e == 15 && f == 7)
+    v = NAN;
+  else if (e == 0)
+    v = std::ldexp(static_cast<float>(f), -9);  // subnormal: f / 8 * 2^-6
+  else
+    v = std::ldexp(static_cast<float>(8 + f), e - 10);
+  return (code & 0x80) ? -v : v;
+}
+
 int build_decoder_model(const kllm_decoder_desc& d, DecoderModel* out) {
   if (d.dim <= 0 || d.hidden_dim <= 0 || d.layer_num <= 0 || d.head_num <= 0 ||
       d.kv_head_num <= 0 || d.vocab_size <= 0 || d.seq_len <= 0)
@@ -115,7 +128,14 @@ int build_decoder_model(const kllm_decoder_desc& d, DecoderModel* out) {
   // head_size from the FULL model: dim / (head_num * tp)
   if (d.dim % (d.head_num * tp) != 0 || d.head_num % d.kv_head_num != 0) return KLLM_E_INVALID;
   if ((d.dim & 3) != 0 || (d.hidden_dim & 3) != 0) return KLLM_E_UNSUPPORTED;
-  if (d.kv_cache != KLLM_KV_F32 && d.kv_cache != KLLM_KV_BF16) return KLLM_E_INVALID;
+  if (d.kv_cache != KLLM_KV_F32 && d.kv_cache != KLLM_KV_BF16 && d.kv_cache != KLLM_KV_FP8) return KLLM_E_INVALID;
+  // the fp8 cache's scales: given for that cache and only for it, each finite and > 0.  A description with kv_cache 2
+  // and no scales -- one written before the fp8 cache existed -- stays refused as it was.
+  if ((d.kv_cache == KLLM_KV_FP8) != (d.kv_scales != nullptr)) return KLLM_E_INVALID;
+  if (d.kv_scales != nullptr) {
+    for (size_t i = 0; i < 2 * static_cast<size_t>(d.layer_num) * d.kv_head_num; ++i)
+      if (!std::isfinite(d.kv_scales[i]) || !(d.kv_scales[i] > 0.f)) return KLLM_E_INVALID;
+  }
   // bf16 weights: fp32 checkpoints' matrices rounded by the caller; one GPU
   if (d.weights != KLLM_WEIGHTS_F32 && d.weights != KLLM_WEIGHTS_BF16) return KLLM_E_INVALID;
   const bool w16 = d.weights == KLLM_WEIGHTS_BF16;
@@ -166,6 +186,10 @@ struct kllm_decoder {
   float *x = nullptr, *q = nullptr, *attn = nullptr, *h = nullptr, *logits = nullptr;
   float *score = nullptr, *kcache = nullptr, *vcache = nullptr, *sin_t = nullptr, *cos_t = nullptr;
   float* tp_tmp = nullptr;
+  // the fp8 KV cache's scales (KLLM_KV_FP8): [2][L][kv_head] s_k, s_v on the host (kllm_decoder_read_kv), and on the
+  // device [4][L][kv_head] s_k, s_v, 1 / s_k, 1 / s_v
+  std::vector<float> kv_scales;
+  float* kv_scales_dev = nullptr;
   MegaEngine mega;
   bool use_mega = false;
   mega::State* st = nullptr;
@@ -379,7 +403,7 @@ int prefill_args(const kllm_decoder* dc, const int32_t* tokens_host, int32_t n_t
 prefill::CacheLayout cache_layout(const kllm_decoder* dc) {
   const DecoderModel& m = dc->m;
   return {dc->use_mega ? 1 : 0, m.seq_len, m.kv_dim, m.head_size, dc->use_mega ? dc->mega.attn_vsplit() : 1,
-          dc->d.kv_cache == KLLM_KV_BF16 ? 1 : 0};
+          dc->d.kv_cache};
 }
 
 int run_prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
@@ -404,7 +428,7 @@ int run_prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, 
     dc->pf_ws.h1 = take(m.hidden_dim), dc->pf_ws.h3 = take(m.hidden_dim);
   }
   KLLM_TRY(prefill_attention_smem_opt_in(static_cast<size_t>(start_pos + n_tokens) * sizeof(float)));
-  const PrefillModel pm{cache_layout(dc), dc->kcache, dc->vcache, dc->sin_t, dc->cos_t};
+  const PrefillModel pm{cache_layout(dc), dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->kv_scales_dev};
 
   std::memcpy(dc->io_host, tokens_host, sizeof(int32_t) * n_tokens);
   KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_tokens, cudaMemcpyHostToDevice, dc->stream));
@@ -441,12 +465,12 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
   DecoderModel model;
   KLLM_TRY(build_decoder_model(d, &model));
   const int tp = d.tp_size > 1 ? d.tp_size : 1;
-  // a bf16 cache exists on the persistent engine's flash form only; the rest of the refusals come from its init
-  const bool kv_bf16 = d.kv_cache == KLLM_KV_BF16;
+  // bf16 and fp8 caches exist on the persistent engine's flash form only; the rest of the refusals come from its init
+  const bool kv_lowp = d.kv_cache != KLLM_KV_F32;
   const char* want = getenv("KLLM_ENGINE");
   const bool force_graph = want != nullptr && strcmp(want, "graph") == 0;
   const bool force_mega = want != nullptr && strcmp(want, "persistent") == 0;
-  if (kv_bf16 && (tp > 1 || force_graph)) return KLLM_E_UNSUPPORTED;
+  if (kv_lowp && (tp > 1 || force_graph)) return KLLM_E_UNSUPPORTED;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return KLLM_E_NODEVICE;
 
@@ -482,7 +506,8 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     return static_cast<int>(cudaMemsetAsync(*p, 0, n * sizeof(float), dc->stream));
   };
   const size_t kv_elems = static_cast<size_t>(m.layer_num) * m.seq_len * m.kv_dim;
-  const size_t kv_floats = kv_bf16 ? (kv_elems + 1) / 2 : kv_elems;  // bf16: half the bytes behind the same pointers
+  // bf16 / fp8: a half / a quarter of the bytes behind the same pointers
+  const size_t kv_floats = (kv_elems * prefill::kv_elem_bytes(d.kv_cache) + 3) / 4;
   if (dev_alloc(&dc->x, m.dim) || dev_alloc(&dc->q, m.q_rows) || dev_alloc(&dc->attn, m.q_rows) ||
       dev_alloc(&dc->h, m.hidden_dim) || dev_alloc(&dc->logits, m.vocab_size) ||
       dev_alloc(&dc->score, static_cast<size_t>(m.head_num) * m.seq_len) ||
@@ -492,6 +517,17 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
       dev_alloc(&dc->tp_tmp, m.dim) || dev_alloc(&dc->penalized, m.vocab_size) ||
       dev_alloc(&dc->bias, m.vocab_size))
     return fail(static_cast<int>(cudaErrorMemoryAllocation));
+  if (d.kv_cache == KLLM_KV_FP8) {
+    const size_t n = static_cast<size_t>(m.layer_num) * m.kv_head_num;
+    dc->kv_scales.assign(d.kv_scales, d.kv_scales + 2 * n);
+    std::vector<float> dev(4 * n);
+    for (size_t i = 0; i < 2 * n; ++i) dev[i] = dc->kv_scales[i], dev[2 * n + i] = 1.0f / dc->kv_scales[i];
+    // a blocking copy into unset memory: no memset on dc->stream may land after it
+    if (cudaMalloc(&dc->kv_scales_dev, 4 * n * sizeof(float)) != cudaSuccess ||
+        cudaMemcpy(dc->kv_scales_dev, dev.data(), 4 * n * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess)
+      return fail(static_cast<int>(cudaErrorMemoryAllocation));
+  }
+  dc->d.kv_scales = nullptr;  // the caller's array is not read after create
   if (cudaMalloc(&dc->st, sizeof(mega::State)) != cudaSuccess ||
       cudaMalloc(&dc->d_cfg, sizeof(DrawSettings)) != cudaSuccess ||
       cudaMalloc(&dc->hist, sizeof(int32_t) * m.seq_len) != cudaSuccess ||
@@ -523,7 +559,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
   // Engine: the persistent megakernel (one cooperative launch per run) when the shape fits its
   // shared-memory ring, else the CUDA-graph chain of fused launches.  KLLM_ENGINE=graph|persistent
   // forces one (persistent fails loudly if unsupported).  Both are CUDA; neither is a fallback to
-  // anything off-device.  A bf16 cache never falls back to the graph engine.
+  // anything off-device.  A bf16 or fp8 cache never falls back to the graph engine.
   // tensor parallel: the persistent engine needs the peer-memory transport (its exchange IS
   // the all-reduce); with NCCL or a caller-supplied callback the graph engine is used
   unsigned long long* tp_areas[8] = {};
@@ -538,6 +574,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     mm.tp_world = tp, mm.tp_rank = tp_rank, mm.tp_stride = tp_stride;
     mm.numerics = d.numerics;
     mm.kv_cache = d.kv_cache;
+    mm.kv_scales = dc->kv_scales_dev;
     for (int r = 0; r < 8; ++r) mm.tp_data[r] = tp_areas[r];
     mm.logits = dc->logits, mm.score = dc->score, mm.key_cache = dc->kcache, mm.value_cache = dc->vcache;
     mm.sin_cache = dc->sin_t, mm.cos_cache = dc->cos_t, mm.state = dc->st, mm.out_tokens = dc->out_tokens;
@@ -548,10 +585,10 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     if (rc == 0) {
       dc->use_mega = true;
       dc->launches_per_step = 1;
-    } else if (rc != KLLM_E_UNSUPPORTED || force_mega || kv_bf16) {
+    } else if (rc != KLLM_E_UNSUPPORTED || force_mega || kv_lowp) {
       return fail(rc);
     }
-  } else if (force_mega || kv_bf16) {
+  } else if (force_mega || kv_lowp) {
     return fail(KLLM_E_UNSUPPORTED);
   }
   if (!dc->use_mega && (rc = capture(dc)) != 0) return fail(rc);
@@ -567,7 +604,8 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->exec) cudaGraphExecDestroy(dc->exec);
   if (dc->graph) cudaGraphDestroy(dc->graph);
   float* bufs[] = {dc->x, dc->q, dc->attn, dc->h, dc->logits, dc->score,
-                   dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->penalized, dc->bias};
+                   dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->penalized, dc->bias,
+                   dc->kv_scales_dev};
   for (float* b : bufs)
     if (b) cudaFree(b);
   if (dc->st) cudaFree(dc->st);
@@ -832,8 +870,8 @@ int kllm_decoder_profile(kllm_decoder* dc, int32_t first_token, int32_t start_po
                          int32_t profiled_step, uint64_t* stamps_host, int32_t capacity,
                          int32_t* grid_out, int32_t* phases_out) {
   if (!dc || !stamps_host || !grid_out || !phases_out || n_steps <= 0) return KLLM_E_INVALID;
-  // no timeline kernel for the bf16 cache or bf16 weights
-  if (!dc->use_mega || dc->d.kv_cache == KLLM_KV_BF16 || dc->m.format == WeightFormat::kBf16) return KLLM_E_UNSUPPORTED;
+  // no timeline kernel for the bf16 or fp8 cache or bf16 weights
+  if (!dc->use_mega || dc->d.kv_cache != KLLM_KV_F32 || dc->m.format == WeightFormat::kBf16) return KLLM_E_UNSUPPORTED;
   if (start_pos < 0 || start_pos + n_steps > dc->m.seq_len) return KLLM_E_INVALID;
   const int grid = dc->mega.grid(), phases = dc->mega.phases();
   const size_t n = static_cast<size_t>(grid) * phases * mega::kProfStamps;
@@ -867,15 +905,17 @@ int kllm_decoder_read_kv(kllm_decoder* dc, float* key_host, float* value_host) {
   KLLM_TRY(cudaStreamSynchronize(dc->stream));
   const DecoderModel& m = dc->m;
   const size_t S = m.seq_len, kvd = m.kv_dim, hs = m.head_size, layer = S * kvd, n = m.layer_num * layer;
-  // each layer in the engine's layout -> reference [L][S][kv_dim], a bf16 element widened exactly
+  // each layer in the engine's layout -> reference [L][S][kv_dim], a bf16 element widened exactly, an fp8 one as
+  // fp32(value(code) * s) at its layer's and kv head's scale s
   const prefill::CacheLayout c = cache_layout(dc);
-  const size_t esz = c.bf16 ? 2 : 4;
+  const size_t esz = prefill::kv_elem_bytes(c.elem);
   std::vector<unsigned char> kraw(n * esz), vraw(n * esz);
   KLLM_TRY(cudaMemcpy(kraw.data(), dc->kcache, n * esz, cudaMemcpyDeviceToHost));
   KLLM_TRY(cudaMemcpy(vraw.data(), dc->vcache, n * esz, cudaMemcpyDeviceToHost));
   auto at = [&](const std::vector<unsigned char>& raw, size_t i) {
     uint32_t u = 0;
-    if (c.bf16) {
+    if (c.elem == KLLM_KV_FP8) return e4m3_value_host(raw[i]);
+    if (c.elem == KLLM_KV_BF16) {
       uint16_t b;
       std::memcpy(&b, raw.data() + 2 * i, sizeof(b));
       u = static_cast<uint32_t>(b) << 16;
@@ -886,14 +926,20 @@ int kllm_decoder_read_kv(kllm_decoder* dc, float* key_host, float* value_host) {
     std::memcpy(&f, &u, sizeof(f));
     return f;
   };
+  const size_t nh = static_cast<size_t>(m.layer_num) * m.kv_head_num;
   for (size_t l = 0; l < static_cast<size_t>(m.layer_num); ++l)
     for (int t = 0; t < m.seq_len; ++t)
-      for (int g = 0; g < m.kv_head_num; ++g)
+      for (int g = 0; g < m.kv_head_num; ++g) {
+        float sk = 1.f, sv = 1.f;
+        if (c.elem == KLLM_KV_FP8) sk = dc->kv_scales[l * m.kv_head_num + g], sv = dc->kv_scales[nh + l * m.kv_head_num + g];
         for (int i = 0; i < m.head_size; ++i) {
           const size_t dst = (l * S + t) * kvd + g * hs + i;
-          key_host[dst] = at(kraw, l * layer + prefill::k_index(c, t, g, i));
-          value_host[dst] = at(vraw, l * layer + prefill::v_index(c, t, g, i));
+          const float k = at(kraw, l * layer + prefill::k_index(c, t, g, i));
+          const float v = at(vraw, l * layer + prefill::v_index(c, t, g, i));
+          key_host[dst] = c.elem == KLLM_KV_FP8 ? k * sk : k;
+          value_host[dst] = c.elem == KLLM_KV_FP8 ? v * sv : v;
         }
+      }
   return 0;
 }
 

@@ -52,8 +52,9 @@ int comm_tagged_areas(kllm_comm* comm, unsigned long long** areas8, int* world, 
 // the caches in the layout of the engine that continues decoding
 struct PrefillModel {
   prefill::CacheLayout cache;
-  float* key_cache; float* value_cache;  // cache.bf16: bf16 elements behind these pointers
+  float* key_cache; float* value_cache;  // cache.elem: bf16 or fp8 elements behind these pointers
   const float* sin_cache; const float* cos_cache;
+  const float* kv_scales;  // KLLM_KV_FP8: device [4][L][kv_head], s_k, s_v, 1 / s_k, 1 / s_v
 };
 struct PrefillWorkspace {  // [block, .] activations
   float *x, *xn, *q, *k, *v, *att, *h1, *h3, *tmp;

@@ -51,6 +51,7 @@
 #include "../../include/kllm_b200.h"
 #include "kllm_device.cuh"
 #include "kllm_host.h"
+#include "kv_fp8.cuh"
 #include "megakernel.h"
 
 namespace kllm {
@@ -350,6 +351,12 @@ __device__ __forceinline__ float lds_bf16(uint32_t a) {
   unsigned short v;
   asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(a));
   return __uint_as_float(static_cast<uint32_t>(v) << 16);
+}
+// fp8 KV cache: value(code) of the e4m3 code at a, exact
+__device__ __forceinline__ float lds_e4m3(uint32_t a) {
+  unsigned short v;
+  asm volatile("ld.shared.u8 %0, [%1];" : "=h"(v) : "r"(a));
+  return e4m3_value(static_cast<uint8_t>(v));
 }
 // the two bf16 elements of a 32-bit word (held as a float's bits): element 2i in the low half, 2i + 1 in the high
 __device__ __forceinline__ float bf16_lo(float w) { return __uint_as_float(__float_as_uint(w) << 16); }
@@ -884,8 +891,9 @@ __device__ __forceinline__ AttnIn poll_attention_inputs(const unsigned long long
 
 // RoPE on q (this head) and -- with_k -- on the new key row (rope_kernel.cu as compiled, elementwise.cu); the
 // rotated key goes to k_s and, by one CTA per kv head, into the cache row of `pos` (rounded to bf16 with
-// KV16, the bf16 KV cache).  Returns this thread's element of the value row (with_v, tid < hs), else 0.
-template <bool KV16 = false>
+// the bf16 KV cache, encoded at its layer's and kv head's scale with the fp8 one: KV, a kllm_decoder_desc::kv_cache
+// value).  Returns this thread's element of the value row (with_v, tid < hs), else 0.
+template <int KV = KLLM_KV_F32>
 __device__ __forceinline__ float attention_inputs(const Params& P, const Phase& ph, int head, int kvh, int pos, unsigned tag_in,
                                                   bool with_k, bool with_v, float* q_s, float* k_s, size_t head_block) {
   const int tid = threadIdx.x;
@@ -916,7 +924,12 @@ __device__ __forceinline__ float attention_inputs(const Params& P, const Phase& 
       k_s[i0] = r0;
       k_s[i1] = r1;
       if (head % P.kv_mul == 0) {  // one writer per kv head stores the rotated key
-        if constexpr (KV16) {
+        if constexpr (KV == KLLM_KV_FP8) {
+          uint8_t* kcache = reinterpret_cast<uint8_t*>(P.key_cache) + head_block;
+          const float inv = P.kv_inv_k[ph.layer * (P.kv_dim / hs) + kvh];
+          kcache[(static_cast<size_t>(i0 >> 4) * seq_len + pos) * 16 + (i0 & 15)] = e4m3_encode(r0, inv);
+          kcache[(static_cast<size_t>(i1 >> 4) * seq_len + pos) * 16 + (i1 & 15)] = e4m3_encode(r1, inv);
+        } else if constexpr (KV == KLLM_KV_BF16) {
           __nv_bfloat16* kcache = reinterpret_cast<__nv_bfloat16*>(P.key_cache) + head_block;
           kcache[(static_cast<size_t>(i0 >> 3) * seq_len + pos) * 8 + (i0 & 7)] = __float2bfloat16_rn(r0);
           kcache[(static_cast<size_t>(i1 >> 3) * seq_len + pos) * 8 + (i1 & 7)] = __float2bfloat16_rn(r1);
@@ -949,6 +962,8 @@ __device__ __forceinline__ float attention_inputs(const Params& P, const Phase& 
 //       block and "thread i walks column i" is conflict-free.
 //   bf16 KV cache (flash form, SP layout 1): K [L][kv_head][head_size/8][seq_len][8] and V [L][kv_head][seq_len]
 //       [head_size] in bf16 -- still 16-byte chunks and contiguous V rows, half the bytes.
+//   fp8 KV cache (the same form): K [L][kv_head][head_size/16][seq_len][16] and V [L][kv_head][seq_len][head_size]
+//       in e4m3 codes -- a quarter of the bytes.
 // Rows t < pos were written by earlier tokens, so -- like weights -- the producer warp streams
 // them through the ring ahead of time; only row pos is handled here from registers.
 __device__ __forceinline__ int attn_tiles(int pos, int T) { return (pos + T - 1) / T; }
@@ -1274,11 +1289,15 @@ __device__ KLLM_PHASE_CALL Pipe attention_pv_phase(const Params& P, int head, in
 // bf16 KV cache (KV16): the same mapping over tiles of half the bytes -- a 16-byte K chunk is 8 dims of a
 // timestep (K tile [hs/8][T][8], so a quarter of the head is hs/32 chunks) and the V tile is [T][hs] bf16;
 // every element is widened exactly to fp32 and the arithmetic is unchanged.
+// fp8 KV cache: a 16-byte K chunk is 16 dims (a quarter of the head is hs/64 chunks, host: head_size % 64 == 0) and
+// the V tile is [T][hs] e4m3 codes; each code widens exactly to value(code), the K scale s_k is folded into the
+// cached rows' score scale and the V scale s_v into the warp partials o[] (the row of pos, from registers, is
+// unscaled).
 // At the end the CW warp partials (m, l, o[hs]) are merged through shared memory, CTA 0 of the head folds
 // in the current position's row from registers and merges the partials of the other CTAs that had
 // tiles (tagged words in the scores area: [head][s][hs + 2]); at short contexts (pos <= T) that is
 // nobody, and the phase costs what the fused one does.
-template <int CW, bool KV16>
+template <int CW, int KV>
 __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head, int split, int pos, Pipe pipe,
                                                        unsigned tag_in, unsigned tag_out, unsigned long long* stamp) {
   const Phase& ph = g_ph_cons;
@@ -1301,11 +1320,15 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
   const int kvh = head / P.kv_mul;
   const size_t head_block = (static_cast<size_t>(ph.layer) * (P.kv_dim / hs) + kvh) * seq_len * hs;
   // q, and in CTA 0 of the head the new key row (rotated) and the value row of the current position
-  const float v_pos = attention_inputs<KV16>(P, ph, head, kvh, pos, tag_in, split == 0, split == 0, q_s, k_s, head_block);
+  const float v_pos = attention_inputs<KV>(P, ph, head, kvh, pos, tag_in, split == 0, split == 0, q_s, k_s, head_block);
   consumer_sync<CT>();
   const long long c_rope = stamp ? clock64() : 0;
 
+  constexpr bool KV16 = KV == KLLM_KV_BF16, KV8 = KV == KLLM_KV_FP8;
   const float scale = 1.f / sqrtf(static_cast<float>(hs));
+  // the cached rows' score scale: with the fp8 cache s_k folded in
+  float tile_scale = scale;
+  if constexpr (KV8) tile_scale = scale * P.kv_scale_k[ph.layer * (P.kv_dim / hs) + kvh];
   const float4* q4 = reinterpret_cast<const float4*>(q_s);
   const int cg = lane >> 3, tt = lane & 7;
   const int cpg = hs >> 4;        // 16-byte chunks per quarter of head_size (host: head_size % 16 == 0)
@@ -1330,7 +1353,22 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
       const int tl = b * 8 + tt;  // this lane's timestep within the tile
       const bool valid = tl < nt;
       float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-      if (KV16 && valid) {  // chunk c = dims 8c .. 8c + 7 of the timestep, 8 bf16 (host: head_size % 32 == 0)
+      if (KV8 && valid) {  // chunk c = dims 16c .. 16c + 15 of the timestep, 16 e4m3 codes (host: head_size % 64 == 0)
+#pragma unroll 2
+        for (int c = cg * (cpg >> 2); c < (cg + 1) * (cpg >> 2); ++c) {
+          const float4 kw = lds_f4(ktile + static_cast<uint32_t>(c * T + tl) * 16u);
+          const float kword[4] = {kw.x, kw.y, kw.z, kw.w};
+#pragma unroll
+          for (int w = 0; w < 4; ++w) {
+            const float4 kv = e4m3x4_values(__float_as_uint(kword[w]));
+            const float4 qv = q4[4 * c + w];
+            a0 = __fmaf_rn(kv.x, qv.x, a0);
+            a1 = __fmaf_rn(kv.y, qv.y, a1);
+            a2 = __fmaf_rn(kv.z, qv.z, a2);
+            a3 = __fmaf_rn(kv.w, qv.w, a3);
+          }
+        }
+      } else if (KV16 && valid) {  // chunk c = dims 8c .. 8c + 7 of the timestep, 8 bf16 (host: head_size % 32 == 0)
 #pragma unroll 2
         for (int c = cg * (cpg >> 1); c < (cg + 1) * (cpg >> 1); ++c) {
           const float4 kw = lds_f4(ktile + static_cast<uint32_t>(c * T + tl) * 16u);
@@ -1358,7 +1396,7 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
       float sc = (a0 + a1) + (a2 + a3);
       sc += __shfl_xor_sync(kFull, sc, 8);
       sc += __shfl_xor_sync(kFull, sc, 16);
-      sc = valid ? sc * scale : -FLT_MAX;
+      sc = valid ? sc * tile_scale : -FLT_MAX;
       float mb = sc;
       mb = fmaxf(mb, __shfl_xor_sync(kFull, mb, 1));
       mb = fmaxf(mb, __shfl_xor_sync(kFull, mb, 2));
@@ -1379,7 +1417,7 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
       float acc[4] = {0.f, 0.f, 0.f, 0.f};
       // element (timestep, dim) of the V tile [T][hs] at byte (timestep * hs + dim) << esh: the 32 lanes read
       // 32 consecutive elements, conflict-free in either width
-      constexpr uint32_t esh = KV16 ? 1u : 2u;
+      constexpr uint32_t esh = KV8 ? 0u : KV16 ? 1u : 2u;
       const uint32_t vrow = vtile + (static_cast<uint32_t>(b * 8 * hs + lane) << esh);
       for (int k = 0; k < nv; ++k) {
         const float pk = __shfl_sync(kFull, pr, k);
@@ -1388,7 +1426,7 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
         for (int i = 0; i < 4; ++i)
           if (lane + 32 * i < hs) {
             const uint32_t a = va + ((32u * i) << esh);
-            acc[i] = __fmaf_rn(pk, KV16 ? lds_bf16(a) : lds_f32(a), acc[i]);
+            acc[i] = __fmaf_rn(pk, KV8 ? lds_e4m3(a) : KV16 ? lds_bf16(a) : lds_f32(a), acc[i]);
           }
       }
 #pragma unroll
@@ -1408,6 +1446,11 @@ __device__ KLLM_PHASE_CALL Pipe attention_flash_phase(const Params& P, int head,
   {
     float* mine = red + warp * (hs + 2);
     if (lane == 0) mine[0] = m, mine[1] = l;
+    if constexpr (KV8) {  // the cached rows' values times s_v
+      const float sv = P.kv_scale_v[ph.layer * (P.kv_dim / hs) + kvh];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) o[i] = __fmul_rn(o[i], sv);
+    }
 #pragma unroll
     for (int i = 0; i < 4; ++i)
       if (lane + 32 * i < hs) mine[2 + lane + 32 * i] = o[i];
@@ -1636,7 +1679,7 @@ __device__ __forceinline__ void record_fed(const Params& P, int pos, int token) 
 // Stages the phase's input vector (tagged residual exchange / tagged hand-off / embedding row) into
 // shared memory, RMS-normalises it when the phase asks for it, consumes this CTA's ring stages
 // task by task, runs the epilogues and, for the classifier, leaves the CTA's (max, index).
-template <int CW, bool INT8, bool PROF, bool LP, bool KV16, bool W16>
+template <int CW, bool INT8, bool PROF, bool LP, int KV, bool W16>
 __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int tok, int pos, const float* emb_row,
                                             unsigned long long* stamp) {
   constexpr int CT = CW * 32;
@@ -1798,11 +1841,13 @@ __device__ KLLM_PHASE_CALL Carry gemv_phase(const Params& P, Carry carry, int to
     if (sg.bias != nullptr) v = __fadd_rn(v, bias_v);       // matmul.cpp:74-77: out + bias
     if (sg.tag_out != nullptr) st_tagged_gpu(sg.tag_out + rr.row, v, hand_tag(ph.hand_out));
     if (sg.out == nullptr) {
-    } else if (sg.head_major) {  // value cache [kv_head][SP][seq_len][dv], bf16 elements with KV16
+    } else if (sg.head_major) {  // value cache [kv_head][SP][seq_len][dv], bf16 or fp8 elements with those caches
       const int hs = P.head_size, dv = hs / P.attn_vsplit;
       const int kvh = rr.row / hs, d = rr.row % hs;
       const size_t at = ((static_cast<size_t>(kvh) * P.attn_vsplit + d / dv) * P.seq_len + pos) * dv + d % dv;
-      if constexpr (KV16)
+      if constexpr (KV == KLLM_KV_FP8)
+        reinterpret_cast<uint8_t*>(sg.out)[at] = e4m3_encode(v, P.kv_inv_v[ph.layer * (P.kv_dim / hs) + kvh]);
+      else if constexpr (KV == KLLM_KV_BF16)
         reinterpret_cast<__nv_bfloat16*>(sg.out)[at] = __float2bfloat16_rn(v);
       else
         sg.out[at] = v;
@@ -2008,9 +2053,10 @@ __device__ __noinline__ int draw_with_logprobs(const Params& P, int pos, int ste
 // ---- the kernel ---------------------------------------------------------------------------------
 // LP: the logprob_megakernel instantiation, launched while log-probabilities are on.  decode_megakernel (LP false)
 // compiles to the code it has without the feature: the off path adds nothing to it, not even a test.
-// KV16: the bf16 KV cache (kv16_megakernel), fast numerics' flash form only; the same holds for it.
-// W16: bf16 weight rows (w16_megakernel), never with INT8; the same holds for it.
-template <int CW, bool INT8, bool PROF, bool LP, bool KV16, bool W16 = false>
+// KV: the KV cache's element, a kllm_decoder_desc::kv_cache value -- the bf16 cache (kv16_megakernel) and the fp8
+// one (kv8_megakernel) are fast numerics' flash form only; the same holds for them.
+// W16: bf16 weight rows (w16_megakernel, w16kv8_megakernel), never with INT8; the same holds for it.
+template <int CW, bool INT8, bool PROF, bool LP, int KV, bool W16 = false>
 __device__ __forceinline__ void megakernel_body(const Params& P) {
   constexpr int CT = CW * 32;  // consumer threads
   uint64_t* full_bar = g_full_bar;
@@ -2106,8 +2152,9 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
           const size_t head_block =
               (static_cast<size_t>(ph.layer) * (P.kv_dim / hs) + kvh) * P.seq_len * hs;
           if (ph.kind == kPhaseAttnFlash) {  // tiles j = split, split + SP, ...: K tile, then V tile
-            // K: hs * esz / 16 chunk columns of 16 bytes (4 fp32 or 8 bf16 dims) per timestep; V: rows of hs * esz
-            constexpr int esz = KV16 ? 2 : 4;
+            // K: hs * esz / 16 chunk columns of 16 bytes (4 fp32, 8 bf16 or 16 fp8 dims) per timestep; V: rows of
+            // hs * esz
+            constexpr int esz = KV == KLLM_KV_FP8 ? 1 : KV == KLLM_KV_BF16 ? 2 : 4;
             const int T = P.attn_tile, row_bytes = hs * esz;
             const unsigned char* kbase = reinterpret_cast<const unsigned char*>(P.key_cache) + head_block * esz;
             const unsigned char* vbase = reinterpret_cast<const unsigned char*>(P.value_cache) + head_block * esz;
@@ -2267,7 +2314,7 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
         const int SP = P.attn_split;
         if (cta < P.head_num * SP) {
           if (ph.kind == kPhaseAttnFlash)
-            pipe = attention_flash_phase<CW, KV16>(P, cta / SP, cta % SP, pos, pipe, hand_tag(ph.hand_in), hand_tag(ph.hand_out), stamp);
+            pipe = attention_flash_phase<CW, KV>(P, cta / SP, cta % SP, pos, pipe, hand_tag(ph.hand_in), hand_tag(ph.hand_out), stamp);
           else if (ph.kind == kPhaseAttnFused)
             pipe = attention_fused_phase<CW>(P, cta, pos, pipe, hand_tag(ph.hand_in), hand_tag(ph.hand_out), stamp);
           else if (ph.kind == kPhaseAttention)
@@ -2281,7 +2328,7 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
         // A prompt token (llama3.cpp:733-745: predict(..., is_prompt = true) discards the logits and
         // returns -1) skips the classifier -- its weights are not even streamed -- but keeps the grid
         // barrier that closes the token.
-        const Carry out = gemv_phase<CW, INT8, PROF, LP, KV16, W16>(P, Carry{pipe, best.v, best.i}, tok, pos, emb_row, stamp);
+        const Carry out = gemv_phase<CW, INT8, PROF, LP, KV, W16>(P, Carry{pipe, best.v, best.i}, tok, pos, emb_row, stamp);
         pipe = out.pipe;
         best.v = out.best_v, best.i = out.best_i;
       }
@@ -2343,25 +2390,37 @@ __device__ __forceinline__ void megakernel_body(const Params& P) {
 
 template <int CW, bool INT8, bool PROF>
 __global__ void __launch_bounds__(CW * 32 + 32, 1) decode_megakernel(const __grid_constant__ Params P) {
-  megakernel_body<CW, INT8, PROF, false, false>(P);
+  megakernel_body<CW, INT8, PROF, false, KLLM_KV_F32>(P);
 }
 
 template <int CW, bool INT8>
 __global__ void __launch_bounds__(CW * 32 + 32, 1) logprob_megakernel(const __grid_constant__ Params P) {
-  megakernel_body<CW, INT8, false, true, false>(P);
+  megakernel_body<CW, INT8, false, true, KLLM_KV_F32>(P);
 }
 
 // The bf16 KV cache's instantiations, with (LP) and without log-probabilities; no profiling one.
 template <int CW, bool INT8, bool LP>
 __global__ void __launch_bounds__(CW * 32 + 32, 1) kv16_megakernel(const __grid_constant__ Params P) {
-  megakernel_body<CW, INT8, false, LP, true>(P);
+  megakernel_body<CW, INT8, false, LP, KLLM_KV_BF16>(P);
+}
+
+// The fp8 KV cache's instantiations, with (LP) and without log-probabilities; no profiling one.
+template <int CW, bool INT8, bool LP>
+__global__ void __launch_bounds__(CW * 32 + 32, 1) kv8_megakernel(const __grid_constant__ Params P) {
+  megakernel_body<CW, INT8, false, LP, KLLM_KV_FP8>(P);
 }
 
 // bf16 weights (KLLM_WEIGHTS_BF16): with (LP) and without log-probabilities, over an fp32 or (KV16) a bf16 cache; no
 // profiling one.
 template <int CW, bool LP, bool KV16>
 __global__ void __launch_bounds__(CW * 32 + 32, 1) w16_megakernel(const __grid_constant__ Params P) {
-  megakernel_body<CW, false, false, LP, KV16, true>(P);
+  megakernel_body<CW, false, false, LP, KV16 ? KLLM_KV_BF16 : KLLM_KV_F32, true>(P);
+}
+
+// bf16 weights over the fp8 KV cache, with (LP) and without log-probabilities; no profiling one.
+template <int CW, bool LP>
+__global__ void __launch_bounds__(CW * 32 + 32, 1) w16kv8_megakernel(const __grid_constant__ Params P) {
+  megakernel_body<CW, false, false, LP, KLLM_KV_FP8, true>(P);
 }
 
 }  // namespace mega
@@ -2375,15 +2434,22 @@ template <typename K>
 const void* fn(K* kernel) {
   return reinterpret_cast<const void*>(kernel);
 }
-// The instantiations that run a model of weight format `f` over an fp32 or (kv16) a bf16 cache: the plain one, the
-// profiling one kllm_decoder_profile launches (its stamps cost registers in the row loops; none for a bf16 cache
-// or bf16 weights) and the log-probability one.
+// The instantiations that run a model of weight format `f` over a cache of element `kv` (a kllm_decoder_desc::kv_cache
+// value): the plain one, the profiling one kllm_decoder_profile launches (its stamps cost registers in the row loops;
+// none for a bf16 or fp8 cache or bf16 weights) and the log-probability one.
 struct Kernels {
   const void *plain, *prof, *lp;
 };
-Kernels kernels_for(WeightFormat f, bool kv16) {
+Kernels kernels_for(WeightFormat f, int kv) {
   using namespace mega;
   constexpr int CW = kConsumerWarps;
+  if (kv == KLLM_KV_FP8) {
+    if (f == WeightFormat::kBf16) return Kernels{fn(w16kv8_megakernel<CW, false>), nullptr, fn(w16kv8_megakernel<CW, true>)};
+    if (f == WeightFormat::kInt8)
+      return Kernels{fn(kv8_megakernel<CW, true, false>), nullptr, fn(kv8_megakernel<CW, true, true>)};
+    return Kernels{fn(kv8_megakernel<CW, false, false>), nullptr, fn(kv8_megakernel<CW, false, true>)};
+  }
+  const bool kv16 = kv == KLLM_KV_BF16;
   if (f == WeightFormat::kBf16)
     return kv16 ? Kernels{fn(w16_megakernel<CW, false, true>), nullptr, fn(w16_megakernel<CW, true, true>)}
                 : Kernels{fn(w16_megakernel<CW, false, false>), nullptr, fn(w16_megakernel<CW, true, false>)};
@@ -2446,12 +2512,15 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
   fast_ = m.numerics == 1 ? 1 : 0;
   if (const char* e = getenv("KLLM_MODE")) fast_ = std::string(e) == "fast" ? 1 : 0;
   int8_fast_ = (int8 && fast_) ? 1 : 0;
-  // bf16 KV cache: a toleranced variant of the flash attention only, over 16-byte chunks of 8 dims with a
-  // quarter of the head per lane (head_size % 32 == 0); refused rather than run in any other form
-  if (m.kv_cache != KLLM_KV_F32 && m.kv_cache != KLLM_KV_BF16) return KLLM_E_INVALID;
-  kv_bf16_ = m.kv_cache == KLLM_KV_BF16 ? 1 : 0;
-  if (kv_bf16_ && (!fast_ || m.tp_world > 1 || hs % 32 != 0)) return KLLM_E_UNSUPPORTED;
-  const Kernels ks = kernels_for(dm.format, kv_bf16_);
+  // bf16 and fp8 KV caches: toleranced variants of the flash attention only, over 16-byte chunks of 8 (bf16) or 16
+  // (fp8) dims with a quarter of the head per lane (head_size % 32 == 0, % 64 == 0); refused rather than run in any
+  // other form
+  if (m.kv_cache != KLLM_KV_F32 && m.kv_cache != KLLM_KV_BF16 && m.kv_cache != KLLM_KV_FP8) return KLLM_E_INVALID;
+  kv_elem_ = m.kv_cache;
+  const int kv_esz = prefill::kv_elem_bytes(kv_elem_);  // bytes per cached element
+  if (kv_elem_ != KLLM_KV_F32 && (!fast_ || m.tp_world > 1 || hs % (64 / kv_esz) != 0)) return KLLM_E_UNSUPPORTED;
+  if (kv_elem_ == KLLM_KV_FP8 && m.kv_scales == nullptr) return KLLM_E_INVALID;
+  const Kernels ks = kernels_for(dm.format, kv_elem_);
   kernel_ = ks.plain, kernel_prof_ = ks.prof, kernel_lp_ = ks.lp;
 
   // The residual exchange after o_proj and down_proj is tagged (under tensor parallelism it IS the
@@ -2476,12 +2545,11 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
   // against 627 with 32 KB (20 KB: 649, 24 KB: 645), Qwen2.5-0.5B 1058 against 1032.  At dim 4096 a 16 KB stage is
   // ONE row, a task no longer shares its x loads, and Llama-2-7B fell from 108 to 80 tok/s.  The flash tiles shrink
   // with the stage (head_size 64: 64 timesteps).
-  const bool small_stages = fast_ && !kv_bf16_ && !w16 && 2 * dim * 4 <= 16 * 1024;
+  const bool small_stages = fast_ && kv_elem_ == KLLM_KV_F32 && !w16 && 2 * dim * 4 <= 16 * 1024;
   int stage_bytes = int8 ? 27 * 1024 : w16 ? (fast_ ? kW16FastStageBytes : kW16StageBytes) : small_stages ? 16 * 1024
                                                                                                  : 32 * 1024;
   if (const char* e = getenv("KLLM_STAGE_BYTES")) stage_bytes = atoi(e);
   stage_bytes = (stage_bytes + 127) & ~127;
-  const int kv_esz = kv_bf16_ ? 2 : 4;  // bytes per cached element
   attn_tile_ = std::min(stage_bytes / (hs * kv_esz), mega::kConsumerWarps * 32) & ~31;  // one timestep per consumer thread
   if (attn_tile_ < 32) return KLLM_E_UNSUPPORTED;
   if (fast_) {  // flash attention: a lane quartet per timestep, warp partials (m, l, o[hs]) in the input buffer
@@ -2612,9 +2680,10 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
       p.norm_eps = dm.eps;
       p.seg[0] = seg(lw.q, nullptr, q_rows, 0, t_q);
       p.seg[1] = seg(lw.k, nullptr, kvd, 0, t_k);
-      float* vrows = kv_bf16_ ? reinterpret_cast<float*>(reinterpret_cast<__nv_bfloat16*>(m.value_cache) + layer_off)
-                              : m.value_cache + layer_off;  // kv16_megakernel's epilogue stores bf16 elements
+      // kv16_megakernel's and kv8_megakernel's epilogues store bf16 or fp8 elements
+      float* vrows = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(m.value_cache) + layer_off * kv_esz);
       p.seg[2] = seg(lw.v, vrows, kvd, 1, t_v);
+      p.layer = l;  // the fp8 cache's value epilogue reads its layer's scales
       p.units = q_rows + 2 * kvd;
       if (int rc = plan(p)) return rc;
       p.hand_out = hands;
@@ -2853,6 +2922,11 @@ Params MegaEngine::params(const DrawSettings& cfg, int n_tokens, const int32_t* 
   P.lp_cand_v = reinterpret_cast<float*>(P.lp_part + grid_);
   P.lp_cand_i = reinterpret_cast<int*>(P.lp_cand_v + static_cast<size_t>(grid_) * sampling::kMaxTopLogprobs);
   P.lp_rec = m.lp_rec;
+  if (kv_elem_ == KLLM_KV_FP8) {
+    const size_t n = static_cast<size_t>(dm.layer_num) * dm.kv_head_num;
+    P.kv_scale_k = m.kv_scales, P.kv_scale_v = m.kv_scales + n;
+    P.kv_inv_k = m.kv_scales + 2 * n, P.kv_inv_v = m.kv_scales + 3 * n;
+  }
   return P;
 }
 

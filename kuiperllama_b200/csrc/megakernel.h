@@ -116,6 +116,7 @@ struct Params {
   //   K [L][kv_head][head_size/4][seq_len][4]    V [L][kv_head][attn_split][seq_len][head_size/attn_split]
   // kv16_megakernel (KLLM_KV_BF16, flash form only): both caches hold bf16 elements behind these pointers,
   //   K [L][kv_head][head_size/8][seq_len][8]    V [L][kv_head][seq_len][head_size]
+  // kv8_megakernel (KLLM_KV_FP8, flash form only): e4m3 codes, K [L][kv_head][head_size/16][seq_len][16], V as bf16's
   float* key_cache;
   const float* value_cache;
   const float* sin_cache;
@@ -163,6 +164,11 @@ struct Params {
   float* lp_cand_v;
   int* lp_cand_i;
   sampling::LogprobRecord lp_rec;
+  // the fp8 KV cache's scales (kv8_megakernel; null otherwise), each [L][kv_head]: s_k, s_v and their fp32 inverses
+  const float* kv_scale_k;
+  const float* kv_scale_v;
+  const float* kv_inv_k;
+  const float* kv_inv_v;
 };
 
 }  // namespace mega
@@ -183,7 +189,8 @@ struct MegaModel {
   unsigned long long* tp_data[8];
   int tp_stride;
   int numerics;  // kllm_decoder_desc::numerics
-  int kv_cache;  // kllm_decoder_desc::kv_cache: KLLM_KV_BF16 needs the fast numerics (flash attention)
+  int kv_cache;  // kllm_decoder_desc::kv_cache: KLLM_KV_BF16 and KLLM_KV_FP8 need the fast numerics (flash attention)
+  const float* kv_scales;  // KLLM_KV_FP8: device [4][L][kv_head], s_k, s_v, 1 / s_k, 1 / s_v
 };
 
 class MegaEngine {
@@ -235,11 +242,11 @@ class MegaEngine {
   int int8_fast_ = 0;
   int fast_ = 0;  // numerics: 0 = bit-exact with the reference, 1 = toleranced (free summation order)
   int attn_vsplit_ = 1;
-  int kv_bf16_ = 0;  // bf16 KV cache
+  int kv_elem_ = KLLM_KV_F32;  // the KV cache's element, a kllm_decoder_desc::kv_cache value
   int cls_rows_ = 0, n_cls_phases_ = 1;
   // the instantiations of the weight format and KV cache (megakernel.cu, kernels_for)
   const void* kernel_ = nullptr;       // plain
-  const void* kernel_prof_ = nullptr;  // records the phase timeline stamps; none with a bf16 cache or bf16 weights
+  const void* kernel_prof_ = nullptr;  // records the phase timeline stamps; none with a bf16 or fp8 cache or bf16 weights
   const void* kernel_lp_ = nullptr;    // log-probabilities on
   size_t smem_bytes_ = 0;
   unsigned barrier_base_ = 0;

@@ -17,11 +17,13 @@
 
 #include <cfloat>
 #include <cstdint>
+#include <type_traits>
 
 #include "../../include/kllm_b200.h"
 #include "cache_layout.h"
 #include "kllm_device.cuh"
 #include "kllm_host.h"
+#include "kv_fp8.cuh"
 
 namespace kllm {
 namespace prefill {
@@ -86,19 +88,32 @@ __global__ void swiglu_rows_kernel(float* __restrict__ h1, const float* __restri
 }
 
 // A cache element of type E (float, or __nv_bfloat16 for the bf16 KV cache: rounded to nearest even on the way
-// in, widened exactly on the way out)
-__device__ __forceinline__ void put(float* p, float v) { *p = v; }
-__device__ __forceinline__ void put(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
-__device__ __forceinline__ float get(const float* p) { return *p; }
-__device__ __forceinline__ float get(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+// in, widened exactly on the way out; or __nv_fp8_e4m3 for the fp8 one: encoded at the inverse `inv` of its scale on
+// the way in, fp32(value(code) * s) on the way out).  The float and bf16 forms take no scale.
+__device__ __forceinline__ void put(float* p, float v, float) { *p = v; }
+__device__ __forceinline__ void put(__nv_bfloat16* p, float v, float) { *p = __float2bfloat16_rn(v); }
+__device__ __forceinline__ void put(__nv_fp8_e4m3* p, float v, float inv) { p->__x = e4m3_encode(v, inv); }
+__device__ __forceinline__ float get(const float* p, float) { return *p; }
+__device__ __forceinline__ float get(const __nv_bfloat16* p, float) { return __bfloat162float(*p); }
+__device__ __forceinline__ float get(const __nv_fp8_e4m3* p, float s) { return __fmul_rn(e4m3_value(p->__x), s); }
+template <typename E>
+constexpr bool kScaled = std::is_same_v<E, __nv_fp8_e4m3>;
+
+// The fp8 cache's scales of one layer, [kv_head] each (null for the other caches): the K and V scales, or their
+// inverses
+struct KvScales {
+  const float* k;
+  const float* v;
+};
 
 // RoPE (rope_kernel.cu) on the T query rows in place, and on the T key rows while they are scattered,
-// with the value rows, into the layer's cache (of element type E).  grid = T, one thread per rotation pair.
+// with the value rows, into the layer's cache (of element type E; fp8: at the inverses `inv` of the layer's scales).
+// grid = T, one thread per rotation pair.
 template <typename E>
 __global__ void rope_scatter_kernel(float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                                     const float* __restrict__ sin_t, const float* __restrict__ cos_t,
                                     E* __restrict__ kcache, E* __restrict__ vcache, CacheLayout c, int heads,
-                                    int kv_heads, int flavour, int start_pos) {
+                                    int kv_heads, int flavour, int start_pos, KvScales inv) {
   const int t = blockIdx.x, pos = start_pos + t, hs = c.head_size, half = hs >> 1;
   float* qrow = q + static_cast<size_t>(t) * heads * hs;
   const float* krow = k + static_cast<size_t>(t) * kv_heads * hs;
@@ -121,29 +136,32 @@ __global__ void rope_scatter_kernel(float* __restrict__ q, const float* __restri
     } else {
       const int kvh = h - heads;
       const float a = krow[kvh * hs + i0], b = krow[kvh * hs + i1];
-      put(kcache + k_index(c, pos, kvh, i0), __fmaf_rn(fcr, a, -__fmul_rn(fci, b)));
-      put(kcache + k_index(c, pos, kvh, i1), __fmaf_rn(fci, a, __fmul_rn(fcr, b)));
+      const float ik = kScaled<E> ? inv.k[kvh] : 1.f;
+      put(kcache + k_index(c, pos, kvh, i0), __fmaf_rn(fcr, a, -__fmul_rn(fci, b)), ik);
+      put(kcache + k_index(c, pos, kvh, i1), __fmaf_rn(fci, a, __fmul_rn(fcr, b)), ik);
     }
   }
   for (int p = threadIdx.x; p < kv_heads * hs; p += blockDim.x)
-    put(vcache + v_index(c, pos, p / hs, p % hs), vrow[p]);
+    put(vcache + v_index(c, pos, p / hs, p % hs), vrow[p], kScaled<E> ? inv.v[p / hs] : 1.f);
 }
 
 // Causal attention of query (t, head) over cache positions 0 .. start_pos + t (mha_kernel.cu:47-110
-// arithmetic, fp32, over cache elements of type E).  grid = (heads, T); scores in dynamic shared memory.
+// arithmetic, fp32, over cache elements of type E; fp8: at the layer's scales `sc`).  grid = (heads, T); scores in
+// dynamic shared memory.
 template <typename E>
 __global__ void attn_rows_kernel(const float* __restrict__ q, const E* __restrict__ kcache,
                                  const E* __restrict__ vcache, float* __restrict__ out, CacheLayout c, int heads,
-                                 int kv_mul, int start_pos) {
+                                 int kv_mul, int start_pos, KvScales scales) {
   extern __shared__ float sc[];
   __shared__ float scratch[32];
   const int head = blockIdx.x, t = blockIdx.y, pos = start_pos + t, hs = c.head_size, kvh = head / kv_mul;
+  const float s_k = kScaled<E> ? scales.k[kvh] : 1.f, s_v = kScaled<E> ? scales.v[kvh] : 1.f;
   const float* qh = q + (static_cast<size_t>(t) * heads + head) * hs;
   const float scale = 1.f / sqrtf(static_cast<float>(hs));
   float mx = -FLT_MAX;
   for (int j = threadIdx.x; j <= pos; j += blockDim.x) {
     float s = 0.f;
-    for (int i = 0; i < hs; ++i) s = __fmaf_rn(get(kcache + k_index(c, j, kvh, i)), qh[i], s);
+    for (int i = 0; i < hs; ++i) s = __fmaf_rn(get(kcache + k_index(c, j, kvh, i), s_k), qh[i], s);
     s *= scale;
     sc[j] = s;
     mx = fmaxf(mx, s);
@@ -159,7 +177,7 @@ __global__ void attn_rows_kernel(const float* __restrict__ q, const E* __restric
   __syncthreads();
   for (int i = threadIdx.x; i < hs; i += blockDim.x) {
     float acc = 0.f;
-    for (int j = 0; j <= pos; ++j) acc = __fmaf_rn(sc[j] / sum, get(vcache + v_index(c, j, kvh, i)), acc);
+    for (int j = 0; j <= pos; ++j) acc = __fmaf_rn(sc[j] / sum, get(vcache + v_index(c, j, kvh, i), s_v), acc);
     out[(static_cast<size_t>(t) * heads + head) * hs + i] = acc;
   }
 }
@@ -208,19 +226,25 @@ int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspac
     PF_TRY(gemm(ws.xn, lw.k, ws.k, dim, kvd));
     PF_TRY(gemm(ws.xn, lw.v, ws.v, dim, kvd));
     const size_t sc_bytes = static_cast<size_t>(start_pos + T) * sizeof(float);
-    if (cl.bf16) {
-      __nv_bfloat16* kc = reinterpret_cast<__nv_bfloat16*>(m.key_cache) + layer_off;
-      __nv_bfloat16* vc = reinterpret_cast<__nv_bfloat16*>(m.value_cache) + layer_off;
-      rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc, vc, cl, heads, kvh,
-                                            dm.flavour, start_pos);
+    // the layer's cache, of element type E
+    auto attend = [&](auto* kc, auto* vc, KvScales inv, KvScales sc) {
+      rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc + layer_off,
+                                            vc + layer_off, cl, heads, kvh, dm.flavour, start_pos, inv);
       PF_TRY(count());
-      attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, kc, vc, ws.att, cl, heads, dm.kv_mul, start_pos);
+      attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, kc + layer_off, vc + layer_off, ws.att, cl, heads,
+                                                             dm.kv_mul, start_pos, sc);
+      return 0;
+    };
+    if (cl.elem == KLLM_KV_FP8) {
+      const size_t n = static_cast<size_t>(dm.layer_num) * kvh, h0 = static_cast<size_t>(l) * kvh;
+      const float* ks = m.kv_scales;  // [4][L][kv_head]: s_k, s_v, 1 / s_k, 1 / s_v
+      PF_TRY(attend(reinterpret_cast<__nv_fp8_e4m3*>(m.key_cache), reinterpret_cast<__nv_fp8_e4m3*>(m.value_cache),
+                    KvScales{ks + 2 * n + h0, ks + 3 * n + h0}, KvScales{ks + h0, ks + n + h0}));
+    } else if (cl.elem == KLLM_KV_BF16) {
+      PF_TRY(attend(reinterpret_cast<__nv_bfloat16*>(m.key_cache), reinterpret_cast<__nv_bfloat16*>(m.value_cache),
+                    KvScales{}, KvScales{}));
     } else {
-      rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, m.key_cache + layer_off,
-                                            m.value_cache + layer_off, cl, heads, kvh, dm.flavour, start_pos);
-      PF_TRY(count());
-      attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, m.key_cache + layer_off, m.value_cache + layer_off,
-                                                             ws.att, cl, heads, dm.kv_mul, start_pos);
+      PF_TRY(attend(m.key_cache, m.value_cache, KvScales{}, KvScales{}));
     }
     PF_TRY(count());
     PF_TRY(gemm(ws.att, lw.o, ws.tmp, q_rows, dim));
@@ -242,7 +266,8 @@ int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspac
 int prefill_attention_smem_opt_in(size_t bytes) {
   if (bytes <= 48 * 1024) return 0;
   for (const void* k : {reinterpret_cast<const void*>(attn_rows_kernel<float>),
-                        reinterpret_cast<const void*>(attn_rows_kernel<__nv_bfloat16>)})
+                        reinterpret_cast<const void*>(attn_rows_kernel<__nv_bfloat16>),
+                        reinterpret_cast<const void*>(attn_rows_kernel<__nv_fp8_e4m3>)})
     if (int rc = smem_opt_in(k, bytes)) return rc;
   return 0;
 }

@@ -57,8 +57,12 @@ class ModelShape:
             extra += L * (d + 2 * kv) * 4
         return wbytes + extra
 
-    def kv_bytes_at(self, pos: int) -> int:
-        return 2 * self.layer_num * (pos + 1) * self.kv_dim * 4
+    def kv_bytes_at(self, pos: int, kv_cache: str = "fp32") -> int:
+        """Bytes of the K and V rows 0 .. pos: 4 per element, 2 with kv_cache="bf16", 1 with "fp8"."""
+        return 2 * self.layer_num * (pos + 1) * self.kv_dim * KV_ELEM_BYTES[kv_cache]
+
+
+KV_ELEM_BYTES = {"fp32": 4, "bf16": 2, "fp8": 1}  # per cached element, by Decoder(kv_cache=...)
 
 
 SHAPES = {
@@ -168,6 +172,28 @@ def widen_weights(weights16: dict) -> dict:
     return out
 
 
+FP8_MAX = 448.0  # the largest finite e4m3 value
+
+
+def fp8_kv_scales(k, v, kv_heads=None):
+    """Calibrated scales for Decoder(kv_cache="fp8", kv_scales=...): amax / 448 per (layer, KV head) of the (key,
+    value) arrays Decoder.kv_cache() returns from an fp32-cache run, so that the largest element of each maps to
+    the largest finite e4m3 value; 1 where the amax is 0.  k and v are [L, seq_len, kv_dim] with `kv_heads` heads
+    (or already [L, seq_len, kv_heads, head_size]).  Returns float32 numpy [2, L, kv_heads]: the K scales, then the
+    V scales."""
+    import numpy as np
+    out = []
+    for a in (k, v):
+        a = np.asarray(a, dtype=np.float32)
+        if a.ndim == 3:
+            if kv_heads is None or a.shape[2] % kv_heads:
+                raise ValueError(f"kv_heads={kv_heads!r} for arrays of shape {a.shape}")
+            a = a.reshape(a.shape[0], a.shape[1], kv_heads, a.shape[2] // kv_heads)
+        amax = np.abs(a).max(axis=(1, 3))
+        out.append(np.where(amax > 0, amax / np.float32(FP8_MAX), np.float32(1.0)).astype(np.float32))
+    return np.stack(out)
+
+
 def _ptr_array(tensors):
     arr = (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
     return arr
@@ -178,7 +204,7 @@ class Decoder:
 
     def __init__(self, shape: ModelShape, weights: dict, stream=None, tp_size=1, tp_rank=0,
                  allreduce=None, allreduce_ctx=None, full_dim=None, comm=None, numerics="exact",
-                 kv_cache="fp32", weight_format="fp32"):
+                 kv_cache="fp32", weight_format="fp32", kv_scales=None):
         self.lib = load_library()
         self.shape = shape
         self.weights = weights  # keep the tensors alive
@@ -214,9 +240,20 @@ class Decoder:
         d.tp_size, d.tp_rank = tp_size, tp_rank
         # "exact": bit-identical to the reference; "fast": toleranced (kllm_b200.h, kllm_decoder_desc::numerics)
         d.numerics = {"exact": 0, "fast": 1}[numerics]
-        # "fp32": the cache of every other mode; "bf16": rows rounded to bf16 as they are cached, fast numerics on
-        # the persistent engine only (kllm_b200.h, kllm_decoder_desc::kv_cache)
-        d.kv_cache = {"fp32": 0, "bf16": 1}[kv_cache]
+        # "fp32": the cache of every other mode; "bf16": rows rounded to bf16 as they are cached; "fp8": rows stored as
+        # e4m3 codes at a scale per (layer, KV head), kv_scales [2, L, kv_heads] (None: all 1; fp8_kv_scales
+        # calibrates them).  Both fast numerics on the persistent engine only (kllm_b200.h, kllm_decoder_desc::kv_cache)
+        d.kv_cache = {"fp32": 0, "bf16": 1, "fp8": 2}[kv_cache]
+        if kv_cache == "fp8" and kv_scales is None:
+            import numpy as np
+            kv_scales = np.ones((2, L, s.kv_head_num), np.float32)  # the C ABI takes unit scales as an array of ones
+        if kv_scales is not None:
+            import numpy as np
+            sc = np.ascontiguousarray(np.asarray(kv_scales, dtype=np.float32))
+            if sc.shape != (2, L, s.kv_head_num):
+                raise KllmError(f"kv_scales of shape {sc.shape}, not (2, {L}, {s.kv_head_num})")
+            self._kv_scales = sc  # read by kllm_decoder_create only
+            d.kv_scales = sc.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
         # "bf16": the matrices and wcls are bf16 tensors (bf16_weights), the arithmetic fp32 (kllm_decoder_desc::weights)
         d.weights = {"fp32": 0, "bf16": 1}[weight_format]
         want = "torch.bfloat16" if weight_format == "bf16" else None

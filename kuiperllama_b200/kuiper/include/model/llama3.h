@@ -95,6 +95,15 @@ class LLama2Model : public Model {
   void set_bf16_kv_cache(bool on);
   bool bf16_kv_cache() const { return bf16_kv_cache_; }
 
+  // fp8 e4m3 KV cache in the fused decoder (kllm_decoder_desc::kv_cache = KLLM_KV_FP8): call before init(); without a
+  // call init() takes it from KUIPER_KV_CACHE=fp8, with unit scales.  Off by default.  `scales` is empty (every scale
+  // 1) or the [2][layer_num][kv_head_num] array of kllm_decoder_desc::kv_scales: the K scales, then the V scales.  A
+  // quarter of the fp32 cache's memory and reads, toleranced: the fast numerics (KUIPER_NUMERICS=fast), one GPU and
+  // head_size % 64 == 0, and init() fails rather than run without them.  The rows the layer path (forward()) takes
+  // over from the decoder are the codes' values times their scales.
+  void set_fp8_kv_cache(bool on, std::vector<float> scales = {});
+  bool fp8_kv_cache() const { return fp8_kv_cache_; }
+
   // bf16 weights in the fused decoder (kllm_decoder_desc::weights = KLLM_WEIGHTS_BF16): call before init(); without
   // a call init() takes it from KUIPER_WEIGHTS=bf16|fp32 (fp32 by default).  The matrices wq wk wv wo w1 w2 w3 and the
   // classifier (a bf16 copy of the embedding when shared) are rounded to bf16, nearest even, while they are staged
@@ -205,6 +214,10 @@ class LLama2Model : public Model {
   bool batched_prefill_explicit_ = false;
   bool bf16_kv_cache_ = false;
   bool bf16_kv_cache_explicit_ = false;
+  bool fp8_kv_cache_ = false;
+  bool fp8_kv_cache_explicit_ = false;
+  std::vector<float> fp8_kv_scales_;
+  std::vector<float> fp8_unit_scales_;  // the ones passed for an empty fp8_kv_scales_
   bool bf16_weights_ = false;
   bool bf16_weights_explicit_ = false;
   // bf16 weights: the device copies of the matrices, in create_decoder's order (wq.. per layer, then wcls)

@@ -93,6 +93,12 @@ void LLama2Model::set_bf16_kv_cache(bool on) {
   bf16_kv_cache_explicit_ = true;
 }
 
+void LLama2Model::set_fp8_kv_cache(bool on, std::vector<float> scales) {
+  fp8_kv_cache_ = on;
+  fp8_kv_cache_explicit_ = true;
+  fp8_kv_scales_ = std::move(scales);
+}
+
 void LLama2Model::set_bf16_weights(bool on) {
   bf16_weights_ = on;
   bf16_weights_explicit_ = true;
@@ -171,6 +177,15 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
     const char* env = std::getenv("KUIPER_KV_CACHE");
     bf16_kv_cache_ = env != nullptr && std::string(env) == "bf16";
   }
+  if (!fp8_kv_cache_explicit_) {
+    const char* env = std::getenv("KUIPER_KV_CACHE");
+    fp8_kv_cache_ = env != nullptr && std::string(env) == "fp8";
+    fp8_kv_scales_.clear();
+  }
+  if (fp8_kv_cache_ && bf16_kv_cache_)
+    return error::InvalidArgument("KV cache: bf16 and fp8 are both on; choose one (set_bf16_kv_cache / set_fp8_kv_cache)");
+  if (!fp8_kv_cache_ && !fp8_kv_scales_.empty())
+    return error::InvalidArgument("KV cache: fp8 scales were given without the fp8 cache");
   if (!bf16_weights_explicit_) {
     const char* env = std::getenv("KUIPER_WEIGHTS");
     if (env != nullptr && std::string(env) != "bf16" && std::string(env) != "fp32")
@@ -599,13 +614,32 @@ base::Status LLama2Model::create_decoder() {
   }
   if (const char* mode = std::getenv("KUIPER_NUMERICS"); mode && std::string(mode) == "fast") d.numerics = KLLM_NUMERICS_FAST;
   if (bf16_kv_cache_) d.kv_cache = KLLM_KV_BF16;
+  if (fp8_kv_cache_) {
+    d.kv_cache = KLLM_KV_FP8;
+    const size_t want = 2 * static_cast<size_t>(d.layer_num) * d.kv_head_num;
+    if (fp8_kv_scales_.empty()) {
+      fp8_unit_scales_.assign(want, 1.f);  // the C ABI takes unit scales as an array of ones
+      d.kv_scales = fp8_unit_scales_.data();
+    } else {
+      if (fp8_kv_scales_.size() != want)
+        return base::error::InvalidArgument("KV cache: " + std::to_string(fp8_kv_scales_.size()) + " fp8 scales, not 2 x " +
+                                      std::to_string(d.layer_num) + " layers x " + std::to_string(d.kv_head_num) +
+                                      " KV heads");
+      d.kv_scales = fp8_kv_scales_.data();
+    }
+  }
   if (bf16_weights_) d.weights = KLLM_WEIGHTS_BF16;
   const int rc = kllm_decoder_create(&d, cuda_config_->stream, &decoder_);
   if (rc != 0)
     return base::error::InternalError(
         std::string("kllm_decoder_create failed: ") + kllm_error_string(rc) +
-        (bf16_kv_cache_ ? " (the bf16 KV cache needs KUIPER_NUMERICS=fast, one GPU and head_size % 32 == 0)" : ""));
+        (bf16_kv_cache_ ? " (the bf16 KV cache needs KUIPER_NUMERICS=fast, one GPU and head_size % 32 == 0)" : "") +
+        (fp8_kv_cache_ ? " (the fp8 KV cache needs KUIPER_NUMERICS=fast, one GPU, head_size % 64 == 0 and scales that "
+                         "are finite and > 0)" : ""));
   if (bf16_kv_cache_) LOG(INFO) << "KV cache: bf16 (rounded to nearest even as rows are cached)";
+  if (fp8_kv_cache_)
+    LOG(INFO) << "KV cache: fp8 e4m3 (" << (fp8_kv_scales_.empty() ? "unit scales" : "scales per layer and KV head")
+              << ")";
   if (bf16_weights_) LOG(INFO) << "weights: bf16 matrices (rounded to nearest even as they were uploaded)";
   if (base::Status st = sampler::apply_to_decoder(draw_, decoder_); !st) return st;
   LOG(INFO) << "fused decoder engine: " << kllm_decoder_engine(decoder_) << ", "

@@ -28,7 +28,8 @@
 // --score scores the given ids with LLama2Model::score() instead of decoding (n_steps is then unused): one line of
 // the n - 1 log-probabilities, then "perplexity <exp(-mean)>".  The layer path has neither: --layers with either is
 // refused.  --kv-cache bf16 calls LLama2Model::set_bf16_kv_cache(true) instead of leaving it to KUIPER_KV_CACHE (the
-// fused decoder's bf16 KV cache needs KUIPER_NUMERICS=fast); --kv-cache fp32 turns it off.  --weights bf16 / fp32 calls
+// fused decoder's bf16 KV cache needs KUIPER_NUMERICS=fast); --kv-cache fp8 calls set_fp8_kv_cache(true), unit scales
+// (the same numerics); --kv-cache fp32 turns both off.  --weights bf16 / fp32 calls
 // LLama2Model::set_bf16_weights instead of leaving it to KUIPER_WEIGHTS.  After init() the tool reports on stderr the
 // device memory init() took ("device bytes after init: N", from cudaMemGetInfo).
 #include <base/base.h>
@@ -116,8 +117,9 @@ int main(int argc, char** argv) {
     else if (!std::strcmp(argv[i], "--score")) score = true;
     else if (!std::strcmp(argv[i], "--kv-cache") && i + 1 < argc) {
       const std::string v = argv[++i];
-      if (v != "fp32" && v != "bf16") return 2;
+      if (v != "fp32" && v != "bf16" && v != "fp8") return 2;
       m->set_bf16_kv_cache(v == "bf16");
+      m->set_fp8_kv_cache(v == "fp8");
     }
     else if (!std::strcmp(argv[i], "--weights") && i + 1 < argc) {
       const std::string v = argv[++i];

@@ -207,7 +207,7 @@ def make_tp_decoder(shape: ModelShape, full_weights: dict, comm: Comm, stream=No
                     kv_cache="fp32", weight_format="fp32") -> Decoder:
     """Decoder for this rank's shard of `full_weights` (every rank passes the same full dict,
     e.g. synth_weights with the same seed; the shard is cut here and the rest can be freed).
-    A bf16 KV cache and bf16 weights run on one GPU only (kllm_decoder_desc::kv_cache, ::weights)."""
+    A bf16 or fp8 KV cache and bf16 weights run on one GPU only (kllm_decoder_desc::kv_cache, ::weights)."""
     tp, rank = comm.world, comm.rank
     if tp == 1:
         return Decoder(shape, full_weights, stream=stream, numerics=numerics, kv_cache=kv_cache,

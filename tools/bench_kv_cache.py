@@ -1,13 +1,15 @@
 #!/usr/bin/env python
-"""Decode speed of the fast mode with an fp32 and a bf16 KV cache (kllm_decoder_desc::kv_cache), by position.
+"""Decode speed of the fast mode with an fp32, a bf16 and an fp8 KV cache (kllm_decoder_desc::kv_cache), by position.
 
     python tools/bench_kv_cache.py --workloads llama2-7b-int8 qwen2.5-0.5b tinyllama-1.1b
+    python tools/bench_kv_cache.py --caches fp32 bf16 fp8
 
-Per workload, two fast-numerics decoders on one GPU over the same synthetic weights (bench.py's seed for the
-workload), one per cache type, each on its own stream.  Each cache is filled once by the batched prefill up to the last
+Per workload, fast-numerics decoders on one GPU over the same synthetic weights (bench.py's seed for the workload),
+one per cache type of --caches (fp32 and bf16 by default; the fp8 cache at unit scales: its speed does not depend on
+them), each on its own stream.  Each cache is filled once by the batched prefill up to the last
 window; a window at position p then runs --window consecutive decode steps from p (kllm_decoder_generate, one
 launch), which reads the cache rows < p only, so one fill serves every window.  A window is timed by device events
-on the decoder's stream; the two decoders alternate in the same call for --reps rounds after a warm-up, and the
+on the decoder's stream; the decoders alternate in the same call for --reps rounds after a warm-up, and the
 median is reported.
 
 Output: ONE JSON line with, per workload and window, tok/s for each cache type, the bytes one token must read
@@ -39,7 +41,7 @@ def progress(*parts):
 
 
 def kv_bytes(shape, pos, kv_cache):
-    return shape.kv_bytes_at(pos) // (2 if kv_cache == "bf16" else 1)
+    return shape.kv_bytes_at(pos, kv_cache)
 
 
 def main():
@@ -47,6 +49,7 @@ def main():
     ap.add_argument("--workloads", nargs="+", default=list(PLANS), choices=list(PLANS))
     ap.add_argument("--window", type=int, default=64, help="decode steps per timed window")
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--caches", nargs="+", default=["fp32", "bf16"], choices=["fp32", "bf16", "fp8"])
     a = ap.parse_args()
 
     import torch
@@ -64,7 +67,7 @@ def main():
         gen = torch.Generator().manual_seed(SEEDS[name])
         prompt = torch.randint(0, shape.vocab_size, (fill,), generator=gen).tolist()
         decs = {}
-        for kv in ("fp32", "bf16"):
+        for kv in a.caches:
             s = torch.cuda.Stream()
             d = Decoder(shape, w, stream=s.cuda_stream, numerics="fast", kv_cache=kv)
             (d.prefill_w8 if shape.group_size else d.prefill_tf32)(prompt)
@@ -95,10 +98,12 @@ def main():
                 b = shape.weight_bytes_per_token() + kv_bytes(shape, start + W // 2, kv)
                 row[kv] = {"tok_s": round(tok_s, 1), "bytes_per_token": b,
                            "fraction_of_3.35TBps": round(b * tok_s / HBM_BYTES_PER_S, 3)}
-            row["bf16_over_fp32"] = round(row["bf16"]["tok_s"] / row["fp32"]["tok_s"], 3)
+            for x, y in (("bf16", "fp32"), ("fp8", "fp32"), ("fp8", "bf16")):
+                if x in decs and y in decs:
+                    row[f"{x}_over_{y}"] = round(row[x]["tok_s"] / row[y]["tok_s"], 3)
             per[str(p)] = row
             progress(name, json.dumps(row))
-        results[name] = {"seq_len": seq_len, "engine": decs["bf16"][0].engine, "windows": per}
+        results[name] = {"seq_len": seq_len, "engine": next(iter(decs.values()))[0].engine, "windows": per}
         for d, _ in decs.values():
             d.close()
         del w, decs
