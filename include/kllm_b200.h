@@ -416,6 +416,57 @@ int kllm_decoder_generate_until(kllm_decoder* dec, int32_t first_token, int32_t 
                                 kllm_token_callback on_tokens, void* ctx,
                                 int32_t* out_tokens_host, int32_t* n_out);
 
+/* Speculative decoding's verify pass (DESIGN.md 5.13): tokens_host[0] is the id fed at start_pos, tokens_host[1 ..
+ * n_tokens) are drafts for the positions after it, and all n_tokens positions run through every layer in ONE pass
+ * over the weights.
+ *  - At each position start_pos + i the id id_i is drawn by the settings in force (greedy, sampling, top-p,
+ *    penalties, logit bias), over the history as fed, and recorded as any entry records it.
+ *  - a = the number of leading drafts with tokens_host[i] == id_{i-1}.  out_ids_host (capacity n_tokens) receives
+ *    id_0 .. id_a, and *n_accepted = a.
+ *  - The result is bit for bit that of kllm_decoder_generate(dec, tokens_host[0], start_pos, a + 1, NULL, ...) on a
+ *    decoder with the same description and state: the ids, kllm_decoder_logits (the logits of start_pos + a), the KV
+ *    rows of positions <= start_pos + a, the history and the log-probability record.  One exception: on the
+ *    persistent engine a record entry's log-probabilities may differ from that engine's own in the last bits
+ *    (DESIGN.md 5.13); its ids are the same.
+ *  - Past the frontier, at start_pos + a + 1 .. start_pos + n_tokens - 1, the history and the record hold what they
+ *    held before the call; the KV rows there are unspecified (at most n_tokens - 1 rows, none read by an entry that
+ *    does not feed its position first).  A call continues at start_pos + a + 1 with id_a as its input.
+ * Refusals, before any launch, leave the cache, the history, the record and the logits as they were:
+ * KLLM_E_UNSUPPORTED for the fast numerics (after KLLM_MODE; so also the bf16 and fp8 KV caches) and for
+ * tp_size > 1; KLLM_E_INVALID for n_tokens outside [1, KLLM_MAX_VERIFY_TOKENS], a token outside [0, vocab),
+ * start_pos < 0, start_pos + n_tokens > seq_len and NULL pointers.  fp32, int8 and bf16 weights, either engine.
+ * Each length's chain is captured as a CUDA graph on first use: one graph launch and one synchronisation per call. */
+#define KLLM_MAX_VERIFY_TOKENS 8
+int kllm_decoder_verify(kllm_decoder* dec, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
+                        int32_t* out_ids_host, int32_t* n_accepted);
+
+/* Speculative decoding with prompt-lookup drafts: kllm_decoder_generate_until's arguments and semantics, each round
+ * drafting from the decoder's history and checking the draft with kllm_decoder_verify.
+ * Drafting rule (kuiperllama_b200/speculative.py lookup_draft mirrors it): let p be the next position, t the id fed
+ * there, c = history[0 .. p) followed by t, L = p + 1.  For n = ngram_max down to 1, skip n when the suffix
+ * c[L-n .. L) has fewer than n ids or contains -1; else take the LARGEST s with s + n <= L - 1 and
+ * c[s .. s+n) == c[L-n .. L).  The draft is c[s+n ..], cut at the first -1 and after
+ * m = min(draft_len, max_steps - produced - 1, seq_len - p - 1) ids.  The first n with a non-empty draft wins; with
+ * none the round is one plain step on the decoder's engine.
+ *  - Each round streams its accepted ids to on_tokens.  A stop id ends the loop at its position; ids a round drew
+ *    past a stop are rejected as wrong drafts are, with the history and the record put back.
+ *  - The ids, *n_out, the callbacks' concatenation, kllm_decoder_logits, the history, the record and the KV rows
+ *    below start_pos + *n_out are bit for bit those of kllm_decoder_generate_until with the same arguments (the
+ *    record with kllm_decoder_verify's exception).  first_token must lie in [0, vocab).
+ *  - stats (optional): rounds (verify passes and plain steps), drafted (draft ids verified), accepted (draft ids
+ *    accepted); speculative.py simulate_rounds predicts them from the ids.
+ * KLLM_E_INVALID for draft_len outside [1, KLLM_MAX_VERIFY_TOKENS - 1] and ngram_max outside [1, 8], with
+ * kllm_decoder_generate_until's refusals and kllm_decoder_verify's KLLM_E_UNSUPPORTED cases, all before any launch. */
+typedef struct {
+  int32_t rounds;
+  int32_t drafted;
+  int32_t accepted;
+} kllm_spec_stats;
+int kllm_decoder_generate_speculative(kllm_decoder* dec, int32_t first_token, int32_t start_pos, int32_t max_steps,
+                                      const int32_t* stop_ids, int32_t n_stop, int32_t draft_len, int32_t ngram_max,
+                                      kllm_token_callback on_tokens, void* ctx, int32_t* out_tokens_host,
+                                      int32_t* n_out, kllm_spec_stats* stats);
+
 /* Sampling instead of the greedy id, from this call on, for every id the decoder returns: kllm_decoder_step
  * (non-prompt), _prompt, _prefill_tf32 / _w8 and _generate, including the ids generate feeds back on the
  * device.  Each id is the rule of kllm_sample_f32 applied to the logits of the position just processed,

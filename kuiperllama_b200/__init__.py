@@ -44,6 +44,12 @@ ALLREDUCE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_void_p, c_int, c_void_p)
 TOKEN_CALLBACK = ctypes.CFUNCTYPE(None, c_void_p, POINTER(c_int32), c_int32)
 MAX_STOP_IDS = 16  # KLLM_MAX_STOP_IDS
 MAX_TOP_LOGPROBS = 20  # KLLM_MAX_TOP_LOGPROBS
+MAX_VERIFY_TOKENS = 8  # KLLM_MAX_VERIFY_TOKENS: the positions one kllm_decoder_verify pass takes
+
+
+class SpecStats(ctypes.Structure):
+    """kllm_spec_stats: what kllm_decoder_generate_speculative's rounds did."""
+    _fields_ = [("rounds", c_int32), ("drafted", c_int32), ("accepted", c_int32)]
 
 
 class DecoderDesc(ctypes.Structure):
@@ -117,6 +123,11 @@ _SIGNATURES = {
                                       POINTER(c_int32)]),
     "kllm_decoder_generate_until": (c_int, [c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32), c_int32,
                                             TOKEN_CALLBACK, c_void_p, POINTER(c_int32), POINTER(c_int32)]),
+    "kllm_decoder_verify": (c_int, [c_void_p, POINTER(c_int32), c_int32, c_int32, POINTER(c_int32),
+                                    POINTER(c_int32)]),
+    "kllm_decoder_generate_speculative": (c_int, [c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32), c_int32,
+                                                  c_int32, c_int32, TOKEN_CALLBACK, c_void_p, POINTER(c_int32),
+                                                  POINTER(c_int32), POINTER(SpecStats)]),
     "kllm_decoder_set_sampling": (c_int, [c_void_p, c_float, c_int32, c_uint64]),
     "kllm_decoder_set_sampling_top_p": (c_int, [c_void_p, c_float, c_int32, c_float, c_uint64]),
     "kllm_decoder_set_repetition_penalty": (c_int, [c_void_p, c_float, c_int32]),

@@ -52,26 +52,36 @@ __device__ __forceinline__ float block256_max(float v, float* s_warp) {
   return m;  // every thread
 }
 
+// Query position pos_arg + blockIdx.y (kllm_decoder_verify: one row of q, scores and output per position) over a
+// cache in the graph engine's layout [seq][kv_dim], or with kTiled the persistent engine's exact-mode layout
+// (prefill::CacheLayout: K [kv_head][head_size / 4][seq][4], V [kv_head][vsplit][seq][head_size / vsplit]).
+// The layout moves addresses only; every operation is the same.
+template <bool kTiled>
 __global__ void __launch_bounds__(kMhaThreads)
 mha_decode_kernel(PosArg pos_arg, int seq_len, const float* __restrict__ query, float* score_ptr,
                   float* output, const float* __restrict__ key_cache,
                   const float* __restrict__ value_cache, int kv_dim, int kv_mul, int head_size,
-                  long long layer_offset) {
+                  long long layer_offset, int vsplit) {
   extern __shared__ __align__(16) float smem[];
   float* q_s = smem;                           // [head_size]
   float* v_s = smem + head_size;               // [2][kVTile][head_size]
   __shared__ float s_warp[kMhaThreads / 32];
   __shared__ float s_bcast;
 
-  const int head = blockIdx.x;
+  const int head = blockIdx.x + blockIdx.y * gridDim.x;  // the (position, head) row of q, scores and output
   const int tid = threadIdx.x;
-  const int pos = pos_arg.get();
+  const int pos = pos_arg.get() + blockIdx.y;
   const float scale = 1.f / sqrtf(static_cast<float>(head_size));
   const float* query_head = query + static_cast<size_t>(head) * head_size;
   float* score_head = score_ptr + static_cast<size_t>(head) * seq_len;
-  const int head_offset = (head / kv_mul) * head_size;
-  const float* kbase = key_cache + layer_offset + head_offset;
-  const float* vbase = value_cache + layer_offset + head_offset;
+  const int kvh = blockIdx.x / kv_mul;
+  // K row t: float4 chunk i at kbase + t * (4 or kv_dim) + 4 * i * k4_stride; V element (t, i) at vbase + (the tiled
+  // or the flat index)
+  const size_t kv_head_off = kTiled ? static_cast<size_t>(kvh) * head_size * seq_len : static_cast<size_t>(kvh) * head_size;
+  const float* kbase = key_cache + layer_offset + kv_head_off;
+  const float* vbase = value_cache + layer_offset + kv_head_off;
+  const int k4_stride = kTiled ? seq_len : 1;
+  const int dv = head_size / vsplit;
 
   for (int i = tid; i < head_size; i += kMhaThreads) q_s[i] = query_head[i];
   __syncthreads();
@@ -79,11 +89,11 @@ mha_decode_kernel(PosArg pos_arg, int seq_len, const float* __restrict__ query, 
   // ---- scores: mha_kernel.cu:61-91 --------------------------------------------------
   const float4* q4 = reinterpret_cast<const float4*>(q_s);
   for (int t = tid; t <= pos; t += kMhaThreads) {
-    const float4* k4 = reinterpret_cast<const float4*>(kbase + static_cast<size_t>(t) * kv_dim);
+    const float4* k4 = reinterpret_cast<const float4*>(kbase + static_cast<size_t>(t) * (kTiled ? 4 : kv_dim));
     float score = 0.0f;
 #pragma unroll 4
     for (int i = 0; i < (head_size >> 2); ++i) {
-      const float4 kv = k4[i];
+      const float4 kv = k4[static_cast<size_t>(i) * k4_stride];
       const float4 qv = q4[i];
       score = __fmaf_rn(kv.x, qv.x, score);
       score = __fmaf_rn(kv.y, qv.y, score);
@@ -124,7 +134,9 @@ mha_decode_kernel(PosArg pos_arg, int seq_len, const float* __restrict__ query, 
     for (int e = tid; e < kVTile * vec_per_row; e += kMhaThreads) {
       const int tt = e / vec_per_row, c = e % vec_per_row;
       if (t0 + tt <= pos)
-        dst[e] = *reinterpret_cast<const float4*>(vbase + static_cast<size_t>(t0 + tt) * kv_dim + 4 * c);
+        dst[e] = *reinterpret_cast<const float4*>(
+            vbase + (kTiled ? (static_cast<size_t>(4 * c / dv) * seq_len + t0 + tt) * dv + (4 * c) % dv
+                            : static_cast<size_t>(t0 + tt) * kv_dim + 4 * c));
     }
   };
   float value = 0.0f;
@@ -159,13 +171,42 @@ int launch_mha(PosArg pos, int head_num, int layer_index, int seq_len, int kv_di
   // head_size 188 is the largest whose q row and two value tiles fit the default 48 KB; larger
   // heads (up to 256: 66 KB) opt in, as launch_gemv does.  The tiling does not touch the arithmetic.
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(mha_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(mha_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(smem));
     if (e != cudaSuccess) return static_cast<int>(e);
   }
-  mha_decode_kernel<<<head_num, kMhaThreads, smem, stream>>>(pos, seq_len, query, score, mha_out,
-                                                            key_cache, value_cache, kv_dim,
-                                                            kv_mul, head_size, layer_offset);
+  mha_decode_kernel<false><<<head_num, kMhaThreads, smem, stream>>>(pos, seq_len, query, score, mha_out,
+                                                                   key_cache, value_cache, kv_dim,
+                                                                   kv_mul, head_size, layer_offset, 1);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, int head_num, int layer_index,
+                    int kv_mul, float* mha_out, const float* query, float* score, const float* key_cache,
+                    const float* value_cache, cudaStream_t stream) {
+  const int hs = c.head_size;
+  if (!mha_out || !query || !score || !key_cache || !value_cache || n_pos <= 0) return KLLM_E_INVALID;
+  if (c.elem != KLLM_KV_F32 || (hs & 3) != 0 || (c.kv_dim & 3) != 0 || hs > kMhaThreads) return KLLM_E_UNSUPPORTED;
+  if (c.mega && (hs % c.split != 0 || (hs / c.split) % 4 != 0)) return KLLM_E_UNSUPPORTED;
+  const long long layer_offset = static_cast<long long>(layer_index) * c.seq_len * c.kv_dim;
+  const size_t smem = sizeof(float) * (hs + 2 * kVTile * hs);
+  const dim3 grid(head_num, n_pos);
+  if (c.mega) {
+    if (smem > 48 * 1024) {
+      if (const int rc = smem_opt_in(reinterpret_cast<const void*>(mha_decode_kernel<true>), smem)) return rc;
+    }
+    mha_decode_kernel<true><<<grid, kMhaThreads, smem, stream>>>(first_pos, c.seq_len, query, score, mha_out,
+                                                                key_cache, value_cache, c.kv_dim, kv_mul, hs,
+                                                                layer_offset, c.split);
+  } else {
+    if (smem > 48 * 1024) {
+      if (const int rc = smem_opt_in(reinterpret_cast<const void*>(mha_decode_kernel<false>), smem)) return rc;
+    }
+    mha_decode_kernel<false><<<grid, kMhaThreads, smem, stream>>>(first_pos, c.seq_len, query, score, mha_out,
+                                                                 key_cache, value_cache, c.kv_dim, kv_mul, hs,
+                                                                 layer_offset, 1);
+  }
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }

@@ -20,6 +20,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <utility>
@@ -30,6 +31,7 @@
 #include "kllm_host.h"
 #include "megakernel.h"
 #include "sampling.cuh"
+#include "verify.h"
 
 namespace kllm {
 
@@ -214,6 +216,12 @@ struct kllm_decoder {
   // batched wgmma prefill (kllm_decoder_prefill_tf32 / _w8): activations of one block of prompt positions
   float* pf_buf = nullptr;
   PrefillWorkspace pf_ws{};
+  // kllm_decoder_verify (verify.cu): the per-position workspace, and the chain of each length captured on first use
+  void* vf_buf = nullptr;
+  VerifyWorkspace vf{};
+  VerifyIo* vf_io_host = nullptr;  // pinned
+  cudaGraphExec_t vf_exec[KLLM_MAX_VERIFY_TOKENS] = {};
+  int vf_launches[KLLM_MAX_VERIFY_TOKENS] = {};
 };
 
 namespace {
@@ -455,6 +463,117 @@ int run_prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, 
   return 0;
 }
 
+// What the verify pass has no counterpart of: the fast numerics' fixed-point rows and flash attention (and with them
+// the bf16 and fp8 caches), and tensor parallelism
+int verify_supported(const kllm_decoder* dc) {
+  if (dc->d.tp_size > 1 || dc->d.kv_cache != KLLM_KV_F32) return KLLM_E_UNSUPPORTED;
+  if (dc->use_mega && dc->mega.fast()) return KLLM_E_UNSUPPORTED;
+  return 0;
+}
+
+// The verify workspace (once per decoder) and the captured chain of n positions (once per length)
+int verify_prepare(kllm_decoder* dc, int n) {
+  const DecoderModel& m = dc->m;
+  constexpr int N = KLLM_MAX_VERIFY_TOKENS;
+  if (dc->vf_buf == nullptr) {
+    const size_t V = m.vocab_size, T = sampling::kMaxTopLogprobs;
+    const size_t floats = N * (2 * static_cast<size_t>(m.dim) + 2 * m.q_rows + 2 * m.kv_dim + m.hidden_dim + 2 * V +
+                               static_cast<size_t>(m.head_num) * m.seq_len);
+    const size_t words = N * (V + 2 + 2 * T);  // marks, saved history, saved record
+    const size_t bytes = (floats + words) * 4 + sizeof(VerifyIo);
+    // both or neither: a later call allocates again
+    if (cudaMalloc(&dc->vf_buf, bytes) != cudaSuccess) {
+      dc->vf_buf = nullptr;
+      return static_cast<int>(cudaErrorMemoryAllocation);
+    }
+    if (cudaMallocHost(&dc->vf_io_host, sizeof(VerifyIo)) != cudaSuccess) {
+      cudaFree(dc->vf_buf);
+      dc->vf_buf = nullptr, dc->vf_io_host = nullptr;
+      return static_cast<int>(cudaErrorMemoryAllocation);
+    }
+    KLLM_TRY(cudaMemsetAsync(dc->vf_buf, 0, bytes, dc->stream));  // the marks start at zero
+    float* f = static_cast<float*>(dc->vf_buf);
+    auto take = [&](size_t per) {
+      float* r = f;
+      f += per * N;
+      return r;
+    };
+    VerifyWorkspace& w = dc->vf;
+    w.x = take(m.dim), w.q = take(m.q_rows), w.k = take(m.kv_dim), w.v = take(m.kv_dim), w.att = take(m.q_rows);
+    w.h = take(m.hidden_dim), w.logits = take(V), w.penalized = take(V);
+    w.score = take(static_cast<size_t>(m.head_num) * m.seq_len);
+    w.marks = reinterpret_cast<int32_t*>(take(V));
+    w.saved_hist = reinterpret_cast<int32_t*>(take(1));
+    w.saved.id = reinterpret_cast<int32_t*>(take(1));
+    w.saved.lp = take(1);
+    w.saved.top_ids = reinterpret_cast<int32_t*>(take(T));
+    w.saved.top_lp = take(T);
+    w.io = reinterpret_cast<VerifyIo*>(f);
+  }
+  if (dc->vf_exec[n - 1] != nullptr) return 0;
+  const VerifyTarget t{cache_layout(dc), dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->d_cfg, dc->st, dc->hist,
+                       dc->rec, dc->logits};
+  const uint64_t before = launch_counter().load();
+  (void)cudaGetLastError();  // the chain checks its launches with cudaGetLastError: no earlier call's error is its own
+  KLLM_TRY(cudaStreamBeginCapture(dc->stream, cudaStreamCaptureModeRelaxed));
+  const int rc = enqueue_verify(dc->m, t, dc->vf, n, dc->stream);
+  cudaGraph_t g = nullptr;
+  const cudaError_t end = cudaStreamEndCapture(dc->stream, &g);
+  // capturing does not execute: undo the launch accounting of the capture pass
+  const uint64_t launches = launch_counter().load() - before;
+  launch_counter().fetch_sub(launches);
+  if (rc != 0 || end != cudaSuccess) {
+    if (g) cudaGraphDestroy(g);
+    return rc != 0 ? rc : static_cast<int>(end);
+  }
+  const cudaError_t inst = cudaGraphInstantiate(&dc->vf_exec[n - 1], g, 0);
+  cudaGraphDestroy(g);
+  KLLM_TRY(inst);
+  dc->vf_launches[n - 1] = static_cast<int>(launches);
+  return 0;
+}
+
+// One verify pass of tokens[0 .. n) at start_pos, acceptance ended at the first of the n_stop stop ids; the caller
+// checked the arguments.  out_ids receives id_0 .. id_a.
+int run_verify(kllm_decoder* dc, const int32_t* tokens, int n, int start_pos, const int32_t* stop_ids, int n_stop,
+               int32_t* out_ids, int32_t* accepted) {
+  KLLM_TRY(verify_prepare(dc, n));
+  VerifyIo& io = *dc->vf_io_host;
+  std::memcpy(io.tokens, tokens, sizeof(int32_t) * n);
+  io.start_pos = start_pos;
+  io.n_stop = n_stop;
+  if (n_stop > 0) std::memcpy(io.stop, stop_ids, sizeof(int32_t) * n_stop);
+  KLLM_TRY(cudaMemcpyAsync(dc->vf.io, &io, offsetof(VerifyIo, ids), cudaMemcpyHostToDevice, dc->stream));
+  KLLM_TRY(cudaGraphLaunch(dc->vf_exec[n - 1], dc->stream));
+  count_launch(static_cast<uint64_t>(dc->vf_launches[n - 1]));
+  KLLM_TRY(cudaMemcpyAsync(io.ids, dc->vf.io->ids, sizeof(int32_t) * (KLLM_MAX_VERIFY_TOKENS + 1),
+                           cudaMemcpyDeviceToHost, dc->stream));
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  *accepted = io.accepted;
+  std::memcpy(out_ids, io.ids, sizeof(int32_t) * (io.accepted + 1));
+  return 0;
+}
+
+// The prompt-lookup draft (kllm_b200.h, kllm_decoder_generate_speculative) of c[0 .. L) into draft, at most m ids
+int lookup_draft(const int32_t* c, int L, int ngram_max, int m, int32_t* draft) {
+  if (m <= 0) return 0;
+  for (int n = ngram_max; n >= 1; --n) {
+    if (L < n) continue;
+    const int32_t* suf = c + L - n;
+    bool hole = false;
+    for (int i = 0; i < n; ++i) hole |= suf[i] < 0;
+    if (hole) continue;
+    for (int s = L - 1 - n; s >= 0; --s) {
+      if (std::memcmp(c + s, suf, sizeof(int32_t) * n) != 0) continue;
+      int k = 0;
+      for (int j = s + n; j < L && k < m && c[j] >= 0; ++j) draft[k++] = c[j];
+      if (k > 0) return k;
+      break;  // the largest match gives the draft for this n, empty or not
+    }
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -615,6 +734,10 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->out_tokens) cudaFree(dc->out_tokens);
   if (dc->teacher) cudaFree(dc->teacher);
   if (dc->pf_buf) cudaFree(dc->pf_buf);
+  for (cudaGraphExec_t e : dc->vf_exec)
+    if (e) cudaGraphExecDestroy(e);
+  if (dc->vf_buf) cudaFree(dc->vf_buf);
+  if (dc->vf_io_host) cudaFreeHost(dc->vf_io_host);
   if (dc->st_host) cudaFreeHost(dc->st_host);
   if (dc->rec.id) cudaFree(dc->rec.id);
   if (dc->rec.lp) cudaFree(dc->rec.lp);
@@ -761,6 +884,71 @@ int kllm_decoder_generate_until(kllm_decoder* dc, int32_t first_token, int32_t s
   }
   std::memcpy(out_tokens_host, ids, sizeof(int32_t) * n);
   *n_out = n;
+  return 0;
+}
+
+int kllm_decoder_verify(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
+                        int32_t* out_ids_host, int32_t* n_accepted) {
+  // every refusal comes before the first launch, so a refused call leaves the decoder as it was
+  if (!dc || !tokens_host || !out_ids_host || !n_accepted) return KLLM_E_INVALID;
+  KLLM_TRY(verify_supported(dc));
+  if (n_tokens < 1 || n_tokens > KLLM_MAX_VERIFY_TOKENS || start_pos < 0) return KLLM_E_INVALID;
+  if (static_cast<int64_t>(start_pos) + n_tokens > dc->m.seq_len) return KLLM_E_INVALID;
+  for (int32_t i = 0; i < n_tokens; ++i)
+    if (tokens_host[i] < 0 || tokens_host[i] >= dc->m.vocab_size) return KLLM_E_INVALID;
+  return run_verify(dc, tokens_host, n_tokens, start_pos, nullptr, 0, out_ids_host, n_accepted);
+}
+
+int kllm_decoder_generate_speculative(kllm_decoder* dc, int32_t first_token, int32_t start_pos, int32_t max_steps,
+                                      const int32_t* stop_ids, int32_t n_stop, int32_t draft_len, int32_t ngram_max,
+                                      kllm_token_callback on_tokens, void* ctx, int32_t* out_tokens_host,
+                                      int32_t* n_out, kllm_spec_stats* stats) {
+  // every refusal comes before the first launch, so a refused call leaves the decoder as it was
+  if (!dc || !out_tokens_host || !n_out || max_steps <= 0 || start_pos < 0) return KLLM_E_INVALID;
+  if (static_cast<int64_t>(start_pos) + max_steps > dc->m.seq_len) return KLLM_E_INVALID;
+  if (n_stop < 0 || n_stop > KLLM_MAX_STOP_IDS || (n_stop > 0 && stop_ids == nullptr)) return KLLM_E_INVALID;
+  for (int i = 0; i < n_stop; ++i)
+    if (stop_ids[i] < 0 || stop_ids[i] >= dc->m.vocab_size) return KLLM_E_INVALID;
+  if (draft_len < 1 || draft_len >= KLLM_MAX_VERIFY_TOKENS || ngram_max < 1 || ngram_max > 8) return KLLM_E_INVALID;
+  if (first_token < 0 || first_token >= dc->m.vocab_size) return KLLM_E_INVALID;
+  KLLM_TRY(verify_supported(dc));
+  *n_out = 0;
+  if (stats) *stats = kllm_spec_stats{0, 0, 0};
+  // c: the history up to the next position, then the id fed there; the drafts are looked up in it
+  std::vector<int32_t> c(static_cast<size_t>(start_pos) + max_steps + 1);
+  if (start_pos > 0) {
+    KLLM_TRY(cudaMemcpyAsync(dc->io_host, dc->hist, sizeof(int32_t) * start_pos, cudaMemcpyDeviceToHost, dc->stream));
+    KLLM_TRY(cudaStreamSynchronize(dc->stream));
+    std::memcpy(c.data(), dc->io_host, sizeof(int32_t) * start_pos);
+  }
+  c[start_pos] = first_token;
+  int32_t produced = 0;
+  int32_t tokens[KLLM_MAX_VERIFY_TOKENS], ids[KLLM_MAX_VERIFY_TOKENS];
+  while (produced < max_steps) {
+    const int p = start_pos + produced;
+    const int m = std::min({draft_len, max_steps - produced - 1, dc->m.seq_len - p - 1});
+    const int k = lookup_draft(c.data(), p + 1, ngram_max, m, tokens + 1);
+    int32_t a = 0;
+    if (k == 0) {  // no draft: one plain step on the decoder's engine
+      KLLM_TRY(put_state(dc, c[p], p, 0, 0, 0, 0));
+      KLLM_TRY(run_positions(dc, 1));
+      KLLM_TRY(cudaMemcpyAsync(dc->st_host, dc->st, sizeof(mega::State), cudaMemcpyDeviceToHost, dc->stream));
+      KLLM_TRY(cudaStreamSynchronize(dc->stream));
+      ids[0] = dc->st_host->next;
+    } else {
+      tokens[0] = c[p];
+      KLLM_TRY(run_verify(dc, tokens, k + 1, p, stop_ids, n_stop, ids, &a));
+    }
+    if (stats) stats->rounds += 1, stats->drafted += k, stats->accepted += a;
+    if (on_tokens != nullptr) on_tokens(ctx, ids, a + 1);
+    std::memcpy(out_tokens_host + produced, ids, sizeof(int32_t) * (a + 1));
+    std::memcpy(c.data() + p + 1, ids, sizeof(int32_t) * (a + 1));
+    produced += a + 1;
+    bool stop = false;
+    for (int j = 0; j < n_stop; ++j) stop |= stop_ids[j] == ids[a];
+    if (stop) break;
+  }
+  *n_out = produced;
   return 0;
 }
 

@@ -37,13 +37,22 @@ struct GemvExtra {
   WeightFormat format = WeightFormat::kF32;
 };
 
-int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t stream);
+// The fused GEMV of `job` over nv <= 8 input vectors x[nv][in_dim] (nv > 1: kllm_decoder_verify's positions), each
+// with the single vector's arithmetic.  Vector v's rows land at seg.out + v * seg.rows (SwiGLU: + v * rows of the
+// pair) and its residual is residual + v * rows.
+int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t stream, int nv = 1);
 int launch_rope(int flavour, int dim, int kv_dim, int head_size, float* q, float* k_base,
                 long long k_pos_stride, PosArg pos, const float* sin_cache,
                 const float* cos_cache, cudaStream_t stream);
 int launch_mha(PosArg pos, int head_num, int layer_index, int seq_len, int kv_dim, int kv_mul,
                int head_size, float* mha_out, const float* query, float* score,
                const float* key_cache, const float* value_cache, cudaStream_t stream);
+
+// launch_mha for the n_pos query positions first_pos, first_pos + 1, .. (kllm_decoder_verify: q, output
+// [n_pos][head_num * head_size], scores [n_pos][head_num][seq_len]) over an fp32 cache in either engine's layout
+int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, int head_num, int layer_index,
+                    int kv_mul, float* mha_out, const float* query, float* score, const float* key_cache,
+                    const float* value_cache, cudaStream_t stream);
 
 // tp_comm.cu: exchange areas [2][world][stride] of 64-bit tagged words, one per rank (peer transport)
 int comm_tagged_areas(kllm_comm* comm, unsigned long long** areas8, int* world, int* rank, int* stride);
@@ -62,6 +71,11 @@ struct PrefillWorkspace {  // [block, .] activations
 int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspace& ws, const int32_t* tokens_dev, int T,
                   int start_pos, cudaStream_t stream);
 int prefill_attention_smem_opt_in(size_t bytes);
+// RoPE on T query rows [T][q_rows] in place and on T key rows [T][kv_dim], scattered with the value rows into layer
+// `layer` of an fp32 cache at positions start_pos .. start_pos + T - 1: launch_rope's arithmetic (prefill.cu)
+int launch_rope_scatter_f32(const DecoderModel& dm, const prefill::CacheLayout& c, int layer, float* q, const float* k,
+                            const float* v, const float* sin_cache, const float* cos_cache, float* key_cache,
+                            float* value_cache, PosArg start_pos, int T, cudaStream_t s);
 
 inline float flavour_eps(int flavour) { return flavour == KLLM_FLAVOUR_QWEN2 ? 1e-6f : 1e-5f; }
 }  // namespace kllm

@@ -214,6 +214,7 @@ class MegaEngine {
   int grid() const { return grid_; }
   int phases() const { return n_phases_; }
   int attn_vsplit() const { return attn_vsplit_; }  // slices of the V cache layout
+  int fast() const { return fast_; }                // numerics: 1 = toleranced (free summation order)
   int attn_tile() const { return attn_tile_; }      // timesteps per K (flash: K and V) ring stage
   int attn_split() const { return attn_split_; }    // CTAs per query head
   int attn_tile_v() const { return attn_tile_v_; }  // timesteps per V ring stage

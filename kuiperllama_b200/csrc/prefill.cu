@@ -113,8 +113,8 @@ template <typename E>
 __global__ void rope_scatter_kernel(float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                                     const float* __restrict__ sin_t, const float* __restrict__ cos_t,
                                     E* __restrict__ kcache, E* __restrict__ vcache, CacheLayout c, int heads,
-                                    int kv_heads, int flavour, int start_pos, KvScales inv) {
-  const int t = blockIdx.x, pos = start_pos + t, hs = c.head_size, half = hs >> 1;
+                                    int kv_heads, int flavour, PosArg start_pos, KvScales inv) {
+  const int t = blockIdx.x, pos = start_pos.get() + t, hs = c.head_size, half = hs >> 1;
   float* qrow = q + static_cast<size_t>(t) * heads * hs;
   const float* krow = k + static_cast<size_t>(t) * kv_heads * hs;
   const float* vrow = v + static_cast<size_t>(t) * kv_heads * hs;
@@ -229,7 +229,7 @@ int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspac
     // the layer's cache, of element type E
     auto attend = [&](auto* kc, auto* vc, KvScales inv, KvScales sc) {
       rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc + layer_off,
-                                            vc + layer_off, cl, heads, kvh, dm.flavour, start_pos, inv);
+                                            vc + layer_off, cl, heads, kvh, dm.flavour, PosArg{nullptr, start_pos}, inv);
       PF_TRY(count());
       attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, kc + layer_off, vc + layer_off, ws.att, cl, heads,
                                                              dm.kv_mul, start_pos, sc);
@@ -261,6 +261,17 @@ int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspac
     PF_TRY(count());
   }
   return 0;
+}
+
+int launch_rope_scatter_f32(const DecoderModel& dm, const CacheLayout& c, int layer, float* q, const float* k,
+                            const float* v, const float* sin_cache, const float* cos_cache, float* key_cache,
+                            float* value_cache, PosArg start_pos, int T, cudaStream_t s) {
+  if (c.elem != KLLM_KV_F32) return KLLM_E_UNSUPPORTED;
+  const size_t layer_off = static_cast<size_t>(layer) * dm.seq_len * dm.kv_dim;
+  rope_scatter_kernel<<<T, 256, 0, s>>>(q, k, v, sin_cache, cos_cache, key_cache + layer_off, value_cache + layer_off, c,
+                                        dm.head_num, dm.kv_head_num, dm.flavour, start_pos, KvScales{});
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
 }
 
 int prefill_attention_smem_opt_in(size_t bytes) {

@@ -11,6 +11,7 @@ import math
 from dataclasses import dataclass, replace
 
 from . import DecoderDesc, FLAVOURS, KllmError, check, load_library
+from .speculative import DEFAULT_DRAFT_LEN
 
 
 @dataclass(frozen=True)
@@ -381,6 +382,48 @@ class Decoder:
         if errors:
             raise errors[0]
         return list(out[:n_out.value])
+
+    def verify(self, tokens, start_pos: int):
+        """Speculative decoding's verify pass (kllm_decoder_verify): tokens[0] fed at start_pos, tokens[1:] drafts for
+        the positions after it, all in one pass over the weights.  Returns id_0 .. id_a, the ids drawn at
+        start_pos .. start_pos + a, where a is the number of leading drafts equal to the id drawn before them: bit for
+        bit generate(tokens[0], start_pos, a + 1)."""
+        toks = [int(t) for t in tokens]
+        arr = (ctypes.c_int32 * max(len(toks), 1))(*toks)
+        out = (ctypes.c_int32 * max(len(toks), 1))()
+        a = ctypes.c_int32(0)
+        check(self.lib.kllm_decoder_verify(self.handle, arr, len(toks), int(start_pos), out, ctypes.byref(a)),
+              "kllm_decoder_verify")
+        return list(out[:a.value + 1])
+
+    def generate_speculative(self, first_token: int, start_pos: int, max_steps: int, stop_ids=(), on_tokens=None,
+                             draft_len: int = DEFAULT_DRAFT_LEN, ngram_max: int = 3):
+        """generate_until with prompt-lookup drafts checked by verify passes (kllm_decoder_generate_speculative):
+        the same ids, logits, history, record and cache rows.  Returns (ids, stats) with stats a dict of rounds,
+        drafted and accepted (speculative.simulate_rounds predicts them)."""
+        from . import TOKEN_CALLBACK, SpecStats
+        stops = [int(t) for t in stop_ids]
+        sarr = (ctypes.c_int32 * max(len(stops), 1))(*stops)
+        out = (ctypes.c_int32 * max(int(max_steps), 1))()
+        n_out = ctypes.c_int32(0)
+        stats = SpecStats()
+        errors = []
+
+        def relay(_ctx, ids, n):
+            try:
+                on_tokens([ids[i] for i in range(n)])
+            except BaseException as e:  # an exception cannot cross the C frames: re-raised after the call
+                errors.append(e)
+
+        cb = TOKEN_CALLBACK(relay) if on_tokens is not None else TOKEN_CALLBACK()
+        check(self.lib.kllm_decoder_generate_speculative(self.handle, int(first_token), int(start_pos), int(max_steps),
+                                                         sarr, len(stops), int(draft_len), int(ngram_max), cb, None,
+                                                         out, ctypes.byref(n_out), ctypes.byref(stats)),
+              "kllm_decoder_generate_speculative")
+        if errors:
+            raise errors[0]
+        return list(out[:n_out.value]), {"rounds": stats.rounds, "drafted": stats.drafted,
+                                         "accepted": stats.accepted}
 
     def set_sampling(self, temperature: float, top_k: int = 0, seed: int = 0, top_p: float = 1.0):
         """Draw every later id by the sampling rule (kllm_decoder_set_sampling; sampling.py mirrors it)

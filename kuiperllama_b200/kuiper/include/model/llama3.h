@@ -114,6 +114,15 @@ class LLama2Model : public Model {
   void set_bf16_weights(bool on);
   bool bf16_weights() const { return bf16_weights_; }
 
+  // Speculative decoding in generate()'s step 3 (kllm_decoder_generate_speculative, DESIGN.md 5.13): prompt-lookup
+  // drafts of up to draft_len ids (1..7) from the n-grams of up to ngram_max ids (1..8) of the sequence, each checked
+  // by one verify pass over the weights.  The ids are generate()'s without it.  Call before init(); without a call
+  // init() takes draft_len from KUIPER_SPECULATIVE=<draft_len> (0, the default, is off; ngram_max 3).  It needs the
+  // exact numerics on one GPU: init() fails under KUIPER_NUMERICS=fast or tensor parallelism, or for a value outside
+  // those ranges.
+  void set_speculative(int32_t draft_len, int32_t ngram_max = 3);
+  int32_t speculative() const { return spec_draft_len_; }
+
   // Seeded sampling instead of the greedy id (DESIGN.md "Sampling"): call before init(); without a call
   // init() takes it from KUIPER_TEMPERATURE, KUIPER_TOP_K and KUIPER_SEED, so the reference's unchanged
   // demos can sample.  Unset or temperature 0 is greedy.  predict() on the fused decoder and forward() +
@@ -145,7 +154,8 @@ class LLama2Model : public Model {
   //   1. the prompt from position 0 (the batched prefill for all but its last token when batched_prefill() is
   //      on, else kllm_decoder_prompt -- also under tensor parallelism);
   //   2. the id after the prompt; if it is a stop id, that one id is the result;
-  //   3. kllm_decoder_generate_until for the rest, which stops on the device at the first stop id.
+  //   3. kllm_decoder_generate_until for the rest, which stops on the device at the first stop id (with
+  //      set_speculative: kllm_decoder_generate_speculative, the same ids).
   // `ids` receives at most max_new_tokens ids (fewer where the context ends), counting the stop id.  on_tokens,
   // if set, receives every id exactly once, in order, while the loop runs.  The stop set is the tokenizer's
   // generation-ending ids (what is_sentence_ending() accepts) plus set_stop_ids().  Afterwards predict() at
@@ -220,6 +230,9 @@ class LLama2Model : public Model {
   std::vector<float> fp8_unit_scales_;  // the ones passed for an empty fp8_kv_scales_
   bool bf16_weights_ = false;
   bool bf16_weights_explicit_ = false;
+  int32_t spec_draft_len_ = 0;  // 0: generate() runs kllm_decoder_generate_until
+  int32_t spec_ngram_max_ = 3;
+  bool spec_explicit_ = false;
   // bf16 weights: the device copies of the matrices, in create_decoder's order (wq.. per layer, then wcls)
   std::vector<std::shared_ptr<base::Buffer>> bf16_matrices_;
   base::Status upload_bf16_matrices();

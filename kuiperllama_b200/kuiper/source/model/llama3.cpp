@@ -99,6 +99,12 @@ void LLama2Model::set_fp8_kv_cache(bool on, std::vector<float> scales) {
   fp8_kv_scales_ = std::move(scales);
 }
 
+void LLama2Model::set_speculative(int32_t draft_len, int32_t ngram_max) {
+  spec_draft_len_ = draft_len;
+  spec_ngram_max_ = ngram_max;
+  spec_explicit_ = true;
+}
+
 void LLama2Model::set_bf16_weights(bool on) {
   bf16_weights_ = on;
   bf16_weights_explicit_ = true;
@@ -198,6 +204,29 @@ base::Status LLama2Model::init(base::DeviceType device_type) {
   if (bf16_weights_ && tp_.on())
     return error::InvalidArgument(
         "bf16 weights (KUIPER_WEIGHTS / set_bf16_weights) run on one GPU: turn them off under tensor parallelism");
+  if (!spec_explicit_) {
+    const char* env = std::getenv("KUIPER_SPECULATIVE");
+    char* end = nullptr;
+    spec_draft_len_ = env != nullptr ? static_cast<int32_t>(std::strtol(env, &end, 10)) : 0;
+    if (env != nullptr && (*env == '\0' || *end != '\0'))
+      return error::InvalidArgument("KUIPER_SPECULATIVE must be a draft length in [0, " +
+                                    std::to_string(KLLM_MAX_VERIFY_TOKENS - 1) + "], not '" + std::string(env) + "'");
+    spec_ngram_max_ = 3;
+  }
+  if (spec_draft_len_ < 0 || spec_draft_len_ >= KLLM_MAX_VERIFY_TOKENS || spec_ngram_max_ < 1 || spec_ngram_max_ > 8)
+    return error::InvalidArgument("speculative decoding (KUIPER_SPECULATIVE / set_speculative): draft_len must lie in [0, " +
+                                  std::to_string(KLLM_MAX_VERIFY_TOKENS - 1) + "] and ngram_max in [1, 8]");
+  if (spec_draft_len_ > 0) {
+    const char* mode = std::getenv("KUIPER_NUMERICS");
+    if (mode != nullptr && std::string(mode) == "fast")
+      return error::InvalidArgument(
+          "speculative decoding (KUIPER_SPECULATIVE / set_speculative) needs the exact numerics: unset "
+          "KUIPER_NUMERICS=fast or turn it off");
+    if (tp_.on())
+      return error::InvalidArgument(
+          "speculative decoding (KUIPER_SPECULATIVE / set_speculative) runs on one GPU: turn it off under tensor "
+          "parallelism");
+  }
   sampler::fill_from_env(draw_, draw_set_);
   if (Status st = sampler::validate(draw_); !st) return st;
   if (cudaSetDevice(tp_.cuda_device()) != cudaSuccess)
@@ -831,11 +860,18 @@ base::Status LLama2Model::generate(const std::vector<int32_t>& prompt, int32_t m
   auto relay = [](void* ctx, const int32_t* t, int32_t k) {
     (*static_cast<const std::function<void(const int32_t*, int32_t)>*>(ctx))(t, k);
   };
-  rc = kllm_decoder_generate_until(decoder_, first, n, rest, stops.data(), static_cast<int32_t>(stops.size()),
-                                   on_tokens ? +relay : nullptr,
-                                   const_cast<std::function<void(const int32_t*, int32_t)>*>(&on_tokens), more.data(),
-                                   &n_out);
-  if (rc != 0) return base::error::InternalError(std::string("kllm_decoder_generate_until: ") + kllm_error_string(rc));
+  void* ctx = const_cast<std::function<void(const int32_t*, int32_t)>*>(&on_tokens);
+  if (spec_draft_len_ > 0) {
+    what = "kllm_decoder_generate_speculative";
+    rc = kllm_decoder_generate_speculative(decoder_, first, n, rest, stops.data(), static_cast<int32_t>(stops.size()),
+                                           spec_draft_len_, spec_ngram_max_, on_tokens ? +relay : nullptr, ctx,
+                                           more.data(), &n_out, nullptr);
+  } else {
+    what = "kllm_decoder_generate_until";
+    rc = kllm_decoder_generate_until(decoder_, first, n, rest, stops.data(), static_cast<int32_t>(stops.size()),
+                                     on_tokens ? +relay : nullptr, ctx, more.data(), &n_out);
+  }
+  if (rc != 0) return base::error::InternalError(std::string(what) + ": " + kllm_error_string(rc));
   ids.insert(ids.end(), more.begin(), more.begin() + n_out);
   decoder_rows_ = n + n_out;  // == prompt.size() + ids.size() - 1: predict() continues at that position
   return base::error::Success();

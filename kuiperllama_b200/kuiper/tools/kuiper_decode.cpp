@@ -30,7 +30,9 @@
 // refused.  --kv-cache bf16 calls LLama2Model::set_bf16_kv_cache(true) instead of leaving it to KUIPER_KV_CACHE (the
 // fused decoder's bf16 KV cache needs KUIPER_NUMERICS=fast); --kv-cache fp8 calls set_fp8_kv_cache(true), unit scales
 // (the same numerics); --kv-cache fp32 turns both off.  --weights bf16 / fp32 calls
-// LLama2Model::set_bf16_weights instead of leaving it to KUIPER_WEIGHTS.  After init() the tool reports on stderr the
+// LLama2Model::set_bf16_weights instead of leaving it to KUIPER_WEIGHTS.  --speculative K calls
+// LLama2Model::set_speculative(K) (0 off) instead of leaving it to KUIPER_SPECULATIVE: --generate then drafts by prompt
+// lookup and verifies up to K drafts per pass, with the same ids.  After init() the tool reports on stderr the
 // device memory init() took ("device bytes after init: N", from cudaMemGetInfo).
 #include <base/base.h>
 #include <cuda_runtime_api.h>
@@ -55,7 +57,7 @@ int main(int argc, char** argv) {
     std::fprintf(stderr, "usage: %s <checkpoint> <llama|qwen> <fp32|int8> <n_steps> <id0> [id1 ...] "
                          "[--layers] [--copy-at K] [--logits out.f32] [--sampling T K SEED] [--top-p P] "
                          "[--repetition-penalty P N] [--frequency-presence F P [FROM]] [--logit-bias ID:B,...] "
-                         "[--generate N [--stop ID]... [--then K]] [--kv-cache fp32|bf16] [--weights fp32|bf16]\n", argv[0]);
+                         "[--generate N [--stop ID]... [--then K]] [--kv-cache fp32|bf16] [--weights fp32|bf16] [--speculative K]\n", argv[0]);
     return 2;
   }
   const std::string checkpoint = argv[1], family = argv[2], prec = argv[3];
@@ -126,6 +128,7 @@ int main(int argc, char** argv) {
       if (v != "fp32" && v != "bf16") return 2;
       m->set_bf16_weights(v == "bf16");
     }
+    else if (!std::strcmp(argv[i], "--speculative") && i + 1 < argc) m->set_speculative(std::atoi(argv[++i]));
     else if (!std::strcmp(argv[i], "--logits") && i + 1 < argc) logits_path = argv[++i];
     else prompt.push_back(std::atoi(argv[i]));
   }
