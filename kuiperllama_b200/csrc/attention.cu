@@ -52,7 +52,7 @@ __device__ __forceinline__ float block256_max(float v, float* s_warp) {
   return m;  // every thread
 }
 
-// Query position pos_arg + blockIdx.y (kllm_decoder_verify: one row of q, scores and output per position) over a
+// Query position pos_arg + blockIdx.y (one row of q, scores and output per position) over a
 // cache in the graph engine's layout [seq][kv_dim], or with kTiled the persistent engine's exact-mode layout
 // (prefill::CacheLayout: K [kv_head][head_size / 4][seq][4], V [kv_head][vsplit][seq][head_size / vsplit]).
 // The layout moves addresses only; every operation is the same.
@@ -158,30 +158,6 @@ mha_decode_kernel(PosArg pos_arg, int seq_len, const float* __restrict__ query, 
   if (tid < head_size) output[static_cast<size_t>(head) * head_size + tid] = value;
 }
 
-int launch_mha(PosArg pos, int head_num, int layer_index, int seq_len, int kv_dim, int kv_mul,
-               int head_size, float* mha_out, const float* query, float* score,
-               const float* key_cache, const float* value_cache, cudaStream_t stream) {
-  if (!mha_out || !query || !score || !key_cache || !value_cache) return KLLM_E_INVALID;
-  if (head_num <= 0 || kv_mul <= 0 || head_size <= 0 || layer_index < 0 || seq_len <= 0)
-    return KLLM_E_INVALID;
-  if ((head_size & 3) != 0 || (kv_dim & 3) != 0 || head_size > kMhaThreads)
-    return KLLM_E_UNSUPPORTED;
-  const long long layer_offset = static_cast<long long>(layer_index) * seq_len * kv_dim;
-  const size_t smem = sizeof(float) * (head_size + 2 * kVTile * head_size);
-  // head_size 188 is the largest whose q row and two value tiles fit the default 48 KB; larger
-  // heads (up to 256: 66 KB) opt in, as launch_gemv does.  The tiling does not touch the arithmetic.
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(mha_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(smem));
-    if (e != cudaSuccess) return static_cast<int>(e);
-  }
-  mha_decode_kernel<false><<<head_num, kMhaThreads, smem, stream>>>(pos, seq_len, query, score, mha_out,
-                                                                   key_cache, value_cache, kv_dim,
-                                                                   kv_mul, head_size, layer_offset, 1);
-  count_launch();
-  return static_cast<int>(cudaGetLastError());
-}
-
 int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, int head_num, int layer_index,
                     int kv_mul, float* mha_out, const float* query, float* score, const float* key_cache,
                     const float* value_cache, cudaStream_t stream) {
@@ -190,6 +166,8 @@ int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, 
   if (c.elem != KLLM_KV_F32 || (hs & 3) != 0 || (c.kv_dim & 3) != 0 || hs > kMhaThreads) return KLLM_E_UNSUPPORTED;
   if (c.mega && (hs % c.split != 0 || (hs / c.split) % 4 != 0)) return KLLM_E_UNSUPPORTED;
   const long long layer_offset = static_cast<long long>(layer_index) * c.seq_len * c.kv_dim;
+  // head_size 188 is the largest whose q row and two value tiles fit the default 48 KB; larger
+  // heads (up to 256: 66 KB) opt in.  The tiling does not touch the arithmetic.
   const size_t smem = sizeof(float) * (hs + 2 * kVTile * hs);
   const dim3 grid(head_num, n_pos);
   if (c.mega) {
@@ -217,8 +195,9 @@ extern "C" int kllm_mha_decode_f32(int pos, int head_num, int layer_index, int s
                                    int kv_mul, int head_size, float* mha_out, const float* query,
                                    float* score, const float* key_cache, const float* value_cache,
                                    void* stream) {
-  if (pos < 0 || pos >= seq_len) return KLLM_E_INVALID;
-  return kllm::launch_mha(kllm::PosArg{nullptr, pos}, head_num, layer_index, seq_len, kv_dim,
-                          kv_mul, head_size, mha_out, query, score, key_cache, value_cache,
-                          static_cast<cudaStream_t>(stream));
+  if (pos < 0 || pos >= seq_len || head_num <= 0 || kv_mul <= 0 || head_size <= 0 || layer_index < 0)
+    return KLLM_E_INVALID;
+  const kllm::prefill::CacheLayout flat{0, seq_len, kv_dim, head_size, 1, KLLM_KV_F32};
+  return kllm::launch_mha_rows(kllm::PosArg{nullptr, pos}, 1, flat, head_num, layer_index, kv_mul, mha_out, query,
+                               score, key_cache, value_cache, static_cast<cudaStream_t>(stream));
 }

@@ -119,14 +119,11 @@ __global__ void sincos_kernel(int head_size, int seq_len, float* sin_cache, floa
 
 // rope_kernel.cu:97-122 (interleaved) as compiled:
 //   x' = fma(fcr, x, -(fci*y));  y' = fma(fci, x, fcr*y)
-__global__ void rope_interleaved_kernel(PosArg pos_arg, long long k_pos_stride, int dim,
-                                        int kv_dim, int head_size, float* q, float* k,
+__global__ void rope_interleaved_kernel(int pos, int dim, int kv_dim, int head_size, float* q, float* k,
                                         const float* __restrict__ sin_cache,
                                         const float* __restrict__ cos_cache) {
   const int idx = (blockIdx.x * blockDim.x + threadIdx.x) * 2;
   if (idx >= dim) return;
-  const int pos = pos_arg.get();
-  k += pos * k_pos_stride;
   const int head_dim = idx % head_size;
   const float fci = sin_cache[pos * head_size + head_dim];
   const float fcr = cos_cache[pos * head_size + head_dim];
@@ -150,13 +147,10 @@ __global__ void rope_interleaved_kernel(PosArg pos_arg, long long k_pos_stride, 
 //   v0' = fma(fcr, v0, -(fci*v1));  v1' = fma(fci, v0, fcr*v1)
 // One thread per pair; the reference's `idx > total_pairs` lets thread total_pairs run past
 // the end of q -- here the bound is exact.
-__global__ void rope_halfsplit_kernel(PosArg pos_arg, long long k_pos_stride, int dim, int kv_dim,
-                                      int head_size, float* q, float* k,
+__global__ void rope_halfsplit_kernel(int pos, int dim, int kv_dim, int head_size, float* q, float* k,
                                       const float* __restrict__ sin_cache,
                                       const float* __restrict__ cos_cache) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  const int pos = pos_arg.get();
-  k += pos * k_pos_stride;
   const int half = head_size / 2;
   const int total_pairs = (dim / head_size) * half;
   if (idx >= total_pairs) return;
@@ -253,30 +247,10 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const float* __restrict__ 
   if (threadIdx.x == 0) *out = best.i < 0 ? 0 : best.i;
 }
 
-int launch_rope(int flavour, int dim, int kv_dim, int head_size, float* q, float* k_base,
-                long long k_pos_stride, PosArg pos, const float* sin_cache,
-                const float* cos_cache, cudaStream_t s) {
-  if (!q || !k_base || !sin_cache || !cos_cache || dim <= 0 || kv_dim <= 0 || head_size <= 0 ||
-      (head_size & 1) || dim % head_size != 0)
-    return KLLM_E_INVALID;
-  const int pairs = dim / 2;
-  if (flavour == KLLM_FLAVOUR_LLAMA2) {
-    rope_interleaved_kernel<<<(pairs + 127) / 128, 128, 0, s>>>(
-        pos, k_pos_stride, dim, kv_dim, head_size, q, k_base, sin_cache, cos_cache);
-  } else if (flavour == KLLM_FLAVOUR_LLAMA3 || flavour == KLLM_FLAVOUR_QWEN2) {
-    rope_halfsplit_kernel<<<(pairs + 127) / 128, 128, 0, s>>>(
-        pos, k_pos_stride, dim, kv_dim, head_size, q, k_base, sin_cache, cos_cache);
-  } else {
-    return KLLM_E_INVALID;
-  }
-  count_launch();
-  return static_cast<int>(cudaGetLastError());
-}
-
 // kllm_sample_f32: one block draws the id by the rule of sampling.cuh
 __global__ void __launch_bounds__(1024) sample_kernel(const float* __restrict__ logits, int n, SampleParams sp, int pos,
                                                       long long* out_index) {
-  constexpr int kScratch = sampling::kDrawScratchBase + 2048 * 8;
+  constexpr int kScratch = sampling::kDrawScratchBytes;
   __shared__ __align__(16) unsigned char scratch[kScratch];
   const int i = sampling::draw_block<1024>(logits, n, sp, pos, nullptr, nullptr, 0, scratch, kScratch,
                                            [] { __syncthreads(); });
@@ -392,9 +366,22 @@ int kllm_sincos_init(int head_size, int seq_len, int flavour, float* sin_cache, 
 
 int kllm_rope_f32(int flavour, int dim, int kv_dim, int head_size, float* q, float* k, int pos,
                   const float* sin_cache, const float* cos_cache, void* stream) {
-  if (pos < 0) return KLLM_E_INVALID;
-  return launch_rope(flavour, dim, kv_dim, head_size, q, k, 0, PosArg{nullptr, pos}, sin_cache,
-                     cos_cache, static_cast<cudaStream_t>(stream));
+  if (!q || !k || !sin_cache || !cos_cache || pos < 0 || dim <= 0 || kv_dim <= 0 || head_size <= 0 ||
+      (head_size & 1) || dim % head_size != 0)
+    return KLLM_E_INVALID;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int pairs = dim / 2;
+  if (flavour == KLLM_FLAVOUR_LLAMA2) {
+    rope_interleaved_kernel<<<(pairs + 127) / 128, 128, 0, s>>>(pos, dim, kv_dim, head_size, q, k, sin_cache,
+                                                                cos_cache);
+  } else if (flavour == KLLM_FLAVOUR_LLAMA3 || flavour == KLLM_FLAVOUR_QWEN2) {
+    rope_halfsplit_kernel<<<(pairs + 127) / 128, 128, 0, s>>>(pos, dim, kv_dim, head_size, q, k, sin_cache,
+                                                              cos_cache);
+  } else {
+    return KLLM_E_INVALID;
+  }
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
 }
 
 int kllm_embedding_f32(const int32_t* tokens, int n_tokens, const float* table, float* out,

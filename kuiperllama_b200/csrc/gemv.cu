@@ -28,7 +28,6 @@ struct SegDev {
   const float* scales;
   const float* bias;
   float* out;
-  long long pos_stride;  // out += pos * pos_stride (KV-cache row of the current position)
   int rows;
 };
 
@@ -44,7 +43,6 @@ struct GemvParams {
   int vec_ok;       // fp32 / bf16: every weight row is 16- / 8-byte aligned (in_dim % 4 == 0, aligned bases)
   int n_seg;
   int units;  // output rows (or w1/w3 row pairs when swiglu)
-  PosArg pos;
   SegDev seg[3];
 };
 
@@ -129,7 +127,6 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
   const int pack_num = M >> 2;
   const int P4 = Mp >> 2;  // per-vector stride in packs
   const float4* xs4 = reinterpret_cast<const float4*>(xs);
-  const long long pos = p.pos.get();
   constexpr int kRowsPerUnit = kSwiglu ? 2 : 1;
   constexpr int kUnits = R / kRowsPerUnit;
   const int warps_total = gridDim.x * kGemvWarps;
@@ -353,8 +350,7 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
             if (p.seg[seg].bias != nullptr) val = __fadd_rn(val, p.seg[seg].bias[row]);
             // llama3.cpp:683-684,719: add_kernel(x, matmul_out) -> x + matmul_out
             if (p.residual != nullptr) val = __fadd_rn(p.residual[row + v * p.units], val);
-            float* out = p.seg[seg].out + (NV == 1 ? 0 : v * p.seg[seg].rows);
-            out[pos * p.seg[seg].pos_stride + row] = val;
+            p.seg[seg].out[(NV == 1 ? 0 : v * p.seg[seg].rows) + row] = val;
           }
         }
       }
@@ -421,12 +417,12 @@ static int launch_gemv_multi(const GemvParams& p, int nv, cudaStream_t stream) {
   return static_cast<int>(cudaGetLastError());
 }
 
-int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t stream, int nv) {
+int gemv_dispatch(const kllm_gemv_job* job, WeightFormat format, cudaStream_t stream, int nv) {
   if (job == nullptr || job->x == nullptr || job->in_dim <= 0 || nv < 1 || nv > kMaxVecs) return KLLM_E_INVALID;
   if (job->n_seg < 1 || job->n_seg > 3) return KLLM_E_INVALID;
   if (nv > 1 && job->residual != nullptr && job->n_seg != 1) return KLLM_E_INVALID;  // residual rows are the units
-  const bool int8 = extra.format == WeightFormat::kInt8;
-  const bool bf16 = extra.format == WeightFormat::kBf16;
+  const bool int8 = format == WeightFormat::kInt8;
+  const bool bf16 = format == WeightFormat::kBf16;
   if (job->swiglu_pair && (job->n_seg != 2 || job->seg[0].rows != job->seg[1].rows ||
                            job->residual != nullptr))
     return KLLM_E_INVALID;
@@ -445,7 +441,6 @@ int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t
   p.group_size = job->group_size;
   p.group_shift = int8 ? group_shift_of(job->group_size) : -1;
   p.n_seg = job->n_seg;
-  p.pos = extra.pos;
   p.vec_ok = (job->in_dim & 3) == 0;
   int total = 0;
   for (int s = 0; s < job->n_seg; ++s) {
@@ -457,7 +452,7 @@ int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t
       if (int8) return KLLM_E_UNSUPPORTED;
       p.vec_ok = 0;
     }
-    p.seg[s] = SegDev{g.w, g.scales, g.bias, g.out, extra.pos_stride[s], g.rows};
+    p.seg[s] = SegDev{g.w, g.scales, g.bias, g.out, g.rows};
     total += g.rows;
   }
   p.units = job->swiglu_pair ? job->seg[0].rows : total;
@@ -521,9 +516,9 @@ int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t
 extern "C" {
 
 int kllm_gemv_fused(const kllm_gemv_job* job, void* stream) {
-  kllm::GemvExtra ex;
-  if (job != nullptr && job->group_size > 0) ex.format = kllm::WeightFormat::kInt8;
-  return kllm::gemv_dispatch(job, ex, static_cast<cudaStream_t>(stream));
+  const bool int8 = job != nullptr && job->group_size > 0;
+  return kllm::gemv_dispatch(job, int8 ? kllm::WeightFormat::kInt8 : kllm::WeightFormat::kF32,
+                             static_cast<cudaStream_t>(stream));
 }
 
 int kllm_gemv_f32(const float* x, const float* w, float* out, int in_dim, int out_dim,
@@ -548,9 +543,7 @@ int kllm_gemv_bf16(const float* x, const uint16_t* w, float* out, int in_dim, in
   job.seg[0].w = w;
   job.seg[0].out = out;
   job.seg[0].rows = out_dim;
-  kllm::GemvExtra ex;
-  ex.format = kllm::WeightFormat::kBf16;
-  return kllm::gemv_dispatch(&job, ex, static_cast<cudaStream_t>(stream));
+  return kllm::gemv_dispatch(&job, kllm::WeightFormat::kBf16, static_cast<cudaStream_t>(stream));
 }
 
 int kllm_gemv_w8(const float* x, const int8_t* w, const float* scales, float* out, int in_dim,

@@ -22,33 +22,27 @@ inline void count_launch(uint64_t n = 1) { launch_counter().fetch_add(n, std::me
 int smem_opt_in(const void* kernel, size_t bytes);
 
 // A position that is either a host value or read from device memory at kernel run time; the
-// decoder's CUDA graph uses the device form so ONE captured graph serves every position.
+// decoder's CUDA graphs use the device form so ONE captured graph serves every position.
 struct PosArg {
   const int* ptr;
   int val;
   __host__ __device__ int get() const { return ptr != nullptr ? *ptr : val; }
 };
 
-// Output rows of segment s land at seg[s].out + pos * pos_stride[s] (KV-cache rows).  `format` is the segments'
-// weights': kInt8 with the job's group_size > 0, kF32 or kBf16 with group_size 0.
-struct GemvExtra {
-  PosArg pos{nullptr, 0};
-  long long pos_stride[3] = {0, 0, 0};
-  WeightFormat format = WeightFormat::kF32;
-};
+// Returns the first nonzero status of a call (a KLLM_E_* code or a cudaError_t)
+#define KLLM_TRY(expr)                      \
+  do {                                      \
+    const int rc_ = static_cast<int>(expr); \
+    if (rc_ != 0) return rc_;               \
+  } while (0)
 
 // The fused GEMV of `job` over nv <= 8 input vectors x[nv][in_dim] (nv > 1: kllm_decoder_verify's positions), each
-// with the single vector's arithmetic.  Vector v's rows land at seg.out + v * seg.rows (SwiGLU: + v * rows of the
-// pair) and its residual is residual + v * rows.
-int gemv_dispatch(const kllm_gemv_job* job, const GemvExtra& extra, cudaStream_t stream, int nv = 1);
-int launch_rope(int flavour, int dim, int kv_dim, int head_size, float* q, float* k_base,
-                long long k_pos_stride, PosArg pos, const float* sin_cache,
-                const float* cos_cache, cudaStream_t stream);
-int launch_mha(PosArg pos, int head_num, int layer_index, int seq_len, int kv_dim, int kv_mul,
-               int head_size, float* mha_out, const float* query, float* score,
-               const float* key_cache, const float* value_cache, cudaStream_t stream);
+// with the single vector's arithmetic, of weights in `format`: kInt8 with the job's group_size > 0, kF32 or kBf16
+// with group_size 0.  Vector v's rows land at seg.out + v * seg.rows (SwiGLU: + v * rows of the pair) and its
+// residual is residual + v * rows.
+int gemv_dispatch(const kllm_gemv_job* job, WeightFormat format, cudaStream_t stream, int nv = 1);
 
-// launch_mha for the n_pos query positions first_pos, first_pos + 1, .. (kllm_decoder_verify: q, output
+// mha_decode_kernel for the n_pos query positions first_pos, first_pos + 1, .. (q, output
 // [n_pos][head_num * head_size], scores [n_pos][head_num][seq_len]) over an fp32 cache in either engine's layout
 int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, int head_num, int layer_index,
                     int kv_mul, float* mha_out, const float* query, float* score, const float* key_cache,
@@ -57,9 +51,9 @@ int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, 
 // tp_comm.cu: exchange areas [2][world][stride] of 64-bit tagged words, one per rank (peer transport)
 int comm_tagged_areas(kllm_comm* comm, unsigned long long** areas8, int* world, int* rank, int* stride);
 
-// prefill.cu: one block of T prompt positions of the model through every layer with batched wgmma GEMMs, into
-// the caches in the layout of the engine that continues decoding
-struct PrefillModel {
+// The decoder's KV cache, in the layout of its engine, and its RoPE tables: what the batched prefill (prefill.cu) and
+// the decode chain (verify.cu) write and read
+struct DecoderCache {
   prefill::CacheLayout cache;
   float* key_cache; float* value_cache;  // cache.elem: bf16 or fp8 elements behind these pointers
   const float* sin_cache; const float* cos_cache;
@@ -68,14 +62,15 @@ struct PrefillModel {
 struct PrefillWorkspace {  // [block, .] activations
   float *x, *xn, *q, *k, *v, *att, *h1, *h3, *tmp;
 };
-int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspace& ws, const int32_t* tokens_dev, int T,
+// prefill.cu: one block of T prompt positions of the model through every layer with batched wgmma GEMMs, into
+// the caches in the layout of the engine that continues decoding
+int prefill_block(const DecoderModel& dm, const DecoderCache& m, PrefillWorkspace& ws, const int32_t* tokens_dev, int T,
                   int start_pos, cudaStream_t stream);
 int prefill_attention_smem_opt_in(size_t bytes);
 // RoPE on T query rows [T][q_rows] in place and on T key rows [T][kv_dim], scattered with the value rows into layer
-// `layer` of an fp32 cache at positions start_pos .. start_pos + T - 1: launch_rope's arithmetic (prefill.cu)
-int launch_rope_scatter_f32(const DecoderModel& dm, const prefill::CacheLayout& c, int layer, float* q, const float* k,
-                            const float* v, const float* sin_cache, const float* cos_cache, float* key_cache,
-                            float* value_cache, PosArg start_pos, int T, cudaStream_t s);
+// `layer` of an fp32 cache at positions start_pos .. start_pos + T - 1: kllm_rope_f32's arithmetic (prefill.cu)
+int launch_rope_scatter_f32(const DecoderModel& dm, const DecoderCache& c, int layer, float* q, const float* k,
+                            const float* v, PosArg start_pos, int T, cudaStream_t s);
 
 inline float flavour_eps(int flavour) { return flavour == KLLM_FLAVOUR_QWEN2 ? 1e-6f : 1e-5f; }
 }  // namespace kllm

@@ -108,17 +108,18 @@ struct KvScales {
 
 // RoPE (rope_kernel.cu) on the T query rows in place, and on the T key rows while they are scattered,
 // with the value rows, into the layer's cache (of element type E; fp8: at the inverses `inv` of the layer's scales).
-// grid = T, one thread per rotation pair.
+// grid = (T, rope_blocks): one thread per rotation pair and per value element.
 template <typename E>
 __global__ void rope_scatter_kernel(float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                                     const float* __restrict__ sin_t, const float* __restrict__ cos_t,
                                     E* __restrict__ kcache, E* __restrict__ vcache, CacheLayout c, int heads,
                                     int kv_heads, int flavour, PosArg start_pos, KvScales inv) {
   const int t = blockIdx.x, pos = start_pos.get() + t, hs = c.head_size, half = hs >> 1;
+  const int p0 = blockIdx.y * blockDim.x + threadIdx.x, stride = gridDim.y * blockDim.x;
   float* qrow = q + static_cast<size_t>(t) * heads * hs;
   const float* krow = k + static_cast<size_t>(t) * kv_heads * hs;
   const float* vrow = v + static_cast<size_t>(t) * kv_heads * hs;
-  for (int p = threadIdx.x; p < (heads + kv_heads) * half; p += blockDim.x) {
+  for (int p = p0; p < (heads + kv_heads) * half; p += stride) {
     const int h = p / half, j = p % half;
     int i0, i1;
     if (flavour == KLLM_FLAVOUR_LLAMA2) {
@@ -141,8 +142,13 @@ __global__ void rope_scatter_kernel(float* __restrict__ q, const float* __restri
       put(kcache + k_index(c, pos, kvh, i1), __fmaf_rn(fci, a, __fmul_rn(fcr, b)), ik);
     }
   }
-  for (int p = threadIdx.x; p < kv_heads * hs; p += blockDim.x)
+  for (int p = p0; p < kv_heads * hs; p += stride)
     put(vcache + v_index(c, pos, p / hs, p % hs), vrow[p], kScaled<E> ? inv.v[p / hs] : 1.f);
+}
+
+// rope_scatter_kernel's grid of 256-thread blocks for T positions: the rotation pairs of one position over blocks
+inline dim3 rope_grid(int T, int heads, int kv_heads, int head_size) {
+  return dim3(T, ((heads + kv_heads) * (head_size >> 1) + 255) / 256);
 }
 
 // Causal attention of query (t, head) over cache positions 0 .. start_pos + t (mha_kernel.cu:47-110
@@ -186,13 +192,7 @@ __global__ void attn_rows_kernel(const float* __restrict__ q, const E* __restric
 
 using namespace prefill;
 
-#define PF_TRY(expr)                       \
-  do {                                     \
-    const int rc_ = static_cast<int>(expr); \
-    if (rc_ != 0) return rc_;              \
-  } while (0)
-
-int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspace& ws, const int32_t* tokens_dev, int T,
+int prefill_block(const DecoderModel& dm, const DecoderCache& m, PrefillWorkspace& ws, const int32_t* tokens_dev, int T,
                   int start_pos, cudaStream_t s) {
   const int dim = dm.dim, hid = dm.hidden_dim, heads = dm.head_num, kvh = dm.kv_head_num;
   const int q_rows = dm.q_rows, kvd = dm.kv_dim;
@@ -215,22 +215,23 @@ int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspac
   };
   const int ew_grid = 528;  // 4 x 132 SMs for the grid-stride elementwise kernels
   embed_rows_kernel<<<T, 256, 0, s>>>(tokens_dev, dm.tok_emb, ws.x, dim, dm.vocab_size);
-  PF_TRY(count());
+  KLLM_TRY(count());
   const CacheLayout& cl = m.cache;
   for (int l = 0; l < dm.layer_num; ++l) {
     const LayerWeights& lw = dm.layers[l];
     const size_t layer_off = static_cast<size_t>(l) * dm.seq_len * kvd;
     rmsnorm_rows_kernel<<<T, 256, 0, s>>>(ws.x, lw.attn_norm, ws.xn, dim, dm.eps);
-    PF_TRY(count());
-    PF_TRY(gemm(ws.xn, lw.q, ws.q, dim, q_rows));
-    PF_TRY(gemm(ws.xn, lw.k, ws.k, dim, kvd));
-    PF_TRY(gemm(ws.xn, lw.v, ws.v, dim, kvd));
+    KLLM_TRY(count());
+    KLLM_TRY(gemm(ws.xn, lw.q, ws.q, dim, q_rows));
+    KLLM_TRY(gemm(ws.xn, lw.k, ws.k, dim, kvd));
+    KLLM_TRY(gemm(ws.xn, lw.v, ws.v, dim, kvd));
     const size_t sc_bytes = static_cast<size_t>(start_pos + T) * sizeof(float);
     // the layer's cache, of element type E
     auto attend = [&](auto* kc, auto* vc, KvScales inv, KvScales sc) {
-      rope_scatter_kernel<<<T, 256, 0, s>>>(ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc + layer_off,
-                                            vc + layer_off, cl, heads, kvh, dm.flavour, PosArg{nullptr, start_pos}, inv);
-      PF_TRY(count());
+      rope_scatter_kernel<<<rope_grid(T, heads, kvh, dm.head_size), 256, 0, s>>>(
+          ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc + layer_off, vc + layer_off, cl, heads, kvh, dm.flavour,
+          PosArg{nullptr, start_pos}, inv);
+      KLLM_TRY(count());
       attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, kc + layer_off, vc + layer_off, ws.att, cl, heads,
                                                              dm.kv_mul, start_pos, sc);
       return 0;
@@ -238,38 +239,38 @@ int prefill_block(const DecoderModel& dm, const PrefillModel& m, PrefillWorkspac
     if (cl.elem == KLLM_KV_FP8) {
       const size_t n = static_cast<size_t>(dm.layer_num) * kvh, h0 = static_cast<size_t>(l) * kvh;
       const float* ks = m.kv_scales;  // [4][L][kv_head]: s_k, s_v, 1 / s_k, 1 / s_v
-      PF_TRY(attend(reinterpret_cast<__nv_fp8_e4m3*>(m.key_cache), reinterpret_cast<__nv_fp8_e4m3*>(m.value_cache),
+      KLLM_TRY(attend(reinterpret_cast<__nv_fp8_e4m3*>(m.key_cache), reinterpret_cast<__nv_fp8_e4m3*>(m.value_cache),
                     KvScales{ks + 2 * n + h0, ks + 3 * n + h0}, KvScales{ks + h0, ks + n + h0}));
     } else if (cl.elem == KLLM_KV_BF16) {
-      PF_TRY(attend(reinterpret_cast<__nv_bfloat16*>(m.key_cache), reinterpret_cast<__nv_bfloat16*>(m.value_cache),
+      KLLM_TRY(attend(reinterpret_cast<__nv_bfloat16*>(m.key_cache), reinterpret_cast<__nv_bfloat16*>(m.value_cache),
                     KvScales{}, KvScales{}));
     } else {
-      PF_TRY(attend(m.key_cache, m.value_cache, KvScales{}, KvScales{}));
+      KLLM_TRY(attend(m.key_cache, m.value_cache, KvScales{}, KvScales{}));
     }
-    PF_TRY(count());
-    PF_TRY(gemm(ws.att, lw.o, ws.tmp, q_rows, dim));
+    KLLM_TRY(count());
+    KLLM_TRY(gemm(ws.att, lw.o, ws.tmp, q_rows, dim));
     add_rows_kernel<<<ew_grid, 256, 0, s>>>(ws.x, ws.tmp, static_cast<size_t>(T) * dim);
-    PF_TRY(count());
+    KLLM_TRY(count());
     rmsnorm_rows_kernel<<<T, 256, 0, s>>>(ws.x, lw.ffn_norm, ws.xn, dim, dm.eps);
-    PF_TRY(count());
-    PF_TRY(gemm(ws.xn, lw.w1, ws.h1, dim, hid));
-    PF_TRY(gemm(ws.xn, lw.w3, ws.h3, dim, hid));
+    KLLM_TRY(count());
+    KLLM_TRY(gemm(ws.xn, lw.w1, ws.h1, dim, hid));
+    KLLM_TRY(gemm(ws.xn, lw.w3, ws.h3, dim, hid));
     swiglu_rows_kernel<<<ew_grid, 256, 0, s>>>(ws.h1, ws.h3, static_cast<size_t>(T) * hid);
-    PF_TRY(count());
-    PF_TRY(gemm(ws.h1, lw.w2, ws.tmp, hid, dim));
+    KLLM_TRY(count());
+    KLLM_TRY(gemm(ws.h1, lw.w2, ws.tmp, hid, dim));
     add_rows_kernel<<<ew_grid, 256, 0, s>>>(ws.x, ws.tmp, static_cast<size_t>(T) * dim);
-    PF_TRY(count());
+    KLLM_TRY(count());
   }
   return 0;
 }
 
-int launch_rope_scatter_f32(const DecoderModel& dm, const CacheLayout& c, int layer, float* q, const float* k,
-                            const float* v, const float* sin_cache, const float* cos_cache, float* key_cache,
-                            float* value_cache, PosArg start_pos, int T, cudaStream_t s) {
-  if (c.elem != KLLM_KV_F32) return KLLM_E_UNSUPPORTED;
+int launch_rope_scatter_f32(const DecoderModel& dm, const DecoderCache& c, int layer, float* q, const float* k,
+                            const float* v, PosArg start_pos, int T, cudaStream_t s) {
+  if (c.cache.elem != KLLM_KV_F32) return KLLM_E_UNSUPPORTED;
   const size_t layer_off = static_cast<size_t>(layer) * dm.seq_len * dm.kv_dim;
-  rope_scatter_kernel<<<T, 256, 0, s>>>(q, k, v, sin_cache, cos_cache, key_cache + layer_off, value_cache + layer_off, c,
-                                        dm.head_num, dm.kv_head_num, dm.flavour, start_pos, KvScales{});
+  rope_scatter_kernel<<<rope_grid(T, dm.head_num, dm.kv_head_num, dm.head_size), 256, 0, s>>>(
+      q, k, v, c.sin_cache, c.cos_cache, c.key_cache + layer_off, c.value_cache + layer_off, c.cache, dm.head_num,
+      dm.kv_head_num, dm.flavour, start_pos, KvScales{});
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }

@@ -891,5 +891,37 @@ __device__ __forceinline__ void logprobs_block(const float* l, int n, int N, uns
     sync();
 }
 
+// Shared memory of a 1024-thread block's draw (up to 2048 candidates) and, after it, of its logprob routines
+constexpr int kDrawScratchBytes = kDrawScratchBase + 2048 * 8;
+static_assert(kDrawScratchBytes >= logprob_scratch_bytes(1024), "one scratch for the draw and the logprobs");
+
+// The draw and record entry of one position by a block of 1024 threads (the graph engine's step and each position of
+// kllm_decoder_verify): with step 0 on, the block first writes the adjusted logits to `penalized` (with pen's mark
+// words) and draws from those; the raw logits are left as they are.  Then, with `record` and logprobs on, it writes
+// the record entry at `pos` from the raw logits: of the drawn id, or of *target when target is set, which records
+// even with logprobs off (kllm_decoder_score's targets).  Returns the drawn id (0 when the draw found none) in every
+// thread.
+__device__ __forceinline__ int draw_and_record(const float* logits, int n, const DrawSettings* cfg, PenaltyParams pen,
+                                               float* penalized, const int32_t* hist, int pos, bool record,
+                                               const int32_t* target, LogprobRecord rec) {
+  __shared__ __align__(16) unsigned char scratch[kDrawScratchBytes];
+  const float* l = logits;
+  if (step0_active(pen)) {
+    step0_history<1024>(logits, penalized, 0, n, pen, hist, pos, [] { __syncthreads(); });
+    l = penalized;
+  }
+  const int bi = draw_block<1024>(l, n, cfg->sample, pos, nullptr, nullptr, 0, scratch, kDrawScratchBytes,
+                                  [] { __syncthreads(); });
+  const int id = bi < 0 ? 0 : bi;
+  const int top_n = target != nullptr ? max(cfg->lp_top_n, 0) : cfg->lp_top_n;
+  if (top_n >= 0 && record) {
+    logprobs_block<1024>(logits, n, top_n, scratch, kDrawScratchBytes, [] { __syncthreads(); });
+    const size_t row = static_cast<size_t>(pos) * kMaxTopLogprobs;
+    write_entry(logits, n, target != nullptr ? *target : id, top_n, *reinterpret_cast<const LogprobScratch*>(scratch),
+                rec.id + pos, rec.lp + pos, rec.top_ids + row, rec.top_lp + row);
+  }
+  return id;
+}
+
 }  // namespace sampling
 }  // namespace kllm

@@ -1,17 +1,20 @@
-// kllm_decoder_verify: n <= KLLM_MAX_VERIFY_TOKENS positions through every layer in ONE pass over the weights, for
-// speculative decoding (DESIGN.md 5.13).  Each position's arithmetic is the graph engine's step operation for
-// operation (decoder.cu enqueue_step), so position start_pos + i yields the bits a step there yields on either engine
-// in the exact numerics:
+// The decode chain: n <= KLLM_MAX_VERIFY_TOKENS positions through every layer in ONE pass over the weights.  The graph
+// engine's step (decoder.cu enqueue_step) is the chain at n = 1 between its embedding and its draw, and
+// kllm_decoder_verify (speculative decoding, DESIGN.md 5.13) runs it at n positions.  Each launch computes every
+// position with the arithmetic of a single one, so position start_pos + i yields the bits a step there yields on
+// either engine in the exact numerics:
 //
-//   step (per position)                          here (per block of n positions)
-//   embed_token_kernel                      ->   verify_embed_kernel: n rows; saves the history and record entries
-//   gemv_fused(norm -> q | k@cache | v@cache) ->  gemv_multi(norm -> q | k | v), n vectors per weight pack
-//   rope (in place in the cache row)         ->   rope_scatter: the same rotation, written through CacheLayout
-//   mha                                      ->   mha over (heads, positions), the same kernel and order
-//   gemv_fused(wo, + residual)               ->   gemv_multi(wo, + residual)
-//   gemv_fused(norm -> w1|w3 -> silu*gate)   ->   gemv_multi(norm -> w1|w3 -> silu*gate)
-//   gemv_fused(w2, + residual)               ->   gemv_multi(w2, + residual)
-//   gemv_fused(norm -> cls), argmax+advance  ->   gemv_multi(norm -> cls), one draw block per position, accept
+//   reference, per layer (15-18 launches)          here (6 launches for n positions)
+//   rmsnorm, wq, wk, wv [+3 bias adds]        ->   gemv(norm -> q | k | v [+bias]), n vectors per weight pack
+//   rope (pos read on the host)               ->   rope_scatter: q in place, k and v into the cache rows
+//   mha                                       ->   mha over (heads, positions)
+//   wo, add                                   ->   gemv(wo, + residual)
+//   rmsnorm, w1, w3, swiglu                   ->   gemv(norm -> w1|w3 -> silu*gate)
+//   w2, add                                   ->   gemv(w2, + residual)
+//   final: rmsnorm, cls                       ->   gemv(norm -> cls)
+//
+// The verify pass wraps the chain in verify_embed_kernel (n rows; saves the history and record entries), one draw
+// block per position and verify_accept_kernel.
 #include <cuda_runtime.h>
 
 #include "../../include/kllm_b200.h"
@@ -42,35 +45,16 @@ __global__ void verify_embed_kernel(VerifyIo* io, const float* __restrict__ tabl
   for (int e = threadIdx.x; e < (dim >> 2); e += blockDim.x) d4[e] = s4[e];
 }
 
-// argmax_advance_kernel's draw and record entry at position start_pos + blockIdx.x, from that position's logits row,
-// with its own step-0 marks and penalised row so that the blocks run at once
-constexpr int kDrawScratchBytes = sampling::kDrawScratchBase + 2048 * 8;
-static_assert(kDrawScratchBytes >= sampling::logprob_scratch_bytes(1024), "one scratch for the draw and the logprobs");
-
+// The draw and record entry at position start_pos + blockIdx.x from that position's logits row, with its own step-0
+// marks and penalised row so that the blocks run at once
 __global__ void __launch_bounds__(1024)
 verify_draw_kernel(const float* __restrict__ logits_rows, float* penalized_rows, int32_t* marks_rows, int n,
                    const DrawSettings* cfg, VerifyIo* io, const int32_t* hist, sampling::LogprobRecord rec) {
-  __shared__ __align__(16) unsigned char scratch[kDrawScratchBytes];
   const int i = blockIdx.x, pos = io->start_pos + i;
-  const float* logits = logits_rows + static_cast<size_t>(i) * n;
-  const float* l = logits;
   PenaltyParams pen = cfg->penalty;
   pen.marks = marks_rows + static_cast<size_t>(i) * n;
-  if (sampling::step0_active(pen)) {
-    float* penalized = penalized_rows + static_cast<size_t>(i) * n;
-    sampling::step0_history<1024>(logits, penalized, 0, n, pen, hist, pos, [] { __syncthreads(); });
-    l = penalized;
-  }
-  const int bi = sampling::draw_block<1024>(l, n, cfg->sample, pos, nullptr, nullptr, 0, scratch, kDrawScratchBytes,
-                                            [] { __syncthreads(); });
-  const int id = bi < 0 ? 0 : bi;
-  const int top_n = cfg->lp_top_n;
-  if (top_n >= 0) {
-    sampling::logprobs_block<1024>(logits, n, top_n, scratch, kDrawScratchBytes, [] { __syncthreads(); });
-    const size_t row = static_cast<size_t>(pos) * sampling::kMaxTopLogprobs;
-    sampling::write_entry(logits, n, id, top_n, *reinterpret_cast<const sampling::LogprobScratch*>(scratch),
-                          rec.id + pos, rec.lp + pos, rec.top_ids + row, rec.top_lp + row);
-  }
+  const int id = sampling::draw_and_record(logits_rows + static_cast<size_t>(i) * n, n, cfg, pen,
+                                           penalized_rows + static_cast<size_t>(i) * n, hist, pos, true, nullptr, rec);
   if (threadIdx.x == 0) io->ids[i] = id;
 }
 
@@ -115,74 +99,88 @@ __global__ void verify_accept_kernel(VerifyIo* io, int n, const float* __restric
   for (int e = threadIdx.x; e < vocab; e += blockDim.x) logits[e] = row[e];
 }
 
-#define VF_TRY(expr)                        \
-  do {                                      \
-    const int rc_ = static_cast<int>(expr); \
-    if (rc_ != 0) return rc_;               \
-  } while (0)
+namespace {
 
-int enqueue_verify(const DecoderModel& m, const VerifyTarget& t, const VerifyWorkspace& ws, int n, cudaStream_t s) {
-  const int dim = m.dim, hid = m.hidden_dim, q_rows = m.q_rows, kvd = m.kv_dim;
-  const PosArg first{&ws.io->start_pos, 0};
-  GemvExtra wx;
-  wx.format = m.format;
-  auto job = [&](const float* x, int in_dim, int n_seg, const float* norm_w) {
-    kllm_gemv_job j{};
-    j.x = x;
-    j.norm_w = norm_w;
-    j.norm_eps = m.eps;
-    j.in_dim = in_dim;
-    j.group_size = m.group_size;
-    j.n_seg = n_seg;
-    return j;
-  };
-  auto seg = [](const Matrix& w, float* out, int rows) { return kllm_gemv_seg{w.w, w.scales, w.bias, out, rows}; };
+kllm_gemv_seg seg(const Matrix& w, float* out, int rows) { return {w.w, w.scales, w.bias, out, rows}; }
 
-  verify_embed_kernel<<<n, 256, 0, s>>>(ws.io, m.tok_emb, ws.x, dim, t.hist, t.rec, ws.saved_hist, ws.saved);
-  count_launch();
-  VF_TRY(cudaGetLastError());
+// A GEMV of the model's matrices over x, RMS-normalised first with norm_w when it is set
+kllm_gemv_job job(const DecoderModel& m, const float* x, int in_dim, int n_seg, const float* norm_w = nullptr) {
+  kllm_gemv_job j{};
+  j.x = x;
+  j.norm_w = norm_w;
+  j.norm_eps = m.eps;
+  j.in_dim = in_dim;
+  j.group_size = m.group_size;
+  j.n_seg = n_seg;
+  return j;
+}
+
+// x += w . in (feed_forward's adds, llama3.cpp:683-684, 719): in the GEMV's residual epilogue, or under tensor
+// parallelism x += all-reduce(this rank's partial sums) (SURVEY.md 8e)
+int residual_gemv(const DecoderModel& m, const Matrix& w, const float* in, int in_dim, float* x, const TpReduce* tp,
+                  int n, cudaStream_t s) {
+  kllm_gemv_job j = job(m, in, in_dim, 1);
+  j.seg[0] = seg(w, tp ? tp->partial : x, m.dim);
+  j.residual = tp ? nullptr : x;
+  KLLM_TRY(gemv_dispatch(&j, m.format, s, n));
+  if (tp == nullptr) return 0;
+  const kllm_decoder_desc& d = *tp->desc;
+  if (d.comm != nullptr) return kllm_comm_allreduce_residual(d.comm, tp->partial, x, x, d.dim, s);
+  KLLM_TRY(d.allreduce(d.allreduce_ctx, tp->partial, d.dim, s));
+  return kllm_add_f32(x, tp->partial, x, d.dim, s);
+}
+
+}  // namespace
+
+int enqueue_classifier(const DecoderModel& m, const float* x, float* logits, int n, cudaStream_t s) {
+  kllm_gemv_job j = job(m, x, m.dim, 1, m.final_norm);
+  j.seg[0] = seg(m.cls, logits, m.vocab_size);
+  return gemv_dispatch(&j, m.format, s, n);
+}
+
+int enqueue_layers(const DecoderModel& m, const DecoderCache& c, const ChainRows& r, int n, PosArg first_pos,
+                   const TpReduce* tp, cudaStream_t s) {
+  const int dim = m.dim, hid = m.hidden_dim, q_rows = m.q_rows, kvd = m.kv_dim;  // q_rows == dim unless tensor-parallel
   for (int l = 0; l < m.layer_num; ++l) {
     const LayerWeights& lw = m.layers[l];
+    // attention_rms + attention_qkv (llama3.cpp:600-640)
     {
-      kllm_gemv_job j = job(ws.x, dim, 3, lw.attn_norm);
-      j.seg[0] = seg(lw.q, ws.q, q_rows);
-      j.seg[1] = seg(lw.k, ws.k, kvd);
-      j.seg[2] = seg(lw.v, ws.v, kvd);
-      VF_TRY(gemv_dispatch(&j, wx, s, n));
+      kllm_gemv_job j = job(m, r.x, dim, 3, lw.attn_norm);
+      j.seg[0] = seg(lw.q, r.q, q_rows);
+      j.seg[1] = seg(lw.k, r.k, kvd);
+      j.seg[2] = seg(lw.v, r.v, kvd);
+      KLLM_TRY(gemv_dispatch(&j, m.format, s, n));
     }
-    VF_TRY(launch_rope_scatter_f32(m, t.cache, l, ws.q, ws.k, ws.v, t.sin_cache, t.cos_cache, t.key_cache,
-                                   t.value_cache, first, n, s));
-    VF_TRY(launch_mha_rows(first, n, t.cache, m.head_num, l, m.kv_mul, ws.att, ws.q, ws.score, t.key_cache,
-                           t.value_cache, s));
+    KLLM_TRY(launch_rope_scatter_f32(m, c, l, r.q, r.k, r.v, first_pos, n, s));
+    // attention_mha (llama3.cpp:652-676)
+    KLLM_TRY(launch_mha_rows(first_pos, n, c.cache, m.head_num, l, m.kv_mul, r.att, r.q, r.score, c.key_cache,
+                             c.value_cache, s));
+    KLLM_TRY(residual_gemv(m, lw.o, r.att, q_rows, r.x, tp, n, s));
+    // feed_forward (llama3.cpp:686-720)
     {
-      kllm_gemv_job j = job(ws.att, q_rows, 1, nullptr);
-      j.seg[0] = seg(lw.o, ws.x, dim);
-      j.residual = ws.x;
-      VF_TRY(gemv_dispatch(&j, wx, s, n));
-    }
-    {
-      kllm_gemv_job j = job(ws.x, dim, 2, lw.ffn_norm);
-      j.seg[0] = seg(lw.w1, ws.h, hid);
+      kllm_gemv_job j = job(m, r.x, dim, 2, lw.ffn_norm);
+      j.seg[0] = seg(lw.w1, r.h, hid);
       j.seg[1] = seg(lw.w3, nullptr, hid);
       j.swiglu_pair = 1;
-      VF_TRY(gemv_dispatch(&j, wx, s, n));
+      KLLM_TRY(gemv_dispatch(&j, m.format, s, n));
     }
-    {
-      kllm_gemv_job j = job(ws.h, hid, 1, nullptr);
-      j.seg[0] = seg(lw.w2, ws.x, dim);
-      j.residual = ws.x;
-      VF_TRY(gemv_dispatch(&j, wx, s, n));
-    }
+    KLLM_TRY(residual_gemv(m, lw.w2, r.h, hid, r.x, tp, n, s));
   }
-  {
-    kllm_gemv_job j = job(ws.x, dim, 1, m.final_norm);
-    j.seg[0] = seg(m.cls, ws.logits, m.vocab_size);
-    VF_TRY(gemv_dispatch(&j, wx, s, n));
-  }
-  verify_draw_kernel<<<n, 1024, 0, s>>>(ws.logits, ws.penalized, ws.marks, m.vocab_size, t.cfg, ws.io, t.hist, t.rec);
+  // cls_logits (llama3.cpp:722-731)
+  return enqueue_classifier(m, r.x, r.logits, n, s);
+}
+
+int enqueue_verify(const DecoderModel& m, const DecoderCache& c, const VerifyTarget& t, const VerifyWorkspace& ws,
+                   int n, cudaStream_t s) {
+  verify_embed_kernel<<<n, 256, 0, s>>>(ws.io, m.tok_emb, ws.rows.x, m.dim, t.hist, t.rec, ws.saved_hist, ws.saved);
   count_launch();
-  VF_TRY(cudaGetLastError());
-  verify_accept_kernel<<<1, 1024, 0, s>>>(ws.io, n, ws.logits, t.logits, m.vocab_size, t.state, t.hist, t.rec,
+  KLLM_TRY(cudaGetLastError());
+  KLLM_TRY(enqueue_layers(m, c, ws.rows, n, PosArg{&ws.io->start_pos, 0}, nullptr, s));
+  verify_draw_kernel<<<n, 1024, 0, s>>>(ws.rows.logits, ws.penalized, ws.marks, m.vocab_size, t.cfg, ws.io, t.hist,
+                                        t.rec);
+  count_launch();
+  KLLM_TRY(cudaGetLastError());
+  verify_accept_kernel<<<1, 1024, 0, s>>>(ws.io, n, ws.rows.logits, t.logits, m.vocab_size, t.state, t.hist, t.rec,
                                           ws.saved_hist, ws.saved);
   count_launch();
   return static_cast<int>(cudaGetLastError());

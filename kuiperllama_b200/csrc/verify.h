@@ -1,5 +1,5 @@
-// kllm_decoder_verify's chain (verify.cu): a block of up to KLLM_MAX_VERIFY_TOKENS positions through every layer in one
-// pass over the weights, each position's arithmetic that of the graph engine's step (decoder.cu enqueue_step).
+// The decode chain (verify.cu): n <= KLLM_MAX_VERIFY_TOKENS positions through every layer and the classifier in one
+// pass over the weights.  The graph engine's step is the chain at n = 1; kllm_decoder_verify runs it at n positions.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -11,6 +11,28 @@
 #include "sampling.cuh"
 
 namespace kllm {
+
+// The chain's per-position rows, [n][.] each: x [dim] (the embeddings in, the residual stream), q and att
+// [q_rows], k and v [kv_dim], h [hidden_dim], score [head_num][seq_len], logits [vocab_size]
+struct ChainRows {
+  float *x, *q, *k, *v, *att, *h, *score, *logits;
+};
+
+// Tensor parallelism (n = 1): the row-parallel matmuls Wo and W2 write this rank's partial sums to `partial` [dim],
+// and x += their all-reduce over the description's transport
+struct TpReduce {
+  const kllm_decoder_desc* desc;
+  float* partial;
+};
+
+// Enqueues, for the n positions first_pos, first_pos + 1, .., every layer (q|k|v GEMV, RoPE with the k and v rows
+// written into the cache, attention, Wo with residual, W1|W3 SwiGLU, W2 with residual) and then the final-norm
+// classifier.  tp: null on one GPU.
+int enqueue_layers(const DecoderModel& m, const DecoderCache& c, const ChainRows& rows, int n, PosArg first_pos,
+                   const TpReduce* tp, cudaStream_t s);
+
+// The final RMSNorm and classifier of n rows x [n][dim] into logits [n][vocab_size]: the chain's last step
+int enqueue_classifier(const DecoderModel& m, const float* x, float* logits, int n, cudaStream_t s);
 
 // The call's arguments and result in device memory, so that one captured chain per block length serves every
 // position: the host uploads the first part and reads `ids` and `accepted` back.
@@ -25,18 +47,16 @@ struct VerifyIo {
 
 // Per-position scratch [KLLM_MAX_VERIFY_TOKENS][.] and the saved history and record entries of the block
 struct VerifyWorkspace {
-  float *x, *q, *k, *v, *att, *h, *logits, *penalized, *score;
+  ChainRows rows;
+  float* penalized;
   int32_t* marks;  // step 0's mark words, one row per position, zero between calls
   int32_t* saved_hist;
   sampling::LogprobRecord saved;  // indexed by the position's offset in the block
   VerifyIo* io;
 };
 
-// What the chain reads and writes of the decoder
+// What the verify pass reads and writes of the decoder besides its cache
 struct VerifyTarget {
-  prefill::CacheLayout cache;
-  float *key_cache, *value_cache;
-  const float *sin_cache, *cos_cache;
   const DrawSettings* cfg;
   mega::State* state;  // left as kllm_decoder_generate of a + 1 steps leaves it
   int32_t* hist;
@@ -44,7 +64,9 @@ struct VerifyTarget {
   float* logits;  // receives row a
 };
 
-// Enqueues the chain for n positions; every position is read from ws.io
-int enqueue_verify(const DecoderModel& m, const VerifyTarget& t, const VerifyWorkspace& ws, int n, cudaStream_t s);
+// Enqueues the verify pass of n positions: the embeddings, the chain, a draw per position and the acceptance; every
+// position is read from ws.io
+int enqueue_verify(const DecoderModel& m, const DecoderCache& c, const VerifyTarget& t, const VerifyWorkspace& ws,
+                   int n, cudaStream_t s);
 
 }  // namespace kllm

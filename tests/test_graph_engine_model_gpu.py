@@ -1,6 +1,6 @@
-"""-m gpu: the graph engine (csrc/decoder.cu enqueue_step: gemv.cu, attention.cu, elementwise.cu), and both engines
-at int8 group sizes other than 64, against tests/prefill_model.py, with the harness and bounds of
-test_decode_model_gpu.py (tests/decode_model_util.py).
+"""-m gpu: the graph engine (csrc/decoder.cu enqueue_step, the decode chain of csrc/verify.cu at one position: gemv.cu,
+prefill.cu's RoPE scatter, attention.cu), and both engines at int8 group sizes other than 64, against
+tests/prefill_model.py, with the harness and bounds of test_decode_model_gpu.py (tests/decode_model_util.py).
 
 1. Every case of test_decode_model_gpu.py on the graph engine in exact numerics, teacher-forced over every position
    to seq_len - 1: the logits at each segment end and every K / V row of every layer against the model, and both

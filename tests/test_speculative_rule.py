@@ -74,9 +74,9 @@ def test_header_declares_the_entries(kllm_lib):
 
 def test_verify_kernels_keep_out_of_local_memory(kllm_lib):
     """The verify chain's kernels stay out of local memory: none at all for the embedding, accept and attention
-    kernels; the draw block carries argmax_advance_kernel's sampling helpers (24 bytes of stack and 32 local accesses
-    there) and a per-position copy of the step-0 settings; the multi-vector GEMV may keep the 8-byte frame that
-    gemv_kernel's widest fp32 form has, with a few accesses to it."""
+    kernels; the draw block carries the sampling helpers it shares with argmax_advance_kernel (sampling.cuh
+    draw_and_record) and a per-position copy of the step-0 settings; the multi-vector GEMV may keep an 8-byte frame,
+    with a few accesses to it."""
     from kuiperllama_b200 import build as kbuild
     lib = str(kbuild.LIB)
     res = subprocess.run(["cuobjdump", "-res-usage", lib], capture_output=True, text=True, check=True).stdout
