@@ -1,6 +1,7 @@
 // The decoder's model as its three consumers read it -- the graph engine (decoder.cu), the persistent engine
 // (megakernel.cu) and the batched prefill (prefill.cu): the shape, one weight format for every matrix, and each
 // matrix with its scales and bias.  build_decoder_model is the one place a kllm_decoder_desc becomes a format.
+// Only .cu files include it: the format and its element size are also the kernels' template parameter.
 #pragma once
 #include <cstddef>
 #include <vector>
@@ -11,7 +12,9 @@ namespace kllm {
 
 enum class WeightFormat { kF32, kInt8, kBf16 };
 
-inline int weight_bytes(WeightFormat f) { return f == WeightFormat::kInt8 ? 1 : f == WeightFormat::kBf16 ? 2 : 4; }
+constexpr __host__ __device__ int weight_bytes(WeightFormat f) {
+  return f == WeightFormat::kInt8 ? 1 : f == WeightFormat::kBf16 ? 2 : 4;
+}
 
 // log2(group_size) for a power of two, else -1 (the kernels then divide)
 inline int group_shift_of(int group_size) {

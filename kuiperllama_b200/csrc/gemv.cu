@@ -16,6 +16,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cstdint>
+#include <type_traits>
 
 #include "../../include/kllm_b200.h"
 #include "kllm_device.cuh"
@@ -48,6 +49,7 @@ struct GemvParams {
 
 constexpr int kGemvWarps = 8;
 constexpr int kGemvThreads = kGemvWarps * 32;
+constexpr size_t kStageBytes = 200 * 1024;  // x staged in shared memory, [nv][in_dim rounded up to 4]
 
 // rmsnorm_kernel.cu:4-50 on the CTA's private copy of x in shared memory.  Executed by warp 0
 // with the 128 virtual threads of the reference laid out as lane + 32*j.
@@ -77,17 +79,42 @@ __device__ __forceinline__ float rms_scale_ref(const float* xs, int n, float eps
   return rsqrtf(__fadd_rn(__fdiv_rn(sum, static_cast<float>(n)), eps));
 }
 
+// A pack of four fp32 or bf16 weights, widened exactly to fp32: one 16- or 8-byte streaming load
+__device__ __forceinline__ float4 ldg_pack(const float4* p) { return ldg_stream_f4(p); }
+__device__ __forceinline__ float4 ldg_pack(const uint2* p) { return ldg_stream_bf16x4(p); }
+// Pack idx of a weight row that is not aligned for it: four scalar loads
+template <WeightFormat F>
+__device__ __forceinline__ float4 scalar_pack(const void* row, int idx) {
+  if constexpr (F == WeightFormat::kBf16) {
+    const unsigned short* wp = static_cast<const unsigned short*>(row) + 4 * idx;
+    return make_float4(widen_bf16(__ldg(wp)), widen_bf16(__ldg(wp + 1)), widen_bf16(__ldg(wp + 2)),
+                       widen_bf16(__ldg(wp + 3)));
+  } else {
+    const float* wp = static_cast<const float*>(row) + 4 * idx;
+    return make_float4(__ldg(wp), __ldg(wp + 1), __ldg(wp + 2), __ldg(wp + 3));
+  }
+}
+// weight i of a row (the scalar tail)
+template <WeightFormat F>
+__device__ __forceinline__ float weight_at(const void* row, int i) {
+  if constexpr (F == WeightFormat::kBf16) return widen_bf16(__ldg(static_cast<const unsigned short*>(row) + i));
+  else return static_cast<const float*>(row)[i];
+}
+
 // The GEMV body over NV input vectors x[nv][in_dim] (nv <= NV; gemv_kernel runs NV = nv = 1, gemv_multi_kernel the
 // positions of kllm_decoder_verify).  Each warp loads a weight pack once and runs every vector's virtual-thread chain on
 // it, so vector v's arithmetic is the single-vector kernel's operation for operation, with its own RMSNorm prologue,
 // bias, residual and SwiGLU epilogues.  Vector v's output row lands at seg.out[v * seg.rows + row] (SwiGLU:
 // out[v * units + u]), its residual is residual[v * units + row].  x is staged in shared memory
 // [nv][in_dim rounded up to 4].
-// kBf16: bf16 weights widened exactly to fp32 on load; every operation is the fp32 path's.
+// F = kBf16: bf16 weights widened exactly to fp32 on load; every operation is the fp32 path's.
 constexpr int kMaxVecs = 8;
 
-template <int R, bool kInt8, bool kSwiglu, bool kBf16, int NV>
+template <int R, WeightFormat F, bool kSwiglu, int NV>
 __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
+  constexpr bool kInt8 = F == WeightFormat::kInt8;
+  using Elem = std::conditional_t<kInt8, int8_t, std::conditional_t<F == WeightFormat::kBf16, unsigned short, float>>;
+  using Pack = std::conditional_t<F == WeightFormat::kBf16, uint2, float4>;  // fp32 and bf16: four weights
   extern __shared__ __align__(16) float xs[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -158,9 +185,7 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
       const long long e = static_cast<long long>(row) * M;
       ebase[r] = e;
       srow[r] = p.seg[seg].scales;
-      wrow[r] = kInt8    ? static_cast<const void*>(static_cast<const int8_t*>(p.seg[seg].w) + e)
-                : kBf16 ? static_cast<const void*>(static_cast<const unsigned short*>(p.seg[seg].w) + e)
-                        : static_cast<const void*>(static_cast<const float*>(p.seg[seg].w) + e);
+      wrow[r] = static_cast<const Elem*>(p.seg[seg].w) + e;
     }
 
     float acc[NV][R][4];
@@ -169,65 +194,7 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
 #pragma unroll
       for (int r = 0; r < R; ++r) acc[v][r][0] = acc[v][r][1] = acc[v][r][2] = acc[v][r][3] = 0.f;
 
-    if constexpr (kBf16) {
-      // the fp32 path below with 8-byte packs of four bf16 weights (scalar loads for unaligned rows)
-      auto pack = [&](int r, int idx) {
-        if (p.vec_ok) return ldg_stream_bf16x4(static_cast<const uint2*>(wrow[r]) + idx);
-        const unsigned short* wp = static_cast<const unsigned short*>(wrow[r]) + 4 * idx;
-        return make_float4(widen_bf16(__ldg(wp)), widen_bf16(__ldg(wp + 1)), widen_bf16(__ldg(wp + 2)),
-                           widen_bf16(__ldg(wp + 3)));
-      };
-      const int full = p.vec_ok ? (pack_num & ~127) : 0;
-      for (int base = 0; base < full; base += 128) {
-        float4 wv[R][4];
-#pragma unroll
-        for (int r = 0; r < R; ++r)
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            wv[r][j] = ldg_stream_bf16x4(static_cast<const uint2*>(wrow[r]) + base + 32 * j + lane);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-#pragma unroll
-          for (int v = 0; v < NV; ++v) {
-            if (v < nv) {
-              const float4 xv = xs4[v * P4 + base + 32 * j + lane];
-#pragma unroll
-              for (int r = 0; r < R; ++r) acc[v][r][j] = __fadd_rn(dot4_ref(xv, wv[r][j]), acc[v][r][j]);
-            }
-          }
-        }
-      }
-      for (int base = full; base < pack_num; base += 128) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int idx = base + 32 * j + lane;
-          if (idx < pack_num) {
-            float4 xv[NV];
-#pragma unroll
-            for (int v = 0; v < NV; ++v)
-              if (v < nv) xv[v] = xs4[v * P4 + idx];
-#pragma unroll
-            for (int r = 0; r < R; ++r) {
-              const float4 wv = pack(r, idx);
-#pragma unroll
-              for (int v = 0; v < NV; ++v)
-                if (v < nv) acc[v][r][j] = __fadd_rn(dot4_ref(xv[v], wv), acc[v][r][j]);
-            }
-          }
-        }
-      }
-      for (int i = (pack_num << 2) + lane; i < M; i += 128) {
-#pragma unroll
-        for (int v = 0; v < NV; ++v) {
-          if (v < nv) {
-#pragma unroll
-            for (int r = 0; r < R; ++r)
-              acc[v][r][0] = __fmaf_rn(xs[v * Mp + i], widen_bf16(__ldg(static_cast<const unsigned short*>(wrow[r]) + i)),
-                                       acc[v][r][0]);
-          }
-        }
-      }
-    } else if constexpr (!kInt8) {
+    if constexpr (!kInt8) {
       // virtual thread (lane + 32 j) <- packs base + 32 j + lane, base += 128
       const int full = p.vec_ok ? (pack_num & ~127) : 0;
       for (int base = 0; base < full; base += 128) {
@@ -236,7 +203,7 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
         for (int r = 0; r < R; ++r)
 #pragma unroll
           for (int j = 0; j < 4; ++j)
-            wv[r][j] = ldg_stream_f4(static_cast<const float4*>(wrow[r]) + base + 32 * j + lane);
+            wv[r][j] = ldg_pack(static_cast<const Pack*>(wrow[r]) + base + 32 * j + lane);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
 #pragma unroll
@@ -249,8 +216,8 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
           }
         }
       }
-      // remainder packs (and every pack when rows are not 16-byte aligned: ragged in_dim --
-      // the reference's float4 loads would fault there; same arithmetic, scalar loads)
+      // remainder packs (and every pack when rows are not aligned: ragged in_dim -- the reference's float4 loads
+      // would fault there; same arithmetic, scalar loads)
       for (int base = full; base < pack_num; base += 128) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -262,13 +229,8 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
               if (v < nv) xv[v] = xs4[v * P4 + idx];
 #pragma unroll
             for (int r = 0; r < R; ++r) {
-              float4 wv;
-              if (p.vec_ok) {
-                wv = ldg_stream_f4(static_cast<const float4*>(wrow[r]) + idx);
-              } else {
-                const float* wp = static_cast<const float*>(wrow[r]) + 4 * idx;
-                wv = make_float4(__ldg(wp), __ldg(wp + 1), __ldg(wp + 2), __ldg(wp + 3));
-              }
+              const float4 wv =
+                  p.vec_ok ? ldg_pack(static_cast<const Pack*>(wrow[r]) + idx) : scalar_pack<F>(wrow[r], idx);
 #pragma unroll
               for (int v = 0; v < NV; ++v)
                 if (v < nv) acc[v][r][j] = __fadd_rn(dot4_ref(xv[v], wv), acc[v][r][j]);
@@ -282,7 +244,7 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
         for (int r = 0; r < R; ++r) {
 #pragma unroll
           for (int v = 0; v < NV; ++v)
-            if (v < nv) acc[v][r][0] = __fmaf_rn(xs[v * Mp + i], static_cast<const float*>(wrow[r])[i], acc[v][r][0]);
+            if (v < nv) acc[v][r][0] = __fmaf_rn(xs[v * Mp + i], weight_at<F>(wrow[r], i), acc[v][r][0]);
         }
       }
     } else {
@@ -358,15 +320,15 @@ __device__ __forceinline__ void gemv_rows(const GemvParams& p, int nv) {
   }
 }
 
-template <int R, bool kInt8, bool kSwiglu, bool kBf16 = false>
+template <int R, WeightFormat F, bool kSwiglu>
 __global__ void __launch_bounds__(kGemvThreads) gemv_kernel(const GemvParams p) {
-  gemv_rows<R, kInt8, kSwiglu, kBf16, 1>(p, 1);
+  gemv_rows<R, F, kSwiglu, 1>(p, 1);
 }
 
 // nv <= kMaxVecs vectors; the caller splits them into groups whose x fits shared memory (gemv_dispatch)
-template <int R, bool kInt8, bool kSwiglu, bool kBf16>
+template <int R, WeightFormat F, bool kSwiglu>
 __global__ void __launch_bounds__(kGemvThreads) gemv_multi_kernel(const GemvParams p, int nv) {
-  gemv_rows<R, kInt8, kSwiglu, kBf16, kMaxVecs>(p, nv);
+  gemv_rows<R, F, kSwiglu, kMaxVecs>(p, nv);
 }
 
 static int g_sm_count = 0;
@@ -381,11 +343,11 @@ static int sm_count() {
   return g_sm_count;
 }
 
-template <int R, bool kInt8, bool kSwiglu, bool kBf16 = false>
+template <int R, WeightFormat F, bool kSwiglu>
 static int launch_gemv(const GemvParams& p, cudaStream_t stream) {
   constexpr int kUnits = R / (kSwiglu ? 2 : 1);
   const size_t smem = static_cast<size_t>(p.in_dim) * sizeof(float);
-  auto kern = gemv_kernel<R, kInt8, kSwiglu, kBf16>;
+  auto kern = gemv_kernel<R, F, kSwiglu>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(smem));
@@ -402,11 +364,11 @@ static int launch_gemv(const GemvParams& p, cudaStream_t stream) {
   return static_cast<int>(cudaGetLastError());
 }
 
-template <bool kInt8, bool kSwiglu, bool kBf16>
+template <WeightFormat F, bool kSwiglu>
 static int launch_gemv_multi(const GemvParams& p, int nv, cudaStream_t stream) {
   constexpr int R = kSwiglu ? 2 : 1;  // one output row (pair) per warp: the vectors give each lane its loads in flight
   const size_t smem = static_cast<size_t>(nv) * ((p.in_dim + 3) & ~3) * sizeof(float);
-  auto kern = gemv_multi_kernel<R, kInt8, kSwiglu, kBf16>;
+  auto kern = gemv_multi_kernel<R, F, kSwiglu>;
   // the kernel's static shared memory counts against the default 48 KB too: opt in at every size (a cached no-op
   // once granted)
   if (const int rc = smem_opt_in(reinterpret_cast<const void*>(kern), smem)) return rc;
@@ -417,17 +379,47 @@ static int launch_gemv_multi(const GemvParams& p, int nv, cudaStream_t stream) {
   return static_cast<int>(cudaGetLastError());
 }
 
+// A job's launches in weight format F: groups of up to kMaxVecs vectors on gemv_multi_kernel, or one vector on
+// gemv_kernel with R rows per warp
+template <WeightFormat F>
+static int launch_job(const kllm_gemv_job& job, GemvParams p, int nv, size_t per_vec, cudaStream_t stream) {
+  if (nv > 1) {
+    // Vectors per launch: as many as fit the x staging.  Llama-2-7B's W2 (in_dim 11008) takes four, so 5..8 vectors
+    // read that matrix twice; every vector's arithmetic is the same in any group.
+    const int group = static_cast<int>(std::min<size_t>(kMaxVecs, kStageBytes / per_vec));
+    for (int v0 = 0; v0 < nv; v0 += group) {
+      const int n = std::min(group, nv - v0);
+      p.x = job.x + static_cast<size_t>(v0) * job.in_dim;
+      p.residual = job.residual ? job.residual + static_cast<size_t>(v0) * p.units : nullptr;
+      for (int s = 0; s < job.n_seg; ++s) {
+        const size_t stride = job.swiglu_pair ? p.units : job.seg[s].rows;
+        p.seg[s].out = job.seg[s].out ? job.seg[s].out + v0 * stride : nullptr;
+      }
+      const int rc = job.swiglu_pair ? launch_gemv_multi<F, true>(p, n, stream) : launch_gemv_multi<F, false>(p, n, stream);
+      if (rc != 0) return rc;
+    }
+    return 0;
+  }
+
+  // Rows per warp: enough independent 128-bit loads in flight per lane (R*4) while still
+  // giving every SM work for the small matrices (kv projections: 256 rows).
+  const int warps_1wave = sm_count() * kGemvWarps;
+  if (job.swiglu_pair)
+    return p.units >= warps_1wave * 2 ? launch_gemv<4, F, true>(p, stream) : launch_gemv<2, F, true>(p, stream);
+  if (p.units >= warps_1wave * 4) return launch_gemv<4, F, false>(p, stream);
+  if (p.units >= warps_1wave * 2) return launch_gemv<2, F, false>(p, stream);
+  return launch_gemv<1, F, false>(p, stream);
+}
+
 int gemv_dispatch(const kllm_gemv_job* job, WeightFormat format, cudaStream_t stream, int nv) {
   if (job == nullptr || job->x == nullptr || job->in_dim <= 0 || nv < 1 || nv > kMaxVecs) return KLLM_E_INVALID;
   if (job->n_seg < 1 || job->n_seg > 3) return KLLM_E_INVALID;
   if (nv > 1 && job->residual != nullptr && job->n_seg != 1) return KLLM_E_INVALID;  // residual rows are the units
   const bool int8 = format == WeightFormat::kInt8;
-  const bool bf16 = format == WeightFormat::kBf16;
   if (job->swiglu_pair && (job->n_seg != 2 || job->seg[0].rows != job->seg[1].rows ||
                            job->residual != nullptr))
     return KLLM_E_INVALID;
   if (int8 && ((job->in_dim & 3) != 0 || (job->group_size & 3) != 0)) return KLLM_E_UNSUPPORTED;
-  constexpr size_t kStageBytes = 200 * 1024;  // x staged in shared memory, [nv][in_dim rounded up to 4]
   const size_t per_vec = static_cast<size_t>(nv == 1 ? job->in_dim : (job->in_dim + 3) & ~3) * sizeof(float);
   if (per_vec > kStageBytes) return KLLM_E_UNSUPPORTED;
 
@@ -448,7 +440,7 @@ int gemv_dispatch(const kllm_gemv_job* job, WeightFormat format, cudaStream_t st
     if (g.w == nullptr || g.rows <= 0) return KLLM_E_INVALID;
     if (int8 && g.scales == nullptr) return KLLM_E_INVALID;
     if (g.out == nullptr && !(job->swiglu_pair && s == 1)) return KLLM_E_INVALID;
-    if ((reinterpret_cast<uintptr_t>(g.w) & (int8 ? 3 : bf16 ? 7 : 15)) != 0) {
+    if ((reinterpret_cast<uintptr_t>(g.w) & (4 * weight_bytes(format) - 1)) != 0) {  // a pack of four weights
       if (int8) return KLLM_E_UNSUPPORTED;
       p.vec_ok = 0;
     }
@@ -457,58 +449,11 @@ int gemv_dispatch(const kllm_gemv_job* job, WeightFormat format, cudaStream_t st
   }
   p.units = job->swiglu_pair ? job->seg[0].rows : total;
 
-  if (nv > 1) {
-    // Vectors per launch: as many as fit the x staging.  Llama-2-7B's W2 (in_dim 11008) takes four, so 5..8 vectors
-    // read that matrix twice; every vector's arithmetic is the same in any group.
-    const int group = static_cast<int>(std::min<size_t>(kMaxVecs, kStageBytes / per_vec));
-    for (int v0 = 0; v0 < nv; v0 += group) {
-      const int n = std::min(group, nv - v0);
-      p.x = job->x + static_cast<size_t>(v0) * job->in_dim;
-      p.residual = job->residual ? job->residual + static_cast<size_t>(v0) * p.units : nullptr;
-      for (int s = 0; s < job->n_seg; ++s) {
-        const size_t stride = job->swiglu_pair ? p.units : job->seg[s].rows;
-        p.seg[s].out = job->seg[s].out ? job->seg[s].out + v0 * stride : nullptr;
-      }
-      int rc;
-      if (int8)
-        rc = job->swiglu_pair ? launch_gemv_multi<true, true, false>(p, n, stream)
-                              : launch_gemv_multi<true, false, false>(p, n, stream);
-      else if (bf16)
-        rc = job->swiglu_pair ? launch_gemv_multi<false, true, true>(p, n, stream)
-                              : launch_gemv_multi<false, false, true>(p, n, stream);
-      else
-        rc = job->swiglu_pair ? launch_gemv_multi<false, true, false>(p, n, stream)
-                              : launch_gemv_multi<false, false, false>(p, n, stream);
-      if (rc != 0) return rc;
-    }
-    return 0;
+  switch (format) {
+    case WeightFormat::kInt8: return launch_job<WeightFormat::kInt8>(*job, p, nv, per_vec, stream);
+    case WeightFormat::kBf16: return launch_job<WeightFormat::kBf16>(*job, p, nv, per_vec, stream);
+    default: return launch_job<WeightFormat::kF32>(*job, p, nv, per_vec, stream);
   }
-
-  // Rows per warp: enough independent 128-bit loads in flight per lane (R*4) while still
-  // giving every SM work for the small matrices (kv projections: 256 rows).
-  const int warps_1wave = sm_count() * kGemvWarps;
-  if (bf16) {
-    if (job->swiglu_pair)
-      return p.units >= warps_1wave * 2 ? launch_gemv<4, false, true, true>(p, stream)
-                                        : launch_gemv<2, false, true, true>(p, stream);
-    if (p.units >= warps_1wave * 4) return launch_gemv<4, false, false, true>(p, stream);
-    if (p.units >= warps_1wave * 2) return launch_gemv<2, false, false, true>(p, stream);
-    return launch_gemv<1, false, false, true>(p, stream);
-  }
-  if (job->swiglu_pair) {
-    if (int8) return p.units >= warps_1wave * 2 ? launch_gemv<4, true, true>(p, stream)
-                                                : launch_gemv<2, true, true>(p, stream);
-    return p.units >= warps_1wave * 2 ? launch_gemv<4, false, true>(p, stream)
-                                      : launch_gemv<2, false, true>(p, stream);
-  }
-  if (int8) {
-    if (p.units >= warps_1wave * 4) return launch_gemv<4, true, false>(p, stream);
-    if (p.units >= warps_1wave * 2) return launch_gemv<2, true, false>(p, stream);
-    return launch_gemv<1, true, false>(p, stream);
-  }
-  if (p.units >= warps_1wave * 4) return launch_gemv<4, false, false>(p, stream);
-  if (p.units >= warps_1wave * 2) return launch_gemv<2, false, false>(p, stream);
-  return launch_gemv<1, false, false>(p, stream);
 }
 
 }  // namespace kllm

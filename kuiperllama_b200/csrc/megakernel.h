@@ -114,9 +114,9 @@ struct Params {
   float* score;
   // KV cache in the persistent engine's own layout (see megakernel.cu "KV layout"):
   //   K [L][kv_head][head_size/4][seq_len][4]    V [L][kv_head][attn_split][seq_len][head_size/attn_split]
-  // kv16_megakernel (KLLM_KV_BF16, flash form only): both caches hold bf16 elements behind these pointers,
+  // KLLM_KV_BF16 (flash form only): both caches hold bf16 elements behind these pointers,
   //   K [L][kv_head][head_size/8][seq_len][8]    V [L][kv_head][seq_len][head_size]
-  // kv8_megakernel (KLLM_KV_FP8, flash form only): e4m3 codes, K [L][kv_head][head_size/16][seq_len][16], V as bf16's
+  // KLLM_KV_FP8 (flash form only): e4m3 codes, K [L][kv_head][head_size/16][seq_len][16], V as bf16's
   float* key_cache;
   const float* value_cache;
   const float* sin_cache;

@@ -20,7 +20,7 @@
 //                  released once the wgmma group after it has been issued and the one reading it retired
 //   epilogue       each consumer thread stores its accumulator fragment straight to out
 //
-// int8 weights (template parameter W8): the producer loads the weight tile as bytes [128 x 32 int8] into
+// int8 weights (template parameter F = WeightFormat::kInt8): the producer loads the weight tile as bytes [128 x 32 int8] into
 // a 4 KB staging area of the stage; each consumer warpgroup dequantises its 64 rows (scale * q in fp32,
 // rounded to the nearest tf32) into the same 128-byte-swizzled fp32 A tile TMA would have written, so the
 // wgmma descriptors and instructions are the fp32 path's.  The scale of a row is constant over a 32-column
@@ -28,7 +28,7 @@
 // one K block ahead: scale rows can be 4 bytes, which TMA cannot copy.  A stage is dequantised while the
 // wgmma group of the stage before it is still running.
 //
-// bf16 weights (template parameter W16, kllm_gemm_bf16_tf32): the same staging with a [128 x 32 bf16] tile of
+// bf16 weights (F = WeightFormat::kBf16, kllm_gemm_bf16_tf32): the same staging with a [128 x 32 bf16] tile of
 // 64-byte rows, widened into the fp32 A tile.  A bf16 value widens exactly and is already a tf32 value, so the A
 // tile holds what kllm_gemm_tf32 holds after its rounding of the widened weights: the results are bit-identical.
 #include <cuda.h>
@@ -47,12 +47,10 @@ constexpr int BK = 32;      // fp32 elements per K block = 128 bytes = one swizz
 constexpr int WG_K = 8;     // tf32: 32 bytes of K per wgmma
 constexpr int STAGES = 4;
 constexpr int A_BYTES = BM * BK * 4;  // 16 KB
-constexpr int W8_BYTES = BM * BK;     // 4 KB: the int8 weight tile as loaded, rows of 32 bytes
-constexpr int W16_BYTES = BM * BK * 2;  // 8 KB: the bf16 weight tile as loaded, rows of 64 bytes
-// bytes of the weight staging area per stage
-template <bool W8, bool W16>
-__host__ __device__ constexpr int staging_bytes() {
-  return W8 ? W8_BYTES : W16 ? W16_BYTES : 0;
+// bytes of the weight staging area per stage: the int8 (4 KB, rows of 32 bytes) or bf16 (8 KB, rows of 64 bytes)
+// weight tile as loaded; fp32 tiles land in the A tile directly
+__host__ __device__ constexpr int staging_bytes(WeightFormat f) {
+  return f == WeightFormat::kF32 ? 0 : BM * BK * weight_bytes(f);
 }
 constexpr int THREADS = 384;
 
@@ -225,7 +223,7 @@ __device__ __forceinline__ void widen_w16(const uint8_t* src, uint8_t* a_rows, i
   }
 }
 
-template <int BN, bool W8, bool W16 = false>
+template <int BN, WeightFormat F>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x,
                  float* __restrict__ out, const float* __restrict__ scales, int T, int N, int K, int group_size) {
@@ -234,8 +232,9 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* a_tiles = base;
   uint8_t* b_tiles = base + STAGES * A_BYTES;
-  uint8_t* w8_tiles = b_tiles + STAGES * B_BYTES;  // W8 / W16 only: the weight staging area
-  constexpr int WS_BYTES = staging_bytes<W8, W16>();
+  uint8_t* w8_tiles = b_tiles + STAGES * B_BYTES;  // int8 / bf16 only: the weight staging area
+  constexpr int WS_BYTES = staging_bytes(F);
+  constexpr bool W8 = F == WeightFormat::kInt8;
   uint64_t* bars = reinterpret_cast<uint64_t*>(w8_tiles + STAGES * WS_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
@@ -289,10 +288,10 @@ gemm_tf32_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constan
     // half of the token rows, which both read, so the two meet at a named barrier before the wgmma (async proxy)
     // reads the tiles.
     if constexpr (W8)
-      dequant_w8(w8_tiles + s * W8_BYTES + ((wg - 1) * 64 + dq_row) * BK + dq_half * 16, a_tiles + s * A_BYTES + a_off,
+      dequant_w8(w8_tiles + s * WS_BYTES + ((wg - 1) * 64 + dq_row) * BK + dq_half * 16, a_tiles + s * A_BYTES + a_off,
                  dq_row, dq_half, sc);
-    else if constexpr (W16)
-      widen_w16(w8_tiles + s * W16_BYTES + ((wg - 1) * 64 + dq_row) * BK * 2 + dq_half * 32,
+    else if constexpr (F == WeightFormat::kBf16)
+      widen_w16(w8_tiles + s * WS_BYTES + ((wg - 1) * 64 + dq_row) * BK * 2 + dq_half * 32,
                 a_tiles + s * A_BYTES + a_off, dq_row, dq_half);
     else
       round_tf32(reinterpret_cast<float4*>(a_tiles + s * A_BYTES + a_off), 64 * BK / 4, t);
@@ -360,34 +359,34 @@ static int make_map(CUtensorMap* map, const void* ptr, int elem, int rows, int c
   return r == CUDA_SUCCESS ? 0 : KLLM_E_INVALID;
 }
 
-template <int BN, bool W8, bool W16 = false>
+template <int BN, WeightFormat F>
 static int launch(const float* x, const void* w, const float* scales, float* out, int T, int K, int N, int group_size,
                   cudaStream_t stream) {
   CUtensorMap map_w, map_x;
-  if (int rc = make_map(&map_w, w, W8 ? 1 : W16 ? 2 : 4, N, K, BM)) return rc;
+  if (int rc = make_map(&map_w, w, weight_bytes(F), N, K, BM)) return rc;
   if (int rc = make_map(&map_x, x, 4, T, K, BN)) return rc;
-  const size_t smem = 1024 + static_cast<size_t>(STAGES) * (A_BYTES + BN * BK * 4 + staging_bytes<W8, W16>()) + 128;
+  const size_t smem = 1024 + static_cast<size_t>(STAGES) * (A_BYTES + BN * BK * 4 + staging_bytes(F)) + 128;
   static bool configured = false;
   if (!configured) {
-    const cudaError_t e = cudaFuncSetAttribute(gemm_tf32_kernel<BN, W8, W16>,
+    const cudaError_t e = cudaFuncSetAttribute(gemm_tf32_kernel<BN, F>,
                                                cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return static_cast<int>(e);
     configured = true;
   }
   const dim3 grid((N + BM - 1) / BM, (T + BN - 1) / BN);
-  gemm_tf32_kernel<BN, W8, W16><<<grid, THREADS, smem, stream>>>(map_w, map_x, out, scales, T, N, K, group_size);
+  gemm_tf32_kernel<BN, F><<<grid, THREADS, smem, stream>>>(map_w, map_x, out, scales, T, N, K, group_size);
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }
 
 // token-block width: the smallest wgmma N that covers the tokens, 256 at most
-template <bool W8, bool W16 = false>
+template <WeightFormat F>
 static int dispatch(const float* x, const void* w, const float* scales, float* out, int T, int K, int N, int group_size,
                     cudaStream_t s) {
-  if (T <= 32) return launch<32, W8, W16>(x, w, scales, out, T, K, N, group_size, s);
-  if (T <= 64) return launch<64, W8, W16>(x, w, scales, out, T, K, N, group_size, s);
-  if (T <= 128) return launch<128, W8, W16>(x, w, scales, out, T, K, N, group_size, s);
-  return launch<256, W8, W16>(x, w, scales, out, T, K, N, group_size, s);
+  if (T <= 32) return launch<32, F>(x, w, scales, out, T, K, N, group_size, s);
+  if (T <= 64) return launch<64, F>(x, w, scales, out, T, K, N, group_size, s);
+  if (T <= 128) return launch<128, F>(x, w, scales, out, T, K, N, group_size, s);
+  return launch<256, F>(x, w, scales, out, T, K, N, group_size, s);
 }
 
 }  // namespace tc
@@ -398,7 +397,8 @@ extern "C" int kllm_gemm_tf32(const float* x, const float* w, float* out, int n_
   if (!x || !w || !out || n_tokens <= 0 || in_dim <= 0 || out_dim <= 0) return KLLM_E_INVALID;
   // TMA needs 16-byte aligned bases and row pitches
   if ((in_dim & 3) || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(w) & 15)) return KLLM_E_UNSUPPORTED;
-  return kllm::tc::dispatch<false>(x, w, nullptr, out, n_tokens, in_dim, out_dim, 0, static_cast<cudaStream_t>(stream));
+  return kllm::tc::dispatch<kllm::WeightFormat::kF32>(x, w, nullptr, out, n_tokens, in_dim, out_dim, 0,
+                                                     static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int kllm_gemm_w8_tf32(const float* x, const int8_t* w, const float* scales, float* out, int n_tokens,
@@ -410,8 +410,8 @@ extern "C" int kllm_gemm_w8_tf32(const float* x, const int8_t* w, const float* s
   if ((in_dim % 16) || (in_dim % group_size) || (group_size % 32) || (reinterpret_cast<uintptr_t>(x) & 15) ||
       (reinterpret_cast<uintptr_t>(w) & 15))
     return KLLM_E_UNSUPPORTED;
-  return kllm::tc::dispatch<true>(x, w, scales, out, n_tokens, in_dim, out_dim, group_size,
-                                  static_cast<cudaStream_t>(stream));
+  return kllm::tc::dispatch<kllm::WeightFormat::kInt8>(x, w, scales, out, n_tokens, in_dim, out_dim, group_size,
+                                                      static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int kllm_gemm_bf16_tf32(const float* x, const uint16_t* w, float* out, int n_tokens, int in_dim, int out_dim,
@@ -420,6 +420,6 @@ extern "C" int kllm_gemm_bf16_tf32(const float* x, const uint16_t* w, float* out
   // TMA needs 16-byte aligned bases and row pitches (2 in_dim bytes for the bf16 rows)
   if ((in_dim & 7) || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(w) & 15))
     return KLLM_E_UNSUPPORTED;
-  return kllm::tc::dispatch<false, true>(x, w, nullptr, out, n_tokens, in_dim, out_dim, 0,
-                                         static_cast<cudaStream_t>(stream));
+  return kllm::tc::dispatch<kllm::WeightFormat::kBf16>(x, w, nullptr, out, n_tokens, in_dim, out_dim, 0,
+                                                      static_cast<cudaStream_t>(stream));
 }

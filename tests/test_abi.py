@@ -71,31 +71,36 @@ def test_argument_validation_without_device(kllm_lib):
     assert kllm_lib.kllm_decoder_create(None, None, None) == -1
 
 
-def test_megakernel_keeps_its_state_out_of_local_memory(kllm_lib):
+def test_every_megakernel_instantiation_keeps_its_state_out_of_local_memory(kllm_lib):
     """The persistent kernel's ring takes the whole unified L1, so a local-memory access is a round trip to L2
-    (DESIGN.md 5.2, "No local memory").  Gate: the default instantiations -- 8 fp32 and 8 int8 consumer warps --
-    carry no parameter copy on the stack (it was 456 bytes before the parameters became __grid_constant__) and
-    only a handful of local loads / stores (per-token spills and the cold trap-message path), none of them in
-    the row loops' register budget class; nvcc / ptxas regressions of that kind show up here, on the CPU."""
-    import re
-    import subprocess
+    (DESIGN.md 5.2, "No local memory").  The library holds exactly the decode_megakernel<F, KV, LP, PROF>
+    instantiations of the table -- {fp32, int8, bf16} weights x {fp32, bf16, fp8} caches x {plain, log-probabilities},
+    plus the profiling kernels of fp32 and int8 weights over the fp32 cache -- and every one of them carries no
+    parameter copy on the stack (it was 456 bytes before the parameters became __grid_constant__) and only a handful of
+    local loads / stores (per-token spills and the cold trap-message path), is fed by TMA bulk copies on mbarriers, and
+    with the fp8 cache widens and encodes e4m3 in hardware.  The plain fp32 and int8 kernels over the fp32 cache keep
+    the row loops' register budget.  nvcc / ptxas regressions of that kind show up here, on the CPU."""
     from kuiperllama_b200 import build as kbuild
     lib = str(kbuild.LIB)
     res = subprocess.run(["cuobjdump", "-res-usage", lib], capture_output=True, text=True, check=True).stdout
-    usage = {}
-    for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+)", res):
-        usage[m.group(1)] = (int(m.group(2)), int(m.group(3)))
-    defaults = {"_ZN4kllm4mega17decode_megakernelILi8ELb0ELb0EEEvNS0_6ParamsE": 168,
-                "_ZN4kllm4mega17decode_megakernelILi8ELb1ELb0EEEvNS0_6ParamsE": 168}
-    # one consumer-warp count: {fp32, int8} x {plain, profiling}
-    assert sorted(k for k in usage if "decode_megakernel" in k) == sorted(
-        f"_ZN4kllm4mega17decode_megakernelILi8ELb{int8}ELb{prof}EEEvNS0_6ParamsE" for int8 in (0, 1) for prof in (0, 1))
-    for name, reg_cap in defaults.items():
-        assert name in usage, sorted(k for k in usage if "megakernel" in k)
-        regs, stack = usage[name]
-        assert regs <= reg_cap, (name, regs)
-        assert stack <= 64, f"{name}: {stack} bytes of stack (a parameter copy or a local array is back)"
-        sass = subprocess.run(["cuobjdump", "-sass", "-fun", name, lib], capture_output=True, text=True, check=True).stdout
+    usage = {m.group(1): (int(m.group(2)), int(m.group(3)))
+             for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+)", res)}
+    F32, INT8, BF16 = 0, 1, 2  # WeightFormat
+    KV_F32, KV_FP8 = 0, 2      # kllm_decoder_desc::kv_cache
+    table = [(f, kv, lp, 0) for f in (F32, INT8, BF16) for kv in (0, 1, 2) for lp in (0, 1)] + \
+            [(f, KV_F32, 0, 1) for f in (F32, INT8)]
+    name = {t: "_ZN4kllm4mega17decode_megakernelILNS_12WeightFormatE{}ELi{}ELb{}ELb{}EEEvNS0_6ParamsE".format(*t)
+            for t in table}
+    assert len(name) == 20
+    assert sorted(k for k in usage if "megakernel" in k) == sorted(name.values())
+    for (f, kv, lp, prof), n in name.items():
+        regs, stack = usage[n]
+        assert stack <= 64, f"{n}: {stack} bytes of stack (a parameter copy or a local array is back)"
+        if f != BF16 and kv == KV_F32 and not lp and not prof:
+            assert regs <= 168, (n, regs)
+        sass = subprocess.run(["cuobjdump", "-sass", "-fun", n, lib], capture_output=True, text=True, check=True).stdout
         local = len(re.findall(r"\b(?:LDL|STL)\b", sass))
-        assert local <= 32, f"{name}: {local} local-memory instructions"
-        assert "UBLKCP" in sass and "SYNCS" in sass  # TMA bulk copies + mbarriers are what feeds the ring
+        assert local <= 32, f"{n}: {local} local-memory instructions"
+        assert "UBLKCP" in sass and "SYNCS" in sass, n  # TMA bulk copies + mbarriers are what feeds the ring
+        if kv == KV_FP8:
+            assert "F2FP.F16.E4M3.UNPACK_B" in sass and "SATFINITE.E4M3" in sass, n  # hardware e4m3 conversions

@@ -5,10 +5,9 @@
    the graph engine.  They come
    before the device lookup, so each returns its code on any machine.
 2. The descriptor's new trailing field matches the header's layout.
-3. The six fp8 megakernel instantiations pass test_abi.py's gate of the defaults.
+(test_abi.py gates the fp8 cache's megakernel instantiations with every other one.)
 """
 import ctypes
-import re
 import subprocess
 
 import pytest
@@ -108,24 +107,3 @@ def test_descriptor_layout_matches_the_header(tmp_path):
     assert (size, off, fp8_value) == (ctypes.sizeof(DecoderDesc), DecoderDesc.kv_scales.offset, 2)
     assert not DecoderDesc().kv_scales  # a zeroed struct: unit scales
 
-
-def test_fp8_megakernels_keep_their_state_out_of_local_memory(kllm_lib):
-    """kv8_megakernel ({fp32, int8} x {plain, logprobs}) and w16kv8_megakernel ({plain, logprobs}): at most 64 bytes of
-    stack, at most 32 local loads / stores, and the ring fed by TMA bulk copies on mbarriers."""
-    from kuiperllama_b200 import build as kbuild
-    lib = str(kbuild.LIB)
-    res = subprocess.run(["cuobjdump", "-res-usage", lib], capture_output=True, text=True, check=True).stdout
-    usage = {m.group(1): (int(m.group(2)), int(m.group(3)))
-             for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+)", res)}
-    names = sorted(k for k in usage if "kv8_megakernel" in k)
-    assert names == sorted([f"_ZN4kllm4mega14kv8_megakernelILi8ELb{i}ELb{lp}EEEvNS0_6ParamsE"
-                            for i in (0, 1) for lp in (0, 1)] +
-                           [f"_ZN4kllm4mega17w16kv8_megakernelILi8ELb{lp}EEEvNS0_6ParamsE" for lp in (0, 1)])
-    for name in names:
-        regs, stack = usage[name]
-        assert stack <= 64, (name, stack)
-        sass = subprocess.run(["cuobjdump", "-sass", "-fun", name, lib], capture_output=True, text=True,
-                              check=True).stdout
-        assert len(re.findall(r"\b(?:LDL|STL)\b", sass)) <= 32, name
-        assert "UBLKCP" in sass and "SYNCS" in sass, name
-        assert "F2FP.F16.E4M3.UNPACK_B" in sass and "SATFINITE.E4M3" in sass, name  # hardware e4m3 conversions

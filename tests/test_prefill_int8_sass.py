@@ -9,7 +9,7 @@ import pytest
 from conftest import ROOT
 
 
-def test_int8_prefill_gemm_runs_on_the_tensor_cores_without_local_memory(kllm_lib):
+def test_int8_weight_prefill_gemms_run_on_the_tensor_cores_without_local_memory(kllm_lib):
     """Every instantiation of gemm_tf32_kernel for int8 weights (kllm_gemm_w8_tf32) is fed by TMA (UTMALDG) and
     multiplies with wgmma (HGMMA), with no stack and no local-memory access: its 128 accumulators per thread at
     BN = 256 live in registers."""
@@ -18,7 +18,7 @@ def test_int8_prefill_gemm_runs_on_the_tensor_cores_without_local_memory(kllm_li
     res = subprocess.run(["cuobjdump", "-res-usage", lib], capture_output=True, text=True, check=True).stdout
     usage = {m.group(1): int(m.group(2))
              for m in re.finditer(r"Function (\S+):\s*\n\s*REG:\d+ STACK:(\d+)", res)}
-    w8 = sorted(n for n in usage if "gemm_tf32_kernel" in n and re.search(r"ILi\d+ELb1E", n))
+    w8 = sorted(n for n in usage if "gemm_tf32_kernel" in n and re.search(r"ILi\d+ELNS_12WeightFormatE1E", n))
     assert len(w8) == 4, sorted(n for n in usage if "gemm_tf32_kernel" in n)  # BN = 32, 64, 128, 256
     for name in w8:
         assert usage[name] == 0, f"{name}: {usage[name]} bytes of stack"
