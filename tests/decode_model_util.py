@@ -82,24 +82,45 @@ WEIGHTS = {"synth": lambda shape, device, seed: synth_weights(shape, device, see
 
 
 # ---- the persistent engine's attention geometry (MegaEngine::init) -----------------------------------------------
-def engine_geometry(shape, numerics, env, sms, kv_cache="fp32"):
+KV_ELEM_BYTES = {"fp32": 4, "bf16": 2, "fp8": 1}
+
+
+def weight_format_of(shape, weight_format="fp32"):
+    """The decoder's weight format: "int8" for a shape with an int8 group size, else the one asked for (fp32 or the
+    bf16 weights of decoder.bf16_weights)."""
+    assert weight_format in ("fp32", "bf16") or (weight_format == "int8" and shape.group_size), weight_format
+    return "int8" if shape.group_size else weight_format
+
+
+def stage_bytes(shape, numerics, env, kv_cache="fp32", weight_format="fp32"):
+    """The ring stage MegaEngine::init picks: KLLM_STAGE_BYTES, else 27 KB for int8 weights, 24 KB for bf16 weights in
+    the fast mode and 32 KB in the exact mode, 16 KB for fp32 weights in the fast mode with an fp32 cache when two input
+    rows of dim fit (dim <= 2048), else 32 KB; rounded up to 128 bytes."""
+    wf = weight_format_of(shape, weight_format)
+    fast = numerics == "fast"
+    if wf == "int8":
+        default = 27 * 1024
+    elif wf == "bf16":
+        default = 24 * 1024 if fast else 32 * 1024
+    else:
+        default = 16 * 1024 if fast and kv_cache == "fp32" and 2 * shape.dim * 4 <= 16 * 1024 else 32 * 1024
+    return (int(env.get("KLLM_STAGE_BYTES", default)) + 127) & ~127
+
+
+def engine_geometry(shape, numerics, env, sms, kv_cache="fp32", weight_format="fp32"):
     """(tile T, split SP, V tile, stage bytes) the persistent engine chooses, which Decoder.attention_geometry
     reports; every persistent case asserts the two agree, so that a change to the rules fails loudly instead of
     moving the segment ends off the tiles' edges.
-    Stage: KLLM_STAGE_BYTES, else 27 KB for int8, 16 KB for fp32 in the fast mode with an fp32 cache when two input
-    rows of dim fit (dim <= 2048), else 32 KB; rounded up to 128 bytes.  T = min(stage / (hs * elem), 256) & ~31.
+    Stage: stage_bytes.  T = min(stage / (hs * elem), 256) & ~31, elem the cache's element: 4 bytes for fp32, 2 for
+    bf16, 1 for fp8.
     Split: the largest power of two <= 8 with heads * SP <= grid and, in the fast mode, SP * (hs + 2) <= seq_len, in
     the exact mode hs / SP a multiple of 4 (the exact mode splits only head sizes >= 128 unless asked); a
     KLLM_ATTN_SPLIT power of two up to that cap replaces it.  V tile: stage / ((hs / SP) * elem) & ~31 in the exact
     mode (V slices of hs / SP dims), stage / (hs * elem) & ~31 in the fast mode."""
-    int8 = shape.group_size != 0
     fast = numerics == "fast"
-    bf16 = kv_cache == "bf16"
     hs = shape.head_size
-    small_stages = fast and not bf16 and 2 * shape.dim * 4 <= 16 * 1024
-    stage = int(env.get("KLLM_STAGE_BYTES", 27 * 1024 if int8 else 16 * 1024 if small_stages else 32 * 1024))
-    stage = (stage + 127) & ~127
-    esz = 2 if bf16 else 4
+    stage = stage_bytes(shape, numerics, env, kv_cache, weight_format)
+    esz = KV_ELEM_BYTES[kv_cache]
     T = min(stage // (hs * esz), 8 * 32) & ~31
     grid = min(sms, shape.dim, shape.hidden_dim)
     cap = 1
@@ -129,6 +150,15 @@ def edge_ends(T, SP, seq_len):
     return sorted(p for p in e if 0 <= p < seq_len)
 
 
+def continue_ends(T, n, seq_len):
+    """Segment ends of a decode that continues at position n (after a prefill of n rows) across the next edge of its
+    T-timestep tiles."""
+    edge = (n // T + 1) * T
+    ends = sorted(p for p in {n, n + 1, edge - 1, edge, edge + 1} if n <= p < seq_len)
+    assert ends[-1] >= edge, (T, n, seq_len)
+    return ends
+
+
 def sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
@@ -151,6 +181,9 @@ GEOMETRIES = {
     "qwen2.5-reduced": ModelShape("qwen2.5-reduced", 896, 4864, 2, 14, 2, 4096, 16384, True,
                                   flavour="qwen2"),  # T = 64
     "tinyllama-1.1b": replace(SHAPES["tinyllama-1.1b"], seq_len=1024),  # T = 64
+    # head_size 64, four query heads per KV head: the smallest head the fp8 cache's tile mapping takes (one 16-byte K
+    # chunk per lane quarter); the reduced-precision caches' cases only
+    "gqa-hs64": ModelShape("decode-gqa-hs64", 256, 688, 2, 4, 1, 1024, 1100),
 }
 # (geometry, weights, environment of the fast mode)
 CASES = [("hs16", "loud", {}), ("small", "synth", {}), ("small", "loud", {}), ("small-hs48", "loud", {}),

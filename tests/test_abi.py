@@ -74,33 +74,29 @@ def test_argument_validation_without_device(kllm_lib):
 def test_every_megakernel_instantiation_keeps_its_state_out_of_local_memory(kllm_lib):
     """The persistent kernel's ring takes the whole unified L1, so a local-memory access is a round trip to L2
     (DESIGN.md 5.2, "No local memory").  The library holds exactly the decode_megakernel<F, KV, LP, PROF>
-    instantiations of the table -- {fp32, int8, bf16} weights x {fp32, bf16, fp8} caches x {plain, log-probabilities},
-    plus the profiling kernels of fp32 and int8 weights over the fp32 cache -- and every one of them carries no
-    parameter copy on the stack (it was 456 bytes before the parameters became __grid_constant__) and only a handful of
-    local loads / stores (per-token spills and the cold trap-message path), is fed by TMA bulk copies on mbarriers, and
-    with the fp8 cache widens and encodes e4m3 in hardware.  The plain fp32 and int8 kernels over the fp32 cache keep
-    the row loops' register budget.  nvcc / ptxas regressions of that kind show up here, on the CPU."""
+    instantiations of tests/megakernel_table.py -- {fp32, int8, bf16} weights x {fp32, bf16, fp8} caches x {plain,
+    log-probabilities}, plus the profiling kernels of fp32 and int8 weights over the fp32 cache -- and every one of
+    them carries no parameter copy on the stack (it was 456 bytes before the parameters became __grid_constant__) and
+    only a handful of local loads / stores (per-token spills and the cold trap-message path), is fed by TMA bulk copies
+    on mbarriers, and with the fp8 cache widens and encodes e4m3 in hardware.  The plain fp32 and int8 kernels over the
+    fp32 cache keep the row loops' register budget.  nvcc / ptxas regressions of that kind show up here, on the CPU."""
+    from megakernel_table import TABLE, symbol
     from kuiperllama_b200 import build as kbuild
     lib = str(kbuild.LIB)
     res = subprocess.run(["cuobjdump", "-res-usage", lib], capture_output=True, text=True, check=True).stdout
     usage = {m.group(1): (int(m.group(2)), int(m.group(3)))
              for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+)", res)}
-    F32, INT8, BF16 = 0, 1, 2  # WeightFormat
-    KV_F32, KV_FP8 = 0, 2      # kllm_decoder_desc::kv_cache
-    table = [(f, kv, lp, 0) for f in (F32, INT8, BF16) for kv in (0, 1, 2) for lp in (0, 1)] + \
-            [(f, KV_F32, 0, 1) for f in (F32, INT8)]
-    name = {t: "_ZN4kllm4mega17decode_megakernelILNS_12WeightFormatE{}ELi{}ELb{}ELb{}EEEvNS0_6ParamsE".format(*t)
-            for t in table}
+    name = {t: symbol(*t) for t in TABLE}
     assert len(name) == 20
     assert sorted(k for k in usage if "megakernel" in k) == sorted(name.values())
     for (f, kv, lp, prof), n in name.items():
         regs, stack = usage[n]
         assert stack <= 64, f"{n}: {stack} bytes of stack (a parameter copy or a local array is back)"
-        if f != BF16 and kv == KV_F32 and not lp and not prof:
+        if f != "bf16" and kv == "fp32" and not lp and not prof:
             assert regs <= 168, (n, regs)
         sass = subprocess.run(["cuobjdump", "-sass", "-fun", n, lib], capture_output=True, text=True, check=True).stdout
         local = len(re.findall(r"\b(?:LDL|STL)\b", sass))
         assert local <= 32, f"{n}: {local} local-memory instructions"
         assert "UBLKCP" in sass and "SYNCS" in sass, n  # TMA bulk copies + mbarriers are what feeds the ring
-        if kv == KV_FP8:
+        if kv == "fp8":
             assert "F2FP.F16.E4M3.UNPACK_B" in sass and "SATFINITE.E4M3" in sass, n  # hardware e4m3 conversions

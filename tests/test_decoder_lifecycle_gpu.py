@@ -32,7 +32,7 @@ import pytest
 import torch
 
 from decode_model_util import (GEOMETRIES, KV_TAU, KV_TAU_FIRST, LOGIT_TAU, WEIGHTS, device_sincos, edge_ends, fmt,
-                               kv_ratios, logit_ratio, make_decoder, same_bits, sequence)
+                               kv_ratios, logit_ratio, make_decoder, same_bits, sequence, stage_bytes)
 from kv_bf16_model import bf16_rne, prefill_ref_bf16
 from prefill_model import prefill_ref
 from test_kv_bf16_gpu import ulp_bf16
@@ -62,12 +62,10 @@ def mega_smem_bytes(shape, numerics, kv_cache="fp32", env=None, max_smem=H100_SM
     up to 128; stages: as many as fit max_smem - xbuf - xres - 3584, at most 16.  Both rings fill that budget to
     within one stage, so the remainder decides which of two models asks for more."""
     env = env or {}
-    int8, fast = shape.group_size != 0, numerics == "fast"
+    fast = numerics == "fast"
     dim, hs = shape.dim, shape.head_size
     xbuf = max(max(dim, shape.hidden_dim, shape.head_num * hs) * 4, 2 * hs * 4)
-    small_stages = fast and kv_cache == "fp32" and 2 * dim * 4 <= 16 * 1024
-    stage = int(env.get("KLLM_STAGE_BYTES", 27 * 1024 if int8 else 16 * 1024 if small_stages else 32 * 1024))
-    stage = (stage + 127) & ~127
+    stage = stage_bytes(shape, numerics, env, kv_cache)
     if fast:
         xbuf = max(xbuf, (2 * hs + 8 * (hs + 2)) * 4)
     xbuf = (max(xbuf, DRAW_SCRATCH + 64 * 8, LOGPROB_SCRATCH) + 127) & ~127

@@ -1,7 +1,8 @@
 """-m gpu: the bf16 KV cache (kllm_decoder_desc::kv_cache = KLLM_KV_BF16) of the fast decode mode.
 
 Against the fp64 model (tests/kv_bf16_model.py, rule "decode"), teacher-forced over every position of the decode-model
-cases whose head size the bf16 tile mapping takes (head_size % 32 == 0), at the flash geometry's tile and split edges.
+cases whose head size the bf16 tile mapping takes (head_size % 32 == 0), and of bf16 weights at their own ring stage
+(the model fed the weights widened to fp32), at the flash geometry's tile and split edges.
 The model is fed the GPU's own cache rows (kv_rows): each position attends over the rows the decoder cached, which
 isolates the kernel from the rounding -- a row whose fp32 value lies on the other side of a rounding boundary on the
 GPU than in the model differs by one ulp, and with sharp attention that moves every later row of the next layers by
@@ -13,8 +14,9 @@ far more than the fp32 bound.  Then:
     bf16 model's from the fp32 one (triangle inequality); the factor covers the rows where the GPU's fp32 value lies
     on the other side of a bf16 rounding boundary than the model's (one ulp).
 Entries: prompt, generate and generate_until equal stepping bit for bit; sampled and penalised ids follow the rule of
-kuiperllama_b200/sampling.py on the bf16 decoder's logits; both batched prefills write bf16 rows within their bounds and
-decode continues from them; score and logprobs run; Llama-2-7B int8 at seq_len 4096 decoding past position 4000 agrees
+kuiperllama_b200/sampling.py on the bf16 decoder's logits; both batched prefills write bf16 rows within their bounds,
+and decode continues from them across a tile edge within the fast-mode bound of the model; Llama-2-7B int8 at seq_len
+4096 decoding past position 4000 agrees
 with the fp32 cache; the cache takes half the memory; every refusal of kllm_decoder_create.
 
 Measured worst values (an NVIDIA H100 80GB HBM3 at a 700 W power limit) are printed with the [kv-bf16] tag.
@@ -26,42 +28,56 @@ import numpy as np
 import pytest
 import torch
 
-from decode_model_util import (CASES, GEOMETRIES, KNOBS, WEIGHTS, case_id, device_sincos, engine_geometry, sequence, sms,
-                               taus)
+from decode_model_util import (CASES, GEOMETRIES, KNOBS, LOGIT_TAU, WEIGHTS, case_id, continue_ends, device_sincos,
+                               engine_geometry, sequence, sms, taus)
 from kv_bf16_model import bf16_rne, prefill_ref_bf16
 from prefill_model import prefill_ref
 
 from kuiperllama_b200 import ALLREDUCE_FN, SHAPES, Decoder, KllmError, synth_weights
 from kuiperllama_b200 import sampling as ref_sampling
+from kuiperllama_b200.decoder import bf16_weights, widen_weights
 
 pytestmark = pytest.mark.gpu
 
 # Measured worst values, an NVIDIA H100 80GB HBM3 at 700 W: K / V err / (ulp + KV_TAU rms) 0.999 (tinyllama-1.1b);
 # logits err / fast-mode bound against the model on the GPU's rows 0.228 (tinyllama-1.1b); distance from the fp32-cache
-# model over the bf16 model's own distance 1.01 (small-loud, KLLM_ATTN_SPLIT=2), against BF16_GAIN.
+# model over the bf16 model's own distance 1.01 (small-loud, KLLM_ATTN_SPLIT=2), against BF16_GAIN.  bf16 weights at
+# their own 24 KB stage (same card and limit): K / V 0.997 (hs128), logits 0.0931 (gqa-hs64, KLLM_ATTN_SPLIT=4),
+# distance 1.00 of the bf16 model's own (hs128).  Decode after the batched prefill, logits err / fast-mode bound:
+# 0.0244 (small-int8), 0.014 (small).
 BF16_GAIN = 2.0
-BF16_CASES = [c for c in CASES if GEOMETRIES[c[0]].head_size % 32 == 0]
+# (geometry, weights, environment, weight format)
+BF16_CASES = [c + ("int8" if GEOMETRIES[c[0]].group_size else "fp32",) for c in CASES
+              if GEOMETRIES[c[0]].head_size % 32 == 0]
 # tile and split geometries of the bf16 cache: a smaller ring stage and a smaller split on one case each
-BF16_CASES += [("hs128", "loud", {"KLLM_STAGE_BYTES": "8192"}), ("small", "loud", {"KLLM_ATTN_SPLIT": "2"}),
-               ("llama2-7b-int8-2l", "outliers", {"KLLM_STAGE_BYTES": "16384", "KLLM_ATTN_SPLIT": "2"})]
+BF16_CASES += [("hs128", "loud", {"KLLM_STAGE_BYTES": "8192"}, "fp32"),
+               ("small", "loud", {"KLLM_ATTN_SPLIT": "2"}, "fp32"),
+               ("llama2-7b-int8-2l", "outliers", {"KLLM_STAGE_BYTES": "16384", "KLLM_ATTN_SPLIT": "2"}, "int8")]
+# bf16 weights at their 24 KB stages: T = 96 at hs 128, T = 192 at hs 64 (a split of 4 puts SP * T inside the sequence)
+BF16_CASES += [("hs128", "loud", {}, "bf16"), ("gqa-hs64", "loud", {}, "bf16"),
+               ("gqa-hs64", "loud", {"KLLM_ATTN_SPLIT": "4"}, "bf16")]
 
 
 def report(*parts):
     print("[kv-bf16]", *parts, flush=True)
 
 
-def make(monkeypatch, shape, w, env=None, kv_cache="bf16", numerics="fast"):
+def bf16_id(c):
+    return case_id(c[:3]) + ("-bf16w" if c[3] == "bf16" else "")
+
+
+def make(monkeypatch, shape, w, env=None, kv_cache="bf16", numerics="fast", weight_format="fp32"):
     for name in KNOBS:
         monkeypatch.delenv(name, raising=False)
     for name, value in (env or {}).items():
         monkeypatch.setenv(name, value)
-    return Decoder(shape, w, numerics=numerics, kv_cache=kv_cache)
+    return Decoder(shape, w, numerics=numerics, kv_cache=kv_cache, weight_format=weight_format)
 
 
-def bf16_geometry(shape, env):
-    """(T, SP) of the flash form with a bf16 cache: T = min(stage / (hs * 2), 256) & ~31; the split as fp32's
-    (decode_model_util.engine_geometry)."""
-    return engine_geometry(shape, "fast", env, sms(), "bf16")[:2]
+def bf16_geometry(shape, env, weight_format="fp32"):
+    """(T, SP) of the flash form with a bf16 cache (decode_model_util.engine_geometry): the weight format's stage,
+    T = min(stage / (hs * 2), 256) & ~31, the split as fp32's."""
+    return engine_geometry(shape, "fast", env, sms(), "bf16", weight_format)[:2]
 
 
 def ends_for(T, SP, seq_len):
@@ -75,17 +91,22 @@ def ulp_bf16(x):
     return torch.pow(2.0, e - 7)
 
 
-@pytest.mark.parametrize("key,weights,env", BF16_CASES, ids=[case_id(c) for c in BF16_CASES])
-def test_bf16_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env):
+@pytest.mark.parametrize("key,weights,env,weight_format", BF16_CASES, ids=[bf16_id(c) for c in BF16_CASES])
+def test_bf16_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env, weight_format):
     shape = GEOMETRIES[key]
-    decode_against_the_bf16_model(kllm_lib, monkeypatch, case_id((key, weights, env)), shape,
-                                  WEIGHTS[weights](shape, "cuda", 77), env, *taus(key))
+    w = WEIGHTS[weights](shape, "cuda", 77)
+    w_dec = bf16_weights(w) if weight_format == "bf16" else None
+    decode_against_the_bf16_model(kllm_lib, monkeypatch, bf16_id((key, weights, env, weight_format)), shape,
+                                  w if w_dec is None else widen_weights(w_dec), env, *taus(key), w_dec=w_dec)
 
 
-def decode_against_the_bf16_model(kllm_lib, monkeypatch, what, shape, w, env, kv_tau, logit_tau, tag="[kv-bf16]"):
+def decode_against_the_bf16_model(kllm_lib, monkeypatch, what, shape, w, env, kv_tau, logit_tau, tag="[kv-bf16]",
+                                  w_dec=None):
     """One bf16-cache decoder teacher-forced over every position in segments ending on the edges of the tiles it
-    reports (which must be bf16_geometry's), held to the bounds of the module docstring."""
-    T, SP = bf16_geometry(shape, env)
+    reports (which must be bf16_geometry's), held to the bounds of the module docstring.  w_dec: bf16 weights for the
+    decoder (decoder.bf16_weights), w then being their widening; None runs the decoder over w."""
+    weight_format = "fp32" if w_dec is None else "bf16"
+    T, SP = bf16_geometry(shape, env, weight_format)
     ends = ends_for(T, SP, shape.seq_len)
     toks = sequence(shape.vocab_size, shape.seq_len, 5)
     sin, cos = device_sincos(kllm_lib, shape)
@@ -93,9 +114,10 @@ def decode_against_the_bf16_model(kllm_lib, monkeypatch, what, shape, w, env, kv
     model = prefill_ref_bf16(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends, fixed_point=fixed,
                              rule="decode")
     plain = prefill_ref(w, shape, toks, 0, sin, cos, tf32=False, logits_at=ends, fixed_point=fixed)
-    dec = make(monkeypatch, shape, w, env)
+    dec = make(monkeypatch, shape, w if w_dec is None else w_dec, env, weight_format=weight_format)
     assert dec.engine == "persistent"
-    assert dec.attention_geometry == engine_geometry(shape, "fast", env, sms(), "bf16"), (what, dec.attention_geometry)
+    assert dec.attention_geometry == engine_geometry(shape, "fast", env, sms(), "bf16", weight_format), \
+        (what, dec.attention_geometry)
     start, logits = 0, {}
     for end in ends:
         dec.generate(0, start, end + 1 - start, teacher=toks[start:end + 1])
@@ -215,22 +237,24 @@ def test_batched_prefill_writes_bf16_rows_and_decode_continues(kllm_lib, monkeyp
     assert worst <= 1.0
     lg = torch.from_numpy(dec.logits()).cuda().double()
     assert float((lg - model["logits"]).abs().max()) <= 2e-2 * float(model["logits"].abs().max())
-    ids = dec.generate(nxt, n, 20)  # decode continues over the prefilled bf16 rows
-    assert len(ids) == 20 and all(0 <= i < shape.vocab_size for i in ids)
-    dec.close()
-
-
-def test_score_and_logprobs_run(kllm_lib, monkeypatch, small):
-    shape, w = small
-    toks = sequence(shape.vocab_size, 80, 8)
-    dec = make(monkeypatch, shape, w)
-    dec.set_logprobs(3)
-    lp = dec.score(toks)
-    assert len(lp) == len(toks) - 1 and np.all(np.isfinite(lp)) and np.all(np.asarray(lp) <= 0)
-    nxt = dec.prompt(toks)
-    dec.generate(nxt, len(toks), 8)
-    rec = dec.logprobs(len(toks), 8)
-    assert all(i >= 0 for i in rec[0])
+    # decode continues over the prefilled bf16 rows, teacher-forced across the next tile edge: each segment end's logits
+    # within the fast-mode bound of the model attending over the GPU's prefilled rows (kv_in) and decoded rows (kv_rows)
+    assert dec.attention_geometry == engine_geometry(shape, "fast", {}, sms(), "bf16"), dec.attention_geometry
+    ends = continue_ends(dec.attention_geometry[0], n, shape.seq_len)
+    more = sequence(shape.vocab_size, ends[-1] + 1 - n, 16)
+    start, logits = n, {}
+    for end in ends:
+        dec.generate(0, start, end + 1 - start, teacher=more[start - n:end + 1 - n])
+        logits[end] = torch.from_numpy(dec.logits()).cuda().double()
+        start = end + 1
+    k, v = (torch.from_numpy(a).cuda() for a in dec.kv_cache())
+    fed = prefill_ref_bf16(w, shape, more, n, sin, cos, tf32=False, logits_at=[e - n for e in ends],
+                           fixed_point=shape.group_size == 64, rule="decode", kv_in=(k, v),
+                           kv_rows=(k[:, n:], v[:, n:]))
+    worst = max(float((logits[e] - fed["logits_at"][e - n]).abs().max())
+                / (LOGIT_TAU * float(fed["logits_at"][e - n].pow(2).mean().sqrt())) for e in ends)
+    report(f"{key} decode after the prefill, segments {ends}: logits err / fast bound {worst:.3g}")
+    assert worst <= 1.0
     dec.close()
 
 

@@ -1,9 +1,10 @@
 """-m gpu: the fp8 KV cache (kllm_decoder_desc::kv_cache = KLLM_KV_FP8) of the fast decode mode.
 
-Against the fp64 model (tests/kv_fp8_model.py, rule "decode"), teacher-forced over every position of the decode-model
-cases whose head size the fp8 tile mapping takes (head_size % 64 == 0) and a small hs-64 GQA shape, with unit scales
-and with scales calibrated on the model's fp32 rows (decoder.fp8_kv_scales), at the flash geometry's tile and split
-edges and at smaller stages and splits.  As in tests/test_kv_bf16_gpu.py the model is fed the GPU's own cache rows
+Against the fp64 model (tests/kv_fp8_model.py, rule "decode"), teacher-forced over every position of decode-model
+geometries whose head size the fp8 tile mapping takes (head_size % 64 == 0), with fp32, int8 and bf16 weights (the
+model fed bf16 weights widened to fp32, and the int8 decode step's fixed point), with unit scales and with scales
+calibrated on the model's fp32 rows (decoder.fp8_kv_scales), at the flash geometry's tile and split edges and at
+smaller stages and splits.  As in tests/test_kv_bf16_gpu.py the model is fed the GPU's own cache rows
 (kv_rows), so each position attends over the rows the decoder cached.  Then:
   - every read_kv element is within one e4m3 ulp (at its magnitude, times its scale) plus KV_TAU * rms(row) of the
     model's rounded row, and where the model's scaled value lies farther than that tolerance from an e4m3 rounding
@@ -12,12 +13,19 @@ edges and at smaller stages and splits.  As in tests/test_kv_bf16_gpu.py the mod
   - and within FP8_GAIN x the fp8 model's own distance from the fp32-cache model, plus that bound, of the fp32-cache
     model.
 Entries: prompt, generate and generate_until equal stepping bit for bit; sampled and penalised ids follow
-kuiperllama_b200/sampling.py on the decoder's logits; both batched prefills write fp8 rows and decode continues from
-them; score and logprobs run; bf16 weights over the fp8 cache equal fp32 weights over the widened ones bit for bit;
-Llama-2-7B int8 at seq_len 4096 agrees with the fp32 cache past position 4000; the cache takes a quarter of the
-memory; every refusal; the C++ host against the C ABI.
+kuiperllama_b200/sampling.py on the decoder's logits; both batched prefills write fp8 rows, and decode continues from
+them across a tile edge within the fast-mode bound of the model; bf16 weights over the fp8 cache equal fp32 weights
+over the widened ones bit for bit; Llama-2-7B int8 at seq_len 4096 agrees with the fp32 cache past position 4000; the
+cache takes a quarter of the memory; every refusal; the C++ host against the C ABI.
 
-Measured worst values (an NVIDIA H100 80GB HBM3 at a 700 W power limit) are printed with the [kv-fp8] tag.
+Measured worst values (an NVIDIA H100 80GB HBM3 at a 700 W power limit) are printed with the [kv-fp8] tag.  Of the
+int8-weight cases: K / V err / (ulp + KV_TAU rms) 1.00 (llama2-7b-int8-2l, one ulp where the GPU's fp32 value and the
+model's lie on either side of a rounding boundary), logits err / fast-mode bound 0.0575 (llama2-7b-int8-2l,
+calibrated), distance from the fp32-cache model 1.00 of the fp8 model's own (FP8_GAIN 2).  Of the bf16-weight cases:
+K / V 1.00 (hs128), logits 0.0659 (hs128, calibrated), distance 1.00 of the fp8 model's own.  Decode after the
+batched prefill, logits err / fast-mode bound: 0.0233 (small-int8), 0.0102 (prefill-hs64).  These int8- and
+bf16-weight cases, the bf16 cache's bf16-weight cases and the log-probability kernel pairs of test_logprobs_gpu.py
+take about 7 s together on that card.
 """
 import ctypes
 from dataclasses import replace
@@ -26,7 +34,8 @@ import numpy as np
 import pytest
 import torch
 
-from decode_model_util import GEOMETRIES, KNOBS, WEIGHTS, case_id, device_sincos, sequence, sms, taus
+from decode_model_util import (GEOMETRIES, KNOBS, LOGIT_TAU, WEIGHTS, case_id, continue_ends, device_sincos,
+                               engine_geometry, sequence, sms, taus)
 from kv_fp8_model import e4m3_rne, fp8_round_rows, prefill_ref_fp8
 from prefill_model import prefill_ref
 
@@ -40,17 +49,25 @@ FP8_GAIN = 2.0
 # Llama-2-7B int8 past position 4000: |fp8 - fp32 cache| / max|logit|, measured 0.175 (the bf16 cache: 0.013) on an
 # NVIDIA H100 80GB HBM3 at 700 W
 LONG_BOUND = 0.3
-# head_size 64, four query heads per KV head: the smallest head the fp8 tile mapping takes (one 16-byte K chunk per
-# lane quarter), T = 256
-GEOMETRIES_FP8 = dict(GEOMETRIES, **{"gqa-hs64": ModelShape("decode-gqa-hs64", 256, 688, 2, 4, 1, 1024, 1100)})
-FP8_CASES = [(key, weights, env, calibrated)
+# (geometry, weights, environment, calibrated scales, weight format)
+FP8_CASES = [(key, weights, env, calibrated, "fp32")
              for key, weights, env in [("hs128", "loud", {}), ("qwen2.5-reduced", "synth", {}),
                                        ("llama3-reduced", "loud", {}), ("gqa-hs64", "loud", {})]
              for calibrated in (False, True)]
 # smaller stages and splits: T = 64 at hs128, and a split of 2
-FP8_CASES += [("hs128", "loud", {"KLLM_STAGE_BYTES": "8192"}, True), ("gqa-hs64", "loud", {"KLLM_ATTN_SPLIT": "2"}, True),
-              ("gqa-hs64", "loud", {"KLLM_STAGE_BYTES": "4096", "KLLM_ATTN_SPLIT": "4"}, False)]
-assert all(GEOMETRIES_FP8[c[0]].head_size % 64 == 0 for c in FP8_CASES)
+FP8_CASES += [("hs128", "loud", {"KLLM_STAGE_BYTES": "8192"}, True, "fp32"),
+              ("gqa-hs64", "loud", {"KLLM_ATTN_SPLIT": "2"}, True, "fp32"),
+              ("gqa-hs64", "loud", {"KLLM_STAGE_BYTES": "4096", "KLLM_ATTN_SPLIT": "4"}, False, "fp32")]
+# int8 weights at their 27 KB stages: T = 256 at hs 64 and T = 192 at hs 128 (Llama-2-7B int8's tile over this cache);
+# a split of 2 puts the split edge SP * T inside the sequence
+FP8_CASES += [(key, "outliers", {}, calibrated, "int8")
+              for key in ("small-int8", "llama2-7b-int8-2l") for calibrated in (False, True)]
+FP8_CASES += [("small-int8", "outliers", {"KLLM_ATTN_SPLIT": "2"}, False, "int8"),
+              ("llama2-7b-int8-2l", "outliers", {"KLLM_ATTN_SPLIT": "2"}, True, "int8")]
+# bf16 weights at their 24 KB stages: T = 192 at hs 128, T = 256 at hs 64
+FP8_CASES += [(key, "loud", {}, calibrated, "bf16") for key in ("hs128", "gqa-hs64") for calibrated in (False, True)]
+FP8_CASES += [("hs128", "loud", {"KLLM_ATTN_SPLIT": "4"}, True, "bf16")]
+assert all(GEOMETRIES[c[0]].head_size % 64 == 0 for c in FP8_CASES)
 
 
 def report(*parts):
@@ -58,7 +75,7 @@ def report(*parts):
 
 
 def fp8_id(c):
-    return case_id(c[:3]) + ("-calibrated" if c[3] else "-unit")
+    return case_id(c[:3]) + ("-calibrated" if c[3] else "-unit") + ("-bf16w" if c[4] == "bf16" else "")
 
 
 def make(monkeypatch, shape, w, env=None, kv_cache="fp8", numerics="fast", **kw):
@@ -69,23 +86,19 @@ def make(monkeypatch, shape, w, env=None, kv_cache="fp8", numerics="fast", **kw)
     return Decoder(shape, w, numerics=numerics, kv_cache=kv_cache, **kw)
 
 
-def fp8_geometry(shape, env):
-    """(T, SP, T_v, stage) of the flash form with an fp8 cache: stage KLLM_STAGE_BYTES, else 27 KB for int8 and 32 KB
-    (never the fp32 cache's 16 KB), rounded up to 128 bytes; T = min(stage / hs, 256) & ~31 and T_v the same; the
-    split as fp32's (decode_model_util.engine_geometry)."""
-    hs = shape.head_size
-    stage = int(env.get("KLLM_STAGE_BYTES", 27 * 1024 if shape.group_size else 32 * 1024))
-    stage = (stage + 127) & ~127
-    T = min(stage // hs, 256) & ~31
-    grid = min(sms(), shape.dim, shape.hidden_dim)
-    cap = 1
-    while cap * 2 <= 8 and shape.head_num * cap * 2 <= grid and cap * 2 * (hs + 2) <= shape.seq_len:
-        cap *= 2
-    sp = cap
-    asked = int(env.get("KLLM_ATTN_SPLIT", 0))
-    if 1 <= asked <= cap and (asked & (asked - 1)) == 0:
-        sp = asked
-    return T, sp, (stage // hs) & ~31, stage
+def fp8_geometry(shape, env, weight_format="fp32"):
+    """(T, SP, T_v, stage) of the flash form with an fp8 cache (decode_model_util.engine_geometry): the weight
+    format's stage, T = min(stage / hs, 256) & ~31 and T_v the same, the split as fp32's."""
+    return engine_geometry(shape, "fast", env, sms(), "fp8", weight_format)
+
+
+def case_weights(shape, weights, weight_format):
+    """(the decoder's weights, the model's): bf16 weights and their exact fp32 widening, else the same dict."""
+    w = WEIGHTS[weights](shape, "cuda", 77)
+    if weight_format != "bf16":
+        return w, w
+    w16 = bf16_weights(w)
+    return w16, widen_weights(w16)
 
 
 def ends_for(T, SP, seq_len):
@@ -106,13 +119,13 @@ def per_head(scales, which, L, kvh, hs, device):
     return s.repeat_interleave(hs, dim=1).reshape(L, 1, kvh * hs)
 
 
-@pytest.mark.parametrize("key,weights,env,calibrated", FP8_CASES, ids=[fp8_id(c) for c in FP8_CASES])
-def test_fp8_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env, calibrated):
-    shape = GEOMETRIES_FP8[key]
-    w = WEIGHTS[weights](shape, "cuda", 77)
+@pytest.mark.parametrize("key,weights,env,calibrated,weight_format", FP8_CASES, ids=[fp8_id(c) for c in FP8_CASES])
+def test_fp8_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env, calibrated, weight_format):
+    shape = GEOMETRIES[key]
+    w_dec, w = case_weights(shape, weights, weight_format)
     kv_tau, logit_tau = taus(key)
-    what = fp8_id((key, weights, env, calibrated))
-    T, SP = fp8_geometry(shape, env)[:2]
+    what = fp8_id((key, weights, env, calibrated, weight_format))
+    T, SP = fp8_geometry(shape, env, weight_format)[:2]
     ends = ends_for(T, SP, shape.seq_len)
     toks = sequence(shape.vocab_size, shape.seq_len, 5)
     sin, cos = device_sincos(kllm_lib, shape)
@@ -123,9 +136,10 @@ def test_fp8_decode_against_the_model(kllm_lib, monkeypatch, key, weights, env, 
               else np.ones((2, L, kvh), np.float32))
     model = prefill_ref_fp8(w, shape, toks, 0, sin, cos, scales=scales, tf32=False, logits_at=ends, fixed_point=fixed,
                             rule="decode")
-    dec = make(monkeypatch, shape, w, env, kv_scales=scales if calibrated else None)
+    dec = make(monkeypatch, shape, w_dec, env, kv_scales=scales if calibrated else None,
+               weight_format="bf16" if weight_format == "bf16" else "fp32")
     assert dec.engine == "persistent"
-    assert dec.attention_geometry == fp8_geometry(shape, env), (what, dec.attention_geometry)
+    assert dec.attention_geometry == fp8_geometry(shape, env, weight_format), (what, dec.attention_geometry)
     start, logits = 0, {}
     for end in ends:
         dec.generate(0, start, end + 1 - start, teacher=toks[start:end + 1])
@@ -268,22 +282,23 @@ def test_batched_prefill_writes_fp8_rows_and_decode_continues(kllm_lib, monkeypa
     lg = torch.from_numpy(dec.logits()).cuda().double()
     report(f"{key} prefill logits err / max|logit| {float((lg - model['logits']).abs().max()) / float(model['logits'].abs().max()):.3g}")
     assert float((lg - model["logits"]).abs().max()) <= 2e-2 * float(model["logits"].abs().max())
-    ids = dec.generate(nxt, n, 20)  # decode continues over the prefilled fp8 rows
-    assert len(ids) == 20 and all(0 <= i < shape.vocab_size for i in ids)
-    dec.close()
-
-
-def test_score_and_logprobs_run(kllm_lib, monkeypatch, small):
-    shape, w = small
-    toks = sequence(shape.vocab_size, 80, 8)
-    dec = make(monkeypatch, shape, w)
-    dec.set_logprobs(3)
-    lp = dec.score(toks)
-    assert len(lp) == len(toks) - 1 and np.all(np.isfinite(lp)) and np.all(np.asarray(lp) <= 0)
-    nxt = dec.prompt(toks)
-    dec.generate(nxt, len(toks), 8)
-    rec = dec.logprobs(len(toks), 8)
-    assert all(i >= 0 for i in rec[0])
+    # decode continues over the prefilled fp8 rows, teacher-forced across the next tile edge: each segment end's logits
+    # within the fast-mode bound of the model attending over the GPU's prefilled rows (kv_in) and decoded rows (kv_rows)
+    assert dec.attention_geometry == fp8_geometry(shape, {}), dec.attention_geometry
+    ends = continue_ends(dec.attention_geometry[0], n, shape.seq_len)
+    more = sequence(shape.vocab_size, ends[-1] + 1 - n, 16)
+    start, logits = n, {}
+    for end in ends:
+        dec.generate(0, start, end + 1 - start, teacher=more[start - n:end + 1 - n])
+        logits[end] = torch.from_numpy(dec.logits()).cuda().double()
+        start = end + 1
+    k, v = (torch.from_numpy(a).cuda() for a in dec.kv_cache())
+    fed = prefill_ref_fp8(w, shape, more, n, sin, cos, scales=scales, tf32=False, logits_at=[e - n for e in ends],
+                          fixed_point=shape.group_size == 64, rule="decode", kv_in=(k, v), kv_rows=(k[:, n:], v[:, n:]))
+    worst = max(float((logits[e] - fed["logits_at"][e - n]).abs().max())
+                / (LOGIT_TAU * float(fed["logits_at"][e - n].pow(2).mean().sqrt())) for e in ends)
+    report(f"{key} decode after the prefill, segments {ends}: logits err / fast bound {worst:.3g}")
+    assert worst <= 1.0
     dec.close()
 
 
@@ -368,7 +383,7 @@ def rc_of(fn):
 
 @pytest.mark.parametrize("what", ["exact", "mode-env-exact", "engine-graph", "tp2", "hs32", "hs48", "hs16", "hs256"])
 def test_refusals(kllm_lib, monkeypatch, what):
-    shape, env, kw = GEOMETRIES_FP8["gqa-hs64"], {}, {}
+    shape, env, kw = GEOMETRIES["gqa-hs64"], {}, {}
     if what == "exact":
         kw["numerics"] = "exact"
     elif what == "mode-env-exact":

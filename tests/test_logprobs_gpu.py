@@ -1,13 +1,23 @@
 """-m gpu: log-probabilities (kllm_logprobs_f32, kllm_decoder_set_logprobs / _read_logprobs / _score) against the
 numpy mirror of kuiperllama_b200/sampling.py, on both engines.  Each record entry is checked against the mirror
 applied to the logits obtained by stepping the same positions (kllm_decoder_logits): top-N ids exactly, lp within
-the bound of DESIGN.md 5.8 for the engine's partition."""
+the bound of DESIGN.md 5.8 for the engine's partition.
+
+The persistent engine runs its log-probability kernel whenever they are on (set_logprobs >= 0, and every score): one
+per weight format and KV cache (tests/megakernel_table.py).  The KERNEL_PAIRS tests run each of them in the fast
+numerics, across a tile edge of its own attention geometry: not perturbing what the plain kernel decodes, records and
+score against the mirror of the plain kernel's logits."""
+from dataclasses import replace
+
 import numpy as np
 import pytest
 import torch
 
+from decode_model_util import KNOBS, engine_geometry, sequence, sms
 from gpu_util import dev, ptr, sync
-from kuiperllama_b200 import KllmError, SHAPES, check, load_library, sampling, synth_weights
+from megakernel_table import KV_CACHES, WEIGHT_FORMATS
+from kuiperllama_b200 import KllmError, SHAPES, Decoder, check, load_library, sampling, synth_weights
+from kuiperllama_b200.decoder import bf16_weights
 
 pytestmark = pytest.mark.gpu
 
@@ -290,3 +300,117 @@ def test_score_full_size_tinyllama(engine):
             m = lg.max()
             want = lg[tokens[pos + 1]] - m - np.log(np.exp(lg - m).sum())
             assert abs(lp[pos] - want) <= sampling.logprob_bound(want, k, shape.vocab_size), (pos, lp[pos], want)
+
+
+# ---- every log-probability kernel of the persistent engine ----------------------------------------------------------
+# (weight format, KV cache): every pair the persistent engine has kernels for, at small-int8's dimensions (head_size 64,
+# two query heads per KV head), the fp32 and bf16 weights built at the same dimensions without int8 groups.  Flash
+# tiles (engine_geometry): 64 / 256 / 256 timesteps for fp32 weights over the fp32 / bf16 / fp8 caches, 96 / 192 / 256
+# for int8 and for bf16 weights.
+KERNEL_PAIRS = [(f, kv) for f in WEIGHT_FORMATS for kv in KV_CACHES]
+PAIR_SHAPE = replace(SHAPES["small-int8"], seq_len=320)
+PENALISED = (0.8, 40, 0.9, 1.3)  # temperature, top-k, top-p, repetition penalty
+
+
+def pair_id(p):
+    return f"{p[0]}w-{p[1]}kv"
+
+
+@pytest.fixture(scope="module")
+def pair_weights():
+    fp32 = synth_weights(replace(PAIR_SHAPE, group_size=0), "cuda", 2024)
+    return {"fp32": fp32, "int8": synth_weights(PAIR_SHAPE, "cuda", 2024), "bf16": bf16_weights(fp32)}
+
+
+def make_pair(monkeypatch, pair_weights, weight_format, kv_cache):
+    """The persistent engine in the fast numerics with `weight_format` weights over a `kv_cache` cache (fp8 at a
+    scale of 0.02); its attention geometry must be engine_geometry's."""
+    for name in KNOBS:
+        monkeypatch.delenv(name, raising=False)
+    monkeypatch.setenv("KLLM_ENGINE", "persistent")
+    shape = PAIR_SHAPE if weight_format == "int8" else replace(PAIR_SHAPE, group_size=0)
+    sc = np.full((2, shape.layer_num, shape.kv_head_num), 0.02, np.float32) if kv_cache == "fp8" else None
+    dec = Decoder(shape, pair_weights[weight_format], numerics="fast", kv_cache=kv_cache, kv_scales=sc,
+                  weight_format="bf16" if weight_format == "bf16" else "fp32")
+    assert dec.engine == "persistent"
+    assert dec.attention_geometry == engine_geometry(shape, "fast", {}, sms(), kv_cache, weight_format), \
+        (weight_format, kv_cache, dec.attention_geometry)
+    return dec
+
+
+@pytest.mark.parametrize("weight_format,kv_cache", KERNEL_PAIRS, ids=[pair_id(p) for p in KERNEL_PAIRS])
+def test_kernel_pair_logprobs_do_not_perturb(monkeypatch, pair_weights, weight_format, kv_cache):
+    """Teacher-forced generate over the first tile and three positions past it, greedy and sampled-and-penalised (the
+    penalised classifier partials are the log-probability kernel's own branch): ids, logits, cache rows and history
+    bit-identical with log-probabilities off (the plain kernel), on without alternatives and on with 20."""
+    dec = make_pair(monkeypatch, pair_weights, weight_format, kv_cache)
+    T = dec.attention_geometry[0]
+    V = dec.shape.vocab_size
+    toks = sequence(V, T + 3, 11)
+    for temperature, top_k, top_p, theta in ((0.0, 0, 1.0, 1.0), PENALISED):
+        dec.set_sampling(temperature, top_k, 50, top_p=top_p)
+        dec.set_repetition_penalty(theta, 0)
+        out = []
+        for top_n in (-1, 0, 20):
+            dec.set_logprobs(top_n)
+            ids = dec.generate(0, 0, len(toks), teacher=toks)
+            out.append((ids, dec.logits(), *dec.kv_cache(), dec.history()))
+        for top_n, other in zip((0, 20), out[1:]):
+            what = (weight_format, kv_cache, temperature, top_n)
+            assert other[0] == out[0][0], what
+            for a, b in zip(other[1:], out[0][1:]):
+                assert (np.asarray(a).view(np.uint32) == np.asarray(b).view(np.uint32)).all(), what
+    dec.close()
+
+
+@pytest.mark.parametrize("weight_format,kv_cache", KERNEL_PAIRS, ids=[pair_id(p) for p in KERNEL_PAIRS])
+def test_kernel_pair_records_match_the_mirror(monkeypatch, pair_weights, weight_format, kv_cache):
+    """Sampled generate across the first tile edge with 5 alternatives recorded; each entry against the mirror of the
+    logits the plain kernel gives when it steps the same ids at the same positions."""
+    dec = make_pair(monkeypatch, pair_weights, weight_format, kv_cache)
+    T = dec.attention_geometry[0]
+    V = dec.shape.vocab_size
+    start, n, top_n = T - 8, 16, 5
+    dec.set_logprobs(top_n)
+    dec.set_sampling(0.9, 0, 77)
+    nxt = dec.prompt(sequence(V, start, 12))
+    ids = dec.generate(nxt, start, n)
+    rec = dec.logprobs(start, n)
+    assert (rec[0] == ids).all()
+    dec.set_logprobs(-1)
+    k = sampling.chain_persistent(V, GRID)
+    for i, lg in enumerate(stepped_logits(dec, [nxt] + ids[:-1], start)):
+        check_entry(lg, k, rec[0][i], rec[1][i], rec[2][i], rec[3][i], top_n, (weight_format, kv_cache, start + i))
+    dec.close()
+
+
+@pytest.mark.parametrize("weight_format,kv_cache", KERNEL_PAIRS, ids=[pair_id(p) for p in KERNEL_PAIRS])
+def test_kernel_pair_score_matches_teacher_stepping(monkeypatch, pair_weights, weight_format, kv_cache):
+    """score over the first tile and past its edge, sampled and penalised settings in force (no effect on scoring):
+    each value and its alternatives against the mirror of the plain kernel's stepped logits, and the cache rows bit for
+    bit those prompt writes over the same tokens."""
+    dec = make_pair(monkeypatch, pair_weights, weight_format, kv_cache)
+    T = dec.attention_geometry[0]
+    V = dec.shape.vocab_size
+    tokens = sequence(V, T + 4, 4)
+    n = len(tokens) - 1
+    dec.set_sampling(0.8, 40, 9)
+    dec.set_repetition_penalty(1.3, 0)
+    dec.set_logprobs(6)
+    lp = dec.score(tokens)
+    assert lp.shape == (n,)
+    ids, rlp, ti, tl = dec.logprobs(0, n)
+    assert (ids == tokens[1:]).all() and (bits(rlp) == bits(lp)).all()
+    kv_score = dec.kv_cache()
+    dec.set_logprobs(-1)
+    dec.set_sampling(0.0)
+    dec.set_repetition_penalty(1.0)
+    k = sampling.chain_persistent(V, GRID)
+    for pos, lg in enumerate(stepped_logits(dec, tokens[:n], 0)):
+        check_entry(lg, k, tokens[pos + 1], lp[pos], ti[pos], tl[pos], 6, (weight_format, kv_cache, pos))
+    fresh = make_pair(monkeypatch, pair_weights, weight_format, kv_cache)
+    fresh.prompt(tokens[:n])
+    for a, b in zip(kv_score, fresh.kv_cache()):
+        assert (a[:, :n].view(np.uint32) == b[:, :n].view(np.uint32)).all(), (weight_format, kv_cache)
+    dec.close()
+    fresh.close()
