@@ -467,6 +467,50 @@ int kllm_decoder_generate_speculative(kllm_decoder* dec, int32_t first_token, in
                                       kllm_token_callback on_tokens, void* ctx, int32_t* out_tokens_host,
                                       int32_t* n_out, kllm_spec_stats* stats);
 
+/* A batch of decoders sharing one model (DESIGN.md 5.14): up to KLLM_MAX_BATCH sequences decoded in ONE pass over
+ * the weights per step.  Member b is row b; each member has its own position, so sequences of different lengths
+ * share a pass, and its own history, draw settings, log-probability record, logits and cache.
+ *  - kllm_batch_step / kllm_batch_generate leave every member bit for bit as its own kllm_decoder_step (is_prompt
+ *    0) / kllm_decoder_generate (teacher NULL) with the same arguments would: the ids, kllm_decoder_logits (the
+ *    logits of its last position), the KV rows of the positions fed, the history, the log-probability record and
+ *    the state its own next entry continues from.  Every draw uses that member's settings in force.  One exception,
+ *    kllm_decoder_verify's: on the persistent engine a record entry's log-probabilities may differ from that
+ *    engine's own in the last bits; the ids and top-N ids are exact.
+ *  - Members may be used on their own between batch calls and may belong to several batches; calls must not overlap.
+ *    A batch is destroyed before its members.
+ *  - Each call synchronises every member's stream, runs on the batch's stream (NULL at create: a private
+ *    non-blocking one) and returns after a synchronisation.  The chain of one step is captured as a CUDA graph at
+ *    create; generate launches it n_steps times, each member's id fed back on the device.
+ * kllm_batch_create refuses, before any launch and leaving every member unchanged: KLLM_E_INVALID for n outside
+ * [1, KLLM_MAX_BATCH], NULL pointers and the same decoder twice; KLLM_E_UNSUPPORTED for a member
+ * kllm_decoder_verify refuses (the fast numerics, so the bf16 and fp8 caches, and tp_size > 1) and for members
+ * that do not describe the same model: the same shape, flavour, group size, weight format and weight device
+ * pointers, on one engine with one cache layout (so one KLLM_ATTN_SPLIT). */
+#define KLLM_MAX_BATCH 8
+typedef struct kllm_batch kllm_batch;
+int kllm_batch_create(kllm_decoder* const* members, int32_t n, void* stream, kllm_batch** out);
+void kllm_batch_destroy(kllm_batch* batch);
+/* One step of every member: tokens_host[b] fed at pos_host[b]; next_host[b] receives member b's id.
+ * KLLM_E_INVALID, before any launch and leaving every member unchanged, for NULL pointers, a token outside
+ * [0, vocab), pos < 0 and pos >= seq_len. */
+int kllm_batch_step(kllm_batch* batch, const int32_t* tokens_host, const int32_t* pos_host, int32_t* next_host);
+/* n_steps steps of every member from first_tokens_host[b] at start_pos_host[b]; out_tokens_host [n][n_steps]
+ * receives member b's ids in row b.  KLLM_E_INVALID, before any launch and leaving every member unchanged, for
+ * NULL pointers, n_steps <= 0, a token outside [0, vocab), start_pos < 0 and start_pos + n_steps > seq_len. */
+int kllm_batch_generate(kllm_batch* batch, const int32_t* first_tokens_host, const int32_t* start_pos_host,
+                        int32_t n_steps, int32_t* out_tokens_host);
+
+/* Copies into dst what src holds for positions [0, n_pos): the K/V rows (cache elements as stored: fp32, bf16, or
+ * fp8 codes at equal scales, in any layout), the history and the log-probability record entries.  Afterwards any
+ * entry on dst that continues at a position <= n_pos returns what it would on src, bit for bit; dst keeps its own
+ * draw settings, so forks of one prompt can sample with different seeds.  One prefill and n - 1 copies give n
+ * sequences of one prompt to batch.
+ * KLLM_E_INVALID for NULL pointers, src == dst and n_pos outside [0, seq_len]; KLLM_E_UNSUPPORTED unless both
+ * describe the same model (as kllm_batch_create), on the same engine with the same cache layout, kv_cache and fp8
+ * scales, with tp_size 1; both before any launch, with nothing copied.  Runs on dst's stream after synchronising
+ * src's, one kernel over the layout's indices, and returns after a synchronisation. */
+int kllm_decoder_copy_prefix(kllm_decoder* dst, const kllm_decoder* src, int32_t n_pos);
+
 /* Sampling instead of the greedy id, from this call on, for every id the decoder returns: kllm_decoder_step
  * (non-prompt), _prompt, _prefill_tf32 / _w8 and _generate, including the ids generate feeds back on the
  * device.  Each id is the rule of kllm_sample_f32 applied to the logits of the position just processed,

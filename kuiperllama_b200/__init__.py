@@ -45,6 +45,7 @@ TOKEN_CALLBACK = ctypes.CFUNCTYPE(None, c_void_p, POINTER(c_int32), c_int32)
 MAX_STOP_IDS = 16  # KLLM_MAX_STOP_IDS
 MAX_TOP_LOGPROBS = 20  # KLLM_MAX_TOP_LOGPROBS
 MAX_VERIFY_TOKENS = 8  # KLLM_MAX_VERIFY_TOKENS: the positions one kllm_decoder_verify pass takes
+MAX_BATCH = 8  # KLLM_MAX_BATCH: the members of one kllm_batch
 
 
 class SpecStats(ctypes.Structure):
@@ -128,6 +129,11 @@ _SIGNATURES = {
     "kllm_decoder_generate_speculative": (c_int, [c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32), c_int32,
                                                   c_int32, c_int32, TOKEN_CALLBACK, c_void_p, POINTER(c_int32),
                                                   POINTER(c_int32), POINTER(SpecStats)]),
+    "kllm_batch_create": (c_int, [POINTER(c_void_p), c_int32, c_void_p, POINTER(c_void_p)]),
+    "kllm_batch_destroy": (None, [c_void_p]),
+    "kllm_batch_step": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32)]),
+    "kllm_batch_generate": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int32), c_int32, POINTER(c_int32)]),
+    "kllm_decoder_copy_prefix": (c_int, [c_void_p, c_void_p, c_int32]),
     "kllm_decoder_set_sampling": (c_int, [c_void_p, c_float, c_int32, c_uint64]),
     "kllm_decoder_set_sampling_top_p": (c_int, [c_void_p, c_float, c_int32, c_float, c_uint64]),
     "kllm_decoder_set_repetition_penalty": (c_int, [c_void_p, c_float, c_int32]),
@@ -184,7 +190,7 @@ def check(rc: int, what: str = "kllm call") -> None:
         raise KllmError(f"{what} failed: {rc} ({lib.kllm_error_string(rc).decode()})")
 
 
-from .decoder import Decoder, ModelShape, SHAPES, synth_weights  # noqa: E402
+from .decoder import Batch, Decoder, ModelShape, SHAPES, synth_weights  # noqa: E402
 
-__all__ = ["load_library", "check", "KllmError", "GemvJob", "GemvSeg", "DecoderDesc", "Decoder",
-           "ModelShape", "SHAPES", "synth_weights", "FLAVOURS", "LIB_PATH", "HEADER_PATH"]
+__all__ = ["load_library", "check", "KllmError", "GemvJob", "GemvSeg", "DecoderDesc", "Decoder", "Batch",
+           "ModelShape", "SHAPES", "synth_weights", "FLAVOURS", "LIB_PATH", "HEADER_PATH", "MAX_BATCH"]

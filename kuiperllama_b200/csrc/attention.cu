@@ -52,16 +52,16 @@ __device__ __forceinline__ float block256_max(float v, float* s_warp) {
   return m;  // every thread
 }
 
-// Query position pos_arg + blockIdx.y (one row of q, scores and output per position) over a
-// cache in the graph engine's layout [seq][kv_dim], or with kTiled the persistent engine's exact-mode layout
+// Query row blockIdx.y (one row of q, scores and output per row) at position `pos` over a cache in the graph
+// engine's layout [seq][kv_dim], or with kTiled the persistent engine's exact-mode layout
 // (prefill::CacheLayout: K [kv_head][head_size / 4][seq][4], V [kv_head][vsplit][seq][head_size / vsplit]).
-// The layout moves addresses only; every operation is the same.
+// The layout, the row's position and its cache move addresses only; every operation is the same in each kernel
+// below.
 template <bool kTiled>
-__global__ void __launch_bounds__(kMhaThreads)
-mha_decode_kernel(PosArg pos_arg, int seq_len, const float* __restrict__ query, float* score_ptr,
-                  float* output, const float* __restrict__ key_cache,
-                  const float* __restrict__ value_cache, int kv_dim, int kv_mul, int head_size,
-                  long long layer_offset, int vsplit) {
+__device__ __forceinline__ void mha_decode_row(int pos, int seq_len, const float* __restrict__ query,
+                                               float* score_ptr, float* output, const float* __restrict__ key_cache,
+                                               const float* __restrict__ value_cache, int kv_dim, int kv_mul,
+                                               int head_size, long long layer_offset, int vsplit) {
   extern __shared__ __align__(16) float smem[];
   float* q_s = smem;                           // [head_size]
   float* v_s = smem + head_size;               // [2][kVTile][head_size]
@@ -70,7 +70,6 @@ mha_decode_kernel(PosArg pos_arg, int seq_len, const float* __restrict__ query, 
 
   const int head = blockIdx.x + blockIdx.y * gridDim.x;  // the (position, head) row of q, scores and output
   const int tid = threadIdx.x;
-  const int pos = pos_arg.get() + blockIdx.y;
   const float scale = 1.f / sqrtf(static_cast<float>(head_size));
   const float* query_head = query + static_cast<size_t>(head) * head_size;
   float* score_head = score_ptr + static_cast<size_t>(head) * seq_len;
@@ -158,11 +157,34 @@ mha_decode_kernel(PosArg pos_arg, int seq_len, const float* __restrict__ query, 
   if (tid < head_size) output[static_cast<size_t>(head) * head_size + tid] = value;
 }
 
-int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, int head_num, int layer_index,
+// Position pos_arg + blockIdx.y of one cache
+template <bool kTiled>
+__global__ void __launch_bounds__(kMhaThreads)
+mha_decode_kernel(PosArg pos_arg, int seq_len, const float* __restrict__ query, float* score_ptr,
+                  float* output, const float* __restrict__ key_cache,
+                  const float* __restrict__ value_cache, int kv_dim, int kv_mul, int head_size,
+                  long long layer_offset, int vsplit) {
+  mha_decode_row<kTiled>(pos_arg.get() + blockIdx.y, seq_len, query, score_ptr, output, key_cache, value_cache,
+                         kv_dim, kv_mul, head_size, layer_offset, vsplit);
+}
+
+// A batch's row blockIdx.y: member blockIdx.y's cache at that member's position (kllm_batch, DESIGN.md 5.14)
+template <bool kTiled>
+__global__ void __launch_bounds__(kMhaThreads)
+mha_members_kernel(const ChainMember* __restrict__ members, int seq_len, const float* __restrict__ query,
+                   float* score_ptr, float* output, int kv_dim, int kv_mul, int head_size, long long layer_offset,
+                   int vsplit) {
+  const ChainMember& mb = members[blockIdx.y];
+  mha_decode_row<kTiled>(*mb.pos, seq_len, query, score_ptr, output, mb.key_cache, mb.value_cache, kv_dim, kv_mul,
+                         head_size, layer_offset, vsplit);
+}
+
+int launch_mha_rows(ChainPos at, int n_pos, const prefill::CacheLayout& c, int head_num, int layer_index,
                     int kv_mul, float* mha_out, const float* query, float* score, const float* key_cache,
                     const float* value_cache, cudaStream_t stream) {
   const int hs = c.head_size;
-  if (!mha_out || !query || !score || !key_cache || !value_cache || n_pos <= 0) return KLLM_E_INVALID;
+  if (!mha_out || !query || !score || n_pos <= 0) return KLLM_E_INVALID;
+  if (at.members == nullptr && (!key_cache || !value_cache)) return KLLM_E_INVALID;
   if (c.elem != KLLM_KV_F32 || (hs & 3) != 0 || (c.kv_dim & 3) != 0 || hs > kMhaThreads) return KLLM_E_UNSUPPORTED;
   if (c.mega && (hs % c.split != 0 || (hs / c.split) % 4 != 0)) return KLLM_E_UNSUPPORTED;
   const long long layer_offset = static_cast<long long>(layer_index) * c.seq_len * c.kv_dim;
@@ -170,21 +192,23 @@ int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, 
   // heads (up to 256: 66 KB) opt in.  The tiling does not touch the arithmetic.
   const size_t smem = sizeof(float) * (hs + 2 * kVTile * hs);
   const dim3 grid(head_num, n_pos);
-  if (c.mega) {
+  const int vsplit = c.mega ? c.split : 1;
+  auto launch = [&](auto one, auto rows) {
+    const void* k = at.members ? reinterpret_cast<const void*>(rows) : reinterpret_cast<const void*>(one);
     if (smem > 48 * 1024) {
-      if (const int rc = smem_opt_in(reinterpret_cast<const void*>(mha_decode_kernel<true>), smem)) return rc;
+      if (const int rc = smem_opt_in(k, smem)) return rc;
     }
-    mha_decode_kernel<true><<<grid, kMhaThreads, smem, stream>>>(first_pos, c.seq_len, query, score, mha_out,
-                                                                key_cache, value_cache, c.kv_dim, kv_mul, hs,
-                                                                layer_offset, c.split);
-  } else {
-    if (smem > 48 * 1024) {
-      if (const int rc = smem_opt_in(reinterpret_cast<const void*>(mha_decode_kernel<false>), smem)) return rc;
-    }
-    mha_decode_kernel<false><<<grid, kMhaThreads, smem, stream>>>(first_pos, c.seq_len, query, score, mha_out,
-                                                                 key_cache, value_cache, c.kv_dim, kv_mul, hs,
-                                                                 layer_offset, 1);
-  }
+    if (at.members)
+      rows<<<grid, kMhaThreads, smem, stream>>>(at.members, c.seq_len, query, score, mha_out, c.kv_dim, kv_mul, hs,
+                                                layer_offset, vsplit);
+    else
+      one<<<grid, kMhaThreads, smem, stream>>>(at.first, c.seq_len, query, score, mha_out, key_cache, value_cache,
+                                               c.kv_dim, kv_mul, hs, layer_offset, vsplit);
+    return 0;
+  };
+  const int rc = c.mega ? launch(mha_decode_kernel<true>, mha_members_kernel<true>)
+                        : launch(mha_decode_kernel<false>, mha_members_kernel<false>);
+  if (rc != 0) return rc;
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }
@@ -198,6 +222,7 @@ extern "C" int kllm_mha_decode_f32(int pos, int head_num, int layer_index, int s
   if (pos < 0 || pos >= seq_len || head_num <= 0 || kv_mul <= 0 || head_size <= 0 || layer_index < 0)
     return KLLM_E_INVALID;
   const kllm::prefill::CacheLayout flat{0, seq_len, kv_dim, head_size, 1, KLLM_KV_F32};
-  return kllm::launch_mha_rows(kllm::PosArg{nullptr, pos}, 1, flat, head_num, layer_index, kv_mul, mha_out, query,
-                               score, key_cache, value_cache, static_cast<cudaStream_t>(stream));
+  return kllm::launch_mha_rows(kllm::ChainPos{kllm::PosArg{nullptr, pos}, nullptr}, 1, flat, head_num, layer_index,
+                               kv_mul, mha_out, query, score, key_cache, value_cache,
+                               static_cast<cudaStream_t>(stream));
 }

@@ -32,17 +32,23 @@ namespace kllm {
 constexpr int kStreamIds = 32;  // int32 offset of the streamed ids behind the count (kllm_decoder::stream_host)
 static_assert(mega::kMaxStopIds == KLLM_MAX_STOP_IDS, "one stop-set capacity");
 
-// Also records the fed id in the history (sampling.cuh step 0), -1 for an id outside the vocabulary.
-__global__ void embed_token_kernel(const mega::State* st, const float* __restrict__ table,
-                                   float* x, int dim, int vocab, int32_t* hist) {
+// Also records the fed id in the history (sampling.cuh step 0), -1 for an id outside the vocabulary.  Block b of nb
+// copies its share of the embedding row into x.
+__device__ __forceinline__ void embed_token(const mega::State* st, const float* __restrict__ table, float* x, int dim,
+                                            int vocab, int32_t* hist, int b, int nb) {
   const int32_t token = st->token;
   const bool valid = token >= 0 && token < vocab;
-  if (blockIdx.x == 0 && threadIdx.x == 0) hist[st->pos] = valid ? token : -1;
+  if (b == 0 && threadIdx.x == 0) hist[st->pos] = valid ? token : -1;
   if (!valid) return;
   const float4* s4 = reinterpret_cast<const float4*>(table + static_cast<size_t>(token) * dim);
   float4* d4 = reinterpret_cast<float4*>(x);
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < (dim >> 2); i += gridDim.x * blockDim.x)
+  for (int i = b * blockDim.x + threadIdx.x; i < (dim >> 2); i += nb * blockDim.x)
     d4[i] = s4[i];
+}
+
+__global__ void embed_token_kernel(const mega::State* st, const float* __restrict__ table,
+                                   float* x, int dim, int vocab, int32_t* hist) {
+  embed_token(st, table, x, dim, vocab, hist, blockIdx.x, gridDim.x);
 }
 
 // The id of the step (greedy, argmax_kernel.cu:49-71 semantics, or drawn by the sampling rule of
@@ -53,10 +59,11 @@ __global__ void embed_token_kernel(const mega::State* st, const float* __restric
 // the id, then the count with release semantics at system scope, which the host polls.
 // The draw and record entry (sampling.cuh draw_and_record, DESIGN.md 5.8): with logprobs on, from the state's step
 // `lp_from` on, the entry of the drawn id, or of teacher[step + 1] in `lp_target` mode.
-__global__ void __launch_bounds__(1024)
-argmax_advance_kernel(const float* __restrict__ logits, int n, const DrawSettings* cfg, mega::State* st,
-                      int32_t* out_tokens, const int32_t* teacher, int max_steps, int32_t* stream_ids,
-                      int32_t* stream_count, const int32_t* hist, float* penalized, sampling::LogprobRecord rec) {
+// One block of 1024 threads: argmax_advance_kernel, and each member's block of a batch's draw.
+__device__ __forceinline__ void draw_advance(const float* __restrict__ logits, int n, const DrawSettings* cfg,
+                                             mega::State* st, int32_t* out_tokens, const int32_t* teacher,
+                                             int max_steps, int32_t* stream_ids, int32_t* stream_count,
+                                             const int32_t* hist, float* penalized, sampling::LogprobRecord rec) {
   const int step0 = st->step;  // read by every thread before thread 0 advances the state
   const int next = sampling::draw_and_record(logits, n, cfg, cfg->penalty, penalized, hist, st->pos,
                                              step0 >= st->lp_from, st->lp_target ? teacher + step0 + 1 : nullptr, rec);
@@ -71,6 +78,59 @@ argmax_advance_kernel(const float* __restrict__ logits, int n, const DrawSetting
     st->token = (st->teacher && step + 1 < max_steps) ? teacher[step + 1] : next;
     st->pos = st->pos + 1;
     st->step = step + 1;
+  }
+}
+
+__global__ void __launch_bounds__(1024)
+argmax_advance_kernel(const float* __restrict__ logits, int n, const DrawSettings* cfg, mega::State* st,
+                      int32_t* out_tokens, const int32_t* teacher, int max_steps, int32_t* stream_ids,
+                      int32_t* stream_count, const int32_t* hist, float* penalized, sampling::LogprobRecord rec) {
+  draw_advance(logits, n, cfg, st, out_tokens, teacher, max_steps, stream_ids, stream_count, hist, penalized, rec);
+}
+
+// What a batch's embedding and draw read and write of one member: the arguments of argmax_advance_kernel in the
+// member's own step, with no streamed ids
+struct BatchTarget {
+  mega::State* st;
+  const DrawSettings* cfg;
+  int32_t* hist;
+  float* penalized;
+  sampling::LogprobRecord rec;
+  int32_t* out_tokens;
+  const int32_t* teacher;
+  float* logits;  // receives the member's row of the batch's logits
+};
+
+// grid (4, members): member blockIdx.y's embedding into row blockIdx.y, as embed_token_kernel's 4 blocks do it
+__global__ void batch_embed_kernel(const BatchTarget* __restrict__ members, const float* __restrict__ table, float* x,
+                                   int dim, int vocab) {
+  const BatchTarget& mb = members[blockIdx.y];
+  embed_token(mb.st, table, x + static_cast<size_t>(blockIdx.y) * dim, dim, vocab, mb.hist, blockIdx.x, gridDim.x);
+}
+
+// Block b: member b's step draw over row b of the batch's logits, then the row becomes the member's logits
+__global__ void __launch_bounds__(1024)
+batch_draw_kernel(const float* __restrict__ logits_rows, int n, const BatchTarget* __restrict__ members,
+                  int max_steps) {
+  const BatchTarget& mb = members[blockIdx.x];
+  const float* row = logits_rows + static_cast<size_t>(blockIdx.x) * n;
+  draw_advance(row, n, mb.cfg, mb.st, mb.out_tokens, mb.teacher, max_steps, nullptr, nullptr, mb.hist, mb.penalized,
+               mb.rec);
+  for (int e = threadIdx.x; e < n; e += blockDim.x) mb.logits[e] = row[e];
+}
+
+// One prefix of a cache: positions [0, gridDim.x) of every layer (blockIdx.y), element by element through the
+// layout's own index, so any layout and element (T of its size: fp32, bf16 or fp8 codes) is copied as stored
+template <typename T>
+__global__ void copy_prefix_kernel(const T* __restrict__ ks, const T* __restrict__ vs, T* __restrict__ kd,
+                                   T* __restrict__ vd, prefill::CacheLayout c) {
+  const int pos = blockIdx.x;
+  const size_t layer = static_cast<size_t>(blockIdx.y) * c.seq_len * c.kv_dim;
+  for (int p = threadIdx.x; p < c.kv_dim; p += blockDim.x) {
+    const int kvh = p / c.head_size, i = p % c.head_size;
+    const size_t ki = layer + prefill::k_index(c, pos, kvh, i), vi = layer + prefill::v_index(c, pos, kvh, i);
+    kd[ki] = ks[ki];
+    vd[vi] = vs[vi];
   }
 }
 
@@ -195,6 +255,21 @@ struct kllm_decoder {
   int vf_launches[KLLM_MAX_VERIFY_TOKENS] = {};
 };
 
+// A batch of decoders over one model (kllm_batch_create): member b is row b of one chain
+struct kllm_batch {
+  std::vector<kllm_decoder*> members;
+  cudaStream_t stream = nullptr;
+  bool own_stream = false;
+  void* buf = nullptr;  // device: the chain's rows [n][.]
+  ChainRows rows{};
+  void* tables = nullptr;  // device: the members' ChainMember [n], then their BatchTarget [n]
+  ChainMember* chain = nullptr;
+  BatchTarget* targets = nullptr;
+  int32_t* io_host = nullptr;  // pinned [n][seq_len]: the ids read back
+  cudaGraphExec_t exec = nullptr;  // embedding, chain and draw of one step, captured at create
+  int launches = 0;
+};
+
 namespace {
 
 // The settings `next` in force from the next entry on: no step may still be reading the old ones, and the next one
@@ -259,8 +334,8 @@ int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
   KLLM_TRY(cudaGetLastError());
   const ChainRows rows{dc->x, dc->q, dc->k, dc->v, dc->attn, dc->h, dc->score, dc->logits};
   const TpReduce tp{&dc->d, dc->tp_tmp};
-  KLLM_TRY(enqueue_layers(m, decoder_cache(dc), rows, 1, PosArg{&dc->st->pos, 0}, dc->d.tp_size > 1 ? &tp : nullptr,
-                          s));
+  KLLM_TRY(enqueue_layers(m, decoder_cache(dc), rows, 1, ChainPos{PosArg{&dc->st->pos, 0}, nullptr},
+                          dc->d.tp_size > 1 ? &tp : nullptr, s));
   // post_processing (llama3.cpp:733-745)
   argmax_advance_kernel<<<1, 1024, 0, s>>>(dc->logits, m.vocab_size, dc->d_cfg, dc->st, dc->out_tokens, dc->teacher,
                                            m.seq_len, dc->stream_dev + kStreamIds, dc->stream_dev, dc->hist,
@@ -356,6 +431,124 @@ int run_prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, 
 int verify_supported(const kllm_decoder* dc) {
   if (dc->d.tp_size > 1 || dc->d.kv_cache != KLLM_KV_F32) return KLLM_E_UNSUPPORTED;
   if (dc->use_mega && dc->mega.fast()) return KLLM_E_UNSUPPORTED;
+  return 0;
+}
+
+// One model: the same shape, flavour, group size, weight format and weight pointers, on the same engine with the same
+// cache layout (so the same attention split).  Two such decoders run the same arithmetic on the same weights, so
+// one chain serves both, and a cache prefix of one is a cache prefix of the other.
+bool same_model(const kllm_decoder* a, const kllm_decoder* b) {
+  const DecoderModel &x = a->m, &y = b->m;
+  const int xs[] = {x.dim, x.hidden_dim, x.layer_num, x.head_num, x.kv_head_num, x.vocab_size, x.seq_len, x.head_size,
+                    x.kv_dim, x.kv_mul, x.q_rows, x.flavour, x.group_size};
+  const int ys[] = {y.dim, y.hidden_dim, y.layer_num, y.head_num, y.kv_head_num, y.vocab_size, y.seq_len, y.head_size,
+                    y.kv_dim, y.kv_mul, y.q_rows, y.flavour, y.group_size};
+  if (std::memcmp(xs, ys, sizeof(xs)) != 0 || x.format != y.format) return false;
+  auto same = [](const Matrix& p, const Matrix& q) { return p.w == q.w && p.scales == q.scales && p.bias == q.bias; };
+  if (x.tok_emb != y.tok_emb || x.final_norm != y.final_norm || !same(x.cls, y.cls)) return false;
+  for (int l = 0; l < x.layer_num; ++l) {
+    const LayerWeights &p = x.layers[l], &q = y.layers[l];
+    if (p.attn_norm != q.attn_norm || p.ffn_norm != q.ffn_norm || !same(p.q, q.q) || !same(p.k, q.k) ||
+        !same(p.v, q.v) || !same(p.o, q.o) || !same(p.w1, q.w1) || !same(p.w2, q.w2) || !same(p.w3, q.w3))
+      return false;
+  }
+  const prefill::CacheLayout ca = decoder_cache(a).cache, cb = decoder_cache(b).cache;
+  return a->use_mega == b->use_mega && ca.mega == cb.mega && ca.seq_len == cb.seq_len && ca.kv_dim == cb.kv_dim &&
+         ca.head_size == cb.head_size && ca.split == cb.split && ca.elem == cb.elem;
+}
+
+// Embedding, chain and draw of one step of every member: the graph engine's step (enqueue_step) at n rows
+int enqueue_batch(const kllm_batch* b, cudaStream_t s) {
+  const kllm_decoder* d0 = b->members[0];
+  const DecoderModel& m = d0->m;
+  const int n = static_cast<int>(b->members.size());
+  batch_embed_kernel<<<dim3(4, n), 256, 0, s>>>(b->targets, m.tok_emb, b->rows.x, m.dim, m.vocab_size);
+  count_launch();
+  KLLM_TRY(cudaGetLastError());
+  // the RoPE tables are member 0's: every member's hold the same values (kllm_sincos_init of the same shape)
+  KLLM_TRY(enqueue_layers(m, decoder_cache(d0), b->rows, n, ChainPos{PosArg{nullptr, 0}, b->chain}, nullptr, s));
+  batch_draw_kernel<<<n, 1024, 0, s>>>(b->rows.logits, m.vocab_size, b->targets, m.seq_len);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+// The batch's workspace, member tables and captured step
+int batch_prepare(kllm_batch* b) {
+  const DecoderModel& m = b->members[0]->m;
+  const size_t n = b->members.size(), V = m.vocab_size;
+  const size_t per_row = 2 * static_cast<size_t>(m.q_rows) + 2 * m.kv_dim + m.dim + m.hidden_dim + V +
+                         static_cast<size_t>(m.head_num) * m.seq_len;
+  const size_t table_bytes = n * (sizeof(ChainMember) + sizeof(BatchTarget));
+  if (cudaMalloc(&b->buf, per_row * n * sizeof(float)) != cudaSuccess) b->buf = nullptr;
+  if (cudaMalloc(&b->tables, table_bytes) != cudaSuccess) b->tables = nullptr;
+  if (cudaMallocHost(&b->io_host, sizeof(int32_t) * n * m.seq_len) != cudaSuccess) b->io_host = nullptr;
+  if (!b->buf || !b->tables || !b->io_host) return static_cast<int>(cudaErrorMemoryAllocation);
+  float* f = static_cast<float*>(b->buf);
+  auto take = [&](size_t per) {
+    float* r = f;
+    f += per * n;
+    return r;
+  };
+  ChainRows& r = b->rows;
+  r.x = take(m.dim), r.q = take(m.q_rows), r.k = take(m.kv_dim), r.v = take(m.kv_dim), r.att = take(m.q_rows);
+  r.h = take(m.hidden_dim), r.logits = take(V), r.score = take(static_cast<size_t>(m.head_num) * m.seq_len);
+  std::vector<ChainMember> chain(n);
+  std::vector<BatchTarget> targets(n);
+  for (size_t i = 0; i < n; ++i) {
+    kllm_decoder* dc = b->members[i];
+    chain[i] = ChainMember{dc->kcache, dc->vcache, &dc->st->pos};
+    targets[i] = BatchTarget{dc->st, dc->d_cfg, dc->hist, dc->penalized, dc->rec, dc->out_tokens, dc->teacher,
+                             dc->logits};
+  }
+  b->chain = static_cast<ChainMember*>(b->tables);
+  b->targets = reinterpret_cast<BatchTarget*>(static_cast<char*>(b->tables) + n * sizeof(ChainMember));
+  static_assert(sizeof(ChainMember) % alignof(BatchTarget) == 0, "the targets follow the chain table aligned");
+  KLLM_TRY(cudaMemcpy(b->chain, chain.data(), n * sizeof(ChainMember), cudaMemcpyHostToDevice));
+  KLLM_TRY(cudaMemcpy(b->targets, targets.data(), n * sizeof(BatchTarget), cudaMemcpyHostToDevice));
+  const uint64_t before = launch_counter().load();
+  (void)cudaGetLastError();  // the chain checks its launches with cudaGetLastError: no earlier call's error is its own
+  KLLM_TRY(cudaStreamBeginCapture(b->stream, cudaStreamCaptureModeRelaxed));
+  const int rc = enqueue_batch(b, b->stream);
+  cudaGraph_t g = nullptr;
+  const cudaError_t end = cudaStreamEndCapture(b->stream, &g);
+  // capturing does not execute: undo the launch accounting of the capture pass
+  const uint64_t launches = launch_counter().load() - before;
+  launch_counter().fetch_sub(launches);
+  if (rc != 0 || end != cudaSuccess) {
+    if (g) cudaGraphDestroy(g);
+    return rc != 0 ? rc : static_cast<int>(end);
+  }
+  const cudaError_t inst = cudaGraphInstantiate(&b->exec, g, 0);
+  cudaGraphDestroy(g);
+  KLLM_TRY(inst);
+  b->launches = static_cast<int>(launches);
+  return 0;
+}
+
+// n_steps steps of every member from tokens[b] at pos[b]; out [n][n_steps].  Every refusal comes before any launch.
+int run_batch(kllm_batch* b, const int32_t* tokens, const int32_t* pos, int32_t n_steps, int32_t* out) {
+  if (!b || !tokens || !pos || !out || n_steps <= 0) return KLLM_E_INVALID;
+  const DecoderModel& m = b->members[0]->m;
+  const size_t n = b->members.size();
+  for (size_t i = 0; i < n; ++i) {
+    if (tokens[i] < 0 || tokens[i] >= m.vocab_size || pos[i] < 0) return KLLM_E_INVALID;
+    if (static_cast<int64_t>(pos[i]) + n_steps > m.seq_len) return KLLM_E_INVALID;
+  }
+  for (kllm_decoder* dc : b->members) KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  // each member's state as its own kllm_decoder_generate (no teacher) puts it; the pinned copies stay as written
+  // until the synchronisation below
+  for (size_t i = 0; i < n; ++i) {
+    kllm_decoder* dc = b->members[i];
+    *dc->st_host = mega::State{tokens[i], pos[i], 0, -1, 0, 0, 0, 0};
+    KLLM_TRY(cudaMemcpyAsync(dc->st, dc->st_host, sizeof(mega::State), cudaMemcpyHostToDevice, b->stream));
+  }
+  for (int32_t i = 0; i < n_steps; ++i) KLLM_TRY(cudaGraphLaunch(b->exec, b->stream));
+  count_launch(static_cast<uint64_t>(b->launches) * n_steps);
+  for (size_t i = 0; i < n; ++i)
+    KLLM_TRY(cudaMemcpyAsync(b->io_host + i * n_steps, b->members[i]->out_tokens, sizeof(int32_t) * n_steps,
+                             cudaMemcpyDeviceToHost, b->stream));
+  KLLM_TRY(cudaStreamSynchronize(b->stream));
+  std::memcpy(out, b->io_host, sizeof(int32_t) * n * n_steps);
   return 0;
 }
 
@@ -786,6 +979,96 @@ int kllm_decoder_verify(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_
   for (int32_t i = 0; i < n_tokens; ++i)
     if (tokens_host[i] < 0 || tokens_host[i] >= dc->m.vocab_size) return KLLM_E_INVALID;
   return run_verify(dc, tokens_host, n_tokens, start_pos, nullptr, 0, out_ids_host, n_accepted);
+}
+
+int kllm_batch_create(kllm_decoder* const* members, int32_t n, void* stream, kllm_batch** out) {
+  // every refusal comes before the first launch, so a refused call leaves every member as it was
+  if (!members || !out || n < 1 || n > KLLM_MAX_BATCH) return KLLM_E_INVALID;
+  for (int32_t i = 0; i < n; ++i) {
+    if (members[i] == nullptr) return KLLM_E_INVALID;
+    for (int32_t j = 0; j < i; ++j)
+      if (members[j] == members[i]) return KLLM_E_INVALID;
+  }
+  for (int32_t i = 0; i < n; ++i) {
+    KLLM_TRY(verify_supported(members[i]));
+    if (!same_model(members[0], members[i])) return KLLM_E_UNSUPPORTED;
+  }
+  auto* b = new kllm_batch();
+  b->members.assign(members, members + n);
+  auto fail = [&](int rc) {
+    kllm_batch_destroy(b);
+    return rc;
+  };
+  if (stream != nullptr) {
+    b->stream = static_cast<cudaStream_t>(stream);
+  } else {
+    if (cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking) != cudaSuccess) return fail(KLLM_E_NODEVICE);
+    b->own_stream = true;
+  }
+  for (kllm_decoder* dc : b->members)
+    if (const cudaError_t e = cudaStreamSynchronize(dc->stream)) return fail(static_cast<int>(e));
+  if (const int rc = batch_prepare(b)) return fail(rc);
+  *out = b;
+  return 0;
+}
+
+void kllm_batch_destroy(kllm_batch* b) {
+  if (!b) return;
+  if (b->stream) cudaStreamSynchronize(b->stream);
+  if (b->exec) cudaGraphExecDestroy(b->exec);
+  if (b->buf) cudaFree(b->buf);
+  if (b->tables) cudaFree(b->tables);
+  if (b->io_host) cudaFreeHost(b->io_host);
+  if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
+  delete b;
+}
+
+int kllm_batch_step(kllm_batch* b, const int32_t* tokens_host, const int32_t* pos_host, int32_t* next_host) {
+  return run_batch(b, tokens_host, pos_host, 1, next_host);
+}
+
+int kllm_batch_generate(kllm_batch* b, const int32_t* first_tokens_host, const int32_t* start_pos_host,
+                        int32_t n_steps, int32_t* out_tokens_host) {
+  return run_batch(b, first_tokens_host, start_pos_host, n_steps, out_tokens_host);
+}
+
+int kllm_decoder_copy_prefix(kllm_decoder* dst, const kllm_decoder* src, int32_t n_pos) {
+  // every refusal comes before the first launch, so a refused call copies nothing
+  if (!dst || !src || dst == src || n_pos < 0) return KLLM_E_INVALID;
+  if (dst->d.tp_size > 1 || src->d.tp_size > 1 || !same_model(dst, src) || dst->d.kv_cache != src->d.kv_cache ||
+      dst->kv_scales != src->kv_scales)
+    return KLLM_E_UNSUPPORTED;
+  const DecoderModel& m = dst->m;
+  if (n_pos > m.seq_len) return KLLM_E_INVALID;
+  KLLM_TRY(cudaStreamSynchronize(src->stream));
+  if (n_pos == 0) return 0;
+  const prefill::CacheLayout c = decoder_cache(dst).cache;
+  const dim3 grid(n_pos, m.layer_num);
+  cudaStream_t s = dst->stream;
+  if (c.elem == KLLM_KV_FP8) {
+    copy_prefix_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const uint8_t*>(src->kcache),
+                                            reinterpret_cast<const uint8_t*>(src->vcache),
+                                            reinterpret_cast<uint8_t*>(dst->kcache),
+                                            reinterpret_cast<uint8_t*>(dst->vcache), c);
+  } else if (c.elem == KLLM_KV_BF16) {
+    copy_prefix_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const uint16_t*>(src->kcache),
+                                            reinterpret_cast<const uint16_t*>(src->vcache),
+                                            reinterpret_cast<uint16_t*>(dst->kcache),
+                                            reinterpret_cast<uint16_t*>(dst->vcache), c);
+  } else {
+    copy_prefix_kernel<<<grid, 256, 0, s>>>(src->kcache, src->vcache, dst->kcache, dst->vcache, c);
+  }
+  count_launch();
+  KLLM_TRY(cudaGetLastError());
+  // the history and the record entries of the same positions
+  const size_t P = n_pos, T = P * sampling::kMaxTopLogprobs;
+  KLLM_TRY(cudaMemcpyAsync(dst->hist, src->hist, sizeof(int32_t) * P, cudaMemcpyDeviceToDevice, s));
+  KLLM_TRY(cudaMemcpyAsync(dst->rec.id, src->rec.id, sizeof(int32_t) * P, cudaMemcpyDeviceToDevice, s));
+  KLLM_TRY(cudaMemcpyAsync(dst->rec.lp, src->rec.lp, sizeof(float) * P, cudaMemcpyDeviceToDevice, s));
+  KLLM_TRY(cudaMemcpyAsync(dst->rec.top_ids, src->rec.top_ids, sizeof(int32_t) * T, cudaMemcpyDeviceToDevice, s));
+  KLLM_TRY(cudaMemcpyAsync(dst->rec.top_lp, src->rec.top_lp, sizeof(float) * T, cudaMemcpyDeviceToDevice, s));
+  // src may change as soon as this returns
+  return static_cast<int>(cudaStreamSynchronize(s));
 }
 
 int kllm_decoder_generate_speculative(kllm_decoder* dc, int32_t first_token, int32_t start_pos, int32_t max_steps,

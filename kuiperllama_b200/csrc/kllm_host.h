@@ -29,6 +29,22 @@ struct PosArg {
   __host__ __device__ int get() const { return ptr != nullptr ? *ptr : val; }
 };
 
+// One row of a batch's chain (kllm_batch, DESIGN.md 5.14): a member decoder's fp32 KV cache in its engine's layout,
+// and the position word of its step state (mega::State::pos), read at run time so that one captured chain serves
+// every position
+struct ChainMember {
+  float* key_cache;
+  float* value_cache;
+  const int* pos;
+};
+
+// Where the chain's n rows run: row i at first + i in one cache, or, with `members` (a device table of n rows, the
+// batch), row i at *members[i].pos in members[i]'s cache
+struct ChainPos {
+  PosArg first;
+  const ChainMember* members;
+};
+
 // Returns the first nonzero status of a call (a KLLM_E_* code or a cudaError_t)
 #define KLLM_TRY(expr)                      \
   do {                                      \
@@ -42,9 +58,10 @@ struct PosArg {
 // residual is residual + v * rows.
 int gemv_dispatch(const kllm_gemv_job* job, WeightFormat format, cudaStream_t stream, int nv = 1);
 
-// mha_decode_kernel for the n_pos query positions first_pos, first_pos + 1, .. (q, output
-// [n_pos][head_num * head_size], scores [n_pos][head_num][seq_len]) over an fp32 cache in either engine's layout
-int launch_mha_rows(PosArg first_pos, int n_pos, const prefill::CacheLayout& c, int head_num, int layer_index,
+// mha_decode_kernel for the n_pos query positions at.first, at.first + 1, .. (q, output
+// [n_pos][head_num * head_size], scores [n_pos][head_num][seq_len]) over an fp32 cache in either engine's layout;
+// with at.members, mha_members_kernel: row i over members[i]'s cache at its position (key_cache and value_cache unused)
+int launch_mha_rows(ChainPos at, int n_pos, const prefill::CacheLayout& c, int head_num, int layer_index,
                     int kv_mul, float* mha_out, const float* query, float* score, const float* key_cache,
                     const float* value_cache, cudaStream_t stream);
 
@@ -68,9 +85,10 @@ int prefill_block(const DecoderModel& dm, const DecoderCache& m, PrefillWorkspac
                   int start_pos, cudaStream_t stream);
 int prefill_attention_smem_opt_in(size_t bytes);
 // RoPE on T query rows [T][q_rows] in place and on T key rows [T][kv_dim], scattered with the value rows into layer
-// `layer` of an fp32 cache at positions start_pos .. start_pos + T - 1: kllm_rope_f32's arithmetic (prefill.cu)
+// `layer` of an fp32 cache at positions at.first .. at.first + T - 1 (or, with at.members, row t into members[t]'s
+// cache at its position): kllm_rope_f32's arithmetic (prefill.cu)
 int launch_rope_scatter_f32(const DecoderModel& dm, const DecoderCache& c, int layer, float* q, const float* k,
-                            const float* v, PosArg start_pos, int T, cudaStream_t s);
+                            const float* v, ChainPos at, int T, cudaStream_t s);
 
 inline float flavour_eps(int flavour) { return flavour == KLLM_FLAVOUR_QWEN2 ? 1e-6f : 1e-5f; }
 }  // namespace kllm

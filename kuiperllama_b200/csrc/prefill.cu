@@ -107,14 +107,23 @@ struct KvScales {
 };
 
 // RoPE (rope_kernel.cu) on the T query rows in place, and on the T key rows while they are scattered,
-// with the value rows, into the layer's cache (of element type E; fp8: at the inverses `inv` of the layer's scales).
+// with the value rows, into the layer's cache (of element type E; fp8: at the inverses `inv` of the layer's scales):
+// the layer at layer_off elements into kcache / vcache, row t at position at.first + t; or, with at.members (the
+// batch, fp32 only), row t into the layer of members[t]'s cache at *members[t].pos.
 // grid = (T, rope_blocks): one thread per rotation pair and per value element.
 template <typename E>
 __global__ void rope_scatter_kernel(float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                                     const float* __restrict__ sin_t, const float* __restrict__ cos_t,
-                                    E* __restrict__ kcache, E* __restrict__ vcache, CacheLayout c, int heads,
-                                    int kv_heads, int flavour, PosArg start_pos, KvScales inv) {
-  const int t = blockIdx.x, pos = start_pos.get() + t, hs = c.head_size, half = hs >> 1;
+                                    E* kcache, E* vcache, size_t layer_off, CacheLayout c, int heads,
+                                    int kv_heads, int flavour, ChainPos at, KvScales inv) {
+  const int t = blockIdx.x, hs = c.head_size, half = hs >> 1;
+  int pos = at.first.get() + t;
+  if (at.members != nullptr) {
+    const ChainMember& mb = at.members[t];
+    pos = *mb.pos;
+    kcache = reinterpret_cast<E*>(mb.key_cache), vcache = reinterpret_cast<E*>(mb.value_cache);
+  }
+  kcache += layer_off, vcache += layer_off;
   const int p0 = blockIdx.y * blockDim.x + threadIdx.x, stride = gridDim.y * blockDim.x;
   float* qrow = q + static_cast<size_t>(t) * heads * hs;
   const float* krow = k + static_cast<size_t>(t) * kv_heads * hs;
@@ -229,8 +238,8 @@ int prefill_block(const DecoderModel& dm, const DecoderCache& m, PrefillWorkspac
     // the layer's cache, of element type E
     auto attend = [&](auto* kc, auto* vc, KvScales inv, KvScales sc) {
       rope_scatter_kernel<<<rope_grid(T, heads, kvh, dm.head_size), 256, 0, s>>>(
-          ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc + layer_off, vc + layer_off, cl, heads, kvh, dm.flavour,
-          PosArg{nullptr, start_pos}, inv);
+          ws.q, ws.k, ws.v, m.sin_cache, m.cos_cache, kc, vc, layer_off, cl, heads, kvh, dm.flavour,
+          ChainPos{PosArg{nullptr, start_pos}, nullptr}, inv);
       KLLM_TRY(count());
       attn_rows_kernel<<<dim3(heads, T), 128, sc_bytes, s>>>(ws.q, kc + layer_off, vc + layer_off, ws.att, cl, heads,
                                                              dm.kv_mul, start_pos, sc);
@@ -265,12 +274,12 @@ int prefill_block(const DecoderModel& dm, const DecoderCache& m, PrefillWorkspac
 }
 
 int launch_rope_scatter_f32(const DecoderModel& dm, const DecoderCache& c, int layer, float* q, const float* k,
-                            const float* v, PosArg start_pos, int T, cudaStream_t s) {
+                            const float* v, ChainPos at, int T, cudaStream_t s) {
   if (c.cache.elem != KLLM_KV_F32) return KLLM_E_UNSUPPORTED;
   const size_t layer_off = static_cast<size_t>(layer) * dm.seq_len * dm.kv_dim;
   rope_scatter_kernel<<<rope_grid(T, dm.head_num, dm.kv_head_num, dm.head_size), 256, 0, s>>>(
-      q, k, v, c.sin_cache, c.cos_cache, c.key_cache + layer_off, c.value_cache + layer_off, c.cache, dm.head_num,
-      dm.kv_head_num, dm.flavour, start_pos, KvScales{});
+      q, k, v, c.sin_cache, c.cos_cache, c.key_cache, c.value_cache, layer_off, c.cache, dm.head_num,
+      dm.kv_head_num, dm.flavour, at, KvScales{});
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }

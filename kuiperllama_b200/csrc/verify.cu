@@ -14,7 +14,8 @@
 //   final: rmsnorm, cls                       ->   gemv(norm -> cls)
 //
 // The verify pass wraps the chain in verify_embed_kernel (n rows; saves the history and record entries), one draw
-// block per position and verify_accept_kernel.
+// block per position and verify_accept_kernel.  A batch of decoders (kllm_batch, decoder.cu) runs it at n members,
+// each row over its own member's cache at that member's position (ChainPos::members); the GEMVs are the same.
 #include <cuda_runtime.h>
 
 #include "../../include/kllm_b200.h"
@@ -138,7 +139,7 @@ int enqueue_classifier(const DecoderModel& m, const float* x, float* logits, int
   return gemv_dispatch(&j, m.format, s, n);
 }
 
-int enqueue_layers(const DecoderModel& m, const DecoderCache& c, const ChainRows& r, int n, PosArg first_pos,
+int enqueue_layers(const DecoderModel& m, const DecoderCache& c, const ChainRows& r, int n, ChainPos at,
                    const TpReduce* tp, cudaStream_t s) {
   const int dim = m.dim, hid = m.hidden_dim, q_rows = m.q_rows, kvd = m.kv_dim;  // q_rows == dim unless tensor-parallel
   for (int l = 0; l < m.layer_num; ++l) {
@@ -151,9 +152,9 @@ int enqueue_layers(const DecoderModel& m, const DecoderCache& c, const ChainRows
       j.seg[2] = seg(lw.v, r.v, kvd);
       KLLM_TRY(gemv_dispatch(&j, m.format, s, n));
     }
-    KLLM_TRY(launch_rope_scatter_f32(m, c, l, r.q, r.k, r.v, first_pos, n, s));
+    KLLM_TRY(launch_rope_scatter_f32(m, c, l, r.q, r.k, r.v, at, n, s));
     // attention_mha (llama3.cpp:652-676)
-    KLLM_TRY(launch_mha_rows(first_pos, n, c.cache, m.head_num, l, m.kv_mul, r.att, r.q, r.score, c.key_cache,
+    KLLM_TRY(launch_mha_rows(at, n, c.cache, m.head_num, l, m.kv_mul, r.att, r.q, r.score, c.key_cache,
                              c.value_cache, s));
     KLLM_TRY(residual_gemv(m, lw.o, r.att, q_rows, r.x, tp, n, s));
     // feed_forward (llama3.cpp:686-720)
@@ -175,7 +176,7 @@ int enqueue_verify(const DecoderModel& m, const DecoderCache& c, const VerifyTar
   verify_embed_kernel<<<n, 256, 0, s>>>(ws.io, m.tok_emb, ws.rows.x, m.dim, t.hist, t.rec, ws.saved_hist, ws.saved);
   count_launch();
   KLLM_TRY(cudaGetLastError());
-  KLLM_TRY(enqueue_layers(m, c, ws.rows, n, PosArg{&ws.io->start_pos, 0}, nullptr, s));
+  KLLM_TRY(enqueue_layers(m, c, ws.rows, n, ChainPos{PosArg{&ws.io->start_pos, 0}, nullptr}, nullptr, s));
   verify_draw_kernel<<<n, 1024, 0, s>>>(ws.rows.logits, ws.penalized, ws.marks, m.vocab_size, t.cfg, ws.io, t.hist,
                                         t.rec);
   count_launch();

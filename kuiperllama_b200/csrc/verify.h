@@ -25,10 +25,11 @@ struct TpReduce {
   float* partial;
 };
 
-// Enqueues, for the n positions first_pos, first_pos + 1, .., every layer (q|k|v GEMV, RoPE with the k and v rows
-// written into the cache, attention, Wo with residual, W1|W3 SwiGLU, W2 with residual) and then the final-norm
-// classifier.  tp: null on one GPU.
-int enqueue_layers(const DecoderModel& m, const DecoderCache& c, const ChainRows& rows, int n, PosArg first_pos,
+// Enqueues, for the n rows at `at` (the positions at.first, at.first + 1, .. of the cache c, or a batch's members,
+// each at its own position in its own cache), every layer (q|k|v GEMV, RoPE with the k and v rows written into the
+// cache, attention, Wo with residual, W1|W3 SwiGLU, W2 with residual) and then the final-norm classifier.  With
+// at.members, c gives the layout and the RoPE tables only.  tp: null on one GPU.
+int enqueue_layers(const DecoderModel& m, const DecoderCache& c, const ChainRows& rows, int n, ChainPos at,
                    const TpReduce* tp, cudaStream_t s);
 
 // The final RMSNorm and classifier of n rows x [n][dim] into logits [n][vocab_size]: the chain's last step

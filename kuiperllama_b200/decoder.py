@@ -425,6 +425,13 @@ class Decoder:
         return list(out[:n_out.value]), {"rounds": stats.rounds, "drafted": stats.drafted,
                                          "accepted": stats.accepted}
 
+    def copy_prefix(self, src: "Decoder", n_pos: int):
+        """Copy src's K/V rows, history and record entries of positions [0, n_pos) into this decoder
+        (kllm_decoder_copy_prefix): an entry here that continues at a position <= n_pos then returns what it would on
+        src, under this decoder's own draw settings.  Both must describe the same model on the same engine and
+        cache."""
+        check(self.lib.kllm_decoder_copy_prefix(self.handle, src.handle, int(n_pos)), "kllm_decoder_copy_prefix")
+
     def set_sampling(self, temperature: float, top_k: int = 0, seed: int = 0, top_p: float = 1.0):
         """Draw every later id by the sampling rule (kllm_decoder_set_sampling; sampling.py mirrors it)
         instead of the greedy argmax; temperature 0 is greedy again.  top_p < 1 adds nucleus sampling after
@@ -519,3 +526,51 @@ class Decoder:
         check(self.lib.kllm_decoder_read_kv(self.handle, k.ctypes.data_as(ctypes.c_void_p),
                                             v.ctypes.data_as(ctypes.c_void_p)), "kllm_decoder_read_kv")
         return k, v
+
+
+class Batch:
+    """Owns a ``kllm_batch``: up to MAX_BATCH decoders over one model, stepped in one pass over the weights per step.
+    Each member ends bit for bit as its own step / generate with the same arguments would leave it (kllm_b200.h).
+    Close the batch before its members."""
+
+    def __init__(self, decoders, stream=None):
+        self.lib = load_library()
+        self.members = list(decoders)  # keep the decoders alive while the batch is
+        n = len(self.members)
+        arr = (ctypes.c_void_p * max(n, 1))(*[d.handle.value if d.handle else None for d in self.members])
+        handle = ctypes.c_void_p()
+        stream_ptr = ctypes.c_void_p(stream) if stream else None
+        check(self.lib.kllm_batch_create(arr, n, stream_ptr, ctypes.byref(handle)), "kllm_batch_create")
+        self.handle = handle
+
+    def _rows(self, values):
+        vals = [int(v) for v in values]
+        if len(vals) != len(self.members):
+            raise KllmError(f"{len(vals)} values for {len(self.members)} members")
+        return (ctypes.c_int32 * len(vals))(*vals)
+
+    def step(self, tokens, positions):
+        """One step of every member: tokens[b] fed at positions[b]; returns member b's id at b."""
+        out = (ctypes.c_int32 * len(self.members))()
+        check(self.lib.kllm_batch_step(self.handle, self._rows(tokens), self._rows(positions), out),
+              "kllm_batch_step")
+        return list(out)
+
+    def generate(self, first_tokens, start_positions, n_steps: int):
+        """n_steps steps of every member (kllm_batch_generate); returns one list of n_steps ids per member."""
+        n = len(self.members)
+        out = (ctypes.c_int32 * (n * max(int(n_steps), 1)))()
+        check(self.lib.kllm_batch_generate(self.handle, self._rows(first_tokens), self._rows(start_positions),
+                                           int(n_steps), out), "kllm_batch_generate")
+        return [list(out[b * n_steps:(b + 1) * n_steps]) for b in range(n)]
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.lib.kllm_batch_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
