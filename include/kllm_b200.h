@@ -499,6 +499,39 @@ int kllm_batch_step(kllm_batch* batch, const int32_t* tokens_host, const int32_t
  * NULL pointers, n_steps <= 0, a token outside [0, vocab), start_pos < 0 and start_pos + n_steps > seq_len. */
 int kllm_batch_generate(kllm_batch* batch, const int32_t* first_tokens_host, const int32_t* start_pos_host,
                         int32_t n_steps, int32_t* out_tokens_host);
+/* Every member generates on its own terms in one loop (DESIGN.md 5.15): member b from first_tokens_host[b] at
+ * start_pos_host[b] until the first of its n_stop_host[b] stop ids (row b of stop_ids_host [n][KLLM_MAX_STOP_IDS])
+ * or max_steps_host[b] ids, whichever comes first.
+ *  - Member b ends bit for bit as its own kllm_decoder_generate_until(first_tokens_host[b], start_pos_host[b],
+ *    max_steps_host[b], its stop ids, n_stop_host[b], ...) would leave it: the ids, n_out_host[b],
+ *    kllm_decoder_logits, the history, the log-probability record and the state its own next entry continues from.
+ *    The record has kllm_batch_generate's exception: on the persistent engine a record entry's log-probabilities
+ *    may differ from that engine's own in the last bits.
+ *  - Nothing past a member's end is written: once member b has produced its stop id or its max_steps_host[b]-th
+ *    id, no later pass touches its cache, history, record, logits or state.
+ *  - Row b of out_tokens_host [n][M], M = max_b max_steps_host[b], receives member b's n_out_host[b] ids, the stop
+ *    id included; the rest of the row is not written.
+ *  - Every id of member b reaches on_tokens(ctx, b, ...) (if non-null) exactly once, in order, while the loop runs
+ *    and before the call returns.  The order across members is not specified.  The callback runs on the calling
+ *    thread and must not call into the batch or its members.
+ *  - Each pass carries only the members still running: stats (optional) receives passes = max_b n_out_host[b] and
+ *    rows = sum_b n_out_host[b], the rows summed over the passes.
+ *  - kllm_batch_step and kllm_batch_generate behave as before afterwards.
+ * KLLM_E_INVALID, before any launch and leaving every member unchanged, for NULL pointers (on_tokens and stats may
+ * be NULL), max_steps <= 0, start_pos < 0, start_pos + max_steps > seq_len, n_stop outside [0, KLLM_MAX_STOP_IDS],
+ * and a first token or stop id outside [0, vocab).
+ * The host drives the loop: after each pass it waits for the pass's ids through each member's mapped memory and
+ * decides the stops, then launches the next pass.  The step of k rows is captured as a CUDA graph on first use and
+ * kept; the n-row step is the one kllm_batch_create captured. */
+typedef void (*kllm_batch_token_callback)(void* ctx, int32_t member, const int32_t* ids, int32_t n_ids);
+typedef struct {
+  int32_t passes;
+  int32_t rows;
+} kllm_batch_stats;
+int kllm_batch_generate_until(kllm_batch* batch, const int32_t* first_tokens_host, const int32_t* start_pos_host,
+                              const int32_t* max_steps_host, const int32_t* stop_ids_host, const int32_t* n_stop_host,
+                              kllm_batch_token_callback on_tokens, void* ctx, int32_t* out_tokens_host,
+                              int32_t* n_out_host, kllm_batch_stats* stats);
 
 /* Copies into dst what src holds for positions [0, n_pos): the K/V rows (cache elements as stored: fp32, bf16, or
  * fp8 codes at equal scales, in any layout), the history and the log-probability record entries.  Afterwards any

@@ -42,6 +42,8 @@ class GemvJob(ctypes.Structure):
 ALLREDUCE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_void_p, c_int, c_void_p)
 # kllm_token_callback: (ctx, ids, n_ids), called on the calling thread inside kllm_decoder_generate_until
 TOKEN_CALLBACK = ctypes.CFUNCTYPE(None, c_void_p, POINTER(c_int32), c_int32)
+# kllm_batch_token_callback: (ctx, member, ids, n_ids), called on the calling thread inside kllm_batch_generate_until
+BATCH_TOKEN_CALLBACK = ctypes.CFUNCTYPE(None, c_void_p, c_int32, POINTER(c_int32), c_int32)
 MAX_STOP_IDS = 16  # KLLM_MAX_STOP_IDS
 MAX_TOP_LOGPROBS = 20  # KLLM_MAX_TOP_LOGPROBS
 MAX_VERIFY_TOKENS = 8  # KLLM_MAX_VERIFY_TOKENS: the positions one kllm_decoder_verify pass takes
@@ -51,6 +53,11 @@ MAX_BATCH = 8  # KLLM_MAX_BATCH: the members of one kllm_batch
 class SpecStats(ctypes.Structure):
     """kllm_spec_stats: what kllm_decoder_generate_speculative's rounds did."""
     _fields_ = [("rounds", c_int32), ("drafted", c_int32), ("accepted", c_int32)]
+
+
+class BatchStats(ctypes.Structure):
+    """kllm_batch_stats: the passes of kllm_batch_generate_until and the rows they carried."""
+    _fields_ = [("passes", c_int32), ("rows", c_int32)]
 
 
 class DecoderDesc(ctypes.Structure):
@@ -133,6 +140,9 @@ _SIGNATURES = {
     "kllm_batch_destroy": (None, [c_void_p]),
     "kllm_batch_step": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32)]),
     "kllm_batch_generate": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int32), c_int32, POINTER(c_int32)]),
+    "kllm_batch_generate_until": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
+                                          POINTER(c_int32), POINTER(c_int32), BATCH_TOKEN_CALLBACK, c_void_p,
+                                          POINTER(c_int32), POINTER(c_int32), POINTER(BatchStats)]),
     "kllm_decoder_copy_prefix": (c_int, [c_void_p, c_void_p, c_int32]),
     "kllm_decoder_set_sampling": (c_int, [c_void_p, c_float, c_int32, c_uint64]),
     "kllm_decoder_set_sampling_top_p": (c_int, [c_void_p, c_float, c_int32, c_float, c_uint64]),

@@ -89,7 +89,7 @@ argmax_advance_kernel(const float* __restrict__ logits, int n, const DrawSetting
 }
 
 // What a batch's embedding and draw read and write of one member: the arguments of argmax_advance_kernel in the
-// member's own step, with no streamed ids
+// member's own step.  The streamed ids go to the member's own mapped area, as in its own kllm_decoder_generate_until.
 struct BatchTarget {
   mega::State* st;
   const DrawSettings* cfg;
@@ -99,6 +99,8 @@ struct BatchTarget {
   int32_t* out_tokens;
   const int32_t* teacher;
   float* logits;  // receives the member's row of the batch's logits
+  int32_t* stream_ids;
+  int32_t* stream_count;
 };
 
 // grid (4, members): member blockIdx.y's embedding into row blockIdx.y, as embed_token_kernel's 4 blocks do it
@@ -114,8 +116,8 @@ batch_draw_kernel(const float* __restrict__ logits_rows, int n, const BatchTarge
                   int max_steps) {
   const BatchTarget& mb = members[blockIdx.x];
   const float* row = logits_rows + static_cast<size_t>(blockIdx.x) * n;
-  draw_advance(row, n, mb.cfg, mb.st, mb.out_tokens, mb.teacher, max_steps, nullptr, nullptr, mb.hist, mb.penalized,
-               mb.rec);
+  draw_advance(row, n, mb.cfg, mb.st, mb.out_tokens, mb.teacher, max_steps, mb.stream_ids, mb.stream_count, mb.hist,
+               mb.penalized, mb.rec);
   for (int e = threadIdx.x; e < n; e += blockDim.x) mb.logits[e] = row[e];
 }
 
@@ -262,12 +264,17 @@ struct kllm_batch {
   bool own_stream = false;
   void* buf = nullptr;  // device: the chain's rows [n][.]
   ChainRows rows{};
-  void* tables = nullptr;  // device: the members' ChainMember [n], then their BatchTarget [n]
+  // device: the rows' ChainMember [n], then their BatchTarget [n].  Row r is member r, except inside
+  // kllm_batch_generate_until, which puts the running members first and restores this order before it returns.
+  void* tables = nullptr;
   ChainMember* chain = nullptr;
   BatchTarget* targets = nullptr;
+  void* tables_host = nullptr;  // pinned: the staging of the tables' uploads
   int32_t* io_host = nullptr;  // pinned [n][seq_len]: the ids read back
-  cudaGraphExec_t exec = nullptr;  // embedding, chain and draw of one step, captured at create
-  int launches = 0;
+  // exec[k - 1]: embedding, chain and draw of one step of rows [0, k).  The n-row step is captured at create, the
+  // others on first use by kllm_batch_generate_until.
+  cudaGraphExec_t exec[KLLM_MAX_BATCH] = {};
+  int launches[KLLM_MAX_BATCH] = {};
 };
 
 namespace {
@@ -457,58 +464,27 @@ bool same_model(const kllm_decoder* a, const kllm_decoder* b) {
          ca.head_size == cb.head_size && ca.split == cb.split && ca.elem == cb.elem;
 }
 
-// Embedding, chain and draw of one step of every member: the graph engine's step (enqueue_step) at n rows
-int enqueue_batch(const kllm_batch* b, cudaStream_t s) {
+// Embedding, chain and draw of one step of rows [0, k): the graph engine's step (enqueue_step) at k rows
+int enqueue_batch(const kllm_batch* b, int k, cudaStream_t s) {
   const kllm_decoder* d0 = b->members[0];
   const DecoderModel& m = d0->m;
-  const int n = static_cast<int>(b->members.size());
-  batch_embed_kernel<<<dim3(4, n), 256, 0, s>>>(b->targets, m.tok_emb, b->rows.x, m.dim, m.vocab_size);
+  batch_embed_kernel<<<dim3(4, k), 256, 0, s>>>(b->targets, m.tok_emb, b->rows.x, m.dim, m.vocab_size);
   count_launch();
   KLLM_TRY(cudaGetLastError());
   // the RoPE tables are member 0's: every member's hold the same values (kllm_sincos_init of the same shape)
-  KLLM_TRY(enqueue_layers(m, decoder_cache(d0), b->rows, n, ChainPos{PosArg{nullptr, 0}, b->chain}, nullptr, s));
-  batch_draw_kernel<<<n, 1024, 0, s>>>(b->rows.logits, m.vocab_size, b->targets, m.seq_len);
+  KLLM_TRY(enqueue_layers(m, decoder_cache(d0), b->rows, k, ChainPos{PosArg{nullptr, 0}, b->chain}, nullptr, s));
+  batch_draw_kernel<<<k, 1024, 0, s>>>(b->rows.logits, m.vocab_size, b->targets, m.seq_len);
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }
 
-// The batch's workspace, member tables and captured step
-int batch_prepare(kllm_batch* b) {
-  const DecoderModel& m = b->members[0]->m;
-  const size_t n = b->members.size(), V = m.vocab_size;
-  const size_t per_row = 2 * static_cast<size_t>(m.q_rows) + 2 * m.kv_dim + m.dim + m.hidden_dim + V +
-                         static_cast<size_t>(m.head_num) * m.seq_len;
-  const size_t table_bytes = n * (sizeof(ChainMember) + sizeof(BatchTarget));
-  if (cudaMalloc(&b->buf, per_row * n * sizeof(float)) != cudaSuccess) b->buf = nullptr;
-  if (cudaMalloc(&b->tables, table_bytes) != cudaSuccess) b->tables = nullptr;
-  if (cudaMallocHost(&b->io_host, sizeof(int32_t) * n * m.seq_len) != cudaSuccess) b->io_host = nullptr;
-  if (!b->buf || !b->tables || !b->io_host) return static_cast<int>(cudaErrorMemoryAllocation);
-  float* f = static_cast<float*>(b->buf);
-  auto take = [&](size_t per) {
-    float* r = f;
-    f += per * n;
-    return r;
-  };
-  ChainRows& r = b->rows;
-  r.x = take(m.dim), r.q = take(m.q_rows), r.k = take(m.kv_dim), r.v = take(m.kv_dim), r.att = take(m.q_rows);
-  r.h = take(m.hidden_dim), r.logits = take(V), r.score = take(static_cast<size_t>(m.head_num) * m.seq_len);
-  std::vector<ChainMember> chain(n);
-  std::vector<BatchTarget> targets(n);
-  for (size_t i = 0; i < n; ++i) {
-    kllm_decoder* dc = b->members[i];
-    chain[i] = ChainMember{dc->kcache, dc->vcache, &dc->st->pos};
-    targets[i] = BatchTarget{dc->st, dc->d_cfg, dc->hist, dc->penalized, dc->rec, dc->out_tokens, dc->teacher,
-                             dc->logits};
-  }
-  b->chain = static_cast<ChainMember*>(b->tables);
-  b->targets = reinterpret_cast<BatchTarget*>(static_cast<char*>(b->tables) + n * sizeof(ChainMember));
-  static_assert(sizeof(ChainMember) % alignof(BatchTarget) == 0, "the targets follow the chain table aligned");
-  KLLM_TRY(cudaMemcpy(b->chain, chain.data(), n * sizeof(ChainMember), cudaMemcpyHostToDevice));
-  KLLM_TRY(cudaMemcpy(b->targets, targets.data(), n * sizeof(BatchTarget), cudaMemcpyHostToDevice));
+// The step of k rows, captured once
+int batch_capture(kllm_batch* b, int k) {
+  if (b->exec[k - 1] != nullptr) return 0;
   const uint64_t before = launch_counter().load();
   (void)cudaGetLastError();  // the chain checks its launches with cudaGetLastError: no earlier call's error is its own
   KLLM_TRY(cudaStreamBeginCapture(b->stream, cudaStreamCaptureModeRelaxed));
-  const int rc = enqueue_batch(b, b->stream);
+  const int rc = enqueue_batch(b, k, b->stream);
   cudaGraph_t g = nullptr;
   const cudaError_t end = cudaStreamEndCapture(b->stream, &g);
   // capturing does not execute: undo the launch accounting of the capture pass
@@ -518,11 +494,60 @@ int batch_prepare(kllm_batch* b) {
     if (g) cudaGraphDestroy(g);
     return rc != 0 ? rc : static_cast<int>(end);
   }
-  const cudaError_t inst = cudaGraphInstantiate(&b->exec, g, 0);
+  const cudaError_t inst = cudaGraphInstantiate(&b->exec[k - 1], g, 0);
   cudaGraphDestroy(g);
   KLLM_TRY(inst);
-  b->launches = static_cast<int>(launches);
+  b->launches[k - 1] = static_cast<int>(launches);
   return 0;
+}
+
+size_t table_bytes(const kllm_batch* b) { return b->members.size() * (sizeof(ChainMember) + sizeof(BatchTarget)); }
+
+// Queues the upload of the tables with rows[r] in row r, r < k, from the pinned staging: the caller does not write
+// the staging again before this copy has run
+int put_tables(kllm_batch* b, const int* rows, int k) {
+  const size_t n = b->members.size();
+  auto* chain = static_cast<ChainMember*>(b->tables_host);
+  auto* targets = reinterpret_cast<BatchTarget*>(static_cast<char*>(b->tables_host) + n * sizeof(ChainMember));
+  for (int r = 0; r < k; ++r) {
+    kllm_decoder* dc = b->members[rows[r]];
+    chain[r] = ChainMember{dc->kcache, dc->vcache, &dc->st->pos};
+    targets[r] = BatchTarget{dc->st, dc->d_cfg, dc->hist, dc->penalized, dc->rec, dc->out_tokens, dc->teacher,
+                             dc->logits, dc->stream_dev + kStreamIds, dc->stream_dev};
+  }
+  return static_cast<int>(
+      cudaMemcpyAsync(b->tables, b->tables_host, table_bytes(b), cudaMemcpyHostToDevice, b->stream));
+}
+
+// The batch's workspace, member tables and captured step
+int batch_prepare(kllm_batch* b) {
+  const DecoderModel& m = b->members[0]->m;
+  const int n = static_cast<int>(b->members.size());
+  const size_t V = m.vocab_size;
+  const size_t per_row = 2 * static_cast<size_t>(m.q_rows) + 2 * m.kv_dim + m.dim + m.hidden_dim + V +
+                         static_cast<size_t>(m.head_num) * m.seq_len;
+  if (cudaMalloc(&b->buf, per_row * n * sizeof(float)) != cudaSuccess) b->buf = nullptr;
+  if (cudaMalloc(&b->tables, table_bytes(b)) != cudaSuccess) b->tables = nullptr;
+  if (cudaMallocHost(&b->tables_host, table_bytes(b)) != cudaSuccess) b->tables_host = nullptr;
+  if (cudaMallocHost(&b->io_host, sizeof(int32_t) * n * m.seq_len) != cudaSuccess) b->io_host = nullptr;
+  if (!b->buf || !b->tables || !b->tables_host || !b->io_host) return static_cast<int>(cudaErrorMemoryAllocation);
+  float* f = static_cast<float*>(b->buf);
+  auto take = [&](size_t per) {
+    float* r = f;
+    f += per * n;
+    return r;
+  };
+  ChainRows& r = b->rows;
+  r.x = take(m.dim), r.q = take(m.q_rows), r.k = take(m.kv_dim), r.v = take(m.kv_dim), r.att = take(m.q_rows);
+  r.h = take(m.hidden_dim), r.logits = take(V), r.score = take(static_cast<size_t>(m.head_num) * m.seq_len);
+  b->chain = static_cast<ChainMember*>(b->tables);
+  b->targets = reinterpret_cast<BatchTarget*>(static_cast<char*>(b->tables) + n * sizeof(ChainMember));
+  static_assert(sizeof(ChainMember) % alignof(BatchTarget) == 0, "the targets follow the chain table aligned");
+  int all[KLLM_MAX_BATCH];
+  for (int i = 0; i < n; ++i) all[i] = i;
+  KLLM_TRY(put_tables(b, all, n));
+  KLLM_TRY(cudaStreamSynchronize(b->stream));
+  return batch_capture(b, n);
 }
 
 // n_steps steps of every member from tokens[b] at pos[b]; out [n][n_steps].  Every refusal comes before any launch.
@@ -542,13 +567,83 @@ int run_batch(kllm_batch* b, const int32_t* tokens, const int32_t* pos, int32_t 
     *dc->st_host = mega::State{tokens[i], pos[i], 0, -1, 0, 0, 0, 0};
     KLLM_TRY(cudaMemcpyAsync(dc->st, dc->st_host, sizeof(mega::State), cudaMemcpyHostToDevice, b->stream));
   }
-  for (int32_t i = 0; i < n_steps; ++i) KLLM_TRY(cudaGraphLaunch(b->exec, b->stream));
-  count_launch(static_cast<uint64_t>(b->launches) * n_steps);
+  for (int32_t i = 0; i < n_steps; ++i) KLLM_TRY(cudaGraphLaunch(b->exec[n - 1], b->stream));
+  count_launch(static_cast<uint64_t>(b->launches[n - 1]) * n_steps);
   for (size_t i = 0; i < n; ++i)
     KLLM_TRY(cudaMemcpyAsync(b->io_host + i * n_steps, b->members[i]->out_tokens, sizeof(int32_t) * n_steps,
                              cudaMemcpyDeviceToHost, b->stream));
   KLLM_TRY(cudaStreamSynchronize(b->stream));
   std::memcpy(out, b->io_host, sizeof(int32_t) * n * n_steps);
+  return 0;
+}
+
+// kllm_batch_generate_until's loop, after its refusals.  Pass p launches the step of the k members still running,
+// which are rows [0, k) of the tables, waits for each one's id p through its mapped count and hands it over.  A member
+// whose id p is one of its stop ids or its max_steps-th id is done: the tables are uploaded again with the members
+// still running first, in member order, and the next pass launches the step of their number.  A finished member is
+// in no later pass, so nothing of it is written after its end.
+int run_batch_until(kllm_batch* b, const int32_t* tokens, const int32_t* pos, const int32_t* max_steps,
+                    const int32_t* stop_ids, const int32_t* n_stop, kllm_batch_token_callback on_tokens, void* ctx,
+                    int32_t* out, int32_t* n_out, kllm_batch_stats* stats) {
+  const int n = static_cast<int>(b->members.size());
+  int32_t M = 0;
+  for (int i = 0; i < n; ++i) M = std::max(M, max_steps[i]);
+  for (kllm_decoder* dc : b->members) KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  // each member's state as its own kllm_decoder_generate_until puts it, streamed through its own mapped area
+  for (int i = 0; i < n; ++i) {
+    kllm_decoder* dc = b->members[i];
+    __atomic_store_n(dc->stream_host, 0, __ATOMIC_SEQ_CST);  // before the launch that writes it
+    *dc->st_host = mega::State{tokens[i], pos[i], 0, -1, 0, 1, 0, 0};
+    KLLM_TRY(cudaMemcpyAsync(dc->st, dc->st_host, sizeof(mega::State), cudaMemcpyHostToDevice, b->stream));
+  }
+  int running[KLLM_MAX_BATCH];
+  for (int i = 0; i < n; ++i) running[i] = i, n_out[i] = 0;
+  int k = n, passes = 0, rows = 0;
+  bool reordered = false;
+  int rc = 0;
+  for (int p = 0; k > 0 && rc == 0; ++p) {
+    if (b->exec[k - 1] == nullptr) {  // first use of k rows: captured with nothing in flight
+      if ((rc = static_cast<int>(cudaStreamSynchronize(b->stream))) != 0 || (rc = batch_capture(b, k)) != 0) break;
+    }
+    if ((rc = static_cast<int>(cudaGraphLaunch(b->exec[k - 1], b->stream))) != 0) break;
+    count_launch(static_cast<uint64_t>(b->launches[k - 1]));
+    ++passes, rows += k;
+    int still = 0;
+    for (int r = 0; r < k && rc == 0; ++r) {
+      const int i = running[r];
+      const int32_t* count = b->members[i]->stream_host;
+      while (__atomic_load_n(count, __ATOMIC_ACQUIRE) <= p) {
+        const cudaError_t q = cudaStreamQuery(b->stream);
+        if (q == cudaSuccess && __atomic_load_n(count, __ATOMIC_ACQUIRE) <= p) rc = KLLM_E_STATE;
+        if (q != cudaSuccess && q != cudaErrorNotReady) rc = static_cast<int>(q);
+        if (rc != 0) break;
+      }
+      if (rc != 0) break;
+      const int32_t id = b->members[i]->stream_host[kStreamIds + p];
+      n_out[i] = p + 1;
+      if (on_tokens != nullptr) on_tokens(ctx, i, &id, 1);
+      bool stop = p + 1 == max_steps[i];
+      for (int j = 0; j < n_stop[i]; ++j) stop |= stop_ids[i * KLLM_MAX_STOP_IDS + j] == id;
+      if (!stop) running[still++] = i;
+    }
+    if (rc != 0) break;
+    // the previous upload ran before this pass's step, so the staging is free
+    if (still > 0 && still < k) rc = put_tables(b, running, still), reordered = true;
+    k = still;
+  }
+  // the next call sees every member in its own row again
+  cudaError_t s = cudaStreamSynchronize(b->stream);
+  if (reordered && s == cudaSuccess) {
+    int all[KLLM_MAX_BATCH];
+    for (int i = 0; i < n; ++i) all[i] = i;
+    s = static_cast<cudaError_t>(put_tables(b, all, n));
+    if (s == cudaSuccess) s = cudaStreamSynchronize(b->stream);
+  }
+  if (rc == 0) rc = static_cast<int>(s);
+  if (rc != 0) return rc;
+  for (int i = 0; i < n; ++i)
+    std::memcpy(out + static_cast<size_t>(i) * M, b->members[i]->stream_host + kStreamIds, sizeof(int32_t) * n_out[i]);
+  if (stats != nullptr) *stats = kllm_batch_stats{passes, rows};
   return 0;
 }
 
@@ -1015,9 +1110,11 @@ int kllm_batch_create(kllm_decoder* const* members, int32_t n, void* stream, kll
 void kllm_batch_destroy(kllm_batch* b) {
   if (!b) return;
   if (b->stream) cudaStreamSynchronize(b->stream);
-  if (b->exec) cudaGraphExecDestroy(b->exec);
+  for (cudaGraphExec_t e : b->exec)
+    if (e) cudaGraphExecDestroy(e);
   if (b->buf) cudaFree(b->buf);
   if (b->tables) cudaFree(b->tables);
+  if (b->tables_host) cudaFreeHost(b->tables_host);
   if (b->io_host) cudaFreeHost(b->io_host);
   if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
   delete b;
@@ -1030,6 +1127,30 @@ int kllm_batch_step(kllm_batch* b, const int32_t* tokens_host, const int32_t* po
 int kllm_batch_generate(kllm_batch* b, const int32_t* first_tokens_host, const int32_t* start_pos_host,
                         int32_t n_steps, int32_t* out_tokens_host) {
   return run_batch(b, first_tokens_host, start_pos_host, n_steps, out_tokens_host);
+}
+
+int kllm_batch_generate_until(kllm_batch* b, const int32_t* first_tokens_host, const int32_t* start_pos_host,
+                              const int32_t* max_steps_host, const int32_t* stop_ids_host, const int32_t* n_stop_host,
+                              kllm_batch_token_callback on_tokens, void* ctx, int32_t* out_tokens_host,
+                              int32_t* n_out_host, kllm_batch_stats* stats) {
+  // every refusal comes before the first launch, so a refused call leaves every member as it was
+  if (!b || !first_tokens_host || !start_pos_host || !max_steps_host || !stop_ids_host || !n_stop_host ||
+      !out_tokens_host || !n_out_host)
+    return KLLM_E_INVALID;
+  const DecoderModel& m = b->members[0]->m;
+  for (size_t i = 0; i < b->members.size(); ++i) {
+    const int32_t first = first_tokens_host[i], start = start_pos_host[i], steps = max_steps_host[i];
+    const int32_t n_stop = n_stop_host[i];
+    if (first < 0 || first >= m.vocab_size || start < 0 || steps <= 0) return KLLM_E_INVALID;
+    if (static_cast<int64_t>(start) + steps > m.seq_len) return KLLM_E_INVALID;
+    if (n_stop < 0 || n_stop > KLLM_MAX_STOP_IDS) return KLLM_E_INVALID;
+    for (int32_t j = 0; j < n_stop; ++j) {
+      const int32_t id = stop_ids_host[i * KLLM_MAX_STOP_IDS + j];
+      if (id < 0 || id >= m.vocab_size) return KLLM_E_INVALID;
+    }
+  }
+  return run_batch_until(b, first_tokens_host, start_pos_host, max_steps_host, stop_ids_host, n_stop_host, on_tokens,
+                         ctx, out_tokens_host, n_out_host, stats);
 }
 
 int kllm_decoder_copy_prefix(kllm_decoder* dst, const kllm_decoder* src, int32_t n_pos) {

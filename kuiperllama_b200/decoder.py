@@ -564,6 +564,46 @@ class Batch:
                                            int(n_steps), out), "kllm_batch_generate")
         return [list(out[b * n_steps:(b + 1) * n_steps]) for b in range(n)]
 
+    def generate_until(self, first_tokens, start_positions, max_steps, stop_ids, on_tokens=None):
+        """Member b generates from first_tokens[b] at start_positions[b] until the first id in stop_ids[b] (included)
+        or max_steps[b] ids, and ends as its own Decoder.generate_until would leave it; each pass carries only the
+        members still running (kllm_batch_generate_until).  `on_tokens(member, list_of_ints)` receives every id of
+        every member exactly once, in order per member, while the loop runs; it must not call into the batch or its
+        members.  Returns (one list of ids per member, {"passes": .., "rows": ..})."""
+        from . import BATCH_TOKEN_CALLBACK, MAX_STOP_IDS, BatchStats
+        n = len(self.members)
+        steps = self._rows(max_steps)
+        if len(stop_ids) != n:
+            raise KllmError(f"{len(stop_ids)} stop lists for {n} members")
+        stops = (ctypes.c_int32 * (n * MAX_STOP_IDS))()
+        n_stop = (ctypes.c_int32 * n)()
+        for b, ids in enumerate(stop_ids):
+            ids = [int(t) for t in ids]
+            if len(ids) > MAX_STOP_IDS:
+                raise KllmError(f"member {b}: {len(ids)} stop ids, at most {MAX_STOP_IDS}")
+            stops[b * MAX_STOP_IDS:b * MAX_STOP_IDS + len(ids)] = ids
+            n_stop[b] = len(ids)
+        M = max(list(steps) + [1])
+        out = (ctypes.c_int32 * (n * M))()
+        n_out = (ctypes.c_int32 * n)()
+        stats = BatchStats()
+        errors = []
+
+        def relay(_ctx, member, ids, k):
+            try:
+                on_tokens(member, [ids[i] for i in range(k)])
+            except BaseException as e:  # an exception cannot cross the C frames: re-raised after the call
+                errors.append(e)
+
+        cb = BATCH_TOKEN_CALLBACK(relay) if on_tokens is not None else BATCH_TOKEN_CALLBACK()
+        check(self.lib.kllm_batch_generate_until(self.handle, self._rows(first_tokens), self._rows(start_positions),
+                                                 steps, stops, n_stop, cb, None, out, n_out, ctypes.byref(stats)),
+              "kllm_batch_generate_until")
+        if errors:
+            raise errors[0]
+        return ([list(out[b * M:b * M + n_out[b]]) for b in range(n)],
+                {"passes": stats.passes, "rows": stats.rows})
+
     def close(self):
         if getattr(self, "handle", None):
             self.lib.kllm_batch_destroy(self.handle)
