@@ -239,7 +239,6 @@ struct kllm_decoder {
   mega::State* st_host = nullptr;  // pinned: the state of an entry's first position (put_state), then its last
   sampling::LogprobRecord rec{};   // log-probabilities (kllm_decoder_set_logprobs), indexed by position
   int32_t* io_host = nullptr;     // pinned scratch
-  cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;  // the graph engine's captured step, in the mode of the uploaded state
   int launches_per_step = 0;
   // Mapped pinned host memory that kllm_decoder_generate_until streams the ids through: the count at
@@ -301,11 +300,109 @@ int clear_record(kllm_decoder* dc) {
 
 // An entry's first position, queued for upload with the entry's mode (mega::State): `teacher` feeds the teacher's
 // ids, `streamed` publishes every id to mapped host memory, the steps before `lp_from` are prompt positions, and
-// `lp_target` is kllm_decoder_score's.  The pinned copy stays as written until the entry reads the state back.
-int put_state(kllm_decoder* dc, int32_t token, int32_t pos, int teacher, int streamed, int lp_from, int lp_target) {
+// `lp_target` is kllm_decoder_score's.  The upload goes on stream s, the decoder's own when s is null.  The pinned
+// copy stays as written until the entry reads the state back.
+int put_state(kllm_decoder* dc, int32_t token, int32_t pos, int teacher, int streamed, int lp_from, int lp_target,
+              cudaStream_t s = nullptr) {
   *dc->st_host = mega::State{token, pos, 0, -1, teacher, streamed, lp_from, lp_target};
   return static_cast<int>(cudaMemcpyAsync(dc->st, dc->st_host, sizeof(mega::State), cudaMemcpyHostToDevice,
-                                          dc->stream));
+                                          s != nullptr ? s : dc->stream));
+}
+
+// Reads the state back after an entry's last position: *next is the id drawn there
+int read_next(kllm_decoder* dc, int32_t* next) {
+  KLLM_TRY(cudaMemcpyAsync(dc->st_host, dc->st, sizeof(mega::State), cudaMemcpyDeviceToHost, dc->stream));
+  KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  *next = dc->st_host->next;
+  return 0;
+}
+
+// Queues the upload of tokens[0 .. n) into the teacher through the pinned scratch
+int put_teacher(kllm_decoder* dc, const int32_t* tokens, int n) {
+  std::memcpy(dc->io_host, tokens, sizeof(int32_t) * n);
+  return static_cast<int>(
+      cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n, cudaMemcpyHostToDevice, dc->stream));
+}
+
+// Captures what enqueue() queues on stream s into *exec, and the number of kernels it launched into *launches.
+// Capturing does not execute: the launch accounting of the capture pass is undone.
+template <typename Enqueue>
+int capture_graph(cudaStream_t s, Enqueue&& enqueue, cudaGraphExec_t* exec, int* launches) {
+  (void)cudaGetLastError();  // the chain checks its launches with cudaGetLastError: no earlier call's error is its own
+  const uint64_t before = launch_counter().load();
+  KLLM_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
+  const int rc = enqueue();
+  cudaGraph_t g = nullptr;
+  const cudaError_t end = cudaStreamEndCapture(s, &g);
+  const uint64_t n = launch_counter().load() - before;
+  launch_counter().fetch_sub(n);
+  if (rc != 0 || end != cudaSuccess) {
+    if (g) cudaGraphDestroy(g);
+    return rc != 0 ? rc : static_cast<int>(end);
+  }
+  const cudaError_t inst = cudaGraphInstantiate(exec, g, 0);
+  cudaGraphDestroy(g);
+  KLLM_TRY(inst);
+  *launches = static_cast<int>(n);
+  return 0;
+}
+
+// n launches of a captured graph on stream s, counted as `launches` kernels each
+int replay(cudaGraphExec_t exec, int launches, int n, cudaStream_t s) {
+  for (int i = 0; i < n; ++i) KLLM_TRY(cudaGraphLaunch(exec, s));
+  count_launch(static_cast<uint64_t>(launches) * n);
+  return 0;
+}
+
+// Waits for streamed id i: until the mapped count, which the draw publishes with release semantics, exceeds i.
+// KLLM_E_STATE when stream s finished and the count did not get there, else the stream's own error.  A busy poll,
+// since the wait is on the loop's critical path.
+int wait_streamed(const int32_t* count, int i, cudaStream_t s) {
+  while (__atomic_load_n(count, __ATOMIC_ACQUIRE) <= i) {
+    const cudaError_t q = cudaStreamQuery(s);
+    if (q == cudaSuccess && __atomic_load_n(count, __ATOMIC_ACQUIRE) <= i) return KLLM_E_STATE;
+    if (q != cudaSuccess && q != cudaErrorNotReady) return static_cast<int>(q);
+  }
+  return 0;
+}
+
+// Whether id is one of the stop ids[0 .. n)
+bool hits_stop(const int32_t* ids, int n, int32_t id) {
+  for (int j = 0; j < n; ++j)
+    if (ids[j] == id) return true;
+  return false;
+}
+
+// A stop set of n ids: at most KLLM_MAX_STOP_IDS, given when n > 0, each in the vocabulary
+int stop_args(const int32_t* ids, int32_t n, int vocab) {
+  if (n < 0 || n > KLLM_MAX_STOP_IDS || (n > 0 && ids == nullptr)) return KLLM_E_INVALID;
+  for (int32_t i = 0; i < n; ++i)
+    if (ids[i] < 0 || ids[i] >= vocab) return KLLM_E_INVALID;
+  return 0;
+}
+
+// The arguments kllm_decoder_generate_until and kllm_decoder_generate_speculative share
+int until_args(const kllm_decoder* dc, int32_t start_pos, int32_t max_steps, const int32_t* stop_ids, int32_t n_stop,
+               const int32_t* out_tokens_host, const int32_t* n_out) {
+  if (!dc || !out_tokens_host || !n_out || max_steps <= 0 || start_pos < 0) return KLLM_E_INVALID;
+  if (static_cast<int64_t>(start_pos) + max_steps > dc->m.seq_len) return KLLM_E_INVALID;
+  return stop_args(stop_ids, n_stop, dc->m.vocab_size);
+}
+
+// The next [n][per] floats of a workspace from `cursor`, which moves past them
+float* take(float*& cursor, size_t n, size_t per) {
+  float* r = cursor;
+  cursor += n * per;
+  return r;
+}
+
+// The chain's rows of n positions or members, in the one order the batch and the verify workspace carve them
+ChainRows chain_rows(const DecoderModel& m, size_t n, float*& cursor) {
+  ChainRows r;
+  r.x = take(cursor, n, m.dim), r.q = take(cursor, n, m.q_rows), r.k = take(cursor, n, m.kv_dim);
+  r.v = take(cursor, n, m.kv_dim), r.att = take(cursor, n, m.q_rows), r.h = take(cursor, n, m.hidden_dim);
+  r.logits = take(cursor, n, m.vocab_size), r.score = take(cursor, n, static_cast<size_t>(m.head_num) * m.seq_len);
+  return r;
 }
 
 // Runs n positions from the state put_state queued, in its mode, on the decoder's engine.  The persistent engine
@@ -319,9 +416,7 @@ int run_positions(kllm_decoder* dc, int n) {
     if (s.lp_target) cfg.lp_top_n = std::max(cfg.lp_top_n, 0);
     return dc->mega.run(cfg, n, s.teacher ? dc->teacher : nullptr, nullptr, -1, s.lp_from, s.lp_target);
   }
-  for (int i = 0; i < n; ++i) KLLM_TRY(cudaGraphLaunch(dc->exec, dc->stream));
-  count_launch(static_cast<uint64_t>(dc->launches_per_step) * n);
-  return 0;
+  return replay(dc->exec, dc->launches_per_step, n, dc->stream);
 }
 
 // The decoder's KV cache in its engine's layout -- the persistent engine's, or the graph engine's [seq][kv_dim] --
@@ -335,7 +430,6 @@ DecoderCache decoder_cache(const kllm_decoder* dc) {
 
 int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
   const DecoderModel& m = dc->m;
-  const uint64_t before = launch_counter().load();
   embed_token_kernel<<<4, 256, 0, s>>>(dc->st, m.tok_emb, dc->x, m.dim, m.vocab_size, dc->hist);
   count_launch();
   KLLM_TRY(cudaGetLastError());
@@ -348,26 +442,12 @@ int enqueue_step(kllm_decoder* dc, cudaStream_t s) {
                                            m.seq_len, dc->stream_dev + kStreamIds, dc->stream_dev, dc->hist,
                                            dc->penalized, dc->rec);
   count_launch();
-  KLLM_TRY(cudaGetLastError());
-  dc->launches_per_step = static_cast<int>(launch_counter().load() - before);
-  return 0;
+  return static_cast<int>(cudaGetLastError());
 }
 
+// The graph engine's step, captured once
 int capture(kllm_decoder* dc) {
-  KLLM_TRY(cudaStreamBeginCapture(dc->stream, cudaStreamCaptureModeRelaxed));
-  const int rc = enqueue_step(dc, dc->stream);
-  cudaGraph_t g = nullptr;
-  const cudaError_t end = cudaStreamEndCapture(dc->stream, &g);
-  if (rc != 0) {
-    if (g) cudaGraphDestroy(g);
-    return rc;
-  }
-  KLLM_TRY(end);
-  dc->graph = g;
-  KLLM_TRY(cudaGraphInstantiate(&dc->exec, g, 0));
-  // capturing does not execute: undo the launch accounting of the capture pass
-  launch_counter().fetch_sub(static_cast<uint64_t>(dc->launches_per_step));
-  return 0;
+  return capture_graph(dc->stream, [dc] { return enqueue_step(dc, dc->stream); }, &dc->exec, &dc->launches_per_step);
 }
 
 // The batched prefill behind kllm_decoder_prefill_tf32 / _w8.  Each entry checks the arguments
@@ -393,22 +473,17 @@ int run_prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, 
     const size_t per_row = static_cast<size_t>(3 * m.dim + 2 * q_rows + 2 * kvd + 2 * m.hidden_dim);
     if (cudaMalloc(&dc->pf_buf, per_row * kBlock * sizeof(float)) != cudaSuccess)
       return static_cast<int>(cudaErrorMemoryAllocation);
-    float* p = dc->pf_buf;
-    auto take = [&](size_t n) {
-      float* r = p;
-      p += n * kBlock;
-      return r;
-    };
-    dc->pf_ws.x = take(m.dim), dc->pf_ws.xn = take(m.dim), dc->pf_ws.tmp = take(m.dim);
-    dc->pf_ws.q = take(q_rows), dc->pf_ws.att = take(q_rows);
-    dc->pf_ws.k = take(kvd), dc->pf_ws.v = take(kvd);
-    dc->pf_ws.h1 = take(m.hidden_dim), dc->pf_ws.h3 = take(m.hidden_dim);
+    float* f = dc->pf_buf;
+    PrefillWorkspace& w = dc->pf_ws;
+    w.x = take(f, kBlock, m.dim), w.xn = take(f, kBlock, m.dim), w.tmp = take(f, kBlock, m.dim);
+    w.q = take(f, kBlock, q_rows), w.att = take(f, kBlock, q_rows);
+    w.k = take(f, kBlock, kvd), w.v = take(f, kBlock, kvd);
+    w.h1 = take(f, kBlock, m.hidden_dim), w.h3 = take(f, kBlock, m.hidden_dim);
   }
   KLLM_TRY(prefill_attention_smem_opt_in(static_cast<size_t>(start_pos + n_tokens) * sizeof(float)));
   const DecoderCache pm = decoder_cache(dc);
 
-  std::memcpy(dc->io_host, tokens_host, sizeof(int32_t) * n_tokens);
-  KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_tokens, cudaMemcpyHostToDevice, dc->stream));
+  KLLM_TRY(put_teacher(dc, tokens_host, n_tokens));
   // the prompt rows' history (prefill_args refused ids outside the vocabulary), in stream order before the draw
   KLLM_TRY(cudaMemcpyAsync(dc->hist + start_pos, dc->teacher, sizeof(int32_t) * n_tokens, cudaMemcpyDeviceToDevice,
                            dc->stream));
@@ -427,10 +502,7 @@ int run_prefill(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, 
                                                     m.seq_len, nullptr, nullptr, dc->hist, dc->penalized, dc->rec);
   count_launch();
   KLLM_TRY(cudaGetLastError());
-  KLLM_TRY(cudaMemcpyAsync(dc->st_host, dc->st, sizeof(mega::State), cudaMemcpyDeviceToHost, dc->stream));
-  KLLM_TRY(cudaStreamSynchronize(dc->stream));
-  *next_host = dc->st_host->next;
-  return 0;
+  return read_next(dc, next_host);
 }
 
 // What the verify pass has no counterpart of: the fast numerics' fixed-point rows and flash attention (and with them
@@ -481,24 +553,8 @@ int enqueue_batch(const kllm_batch* b, int k, cudaStream_t s) {
 // The step of k rows, captured once
 int batch_capture(kllm_batch* b, int k) {
   if (b->exec[k - 1] != nullptr) return 0;
-  const uint64_t before = launch_counter().load();
-  (void)cudaGetLastError();  // the chain checks its launches with cudaGetLastError: no earlier call's error is its own
-  KLLM_TRY(cudaStreamBeginCapture(b->stream, cudaStreamCaptureModeRelaxed));
-  const int rc = enqueue_batch(b, k, b->stream);
-  cudaGraph_t g = nullptr;
-  const cudaError_t end = cudaStreamEndCapture(b->stream, &g);
-  // capturing does not execute: undo the launch accounting of the capture pass
-  const uint64_t launches = launch_counter().load() - before;
-  launch_counter().fetch_sub(launches);
-  if (rc != 0 || end != cudaSuccess) {
-    if (g) cudaGraphDestroy(g);
-    return rc != 0 ? rc : static_cast<int>(end);
-  }
-  const cudaError_t inst = cudaGraphInstantiate(&b->exec[k - 1], g, 0);
-  cudaGraphDestroy(g);
-  KLLM_TRY(inst);
-  b->launches[k - 1] = static_cast<int>(launches);
-  return 0;
+  return capture_graph(b->stream, [b, k] { return enqueue_batch(b, k, b->stream); }, &b->exec[k - 1],
+                       &b->launches[k - 1]);
 }
 
 size_t table_bytes(const kllm_batch* b) { return b->members.size() * (sizeof(ChainMember) + sizeof(BatchTarget)); }
@@ -519,6 +575,14 @@ int put_tables(kllm_batch* b, const int* rows, int k) {
       cudaMemcpyAsync(b->tables, b->tables_host, table_bytes(b), cudaMemcpyHostToDevice, b->stream));
 }
 
+// put_tables with every member in its own row
+int put_member_tables(kllm_batch* b) {
+  const int n = static_cast<int>(b->members.size());
+  int all[KLLM_MAX_BATCH];
+  for (int i = 0; i < n; ++i) all[i] = i;
+  return put_tables(b, all, n);
+}
+
 // The batch's workspace, member tables and captured step
 int batch_prepare(kllm_batch* b) {
   const DecoderModel& m = b->members[0]->m;
@@ -532,20 +596,11 @@ int batch_prepare(kllm_batch* b) {
   if (cudaMallocHost(&b->io_host, sizeof(int32_t) * n * m.seq_len) != cudaSuccess) b->io_host = nullptr;
   if (!b->buf || !b->tables || !b->tables_host || !b->io_host) return static_cast<int>(cudaErrorMemoryAllocation);
   float* f = static_cast<float*>(b->buf);
-  auto take = [&](size_t per) {
-    float* r = f;
-    f += per * n;
-    return r;
-  };
-  ChainRows& r = b->rows;
-  r.x = take(m.dim), r.q = take(m.q_rows), r.k = take(m.kv_dim), r.v = take(m.kv_dim), r.att = take(m.q_rows);
-  r.h = take(m.hidden_dim), r.logits = take(V), r.score = take(static_cast<size_t>(m.head_num) * m.seq_len);
+  b->rows = chain_rows(m, n, f);
   b->chain = static_cast<ChainMember*>(b->tables);
   b->targets = reinterpret_cast<BatchTarget*>(static_cast<char*>(b->tables) + n * sizeof(ChainMember));
   static_assert(sizeof(ChainMember) % alignof(BatchTarget) == 0, "the targets follow the chain table aligned");
-  int all[KLLM_MAX_BATCH];
-  for (int i = 0; i < n; ++i) all[i] = i;
-  KLLM_TRY(put_tables(b, all, n));
+  KLLM_TRY(put_member_tables(b));
   KLLM_TRY(cudaStreamSynchronize(b->stream));
   return batch_capture(b, n);
 }
@@ -562,13 +617,8 @@ int run_batch(kllm_batch* b, const int32_t* tokens, const int32_t* pos, int32_t 
   for (kllm_decoder* dc : b->members) KLLM_TRY(cudaStreamSynchronize(dc->stream));
   // each member's state as its own kllm_decoder_generate (no teacher) puts it; the pinned copies stay as written
   // until the synchronisation below
-  for (size_t i = 0; i < n; ++i) {
-    kllm_decoder* dc = b->members[i];
-    *dc->st_host = mega::State{tokens[i], pos[i], 0, -1, 0, 0, 0, 0};
-    KLLM_TRY(cudaMemcpyAsync(dc->st, dc->st_host, sizeof(mega::State), cudaMemcpyHostToDevice, b->stream));
-  }
-  for (int32_t i = 0; i < n_steps; ++i) KLLM_TRY(cudaGraphLaunch(b->exec[n - 1], b->stream));
-  count_launch(static_cast<uint64_t>(b->launches[n - 1]) * n_steps);
+  for (size_t i = 0; i < n; ++i) KLLM_TRY(put_state(b->members[i], tokens[i], pos[i], 0, 0, 0, 0, b->stream));
+  KLLM_TRY(replay(b->exec[n - 1], b->launches[n - 1], n_steps, b->stream));
   for (size_t i = 0; i < n; ++i)
     KLLM_TRY(cudaMemcpyAsync(b->io_host + i * n_steps, b->members[i]->out_tokens, sizeof(int32_t) * n_steps,
                              cudaMemcpyDeviceToHost, b->stream));
@@ -593,8 +643,7 @@ int run_batch_until(kllm_batch* b, const int32_t* tokens, const int32_t* pos, co
   for (int i = 0; i < n; ++i) {
     kllm_decoder* dc = b->members[i];
     __atomic_store_n(dc->stream_host, 0, __ATOMIC_SEQ_CST);  // before the launch that writes it
-    *dc->st_host = mega::State{tokens[i], pos[i], 0, -1, 0, 1, 0, 0};
-    KLLM_TRY(cudaMemcpyAsync(dc->st, dc->st_host, sizeof(mega::State), cudaMemcpyHostToDevice, b->stream));
+    KLLM_TRY(put_state(dc, tokens[i], pos[i], 0, 1, 0, 0, b->stream));
   }
   int running[KLLM_MAX_BATCH];
   for (int i = 0; i < n; ++i) running[i] = i, n_out[i] = 0;
@@ -605,25 +654,16 @@ int run_batch_until(kllm_batch* b, const int32_t* tokens, const int32_t* pos, co
     if (b->exec[k - 1] == nullptr) {  // first use of k rows: captured with nothing in flight
       if ((rc = static_cast<int>(cudaStreamSynchronize(b->stream))) != 0 || (rc = batch_capture(b, k)) != 0) break;
     }
-    if ((rc = static_cast<int>(cudaGraphLaunch(b->exec[k - 1], b->stream))) != 0) break;
-    count_launch(static_cast<uint64_t>(b->launches[k - 1]));
+    if ((rc = replay(b->exec[k - 1], b->launches[k - 1], 1, b->stream)) != 0) break;
     ++passes, rows += k;
     int still = 0;
-    for (int r = 0; r < k && rc == 0; ++r) {
+    for (int r = 0; r < k; ++r) {
       const int i = running[r];
-      const int32_t* count = b->members[i]->stream_host;
-      while (__atomic_load_n(count, __ATOMIC_ACQUIRE) <= p) {
-        const cudaError_t q = cudaStreamQuery(b->stream);
-        if (q == cudaSuccess && __atomic_load_n(count, __ATOMIC_ACQUIRE) <= p) rc = KLLM_E_STATE;
-        if (q != cudaSuccess && q != cudaErrorNotReady) rc = static_cast<int>(q);
-        if (rc != 0) break;
-      }
-      if (rc != 0) break;
+      if ((rc = wait_streamed(b->members[i]->stream_host, p, b->stream)) != 0) break;
       const int32_t id = b->members[i]->stream_host[kStreamIds + p];
       n_out[i] = p + 1;
       if (on_tokens != nullptr) on_tokens(ctx, i, &id, 1);
-      bool stop = p + 1 == max_steps[i];
-      for (int j = 0; j < n_stop[i]; ++j) stop |= stop_ids[i * KLLM_MAX_STOP_IDS + j] == id;
+      const bool stop = p + 1 == max_steps[i] || hits_stop(stop_ids + i * KLLM_MAX_STOP_IDS, n_stop[i], id);
       if (!stop) running[still++] = i;
     }
     if (rc != 0) break;
@@ -634,9 +674,7 @@ int run_batch_until(kllm_batch* b, const int32_t* tokens, const int32_t* pos, co
   // the next call sees every member in its own row again
   cudaError_t s = cudaStreamSynchronize(b->stream);
   if (reordered && s == cudaSuccess) {
-    int all[KLLM_MAX_BATCH];
-    for (int i = 0; i < n; ++i) all[i] = i;
-    s = static_cast<cudaError_t>(put_tables(b, all, n));
+    s = static_cast<cudaError_t>(put_member_tables(b));
     if (s == cudaSuccess) s = cudaStreamSynchronize(b->stream);
   }
   if (rc == 0) rc = static_cast<int>(s);
@@ -669,44 +707,21 @@ int verify_prepare(kllm_decoder* dc, int n) {
     }
     KLLM_TRY(cudaMemsetAsync(dc->vf_buf, 0, bytes, dc->stream));  // the marks start at zero
     float* f = static_cast<float*>(dc->vf_buf);
-    auto take = [&](size_t per) {
-      float* r = f;
-      f += per * N;
-      return r;
-    };
     VerifyWorkspace& w = dc->vf;
-    ChainRows& r = w.rows;
-    r.x = take(m.dim), r.q = take(m.q_rows), r.k = take(m.kv_dim), r.v = take(m.kv_dim), r.att = take(m.q_rows);
-    r.h = take(m.hidden_dim), r.logits = take(V), w.penalized = take(V);
-    r.score = take(static_cast<size_t>(m.head_num) * m.seq_len);
-    w.marks = reinterpret_cast<int32_t*>(take(V));
-    w.saved_hist = reinterpret_cast<int32_t*>(take(1));
-    w.saved.id = reinterpret_cast<int32_t*>(take(1));
-    w.saved.lp = take(1);
-    w.saved.top_ids = reinterpret_cast<int32_t*>(take(T));
-    w.saved.top_lp = take(T);
+    w.rows = chain_rows(m, N, f);
+    w.penalized = take(f, N, V);
+    w.marks = reinterpret_cast<int32_t*>(take(f, N, V));
+    w.saved_hist = reinterpret_cast<int32_t*>(take(f, N, 1));
+    w.saved.id = reinterpret_cast<int32_t*>(take(f, N, 1));
+    w.saved.lp = take(f, N, 1);
+    w.saved.top_ids = reinterpret_cast<int32_t*>(take(f, N, T));
+    w.saved.top_lp = take(f, N, T);
     w.io = reinterpret_cast<VerifyIo*>(f);
   }
   if (dc->vf_exec[n - 1] != nullptr) return 0;
   const VerifyTarget t{dc->d_cfg, dc->st, dc->hist, dc->rec, dc->logits};
-  const uint64_t before = launch_counter().load();
-  (void)cudaGetLastError();  // the chain checks its launches with cudaGetLastError: no earlier call's error is its own
-  KLLM_TRY(cudaStreamBeginCapture(dc->stream, cudaStreamCaptureModeRelaxed));
-  const int rc = enqueue_verify(dc->m, decoder_cache(dc), t, dc->vf, n, dc->stream);
-  cudaGraph_t g = nullptr;
-  const cudaError_t end = cudaStreamEndCapture(dc->stream, &g);
-  // capturing does not execute: undo the launch accounting of the capture pass
-  const uint64_t launches = launch_counter().load() - before;
-  launch_counter().fetch_sub(launches);
-  if (rc != 0 || end != cudaSuccess) {
-    if (g) cudaGraphDestroy(g);
-    return rc != 0 ? rc : static_cast<int>(end);
-  }
-  const cudaError_t inst = cudaGraphInstantiate(&dc->vf_exec[n - 1], g, 0);
-  cudaGraphDestroy(g);
-  KLLM_TRY(inst);
-  dc->vf_launches[n - 1] = static_cast<int>(launches);
-  return 0;
+  return capture_graph(dc->stream, [&] { return enqueue_verify(m, decoder_cache(dc), t, dc->vf, n, dc->stream); },
+                       &dc->vf_exec[n - 1], &dc->vf_launches[n - 1]);
 }
 
 // One verify pass of tokens[0 .. n) at start_pos, acceptance ended at the first of the n_stop stop ids; the caller
@@ -720,8 +735,7 @@ int run_verify(kllm_decoder* dc, const int32_t* tokens, int n, int start_pos, co
   io.n_stop = n_stop;
   if (n_stop > 0) std::memcpy(io.stop, stop_ids, sizeof(int32_t) * n_stop);
   KLLM_TRY(cudaMemcpyAsync(dc->vf.io, &io, offsetof(VerifyIo, ids), cudaMemcpyHostToDevice, dc->stream));
-  KLLM_TRY(cudaGraphLaunch(dc->vf_exec[n - 1], dc->stream));
-  count_launch(static_cast<uint64_t>(dc->vf_launches[n - 1]));
+  KLLM_TRY(replay(dc->vf_exec[n - 1], dc->vf_launches[n - 1], 1, dc->stream));
   KLLM_TRY(cudaMemcpyAsync(io.ids, dc->vf.io->ids, sizeof(int32_t) * (KLLM_MAX_VERIFY_TOKENS + 1),
                            cudaMemcpyDeviceToHost, dc->stream));
   KLLM_TRY(cudaStreamSynchronize(dc->stream));
@@ -840,13 +854,13 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
       cudaHostGetDevicePointer(&dc->stream_dev, dc->stream_host, 0) != cudaSuccess)
     return fail(static_cast<int>(cudaErrorMemoryAllocation));
   std::memset(dc->stream_host, 0, sizeof(int32_t) * (kStreamIds + m.seq_len));
-  cudaMemsetAsync(dc->st, 0, sizeof(mega::State), dc->stream);
-  cudaMemsetAsync(dc->hist, 0xff, sizeof(int32_t) * m.seq_len, dc->stream);  // -1: no id
-  cudaMemsetAsync(dc->marks, 0, sizeof(int32_t) * m.vocab_size, dc->stream);
   DrawSettings off{};  // greedy, step 0 off until a setter turns a sub-step on, logprobs off
   off.penalty.marks = dc->marks;
   off.lp_top_n = -1;
-  int rc = clear_record(dc);
+  int rc = static_cast<int>(cudaMemsetAsync(dc->st, 0, sizeof(mega::State), dc->stream));
+  if (rc == 0) rc = static_cast<int>(cudaMemsetAsync(dc->hist, 0xff, sizeof(int32_t) * m.seq_len, dc->stream));  // -1
+  if (rc == 0) rc = static_cast<int>(cudaMemsetAsync(dc->marks, 0, sizeof(int32_t) * m.vocab_size, dc->stream));
+  if (rc == 0) rc = clear_record(dc);
   if (rc == 0) rc = put_settings(dc, off);
   if (rc != 0) return fail(rc);
 
@@ -888,7 +902,7 @@ int kllm_decoder_create(const kllm_decoder_desc* desc, void* stream, kllm_decode
     return fail(KLLM_E_UNSUPPORTED);
   }
   if (!dc->use_mega && (rc = capture(dc)) != 0) return fail(rc);
-  if (cudaStreamSynchronize(dc->stream) != cudaSuccess) return fail(static_cast<int>(cudaGetLastError()));
+  if (const cudaError_t e = cudaStreamSynchronize(dc->stream)) return fail(static_cast<int>(e));
   *out = dc;
   return 0;
 }
@@ -898,7 +912,6 @@ void kllm_decoder_destroy(kllm_decoder* dc) {
   if (dc->stream) cudaStreamSynchronize(dc->stream);
   dc->mega.destroy();
   if (dc->exec) cudaGraphExecDestroy(dc->exec);
-  if (dc->graph) cudaGraphDestroy(dc->graph);
   float* bufs[] = {dc->x, dc->q, dc->k, dc->v, dc->attn, dc->h, dc->logits, dc->score,
                    dc->kcache, dc->vcache, dc->sin_t, dc->cos_t, dc->tp_tmp, dc->penalized, dc->bias,
                    dc->kv_scales_dev};
@@ -934,9 +947,8 @@ int kllm_decoder_step(kllm_decoder* dc, int32_t token_host, int32_t pos, int is_
   // skips the classifier
   KLLM_TRY(put_state(dc, token_host, pos, 0, 0, is_prompt ? 1 : 0, 0));
   KLLM_TRY(run_positions(dc, 1));
-  KLLM_TRY(cudaMemcpyAsync(dc->st_host, dc->st, sizeof(mega::State), cudaMemcpyDeviceToHost, dc->stream));
-  KLLM_TRY(cudaStreamSynchronize(dc->stream));
-  *next_host = is_prompt ? -1 : dc->st_host->next;
+  KLLM_TRY(read_next(dc, next_host));
+  if (is_prompt) *next_host = -1;
   return 0;
 }
 
@@ -944,17 +956,12 @@ int kllm_decoder_prompt(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_
                         int32_t* next_host) {
   if (!dc || !tokens_host || !next_host || n_tokens <= 0 || start_pos < 0) return KLLM_E_INVALID;
   if (start_pos + n_tokens > dc->m.seq_len) return KLLM_E_INVALID;
-  std::memcpy(dc->io_host, tokens_host, sizeof(int32_t) * n_tokens);
-  KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_tokens, cudaMemcpyHostToDevice,
-                           dc->stream));
+  KLLM_TRY(put_teacher(dc, tokens_host, n_tokens));
   // teacher forced; only the last position records an entry (and, on the persistent engine, runs the classifier:
   // ONE launch for the whole prompt)
   KLLM_TRY(put_state(dc, tokens_host[0], start_pos, 1, 0, n_tokens - 1, 0));
   KLLM_TRY(run_positions(dc, n_tokens));
-  KLLM_TRY(cudaMemcpyAsync(dc->st_host, dc->st, sizeof(mega::State), cudaMemcpyDeviceToHost, dc->stream));
-  KLLM_TRY(cudaStreamSynchronize(dc->stream));
-  *next_host = dc->st_host->next;
-  return 0;
+  return read_next(dc, next_host);
 }
 
 int kllm_decoder_prefill_tf32(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_tokens, int32_t start_pos,
@@ -988,11 +995,7 @@ int kllm_decoder_generate(kllm_decoder* dc, int32_t first_token, int32_t start_p
                           int32_t* out_tokens_host) {
   if (!dc || n_steps <= 0 || start_pos < 0) return KLLM_E_INVALID;
   if (start_pos + n_steps > dc->m.seq_len) return KLLM_E_INVALID;
-  if (teacher_host) {
-    std::memcpy(dc->io_host, teacher_host, sizeof(int32_t) * n_steps);
-    KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_steps,
-                             cudaMemcpyHostToDevice, dc->stream));
-  }
+  if (teacher_host) KLLM_TRY(put_teacher(dc, teacher_host, n_steps));
   KLLM_TRY(put_state(dc, teacher_host ? teacher_host[0] : first_token, start_pos, teacher_host != nullptr, 0, 0, 0));
   KLLM_TRY(run_positions(dc, n_steps));
   if (out_tokens_host) {
@@ -1008,11 +1011,7 @@ int kllm_decoder_generate_until(kllm_decoder* dc, int32_t first_token, int32_t s
                                 const int32_t* stop_ids, int32_t n_stop, kllm_token_callback on_tokens, void* ctx,
                                 int32_t* out_tokens_host, int32_t* n_out) {
   // every refusal comes before the first launch, so a refused call leaves the decoder as it was
-  if (!dc || !out_tokens_host || !n_out || max_steps <= 0 || start_pos < 0) return KLLM_E_INVALID;
-  if (static_cast<int64_t>(start_pos) + max_steps > dc->m.seq_len) return KLLM_E_INVALID;
-  if (n_stop < 0 || n_stop > KLLM_MAX_STOP_IDS || (n_stop > 0 && stop_ids == nullptr)) return KLLM_E_INVALID;
-  for (int i = 0; i < n_stop; ++i)
-    if (stop_ids[i] < 0 || stop_ids[i] >= dc->m.vocab_size) return KLLM_E_INVALID;
+  KLLM_TRY(until_args(dc, start_pos, max_steps, stop_ids, n_stop, out_tokens_host, n_out));
   *n_out = 0;
   int32_t* count = dc->stream_host;
   const int32_t* ids = dc->stream_host + kStreamIds;
@@ -1043,19 +1042,12 @@ int kllm_decoder_generate_until(kllm_decoder* dc, int32_t first_token, int32_t s
     // One captured step per launch, driven from the host: wait for the step's id through the mapped count,
     // then stop or launch the next step.  No step runs after the stop, on any tensor-parallel rank.
     for (int i = 0; i < max_steps;) {
-      KLLM_TRY(cudaGraphLaunch(dc->exec, dc->stream));
-      count_launch(static_cast<uint64_t>(dc->launches_per_step));
-      while (__atomic_load_n(count, __ATOMIC_ACQUIRE) <= i) {
-        const cudaError_t q = cudaStreamQuery(dc->stream);
-        if (q == cudaSuccess && __atomic_load_n(count, __ATOMIC_ACQUIRE) <= i) return KLLM_E_STATE;
-        if (q != cudaSuccess && q != cudaErrorNotReady) return static_cast<int>(q);
-      }
+      KLLM_TRY(replay(dc->exec, dc->launches_per_step, 1, dc->stream));
+      KLLM_TRY(wait_streamed(count, i, dc->stream));
       const int32_t id = ids[i++];
       if (on_tokens != nullptr) on_tokens(ctx, &id, 1);
       n = i;
-      bool stop = false;
-      for (int j = 0; j < n_stop; ++j) stop |= stop_ids[j] == id;
-      if (stop) break;
+      if (hits_stop(stop_ids, n_stop, id)) break;
     }
     KLLM_TRY(cudaStreamSynchronize(dc->stream));
   }
@@ -1140,14 +1132,9 @@ int kllm_batch_generate_until(kllm_batch* b, const int32_t* first_tokens_host, c
   const DecoderModel& m = b->members[0]->m;
   for (size_t i = 0; i < b->members.size(); ++i) {
     const int32_t first = first_tokens_host[i], start = start_pos_host[i], steps = max_steps_host[i];
-    const int32_t n_stop = n_stop_host[i];
     if (first < 0 || first >= m.vocab_size || start < 0 || steps <= 0) return KLLM_E_INVALID;
     if (static_cast<int64_t>(start) + steps > m.seq_len) return KLLM_E_INVALID;
-    if (n_stop < 0 || n_stop > KLLM_MAX_STOP_IDS) return KLLM_E_INVALID;
-    for (int32_t j = 0; j < n_stop; ++j) {
-      const int32_t id = stop_ids_host[i * KLLM_MAX_STOP_IDS + j];
-      if (id < 0 || id >= m.vocab_size) return KLLM_E_INVALID;
-    }
+    KLLM_TRY(stop_args(stop_ids_host + i * KLLM_MAX_STOP_IDS, n_stop_host[i], m.vocab_size));
   }
   return run_batch_until(b, first_tokens_host, start_pos_host, max_steps_host, stop_ids_host, n_stop_host, on_tokens,
                          ctx, out_tokens_host, n_out_host, stats);
@@ -1197,11 +1184,7 @@ int kllm_decoder_generate_speculative(kllm_decoder* dc, int32_t first_token, int
                                       kllm_token_callback on_tokens, void* ctx, int32_t* out_tokens_host,
                                       int32_t* n_out, kllm_spec_stats* stats) {
   // every refusal comes before the first launch, so a refused call leaves the decoder as it was
-  if (!dc || !out_tokens_host || !n_out || max_steps <= 0 || start_pos < 0) return KLLM_E_INVALID;
-  if (static_cast<int64_t>(start_pos) + max_steps > dc->m.seq_len) return KLLM_E_INVALID;
-  if (n_stop < 0 || n_stop > KLLM_MAX_STOP_IDS || (n_stop > 0 && stop_ids == nullptr)) return KLLM_E_INVALID;
-  for (int i = 0; i < n_stop; ++i)
-    if (stop_ids[i] < 0 || stop_ids[i] >= dc->m.vocab_size) return KLLM_E_INVALID;
+  KLLM_TRY(until_args(dc, start_pos, max_steps, stop_ids, n_stop, out_tokens_host, n_out));
   if (draft_len < 1 || draft_len >= KLLM_MAX_VERIFY_TOKENS || ngram_max < 1 || ngram_max > 8) return KLLM_E_INVALID;
   if (first_token < 0 || first_token >= dc->m.vocab_size) return KLLM_E_INVALID;
   KLLM_TRY(verify_supported(dc));
@@ -1225,9 +1208,7 @@ int kllm_decoder_generate_speculative(kllm_decoder* dc, int32_t first_token, int
     if (k == 0) {  // no draft: one plain step on the decoder's engine
       KLLM_TRY(put_state(dc, c[p], p, 0, 0, 0, 0));
       KLLM_TRY(run_positions(dc, 1));
-      KLLM_TRY(cudaMemcpyAsync(dc->st_host, dc->st, sizeof(mega::State), cudaMemcpyDeviceToHost, dc->stream));
-      KLLM_TRY(cudaStreamSynchronize(dc->stream));
-      ids[0] = dc->st_host->next;
+      KLLM_TRY(read_next(dc, &ids[0]));
     } else {
       tokens[0] = c[p];
       KLLM_TRY(run_verify(dc, tokens, k + 1, p, stop_ids, n_stop, ids, &a));
@@ -1237,9 +1218,7 @@ int kllm_decoder_generate_speculative(kllm_decoder* dc, int32_t first_token, int
     std::memcpy(out_tokens_host + produced, ids, sizeof(int32_t) * (a + 1));
     std::memcpy(c.data() + p + 1, ids, sizeof(int32_t) * (a + 1));
     produced += a + 1;
-    bool stop = false;
-    for (int j = 0; j < n_stop; ++j) stop |= stop_ids[j] == ids[a];
-    if (stop) break;
+    if (hits_stop(stop_ids, n_stop, ids[a])) break;
   }
   *n_out = produced;
   return 0;
@@ -1336,8 +1315,7 @@ int kllm_decoder_score(kllm_decoder* dc, const int32_t* tokens_host, int32_t n_t
     if (tokens_host[i] < 0 || tokens_host[i] >= dc->m.vocab_size) return KLLM_E_INVALID;
   const int steps = n_tokens - 1;
   // the targets: the teacher holds all n tokens, one more than the positions run, so step i's target is [i + 1]
-  std::memcpy(dc->io_host, tokens_host, sizeof(int32_t) * n_tokens);
-  KLLM_TRY(cudaMemcpyAsync(dc->teacher, dc->io_host, sizeof(int32_t) * n_tokens, cudaMemcpyHostToDevice, dc->stream));
+  KLLM_TRY(put_teacher(dc, tokens_host, n_tokens));
   KLLM_TRY(put_state(dc, tokens_host[0], start_pos, 1, 0, 0, 1));
   KLLM_TRY(run_positions(dc, steps));
   KLLM_TRY(cudaMemcpyAsync(dc->io_host, dc->rec.lp + start_pos, sizeof(float) * steps, cudaMemcpyDeviceToHost,

@@ -200,6 +200,24 @@ def _ptr_array(tensors):
     return arr
 
 
+def _relay(on_tokens, callback_type):
+    """The `callback_type` callback that hands each call's ids to on_tokens (its leading arguments, then the ids as a
+    list), or a null one for on_tokens None; and the list that keeps what on_tokens raised.  An exception cannot cross
+    the C frames: the caller re-raises errors[0] after the call."""
+    errors = []
+    if on_tokens is None:
+        return callback_type(), errors
+
+    def relay(_ctx, *args):
+        *lead, ids, n = args
+        try:
+            on_tokens(*lead, [ids[i] for i in range(n)])
+        except BaseException as e:
+            errors.append(e)
+
+    return callback_type(relay), errors
+
+
 class Decoder:
     """Owns a ``kllm_decoder`` built over torch-held device weights."""
 
@@ -321,33 +339,27 @@ class Decoder:
               "kllm_decoder_step")
         return nxt.value
 
+    def _feed(self, entry: str, tokens, start_pos: int) -> int:
+        """Calls the prompt-style C entry `entry` (tokens, n, start_pos, &next) and returns next."""
+        n = len(tokens)
+        arr = (ctypes.c_int32 * n)(*[int(t) for t in tokens])
+        nxt = ctypes.c_int32(-1)
+        check(getattr(self.lib, entry)(self.handle, arr, n, start_pos, ctypes.byref(nxt)), entry)
+        return nxt.value
+
     def prompt(self, tokens, start_pos: int = 0) -> int:
         """Feed a whole prompt (one launch on the persistent engine, classifier only for the last
         position); returns the greedy id that follows the prompt."""
-        n = len(tokens)
-        arr = (ctypes.c_int32 * n)(*[int(t) for t in tokens])
-        nxt = ctypes.c_int32(-1)
-        check(self.lib.kllm_decoder_prompt(self.handle, arr, n, start_pos, ctypes.byref(nxt)), "kllm_decoder_prompt")
-        return nxt.value
+        return self._feed("kllm_decoder_prompt", tokens, start_pos)
 
     def prefill_tf32(self, tokens, start_pos: int = 0) -> int:
         """TOLERANCED batched prefill on the Hopper tensor cores (wgmma) (TF32); same contract as prompt()."""
-        n = len(tokens)
-        arr = (ctypes.c_int32 * n)(*[int(t) for t in tokens])
-        nxt = ctypes.c_int32(-1)
-        check(self.lib.kllm_decoder_prefill_tf32(self.handle, arr, n, start_pos, ctypes.byref(nxt)),
-              "kllm_decoder_prefill_tf32")
-        return nxt.value
+        return self._feed("kllm_decoder_prefill_tf32", tokens, start_pos)
 
     def prefill_w8(self, tokens, start_pos: int = 0) -> int:
         """TOLERANCED batched prefill of an int8 checkpoint: the weight tiles are dequantised to TF32 on the way
         to the same wgmma GEMM as prefill_tf32(); same contract as prompt()."""
-        n = len(tokens)
-        arr = (ctypes.c_int32 * n)(*[int(t) for t in tokens])
-        nxt = ctypes.c_int32(-1)
-        check(self.lib.kllm_decoder_prefill_w8(self.handle, arr, n, start_pos, ctypes.byref(nxt)),
-              "kllm_decoder_prefill_w8")
-        return nxt.value
+        return self._feed("kllm_decoder_prefill_w8", tokens, start_pos)
 
     def generate(self, first_token: int, start_pos: int, n_steps: int, teacher=None):
         out = (ctypes.c_int32 * n_steps)()
@@ -367,15 +379,7 @@ class Decoder:
         sarr = (ctypes.c_int32 * max(len(stops), 1))(*stops)
         out = (ctypes.c_int32 * max(int(max_steps), 1))()
         n_out = ctypes.c_int32(0)
-        errors = []
-
-        def relay(_ctx, ids, n):
-            try:
-                on_tokens([ids[i] for i in range(n)])
-            except BaseException as e:  # an exception cannot cross the C frames: re-raised after the call
-                errors.append(e)
-
-        cb = TOKEN_CALLBACK(relay) if on_tokens is not None else TOKEN_CALLBACK()
+        cb, errors = _relay(on_tokens, TOKEN_CALLBACK)
         check(self.lib.kllm_decoder_generate_until(self.handle, int(first_token), int(start_pos), int(max_steps),
                                                    sarr, len(stops), cb, None, out, ctypes.byref(n_out)),
               "kllm_decoder_generate_until")
@@ -407,15 +411,7 @@ class Decoder:
         out = (ctypes.c_int32 * max(int(max_steps), 1))()
         n_out = ctypes.c_int32(0)
         stats = SpecStats()
-        errors = []
-
-        def relay(_ctx, ids, n):
-            try:
-                on_tokens([ids[i] for i in range(n)])
-            except BaseException as e:  # an exception cannot cross the C frames: re-raised after the call
-                errors.append(e)
-
-        cb = TOKEN_CALLBACK(relay) if on_tokens is not None else TOKEN_CALLBACK()
+        cb, errors = _relay(on_tokens, TOKEN_CALLBACK)
         check(self.lib.kllm_decoder_generate_speculative(self.handle, int(first_token), int(start_pos), int(max_steps),
                                                          sarr, len(stops), int(draft_len), int(ngram_max), cb, None,
                                                          out, ctypes.byref(n_out), ctypes.byref(stats)),
@@ -587,15 +583,7 @@ class Batch:
         out = (ctypes.c_int32 * (n * M))()
         n_out = (ctypes.c_int32 * n)()
         stats = BatchStats()
-        errors = []
-
-        def relay(_ctx, member, ids, k):
-            try:
-                on_tokens(member, [ids[i] for i in range(k)])
-            except BaseException as e:  # an exception cannot cross the C frames: re-raised after the call
-                errors.append(e)
-
-        cb = BATCH_TOKEN_CALLBACK(relay) if on_tokens is not None else BATCH_TOKEN_CALLBACK()
+        cb, errors = _relay(on_tokens, BATCH_TOKEN_CALLBACK)
         check(self.lib.kllm_batch_generate_until(self.handle, self._rows(first_tokens), self._rows(start_positions),
                                                  steps, stops, n_stop, cb, None, out, n_out, ctypes.byref(stats)),
               "kllm_batch_generate_until")
