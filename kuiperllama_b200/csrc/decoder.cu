@@ -1340,8 +1340,8 @@ int kllm_decoder_profile(kllm_decoder* dc, int32_t first_token, int32_t start_po
   KLLM_TRY(put_state(dc, first_token, start_pos, 0, 0, 0, 0));
   unsigned long long* d_prof = nullptr;
   KLLM_TRY(cudaMalloc(&d_prof, n * sizeof(unsigned long long)));
-  cudaMemsetAsync(d_prof, 0, n * sizeof(unsigned long long), dc->stream);
-  int rc = dc->mega.run(dc->cfg, n_steps, nullptr, d_prof, profiled_step);
+  int rc = static_cast<int>(cudaMemsetAsync(d_prof, 0, n * sizeof(unsigned long long), dc->stream));
+  if (rc == 0) rc = dc->mega.run(dc->cfg, n_steps, nullptr, d_prof, profiled_step);
   if (rc == 0) rc = static_cast<int>(cudaStreamSynchronize(dc->stream));
   if (rc == 0)
     rc = static_cast<int>(cudaMemcpy(stamps_host, d_prof, n * sizeof(unsigned long long),

@@ -2394,16 +2394,15 @@ constexpr int kW16StageBytes = 32 * 1024;
 constexpr int kW16FastStageBytes = 24 * 1024;
 }  // namespace
 
+// In order: decide the geometry and every refusal, then allocate the scratch block, then fill it and the launch
+// parameters.  Nothing after the allocation refuses.
 int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t stream) {
-  dm_ = &dm;
-  model_ = m;
-  stream_ = stream;
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return KLLM_E_NODEVICE;
   int sms = 0, coop = 0, max_smem = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-  cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  KLLM_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  KLLM_TRY(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+  KLLM_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   if (!coop) return KLLM_E_UNSUPPORTED;
 
   const int dim = dm.dim, hid = dm.hidden_dim, hs = dm.head_size, kvd = dm.kv_dim, q_rows = dm.q_rows;
@@ -2413,8 +2412,8 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
   // One CTA per SM, but never more CTAs than the shortest row-parallel phase has rows: the
   // slot-reuse argument of the tagged hand-offs wants every CTA to own rows in every producing
   // phase (a CTA without rows gates nothing and could be overtaken).  Small test shapes only.
-  grid_ = std::min(sms, std::min(dim, hid));
-  if (grid_ < dm.head_num) return KLLM_E_UNSUPPORTED;  // attention: one CTA per (local) query head
+  const int grid = std::min(sms, std::min(dim, hid));
+  if (grid < dm.head_num) return KLLM_E_UNSUPPORTED;  // attention: one CTA per (local) query head
   // shapes the ring handles: 16-byte rows, 128-byte aligned kv rows (L1-cached reads stay exact);
   // head_size <= 128: the K-tile producer issues one bulk copy per lane for hs/4 <= 32 chunk columns
   if ((dim & 3) || (hid & 3) || (q_rows & 3) || (hs & 3) || hs > 128) return KLLM_E_UNSUPPORTED;
@@ -2430,19 +2429,17 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
   // bit; "fast" is the dp4a fixed-point mode (toleranced, ~3.5x fewer instructions)
   // The same switch frees the attention's summation order (flash-decoding, attention_flash_phase).
   // kllm_decoder_desc::numerics picks the mode; KLLM_MODE=exact|fast overrides.
-  fast_ = m.numerics == 1 ? 1 : 0;
-  if (const char* e = getenv("KLLM_MODE")) fast_ = std::string(e) == "fast" ? 1 : 0;
-  int8_fast_ = (int8 && fast_) ? 1 : 0;
+  int fast = m.numerics == 1 ? 1 : 0;
+  if (const char* e = getenv("KLLM_MODE")) fast = std::string(e) == "fast" ? 1 : 0;
   // bf16 and fp8 KV caches: toleranced variants of the flash attention only, over 16-byte chunks of 8 (bf16) or 16
   // (fp8) dims with a quarter of the head per lane (head_size % 32 == 0, % 64 == 0); refused rather than run in any
   // other form
-  if (m.kv_cache != KLLM_KV_F32 && m.kv_cache != KLLM_KV_BF16 && m.kv_cache != KLLM_KV_FP8) return KLLM_E_INVALID;
-  kv_elem_ = m.kv_cache;
-  const int kv_esz = prefill::kv_elem_bytes(kv_elem_);  // bytes per cached element
-  if (kv_elem_ != KLLM_KV_F32 && (!fast_ || m.tp_world > 1 || hs % (64 / kv_esz) != 0)) return KLLM_E_UNSUPPORTED;
-  if (kv_elem_ == KLLM_KV_FP8 && m.kv_scales == nullptr) return KLLM_E_INVALID;
-  const Kernels ks = kernels_for(dm.format, kv_elem_);
-  kernel_ = ks.plain, kernel_prof_ = ks.prof, kernel_lp_ = ks.lp;
+  const int kv = m.kv_cache;
+  if (kv != KLLM_KV_F32 && kv != KLLM_KV_BF16 && kv != KLLM_KV_FP8) return KLLM_E_INVALID;
+  const int kv_esz = prefill::kv_elem_bytes(kv);  // bytes per cached element
+  if (kv != KLLM_KV_F32 && (!fast || m.tp_world > 1 || hs % (64 / kv_esz) != 0)) return KLLM_E_UNSUPPORTED;
+  if (kv == KLLM_KV_FP8 && m.kv_scales == nullptr) return KLLM_E_INVALID;
+  const Kernels ks = kernels_for(dm.format, kv);
 
   // The residual exchange after o_proj and down_proj is tagged (under tensor parallelism it IS the
   // all-reduce), and so are the hand-offs q|k|v -> attention -> Wo and SwiGLU -> W2: the one grid
@@ -2466,14 +2463,14 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
   // against 627 with 32 KB (20 KB: 649, 24 KB: 645), Qwen2.5-0.5B 1058 against 1032.  At dim 4096 a 16 KB stage is
   // ONE row, a task no longer shares its x loads, and Llama-2-7B fell from 108 to 80 tok/s.  The flash tiles shrink
   // with the stage (head_size 64: 64 timesteps).
-  const bool small_stages = fast_ && kv_elem_ == KLLM_KV_F32 && !w16 && 2 * dim * 4 <= 16 * 1024;
-  int stage_bytes = int8 ? 27 * 1024 : w16 ? (fast_ ? kW16FastStageBytes : kW16StageBytes) : small_stages ? 16 * 1024
-                                                                                                 : 32 * 1024;
+  const bool small_stages = fast && kv == KLLM_KV_F32 && !w16 && 2 * dim * 4 <= 16 * 1024;
+  int stage_bytes = int8 ? 27 * 1024 : w16 ? (fast ? kW16FastStageBytes : kW16StageBytes) : small_stages ? 16 * 1024
+                                                                                                : 32 * 1024;
   if (const char* e = getenv("KLLM_STAGE_BYTES")) stage_bytes = atoi(e);
   stage_bytes = (stage_bytes + 127) & ~127;
-  attn_tile_ = std::min(stage_bytes / (hs * kv_esz), mega::kConsumerThreads) & ~31;  // one timestep per consumer thread
-  if (attn_tile_ < 32) return KLLM_E_UNSUPPORTED;
-  if (fast_) {  // flash attention: a lane quartet per timestep, warp partials (m, l, o[hs]) in the input buffer
+  const int attn_tile = std::min(stage_bytes / (hs * kv_esz), mega::kConsumerThreads) & ~31;  // a timestep per thread
+  if (attn_tile < 32) return KLLM_E_UNSUPPORTED;
+  if (fast) {  // flash attention: a lane quartet per timestep, warp partials (m, l, o[hs]) in the input buffer
     if (hs & 15) return KLLM_E_UNSUPPORTED;
     xbuf = std::max(xbuf, (2 * hs + mega::kConsumerWarps * (hs + 2)) * 4);
   }
@@ -2487,39 +2484,31 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
   int stages = budget / stage_bytes;
   if (stages > mega::kMaxStages) stages = mega::kMaxStages;
   if (stages < 2) return KLLM_E_UNSUPPORTED;
-  stage_bytes_ = stage_bytes;
-  stages_ = stages;
   // attention split: SP CTAs per query head (power of two, <= 8), each owning head_size / SP output dims
   // (a multiple of 4 floats so that V slice rows stay 16-byte units for the bulk copies)
   if (dm.seq_len & 3) return KLLM_E_UNSUPPORTED;
-  attn_split_ = 1;
-  while (attn_split_ * 2 <= 8 && dm.head_num * attn_split_ * 2 <= grid_ && (hs / (attn_split_ * 2)) % 4 == 0 &&
-         hs % (attn_split_ * 2) == 0)
-    attn_split_ *= 2;
-  const int attn_split_max = attn_split_;
+  int split = 1;
+  while (split * 2 <= 8 && dm.head_num * split * 2 <= grid && (hs / (split * 2)) % 4 == 0 && hs % (split * 2) == 0)
+    split *= 2;
+  int split_cap = split;
   // The split costs one more hand-off per layer: worth it when a head's K and V are big
   // (head_size 128: 1 MB per head at context 1024), not for head_size 64.
-  if (hs < 128) attn_split_ = 1;
-  int split_cap = attn_split_max;
-  if (fast_) {  // flash: split by timestep, any power of two whose partial triples fit the scores area
-    attn_split_ = 1;
-    while (attn_split_ * 2 <= 8 && dm.head_num * attn_split_ * 2 <= grid_ && attn_split_ * 2 * (hs + 2) <= dm.seq_len)
-      attn_split_ *= 2;
-    split_cap = attn_split_;
+  if (hs < 128) split = 1;
+  if (fast) {  // flash: split by timestep, any power of two whose partial triples fit the scores area
+    split = 1;
+    while (split * 2 <= 8 && dm.head_num * split * 2 <= grid && split * 2 * (hs + 2) <= dm.seq_len) split *= 2;
+    split_cap = split;
   }
   if (const char* e = getenv("KLLM_ATTN_SPLIT")) {
     const int v = atoi(e);
-    if (v >= 1 && v <= split_cap && (v & (v - 1)) == 0) attn_split_ = v;
+    if (v >= 1 && v <= split_cap && (v & (v - 1)) == 0) split = v;
   }
-  attn_vsplit_ = fast_ ? 1 : attn_split_;
-  attn_tile_v_ = (stage_bytes / ((hs / attn_vsplit_) * kv_esz)) & ~31;
-  if (attn_tile_v_ < 32) return KLLM_E_UNSUPPORTED;
-  xbuf_bytes_ = xbuf;
-  xres_bytes_ = xres;
-  smem_bytes_ = static_cast<size_t>(xbuf) + xres + static_cast<size_t>(stages) * stage_bytes;
+  const int vsplit = fast ? 1 : split;
+  const int attn_tile_v = (stage_bytes / ((hs / vsplit) * kv_esz)) & ~31;
+  if (attn_tile_v < 32) return KLLM_E_UNSUPPORTED;
+  const size_t smem_bytes = static_cast<size_t>(xbuf) + xres + static_cast<size_t>(stages) * stage_bytes;
 
-  // ---- phase table ---------------------------------------------------------------------------------
-  std::vector<Phase> ph;
+  // ---- the ring plan of every GEMV phase ----------------------------------------------------------------
   auto plan = [&](Phase& p) -> int {
     const int row_bytes = p.in_dim * wb;
     p.group_size = dm.group_size;
@@ -2555,26 +2544,55 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
     }
     return 0;
   };
+  // The plan depends only on the input length and the SwiGLU pairing: one per GEMV of the table, decided here.
+  Phase qkv{}, wo{}, ffn{}, w2{}, cls{};
+  qkv.in_dim = dim, wo.in_dim = q_rows, ffn.in_dim = dim, ffn.swiglu = 1, w2.in_dim = hid, cls.in_dim = dim;
+  for (Phase* p : {&qkv, &wo, &ffn, &w2, &cls})
+    if (int rc = plan(*p)) return rc;
+  // Tensor parallel: shard the classifier by vocabulary when the exchange area can carry a rank's
+  // rows (kllm_comm_create(max_count >= vocab / world)); every rank still holds the whole matrix and
+  // reads only its rows.  Otherwise it stays replicated.
+  const int V = dm.vocab_size;
+  const bool shard = W > 1 && V % W == 0 && m.tp_stride >= V / W;
+  const int cls_rows = shard ? V / W : V;
 
-  // tagged hand-off vectors: q | raw k | v | attention output | SwiGLU output h
-  const size_t hand_words = static_cast<size_t>(2 * q_rows + 2 * kvd + hid);
-  if (cudaMalloc(&d_handoff_, sizeof(unsigned long long) * hand_words) != cudaSuccess)
-    return static_cast<int>(cudaErrorMemoryAllocation);
-  cudaMemsetAsync(d_handoff_, 0, sizeof(unsigned long long) * hand_words, stream);
-  unsigned long long *t_q = d_handoff_, *t_k = t_q + q_rows, *t_v = t_k + kvd, *t_attn = t_v + kvd,
-                     *t_h = t_attn + q_rows;
-  {
-    const size_t words = static_cast<size_t>(dm.head_num) * dm.seq_len;
-    if (cudaMalloc(&d_scores_, sizeof(unsigned long long) * words) != cudaSuccess)
-      return static_cast<int>(cudaErrorMemoryAllocation);
-    cudaMemsetAsync(d_scores_, 0, sizeof(unsigned long long) * words, stream);
-  }
+  // process-wide and only ever raised: another decoder's engine launches the same instantiations at its own size
+  for (const void* k : {ks.plain, ks.prof, ks.lp})
+    if (k != nullptr)
+      if (int rc = smem_opt_in(k, smem_bytes)) return rc;
+  int occ_lp = 0;
+  KLLM_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_lp, ks.lp, kThreads, smem_bytes));
+  if (occ_lp < 1) return KLLM_E_UNSUPPORTED;
+  int occ = 0;
+  KLLM_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ks.plain, kThreads, smem_bytes));
+  if (occ < 1) return KLLM_E_UNSUPPORTED;
+
+  // ---- the scratch block: one allocation, each part at a 256-byte aligned offset -------------------------
+  // per layer QKV, the attention (one phase, or the split's two), Wo, W1|W3 and W2; then the classifier
+  const int n_phases = dm.layer_num * ((fast || split == 1) ? 5 : 6) + (shard ? 2 : 1);
+  size_t bytes = 0;
+  auto part = [&bytes](size_t n) {
+    const size_t off = bytes;
+    bytes += (n + 255) & ~static_cast<size_t>(255);
+    return off;
+  };
+  using u64 = unsigned long long;
+  const size_t hand_off = part(sizeof(u64) * (2 * q_rows + 2 * kvd + hid));  // q | raw k | v | attention | h
+  const size_t scores_off = part(sizeof(u64) * dm.head_num * dm.seq_len);    // tagged scores of the split attention
+  const size_t tagged_off = part(W == 1 ? sizeof(u64) * 2 * dim : 0);       // single-GPU exchange area
+  const size_t phases_off = part(sizeof(Phase) * n_phases);
+  const size_t barrier_off = part(128);
+  const size_t arg_val_off = part(sizeof(float) * grid), arg_idx_off = part(sizeof(int) * grid);
+  // lp_part [grid] float2, then lp_cand_v / lp_cand_i [grid][kMaxTopLogprobs]
+  const size_t lp_off = part(static_cast<size_t>(grid) * (sizeof(float2) + 8 * sampling::kMaxTopLogprobs));
+  KLLM_TRY(cudaMalloc(&scratch_, bytes));
+  unsigned char* const s = static_cast<unsigned char*>(scratch_);
+  u64 *t_q = reinterpret_cast<u64*>(s + hand_off), *t_k = t_q + q_rows, *t_v = t_k + kvd, *t_attn = t_v + kvd,
+      *t_h = t_attn + q_rows;
+
+  // ---- phase table ---------------------------------------------------------------------------------
+  std::vector<Phase> ph;
   int hands = 0;
-  if (W == 1) {
-    if (cudaMalloc(&d_tagged_, sizeof(unsigned long long) * 2 * dim) != cudaSuccess)
-      return static_cast<int>(cudaErrorMemoryAllocation);
-    cudaMemsetAsync(d_tagged_, 0, sizeof(unsigned long long) * 2 * dim, stream);
-  }
   int exch = 0;
   // a phase whose input is the residual stream: x_old (shared memory) + partials of the last exchange;
   // before the first exchange (layer 0's QKV) the stream is the embedding row
@@ -2592,9 +2610,8 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
     const LayerWeights& lw = dm.layers[l];
     const size_t layer_off = static_cast<size_t>(l) * dm.seq_len * kvd;
     {  // attention_rms + q | k | v (+bias).  q and the raw k are handed off only; v also goes into the cache.
-      Phase p{};
+      Phase p = qkv;
       p.kind = mega::kPhaseGemv;
-      p.in_dim = dim;
       p.n_seg = 3;
       input_is_x(p);
       p.norm_w = lw.attn_norm;
@@ -2606,13 +2623,12 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
       p.seg[2] = seg(lw.v, vrows, kvd, 1, t_v);
       p.layer = l;  // the fp8 cache's value epilogue reads its layer's scales
       p.units = q_rows + 2 * kvd;
-      if (int rc = plan(p)) return rc;
       p.hand_out = hands;
       ph.push_back(p);
     }
-    if (fast_ || attn_split_ == 1) {  // flash-decoding (attn_split_ CTAs per head by timestep) or fused: one phase
+    if (fast || split == 1) {  // flash-decoding (`split` CTAs per head by timestep) or fused: one phase
       Phase p{};
-      p.kind = fast_ ? mega::kPhaseAttnFlash : mega::kPhaseAttnFused;
+      p.kind = fast ? mega::kPhaseAttnFlash : mega::kPhaseAttnFused;
       p.layer = l;
       p.tq = t_q, p.tk = t_k, p.tv = t_v, p.ta = t_attn;
       p.hand_in = hands++;
@@ -2642,70 +2658,54 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
       }
     }
     {  // wo, added to the residual stream by the readers of the exchange (llama3.cpp:672-684)
-      Phase p{};
+      Phase p = wo;
       p.kind = mega::kPhaseGemv;
-      p.in_dim = q_rows;
       p.n_seg = 1;
       p.tag_in = t_attn;
       p.hand_in = hands++;
       p.seg[0] = seg(lw.o, nullptr, dim);
       p.units = dim;
-      if (int rc = plan(p)) return rc;
       p.tp_out = 1;
       p.exch_out = exch++;
       ph.push_back(p);
     }
     {  // ffn rmsnorm + w1 | w3 -> swiglu (llama3.cpp:686-708)
-      Phase p{};
+      Phase p = ffn;
       p.kind = mega::kPhaseGemv;
-      p.in_dim = dim;
       p.n_seg = 2;
-      p.swiglu = 1;
       input_is_x(p);
       p.norm_w = lw.ffn_norm;
       p.norm_eps = dm.eps;
       p.seg[0] = seg(lw.w1, nullptr, hid, 0, t_h);
       p.seg[1] = seg(lw.w3, nullptr, hid);
       p.units = hid;
-      if (int rc = plan(p)) return rc;
       p.hand_out = hands;
       ph.push_back(p);
     }
     {  // w2, added to the residual stream by the readers of the exchange (llama3.cpp:711-719)
-      Phase p{};
+      Phase p = w2;
       p.kind = mega::kPhaseGemv;
-      p.in_dim = hid;
       p.n_seg = 1;
       p.tag_in = t_h;
       p.hand_in = hands++;
       p.seg[0] = seg(lw.w2, nullptr, dim);
       p.units = dim;
-      if (int rc = plan(p)) return rc;
       p.tp_out = 1;
       p.exch_out = exch++;
       ph.push_back(p);
     }
   }
   {  // final rmsnorm + classifier (+ argmax partials)
-    Phase p{};
+    Phase p = cls;
     p.kind = mega::kPhaseGemv;
-    p.in_dim = dim;
     p.n_seg = 1;
     input_is_x(p);
     p.norm_w = dm.final_norm;
     p.norm_eps = dm.eps;
     p.cls = 1;
-    // Tensor parallel: shard the classifier by vocabulary when the exchange area can carry a rank's
-    // rows (kllm_comm_create(max_count >= vocab / world)); every rank still holds the whole matrix and
-    // reads only its rows.  Otherwise it stays replicated.
-    const int V = dm.vocab_size;
-    const bool shard = W > 1 && V % W == 0 && m.tp_stride >= V / W;
-    cls_rows_ = shard ? V / W : V;
-    n_cls_phases_ = shard ? 2 : 1;
     if (shard) {
-      p.seg[0] = seg(dm.rows_from(dm.cls, static_cast<size_t>(m.tp_rank) * cls_rows_, dim), nullptr, cls_rows_);
-      p.units = cls_rows_;
-      if (int rc = plan(p)) return rc;
+      p.seg[0] = seg(dm.rows_from(dm.cls, static_cast<size_t>(m.tp_rank) * cls_rows, dim), nullptr, cls_rows);
+      p.units = cls_rows;
       p.tp_out = 1;  // rows go to every rank's exchange area as tagged words
       p.exch_out = exch++;
       ph.push_back(p);
@@ -2714,7 +2714,7 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
       g.cls = 1;
       g.argmax = 1;
       g.units = V;
-      g.in_dim = cls_rows_;
+      g.in_dim = cls_rows;
       g.exch = p.exch_out;
       g.seg[0].out = m.logits;
       ph.push_back(g);
@@ -2722,81 +2722,29 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
       p.seg[0] = seg(dm.cls, m.logits, V);
       p.units = V;
       p.argmax = 1;
-      if (int rc = plan(p)) return rc;
       ph.push_back(p);
     }
   }
-  n_phases_ = static_cast<int>(ph.size());
-  exch_per_token_ = exch;
-  hands_per_token_ = hands;
 
-  if (cudaMalloc(&d_phases_, sizeof(Phase) * ph.size()) != cudaSuccess) return static_cast<int>(cudaErrorMemoryAllocation);
-  cudaMemcpyAsync(d_phases_, ph.data(), sizeof(Phase) * ph.size(), cudaMemcpyHostToDevice, stream);
-  if (cudaMalloc(&d_barrier_, 128) != cudaSuccess) return static_cast<int>(cudaErrorMemoryAllocation);
-  cudaMemsetAsync(d_barrier_, 0, 128, stream);
-  if (cudaMalloc(&d_arg_val_, sizeof(float) * grid_) != cudaSuccess ||
-      cudaMalloc(&d_arg_idx_, sizeof(int) * grid_) != cudaSuccess ||
-      cudaMalloc(&d_lp_, static_cast<size_t>(grid_) * (sizeof(float2) + 8 * sampling::kMaxTopLogprobs)) != cudaSuccess)
-    return static_cast<int>(cudaErrorMemoryAllocation);
-  cudaStreamSynchronize(stream);  // ph (host vector) must outlive the async copy
+  // zeroed: the hand-off words, the score words and the exchange area carry tag 0, the barrier word counts from 0
+  KLLM_TRY(cudaMemsetAsync(s, 0, bytes, stream));
+  KLLM_TRY(cudaMemcpyAsync(s + phases_off, ph.data(), sizeof(Phase) * n_phases, cudaMemcpyHostToDevice, stream));
+  KLLM_TRY(cudaStreamSynchronize(stream));  // ph (host vector) must outlive the async copy
 
-  // process-wide and only ever raised: another decoder's engine launches the same instantiations at its own size
-  for (const void* k : {kernel_, kernel_prof_, kernel_lp_})
-    if (k != nullptr)
-      if (int rc = smem_opt_in(k, smem_bytes_)) return rc;
-  int occ_lp = 0;
-  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_lp, kernel_lp_, kThreads, smem_bytes_);
-  if (e != cudaSuccess) return static_cast<int>(e);
-  if (occ_lp < 1) return KLLM_E_UNSUPPORTED;
-  int occ = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel_, kThreads, smem_bytes_);
-  if (e != cudaSuccess) return static_cast<int>(e);
-  if (occ < 1) return KLLM_E_UNSUPPORTED;
-  barrier_base_ = 0;
-  ready_ = true;
-  return 0;
-}
-
-void MegaEngine::destroy() {
-  if (d_phases_) cudaFree(d_phases_);
-  if (d_barrier_) cudaFree(d_barrier_);
-  if (d_arg_val_) cudaFree(d_arg_val_);
-  if (d_arg_idx_) cudaFree(d_arg_idx_);
-  if (d_lp_) cudaFree(d_lp_);
-  d_lp_ = nullptr;
-  if (d_tagged_) cudaFree(d_tagged_);
-  if (d_handoff_) cudaFree(d_handoff_);
-  if (d_scores_) cudaFree(d_scores_);
-  d_scores_ = nullptr;
-  d_handoff_ = nullptr;
-  d_tagged_ = nullptr;
-  d_phases_ = nullptr;
-  d_barrier_ = nullptr;
-  d_arg_val_ = nullptr;
-  d_arg_idx_ = nullptr;
-  ready_ = false;
-}
-
-Params MegaEngine::params(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev,
-                          unsigned long long* prof_dev, int prof_token, int skip_cls_tokens) const {
   Params P{};
-  const DecoderModel& dm = *dm_;
-  const MegaModel& m = model_;
-  P.phases = static_cast<const Phase*>(d_phases_);
-  P.n_phases = n_phases_;
-  P.n_tokens = n_tokens;
-  P.skip_cls_tokens = skip_cls_tokens;
-  P.n_cls_phases = n_cls_phases_;
-  P.int8_fast = int8_fast_;
-  P.num_stages = stages_;
-  P.stage_bytes = stage_bytes_;
-  P.xbuf_bytes = xbuf_bytes_;
-  P.xres_bytes = xres_bytes_;
-  P.attn_tile = attn_tile_;
-  P.attn_tile_v = attn_tile_v_;
-  P.attn_split = attn_split_;
-  P.attn_vsplit = attn_vsplit_;
-  P.scores = d_scores_;
+  P.phases = reinterpret_cast<const Phase*>(s + phases_off);
+  P.n_phases = n_phases;
+  P.n_cls_phases = shard ? 2 : 1;
+  P.int8_fast = (int8 && fast) ? 1 : 0;
+  P.num_stages = stages;
+  P.stage_bytes = stage_bytes;
+  P.xbuf_bytes = xbuf;
+  P.xres_bytes = xres;
+  P.attn_tile = attn_tile;
+  P.attn_tile_v = attn_tile_v;
+  P.attn_split = split;
+  P.attn_vsplit = vsplit;
+  P.scores = reinterpret_cast<u64*>(s + scores_off);
   P.group_size = dm.group_size;
   P.dim = dm.dim;
   P.vocab_size = dm.vocab_size;
@@ -2814,40 +2762,59 @@ Params MegaEngine::params(const DrawSettings& cfg, int n_tokens, const int32_t* 
   P.cos_cache = m.cos_cache;
   P.state = m.state;
   P.out_tokens = m.out_tokens;
-  P.teacher = teacher_dev;
   P.max_steps = dm.seq_len;
-  P.barrier = static_cast<unsigned*>(d_barrier_);
-  P.barrier_base = barrier_base_;
-  P.tp_world = m.tp_world > 1 ? m.tp_world : 1;
-  P.tp_rank = m.tp_world > 1 ? m.tp_rank : 0;
-  P.tp_stride = m.tp_world > 1 ? m.tp_stride : dm.dim;
-  for (int r = 0; r < 8; ++r) P.tp_data[r] = m.tp_world > 1 ? m.tp_data[r] : nullptr;
-  if (m.tp_world <= 1) P.tp_data[0] = d_tagged_;
-  P.exch_per_token = exch_per_token_;
-  P.tp_seq_base = tp_seq_base_;
-  P.hand_base = hand_base_;
-  P.hands_per_token = hands_per_token_;
-  P.arg_val = static_cast<float*>(d_arg_val_);
-  P.arg_idx = static_cast<int*>(d_arg_idx_);
+  P.barrier = reinterpret_cast<unsigned*>(s + barrier_off);
+  P.tp_world = W;
+  P.tp_rank = W > 1 ? m.tp_rank : 0;
+  P.tp_stride = W > 1 ? m.tp_stride : dim;
+  for (int r = 0; r < 8; ++r) P.tp_data[r] = W > 1 ? m.tp_data[r] : nullptr;
+  if (W == 1) P.tp_data[0] = reinterpret_cast<u64*>(s + tagged_off);
+  P.exch_per_token = exch;
+  P.hands_per_token = hands;
+  P.arg_val = reinterpret_cast<float*>(s + arg_val_off);
+  P.arg_idx = reinterpret_cast<int*>(s + arg_idx_off);
   P.sampling = m.sampling;
   P.logits = m.logits;
-  P.penalty = cfg.penalty;
   P.hist = m.hist;
   P.penalized = m.penalized;
-  P.prof = prof_dev;
-  P.prof_token = prof_token;
+  P.prof_token = -1;
   for (int i = 0; i < mega::kMaxStopIds; ++i) P.stop_ids[i] = -1;  // ids are >= 0: no stop
-  P.lp_top_n = cfg.lp_top_n;
-  P.lp_target = 0;
-  P.lp_part = static_cast<float2*>(d_lp_);
-  P.lp_cand_v = reinterpret_cast<float*>(P.lp_part + grid_);
-  P.lp_cand_i = reinterpret_cast<int*>(P.lp_cand_v + static_cast<size_t>(grid_) * sampling::kMaxTopLogprobs);
+  P.lp_part = reinterpret_cast<float2*>(s + lp_off);
+  P.lp_cand_v = reinterpret_cast<float*>(P.lp_part + grid);
+  P.lp_cand_i = reinterpret_cast<int*>(P.lp_cand_v + static_cast<size_t>(grid) * sampling::kMaxTopLogprobs);
   P.lp_rec = m.lp_rec;
-  if (kv_elem_ == KLLM_KV_FP8) {
+  if (kv == KLLM_KV_FP8) {
     const size_t n = static_cast<size_t>(dm.layer_num) * dm.kv_head_num;
     P.kv_scale_k = m.kv_scales, P.kv_scale_v = m.kv_scales + n;
     P.kv_inv_k = m.kv_scales + 2 * n, P.kv_inv_v = m.kv_scales + 3 * n;
   }
+  base_ = P;
+  stream_ = stream;
+  grid_ = grid;
+  fast_ = fast;
+  cls_rows_ = cls_rows;
+  kernel_ = ks.plain, kernel_prof_ = ks.prof, kernel_lp_ = ks.lp;
+  smem_bytes_ = smem_bytes;
+  ready_ = true;
+  return 0;
+}
+
+int MegaEngine::destroy() {
+  const cudaError_t e = cudaFree(scratch_);  // a null pointer frees nothing
+  scratch_ = nullptr;
+  ready_ = false;
+  return static_cast<int>(e);
+}
+
+// base_ with the settings of this launch and the tag and barrier bases the tokens before it left
+Params MegaEngine::params(const DrawSettings& cfg, int n_tokens) const {
+  Params P = base_;
+  P.n_tokens = n_tokens;
+  P.penalty = cfg.penalty;
+  P.lp_top_n = cfg.lp_top_n;
+  P.barrier_base = barrier_base_;
+  P.tp_seq_base = tp_seq_base_;
+  P.hand_base = hand_base_;
   return P;
 }
 
@@ -2856,24 +2823,26 @@ int MegaEngine::launch(const Params& P) {
   // the profiling instantiation records no log-probabilities; the LP one runs while they are on
   const void* k = P.prof != nullptr ? kernel_prof_ : P.lp_top_n >= 0 ? kernel_lp_ : kernel_;
   if (k == nullptr) return KLLM_E_UNSUPPORTED;
-  cudaError_t e = cudaLaunchCooperativeKernel(const_cast<void*>(k), dim3(grid_),
-                                              dim3(kThreads), args, smem_bytes_, stream_);
-  if (e != cudaSuccess) return static_cast<int>(e);
+  KLLM_TRY(cudaLaunchCooperativeKernel(const_cast<void*>(k), dim3(grid_), dim3(kThreads), args, smem_bytes_, stream_));
   count_launch();
   return 0;
 }
 
 // The tags and barrier counts the next launch waits for continue from where the tokens that ran left them.
 void MegaEngine::account(int n_tokens) {
-  tp_seq_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(exch_per_token_);
-  hand_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(hands_per_token_);
+  tp_seq_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(base_.exch_per_token);
+  hand_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(base_.hands_per_token);
   barrier_base_ += static_cast<unsigned>(n_tokens) * static_cast<unsigned>(grid_);  // one grid barrier per token
 }
 
 int MegaEngine::run(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
                     int prof_token, int skip_cls_tokens, int lp_target) {
   if (!ready_) return KLLM_E_STATE;
-  Params P = params(cfg, n_tokens, teacher_dev, prof_dev, prof_token, skip_cls_tokens);
+  Params P = params(cfg, n_tokens);
+  P.teacher = teacher_dev;
+  P.prof = prof_dev;
+  P.prof_token = prof_token;
+  P.skip_cls_tokens = skip_cls_tokens;
   P.lp_target = lp_target;
   if (int rc = launch(P)) return rc;
   account(n_tokens);
@@ -2884,7 +2853,7 @@ int MegaEngine::run_until(const DrawSettings& cfg, int n_tokens, const int32_t* 
                           int32_t* stream_ids, int32_t* stream_count) {
   if (!ready_) return KLLM_E_STATE;
   if (n_stop < 0 || n_stop > mega::kMaxStopIds) return KLLM_E_INVALID;
-  Params P = params(cfg, n_tokens, nullptr, nullptr, -1, 0);
+  Params P = params(cfg, n_tokens);
   for (int i = 0; i < n_stop; ++i) P.stop_ids[i] = stop_ids[i];
   P.stream_ids = stream_ids;
   P.stream_count = stream_count;

@@ -195,9 +195,10 @@ struct MegaModel {
 
 class MegaEngine {
  public:
-  // `dm` is read again by every launch: it outlives the engine
+  // Every refusal (KLLM_E_INVALID, KLLM_E_UNSUPPORTED, KLLM_E_NODEVICE) comes before the one allocation: an engine
+  // that refuses holds nothing.  `dm` and `m` are read here only.
   int init(const DecoderModel& dm, const MegaModel& m, cudaStream_t stream);
-  void destroy();
+  int destroy();  // the status of freeing the scratch block
   // Run n_tokens consecutive positions starting from the device-resident state, under the decoder's settings
   // `cfg` (its step 0 and logprob setting ride in the launch parameters; the sampling parameters are read through
   // MegaModel::sampling).  lp_target: kllm_decoder_score's run, whose record entries hold teacher[step + 1]
@@ -212,45 +213,31 @@ class MegaEngine {
                 int32_t* stream_count);
   void account(int n_tokens);
   int grid() const { return grid_; }
-  int phases() const { return n_phases_; }
-  int attn_vsplit() const { return attn_vsplit_; }  // slices of the V cache layout
-  int fast() const { return fast_; }                // numerics: 1 = toleranced (free summation order)
-  int attn_tile() const { return attn_tile_; }      // timesteps per K (flash: K and V) ring stage
-  int attn_split() const { return attn_split_; }    // CTAs per query head
-  int attn_tile_v() const { return attn_tile_v_; }  // timesteps per V ring stage
-  int stage_bytes() const { return stage_bytes_; }
+  int phases() const { return base_.n_phases; }
+  int attn_vsplit() const { return base_.attn_vsplit; }  // slices of the V cache layout
+  int fast() const { return fast_; }                     // numerics: 1 = toleranced (free summation order)
+  int attn_tile() const { return base_.attn_tile; }      // timesteps per K (flash: K and V) ring stage
+  int attn_split() const { return base_.attn_split; }    // CTAs per query head
+  int attn_tile_v() const { return base_.attn_tile_v; }  // timesteps per V ring stage
+  int stage_bytes() const { return base_.stage_bytes; }
   int cls_rows() const { return cls_rows_; }  // classifier rows this rank streams per token
 
  private:
-  mega::Params params(const DrawSettings& cfg, int n_tokens, const int32_t* teacher_dev, unsigned long long* prof_dev,
-                      int prof_token, int skip_cls_tokens) const;
+  mega::Params params(const DrawSettings& cfg, int n_tokens) const;
   int launch(const mega::Params& P);
-  const DecoderModel* dm_ = nullptr;
-  MegaModel model_{};
-  void* d_lp_ = nullptr;  // lp_part [grid] float2, then lp_cand_v / lp_cand_i [grid][kMaxTopLogprobs]
+  mega::Params base_{};  // every launch parameter that stays the same from launch to launch
+  // hand-off words, score words, exchange area (one GPU), phase table, barrier word, argmax and logprob partials
+  void* scratch_ = nullptr;
   cudaStream_t stream_ = nullptr;
-  void* d_phases_ = nullptr;
-  void* d_barrier_ = nullptr;
-  void* d_arg_val_ = nullptr;
-  void* d_arg_idx_ = nullptr;
-  unsigned long long* d_tagged_ = nullptr;  // single-GPU exchange area (tp_world == 1)
-  unsigned long long* d_handoff_ = nullptr;  // local tagged hand-off vectors (q | k | v | attn | h)
-  int exch_per_token_ = 0, hands_per_token_ = 0;
-  unsigned tp_seq_base_ = 0, hand_base_ = 0;
-  int grid_ = 0, stages_ = 0, stage_bytes_ = 0, xbuf_bytes_ = 0, xres_bytes_ = 0, n_phases_ = 0, attn_tile_ = 0;
-  int attn_split_ = 1, attn_tile_v_ = 0;
-  unsigned long long* d_scores_ = nullptr;  // tagged scores of the split attention
-  int int8_fast_ = 0;
+  unsigned barrier_base_ = 0, tp_seq_base_ = 0, hand_base_ = 0;
+  int grid_ = 0;
   int fast_ = 0;  // numerics: 0 = bit-exact with the reference, 1 = toleranced (free summation order)
-  int attn_vsplit_ = 1;
-  int kv_elem_ = KLLM_KV_F32;  // the KV cache's element, a kllm_decoder_desc::kv_cache value
-  int cls_rows_ = 0, n_cls_phases_ = 1;
+  int cls_rows_ = 0;
   // the instantiations of the weight format and KV cache (megakernel.cu, kernels_for)
   const void* kernel_ = nullptr;       // plain
   const void* kernel_prof_ = nullptr;  // records the phase timeline stamps; none with a bf16 or fp8 cache or bf16 weights
   const void* kernel_lp_ = nullptr;    // log-probabilities on
   size_t smem_bytes_ = 0;
-  unsigned barrier_base_ = 0;
   bool ready_ = false;
 };
 
