@@ -1198,11 +1198,12 @@ __device__ KLLM_PHASE_CALL Pipe attention_pv_phase(const Params& P, int head, in
   const int dv = hs / P.attn_split;
   const int kvh = head / P.kv_mul;
   // scores / probabilities: shared memory when the context fits the workspace (the ring leaves
-  // almost no L1), else the global [head][seq_len] buffer the reference uses (the SP CTAs of a head
-  // then write identical values to it)
+  // almost no L1), else this CTA's own global row: the softmax rewrites its row in place, so a row shared by the
+  // SP CTAs of a head would let one CTA read the other's exponentials as scores
   const int smem_cap = P.xbuf_bytes >> 2;
   const bool score_in_smem = pos + 1 <= smem_cap;
-  float* score_head = score_in_smem ? ws : (P.score + static_cast<size_t>(head) * seq_len);
+  float* score_head =
+      score_in_smem ? ws : (P.probs + (static_cast<size_t>(head) * P.attn_split + split) * seq_len);
 
   // this CTA's dv dims of the value row of the current position (written by the QKV phase of this token)
   float v_pos = 0.f;
@@ -2579,6 +2580,8 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
   using u64 = unsigned long long;
   const size_t hand_off = part(sizeof(u64) * (2 * q_rows + 2 * kvd + hid));  // q | raw k | v | attention | h
   const size_t scores_off = part(sizeof(u64) * dm.head_num * dm.seq_len);    // tagged scores of the split attention
+  // the split P.V phase's probabilities past shared memory, one row per CTA
+  const size_t probs_off = part(fast || split == 1 ? 0 : sizeof(float) * dm.head_num * split * dm.seq_len);
   const size_t tagged_off = part(W == 1 ? sizeof(u64) * 2 * dim : 0);       // single-GPU exchange area
   const size_t phases_off = part(sizeof(Phase) * n_phases);
   const size_t barrier_off = part(128);
@@ -2756,6 +2759,7 @@ int MegaEngine::init(const DecoderModel& dm, const MegaModel& m, cudaStream_t st
   P.flavour = dm.flavour;
   P.tok_emb = dm.tok_emb;
   P.score = m.score;
+  P.probs = reinterpret_cast<float*>(s + probs_off);
   P.key_cache = m.key_cache;
   P.value_cache = m.value_cache;
   P.sin_cache = m.sin_cache;

@@ -112,6 +112,9 @@ struct Params {
   int dim, vocab_size, head_num, head_size, kv_dim, kv_mul, seq_len, flavour;
   const float* tok_emb;
   float* score;
+  // [head][attn_split][seq_len]: the split P.V phase's probabilities when they do not fit shared memory, one row
+  // per CTA (each CTA's softmax runs in place, so the SP CTAs of a head cannot share a row)
+  float* probs;
   // KV cache in the persistent engine's own layout (see megakernel.cu "KV layout"):
   //   K [L][kv_head][head_size/4][seq_len][4]    V [L][kv_head][attn_split][seq_len][head_size/attn_split]
   // KLLM_KV_BF16 (flash form only): both caches hold bf16 elements behind these pointers,

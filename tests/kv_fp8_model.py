@@ -92,3 +92,16 @@ def fp8_round_rows(rows, scales, which):
             inv = float(np.float32(1.0) / np.float32(s))
             out[l].view(n, kvh, -1)[:, h] = read_value(e4m3_rne(scaled(r[:, h], inv)), s)
     return out
+
+
+def ulp_e4m3(v):
+    """One e4m3 ulp at |v|: 2^(e - 3) for |v| in [2^e, 2^(e + 1)), 2^-9 below 2^-6.  The bounds take it at the larger
+    of the two values compared: two elements on either side of a power of two are a step of the upper binade apart."""
+    e = torch.floor(torch.log2(v.abs().clamp_min(2.0 ** -6)))
+    return torch.pow(2.0, e - 3)
+
+
+def per_head(scales, which, L, kvh, hs, device):
+    """The [L, 1, kv_dim] broadcast of scales[which] [L, kv_heads]."""
+    s = torch.as_tensor(np.asarray(scales[which], np.float32), device=device).double()
+    return s.repeat_interleave(hs, dim=1).reshape(L, 1, kvh * hs)

@@ -159,6 +159,51 @@ def _attention(q, k_all, v_all, start_pos, kv_mul, max_bytes=1 << 28):
     return f32(out)
 
 
+def layer_ops(weights, shape, dev, tf32, fixed_point):
+    """(proj, bias), the projections of one layer as prefill_ref computes them: proj(x, name, l) is
+    fp32(operand(x) . W^T) with the layer's matrix widened (int8: dequantised) when it is used, operand(x) x rounded to
+    TF32 (tf32) or the fast mode's fixed point (fixed_point, int8 group size 64); bias(y, name, l) adds the Qwen bias
+    where the weights have one."""
+    g = shape.group_size
+
+    def weight(name, l):
+        w = weights[name][l]
+        if g:
+            return dequant_w8(_t(w, dev), _t(weights["s" + name[1:]][l], dev), g, tf32)
+        return gemm_operand(_t(w, dev), tf32)
+
+    def operand(x):
+        if fixed_point and g == 64 and x.shape[-1] % 64 == 0:
+            return fixed_point_value(x)
+        return gemm_operand(x.to(torch.float32), tf32).to(torch.float64)
+
+    def proj(x, name, l):
+        return f32(operand(x) @ weight(name, l).to(torch.float64).t())
+
+    def bias(y, name, l):
+        b = weights.get(name)
+        return y if b is None else f32(y + _t(b[l], dev).to(torch.float64))
+
+    return proj, bias
+
+
+def classify(weights, shape, x, dev, fixed_point):
+    """The final RMSNorm and the classifier of the rows x [n, dim]: fp64 logits [n, vocab] of the fp32 classifier (no
+    TF32: it is the decode path's GEMV), its input in the fast mode's fixed point with fixed_point."""
+    g = shape.group_size
+    xl = _rmsnorm(x, _t(weights["final_norm"], dev), flavour_eps(shape.flavour))
+    wcls = weights.get("wcls")
+    if wcls is None:
+        wcls = weights["tok_emb"]
+    if g:
+        wc = dequant_w8(_t(wcls, dev), _t(weights["scls"], dev), g, tf32=False)
+    else:
+        wc = _t(wcls, dev)
+    if fixed_point and g == 64 and shape.dim % 64 == 0:
+        xl = fixed_point_value(xl)
+    return xl @ wc.to(torch.float64).t()
+
+
 def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=True, device=None, logits_at=(),
                 fixed_point=False):
     """The forward of prefill_block over `tokens` at positions start_pos .. start_pos + n - 1, then the last
@@ -180,29 +225,12 @@ def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=Tr
     L, hs, heads, kvh = s.layer_num, s.head_size, s.head_num, s.kv_head_num
     n = len(tokens)
     eps = flavour_eps(s.flavour)
-    g = s.group_size
     assert not (fixed_point and tf32), "the fixed point is the decode step's; the prefill's GEMMs are TF32"
     sin, cos = _t(sin, dev), _t(cos, dev)
     pos = torch.arange(start_pos, start_pos + n, device=dev)
     tok = torch.as_tensor(np.asarray(tokens, dtype=np.int64), device=dev)
 
-    def weight(name, l):
-        w = weights[name][l]
-        if g:
-            return dequant_w8(_t(w, dev), _t(weights["s" + name[1:]][l], dev), g, tf32)
-        return gemm_operand(_t(w, dev), tf32)
-
-    def operand(x):
-        if fixed_point and g == 64 and x.shape[-1] % 64 == 0:
-            return fixed_point_value(x)
-        return gemm_operand(x.to(torch.float32), tf32).to(torch.float64)
-
-    def proj(x, name, l):
-        return f32(operand(x) @ weight(name, l).to(torch.float64).t())
-
-    def bias(y, name, l):
-        b = weights.get(name)
-        return y if b is None else f32(y + _t(b[l], dev).to(torch.float64))
+    proj, bias = layer_ops(weights, s, dev, tf32, fixed_point)
 
     x = _t(weights["tok_emb"], dev)[tok].to(torch.float64)
     ks, vs = [], []
@@ -226,17 +254,7 @@ def prefill_ref(weights, shape, tokens, start_pos, sin, cos, kv_in=None, tf32=Tr
         h = f32(h1 * torch.sigmoid(h1) * h3)
         x = f32(x + proj(h, "w2", l))
     rows = sorted({i % n for i in logits_at} | {n - 1})
-    xl = _rmsnorm(x[rows], _t(weights["final_norm"], dev), eps)
-    wcls = weights.get("wcls")
-    if wcls is None:
-        wcls = weights["tok_emb"]
-    if g:
-        wc = dequant_w8(_t(wcls, dev), _t(weights["scls"], dev), g, tf32=False)
-    else:
-        wc = _t(wcls, dev)
-    if fixed_point and g == 64 and s.dim % 64 == 0:
-        xl = fixed_point_value(xl)
-    logits = dict(zip(rows, xl @ wc.to(torch.float64).t()))
+    logits = dict(zip(rows, classify(weights, s, x[rows], dev, fixed_point)))
     last = logits[n - 1]
     return {"k": torch.stack(ks), "v": torch.stack(vs), "logits": last, "next": int(torch.argmax(last)),
             "logits_at": logits}

@@ -36,7 +36,7 @@ import torch
 
 from decode_model_util import (GEOMETRIES, KNOBS, LOGIT_TAU, WEIGHTS, case_id, continue_ends, device_sincos,
                                engine_geometry, sequence, sms, taus)
-from kv_fp8_model import e4m3_rne, fp8_round_rows, prefill_ref_fp8
+from kv_fp8_model import e4m3_rne, fp8_round_rows, per_head, prefill_ref_fp8, ulp_e4m3
 from prefill_model import prefill_ref
 
 from kuiperllama_b200 import ALLREDUCE_FN, SHAPES, Decoder, KllmError, ModelShape, synth_weights
@@ -104,19 +104,6 @@ def case_weights(shape, weights, weight_format):
 def ends_for(T, SP, seq_len):
     e = {0, 1, 7, 8, 9, T - 1, T, T + 1, SP * T - 1, SP * T, SP * T + 1, seq_len - 1}
     return sorted(p for p in e if 0 <= p < seq_len)
-
-
-def ulp_e4m3(v):
-    """One e4m3 ulp at |v|: 2^(e - 3) for |v| in [2^e, 2^(e + 1)), 2^-9 below 2^-6.  The bounds take it at the larger
-    of the two values compared: two elements on either side of a power of two are a step of the upper binade apart."""
-    e = torch.floor(torch.log2(v.abs().clamp_min(2.0 ** -6)))
-    return torch.pow(2.0, e - 3)
-
-
-def per_head(scales, which, L, kvh, hs, device):
-    """The [L, 1, kv_dim] broadcast of scales[which] [L, kv_heads]."""
-    s = torch.as_tensor(np.asarray(scales[which], np.float32), device=device).double()
-    return s.repeat_interleave(hs, dim=1).reshape(L, 1, kvh * hs)
 
 
 @pytest.mark.parametrize("key,weights,env,calibrated,weight_format", FP8_CASES, ids=[fp8_id(c) for c in FP8_CASES])
