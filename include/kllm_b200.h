@@ -533,6 +533,46 @@ int kllm_batch_generate_until(kllm_batch* batch, const int32_t* first_tokens_hos
                               kllm_batch_token_callback on_tokens, void* ctx, int32_t* out_tokens_host,
                               int32_t* n_out_host, kllm_batch_stats* stats);
 
+/* Beam search of one prompt with B = the batch's member count beams (DESIGN.md 5.16): transformers'
+ * generate(num_beams=B, do_sample=False, length_penalty, early_stopping, num_return_sequences=n_return) with no
+ * logits processors, every running beam a row of one pass over the weights.  kuiperllama_b200/beam.py states the
+ * rule; early_stopping is one of the KLLM_BEAM_EARLY_* codes.
+ *  - The caller has filled member 0's cache for positions [0, start_pos) with any entry; first_token is fed at
+ *    start_pos.  The call copies member 0's rows [0, start_pos] into the other members; their earlier contents at
+ *    positions below start_pos + max_new_tokens are overwritten.
+ *  - The results are bit for bit those of beam.py run over each member's own logits, with lp by rule L1-L3 over the
+ *    one-block partition (kllm_logprobs_f32's).  Hypothesis i (h descending) has out_len_host[i] ids in row i of
+ *    out_ids_host [n_return][max_new_tokens] (an eos id that ended it included; the rest of the row is not written),
+ *    its score h = fp32(S / fp32(t ^ length_penalty)) at out_score_host[i] and its sum of log-probabilities S at
+ *    out_sum_host[i].  stats (optional) receives the passes, the cache forks and fork_rows = the positions they
+ *    copied, summed over the forks.
+ *  - Afterwards member 0's rows below start_pos are unchanged; everything else the members hold at or past
+ *    start_pos (K/V rows, position, history, record and logits) is unspecified.  kllm_batch_step,
+ *    kllm_batch_generate and kllm_batch_generate_until behave as before.
+ * Before any launch, leaving every member unchanged: KLLM_E_INVALID for NULL outputs, a first token or eos id outside
+ * [0, vocab), start_pos < 0, max_new_tokens <= 0, start_pos + max_new_tokens > seq_len, n_eos outside
+ * [0, KLLM_MAX_BEAM_EOS] (or n_eos > 0 with NULL ids), n_return outside [1, B], a length_penalty that is not finite
+ * and early_stopping outside {0, 1, 2}; KLLM_E_UNSUPPORTED for a member whose draw settings are not a new
+ * decoder's (greedy, no repetition, frequency or presence penalty, no logit bias; the logprob setting does not
+ * matter) and for vocab < max(2, 1 + n_eos) * B.
+ * Each pass runs the batch's embedding and layer chain over the running beams, then one block per row takes the
+ * row's top B + KLLM_MAX_BEAM_EOS ids and their lp into mapped host memory; the host applies the rule, and a beam
+ * that shares its parent with an earlier one takes a dropped beam's member, whose rows one kernel per pass copies
+ * from the parent's.  The passes of 1 and of B rows are captured as CUDA graphs on first use and kept. */
+#define KLLM_MAX_BEAM_EOS 8
+#define KLLM_BEAM_EARLY_HEURISTIC 0 /* transformers early_stopping=False */
+#define KLLM_BEAM_EARLY_ALL_DONE 1  /* early_stopping=True */
+#define KLLM_BEAM_EARLY_NEVER 2     /* early_stopping="never" */
+typedef struct {
+  int32_t passes;
+  int32_t forks;
+  int64_t fork_rows;
+} kllm_beam_stats;
+int kllm_batch_beam_search(kllm_batch* batch, int32_t first_token, int32_t start_pos, int32_t max_new_tokens,
+                           const int32_t* eos_ids, int32_t n_eos, float length_penalty, int32_t early_stopping,
+                           int32_t n_return, int32_t* out_ids_host, int32_t* out_len_host, float* out_score_host,
+                           float* out_sum_host, kllm_beam_stats* stats);
+
 /* Copies into dst what src holds for positions [0, n_pos): the K/V rows (cache elements as stored: fp32, bf16, or
  * fp8 codes at equal scales, in any layout), the history and the log-probability record entries.  Afterwards any
  * entry on dst that continues at a position <= n_pos returns what it would on src, bit for bit; dst keeps its own

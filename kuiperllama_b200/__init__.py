@@ -48,6 +48,7 @@ MAX_STOP_IDS = 16  # KLLM_MAX_STOP_IDS
 MAX_TOP_LOGPROBS = 20  # KLLM_MAX_TOP_LOGPROBS
 MAX_VERIFY_TOKENS = 8  # KLLM_MAX_VERIFY_TOKENS: the positions one kllm_decoder_verify pass takes
 MAX_BATCH = 8  # KLLM_MAX_BATCH: the members of one kllm_batch
+MAX_BEAM_EOS = 8  # KLLM_MAX_BEAM_EOS: the eos ids of one kllm_batch_beam_search
 
 
 class SpecStats(ctypes.Structure):
@@ -58,6 +59,11 @@ class SpecStats(ctypes.Structure):
 class BatchStats(ctypes.Structure):
     """kllm_batch_stats: the passes of kllm_batch_generate_until and the rows they carried."""
     _fields_ = [("passes", c_int32), ("rows", c_int32)]
+
+
+class BeamStats(ctypes.Structure):
+    """kllm_beam_stats: the passes of kllm_batch_beam_search, its cache forks and the positions they copied."""
+    _fields_ = [("passes", c_int32), ("forks", c_int32), ("fork_rows", c_int64)]
 
 
 class DecoderDesc(ctypes.Structure):
@@ -143,6 +149,9 @@ _SIGNATURES = {
     "kllm_batch_generate_until": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
                                           POINTER(c_int32), POINTER(c_int32), BATCH_TOKEN_CALLBACK, c_void_p,
                                           POINTER(c_int32), POINTER(c_int32), POINTER(BatchStats)]),
+    "kllm_batch_beam_search": (c_int, [c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32), c_int32, c_float,
+                                       c_int32, c_int32, POINTER(c_int32), POINTER(c_int32), POINTER(c_float),
+                                       POINTER(c_float), POINTER(BeamStats)]),
     "kllm_decoder_copy_prefix": (c_int, [c_void_p, c_void_p, c_int32]),
     "kllm_decoder_set_sampling": (c_int, [c_void_p, c_float, c_int32, c_uint64]),
     "kllm_decoder_set_sampling_top_p": (c_int, [c_void_p, c_float, c_int32, c_float, c_uint64]),

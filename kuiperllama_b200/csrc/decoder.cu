@@ -121,18 +121,68 @@ batch_draw_kernel(const float* __restrict__ logits_rows, int n, const BatchTarge
   for (int e = threadIdx.x; e < n; e += blockDim.x) mb.logits[e] = row[e];
 }
 
-// One prefix of a cache: positions [0, gridDim.x) of every layer (blockIdx.y), element by element through the
-// layout's own index, so any layout and element (T of its size: fp32, bf16 or fp8 codes) is copied as stored
+// The K and V rows of position pos in one layer of a cache, element by element through the layout's own index, so
+// any layout and element (T of its size: fp32, bf16 or fp8 codes) is copied as stored.  The block's threads share it.
 template <typename T>
-__global__ void copy_prefix_kernel(const T* __restrict__ ks, const T* __restrict__ vs, T* __restrict__ kd,
-                                   T* __restrict__ vd, prefill::CacheLayout c) {
-  const int pos = blockIdx.x;
-  const size_t layer = static_cast<size_t>(blockIdx.y) * c.seq_len * c.kv_dim;
+__device__ __forceinline__ void copy_kv_position(const T* __restrict__ ks, const T* __restrict__ vs, T* __restrict__ kd,
+                                                 T* __restrict__ vd, const prefill::CacheLayout& c, int pos,
+                                                 int layer_index) {
+  const size_t layer = static_cast<size_t>(layer_index) * c.seq_len * c.kv_dim;
   for (int p = threadIdx.x; p < c.kv_dim; p += blockDim.x) {
     const int kvh = p / c.head_size, i = p % c.head_size;
     const size_t ki = layer + prefill::k_index(c, pos, kvh, i), vi = layer + prefill::v_index(c, pos, kvh, i);
     kd[ki] = ks[ki];
     vd[vi] = vs[vi];
+  }
+}
+
+// One prefix of a cache: positions [0, gridDim.x) of every layer (blockIdx.y)
+template <typename T>
+__global__ void copy_prefix_kernel(const T* __restrict__ ks, const T* __restrict__ vs, T* __restrict__ kd,
+                                   T* __restrict__ vd, prefill::CacheLayout c) {
+  copy_kv_position(ks, vs, kd, vd, c, blockIdx.x, blockIdx.y);
+}
+
+// The (source, destination) caches of a beam-search pass's forks (kllm_batch_beam_search): fork f copies member
+// src's rows into member dst's.  A batch's caches are fp32.
+struct ForkTable {
+  const float* ks[KLLM_MAX_BATCH];
+  const float* vs[KLLM_MAX_BATCH];
+  float* kd[KLLM_MAX_BATCH];
+  float* vd[KLLM_MAX_BATCH];
+};
+
+// Every fork of a pass in one launch: grid (positions [lo, lo + gridDim.x), layers, forks).  Sources are surviving
+// beams' members and destinations dropped ones', so no block reads what another writes.
+__global__ void fork_rows_kernel(const __grid_constant__ ForkTable t, int lo, prefill::CacheLayout c) {
+  const int f = blockIdx.z;
+  copy_kv_position(t.ks[f], t.vs[f], t.kd[f], t.vd[f], c, lo + static_cast<int>(blockIdx.x), blockIdx.y);
+}
+
+// The ids a beam-search pass reads back per row: the top kBeamTop of the logprob rule and their lp, in the rule's
+// order (logit descending, lowest id on ties).  B + KLLM_MAX_BEAM_EOS serves every eos count with one captured pass:
+// a top-N selection is exact, so its first B + n_eos entries are those of top_n = B + n_eos.
+constexpr int kBeamTop = KLLM_MAX_BATCH + KLLM_MAX_BEAM_EOS;
+static_assert(kBeamTop <= sampling::kMaxTopLogprobs, "the logprob rule's top-N holds a pass's candidates");
+struct BeamCandidates {
+  int32_t ids[KLLM_MAX_BATCH][kBeamTop];
+  float lp[KLLM_MAX_BATCH][kBeamTop];
+};
+
+// Block r: rule L1-L3 over row r of the batch's logits (one block, kllm_logprobs_f32's partition), its top top_n ids
+// and their lp into row r of `out` (mapped host memory)
+__global__ void __launch_bounds__(1024)
+beam_candidates_kernel(const float* __restrict__ logits_rows, int n, int top_n, BeamCandidates* out) {
+  constexpr int kScratch = sampling::logprob_scratch_bytes(1024);
+  __shared__ __align__(16) unsigned char scratch[kScratch];
+  const int r = blockIdx.x;
+  sampling::logprobs_block<1024>(logits_rows + static_cast<size_t>(r) * n, n, top_n, scratch, kScratch,
+                                 [] { __syncthreads(); });
+  const sampling::LogprobScratch& ls = *reinterpret_cast<const sampling::LogprobScratch*>(scratch);
+  if (static_cast<int>(threadIdx.x) < top_n) {
+    const int i = ls.top_i[threadIdx.x];
+    out->ids[r][threadIdx.x] = i;
+    out->lp[r][threadIdx.x] = i < 0 ? -INFINITY : sampling::logprob(ls.top_v[threadIdx.x], ls.m, ls.lse_off);
   }
 }
 
@@ -274,6 +324,12 @@ struct kllm_batch {
   // others on first use by kllm_batch_generate_until.
   cudaGraphExec_t exec[KLLM_MAX_BATCH] = {};
   int launches[KLLM_MAX_BATCH] = {};
+  // kllm_batch_beam_search: beam_exec[0] the pass of one row, beam_exec[1] of n rows (embedding, chain,
+  // candidates), captured on first use; the candidates reach the host through mapped memory
+  cudaGraphExec_t beam_exec[2] = {};
+  int beam_launches[2] = {};
+  BeamCandidates* cand_host = nullptr;
+  BeamCandidates* cand_dev = nullptr;
 };
 
 namespace {
@@ -536,15 +592,21 @@ bool same_model(const kllm_decoder* a, const kllm_decoder* b) {
          ca.head_size == cb.head_size && ca.split == cb.split && ca.elem == cb.elem;
 }
 
-// Embedding, chain and draw of one step of rows [0, k): the graph engine's step (enqueue_step) at k rows
-int enqueue_batch(const kllm_batch* b, int k, cudaStream_t s) {
+// Embedding and chain of rows [0, k): each row's logits in the batch's rows
+int enqueue_batch_chain(const kllm_batch* b, int k, cudaStream_t s) {
   const kllm_decoder* d0 = b->members[0];
   const DecoderModel& m = d0->m;
   batch_embed_kernel<<<dim3(4, k), 256, 0, s>>>(b->targets, m.tok_emb, b->rows.x, m.dim, m.vocab_size);
   count_launch();
   KLLM_TRY(cudaGetLastError());
   // the RoPE tables are member 0's: every member's hold the same values (kllm_sincos_init of the same shape)
-  KLLM_TRY(enqueue_layers(m, decoder_cache(d0), b->rows, k, ChainPos{PosArg{nullptr, 0}, b->chain}, nullptr, s));
+  return enqueue_layers(m, decoder_cache(d0), b->rows, k, ChainPos{PosArg{nullptr, 0}, b->chain}, nullptr, s);
+}
+
+// Embedding, chain and draw of one step of rows [0, k): the graph engine's step (enqueue_step) at k rows
+int enqueue_batch(const kllm_batch* b, int k, cudaStream_t s) {
+  const DecoderModel& m = b->members[0]->m;
+  KLLM_TRY(enqueue_batch_chain(b, k, s));
   batch_draw_kernel<<<k, 1024, 0, s>>>(b->rows.logits, m.vocab_size, b->targets, m.seq_len);
   count_launch();
   return static_cast<int>(cudaGetLastError());
@@ -594,7 +656,11 @@ int batch_prepare(kllm_batch* b) {
   if (cudaMalloc(&b->tables, table_bytes(b)) != cudaSuccess) b->tables = nullptr;
   if (cudaMallocHost(&b->tables_host, table_bytes(b)) != cudaSuccess) b->tables_host = nullptr;
   if (cudaMallocHost(&b->io_host, sizeof(int32_t) * n * m.seq_len) != cudaSuccess) b->io_host = nullptr;
-  if (!b->buf || !b->tables || !b->tables_host || !b->io_host) return static_cast<int>(cudaErrorMemoryAllocation);
+  if (cudaHostAlloc(&b->cand_host, sizeof(BeamCandidates), cudaHostAllocMapped) != cudaSuccess ||
+      cudaHostGetDevicePointer(&b->cand_dev, b->cand_host, 0) != cudaSuccess)
+    b->cand_dev = nullptr;
+  if (!b->buf || !b->tables || !b->tables_host || !b->io_host || !b->cand_dev)
+    return static_cast<int>(cudaErrorMemoryAllocation);
   float* f = static_cast<float*>(b->buf);
   b->rows = chain_rows(m, n, f);
   b->chain = static_cast<ChainMember*>(b->tables);
@@ -682,6 +748,164 @@ int run_batch_until(kllm_batch* b, const int32_t* tokens, const int32_t* pos, co
   for (int i = 0; i < n; ++i)
     std::memcpy(out + static_cast<size_t>(i) * M, b->members[i]->stream_host + kStreamIds, sizeof(int32_t) * n_out[i]);
   if (stats != nullptr) *stats = kllm_batch_stats{passes, rows};
+  return 0;
+}
+
+// A beam-search pass of rows [0, k): embedding, chain, and each row's candidates
+int enqueue_beam_pass(const kllm_batch* b, int k, cudaStream_t s) {
+  const DecoderModel& m = b->members[0]->m;
+  KLLM_TRY(enqueue_batch_chain(b, k, s));
+  const int top_n = static_cast<int>(b->members.size()) + KLLM_MAX_BEAM_EOS;
+  beam_candidates_kernel<<<k, 1024, 0, s>>>(b->rows.logits, m.vocab_size, top_n, b->cand_dev);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+// Queues the copy of rows [lo, hi) from member src[f] to member dst[f] for every f < n, in one launch
+int fork_rows(kllm_batch* b, const int* src, const int* dst, int n, int lo, int hi) {
+  if (n == 0 || hi <= lo) return 0;
+  ForkTable t{};
+  for (int f = 0; f < n; ++f) {
+    const kllm_decoder *s = b->members[src[f]], *d = b->members[dst[f]];
+    t.ks[f] = s->kcache, t.vs[f] = s->vcache, t.kd[f] = d->kcache, t.vd[f] = d->vcache;
+  }
+  const kllm_decoder* d0 = b->members[0];
+  fork_rows_kernel<<<dim3(hi - lo, d0->m.layer_num, n), 256, 0, b->stream>>>(t, lo, decoder_cache(d0).cache);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+// kllm_batch_beam_search's loop, after its refusals: the rule of kuiperllama_b200/beam.py, step for step.  Beam r of
+// a pass is row r, carried by member rows[r].  Each pass puts every row's state (the beam's last id at the pass's
+// position), launches the pass, reads the candidates, applies the rule, then queues the next pass's tables and the
+// forks: a child whose parent's member is taken by an earlier child takes a dropped beam's member.
+int run_batch_beam(kllm_batch* b, int32_t first_token, int32_t start_pos, int32_t max_new, const int32_t* eos,
+                   int n_eos, float alpha, int early, int n_return, int32_t* out_ids, int32_t* out_len,
+                   float* out_score, float* out_sum, kllm_beam_stats* stats) {
+  const int B = static_cast<int>(b->members.size()), top = B + n_eos;
+  struct Beam {
+    std::vector<int32_t> ids;
+    float sum;
+    int member;
+  };
+  struct Cand {
+    float s;
+    int beam, k;
+    int32_t id;
+  };
+  struct Hyp {
+    float h, sum;
+    std::vector<int32_t> ids;
+  };
+  for (kllm_decoder* dc : b->members) KLLM_TRY(cudaStreamSynchronize(dc->stream));
+  for (int g = 0; g < (B > 1 ? 2 : 1); ++g) {  // first use: captured with nothing in flight
+    if (b->beam_exec[g] != nullptr) continue;
+    const int k = g == 0 ? 1 : B;
+    KLLM_TRY(capture_graph(b->stream, [b, k] { return enqueue_beam_pass(b, k, b->stream); }, &b->beam_exec[g],
+                           &b->beam_launches[g]));
+  }
+  std::vector<Beam> beams{Beam{{}, 0.f, 0}};
+  std::vector<Hyp> slots;
+  std::vector<Cand> cands;
+  bool unsatisfied = true, reordered = false;
+  kllm_beam_stats st{0, 0, 0};
+  int rc = 0;
+  for (int t = 1; t <= max_new && rc == 0; ++t) {
+    const int k = static_cast<int>(beams.size()), g = k == 1 ? 0 : 1;
+    const int pos = start_pos + t - 1;
+    for (int r = 0; r < k && rc == 0; ++r)
+      rc = put_state(b->members[beams[r].member], t == 1 ? first_token : beams[r].ids.back(), pos, 0, 0, 0, 0,
+                     b->stream);
+    if (rc != 0 || (rc = replay(b->beam_exec[g], b->beam_launches[g], 1, b->stream)) != 0) break;
+    if ((rc = static_cast<int>(cudaStreamSynchronize(b->stream))) != 0) break;
+    ++st.passes;
+    // 2. candidates: s = fp32(S_b + lp), ordered by s descending, beam, the beam's own order
+    const BeamCandidates& c = *b->cand_host;
+    cands.clear();
+    for (int r = 0; r < k; ++r)
+      for (int j = 0; j < top; ++j) cands.push_back(Cand{beams[r].sum + c.lp[r][j], r, j, c.ids[r][j]});
+    std::sort(cands.begin(), cands.end(), [](const Cand& x, const Cand& y) {
+      if (x.s != y.s) return x.s > y.s;
+      return x.beam != y.beam ? x.beam < y.beam : x.k < y.k;
+    });
+    // 3. finished hypotheses from the first B ranks, merged into the slots unless a gate is closed
+    const bool last = t == max_new;
+    auto is_eos = [&](int32_t id) { return hits_stop(eos, n_eos, id); };
+    auto extend = [](const std::vector<int32_t>& ids, int32_t id) {
+      std::vector<int32_t> r = ids;
+      r.push_back(id);
+      return r;
+    };
+    if (unsatisfied && !(static_cast<int>(slots.size()) == B && early == KLLM_BEAM_EARLY_ALL_DONE)) {
+      const float div = static_cast<float>(std::pow(static_cast<double>(t), static_cast<double>(alpha)));
+      for (int r = 0; r < B; ++r)
+        if (last || is_eos(cands[r].id))
+          slots.push_back(Hyp{cands[r].s / div, cands[r].s, extend(beams[cands[r].beam].ids, cands[r].id)});
+      std::stable_sort(slots.begin(), slots.end(), [](const Hyp& x, const Hyp& y) { return x.h > y.h; });
+      if (static_cast<int>(slots.size()) > B) slots.resize(B);
+    }
+    // 4. the next beams: the first B candidates that are not eos ids
+    std::vector<Beam> next;
+    std::vector<int> parent;
+    for (const Cand& x : cands) {
+      if (static_cast<int>(next.size()) == B) break;
+      if (is_eos(x.id)) continue;
+      next.push_back(Beam{extend(beams[x.beam].ids, x.id), x.s, -1});
+      parent.push_back(x.beam);
+    }
+    // 5. the early-stop heuristic and the stop test
+    const bool full = static_cast<int>(slots.size()) == B;
+    if (unsatisfied) {
+      const int L = early == KLLM_BEAM_EARLY_NEVER && alpha > 0.f ? max_new : t;
+      const float best = next[0].sum / static_cast<float>(std::pow(static_cast<double>(L), static_cast<double>(alpha)));
+      unsatisfied = !full || best > slots.back().h;
+    }
+    const bool stop = last || !unsatisfied || (full && early == KLLM_BEAM_EARLY_ALL_DONE);
+    // forks: after pass 0 member 0's prompt rows to every other member, even when the search stops there
+    int src[KLLM_MAX_BATCH], dst[KLLM_MAX_BATCH], nf = 0;
+    if (t == 1) {
+      for (int j = 0; j < B; ++j) next[j].member = j;
+      for (int j = 1; j < B; ++j) src[nf] = 0, dst[nf] = j, ++nf;
+      rc = fork_rows(b, src, dst, nf, 0, start_pos + 1);
+      st.forks += nf, st.fork_rows += static_cast<int64_t>(nf) * (start_pos + 1);
+    } else if (!stop) {
+      bool kept[KLLM_MAX_BATCH] = {};  // old beam r's member went to its first child
+      for (int j = 0; j < B; ++j)
+        if (!kept[parent[j]]) kept[parent[j]] = true, next[j].member = beams[parent[j]].member;
+      int free_members[KLLM_MAX_BATCH], n_free = 0;
+      for (int r = 0; r < k; ++r)
+        if (!kept[r]) free_members[n_free++] = beams[r].member;
+      std::sort(free_members, free_members + n_free);
+      for (int j = 0, f = 0; j < B; ++j)
+        if (next[j].member < 0) {
+          next[j].member = free_members[f++];
+          src[nf] = beams[parent[j]].member, dst[nf] = next[j].member, ++nf;
+        }
+      rc = fork_rows(b, src, dst, nf, start_pos + 1, pos + 1);
+      st.forks += nf, st.fork_rows += static_cast<int64_t>(nf) * (t - 1);
+    }
+    if (rc != 0 || stop) break;
+    // the next pass's rows; the last upload ran before this pass, so the staging is free
+    int rows[KLLM_MAX_BATCH];
+    for (int j = 0; j < B; ++j) rows[j] = next[j].member;
+    rc = put_tables(b, rows, B), reordered = true;
+    beams = std::move(next);
+  }
+  // the next call sees every member in its own row again
+  cudaError_t s = cudaStreamSynchronize(b->stream);
+  if (reordered && s == cudaSuccess) {
+    s = static_cast<cudaError_t>(put_member_tables(b));
+    if (s == cudaSuccess) s = cudaStreamSynchronize(b->stream);
+  }
+  if (rc == 0) rc = static_cast<int>(s);
+  if (rc != 0) return rc;
+  for (int i = 0; i < n_return; ++i) {
+    const Hyp& h = slots[i];
+    std::memcpy(out_ids + static_cast<size_t>(i) * max_new, h.ids.data(), sizeof(int32_t) * h.ids.size());
+    out_len[i] = static_cast<int32_t>(h.ids.size());
+    out_score[i] = h.h, out_sum[i] = h.sum;
+  }
+  if (stats != nullptr) *stats = st;
   return 0;
 }
 
@@ -1104,6 +1328,9 @@ void kllm_batch_destroy(kllm_batch* b) {
   if (b->stream) cudaStreamSynchronize(b->stream);
   for (cudaGraphExec_t e : b->exec)
     if (e) cudaGraphExecDestroy(e);
+  for (cudaGraphExec_t e : b->beam_exec)
+    if (e) cudaGraphExecDestroy(e);
+  if (b->cand_host) cudaFreeHost(b->cand_host);
   if (b->buf) cudaFree(b->buf);
   if (b->tables) cudaFree(b->tables);
   if (b->tables_host) cudaFreeHost(b->tables_host);
@@ -1138,6 +1365,29 @@ int kllm_batch_generate_until(kllm_batch* b, const int32_t* first_tokens_host, c
   }
   return run_batch_until(b, first_tokens_host, start_pos_host, max_steps_host, stop_ids_host, n_stop_host, on_tokens,
                          ctx, out_tokens_host, n_out_host, stats);
+}
+
+int kllm_batch_beam_search(kllm_batch* b, int32_t first_token, int32_t start_pos, int32_t max_new_tokens,
+                           const int32_t* eos_ids, int32_t n_eos, float length_penalty, int32_t early_stopping,
+                           int32_t n_return, int32_t* out_ids_host, int32_t* out_len_host, float* out_score_host,
+                           float* out_sum_host, kllm_beam_stats* stats) {
+  // every refusal comes before the first launch, so a refused call leaves every member as it was
+  if (!b || !out_ids_host || !out_len_host || !out_score_host || !out_sum_host) return KLLM_E_INVALID;
+  const DecoderModel& m = b->members[0]->m;
+  const int B = static_cast<int>(b->members.size());
+  if (first_token < 0 || first_token >= m.vocab_size || start_pos < 0 || max_new_tokens <= 0) return KLLM_E_INVALID;
+  if (static_cast<int64_t>(start_pos) + max_new_tokens > m.seq_len) return KLLM_E_INVALID;
+  if (n_eos < 0 || n_eos > KLLM_MAX_BEAM_EOS || (n_eos > 0 && eos_ids == nullptr)) return KLLM_E_INVALID;
+  for (int32_t i = 0; i < n_eos; ++i)
+    if (eos_ids[i] < 0 || eos_ids[i] >= m.vocab_size) return KLLM_E_INVALID;
+  if (n_return < 1 || n_return > B || !std::isfinite(length_penalty)) return KLLM_E_INVALID;
+  if (early_stopping < KLLM_BEAM_EARLY_HEURISTIC || early_stopping > KLLM_BEAM_EARLY_NEVER) return KLLM_E_INVALID;
+  // the rule is over the raw logits: a member that would draw or adjust them is refused, not silently ignored
+  for (const kllm_decoder* dc : b->members)
+    if (dc->cfg.sample.temperature != 0.f || sampling::step0_active(dc->cfg.penalty)) return KLLM_E_UNSUPPORTED;
+  if (static_cast<int64_t>(m.vocab_size) < static_cast<int64_t>(std::max(2, 1 + n_eos)) * B) return KLLM_E_UNSUPPORTED;
+  return run_batch_beam(b, first_token, start_pos, max_new_tokens, eos_ids, n_eos, length_penalty, early_stopping,
+                        n_return, out_ids_host, out_len_host, out_score_host, out_sum_host, stats);
 }
 
 int kllm_decoder_copy_prefix(kllm_decoder* dst, const kllm_decoder* src, int32_t n_pos) {

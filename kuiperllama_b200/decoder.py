@@ -592,6 +592,31 @@ class Batch:
         return ([list(out[b * M:b * M + n_out[b]]) for b in range(n)],
                 {"passes": stats.passes, "rows": stats.rows})
 
+    def beam_search(self, first_token: int, start_pos: int, max_new_tokens: int, eos_ids=(),
+                    length_penalty: float = 1.0, early_stopping=False, n_return: int = 1):
+        """Beam search with one beam per member (kllm_batch_beam_search): transformers' generate(num_beams=B,
+        length_penalty, early_stopping, num_return_sequences=n_return) with no logits processors, the rule of
+        beam.py.  Member 0 holds the prompt's positions [0, start_pos); first_token is fed at start_pos.
+        early_stopping is False, True or "never"; length_penalty is passed as fp32.  Returns ([{"ids", "score",
+        "sum"}, ...] best first, {"passes", "forks", "fork_rows"})."""
+        from . import BeamStats
+        from .beam import early_stopping_code
+        eos = [int(t) for t in eos_ids]
+        earr = (ctypes.c_int32 * max(len(eos), 1))(*eos)
+        steps, n_ret = max(int(max_new_tokens), 1), max(int(n_return), 1)
+        out = (ctypes.c_int32 * (n_ret * steps))()
+        lens = (ctypes.c_int32 * n_ret)()
+        scores = (ctypes.c_float * n_ret)()
+        sums = (ctypes.c_float * n_ret)()
+        stats = BeamStats()
+        check(self.lib.kllm_batch_beam_search(self.handle, int(first_token), int(start_pos), int(max_new_tokens),
+                                              earr, len(eos), float(length_penalty),
+                                              early_stopping_code(early_stopping), int(n_return), out, lens, scores,
+                                              sums, ctypes.byref(stats)), "kllm_batch_beam_search")
+        hyps = [{"ids": list(out[i * steps:i * steps + lens[i]]), "score": scores[i], "sum": sums[i]}
+                for i in range(int(n_return))]
+        return hyps, {"passes": stats.passes, "forks": stats.forks, "fork_rows": stats.fork_rows}
+
     def close(self):
         if getattr(self, "handle", None):
             self.lib.kllm_batch_destroy(self.handle)
